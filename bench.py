@@ -2,6 +2,7 @@
 """Benchmark of the cross-attention heat-map hot path (BASELINE.json metric: heat-map px/s).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload sd21|sd21_768|sdxl|sdxl70|sd15] [--prompts P]
+                    [--dump-outputs DIR]
 
 Workload (BASELINE.json configs[1]): random-init SD-2.1-base UNet shapes, 64x64 latent, 77 tokens, bf16, the 15 traced
 cross-attention layers of one denoising step. A bench "step" is one pass of the hot path over one step's Q/K:
@@ -9,8 +10,9 @@ cross-attention layers of one denoising step. A bench "step" is one pass of the 
 
 One JSON line is printed by rank 0:
   value         px/s with Q/K already resident in HBM: one persistent `daam_accumulate` launch per step (all 15
-                layers), K steps timed with CUDA events between barriers, max over ranks, x N ranks (weak scaling).
-                Inputs exceed L2: the steps rotate over R independent resident prompt sets (accumulators + Q/K).
+                layers), K timed steps in up to 10 blocks timed with CUDA events between barriers, median block, max
+                over ranks, x N ranks (weak scaling). Inputs exceed L2: the steps rotate over R independent resident
+                prompt sets (accumulators + Q/K).
   roofline      the accumulate kernel against the measured HBM copy bandwidth (MEASURED_PEAKS.json), algorithmic bytes.
   e2e           the same metric through the public API -- `with trace(pipe): pipe(prompt, K steps);
                 compute_global_heat_map()` on the cross-attention skeleton of the UNet -- with the pipeline inputs in
@@ -18,6 +20,12 @@ One JSON line is printed by rank 0:
   cpu_baseline  the oracle's port of the reference hot path (rows a3+a4+a6) timed on this box's host cores on a bounded
                 sample of the same Q/K shapes.
   hook_overhead hooked vs un-hooked forward of a full-cost synthetic UNet (resnets, self-attention, feed-forward), ms/step.
+
+`--dump-outputs DIR` writes, after the timed steps, what they computed as float32 .npy files: the accumulators of the
+prompt set of the last timed step (`acc_layerNN`, [prompts, heads, 77, hw]: what `daam_accumulate` hands its caller)
+and the global heat maps of the timed e2e generation (`e2e_heat_maps`). Inputs are seeded, so two builds run with the
+same arguments can be compared file by file. Above 64 MB in all, each array is replaced by the same fixed seeded sample
+of its flattened elements (`<name>.npy` then holds the values, `<name>.idx.npy` their flat indices).
 
 `--impl reference` times the reference's own CPU implementation of the path instead (the oracle's op-for-op port of
 daam/trace.py's hook, since the Python reference cannot travel to the GPU box) through the same pipeline API on CPU.
@@ -110,7 +118,7 @@ def measured_peak():
         with open(path) as f:
             return float(json.load(f)['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs)'
     except Exception:
-        return 6650.0, 'fallback (B200_PROFILING.md 6.65 TB/s)'
+        return 3350.0, 'fallback (H100 SXM data sheet: 3.35 TB/s HBM3)'
 
 
 def recorded_traffic(workload):
@@ -215,43 +223,44 @@ def build_sets(layers, n_prompts, dtype, n_sets, seed):
 
 
 def leg_value(args, layers, dtype, D: Dist, windows):
-    """K steps (one persistent launch per traced-layer pack each) between CUDA events, repeated over R blocks.
+    """K timed steps (one persistent launch per traced-layer pack each), split into up to 10 blocks between CUDA events.
 
-    Every block is what the contract describes -- barrier + synchronize, K timed steps, synchronize + barrier -- and the
-    reported time is the median block (max over ranks per block). The launches of a block are queued behind a short
+    Every block is barrier + synchronize, its timed steps, synchronize + barrier; the reported time for K steps is K x the
+    per-step time of the median block (max over ranks per block). The launches of a block are queued behind a short
     spin kernel so that the device executes them back to back: the figure is device throughput, not host launch pacing
-    (8 Python processes share one host at N=8)."""
+    (8 Python processes share one host at N=8). Returns also the accumulators of the last timed step's prompt set."""
     from daam_b200 import _native, ops
-    n_sets, _ = value_sets(layers, args.prompts)               # working set >= 320 MB > 126 MB L2
+    n_sets, _ = value_sets(layers, args.prompts)               # working set >= 320 MB > 50 MB L2
     sets = build_sets(layers, args.prompts, dtype, n_sets, 1234 + D.rank)
     stream = torch.cuda.current_stream()
     flags = _native.ACC_AUTO | _native.ACC_EARLY_LOADS       # Q/K are resident inputs: complete long before any launch
     for i in range(args.warmup):
         ops.accumulate(sets[i % n_sets][0], 'cuda', stream, flags)
     torch.cuda.synchronize()
-    blocks = max(10, -(-200 // args.steps))
-    gate_cycles = int(max(2.0, args.steps * 0.04) * 1.9e6)     # ~max(2 ms, 40 us per launch) at 1.9 GHz
+    sizes = block_sizes(args.steps)
+    blocks = len(sizes)
     launches0 = _native.launch_count()
     block_ms, step = [], args.warmup
-    for _ in range(blocks):
+    for size in sizes:
+        gate_cycles = int(max(2.0, size * 0.04) * 1.9e6)       # ~max(2 ms, 40 us per launch) at 1.9 GHz
         D.barrier()
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         t0 = time.time()
         torch.cuda._sleep(gate_cycles)
         e0.record(stream)
-        for _k in range(args.steps):
+        for _k in range(size):
             ops.accumulate(sets[step % n_sets][0], 'cuda', stream, flags)
             step += 1
         e1.record(stream)
         torch.cuda.synchronize()
         D.barrier()
         torch.cuda.synchronize()
-        block_ms.append(e0.elapsed_time(e1))
+        block_ms.append(e0.elapsed_time(e1) / size)                   # per step
         if len(block_ms) == 1:
             t_first = t0
     windows.append((t_first, time.time()))
-    launches = (_native.launch_count() - launches0) // blocks          # per K-step block
+    launches = _native.launch_count() - launches0                      # over the K timed steps
     mine = torch.tensor(block_ms, dtype=torch.float64, device='cuda')
     if D.world > 1:
         allr = torch.empty(D.world, blocks, dtype=torch.float64, device='cuda')
@@ -259,12 +268,12 @@ def leg_value(args, layers, dtype, D: Dist, windows):
     else:
         allr = mine.unsqueeze(0)
     per_block_max = allr.max(dim=0).values                              # max over ranks, block by block
-    ms = float(per_block_max.median())
-    us = allr / args.steps * 1e3                                        # per-launch-step, per rank and block
-    stats = {'blocks': blocks, 'steps_per_block': args.steps,
+    ms = float(per_block_max.median()) * args.steps                     # K steps at the median block's step time
+    us = allr * 1e3                                                     # per step, per rank and block
+    stats = {'blocks': blocks, 'steps_per_block': sizes, 'timed_steps': step - args.warmup,
              'us_per_step_median_block_max_over_ranks': round(ms / args.steps * 1e3, 3),
-             'us_per_step_best_block_max_over_ranks': round(float(per_block_max.min()) / args.steps * 1e3, 3),
-             'us_per_step_worst_block_max_over_ranks': round(float(per_block_max.max()) / args.steps * 1e3, 3),
+             'us_per_step_best_block_max_over_ranks': round(float(per_block_max.min()) * 1e3, 3),
+             'us_per_step_worst_block_max_over_ranks': round(float(per_block_max.max()) * 1e3, 3),
              'per_rank_us_per_step': [{'rank': r, 'min': round(float(us[r].min()), 3),
                                        'median': round(float(us[r].median()), 3), 'max': round(float(us[r].max()), 3)}
                                       for r in range(D.world)]}
@@ -273,7 +282,8 @@ def leg_value(args, layers, dtype, D: Dist, windows):
     visits = len(range(0, step, n_sets))
     got = float(acc[0, 0].double().sum())
     assert abs(got - visits * acc.shape[-1]) < 1e-3 * got, (got, visits)
-    return ms, launches, n_sets, stats
+    last = {f'acc_layer{i:02d}': a for i, (_, _, a) in enumerate(sets[(step - 1) % n_sets][1])}
+    return ms, launches, n_sets, stats, last
 
 
 def leg_e2e(args, spec, dtype, D: Dist, windows, cuda_graph=True):
@@ -315,6 +325,7 @@ def leg_e2e(args, spec, dtype, D: Dist, windows, cuda_graph=True):
             windows.append((t0, time.time()))
             return maps, (e0.elapsed_time(e1), pipe.h2d_bytes_per_step, pipe.d2h_bytes_per_step, out_h)
 
+    # the timed generation's first 3+ steps are untimed: they also capture the step graph
     maps, (ms_local, h2d, d2h_step, out_h) = generate(D.rank, args.steps, True)
     ms = D.max_ms(ms_local)
     d2h = d2h_step + out_h.numel() * 4 / max(1, args.steps) / max(1, D.world)
@@ -336,7 +347,7 @@ def leg_e2e(args, spec, dtype, D: Dist, windows, cuda_graph=True):
             order = {'ok': False, 'error': repr(e)}
         if not order['ok']:
             log(f'[bench] WARNING: gather order check failed: {order}')
-    return ms, h2d, d2h, order
+    return ms, h2d, d2h, order, out_h
 
 
 def leg_hook_overhead(args, spec, dtype, windows):
@@ -490,7 +501,7 @@ def run_reference(args):
     op-for-op port of daam/trace.py's hooks that tests/test_oracle_vs_reference.py pins bit-equal to the verbatim
     reference). Default: on this box's host cores in fp32 -- the contract's reference arm. ``--ref-device cuda`` runs
     the same torch-eager reference hooks on the GPU in the pipeline dtype instead (what a user of the reference gets on
-    this box; a secondary figure recorded under profiles/, never what the driver's ratio is built on)."""
+    this box; a secondary figure, never what the headline ratio is built on)."""
     rank = int(os.environ.get('RANK', '0'))
     if rank != 0:
         return
@@ -563,6 +574,33 @@ def workload_name(args):
     return f'{base[args.workload]}, {args.prompts} prompt(s)/GPU, {args.dtype}'
 
 
+def block_sizes(steps):
+    """The K timed steps of the value leg as up to 10 blocks of (nearly) equal size."""
+    blocks = max(1, min(10, steps))
+    return [steps // blocks + (1 if i < steps % blocks else 0) for i in range(blocks)]
+
+
+DUMP_BYTES = 64_000_000 - 64 * 1024        # --dump-outputs: 64 MB in all, headroom for the .npy headers and indices
+
+
+def dump_outputs(dirname, arrays):
+    """Writes DIR/<name>.npy (float32) for every tensor of `arrays`. Above DUMP_BYTES in all, every array keeps the same
+    fraction of its elements, at flat indices drawn from a fixed seed (stored as DIR/<name>.idx.npy)."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    total = sum(t.numel() for t in arrays.values()) * 4
+    frac = 1.0 if total <= DUMP_BYTES else DUMP_BYTES / (2 * total)              # values + int32 indices
+    for i, (name, t) in enumerate(sorted(arrays.items())):
+        flat = t.detach().reshape(-1)
+        if frac < 1.0:
+            idx = np.unique(np.random.default_rng(i).integers(0, flat.numel(), int(flat.numel() * frac)))
+            np.save(os.path.join(dirname, name + '.idx.npy'), idx.astype(np.int32))
+            flat = flat[torch.from_numpy(idx).to(flat.device)]
+            np.save(os.path.join(dirname, name + '.npy'), flat.float().cpu().numpy())
+        else:
+            np.save(os.path.join(dirname, name + '.npy'), t.detach().float().cpu().numpy())
+
+
 def value_sets(layers, prompts):
     set_bytes = algorithmic_bytes_per_step(layers, prompts) - px_per_step(layers, prompts) * 4   # accumulators once
     return max(2, -(-int(320e6) // max(1, set_bytes))), set_bytes
@@ -571,16 +609,17 @@ def value_sets(layers, prompts):
 def shared_config(args, layers, world):
     """The `config` object: identical for both arms of a run (the reference arm runs `on your arm's config`)."""
     n_sets, set_bytes = value_sets(layers, args.prompts)
-    blocks = max(10, -(-200 // args.steps))
+    sizes = block_sizes(args.steps)
     return {
         'workload': workload_name(args), 'px_per_step': px_per_step(layers, args.prompts),
         'px_definition': 'sum over traced layers of heads*77*h*w',
         'literal_px_per_step': literal_px_per_step(layers, args.prompts),
         'l2': f'inputs larger than L2: steps rotate over {n_sets} resident prompt sets '
-              f'({n_sets * set_bytes / 1e6:.0f} MB of accumulators+Q/K vs 126 MB L2), no flush',
+              f'({n_sets * set_bytes / 1e6:.0f} MB of accumulators+Q/K vs 50 MB L2), no flush',
         'launch': 'one persistent kernel per step per pack of <= 32 traced layers',
-        'timing': f'value: median of {blocks} blocks of K={args.steps} steps (each block between barrier+synchronize, '
-                  f'CUDA events, max over ranks; launches queued behind a spin kernel so host pacing is not timed)',
+        'timing': f'value: K={args.steps} timed steps in {len(sizes)} blocks, K x the median block\'s step time (each '
+                  f'block between barrier+synchronize, CUDA events, max over ranks; launches queued behind a spin kernel '
+                  f'so host pacing is not timed)',
         'parallelism': f'prompts sharded, dp{world}',
     }
 
@@ -601,7 +640,11 @@ def main():
     ap.add_argument('--skip-cpu', action='store_true')
     ap.add_argument('--skip-eager', action='store_true', help='skip the eager (no CUDA graph) e2e leg')
     ap.add_argument('--skip-e2e', action='store_true', help='kernel legs only (profiling runs)')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write what the timed steps computed as DIR/<name>.npy (float32, <= 64 MB in all)')
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error('--steps must be >= 1')
     if args.dtype is None:   # sd15: the reference's default load
         args.dtype = {'sd21': 'bf16', 'sd21_768': 'bf16', 'sdxl': 'fp16', 'sdxl70': 'fp16', 'sd15': 'fp32'}[args.workload]
     args.warmup = max(3, args.warmup)
@@ -621,12 +664,12 @@ def main():
     windows = []
 
     with torch.no_grad():
-        ms, launches, n_sets, value_stats = leg_value(args, layers, dtype, D, windows)
+        ms, launches, n_sets, value_stats, outputs = leg_value(args, layers, dtype, D, windows)
         e2e_ms = eager_ms = float('nan')
         h2d = d2h = 0
         order = None
         if not args.skip_e2e:
-            e2e_ms, h2d, d2h, order = leg_e2e(args, spec, dtype, D, windows, cuda_graph=True)
+            e2e_ms, h2d, d2h, order, outputs['e2e_heat_maps'] = leg_e2e(args, spec, dtype, D, windows, cuda_graph=True)
             if not args.skip_eager:
                 eager_ms = leg_e2e(args, spec, dtype, D, windows, cuda_graph=False)[0]
         overhead = None
@@ -642,6 +685,9 @@ def main():
                 overhead['max_over_ranks'] = {'overhead_ms_per_step': round(float(worst[0]), 4),
                                               'hooked_ms_per_step': round(float(worst[1]), 4),
                                               'unhooked_ms_per_step': round(float(worst[2]), 4), 'ranks': D.world}
+    if args.dump_outputs and D.rank == 0:
+        dump_outputs(args.dump_outputs, outputs)
+    del outputs
     D.barrier()
     if D.rank != 0:
         D.close()

@@ -1,7 +1,7 @@
-"""daam_b200 -- B200-native cross-attention heat-map extraction behind the castorini/daam API.
+"""daam_b200 -- H100-native cross-attention heat-map extraction behind the castorini/daam API.
 
 ``from daam_b200 import trace, set_seed`` is the drop-in for ``from daam import trace, set_seed`` on the hot path
-(reference export surface: ``/root/reference/daam/__init__.py:1-6``)."""
+(reference export surface: the reference's ``daam/__init__.py:1-6``)."""
 from ._version import __version__
 from .evaluate import *     # noqa: F401,F403
 from .experiment import *   # noqa: F401,F403

@@ -1,4 +1,4 @@
-"""Builds ``libdaam_b200.so`` in-tree with nvcc for sm_100a (``python -m daam_b200.build``)."""
+"""Builds ``libdaam_b200.so`` in-tree with nvcc for sm_90a (``python -m daam_b200.build``)."""
 from __future__ import annotations
 
 import os
@@ -9,7 +9,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 SOURCES = ['api.cu', 'accumulate_simt.cu', 'accumulate_mma.cu', 'finalize.cu', 'probs.cu']
 OUT = os.path.join(HERE, 'libdaam_b200.so')
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC',
               '-I', os.path.join(ROOT, 'include'), '-shared']
 
 
@@ -28,94 +28,18 @@ def needs_build() -> bool:
     return any(os.path.getmtime(d) > os.path.getmtime(OUT) for d in deps)
 
 
-def build(force: bool = False, verbose: bool = False, sass_summary: bool = None) -> str:
-    """``sass_summary`` (default: same as ``verbose``): compile with ``-Xptxas -v`` and (re)write ``profiles/r02_sass.md``
-    -- per kernel the registers / spills ptxas reports and the counts of the SASS mnemonics that prove the Blackwell path
-    (UTCHMMA = tcgen05.mma, LDTM = tcgen05.ld, UTMALDG / UTMAREDG = TMA tensor load / reduce, UTCBAR = tcgen05.commit,
-    SYNCS = mbarrier). ``verbose`` also echoes the compiler output."""
+def build(force: bool = False, verbose: bool = False) -> str:
+    """``verbose``: compile with ``-Xptxas -v`` and echo the compiler output (registers, shared memory, spills)."""
     if not force and not needs_build():
         return OUT
-    sass_summary = verbose if sass_summary is None else sass_summary
-    cmd = [_nvcc()] + NVCC_FLAGS + (['-Xptxas', '-v'] if verbose or sass_summary else []) + ['-o', OUT] + \
+    cmd = [_nvcc()] + NVCC_FLAGS + (['-Xptxas', '-v'] if verbose else []) + ['-o', OUT] + \
           [os.path.join(HERE, 'csrc', s) for s in SOURCES]
     res = subprocess.run(cmd, capture_output=True, text=True)
     if verbose or res.returncode != 0:
         sys.stderr.write(res.stdout + res.stderr)
     if res.returncode != 0:
         raise RuntimeError('nvcc failed building libdaam_b200.so')
-    if sass_summary:
-        try:
-            write_sass_summary(res.stdout + res.stderr)
-        except Exception as e:     # the evidence file is a by-product: never fail the build over it
-            sys.stderr.write(f'[daam_b200.build] SASS summary not written: {e!r}\n')
     return OUT
-
-
-SASS_MNEMONICS = ('UTCHMMA', 'UTCQMMA', 'LDTM', 'STTM', 'UTMALDG', 'UTMAREDG', 'UTMASTG', 'UTMACCTL.PF', 'UBLKCP', 'UTCBAR',
-                  'UTCATOMSWS',
-                  'SYNCS', 'HMMA', 'FFMA', 'MUFU.EX2', 'RED.E', 'LDGSTS')
-
-
-def _demangle(names):
-    try:
-        out = subprocess.run(['cu++filt'] + list(names), capture_output=True, text=True).stdout.split('\n')
-        return {n: (o or n) for n, o in zip(names, out)}
-    except Exception:
-        return {n: n for n in names}
-
-
-def write_sass_summary(ptxas_log: str, dst: str = None) -> str:
-    """cuobjdump -sass of the built library -> profiles/r02_sass.md (evidence that does not depend on having the .so)."""
-    import re
-    dst = dst or os.path.join(ROOT, 'profiles', 'r02_sass.md')
-    sass = subprocess.run(['cuobjdump', '-sass', OUT], capture_output=True, text=True).stdout
-    counts, cur = {}, None
-    for line in sass.split('\n'):
-        m = re.match(r'\s*Function : (\S+)', line)
-        if m:
-            cur = m.group(1)
-            counts[cur] = {k: 0 for k in SASS_MNEMONICS}
-            counts[cur]['_instructions'] = 0
-            continue
-        if cur is None or '/*' not in line:
-            continue
-        m = re.search(r'/\*[0-9a-f]{4}\*/\s+(?:@!?U?P\d+\s+)?([A-Z0-9_.]+)', line)
-        if not m:
-            continue
-        op = m.group(1)
-        counts[cur]['_instructions'] += 1
-        for k in SASS_MNEMONICS:
-            if op == k or op.startswith(k + '.') or (k == 'MUFU.EX2' and op.startswith('MUFU.EX2')):
-                counts[cur][k] += 1
-    res = {}
-    for m in re.finditer(r"Compiling entry function '(\S+)' for 'sm_100a'\n(?:ptxas info\s+: Function properties.*\n\s+.*\n)?"
-                         r"ptxas info\s+: Used (\d+) registers(?:, used \d+ barriers)?(?:, (\d+) bytes cumulative stack size)?"
-                         r"(?:, (\d+) bytes smem)?", ptxas_log):
-        res[m.group(1)] = (m.group(2), m.group(4) or '0')
-    spills = dict(re.findall(r"Function properties for (\S+)\n\s+(\d+ bytes stack frame, \d+ bytes spill stores, \d+ bytes spill loads)",
-                             ptxas_log))
-    names = _demangle(list(counts))
-    cols = [k for k in SASS_MNEMONICS if any(c[k] for c in counts.values())]
-    with open(dst, 'w') as f:
-        f.write('# SASS / ptxas summary of libdaam_b200.so (sm_100a)\n\n'
-                'Regenerate: `python -m daam_b200.build --force -v` (writes this file). Source: `cuobjdump -sass` of the built '
-                'library + `nvcc -Xptxas -v`.\n`UTCHMMA` = `tcgen05.mma` (kind::f16 and kind::tf32), `LDTM` = `tcgen05.ld`, '
-                '`UTMALDG` = TMA tensor load, `UTMAREDG` = TMA tensor reduce-add, `UTCBAR` = `tcgen05.commit`, '
-                '`SYNCS` = mbarrier ops, `UTMACCTL.PF` = `prefetch.tensormap`, `UTCATOMSWS` = `tcgen05.alloc` / `dealloc`.\n\n')
-        f.write('| kernel | regs | static smem B | spills | SASS instr | ' + ' | '.join(cols) + ' |\n')
-        f.write('|---|---:|---:|---|---:|' + '---:|' * len(cols) + '\n')
-        for mangled, c in counts.items():
-            full, depth, cut = names[mangled], 0, None
-            for i, ch in enumerate(full):                 # cut the parameter list, keep the template arguments
-                depth += (ch == '<') - (ch == '>')
-                if ch == '(' and depth == 0:
-                    cut = i
-                    break
-            short = full[:cut].replace('daam::<unnamed>::', '').replace('void ', '').replace('(bool)', '')
-            regs, smem = res.get(mangled, ('?', '?'))
-            f.write(f'| `{short}` | {regs} | {smem} | {spills.get(mangled, "n/a")} | {c["_instructions"]} | ' +
-                    ' | '.join(str(c[k]) for k in cols) + ' |\n')
-    return dst
 
 
 if __name__ == '__main__':

@@ -1,33 +1,32 @@
-// Fused softmax(QK^T) -> unravel -> accumulate, tcgen05 / TMA / TMEM variant (head_dim up to 192 in 64-wide K chunks).
+// Fused softmax(QK^T) -> unravel -> accumulate, Hopper wgmma / TMA variant (head_dim up to 256 in 64-wide K chunks).
 //
 // One tile = 128 pixels x 77 tokens of one (layer, prompt, head). Per tile:
-//   TMA        Q tile [128 x 64] and K [77(+3 zero rows) x 64] -> shared memory, 128B-swizzled K-major (the UMMA
+//   TMA        Q tile [128 x 64] and K [77(+3 zero rows) x 64] -> shared memory, 128B-swizzled K-major (the wgmma
 //              canonical layout), straight from the strided `to_q`/`to_k` outputs via 4-D tensor maps
 //              {dim, head, row, prompt}; partial tiles and the 3 padding token rows are zero-filled by the TMA unit.
-//   tcgen05    S = Q K^T as 4 x tcgen05.mma (M128 N80 K16, kind::f16, fp32 accumulate) into a TMEM accumulator
-//              (2 accumulators, so the MMA of tile i+1 overlaps the epilogue of tile i).
-//   epilogue   4 warps: tcgen05.ld gives every thread the 77 logits of ITS pixel (TMEM lane == pixel), so the
-//              softmax is thread-local (no shuffles); the probabilities are then added into the fp32 accumulator
-//              acc[head][token][pixel] either
-//                red mode : staged token-major in shared memory and sent as ONE bulk-tensor reduce-add
-//                           (cp.reduce.async.bulk.tensor .add.f32): the read-modify-write happens in L2, the SM never
-//                           loads the accumulator;
-//                ldst mode: coalesced 128-byte load / add / store per warp and token, straight from registers.
-// Warp roles: 0-3 epilogue, 4 TMA producer (one elected thread), 5 TMEM allocator + MMA issuer (one thread).
-// Persistent: every CTA walks a contiguous chunk of the launch's tiles; up to 2 CTAs per SM (256 TMEM columns each).
+//   wgmma      S = Q K^T: each of the two consumer warpgroups issues wgmma.m64n80k16 (fp32 accumulate) over its 64
+//              pixel rows of the tile, K^T shared; the 64 x 80 logits land in registers (40 per thread).
+//   epilogue   softmax over the 77 tokens of each pixel row (a row lives in the 4 threads of a quad: two shuffles per
+//              reduction), the probabilities are staged token-major in shared memory ([77][128] fp32) and added into
+//              the fp32 accumulator acc[head][token][pixel] either
+//                red mode : as ONE bulk-tensor reduce-add (cp.reduce.async.bulk.tensor .add.f32): the read-modify-write
+//                           happens in L2, the SM never loads the accumulator;
+//                ldst mode: coalesced 16-byte load / add / store of the staged tile by all consumer threads.
+// Warp roles: 0-7 consumers (two warpgroups: MMA + softmax + accumulate), 8 TMA producer (one elected thread) that runs
+// up to two K chunks ahead through a two-stage ring. Persistent: every CTA walks a contiguous chunk of the launch's
+// tiles; two CTAs per SM, so one CTA's loads and MMAs overlap the other's epilogue.
 //
 // fp32 projections (the reference's default dtype for SD-1.x/2.x, daam/run/generate.py:205) take the same kernel in
-// "split" form. Tensor cores have no fp32 operand type and a plain kind::tf32 product would drop 13 mantissa bits, so
-// every value is used as two tf32 terms, x = hi + lo with hi = trunc_tf32(x) -- what the tensor core reads from the raw
-// fp32 container -- and lo = rna_tf32(x - hi) (22 significand bits), and q.k = q_lo.k_hi + q_hi.k_lo + q_hi.k_hi (the
-// dropped terms are ~2^-22 relative): the fp32 Q/K tiles arrive by TMA exactly like the 16-bit ones (two 128-byte-wide
-// swizzled sub-tiles per 64 dims) and ARE the hi operands; eight converter warps emit `lo` into a second buffer (a
-// shared-memory -> shared-memory elementwise pass, swizzle-agnostic), and the MMA thread issues 3 x 8 tcgen05.mma
-// kind::tf32 (K = 8) per tile. One CTA per SM (two 52 KB raw stages + one lo buffer + the staged probabilities).
+// "split" form. Tensor cores have no fp32 operand type and a plain tf32 product would drop 13 mantissa bits, so every
+// value is used as two tf32 terms, x = hi + lo with hi = trunc_tf32(x) and lo = rna_tf32(x - hi) (22 significand bits),
+// and q.k = q_lo.k_hi + q_hi.k_lo + q_hi.k_hi (the dropped terms are ~2^-22 relative): the fp32 Q/K tiles arrive by TMA
+// exactly like the 16-bit ones (two 128-byte-wide swizzled sub-tiles per 64 dims); the consumer threads rewrite them
+// in place as hi and emit `lo` into a second buffer (a shared-memory -> shared-memory elementwise pass, swizzle-
+// agnostic), then issue 3 x 8 wgmma.m64n80k8 tf32 per chunk. One CTA per SM (two 52 KB raw stages + one lo buffer +
+// the staged probabilities).
 //
 // head_dim other than 64 (SD-1.x: 40 / 80 / 160): the contraction runs in 64-wide K chunks, one chunk per smem stage,
-// accumulated into the same TMEM accumulator; the last chunk is zero-filled beyond head_dim (by the TMA unit, or by the
-// converter warps) and issues only the MMAs that cover live columns.
+// accumulated into the same registers; the last chunk is zero-filled beyond head_dim by the TMA unit.
 //
 // Replaces daam/trace.py:276 (get_attention_scores), :219-244 (_unravel_attn) and :293-294 (update loop).
 #include <cuda.h>
@@ -46,16 +45,15 @@ constexpr int kQBytes = kTilePixels * 128;            // 128 rows x 128 B (64 x 
 constexpr int kKBytes = kTokensPad * 128;             // 80 rows x 128 B
 constexpr int kStageBytes = kQBytes + kKBytes;        // 26624 = 26 x 1024 (keeps every tile 1024-byte aligned)
 constexpr int kPBytes = kTokens * kTilePixels * 4;    // staged probabilities [77][128] fp32
-constexpr int kTmemCols = 256;
-constexpr int kAccCols = 128;                         // column distance between the two accumulators
-constexpr int kThreads = 192;
-constexpr int kBarBytes = 256;                        // mbarriers + the TMEM base address slot
+constexpr int kConsumers = 256;                       // two warpgroups, 64 pixel rows each
+constexpr int kThreads = kConsumers + 32;             // + the TMA producer warp
+constexpr int kBarBytes = 64;                         // mbarriers
 constexpr int kSmemBytes = 1024 + kStages * kStageBytes + kPBytes + kBarBytes;
 // split (fp32) form: a raw stage holds the fp32 tiles as [Q sub0][Q sub1][K sub0][K sub1] (sub-tile = 32 floats = one
-// 128-byte swizzle span per row); one more buffer of the same shape holds the lo terms; warps 6-9 convert
+// 128-byte swizzle span per row); one more buffer of the same shape holds the lo terms
 constexpr int kSplitStageBytes = 2 * kStageBytes;     // 53248 = 52 x 1024
-constexpr int kSplitThreads = 448;                   // 6 warps as in the 16-bit form + 8 converter warps
 constexpr int kSplitSmemBytes = 1024 + (kStages + 1) * kSplitStageBytes + kPBytes + kBarBytes;
+static_assert(2 * (kSmemBytes + 1024) <= 233472, "two 16-bit-form CTAs must fit one SM's 228 KB of shared memory");
 static_assert(kSplitSmemBytes <= 232448, "split form exceeds the 227 KB shared-memory limit");
 
 struct MmaParams {
@@ -127,61 +125,56 @@ __device__ __forceinline__ void prefetch_tensormap(const CUtensorMap* map) {
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void epi_barrier() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
+__device__ __forceinline__ void consumer_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory"); }
 
-// UMMA shared-memory descriptor: K-major operand tile, 128B swizzle, rows of 128 bytes, 8-row groups 1024 B apart.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
+// wgmma shared-memory descriptor: K-major operand tile, 128B swizzle, rows of 128 bytes, 8-row groups 1024 B apart.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
   return (uint64_t)((smem_addr & 0x3FFFFu) >> 4) | (1ull << 16) /* LBO (unused with swizzle) */ |
-         ((uint64_t)(1024 >> 4) << 32) /* SBO */ | (1ull << 46) /* descriptor version (sm_100) */ |
-         (2ull << 61) /* SWIZZLE_128B */;
+         ((uint64_t)(1024 >> 4) << 32) /* SBO */ | (1ull << 62) /* SWIZZLE_128B */;
 }
-// Instruction descriptor, kind::f16: fp32 accumulate, A/B both K-major, M = 128, N = 80.
-__device__ __forceinline__ uint32_t umma_idesc(bool bf16) {
-  const uint32_t fmt = bf16 ? 1u : 0u;
-  return (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(kTokensPad >> 3) << 17) |
-         ((uint32_t)(kTilePixels >> 4) << 24);
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                         uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-      "}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// kind::tf32: operands are 32-bit containers read as tf32, K = 8 per instruction (32 bytes along the swizzled row).
-__device__ __forceinline__ uint32_t umma_idesc_tf32() {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(kTokensPad >> 3) << 17) | ((uint32_t)(kTilePixels >> 4) << 24);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                          uint32_t accumulate) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n"
-      "}" ::"r"(tmem_d),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
-      "[%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
+
+// The 64 x 80 fp32 accumulator fragment of one warpgroup: thread (warp w, lane l) holds rows 16w + l/4 (+ 8) and
+// columns 8j + 2(l%4) (+ 1) as d[4j + {0, 1}] (row r0) and d[4j + {2, 3}] (row r0 + 8), j = 0..9.
+using Frag = float[40];
+
+__device__ __forceinline__ void frag_fence(Frag& d) {
 #pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < 40; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+#define DAAM_FRAG_OPERANDS                                                                                          \
+  "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),         \
+      "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),          \
+      "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),         \
+      "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),         \
+      "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
+#define DAAM_FRAG_REGS                                                                                              \
+  "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, " \
+  "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}"
+
+// d += A[64 x 16] B[80 x 16]^T, both K-major in shared memory; 16-bit operands (fp16 or bf16)
+template <bool kBf16>
+__device__ __forceinline__ void wgmma_16bit(Frag& d, uint64_t adesc, uint64_t bdesc) {
+  if constexpr (kBf16)
+    asm volatile("wgmma.mma_async.sync.aligned.m64n80k16.f32.bf16.bf16 " DAAM_FRAG_REGS ", %40, %41, 1, 1, 1, 0, 0;"
+                 : DAAM_FRAG_OPERANDS
+                 : "l"(adesc), "l"(bdesc)
+                 : "memory");
+  else
+    asm volatile("wgmma.mma_async.sync.aligned.m64n80k16.f32.f16.f16 " DAAM_FRAG_REGS ", %40, %41, 1, 1, 1, 0, 0;"
+                 : DAAM_FRAG_OPERANDS
+                 : "l"(adesc), "l"(bdesc)
+                 : "memory");
+}
+// d += A[64 x 8] B[80 x 8]^T with tf32 operands (32-bit containers, K = 8 = 32 bytes along the swizzled row)
+__device__ __forceinline__ void wgmma_tf32(Frag& d, uint64_t adesc, uint64_t bdesc) {
+  asm volatile("wgmma.mma_async.sync.aligned.m64n80k8.f32.tf32.tf32 " DAAM_FRAG_REGS ", %40, %41, 1, 1, 1;"
+               : DAAM_FRAG_OPERANDS
+               : "l"(adesc), "l"(bdesc)
+               : "memory");
 }
 
 struct Tile {
@@ -215,16 +208,14 @@ __device__ __forceinline__ float rna_tf32(float x) {
   asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
   return __uint_as_float(r);
 }
-// hi term of the split as the tensor core sees it: kind::tf32 reads the upper 19 bits of the 32-bit container and
-// ignores the low 13 mantissa bits, i.e. hi = trunc_tf32(x). (Pinned by tests/test_parity_elementwise_gpu.py: were the
-// hardware to round instead, hi + lo would be off by a tf32 ulp and every fp32 parity test would fail at 1e-3.)
 __device__ __forceinline__ float trunc_tf32(float x) { return __uint_as_float(__float_as_uint(x) & 0xffffe000u); }
 
-// Converter warps (split form): for a landed fp32 region [begin, end) of a raw stage (16-byte units, any swizzle -- the
-// pass is elementwise) write lo = rna_tf32(x - trunc_tf32(x)) to the same offsets of the lo buffer. The raw tile itself is
-// the hi operand (see trunc_tf32): it is not rewritten. x - trunc_tf32(x) is exact in fp32 (13 significant bits), so
-// hi + lo carries 22 significand bits of x. Four units per thread are loaded before the first is processed.
-__device__ __forceinline__ void split_region(const uint8_t* raw, uint8_t* lo, int begin, int end, int ctid, int n_conv) {
+// Split pass (fp32 form): for a landed fp32 region [begin, end) of a raw stage (16-byte units, any swizzle -- the pass
+// is elementwise) write hi = trunc_tf32(x) in place and lo = rna_tf32(x - hi) to the same offsets of the lo buffer.
+// Both are exact tf32 values, so the product does not depend on how the tensor core reads the low 13 bits of a
+// container. x - trunc_tf32(x) is exact in fp32 (13 significant bits), so hi + lo carries 22 significand bits of x.
+// Four units per thread are loaded before the first is processed.
+__device__ __forceinline__ void split_region(uint8_t* raw, uint8_t* lo, int begin, int end, int ctid, int n_conv) {
   const int stride = n_conv * 16;
   for (int off = begin + ctid * 16; off < end; off += 4 * stride) {
     float4 x[4];
@@ -234,12 +225,24 @@ __device__ __forceinline__ void split_region(const uint8_t* raw, uint8_t* lo, in
 #pragma unroll
     for (int u = 0; u < 4; ++u)
       if (off + u * stride < end) {
-        float4 l;
-        l.x = rna_tf32(x[u].x - trunc_tf32(x[u].x)); l.y = rna_tf32(x[u].y - trunc_tf32(x[u].y));
-        l.z = rna_tf32(x[u].z - trunc_tf32(x[u].z)); l.w = rna_tf32(x[u].w - trunc_tf32(x[u].w));
+        float4 h, l;
+        h.x = trunc_tf32(x[u].x); h.y = trunc_tf32(x[u].y); h.z = trunc_tf32(x[u].z); h.w = trunc_tf32(x[u].w);
+        l.x = rna_tf32(x[u].x - h.x); l.y = rna_tf32(x[u].y - h.y);
+        l.z = rna_tf32(x[u].z - h.z); l.w = rna_tf32(x[u].w - h.w);
+        *reinterpret_cast<float4*>(raw + off + u * stride) = h;
         *reinterpret_cast<float4*>(lo + off + u * stride) = l;
       }
   }
+}
+
+// One 64-wide K chunk of 16-bit operands: 4 x wgmma.m64n80k16, committed and waited for as one group.
+template <bool kBf16>
+__device__ __forceinline__ void wgmma_chunk_16bit(Frag& d, uint32_t a_src, uint32_t k_src) {
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < 4; ++k) wgmma_16bit<kBf16>(d, wgmma_desc_sw128(a_src + 32 * k), wgmma_desc_sw128(k_src + 32 * k));
+  wgmma_commit();
+  wgmma_wait0();
 }
 
 __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
@@ -247,7 +250,7 @@ __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wa
 // kChunked: some layer of the launch has head_dim > 64 (several K chunks per tile); the common single-chunk case keeps
 // its simpler loops (one load iteration per tile).
 template <bool kSplit, bool kChunked>
-__global__ void __launch_bounds__(kSplit ? kSplitThreads : kThreads, kSplit ? 1 : 2)
+__global__ void __launch_bounds__(kThreads, kSplit ? 1 : 2)
 accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
   constexpr int kStageBytesT = kSplit ? kSplitStageBytes : kStageBytes;
   constexpr int kOperandBytes = (kSplit ? kStages + 1 : kStages) * kStageBytesT;     // stages (+ the lo buffer)
@@ -258,10 +261,8 @@ accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
   uint8_t* gen = smem_raw + (base - raw);
   float* sP = reinterpret_cast<float*>(gen + kOperandBytes);
   const uint32_t sP_u32 = base + kOperandBytes;
-  const uint32_t bars = sP_u32 + kPBytes;                             // 10 mbarriers + the TMEM base address
-  const uint32_t full0 = bars, empty0 = bars + 16, tfull0 = bars + 32, tempty0 = bars + 48;
-  const uint32_t lofull = bars + 64, loempty = bars + 72;             // split form: the lo buffer's hand-off
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(gen + kOperandBytes + kPBytes + 128);
+  const uint32_t bars = sP_u32 + kPBytes;                             // 4 mbarriers
+  const uint32_t full0 = bars, empty0 = bars + 16;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int first, count;
@@ -278,25 +279,12 @@ accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
 #pragma unroll
     for (int s = 0; s < kStages; ++s) {
       mbar_init(full0 + 8 * s, 1);
-      mbar_init(empty0 + 8 * s, 1);
+      mbar_init(empty0 + 8 * s, kConsumers / 32);    // one arrival per consumer warp
     }
-#pragma unroll
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull0 + 8 * a, 1);
-      mbar_init(tempty0 + 8 * a, 4);       // one arrival per epilogue warp
-    }
-    mbar_init(lofull, (kSplitThreads - 192) / 32);  // one arrival per converter warp
-    mbar_init(loempty, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 5) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "n"(kTmemCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  // descriptor fetches of the first tile overlap the barrier / TMEM set-up (and, under PDL, the previous kernel's tail)
-  if (count > 0 && lane == 0 && (warp == 0 || warp == 4)) {
+  // descriptor fetches of the first tile overlap the barrier set-up (and, under PDL, the previous kernel's tail)
+  if (count > 0 && lane == 0 && (warp == 0 || warp == 8)) {
     int li0 = 0;
     const Tile t0 = decode_tile(P, first, li0);
     if (warp == 0) {
@@ -306,11 +294,8 @@ accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
       prefetch_tensormap(&MP.kmap[t0.li]);
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  // Programmatic dependent launch: everything above (barrier init, TMEM allocation) may overlap the tail of the
+  // Programmatic dependent launch: everything above (barrier init, descriptor prefetch) may overlap the tail of the
   // previous kernel on the stream. By default nothing below starts before that kernel has completed and flushed.
   // With `early_loads` (the caller vouches that Q/K were complete before the previous kernel started, DAAM_ACC_EARLY_LOADS)
   // only the accumulator updates wait: loads, MMAs and the first tiles' softmax overlap the previous kernel's tail.
@@ -318,29 +303,7 @@ accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
   if (!P.early_loads) griddep_wait();
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
-  if (kSplit && warp >= 6) {
-    // ===== converter warps (fp32 projections): landed fp32 tile -> hi (in place) + lo (second buffer) =====
-    const int ctid = threadIdx.x - 192, n_conv = kSplitThreads - 192;
-    uint8_t* lo = gen + kStages * kStageBytesT;
-    int li = 0, j = 0;
-    for (int i = 0; i < count; ++i) {
-      const Tile t = decode_tile(P, first + i, li);
-      const LayerParams& L = P.layer[t.li];
-      const int n_chunks = kChunked ? (L.head_dim + 63) >> 6 : 1;
-      for (int c = 0; c < n_chunks; ++c, ++j) {
-        const int s = j % kStages;
-        const int subs = (L.head_dim - 64 * c) > 32 ? 2 : 1;           // live 32-float sub-tiles of this chunk
-        mbar_wait(full0 + 8 * s, (uint32_t)(j / kStages) & 1u);         // TMA has landed the raw tiles
-        mbar_wait(loempty, ((uint32_t)j & 1u) ^ 1u);                   // the MMAs of the previous chunk have read lo
-        uint8_t* stage = gen + s * kStageBytesT;
-        split_region(stage, lo, 0, subs * kQBytes, ctid, n_conv);
-        split_region(stage, lo, 2 * kQBytes, 2 * kQBytes + subs * kKBytes, ctid, n_conv);
-        fence_proxy_async();                           // generic-proxy stores -> visible to the tensor core's reads
-        __syncwarp();
-        if (lane == 0) mbar_arrive(lofull);
-      }
-    }
-  } else if (warp == 4) {
+  if (warp == 8) {
     // ===== TMA producer =====
     if (lane == 0) {
       int li = 0, j = 0;
@@ -352,16 +315,13 @@ accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
           const uint32_t ph = (uint32_t)(j / kStages) & 1u;
           mbar_wait(empty0 + 8 * s, ph ^ 1u);
           const uint32_t q_dst = base + s * kStageBytesT;
-          if constexpr (kSplit) {                      // fp32: up to two 32-float-wide boxes per operand
-            const bool two = (P.layer[t.li].head_dim - 64 * c) > 32;    // the second sub-tile has live columns
-            const uint32_t k_dst = q_dst + 2 * kQBytes;
-            mbar_expect_tx(full0 + 8 * s, two ? kStageBytesT : kStageBytes);
+          if constexpr (kSplit) {                      // fp32: two 32-float-wide boxes per operand
+            const uint32_t k_dst = q_dst + 2 * kQBytes;          // (a box wholly beyond head_dim lands as zeros)
+            mbar_expect_tx(full0 + 8 * s, kStageBytesT);
             tma_load_4d(&MP.qmap[t.li], full0 + 8 * s, q_dst, 64 * c, t.head, t.pixel0, t.prompt);
             tma_load_4d(&MP.kmap[t.li], full0 + 8 * s, k_dst, 64 * c, t.head, 0, t.prompt);
-            if (two) {
-              tma_load_4d(&MP.qmap[t.li], full0 + 8 * s, q_dst + kQBytes, 64 * c + 32, t.head, t.pixel0, t.prompt);
-              tma_load_4d(&MP.kmap[t.li], full0 + 8 * s, k_dst + kKBytes, 64 * c + 32, t.head, 0, t.prompt);
-            }
+            tma_load_4d(&MP.qmap[t.li], full0 + 8 * s, q_dst + kQBytes, 64 * c + 32, t.head, t.pixel0, t.prompt);
+            tma_load_4d(&MP.kmap[t.li], full0 + 8 * s, k_dst + kKBytes, 64 * c + 32, t.head, 0, t.prompt);
           } else {
             const uint32_t k_dst = q_dst + kQBytes;
             mbar_expect_tx(full0 + 8 * s, kStageBytes);
@@ -371,128 +331,138 @@ accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
         }
       }
     }
-  } else if (warp == 5) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      int li = 0, j = 0;
-      for (int i = 0; i < count; ++i) {
-        const Tile t = decode_tile(P, first + i, li);
-        const LayerParams& L = P.layer[t.li];
-        const int a = i & 1;
-        const uint32_t aph = (uint32_t)(i >> 1) & 1u;
-        const int n_chunks = kChunked ? (L.head_dim + 63) >> 6 : 1;
-        const uint32_t d_tmem = tmem_base + a * kAccCols;
-        mbar_wait(tempty0 + 8 * a, aph ^ 1u);          // epilogue has drained this accumulator
-        for (int c = 0; c < n_chunks; ++c, ++j) {
-          const int s = j % kStages;
-          const uint32_t ph = (uint32_t)(j / kStages) & 1u;
-          const uint32_t q_src = base + s * kStageBytesT;
-          const int cols = min(64, L.head_dim - 64 * c);
-          if constexpr (kSplit) {
-            mbar_wait(lofull, (uint32_t)j & 1u);       // hi (in place) and lo are written (implies the TMA has landed)
-            tc_fence_after();
-            // q.k = q_lo.k_hi + q_hi.k_lo + q_hi.k_hi, smallest first; K = 8 floats = 32 bytes per instruction
-            const int k_steps = (cols + 7) >> 3;
-            const uint32_t q_lo = base + kStages * kStageBytesT, idesc = umma_idesc_tf32();
-            const uint32_t qa[3] = {q_lo, q_src, q_src};
-            const uint32_t kb[3] = {q_src + 2 * kQBytes, q_lo + 2 * kQBytes, q_src + 2 * kQBytes};
-#pragma unroll
-            for (int p = 0; p < 3; ++p)
-#pragma unroll
-              for (int k = 0; k < 8; ++k)
-                if (k < k_steps)
-                  umma_tf32(d_tmem, umma_desc_sw128(qa[p] + (k >> 2) * kQBytes + 32 * (k & 3)),
-                            umma_desc_sw128(kb[p] + (k >> 2) * kKBytes + 32 * (k & 3)), idesc, (c | p | k) != 0);
-            umma_commit(loempty);                      // frees the lo buffer ...
-          } else {
-            mbar_wait(full0 + 8 * s, ph);              // the chunk's operand tiles have landed
-            tc_fence_after();
-            const int k_steps = (cols + 15) >> 4;      // UMMA_K 16 = 32 bytes along the swizzled row
-            const uint32_t k_src = q_src + kQBytes;
-            const uint32_t idesc = umma_idesc(L.dtype == DAAM_BF16);
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              if (k < k_steps)
-                umma_f16(d_tmem, umma_desc_sw128(q_src + 32 * k), umma_desc_sw128(k_src + 32 * k), idesc, (c | k) != 0);
-          }
-          umma_commit(empty0 + 8 * s);                 // ... and the smem stage once the MMAs have read them
-        }
-        umma_commit(tfull0 + 8 * a);                   // accumulator ready for the epilogue
-      }
-    }
-  } else if (warp < 4) {
-    // ===== epilogue warps: softmax + accumulate =====
-    int li = 0;
-    const int tid = threadIdx.x;                       // 0..127 == pixel within the tile == TMEM lane
+  } else {
+    // ===== consumer warpgroups: MMA + softmax + accumulate =====
+    const int tid = threadIdx.x;                       // 0..255
+    const int wg = warp >> 2;                          // pixel rows 64 wg .. 64 wg + 63 of the tile
+    const int quad = lane & 3;
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);            // this thread's rows: r0 and r0 + 8
+    int li = 0, j = 0;
     bool issued = false;
     for (int i = 0; i < count; ++i) {
       const Tile t = decode_tile(P, first + i, li);
       const LayerParams& L = P.layer[t.li];
-      const int a = i & 1;
-      const uint32_t aph = (uint32_t)(i >> 1) & 1u;
-      mbar_wait(tfull0 + 8 * a, aph);
-      tc_fence_after();
-      float v[kTokensPad];
-      const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + a * kAccCols;
+      const int n_chunks = kChunked ? (L.head_dim + 63) >> 6 : 1;
+      Frag d;
 #pragma unroll
-      for (int c = 0; c < kTokensPad / 16; ++c) tmem_ld16(taddr + c * 16, v + c * 16);
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty0 + 8 * a);
-
-      float m = v[0];
+      for (int e = 0; e < 40; ++e) d[e] = 0.f;
+      for (int c = 0; c < n_chunks; ++c, ++j) {
+        const int s = j % kStages;
+        mbar_wait(full0 + 8 * s, (uint32_t)(j / kStages) & 1u);        // the chunk's operand tiles have landed
+        const uint32_t q_src = base + s * kStageBytesT;
+        frag_fence(d);
+        if constexpr (kSplit) {
+          uint8_t* stage = gen + s * kStageBytesT;
+          uint8_t* lo = gen + kStages * kStageBytesT;
+          consumer_barrier();                          // both warpgroups' MMAs of the previous chunk have read lo
+          split_region(stage, lo, 0, kSplitStageBytes, tid, kConsumers);
+          fence_proxy_async();                         // generic-proxy stores -> visible to the tensor core's reads
+          consumer_barrier();
+          wgmma_fence();
+          // q.k = q_lo.k_hi + q_hi.k_lo + q_hi.k_hi, smallest first; K = 8 floats = 32 bytes per instruction. Columns
+          // beyond head_dim are zeros in both buffers, so all 24 MMAs run: the compiler serialises a wgmma that sits
+          // behind a per-thread condition.
+          const uint32_t q_lo = base + kStages * kStageBytesT;
+          const uint32_t qa[3] = {q_lo, q_src, q_src};
+          const uint32_t kb[3] = {q_src + 2 * kQBytes, q_lo + 2 * kQBytes, q_src + 2 * kQBytes};
 #pragma unroll
-      for (int j = 1; j < kTokens; ++j) m = fmaxf(m, v[j]);
-      const float c = L.scale_log2e, mc = m * c;
-      float sum = 0.f;
+          for (int p = 0; p < 3; ++p)
 #pragma unroll
-      for (int j = 0; j < kTokens; ++j) {
-        v[j] = fast_exp2(fmaf(v[j], c, -mc));
-        sum += v[j];
+            for (int k = 0; k < 8; ++k)
+              wgmma_tf32(d, wgmma_desc_sw128(qa[p] + (k >> 2) * kQBytes + wg * 64 * 128 + 32 * (k & 3)),
+                         wgmma_desc_sw128(kb[p] + (k >> 2) * kKBytes + 32 * (k & 3)));
+          wgmma_commit();
+          wgmma_wait0();
+        } else {
+          // K 16 = 32 bytes along the swizzled row; columns beyond head_dim are zero-filled by TMA
+          const uint32_t a_src = q_src + wg * 64 * 128, k_src = q_src + kQBytes;
+          if (L.dtype == DAAM_BF16)
+            wgmma_chunk_16bit<true>(d, a_src, k_src);
+          else
+            wgmma_chunk_16bit<false>(d, a_src, k_src);
+        }
+        frag_fence(d);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty0 + 8 * s);    // this warp is done with the stage
       }
-      const float inv = 1.0f / sum;
+
+      // softmax over the 77 live columns of rows r0 (d[4j], d[4j+1]) and r0 + 8 (d[4j+2], d[4j+3]); columns 77..79
+      // (zero-filled token rows) sit in j = 9 of quads 2 (odd column) and 3
+      float m0 = d[0], m1 = d[2];
+#pragma unroll
+      for (int jj = 0; jj < 10; ++jj) {
+        const bool l0 = jj < 9 || quad <= 2, l1 = jj < 9 || quad < 2;   // column 8jj+2q (+1) < 77
+        if (l0) { m0 = fmaxf(m0, d[4 * jj]); m1 = fmaxf(m1, d[4 * jj + 2]); }
+        if (l1) { m0 = fmaxf(m0, d[4 * jj + 1]); m1 = fmaxf(m1, d[4 * jj + 3]); }
+      }
+      m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 1));
+      m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 2));
+      m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 1));
+      m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
+      const float sc = L.scale_log2e, mc0 = m0 * sc, mc1 = m1 * sc;
+      float sum0 = 0.f, sum1 = 0.f;
+#pragma unroll
+      for (int jj = 0; jj < 10; ++jj) {
+        const bool l0 = jj < 9 || quad <= 2, l1 = jj < 9 || quad < 2;
+        d[4 * jj] = l0 ? fast_exp2(fmaf(d[4 * jj], sc, -mc0)) : 0.f;
+        d[4 * jj + 2] = l0 ? fast_exp2(fmaf(d[4 * jj + 2], sc, -mc1)) : 0.f;
+        d[4 * jj + 1] = l1 ? fast_exp2(fmaf(d[4 * jj + 1], sc, -mc0)) : 0.f;
+        d[4 * jj + 3] = l1 ? fast_exp2(fmaf(d[4 * jj + 3], sc, -mc1)) : 0.f;
+        sum0 += d[4 * jj] + d[4 * jj + 1];
+        sum1 += d[4 * jj + 2] + d[4 * jj + 3];
+      }
+      sum0 += __shfl_xor_sync(0xffffffffu, sum0, 1);
+      sum0 += __shfl_xor_sync(0xffffffffu, sum0, 2);
+      sum1 += __shfl_xor_sync(0xffffffffu, sum1, 1);
+      sum1 += __shfl_xor_sync(0xffffffffu, sum1, 2);
+      const float inv0 = 1.0f / sum0, inv1 = 1.0f / sum1;
       // the first accumulator update of this CTA: everything the previous kernel added must be complete and visible
       if (i == 0 && P.early_loads) griddep_wait();
 
-      if (P.rmw_mode == 1) {
-        if (tid == 0 && issued) bulk_wait_read0();     // the previous reduce has finished reading sP
-        epi_barrier();
+      // stage the probabilities token-major: sP[token][pixel]. Quads 0-1 store row r0 while quads 2-3 store row r0 + 8
+      // (and then the other way round), so one store instruction touches 16 banks instead of 8.
+      if (tid == 0 && issued) bulk_wait_read0();       // the previous reduce has finished reading sP
+      consumer_barrier();                              // ... and (ldst mode) every thread has read the previous tile
+      const bool lowq = quad < 2;
 #pragma unroll
-        for (int j = 0; j < kTokens; ++j) sP[j * kTilePixels + tid] = v[j] * inv;
+      for (int jj = 0; jj < 10; ++jj) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int col = 8 * jj + 2 * quad + e;
+          if (col < kTokens) {
+            const float a = d[4 * jj + e] * inv0, b = d[4 * jj + 2 + e] * inv1;
+            sP[col * kTilePixels + (lowq ? r0 : r0 + 8)] = lowq ? a : b;
+            sP[col * kTilePixels + (lowq ? r0 + 8 : r0)] = lowq ? b : a;
+          }
+        }
+      }
+      if (P.rmw_mode == 1) {
         fence_proxy_async();                           // generic-proxy writes -> visible to the bulk-async proxy
-        epi_barrier();
+        consumer_barrier();
         if (tid == 0) {
           tma_reduce_add_2d(&MP.amap[t.li], sP_u32, t.pixel0, (t.prompt * L.heads + t.head) * kTokens);
           bulk_commit();
         }
         issued = true;
       } else {
-        const int pixel = t.pixel0 + tid;
-        if (pixel < L.hw) {
-          const long long hw = L.hw;
-          float* acc = L.acc + ((long long)(t.prompt * L.heads + t.head) * kTokens) * hw + pixel;
-          constexpr int kChunk = 11;
-#pragma unroll
-          for (int j0 = 0; j0 < kTokens; j0 += kChunk) {
-            float old[kChunk];
-#pragma unroll
-            for (int j = 0; j < kChunk; ++j) old[j] = acc[(j0 + j) * hw];
-#pragma unroll
-            for (int j = 0; j < kChunk; ++j) acc[(j0 + j) * hw] = fmaf(v[j0 + j], inv, old[j]);
+        consumer_barrier();
+        const long long hw = L.hw;
+        float* acc = L.acc + ((long long)(t.prompt * L.heads + t.head) * kTokens) * hw + t.pixel0;
+        const int live = min(kTilePixels, L.hw - t.pixel0) >> 2;       // float4 columns inside the map (hw % 4 == 0)
+        for (int u = tid; u < kTokens * (kTilePixels / 4); u += kConsumers) {
+          const int tok = u / (kTilePixels / 4), c4 = u % (kTilePixels / 4);
+          if (c4 < live) {
+            float4* g = reinterpret_cast<float4*>(acc + tok * hw) + c4;
+            const float4 p = reinterpret_cast<const float4*>(sP + tok * kTilePixels)[c4];
+            float4 o = *g;
+            o.x += p.x; o.y += p.y; o.z += p.z; o.w += p.w;
+            *g = o;
           }
         }
       }
     }
     // shared memory must outlive the reduce's reads; its global writes complete with the grid (same rule as a TMA store)
     if (tid == 0 && issued) bulk_wait_read0();
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    __syncwarp();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(kTmemCols) : "memory");
   }
 }
 
@@ -598,7 +568,7 @@ std::once_flag g_attr_once[64];                       // the shared-memory attri
 
 }  // namespace
 
-// Parameter block of one tcgen05 launch, opaque to api.cu (which caches prepared launches by their daam_layer[] input).
+// Parameter block of one wgmma launch, opaque to api.cu (which caches prepared launches by their daam_layer[] input).
 struct PreparedMma {
   MmaParams mp;
   int grid, block, smem, variant;                     // variant: bit 0 split (fp32), bit 1 chunked (head_dim > 64)
@@ -613,7 +583,7 @@ bool mma_supported(const LayerParams& L) {
 
 // Tensor maps, grid and kernel variant of one pack of layers (all fp32, or all 16-bit). `out`: prepared_mma_new().
 int prepare_accumulate_mma(const LaunchParams& p, const DeviceInfo& dev, void* out) {
-  if (dev.cc_major != 10) { set_error("the tcgen05 kernel needs an sm_100 device (found sm_%d%d)", dev.cc_major, dev.cc_minor); return DAAM_E_UNSUPPORTED; }
+  if (dev.cc_major != 9) { set_error("the wgmma kernel needs an sm_90 device (found sm_%d%d)", dev.cc_major, dev.cc_minor); return DAAM_E_UNSUPPORTED; }
   PreparedMma& pm = *static_cast<PreparedMma*>(out);
   MmaParams& mp = pm.mp;
   mp.base = p;
@@ -621,7 +591,7 @@ int prepare_accumulate_mma(const LaunchParams& p, const DeviceInfo& dev, void* o
   bool chunked = false;
   for (int i = 0; i < p.n_layers; ++i) {
     const LayerParams& L = p.layer[i];
-    if ((L.dtype == DAAM_F32) != split) { set_error("mixed fp32 / 16-bit layers in one tcgen05 pack"); return DAAM_E_INVALID; }
+    if ((L.dtype == DAAM_F32) != split) { set_error("mixed fp32 / 16-bit layers in one wgmma pack"); return DAAM_E_INVALID; }
     if (int rc = make_qk_map(L.q, L.dtype, L.head_dim, L.heads, L.hw, L.n_prompts, L.qs_head, L.qs_pixel, L.qs_prompt, kTilePixels, &mp.qmap[i])) return rc;
     if (int rc = make_qk_map(L.k, L.dtype, L.head_dim, L.heads, kTokens, L.n_prompts, L.ks_head, L.ks_token, L.ks_prompt, kTokensPad, &mp.kmap[i])) return rc;
     if (int rc = make_acc_map(L.acc, L.hw, L.n_prompts * L.heads * kTokens, &mp.amap[i])) return rc;
@@ -641,7 +611,7 @@ int prepare_accumulate_mma(const LaunchParams& p, const DeviceInfo& dev, void* o
   DAAM_CUDA_TRY(attr_err);
   pm.grid = dev.sm_count * (split ? 1 : 2);
   if (pm.grid > p.total_tiles) pm.grid = p.total_tiles;
-  pm.block = split ? kSplitThreads : kThreads;
+  pm.block = kThreads;
   pm.smem = split ? kSplitSmemBytes : kSmemBytes;
   pm.variant = (split ? 1 : 0) | (chunked ? 2 : 0);
   return DAAM_OK;

@@ -1,7 +1,7 @@
 // Fused softmax(QK^T) -> unravel -> accumulate, SIMT fp32 variant ("warp dot" path).
 //
 // Serves fp32 projections (BASELINE config 1: the reference's own fp32 numerics, which tensor cores cannot give)
-// and every head_dim the tcgen05 variant does not take (SD-1.x: 40/80/160). One thread owns one pixel: its 77
+// and every layer the wgmma variant does not take (unaligned rows). One thread owns one pixel: its 77
 // logits live in registers, K^T sits in shared memory and is read as warp-wide broadcasts, so softmax needs no
 // shuffles and the accumulator update `acc[t][pixel] += p[t]` is one fully coalesced 128-byte access per warp and
 // token. Replaces daam/trace.py:276 (get_attention_scores), :219-244 (_unravel_attn) and :293-294 (update loop).

@@ -88,14 +88,14 @@ using namespace daam;
 namespace daam {
 namespace {
 
-// One kernel launch of a plan: a pack of layers for the tcgen05 kernel (prepared block, opaque) or the SIMT kernel.
+// One kernel launch of a plan: a pack of layers for the wgmma kernel (prepared block, opaque) or the SIMT kernel.
 struct PlannedLaunch {
   bool is_mma = false;
   LaunchParams simt;                     // SIMT: the parameter block itself
   int grid = 0;
   size_t smem = 0;
   struct MmaDeleter { void operator()(void* p) const { prepared_mma_delete(p); } };
-  std::unique_ptr<void, MmaDeleter> mma; // tcgen05: PreparedMma (tensor maps + parameter block), opaque here
+  std::unique_ptr<void, MmaDeleter> mma; // wgmma: PreparedMma (tensor maps + parameter block), opaque here
 };
 
 // Everything daam_accumulate derives from its input: the packs, their tensor maps, grids. A trace replays the same
@@ -112,9 +112,9 @@ constexpr size_t kMaxPlans = 32;
 
 int build_plan(const daam_layer* layers, int n_layers, uint32_t flags, const DeviceInfo& dev, Plan* plan) {
   const uint32_t path = flags & 3u, rmw = flags & DAAM_ACC_RMW_MASK;
-  // Three packs: 16-bit layers for the tcgen05 kernel (TMA form), fp32 layers for its split form, and the rest for
+  // Three packs: 16-bit layers for the wgmma kernel (TMA form), fp32 layers for its split form, and the rest for
   // the SIMT kernel. Each is closed when its parameter block is full.
-  LaunchParams packs[3];                 // 0: tcgen05 16-bit, 1: tcgen05 fp32, 2: SIMT
+  LaunchParams packs[3];                 // 0: wgmma 16-bit, 1: wgmma fp32, 2: SIMT
   for (LaunchParams& p : packs) {
     p.n_layers = p.total_tiles = 0;
     p.rmw_mode = (rmw == DAAM_ACC_RMW_LDST) ? 0 : 1;     // default: reduce-add
@@ -123,7 +123,7 @@ int build_plan(const daam_layer* layers, int n_layers, uint32_t flags, const Dev
     p.total_weight = 0;
   }
   // The fp32 split form holds a whole SM per CTA (196 KB of shared memory): its CTAs only become resident as the previous
-  // launch's CTAs exit, and early loads measured 2.6 % slower than waiting at the top (31.6 vs 30.8 us per SD-2.1 step).
+  // launch's CTAs exit, so there is no tail to overlap and its loads wait at the top.
   packs[1].early_loads = 0;
   auto close = [&](int which) -> int {
     LaunchParams& p = packs[which];
@@ -147,20 +147,19 @@ int build_plan(const daam_layer* layers, int n_layers, uint32_t flags, const Dev
   for (int i = 0; i < n_layers; ++i) {
     LayerParams L;
     if (int rc = make_layer_params(layers[i], i, &L, /*need_acc=*/true)) return rc;
-    const bool use_mma = path != DAAM_ACC_FORCE_SIMT && dev.cc_major == 10 && mma_supported(L);
+    const bool use_mma = path != DAAM_ACC_FORCE_SIMT && dev.cc_major == 9 && mma_supported(L);
     if (path == DAAM_ACC_FORCE_MMA && !use_mma) {
-      set_error("daam_accumulate: layer %d cannot take the tcgen05 path (dtype %d, head_dim %d, alignment %d, sm_%d%d)", i,
+      set_error("daam_accumulate: layer %d cannot take the wgmma path (dtype %d, head_dim %d, alignment %d, sm_%d%d)", i,
                 L.dtype, L.head_dim, L.vec_ok, dev.cc_major, dev.cc_minor);
       return DAAM_E_UNSUPPORTED;
     }
     const int which = use_mma ? (L.dtype == DAAM_F32 ? 1 : 0) : 2;
     LaunchParams& p = packs[which];
     L.tile_begin = p.total_tiles;
-    // Cost of a tile relative to the launch's other layers, measured on SD-1.5's 40 / 80 / 160 head dims
-    // (profiles/r02_microbench_experiments.json, "weight A+B*chunks"): every 64-wide K chunk is one load -> (convert ->)
-    // MMA round through the two-stage ring. In the fp32 split form that chain is the whole cost of a tile (weight =
-    // chunks; any constant term measured slower); in the 16-bit form 1 + 4 * chunks did best at 1-2 prompts per launch
-    // (0.80 vs 0.73 for 2 + chunks) and the same as every other model at 8.
+    // Cost of a tile relative to the launch's other layers (SD-1.5's 40 / 80 / 160 head dims): every 64-wide K chunk is
+    // one load -> (convert ->) MMA round through the two-stage ring. In the fp32 split form that chain is the whole cost
+    // of a tile (weight = chunks); in the 16-bit form the softmax and accumulator update of the tile add a fixed part
+    // (weight = 1 + 4 * chunks).
     const int n_chunks = (L.head_dim + 63) / 64;
     L.weight = which == 1 ? n_chunks : 1 + 4 * n_chunks;
     L.weight_begin = p.total_weight;

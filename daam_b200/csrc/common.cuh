@@ -28,7 +28,7 @@ struct LayerParams {
   int tiles_per_head;       // ceil(hw / kTilePixels)
   int tile_begin;
   int vec_ok;               // 1: q/k rows are 16-byte aligned -> vector loads
-  int weight;               // relative cost of one tile of this layer (tcgen05 kernel, K-chunked launches)
+  int weight;               // relative cost of one tile of this layer (wgmma kernel, K-chunked launches)
   int weight_begin;         // exclusive prefix of tiles x weight over the launch's layers
   int pad_;
 };

@@ -1,4 +1,4 @@
-"""Mask overlap measures of the reference's evaluation helpers (``/root/reference/daam/evaluate.py:14-35``).
+"""Mask overlap measures of the reference's evaluation helpers (``daam/evaluate.py:14-35``).
 
 Only ``compute_iou`` / ``compute_ioa`` are mirrored -- the part of SURVEY.md section 8f rank 4 that touches heat maps.
 When the two masks differ in size the reference bicubically resizes the first to the second and binarises it at 1;

@@ -1,6 +1,6 @@
 """On-disk record of one generation: image + global heat map + prompt (SURVEY.md section 8f, rank 3).
 
-A reduced mirror of the reference's ``GenerationExperiment`` (``/root/reference/daam/experiment.py:102-344``): the same
+A reduced mirror of the reference's ``GenerationExperiment`` (``daam/experiment.py:102-344``): the same
 fields and the same folder layout -- ``<path>/<id>/<subtype>/generation.pt`` (the pickled dataclass), ``output.png``,
 ``<path>/<id>/prompt.txt``, ``seed.txt``, ``annotations.json`` (experiment.py:140-175). Compatibility is ONE-WAY: dumps
 written by the reference load here (``load`` maps its pickled class path ``daam.experiment.GenerationExperiment`` onto

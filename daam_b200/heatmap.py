@@ -1,6 +1,6 @@
 """Heat-map store and algebra: the accumulator slabs the CUDA kernel sums into, and the global / word heat maps.
 
-Mirror of the reference's L2 (``/root/reference/daam/heatmap.py``) for the hot-path rows of SURVEY.md section 8a:
+Mirror of the reference's L2 (``daam/heatmap.py``) for the hot-path rows of SURVEY.md section 8a:
 
 * :class:`RawHeatMapCollection` (heatmap.py:148-172) -- same interface (``update``, ``factors``, ``layers``, ``heads``,
   iteration over ``((factor, layer, head), tensor[77, h, w])``, ``clear``), but backed by one fp32 device slab per traced

@@ -1,4 +1,4 @@
-"""Context-managed monkey patching (the reference's L0, ``/root/reference/daam/hook.py:22-86``).
+"""Context-managed monkey patching (the reference's L0, ``daam/hook.py:22-86``).
 
 ``ObjectHooker`` wraps one object: ``hook()`` runs the subclass' ``_hook_impl`` (which typically calls
 ``monkey_patch``), ``unhook()`` puts every replaced attribute back and runs ``_unhook_impl``; both are also reachable

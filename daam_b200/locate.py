@@ -1,7 +1,7 @@
 """Enumeration of a UNet's cross-attention layers in the order that defines ``layer_idx``.
 
 The tracer's layer indices, and therefore every ``(factor, layer, head)`` key, follow the reference's walk
-(``/root/reference/daam/hook.py:95-127``): the ``up_blocks`` come first, then the ``down_blocks``, then -- only when
+(the reference's ``daam/hook.py:95-127``): the ``up_blocks`` come first, then the ``down_blocks``, then -- only when
 asked -- the ``mid_block``; inside a block whose class name contains ``CrossAttn`` every
 ``attentions[*].transformer_blocks[*].attn2`` is taken in module order. Names restart at 0 in every block
 (``up-attn-0`` occurs once per up block), exactly like the reference's.

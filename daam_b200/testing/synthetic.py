@@ -2,7 +2,7 @@
 
 ``diffusers`` is not installed on either box and there is no network, so the benchmark and the tests run
 on plain-torch modules that expose exactly the surface the reference touches
-(``/root/reference/daam/trace.py:252-311``, ``/root/reference/daam/hook.py:95-127``):
+(the reference's ``daam/trace.py:252-311``, ``daam/hook.py:95-127``):
 
 * :class:`SyntheticAttention` -- the ``diffusers==0.21.2`` ``Attention`` module surface: ``to_q/to_k/to_v/to_out``,
   ``heads``, ``scale``, ``norm_cross``, ``upcast_attention``, ``upcast_softmax``, ``processor``/``set_processor`` and the

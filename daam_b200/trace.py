@@ -1,6 +1,6 @@
-"""The tracer: ``with trace(pipe) as tc: pipe(prompt); tc.compute_global_heat_map()`` on B200-native kernels.
+"""The tracer: ``with trace(pipe) as tc: pipe(prompt); tc.compute_global_heat_map()`` on H100-native kernels.
 
-Mirror of the reference's L1 (``/root/reference/daam/trace.py``): same classes, constructor arguments, methods and
+Mirror of the reference's L1 (``daam/trace.py``): same classes, constructor arguments, methods and
 exceptions; what differs is what runs underneath.
 
 * The attention processor (:class:`UNetCrossAttentionHooker`, reference trace.py:189-315) owns the whole attn2 forward

@@ -1,4 +1,4 @@
-"""Small helpers kept from the reference's API surface (``/root/reference/daam/utils.py``): seeding, device/autocast
+"""Small helpers kept from the reference's API surface (``daam/utils.py``): seeding, device/autocast
 shims and the word -> token-row lookup (``compute_token_merge_indices``, utils.py:73-91). spaCy and plotting helpers
 are out of scope (SURVEY.md section 2, rows 4)."""
 from __future__ import annotations

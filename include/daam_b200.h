@@ -1,7 +1,7 @@
 /*
- * daam_b200.h -- C ABI of libdaam_b200.so: the B200 (sm_100a) cross-attention heat-map hot path.
+ * daam_b200.h -- C ABI of libdaam_b200.so: the H100 (sm_90a) cross-attention heat-map hot path.
  *
- * The reference (castorini/daam, paths below relative to /root/reference) is pure Python/torch and has no FFI. The
+ * The reference (castorini/daam, paths below relative to its checkout) is pure Python/torch and has no FFI. The
  * entry points here are what a binding for its hot path replaces; each one cites the reference interface it stands
  * in for. INTEGRATION.md shows the ctypes stub a maintainer of the reference would add.
  *
@@ -39,13 +39,13 @@ enum daam_status {
 enum daam_dtype { DAAM_F32 = 0, DAAM_F16 = 1, DAAM_BF16 = 2 };
 
 /* daam_accumulate flags */
-#define DAAM_ACC_AUTO        0u  /* tcgen05 path whenever rows are 16-byte aligned (any dtype, head_dim % 8 == 0),
+#define DAAM_ACC_AUTO        0u  /* wgmma path whenever rows are 16-byte aligned (any dtype, head_dim % 8 == 0),
                                     SIMT fp32 path otherwise */
 #define DAAM_ACC_FORCE_SIMT  1u  /* always the SIMT fp32 ("warp dot") kernel */
-#define DAAM_ACC_FORCE_MMA   2u  /* tcgen05 kernel or DAAM_E_UNSUPPORTED */
+#define DAAM_ACC_FORCE_MMA   2u  /* wgmma kernel or DAAM_E_UNSUPPORTED */
 #define DAAM_ACC_RMW_MASK   0x30u
-#define DAAM_ACC_RMW_AUTO   0x00u /* = RED on both paths (measured faster; one add per element per launch, so
-                                     results stay deterministic) */
+#define DAAM_ACC_RMW_AUTO   0x00u /* = RED on both paths (one add per element per launch, so results stay
+                                     deterministic) */
 #define DAAM_ACC_RMW_LDST   0x10u /* coalesced load / add / store of the accumulator tile */
 #define DAAM_ACC_RMW_RED    0x20u /* red.global.add.f32 (SIMT) / bulk-async reduce-add from shared memory (MMA) */
 #define DAAM_ACC_NO_PDL     0x100u /* launch without programmatic dependent launch (measurement / debugging) */

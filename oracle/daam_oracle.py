@@ -5,10 +5,9 @@ Nothing in the product (``daam_b200/``) imports this file. Only ``tests/``, ``__
 baseline -- never as the thing shipped.
 
 Parity status: the reference holds no tests, golden vectors or fixtures for this path (SURVEY.md section 4 / section 8c), so
-the oracle is pinned the other way the task allows: against outputs of the reference itself. ``tests/
-test_oracle_vs_reference.py`` runs the *verbatim* reference (imported from ``/root/reference`` behind the stubs in
-``oracle/ref_loader.py``) and this restatement on identical seeded inputs and requires bit-equality on CPU fp32;
-``oracle/make_golden.py`` stores reference outputs as fixtures under ``tests/golden/`` that travel to the GPU box.
+the oracle is pinned against outputs of the reference itself: ``oracle/make_golden.py`` runs the *verbatim* reference
+(imported behind the stubs in ``oracle/ref_loader.py``) on seeded inputs and stores its outputs under ``tests/golden/``;
+``tests/test_oracle_vs_reference.py`` requires this restatement to reproduce them bit for bit on CPU fp32.
 
 Two layers live here:
 
@@ -18,7 +17,7 @@ Two layers live here:
   and Keys' cubic-convolution weights), used to check the port's numerics and to bound the CUDA kernels' error.
 
 Row labels (a1..a10) are SURVEY.md section 8a; every function cites the reference lines it follows (paths relative to
-``/root/reference``).
+the reference checkout's root).
 """
 from __future__ import annotations
 

@@ -1,10 +1,11 @@
 """TEST INFRASTRUCTURE -- writes tests/golden/*.npz from the *verbatim* reference (run in the build container only).
 
-    python -m oracle.make_golden
+    DAAM_REFERENCE_ROOT=<castorini/daam checkout> python -m oracle.make_golden [vs_reference]
 
-The reference (a Python package) cannot travel to the GPU box, so its outputs do: each fixture stores seeded inputs
-and what ``/root/reference/daam`` itself computed from them on CPU fp32. ``tests/test_oracle_golden.py`` pins the
-oracle to these on every box; the ``-m gpu`` tests compare the CUDA path with the same files.
+The reference (a Python package) is not part of this repository, so its outputs are: each fixture stores seeded
+inputs and what the reference's ``daam`` package itself computed from them on CPU fp32 (one thread).
+``tests/test_oracle_golden.py`` and ``tests/test_oracle_vs_reference.py`` pin the oracle to these everywhere; the
+``-m gpu`` tests compare the CUDA path with the same files.
 
 Fixtures
   layer_*.npz        q [2, hw, H*d], k [2, 77, H*d] (fp16-representable values stored as fp16) and the maps
@@ -18,6 +19,9 @@ Fixtures
                      (96, 96) global maps from keys at 96^2 / 48^2 / 24^2.
   perkey.npz         the reference's --all-heads sweep (daam/run/generate.py:239-255) over finalize.npz's keys:
                      ``compute_global_heat_map(layer_idx=l, head_idx=h)`` for every key, plain and normalised.
+  vs_reference.npz   the rest of what tests/test_oracle_vs_reference.py compares with: exact fingerprints of the
+                     reference's per-key maps, save_heads files and --all-heads sweep, its error messages and merge
+                     indices, the _unravel_attn permutation, and the files of a GenerationExperiment dump it wrote.
 """
 from __future__ import annotations
 
@@ -162,17 +166,90 @@ def make_perkey_fixture(daam):
     print('perkey', plain.shape)
 
 
+def make_vs_reference_fixture(daam):
+    """What tests/test_oracle_vs_reference.py compares the oracle with, beyond pipeline_tiny*.npz: exact fingerprints
+    (tests.util.digest) of the reference's per-key maps, save_heads files and per-key sweep, its error messages, token
+    merge indices, the _unravel_attn permutation, and the files of a GenerationExperiment dump it wrote."""
+    import tempfile
+    import PIL.Image
+    from tests.util import digest
+    out = {}
+    torch.manual_seed(0)
+    pipe = make_pipeline(TINY_SPEC, dtype=torch.float32, seed=3)
+    with daam.trace(pipe) as tc:
+        pipe(PROMPT, num_inference_steps=2, generator=torch.Generator().manual_seed(11))
+        keys = [(k, v.clone()) for k, v in tc.all_heat_maps]
+    out['keys'] = np.array([k for k, _ in keys])
+    out['key_digests'] = np.stack([digest(v) for _, v in keys])
+    with daam.trace(pipe) as tc:
+        pipe(PROMPT, num_inference_steps=2, generator=torch.Generator().manual_seed(11))
+        sweep = [(f, l, h) for (f, l, h), _ in keys[::5]]
+        out['sweep_keys'] = np.array(sweep)
+        out['sweep_digests'] = np.stack([digest(tc.compute_global_heat_map(layer_idx=l, head_idx=h, normalize=True)
+                                                .heat_maps) for _, l, h in sweep])
+    with daam.trace(pipe) as tc:
+        try:
+            tc.compute_global_heat_map()
+        except RuntimeError as e:
+            out['empty_trace_error'] = str(e)
+    try:
+        daam.compute_token_merge_indices(pipe.tokenizer, PROMPT, 'zebra')
+    except ValueError as e:
+        out['missing_word_error'] = str(e)
+    for word in ['dog', 'red', 'beach']:
+        out[f'merge_{word}'] = repr(daam.compute_token_merge_indices(pipe.tokenizer, PROMPT, word))
+    out['merge_x_idx3'] = repr(daam.compute_token_merge_indices(pipe.tokenizer, PROMPT, 'x', word_idx=3))
+    hooker = daam.trace(pipe).module[0]
+    out['unravel_perm'] = hooker._unravel_attn(torch.arange(8 * 64 * 77, dtype=torch.float64)
+                                               .reshape(8, 64, 77)).numpy().astype(np.uint16)
+    with tempfile.TemporaryDirectory() as tmp:
+        pipe = make_pipeline(TINY_SPEC, dtype=torch.float32, seed=5)
+        gen = lambda: torch.Generator().manual_seed(2)
+        with daam.trace(pipe, save_heads=True, data_dir=tmp) as tc:
+            pipe(PROMPT, num_inference_steps=2, generator=gen())
+            out['saved_global'] = digest(tc.compute_global_heat_map().heat_maps)
+        names = sorted(os.listdir(tmp))
+        out['saved_names'] = np.array(names)
+        out['saved_digests'] = np.stack([digest(torch.load(os.path.join(tmp, n))) for n in names])
+        other = make_pipeline(TINY_SPEC, dtype=torch.float32, seed=6)
+        with daam.trace(other, load_heads=True, data_dir=tmp) as tc:
+            out['loaded_latents'] = digest(other(PROMPT, num_inference_steps=2, generator=gen()).latents)
+            out['loaded_global'] = digest(tc.compute_global_heat_map().heat_maps)
+    with tempfile.TemporaryDirectory() as tmp:
+        maps = torch.rand(6, 16, 16, generator=torch.Generator().manual_seed(4))
+        img = PIL.Image.new('RGB', (16, 16), (10, 20, 30))
+        daam.GenerationExperiment(img, maps, 'a red ball', seed=3, id='q1', path=tmp).save(heat_maps=False)
+        root = os.path.join(tmp, 'q1')
+        files = sorted(os.path.relpath(os.path.join(d, f), root) for d, _, fs in os.walk(root) for f in fs)
+        out['experiment_maps'] = maps.numpy()
+        out['experiment_files'] = np.array(files)
+        for i, f in enumerate(files):
+            with open(os.path.join(root, f), 'rb') as fh:
+                out[f'experiment_file_{i}'] = np.frombuffer(fh.read(), dtype=np.uint8)
+    pipe = make_pipeline(TINY96_SPEC, dtype=torch.float32, seed=5)
+    with daam.trace(pipe) as tc:
+        pipe(PROMPT, num_inference_steps=2, generator=torch.Generator().manual_seed(13))
+        out['keys96'] = np.array([k for k, _ in tc.all_heat_maps])
+        out['key96_digests'] = np.stack([digest(v) for _, v in tc.all_heat_maps])
+    np.savez_compressed(os.path.join(OUT, 'vs_reference.npz'), **out)
+    print('vs_reference', sorted(out))
+
+
 def main():
     warnings.filterwarnings('ignore', category=FutureWarning)
     os.makedirs(OUT, exist_ok=True)
     os.environ.setdefault('XDG_CACHE_HOME', '/tmp/daam_cache')
     torch.set_num_threads(1)   # fixtures must not depend on the thread count
     daam = load_reference()
+    if sys.argv[1:] == ['vs_reference']:
+        make_vs_reference_fixture(daam)
+        return
     make_layers(daam)
     make_finalize(daam)
     make_pipeline_fixture(daam)
     make_pipeline96_fixture(daam)
     make_perkey_fixture(daam)
+    make_vs_reference_fixture(daam)
 
 
 if __name__ == '__main__':

@@ -1,15 +1,14 @@
-"""TEST INFRASTRUCTURE -- imports the *verbatim* reference (castorini/daam) from ``/root/reference`` behind stubs.
+"""TEST INFRASTRUCTURE -- imports the *verbatim* reference (castorini/daam) from ``$DAAM_REFERENCE_ROOT`` behind stubs.
 
-The reference cannot be imported as-is in this container: ``diffusers``, ``matplotlib``, ``spacy`` (and friends) are
+The reference cannot be imported as-is in the build environment: ``diffusers``, ``matplotlib``, ``spacy`` (and friends) are
 not installed and there is no network (SURVEY.md section 8c). None of those packages contributes arithmetic to the hot path
 except ``diffusers.models.attention_processor.Attention``, whose 0.21.2 semantics ``daam_b200.testing.synthetic.
 SyntheticAttention`` restates. This loader registers empty stand-in modules for the missing imports, points
 ``diffusers...Attention`` at that restatement, and then imports ``daam`` from the read-only reference tree.
 
-It exists to (1) pin ``oracle/daam_oracle.py`` against the reference's own code and (2) generate the golden fixtures
-under ``tests/golden/`` (``oracle/make_golden.py``). ``/root/reference`` does not exist on the GPU box: everything
-that calls :func:`load_reference` must skip when :func:`reference_available` is false. Only ``tests/`` and the
-golden-vector generator may use this module; the product (``daam_b200``) never imports anything under ``oracle/``.
+It exists to generate the golden fixtures under ``tests/golden/`` (``oracle/make_golden.py``), which is how the suite
+pins ``oracle/daam_oracle.py`` against the reference's own code without needing the reference. Only the golden-vector
+generator may use this module; the product (``daam_b200``) never imports anything under ``oracle/``.
 """
 from __future__ import annotations
 
@@ -18,7 +17,7 @@ import os
 import sys
 import types
 
-REFERENCE_ROOT = os.environ.get('DAAM_REFERENCE_ROOT', '/root/reference')
+REFERENCE_ROOT = os.environ.get('DAAM_REFERENCE_ROOT', '')   # a castorini/daam v0.2.0 checkout
 
 
 def reference_available() -> bool:
@@ -61,7 +60,8 @@ def _install_stubs():
 def load_reference():
     """Returns the reference's ``daam`` package (verbatim code, stubbed third-party imports)."""
     if not reference_available():
-        raise RuntimeError(f'reference tree not found under {REFERENCE_ROOT}')
+        raise RuntimeError(f'reference tree not found under {REFERENCE_ROOT!r}: set DAAM_REFERENCE_ROOT to a castorini/daam '
+                           f'v0.2.0 checkout')
     repo_root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     if repo_root not in sys.path:
         sys.path.insert(0, repo_root)

@@ -25,10 +25,10 @@ PATHS = [
 
 
 def skip_unless_mma_applies(path, dtype, head_dim):
-    """The tcgen05 kernel takes every head_dim that is a multiple of 8 up to 192 (16-bit operands directly, fp32 as three
+    """The wgmma kernel takes every head_dim that is a multiple of 8 up to 192 (16-bit operands directly, fp32 as three
     bf16 terms, 64-wide K chunks); forcing it elsewhere is an error by design."""
     if path.startswith('mma') and (head_dim % 8 != 0 or head_dim > 192):
-        pytest.skip('tcgen05 path: head_dim multiple of 8, <= 192')
+        pytest.skip('wgmma path: head_dim multiple of 8, <= 192')
 
 
 def assert_close(got, ref, tol, what=''):
@@ -321,7 +321,7 @@ def test_empty_call_and_smallest_maps():
 @pytest.mark.parametrize('dtype', [torch.float16, torch.bfloat16, torch.float32])
 @pytest.mark.parametrize('hw,heads,d', [(4096, 8, 40), (1024, 8, 80), (256, 8, 160), (64, 4, 128), (1024, 4, 8)])
 def test_sd1x_head_dims_on_tensor_cores(hw, heads, d, dtype):
-    """SD-1.x head dims (40 / 80 / 160) and other multiples of 8: K-chunked tcgen05 path == SIMT path == oracle."""
+    """SD-1.x head dims (40 / 80 / 160) and other multiples of 8: K-chunked wgmma path == SIMT path == oracle."""
     g = torch.Generator().manual_seed(d * 7 + hw)
     q = torch.randn(2, hw, heads * d, generator=g).to(dtype).to(DEV)
     k = torch.randn(2, 77, heads * d, generator=g).to(dtype).to(DEV)

@@ -1,7 +1,9 @@
-"""Pins oracle/daam_oracle.py against the verbatim reference (imported from /root/reference behind stubs).
+"""Pins oracle/daam_oracle.py against the verbatim reference's own outputs, stored by oracle/make_golden.py.
 
-Skips where the reference tree is absent (the GPU box); tests/test_oracle_golden.py covers that case with the
-committed fixtures the reference produced here."""
+pipeline_tiny.npz / pipeline_tiny96.npz hold the reference's heat maps of the two generations below in full;
+vs_reference.npz holds exact fingerprints (tests.util.digest: float64 sum + a fixed sample of elements) of the
+per-key maps, the save_heads files and the per-key sweep, and the reference's strings, indices and experiment dump.
+Every comparison is exact."""
 import warnings
 
 import numpy as np
@@ -10,35 +12,36 @@ import torch
 
 from daam_b200.testing.synthetic import TINY_SPEC, make_pipeline
 from oracle import daam_oracle as O
-from oracle.ref_loader import load_reference, reference_available
+from tests.util import digest, golden
 
-pytestmark = pytest.mark.skipif(not reference_available(), reason='/root/reference not present')
 warnings.filterwarnings('ignore', category=FutureWarning)
 
 PROMPT = 'a dog chasing a red ball on the beach'
 
 
+@pytest.fixture(scope='module', autouse=True)
+def one_thread():
+    """The fixtures were computed on one thread (oracle/make_golden.py): the UNet's fp32 matmuls sum in a
+    thread-count-dependent order, and these comparisons are exact."""
+    before = torch.get_num_threads()
+    torch.set_num_threads(1)
+    yield
+    torch.set_num_threads(before)
+
+
 @pytest.fixture(scope='module')
 def ref():
-    return load_reference()
+    return golden('vs_reference')
 
 
 @pytest.fixture(scope='module')
-def runs(ref):
-    """The same 2-step generation under the reference's trace and under the oracle's."""
+def runs():
+    """The reference's 2-step generation (stored) and the same generation under the oracle's trace."""
     torch.manual_seed(0)
     pipe = make_pipeline(TINY_SPEC, dtype=torch.float32, seed=3)
-    with ref.trace(pipe) as tc:
-        pipe(PROMPT, num_inference_steps=2, generator=torch.Generator().manual_seed(11))
-        ref_keys = {k: v.clone() for k, v in tc.all_heat_maps}
-        ref_out = {
-            'global': tc.compute_global_heat_map().heat_maps.clone(),
-            'norm': tc.compute_global_heat_map(normalize=True).heat_maps.clone(),
-            'f2': tc.compute_global_heat_map(factors=[2]).heat_maps.clone(),
-            'l9h0': tc.compute_global_heat_map(layer_idx=9, head_idx=0).heat_maps.clone(),
-            'word': tc.compute_global_heat_map().compute_word_heat_map('ball').heatmap.clone(),
-            'names': list(tc.layer_names),
-        }
+    fx = golden('pipeline_tiny')
+    ref_out = {'global': fx['global'], 'norm': fx['global_norm'], 'f2': fx['factors_2'], 'l9h0': fx['layer9_head0'],
+               'word': fx['word_ball'], 'names': fx['layer_names'].tolist()}
     with O.OracleTrace(pipe) as ot:
         pipe(PROMPT, num_inference_steps=2, generator=torch.Generator().manual_seed(11))
         ora_keys = {k: v.clone() for k, v in ot.heat_maps}
@@ -51,107 +54,94 @@ def runs(ref):
             'word': O.port_word_heat_map(g, pipe.tokenizer, PROMPT, 'ball'),
             'names': list(ot.layer_names),
         }
-    return pipe, ref_keys, ref_out, ora_keys, ora_out
+    return pipe, ref_out, ora_keys, ora_out
 
 
-def test_layer_order_and_names(runs):
-    _, ref_keys, ref_out, ora_keys, ora_out = runs
+def test_layer_order_and_names(ref, runs):
+    _, ref_out, ora_keys, ora_out = runs
     assert ref_out['names'] == ora_out['names']
     assert len(ref_out['names']) == 15
-    assert list(ref_keys.keys()) == list(ora_keys.keys())
-    assert sorted({k[0] for k in ref_keys}) == [1, 2, 4]
+    assert ref['keys'].tolist() == [list(k) for k in ora_keys]
+    assert sorted({k[0] for k in ora_keys}) == [1, 2, 4]
 
 
-def test_per_key_accumulators_bit_equal(runs):
-    _, ref_keys, _, ora_keys, _ = runs
-    for k in ref_keys:
-        assert torch.equal(ref_keys[k], ora_keys[k]), k
+def test_per_key_accumulators_bit_equal(ref, runs):
+    ora_keys = runs[2]
+    for k, want in zip(ora_keys, ref['key_digests']):
+        np.testing.assert_array_equal(digest(ora_keys[k]), want, err_msg=str(k))
 
 
 @pytest.mark.parametrize('name', ['global', 'norm', 'f2', 'l9h0', 'word'])
 def test_finalize_bit_equal(runs, name):
-    _, _, ref_out, _, ora_out = runs
-    assert ref_out[name].shape == ora_out[name].shape
-    assert torch.equal(ref_out[name], ora_out[name])
+    _, ref_out, _, ora_out = runs
+    assert ref_out[name].shape == tuple(ora_out[name].shape)
+    np.testing.assert_array_equal(ora_out[name].numpy(), ref_out[name])
 
 
 def test_error_messages_match(ref, runs):
     pipe = runs[0]
-    with ref.trace(pipe) as tc:
-        with pytest.raises(RuntimeError) as e_ref:
-            tc.compute_global_heat_map()
     with O.OracleTrace(pipe) as ot:
         with pytest.raises(RuntimeError) as e_ora:
             ot.compute_global_heat_map()
-    assert str(e_ref.value) == str(e_ora.value)
-    with pytest.raises(ValueError) as w_ref:
-        ref.compute_token_merge_indices(pipe.tokenizer, PROMPT, 'zebra')
+    assert str(e_ora.value) == str(ref['empty_trace_error'])
     with pytest.raises(ValueError) as w_ora:
         O.port_token_merge_indices(pipe.tokenizer, PROMPT, 'zebra')
-    assert str(w_ref.value) == str(w_ora.value)
+    assert str(w_ora.value) == str(ref['missing_word_error'])
 
 
 def test_unravel_and_merge_indices_match_reference(ref, runs):
     pipe = runs[0]
-    hooker = ref.trace(pipe).module[0]          # a UNetCrossAttentionHooker; _unravel_attn has no state
-    probs = torch.rand(8, 256, 77)
-    assert torch.equal(hooker._unravel_attn(probs), O.port_unravel(probs))
+    probs = torch.arange(8 * 64 * 77, dtype=torch.float64).reshape(8, 64, 77)     # values = positions
+    np.testing.assert_array_equal(O.port_unravel(probs).numpy().astype(np.uint16), ref['unravel_perm'])
     for word in ['dog', 'red', 'beach']:
-        assert ref.compute_token_merge_indices(pipe.tokenizer, PROMPT, word) == \
-            O.port_token_merge_indices(pipe.tokenizer, PROMPT, word)
-    assert ref.compute_token_merge_indices(pipe.tokenizer, PROMPT, 'x', word_idx=3) == \
-        O.port_token_merge_indices(pipe.tokenizer, PROMPT, 'x', word_idx=3)
+        assert repr(O.port_token_merge_indices(pipe.tokenizer, PROMPT, word)) == str(ref[f'merge_{word}'])
+    assert repr(O.port_token_merge_indices(pipe.tokenizer, PROMPT, 'x', word_idx=3)) == str(ref['merge_x_idx3'])
 
 
 def test_math_layer_agrees_with_port(runs):
-    """The float64 restatement and the torch port agree to fp32 rounding on the reference's own key tensors."""
-    _, ref_keys, ref_out, _, _ = runs
-    keys = [v.numpy() for v in ref_keys.values()]
+    """The float64 restatement agrees to fp32 rounding with the reference's maps, from the key tensors the previous
+    tests pin to the reference's."""
+    _, ref_out, ora_keys, _ = runs
+    keys = [v.numpy() for v in ora_keys.values()]
     n_rows = ref_out['global'].shape[0]
     g = O.math_global_heat_map(keys, 64, n_rows)
-    np.testing.assert_allclose(ref_out['global'].numpy(), g, rtol=2e-5, atol=2e-6)
+    np.testing.assert_allclose(ref_out['global'], g, rtol=2e-5, atol=2e-6)
     gn = O.math_global_heat_map(keys, 64, n_rows, normalize=True)
-    np.testing.assert_allclose(ref_out['norm'].numpy(), gn, rtol=2e-5, atol=2e-6)
+    np.testing.assert_allclose(ref_out['norm'], gn, rtol=2e-5, atol=2e-6)
 
 
 def test_save_and_load_heads_match_reference(ref, tmp_path):
     """save_heads writes the same `{gen_idx}.pt` tensors; load_heads replays them into the same maps (trace.py:246-282)."""
     pipe = make_pipeline(TINY_SPEC, dtype=torch.float32, seed=5)
-    d_ref, d_ora = tmp_path / 'ref', tmp_path / 'ora'
+    d_ora = tmp_path / 'ora'
     gen = lambda: torch.Generator().manual_seed(2)
-    with ref.trace(pipe, save_heads=True, data_dir=str(d_ref)) as tc:
-        pipe(PROMPT, num_inference_steps=2, generator=gen())
-        saved_ref = tc.compute_global_heat_map().heat_maps.clone()
-        assert len(tc.layer_names) == 16          # save/load also locate the mid block
     d_ora.mkdir()
     with O.OracleTrace(pipe, save_heads=True, data_dir=d_ora) as ot:
         pipe(PROMPT, num_inference_steps=2, generator=gen())
         saved_ora = ot.compute_global_heat_map()
-    names = sorted(p.name for p in d_ref.iterdir())
-    assert names == sorted(p.name for p in d_ora.iterdir()) and len(names) == 32
-    for nme in names:
-        assert torch.equal(torch.load(d_ref / nme), torch.load(d_ora / nme)), nme
-    assert torch.equal(saved_ref, saved_ora)
+    names = sorted(p.name for p in d_ora.iterdir())
+    assert names == ref['saved_names'].tolist() and len(names) == 32
+    for nme, want in zip(names, ref['saved_digests']):
+        np.testing.assert_array_equal(digest(torch.load(d_ora / nme)), want, err_msg=nme)
+    np.testing.assert_array_equal(digest(saved_ora), ref['saved_global'])
     other = make_pipeline(TINY_SPEC, dtype=torch.float32, seed=6)     # different weights: P comes from the files
-    with ref.trace(other, load_heads=True, data_dir=str(d_ref)) as tc:
-        out_ref = other(PROMPT, num_inference_steps=2, generator=gen()).latents
-        loaded_ref = tc.compute_global_heat_map().heat_maps.clone()
-    with O.OracleTrace(other, load_heads=True, data_dir=d_ref) as ot:
+    with O.OracleTrace(other, load_heads=True, data_dir=d_ora) as ot:
         out_ora = other(PROMPT, num_inference_steps=2, generator=gen()).latents
         loaded_ora = ot.compute_global_heat_map()
-    assert torch.equal(loaded_ref, loaded_ora) and torch.equal(out_ref, out_ora)
-    assert torch.equal(loaded_ref, saved_ref)     # the maps depend on the loaded probabilities only
+    np.testing.assert_array_equal(digest(loaded_ora), ref['loaded_global'])
+    np.testing.assert_array_equal(digest(out_ora), ref['loaded_latents'])
+    np.testing.assert_array_equal(ref['loaded_global'], ref['saved_global'])   # the maps depend on the files only
 
 
 def test_reference_experiment_dump_loads_in_daam_b200(ref, tmp_path):
     """generation.pt written by the reference's GenerationExperiment.save (experiment.py:140-167) loads in ours, and back."""
-    import PIL.Image
     from daam_b200 import GenerationExperiment
-    maps = torch.rand(6, 16, 16)
-    img = PIL.Image.new('RGB', (16, 16), (10, 20, 30))
-    exp = ref.GenerationExperiment(img, maps, 'a red ball', seed=3, id='q1', path=str(tmp_path))
-    exp.save(heat_maps=False)
-    ours = GenerationExperiment.load(tmp_path / 'q1')
+    dump = tmp_path / 'q1'
+    for i, name in enumerate(ref['experiment_files'].tolist()):
+        (dump / name).parent.mkdir(parents=True, exist_ok=True)
+        (dump / name).write_bytes(ref[f'experiment_file_{i}'].tobytes())
+    maps = torch.from_numpy(ref['experiment_maps'])
+    ours = GenerationExperiment.load(dump)
     assert ours.prompt == 'a red ball' and ours.seed == 3 and torch.equal(ours.global_heat_map, maps)
     assert ours.image.size == (16, 16)
     ours.id = '.'
@@ -159,7 +149,7 @@ def test_reference_experiment_dump_loads_in_daam_b200(ref, tmp_path):
     # same folder layout both ways (the reference's own `load` calls torch.load without weights_only=False and therefore
     # cannot read ANY pickled experiment under torch >= 2.6, its own included, so the reverse direction is checked by name)
     listing = lambda root: sorted(str(p.relative_to(root)) for p in root.rglob('*') if p.is_file())
-    assert listing(tmp_path / 'again') == listing(tmp_path / 'q1')
+    assert listing(tmp_path / 'again') == listing(dump)
 
 
 def test_latent96_geometry_bit_equal(ref):
@@ -168,28 +158,24 @@ def test_latent96_geometry_bit_equal(ref):
     from daam_b200.testing.synthetic import TINY96_SPEC
     pipe = make_pipeline(TINY96_SPEC, dtype=torch.float32, seed=5)
     gen = lambda: torch.Generator().manual_seed(13)
-    with ref.trace(pipe) as tc:
-        assert tc.latent_hw == 9216
-        pipe(PROMPT, num_inference_steps=2, generator=gen())
-        ref_keys = {k: v.clone() for k, v in tc.all_heat_maps}
-        ref_g = tc.compute_global_heat_map(normalize=True).heat_maps.clone()
     with O.OracleTrace(pipe) as ot:
         pipe(PROMPT, num_inference_steps=2, generator=gen())
         ora_keys = {k: v.clone() for k, v in ot.heat_maps}
         ora_g = ot.compute_global_heat_map(normalize=True)
-    assert list(ref_keys) == list(ora_keys) and {v.shape[-1] for v in ref_keys.values()} == {96, 48, 24}
-    for k in ref_keys:
-        assert torch.equal(ref_keys[k], ora_keys[k]), k
-    assert ref_g.shape == (11, 96, 96) and torch.equal(ref_g, ora_g)
+    assert ref['keys96'].tolist() == [list(k) for k in ora_keys]
+    assert {v.shape[-1] for v in ora_keys.values()} == {96, 48, 24}
+    for k, want in zip(ora_keys, ref['key96_digests']):
+        np.testing.assert_array_equal(digest(ora_keys[k]), want, err_msg=str(k))
+    ref_g = golden('pipeline_tiny96')['global_norm']
+    assert ref_g.shape == (11, 96, 96)
+    np.testing.assert_array_equal(ora_g.numpy(), ref_g)
 
 
 def test_per_key_sweep_bit_equal(ref, runs):
     """The --all-heads sweep (daam/run/generate.py:239-255): compute_global_heat_map(layer_idx, head_idx) per key."""
-    pipe, ref_keys, _, ora_keys, _ = runs
-    with ref.trace(pipe) as tc:
-        pipe(PROMPT, num_inference_steps=2, generator=torch.Generator().manual_seed(11))
-        for (f, l, h) in list(ref_keys)[::5]:
-            want = tc.compute_global_heat_map(layer_idx=l, head_idx=h, normalize=True).heat_maps
-            got = O.port_global_heat_map(list(ora_keys.items()), 4096, want.shape[0] - 2, layer_idx=l, head_idx=h,
-                                         normalize=True)
-            assert torch.equal(want, got), (f, l, h)
+    _, ref_out, ora_keys, _ = runs
+    assert ref['sweep_keys'].tolist() == [list(k) for k in list(ora_keys)[::5]]
+    for (f, l, h), want in zip(ref['sweep_keys'].tolist(), ref['sweep_digests']):
+        got = O.port_global_heat_map(list(ora_keys.items()), 4096, ref_out['global'].shape[0] - 2, layer_idx=l,
+                                     head_idx=h, normalize=True)
+        np.testing.assert_array_equal(digest(got), want, err_msg=str((f, l, h)))

@@ -272,7 +272,7 @@ def test_collection_interface_update_and_to_experiment(tmp_path):
 
 @pytest.mark.parametrize('dtype,tol', [(torch.float32, 2e-5), (torch.float16, 4e-4)])
 def test_sd1x_style_pipeline(dtype, tol):
-    """SD-1.x style UNet (head_dim = channels // heads: 40 / 80 / 80): the tracer picks the K-chunked tcgen05 path; parity
+    """SD-1.x style UNet (head_dim = channels // heads: 40 / 80 / 80): the tracer picks the K-chunked wgmma path; parity
     with the oracle on the identical Q/K the hooks saw."""
     from daam_b200.testing.synthetic import TINY15_SPEC
     pipe = make_pipeline(TINY15_SPEC, dtype=dtype, device=DEV, seed=3)

@@ -12,6 +12,13 @@ def golden(name):
     return np.load(os.path.join(GOLDEN, name + '.npz'), allow_pickle=False)
 
 
+def digest(t, n=64):
+    """Exact fingerprint of a tensor for the golden files: [float64 sum, then a fixed seeded sample of n elements]."""
+    a = np.ascontiguousarray(torch.as_tensor(t).detach().cpu().numpy()).reshape(-1)
+    idx = np.sort(np.random.default_rng(0).choice(a.size, size=min(n, a.size), replace=False))
+    return np.concatenate([[a.astype(np.float64).sum()], a[idx].astype(np.float64)])
+
+
 def oracle_layer_maps(q, k, heads, scale, steps=1):
     """Oracle rows a3+a4 (+a6 summed over `steps` identical calls) for q [B, hw, C], k [B, 77, C]: [N*H, 77, hw] fp32.
 
