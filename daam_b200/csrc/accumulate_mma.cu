@@ -7,14 +7,13 @@
 //   wgmma      S = Q K^T: each of the two consumer warpgroups issues wgmma.m64n80k16 (fp32 accumulate) over its 64
 //              pixel rows of the tile, K^T shared; the 64 x 80 logits land in registers (40 per thread).
 //   epilogue   softmax over the 77 tokens of each pixel row (a row lives in the 4 threads of a quad: two shuffles per
-//              reduction), the probabilities are staged token-major in shared memory ([77][128] fp32) and added into
-//              the fp32 accumulator acc[head][token][pixel] either
-//                red mode : as ONE bulk-tensor reduce-add (cp.reduce.async.bulk.tensor .add.f32): the read-modify-write
-//                           happens in L2, the SM never loads the accumulator;
-//                ldst mode: coalesced 16-byte load / add / store of the staged tile by all consumer threads.
-// Warp roles: 0-7 consumers (two warpgroups: MMA + softmax + accumulate), 8 TMA producer (one elected thread) that runs
-// up to two K chunks ahead through a two-stage ring. Persistent: every CTA walks a contiguous chunk of the launch's
-// tiles; two CTAs per SM, so one CTA's loads and MMAs overlap the other's epilogue.
+//              reduction), then the probabilities are added into the tile's block of the fp32 accumulator
+//              acc[head][token][pixel] ([77][128]) in shared memory: a separate loader warp has already brought that
+//              block in by TMA, up to kAccStages tiles ahead, and one bulk-tensor store writes it back. The accumulator
+//              is read from HBM well before the tile needs it, and the SM never waits for an L2 read-modify-write.
+// Warp roles: 0-7 consumers (two warpgroups: MMA + softmax + accumulate), 8 Q/K TMA producer (one elected thread) that
+// runs up to two K chunks ahead through a two-stage ring, 9 accumulator loader (one elected thread). Persistent: every
+// CTA walks a contiguous chunk of the launch's tiles, one CTA per SM (the rings fill its shared memory).
 //
 // fp32 projections (the reference's default dtype for SD-1.x/2.x, daam/run/generate.py:205) take the same kernel in
 // "split" form. Tensor cores have no fp32 operand type and a plain tf32 product would drop 13 mantissa bits, so every
@@ -23,7 +22,11 @@
 // exactly like the 16-bit ones (two 128-byte-wide swizzled sub-tiles per 64 dims); the consumer threads rewrite them
 // in place as hi and emit `lo` into a second buffer (a shared-memory -> shared-memory elementwise pass, swizzle-
 // agnostic), then issue 3 x 8 wgmma.m64n80k8 tf32 per chunk. One CTA per SM (two 52 KB raw stages + one lo buffer +
-// the staged probabilities).
+// the staged probabilities). Its shared memory has no room for an accumulator ring, so the staged probabilities go to
+// the accumulator either
+//   red mode : as ONE bulk-tensor reduce-add (cp.reduce.async.bulk.tensor .add.f32): the read-modify-write happens in
+//              L2, the SM never loads the accumulator;
+//   ldst mode: coalesced 16-byte load / add / store of the staged tile by all consumer threads.
 //
 // head_dim other than 64 (SD-1.x: 40 / 80 / 160): the contraction runs in 64-wide K chunks, one chunk per smem stage,
 // accumulated into the same registers; the last chunk is zero-filled beyond head_dim by the TMA unit.
@@ -40,20 +43,23 @@
 namespace daam {
 namespace {
 
-constexpr int kStages = 2;
+constexpr int kStages = 2;                            // Q/K chunk ring
+constexpr int kAccStages = 3;                         // 16-bit form: accumulator tile ring
 constexpr int kQBytes = kTilePixels * 128;            // 128 rows x 128 B (64 x 16-bit, or 32 x fp32: one swizzle span)
 constexpr int kKBytes = kTokensPad * 128;             // 80 rows x 128 B
 constexpr int kStageBytes = kQBytes + kKBytes;        // 26624 = 26 x 1024 (keeps every tile 1024-byte aligned)
-constexpr int kPBytes = kTokens * kTilePixels * 4;    // staged probabilities [77][128] fp32
+constexpr int kPBytes = kTokens * kTilePixels * 4;    // one accumulator / probability tile [77][128] fp32 (128 x 308 B)
 constexpr int kConsumers = 256;                       // two warpgroups, 64 pixel rows each
-constexpr int kThreads = kConsumers + 32;             // + the TMA producer warp
-constexpr int kBarBytes = 64;                         // mbarriers
-constexpr int kSmemBytes = 1024 + kStages * kStageBytes + kPBytes + kBarBytes;
+constexpr int kThreads = kConsumers + 32;             // split form: + the TMA producer warp
+constexpr int kThreads16 = kConsumers + 64;           // 16-bit form: + the Q/K producer warp + the accumulator loader warp
+constexpr int kBarBytes = 64;                         // split form: mbarriers
+constexpr int kBarBytes16 = 8 * 2 * (kStages + kAccStages);
+constexpr int kSmemBytes = 1024 + kStages * kStageBytes + kAccStages * kPBytes + kBarBytes16;
 // split (fp32) form: a raw stage holds the fp32 tiles as [Q sub0][Q sub1][K sub0][K sub1] (sub-tile = 32 floats = one
 // 128-byte swizzle span per row); one more buffer of the same shape holds the lo terms
 constexpr int kSplitStageBytes = 2 * kStageBytes;     // 53248 = 52 x 1024
 constexpr int kSplitSmemBytes = 1024 + (kStages + 1) * kSplitStageBytes + kPBytes + kBarBytes;
-static_assert(2 * (kSmemBytes + 1024) <= 233472, "two 16-bit-form CTAs must fit one SM's 228 KB of shared memory");
+static_assert(kSmemBytes <= 232448, "16-bit form exceeds the 227 KB shared-memory limit");
 static_assert(kSplitSmemBytes <= 232448, "split form exceeds the 227 KB shared-memory limit");
 
 struct MmaParams {
@@ -113,6 +119,18 @@ __device__ __forceinline__ void tma_load_4d(const CUtensorMap* map, uint32_t bar
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+__device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint32_t bar, uint32_t dst, int c0, int c1) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
+      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1)
+      : "memory");
+}
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(map)),
+               "r"(src), "r"(c0), "r"(c1)
+               : "memory");
+}
 __device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
   asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
                    reinterpret_cast<uint64_t>(map)),
@@ -124,6 +142,14 @@ __device__ __forceinline__ void prefetch_tensormap(const CUtensorMap* map) {
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
+// The bulk-tensor reduce-add (cp.reduce.async.bulk .add.f32) flushes subnormal inputs and results to zero; the
+// accumulator updates done in shared memory use the same arithmetic, so both give the same bits.
+__device__ __forceinline__ float add_ftz(float a, float b) {
+  float r;
+  asm("add.rn.ftz.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void consumer_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory"); }
 
@@ -250,10 +276,11 @@ __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wa
 // kChunked: some layer of the launch has head_dim > 64 (several K chunks per tile); the common single-chunk case keeps
 // its simpler loops (one load iteration per tile).
 template <bool kSplit, bool kChunked>
-__global__ void __launch_bounds__(kThreads, kSplit ? 1 : 2)
+__global__ void __launch_bounds__(kSplit ? kThreads : kThreads16, 1)
 accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
   constexpr int kStageBytesT = kSplit ? kSplitStageBytes : kStageBytes;
   constexpr int kOperandBytes = (kSplit ? kStages + 1 : kStages) * kStageBytesT;     // stages (+ the lo buffer)
+  constexpr int kPTiles = kSplit ? 1 : kAccStages;   // staged probabilities (split) / the accumulator ring (16-bit)
   const LaunchParams& P = MP.base;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
@@ -261,8 +288,9 @@ accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
   uint8_t* gen = smem_raw + (base - raw);
   float* sP = reinterpret_cast<float*>(gen + kOperandBytes);
   const uint32_t sP_u32 = base + kOperandBytes;
-  const uint32_t bars = sP_u32 + kPBytes;                             // 4 mbarriers
-  const uint32_t full0 = bars, empty0 = bars + 16;
+  const uint32_t bars = sP_u32 + kPTiles * kPBytes;
+  const uint32_t full0 = bars, empty0 = bars + 8 * kStages;           // Q/K ring
+  const uint32_t afull0 = bars + 16 * kStages, aempty0 = afull0 + 8 * kAccStages;   // accumulator ring (16-bit form)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int first, count;
@@ -281,13 +309,20 @@ accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
       mbar_init(full0 + 8 * s, 1);
       mbar_init(empty0 + 8 * s, kConsumers / 32);    // one arrival per consumer warp
     }
+    if constexpr (!kSplit) {
+#pragma unroll
+      for (int s = 0; s < kAccStages; ++s) {
+        mbar_init(afull0 + 8 * s, 1);
+        mbar_init(aempty0 + 8 * s, 1);               // the consumer thread that stored the tile
+      }
+    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   // descriptor fetches of the first tile overlap the barrier set-up (and, under PDL, the previous kernel's tail)
-  if (count > 0 && lane == 0 && (warp == 0 || warp == 8)) {
+  if (count > 0 && lane == 0 && (warp == (kSplit ? 0 : 9) || warp == 8)) {
     int li0 = 0;
     const Tile t0 = decode_tile(P, first, li0);
-    if (warp == 0) {
+    if (warp != 8) {
       prefetch_tensormap(&MP.amap[t0.li]);
     } else {
       prefetch_tensormap(&MP.qmap[t0.li]);
@@ -298,12 +333,29 @@ accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
   // Programmatic dependent launch: everything above (barrier init, descriptor prefetch) may overlap the tail of the
   // previous kernel on the stream. By default nothing below starts before that kernel has completed and flushed.
   // With `early_loads` (the caller vouches that Q/K were complete before the previous kernel started, DAAM_ACC_EARLY_LOADS)
-  // only the accumulator updates wait: loads, MMAs and the first tiles' softmax overlap the previous kernel's tail.
+  // only the accumulator traffic waits (16-bit form: the accumulator loader's first load; split form: the first
+  // reduce): Q/K loads, MMAs and the first tiles' softmax overlap the previous kernel's tail.
   // Our own dependents may be scheduled as soon as every CTA of this grid is past this point.
   if (!P.early_loads) griddep_wait();
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 
-  if (warp == 8) {
+  if (warp == 9) {
+    // ===== accumulator loader (16-bit form): the CTA's accumulator tiles, in order, through the kAccStages ring =====
+    if constexpr (!kSplit) {
+      if (lane == 0 && count > 0) {
+        if (P.early_loads) griddep_wait();           // everything the previous kernel added is complete and visible
+        int li = 0;
+        for (int i = 0; i < count; ++i) {
+          const Tile t = decode_tile(P, first + i, li);
+          const int a = i % kAccStages;
+          mbar_wait(aempty0 + 8 * a, ((uint32_t)(i / kAccStages) & 1u) ^ 1u);     // its previous tile's store has read it
+          mbar_expect_tx(afull0 + 8 * a, kPBytes);   // (a partial tile's out-of-range pixels land as zeros)
+          tma_load_2d(&MP.amap[t.li], afull0 + 8 * a, sP_u32 + a * kPBytes, t.pixel0,
+                      (t.prompt * P.layer[t.li].heads + t.head) * kTokens);
+        }
+      }
+    }
+  } else if (warp == 8) {
     // ===== TMA producer =====
     if (lane == 0) {
       int li = 0, j = 0;
@@ -416,6 +468,56 @@ accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
       sum1 += __shfl_xor_sync(0xffffffffu, sum1, 1);
       sum1 += __shfl_xor_sync(0xffffffffu, sum1, 2);
       const float inv0 = 1.0f / sum0, inv1 = 1.0f / sum1;
+
+      if constexpr (!kSplit) {
+        // Add the probabilities to the landed accumulator tile sA[token][pixel], then store it back with one bulk-tensor
+        // store (clipped to the map for a partial tile). Quads 0-1 update row r0 while quads 2-3 update row r0 + 8 (and
+        // then the other way round), so one access touches 16 banks instead of 8. All old values are loaded before the
+        // first store: the compiler cannot tell the two rows apart and would otherwise serialise every load behind the
+        // previous store.
+        const int a = i % kAccStages;
+        float* sA = sP + a * (kTokens * kTilePixels);
+        const bool lowq = quad < 2;
+        const int ra = lowq ? r0 : r0 + 8, rb = lowq ? r0 + 8 : r0;
+        mbar_wait(afull0 + 8 * a, (uint32_t)(i / kAccStages) & 1u);
+        float old[40];
+#pragma unroll
+        for (int jj = 0; jj < 10; ++jj) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = 8 * jj + 2 * quad + e;
+            if (col < kTokens) {
+              old[4 * jj + e] = sA[col * kTilePixels + ra];
+              old[4 * jj + 2 + e] = sA[col * kTilePixels + rb];
+            }
+          }
+        }
+#pragma unroll
+        for (int jj = 0; jj < 10; ++jj) {
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int col = 8 * jj + 2 * quad + e;
+            if (col < kTokens) {
+              const float pa = d[4 * jj + e] * inv0, pb = d[4 * jj + 2 + e] * inv1;
+              sA[col * kTilePixels + ra] = add_ftz(old[4 * jj + e], lowq ? pa : pb);
+              sA[col * kTilePixels + rb] = add_ftz(old[4 * jj + 2 + e], lowq ? pb : pa);
+            }
+          }
+        }
+        fence_proxy_async();                           // generic-proxy writes -> visible to the bulk-async proxy
+        consumer_barrier();
+        if (tid == 0) {
+          tma_store_2d(&MP.amap[t.li], sP_u32 + a * kPBytes, t.pixel0, (t.prompt * L.heads + t.head) * kTokens);
+          bulk_commit();
+          if (i > 0) {                                 // one store of slack: the previous tile's store has read its slot
+            bulk_wait_read1();
+            mbar_arrive(aempty0 + 8 * ((i - 1) % kAccStages));
+          }
+        }
+        continue;
+      }
+
+      // ---- split form: the probabilities are staged and reduce-added (or load/add/stored) into the accumulator ----
       // the first accumulator update of this CTA: everything the previous kernel added must be complete and visible
       if (i == 0 && P.early_loads) griddep_wait();
 
@@ -461,8 +563,8 @@ accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
         }
       }
     }
-    // shared memory must outlive the reduce's reads; its global writes complete with the grid (same rule as a TMA store)
-    if (tid == 0 && issued) bulk_wait_read0();
+    // shared memory must outlive the last store's / reduce's reads; the global writes complete with the grid
+    if (tid == 0 && (kSplit ? issued : count > 0)) bulk_wait_read0();
   }
 }
 
@@ -609,9 +711,9 @@ int prepare_accumulate_mma(const LaunchParams& p, const DeviceInfo& dev, void* o
     set((const void*)accumulate_mma_kernel<true, true>, kSplitSmemBytes);
   });
   DAAM_CUDA_TRY(attr_err);
-  pm.grid = dev.sm_count * (split ? 1 : 2);
+  pm.grid = dev.sm_count;                             // one CTA per SM (both forms fill its shared memory)
   if (pm.grid > p.total_tiles) pm.grid = p.total_tiles;
-  pm.block = kThreads;
+  pm.block = split ? kThreads : kThreads16;
   pm.smem = split ? kSplitSmemBytes : kSmemBytes;
   pm.variant = (split ? 1 : 0) | (chunked ? 2 : 0);
   return DAAM_OK;

@@ -110,6 +110,14 @@ struct Plan {
 };
 constexpr size_t kMaxPlans = 32;
 
+// Whether the accumulator slabs [n_prompts][heads][77][hw] (fp32) of two layers share bytes.
+bool acc_overlap(const LayerParams& a, const LayerParams& b) {
+  auto end = [](const LayerParams& l) {
+    return reinterpret_cast<const char*>(l.acc) + (size_t)l.n_prompts * l.heads * kTokens * l.hw * sizeof(float);
+  };
+  return reinterpret_cast<const char*>(a.acc) < end(b) && reinterpret_cast<const char*>(b.acc) < end(a);
+}
+
 int build_plan(const daam_layer* layers, int n_layers, uint32_t flags, const DeviceInfo& dev, Plan* plan) {
   const uint32_t path = flags & 3u, rmw = flags & DAAM_ACC_RMW_MASK;
   // Three packs: 16-bit layers for the wgmma kernel (TMA form), fp32 layers for its split form, and the rest for
@@ -155,6 +163,14 @@ int build_plan(const daam_layer* layers, int n_layers, uint32_t flags, const Dev
     }
     const int which = use_mma ? (L.dtype == DAAM_F32 ? 1 : 0) : 2;
     LaunchParams& p = packs[which];
+    // The 16-bit wgmma form reads, adds and stores whole accumulator tiles, so two layers of one launch must not share
+    // accumulator elements: a layer whose slab overlaps one already in the pack starts the next launch (stream order).
+    if (which == 0)
+      for (int m = 0; m < p.n_layers; ++m)
+        if (acc_overlap(p.layer[m], L)) {
+          if (int rc = close(0)) return rc;
+          break;
+        }
     L.tile_begin = p.total_tiles;
     // Cost of a tile relative to the launch's other layers (SD-1.5's 40 / 80 / 160 head dims): every 64-wide K chunk is
     // one load -> (convert ->) MMA round through the two-stage ring. In the fp32 split form that chain is the whole cost

@@ -36,7 +36,7 @@ struct LayerParams {
 struct LaunchParams {
   int n_layers;
   int total_tiles;
-  int rmw_mode;             // 0: load/add/store, 1: reduce-add
+  int rmw_mode;             // 0: load/add/store, 1: reduce-add (SIMT kernel, wgmma fp32 form)
   int pdl;                  // 1: launch with programmatic stream serialization (prologue overlaps the previous kernel)
   int early_loads;          // 1: only the accumulator updates wait for the previous kernel (DAAM_ACC_EARLY_LOADS)
   int total_weight;         // sum of tiles x weight (K-chunked launches partition by weight, not by tile count)

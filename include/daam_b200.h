@@ -43,6 +43,9 @@ enum daam_dtype { DAAM_F32 = 0, DAAM_F16 = 1, DAAM_BF16 = 2 };
                                     SIMT fp32 path otherwise */
 #define DAAM_ACC_FORCE_SIMT  1u  /* always the SIMT fp32 ("warp dot") kernel */
 #define DAAM_ACC_FORCE_MMA   2u  /* wgmma kernel or DAAM_E_UNSUPPORTED */
+/* Accumulator update of the SIMT kernel and of the wgmma kernel's fp32 form. The wgmma kernel's 16-bit (fp16 / bf16)
+   form ignores these flags: it always adds in shared memory, into accumulator tiles loaded ahead by TMA, and stores
+   them back, with the same arithmetic as RED. */
 #define DAAM_ACC_RMW_MASK   0x30u
 #define DAAM_ACC_RMW_AUTO   0x00u /* = RED on both paths (one add per element per launch, so results stay
                                      deterministic) */
