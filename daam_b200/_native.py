@@ -23,7 +23,9 @@ E_INVALID, E_UNSUPPORTED, E_CUDA = -1, -2, -3
 TOKENS = 77
 EXPAND_SCRATCH_FLOATS = 64   # DAAM_EXPAND_SCRATCH_FLOATS: per word
 
-EXPORTS = ('daam_accumulate', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize', 'daam_finalize_per_key', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words', 'daam_side_launcher_create', 'daam_side_launcher_destroy',
+EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize',
+           'daam_finalize_per_key', 'daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
+           'daam_side_launcher_create', 'daam_side_launcher_destroy',
            'daam_side_launcher_launch', 'daam_side_launcher_join', 'daam_side_launcher_idle', 'daam_abi_version',
            'daam_last_error', 'daam_device_info', 'daam_launch_count')
 
@@ -75,6 +77,10 @@ def load() -> ctypes.CDLL:
     i32, u32, i64, vp, f32 = ctypes.c_int32, ctypes.c_uint32, ctypes.c_int64, ctypes.c_void_p, ctypes.c_float
     lib.daam_accumulate.argtypes = [ctypes.POINTER(DaamLayer), i32, u32, vp]
     lib.daam_accumulate.restype = ctypes.c_int
+    lib.daam_accumulate_steps.argtypes = [ctypes.POINTER(DaamLayer), ctypes.POINTER(vp), i32, u32, vp]
+    lib.daam_accumulate_steps.restype = ctypes.c_int
+    lib.daam_normalize_maps.argtypes = [vp, i32, i32, i32, vp]
+    lib.daam_normalize_maps.restype = ctypes.c_int
     lib.daam_attention_probs.argtypes = [ctypes.POINTER(DaamLayer), vp, vp]
     lib.daam_attention_probs.restype = ctypes.c_int
     lib.daam_accumulate_probs.argtypes = [vp, i32, i32, i32, i32, i32, vp, vp]
@@ -168,6 +174,31 @@ def accumulate(layers, stream: int, flags: int = ACC_AUTO):
     rc = load().daam_accumulate(packed.array, packed.n, flags, stream)
     if rc != 0:
         _check(rc)
+
+
+class StepPointers:
+    """A ready-made ``float* step_acc[]`` (host array of device pointers) for :func:`accumulate_steps`."""
+
+    def __init__(self, ptrs: Sequence[int]):
+        self.array = (ctypes.c_void_p * max(len(ptrs), 1))(*ptrs)
+
+
+def accumulate_steps(layers, steps, stream: int, flags: int = ACC_AUTO):
+    """``daam_accumulate_steps``: ``layers`` as for :func:`accumulate`; ``steps`` a :class:`StepPointers` or a sequence of
+    device pointers, one step slab per layer (the first ``n`` are used)."""
+    packed = layers if isinstance(layers, PackedLayers) else PackedLayers(layers)
+    if packed.n == 0:
+        return
+    arr = steps if isinstance(steps, StepPointers) else StepPointers(steps)
+    if len(arr.array) < packed.n:
+        raise ValueError(f'{len(arr.array)} step slabs for {packed.n} layers')
+    rc = load().daam_accumulate_steps(packed.array, arr.array, packed.n, flags, stream)
+    if rc != 0:
+        _check(rc)
+
+
+def normalize_maps(maps_ptr: int, n_maps: int, n_rows: int, x: int, stream: int):
+    _check(load().daam_normalize_maps(ctypes.c_void_p(maps_ptr), n_maps, n_rows, x, ctypes.c_void_p(stream)))
 
 
 def attention_probs(layer: DaamLayer, probs_ptr: int, stream: int):

@@ -31,10 +31,19 @@
 // head_dim other than 64 (SD-1.x: 40 / 80 / 160): the contraction runs in 64-wide K chunks, one chunk per smem stage,
 // accumulated into the same registers; the last chunk is zero-filled beyond head_dim by the TMA unit.
 //
+// Step-slab instances (kStep, daam_accumulate_steps): every form also STORES what it adds into a second fp32 slab of the
+// accumulator's layout, flushed like the add, so that a caller gets one denoising step's maps next to the time sum.
+//   16-bit form: one more [77][128] shared block sS; the consumers write p there in the pass that adds into the ring
+//                slot, and the thread that stores the accumulator tile issues a second bulk-tensor store from sS in the
+//                same bulk group. Before sS is rewritten, that thread waits for the previous group's reads.
+//   split form : red mode stages the flushed p in sP (the reduce flushes its inputs anyway) and bulk-stores sP next to
+//                the reduce; ldst mode writes p to the step slab in its coalesced load / add / store pass.
+//
 // Replaces daam/trace.py:276 (get_attention_scores), :219-244 (_unravel_attn) and :293-294 (update loop).
 #include <cuda.h>
 
 #include <mutex>
+#include <type_traits>
 #include <unordered_map>
 #include <string>
 
@@ -55,12 +64,14 @@ constexpr int kThreads16 = kConsumers + 64;           // 16-bit form: + the Q/K 
 constexpr int kBarBytes = 64;                         // split form: mbarriers
 constexpr int kBarBytes16 = 8 * 2 * (kStages + kAccStages);
 constexpr int kSmemBytes = 1024 + kStages * kStageBytes + kAccStages * kPBytes + kBarBytes16;
+constexpr int kStepSmemBytes = kSmemBytes + kPBytes;  // 16-bit form with a step slab: + the sS block (207.5 KB in all)
 // split (fp32) form: a raw stage holds the fp32 tiles as [Q sub0][Q sub1][K sub0][K sub1] (sub-tile = 32 floats = one
 // 128-byte swizzle span per row); one more buffer of the same shape holds the lo terms
 constexpr int kSplitStageBytes = 2 * kStageBytes;     // 53248 = 52 x 1024
 constexpr int kSplitSmemBytes = 1024 + (kStages + 1) * kSplitStageBytes + kPBytes + kBarBytes;
 static_assert(kSmemBytes <= 232448, "16-bit form exceeds the 227 KB shared-memory limit");
 static_assert(kSplitSmemBytes <= 232448, "split form exceeds the 227 KB shared-memory limit");
+static_assert(kStepSmemBytes <= 232448, "16-bit step form exceeds the 227 KB shared-memory limit");
 
 struct MmaParams {
   LaunchParams base;
@@ -68,6 +79,14 @@ struct MmaParams {
   CUtensorMap kmap[kMaxLayersPerLaunch];
   CUtensorMap amap[kMaxLayersPerLaunch];
 };
+// Parameter block of the step-slab instances (about 20 KB): the step slab of every layer as a tensor map shaped like
+// amap (bulk stores) and as a plain pointer (split form, ldst mode).
+struct MmaStepParams : MmaParams {
+  CUtensorMap smap[kMaxLayersPerLaunch];
+  float* step[kMaxLayersPerLaunch];
+};
+template <bool kStep>
+using MmaParamsT = std::conditional_t<kStep, MmaStepParams, MmaParams>;
 
 // ---- PTX wrappers -------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -143,13 +162,6 @@ __device__ __forceinline__ void prefetch_tensormap(const CUtensorMap* map) {
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
-// The bulk-tensor reduce-add (cp.reduce.async.bulk .add.f32) flushes subnormal inputs and results to zero; the
-// accumulator updates done in shared memory use the same arithmetic, so both give the same bits.
-__device__ __forceinline__ float add_ftz(float a, float b) {
-  float r;
-  asm("add.rn.ftz.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
-  return r;
-}
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void consumer_barrier() { asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory"); }
 
@@ -274,13 +286,14 @@ __device__ __forceinline__ void wgmma_chunk_16bit(Frag& d, uint32_t a_src, uint3
 __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 // kChunked: some layer of the launch has head_dim > 64 (several K chunks per tile); the common single-chunk case keeps
-// its simpler loops (one load iteration per tile).
-template <bool kSplit, bool kChunked>
+// its simpler loops (one load iteration per tile). kStep: also store each tile's probabilities into the step slab.
+template <bool kSplit, bool kChunked, bool kStep>
 __global__ void __launch_bounds__(kSplit ? kThreads : kThreads16, 1)
-accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
+accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kStep> MP) {
   constexpr int kStageBytesT = kSplit ? kSplitStageBytes : kStageBytes;
   constexpr int kOperandBytes = (kSplit ? kStages + 1 : kStages) * kStageBytesT;     // stages (+ the lo buffer)
-  constexpr int kPTiles = kSplit ? 1 : kAccStages;   // staged probabilities (split) / the accumulator ring (16-bit)
+  // staged probabilities (split) / the accumulator ring (16-bit), + sS (16-bit step form)
+  constexpr int kPTiles = kSplit ? 1 : kAccStages + (kStep ? 1 : 0);
   const LaunchParams& P = MP.base;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
@@ -288,6 +301,8 @@ accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
   uint8_t* gen = smem_raw + (base - raw);
   float* sP = reinterpret_cast<float*>(gen + kOperandBytes);
   const uint32_t sP_u32 = base + kOperandBytes;
+  float* sS = sP + kAccStages * (kTokens * kTilePixels);              // 16-bit step form: the tile's p, stored as is
+  const uint32_t sS_u32 = sP_u32 + kAccStages * kPBytes;
   const uint32_t bars = sP_u32 + kPTiles * kPBytes;
   const uint32_t full0 = bars, empty0 = bars + 8 * kStages;           // Q/K ring
   const uint32_t afull0 = bars + 16 * kStages, aempty0 = afull0 + 8 * kAccStages;   // accumulator ring (16-bit form)
@@ -324,6 +339,7 @@ accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
     const Tile t0 = decode_tile(P, first, li0);
     if (warp != 8) {
       prefetch_tensormap(&MP.amap[t0.li]);
+      if constexpr (kStep) prefetch_tensormap(&MP.smap[t0.li]);
     } else {
       prefetch_tensormap(&MP.qmap[t0.li]);
       prefetch_tensormap(&MP.kmap[t0.li]);
@@ -492,6 +508,10 @@ accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
             }
           }
         }
+        if constexpr (kStep) {                         // the previous tile's step store has finished reading sS
+          if (tid == 0 && i > 0) bulk_wait_read0();
+          consumer_barrier();
+        }
 #pragma unroll
         for (int jj = 0; jj < 10; ++jj) {
 #pragma unroll
@@ -501,6 +521,10 @@ accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
               const float pa = d[4 * jj + e] * inv0, pb = d[4 * jj + 2 + e] * inv1;
               sA[col * kTilePixels + ra] = add_ftz(old[4 * jj + e], lowq ? pa : pb);
               sA[col * kTilePixels + rb] = add_ftz(old[4 * jj + 2 + e], lowq ? pb : pa);
+              if constexpr (kStep) {
+                sS[col * kTilePixels + ra] = add_ftz(0.f, lowq ? pa : pb);
+                sS[col * kTilePixels + rb] = add_ftz(0.f, lowq ? pb : pa);
+              }
             }
           }
         }
@@ -508,6 +532,8 @@ accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
         consumer_barrier();
         if (tid == 0) {
           tma_store_2d(&MP.amap[t.li], sP_u32 + a * kPBytes, t.pixel0, (t.prompt * L.heads + t.head) * kTokens);
+          if constexpr (kStep)                         // same bulk group: the waits below cover both stores
+            tma_store_2d(&MP.smap[t.li], sS_u32, t.pixel0, (t.prompt * L.heads + t.head) * kTokens);
           bulk_commit();
           if (i > 0) {                                 // one store of slack: the previous tile's store has read its slot
             bulk_wait_read1();
@@ -526,13 +552,18 @@ accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
       if (tid == 0 && issued) bulk_wait_read0();       // the previous reduce has finished reading sP
       consumer_barrier();                              // ... and (ldst mode) every thread has read the previous tile
       const bool lowq = quad < 2;
+      // step form, red mode: stage p as the reduce sees it (flushed), so that one buffer serves the reduce and the store
+      const bool stage_ftz = kStep && P.rmw_mode == 1;
 #pragma unroll
       for (int jj = 0; jj < 10; ++jj) {
 #pragma unroll
         for (int e = 0; e < 2; ++e) {
           const int col = 8 * jj + 2 * quad + e;
           if (col < kTokens) {
-            const float a = d[4 * jj + e] * inv0, b = d[4 * jj + 2 + e] * inv1;
+            float a = d[4 * jj + e] * inv0, b = d[4 * jj + 2 + e] * inv1;
+            if constexpr (kStep) {
+              if (stage_ftz) { a = add_ftz(0.f, a); b = add_ftz(0.f, b); }
+            }
             sP[col * kTilePixels + (lowq ? r0 : r0 + 8)] = lowq ? a : b;
             sP[col * kTilePixels + (lowq ? r0 + 8 : r0)] = lowq ? b : a;
           }
@@ -543,6 +574,7 @@ accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
         consumer_barrier();
         if (tid == 0) {
           tma_reduce_add_2d(&MP.amap[t.li], sP_u32, t.pixel0, (t.prompt * L.heads + t.head) * kTokens);
+          if constexpr (kStep) tma_store_2d(&MP.smap[t.li], sP_u32, t.pixel0, (t.prompt * L.heads + t.head) * kTokens);
           bulk_commit();
         }
         issued = true;
@@ -559,6 +591,8 @@ accumulate_mma_kernel(const __grid_constant__ MmaParams MP) {
             float4 o = *g;
             o.x += p.x; o.y += p.y; o.z += p.z; o.w += p.w;
             *g = o;
+            if constexpr (kStep)
+              reinterpret_cast<float4*>(MP.step[t.li] + (acc - L.acc) + tok * hw)[c4] = p;
           }
         }
       }
@@ -672,9 +706,9 @@ std::once_flag g_attr_once[64];                       // the shared-memory attri
 
 // Parameter block of one wgmma launch, opaque to api.cu (which caches prepared launches by their daam_layer[] input).
 struct PreparedMma {
-  MmaParams mp;
-  int grid, block, smem, variant;                     // variant: bit 0 split (fp32), bit 1 chunked (head_dim > 64)
-};
+  MmaStepParams mp;                                   // the plain instances are launched with its MmaParams part
+  int grid, block, smem, variant;                     // variant: bit 0 split (fp32), bit 1 chunked (head_dim > 64),
+};                                                    // bit 2 step slabs
 void* prepared_mma_new() { return new PreparedMma; }                 // (aligned new: CUtensorMap is alignas(64))
 void prepared_mma_delete(void* p) { delete static_cast<PreparedMma*>(p); }
 
@@ -684,10 +718,10 @@ bool mma_supported(const LayerParams& L) {
 }
 
 // Tensor maps, grid and kernel variant of one pack of layers (all fp32, or all 16-bit). `out`: prepared_mma_new().
-int prepare_accumulate_mma(const LaunchParams& p, const DeviceInfo& dev, void* out) {
+int prepare_accumulate_mma(const LaunchParams& p, const StepSlabs* steps, const DeviceInfo& dev, void* out) {
   if (dev.cc_major != 9) { set_error("the wgmma kernel needs an sm_90 device (found sm_%d%d)", dev.cc_major, dev.cc_minor); return DAAM_E_UNSUPPORTED; }
   PreparedMma& pm = *static_cast<PreparedMma*>(out);
-  MmaParams& mp = pm.mp;
+  MmaStepParams& mp = pm.mp;
   mp.base = p;
   const bool split = p.n_layers > 0 && p.layer[0].dtype == DAAM_F32;     // a pack holds one operand class (api.cu)
   bool chunked = false;
@@ -697,6 +731,10 @@ int prepare_accumulate_mma(const LaunchParams& p, const DeviceInfo& dev, void* o
     if (int rc = make_qk_map(L.q, L.dtype, L.head_dim, L.heads, L.hw, L.n_prompts, L.qs_head, L.qs_pixel, L.qs_prompt, kTilePixels, &mp.qmap[i])) return rc;
     if (int rc = make_qk_map(L.k, L.dtype, L.head_dim, L.heads, kTokens, L.n_prompts, L.ks_head, L.ks_token, L.ks_prompt, kTokensPad, &mp.kmap[i])) return rc;
     if (int rc = make_acc_map(L.acc, L.hw, L.n_prompts * L.heads * kTokens, &mp.amap[i])) return rc;
+    if (steps) {                                      // the step slab has the accumulator's shape: same map, other base
+      if (int rc = make_acc_map(steps->step[i], L.hw, L.n_prompts * L.heads * kTokens, &mp.smap[i])) return rc;
+      mp.step[i] = steps->step[i];
+    }
     chunked = chunked || L.head_dim > 64;
   }
   cudaError_t attr_err = cudaSuccess;
@@ -705,19 +743,33 @@ int prepare_accumulate_mma(const LaunchParams& p, const DeviceInfo& dev, void* o
       cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
       if (e != cudaSuccess) attr_err = e;
     };
-    set((const void*)accumulate_mma_kernel<false, false>, kSmemBytes);
-    set((const void*)accumulate_mma_kernel<false, true>, kSmemBytes);
-    set((const void*)accumulate_mma_kernel<true, false>, kSplitSmemBytes);
-    set((const void*)accumulate_mma_kernel<true, true>, kSplitSmemBytes);
+    set((const void*)accumulate_mma_kernel<false, false, false>, kSmemBytes);
+    set((const void*)accumulate_mma_kernel<false, true, false>, kSmemBytes);
+    set((const void*)accumulate_mma_kernel<true, false, false>, kSplitSmemBytes);
+    set((const void*)accumulate_mma_kernel<true, true, false>, kSplitSmemBytes);
+    set((const void*)accumulate_mma_kernel<false, false, true>, kStepSmemBytes);
+    set((const void*)accumulate_mma_kernel<false, true, true>, kStepSmemBytes);
+    set((const void*)accumulate_mma_kernel<true, false, true>, kSplitSmemBytes);
+    set((const void*)accumulate_mma_kernel<true, true, true>, kSplitSmemBytes);
   });
   DAAM_CUDA_TRY(attr_err);
   pm.grid = dev.sm_count;                             // one CTA per SM (both forms fill its shared memory)
   if (pm.grid > p.total_tiles) pm.grid = p.total_tiles;
   pm.block = split ? kThreads : kThreads16;
-  pm.smem = split ? kSplitSmemBytes : kSmemBytes;
-  pm.variant = (split ? 1 : 0) | (chunked ? 2 : 0);
+  pm.smem = split ? kSplitSmemBytes : (steps ? kStepSmemBytes : kSmemBytes);
+  pm.variant = (split ? 1 : 0) | (chunked ? 2 : 0) | (steps ? 4 : 0);
   return DAAM_OK;
 }
+
+namespace {
+template <bool kSplit, bool kChunked, bool kStep>
+cudaError_t launch_variant(const cudaLaunchConfig_t& cfg, const PreparedMma& pm) {
+  if constexpr (kStep)
+    return cudaLaunchKernelEx(&cfg, accumulate_mma_kernel<kSplit, kChunked, true>, pm.mp);
+  else
+    return cudaLaunchKernelEx(&cfg, accumulate_mma_kernel<kSplit, kChunked, false>, static_cast<const MmaParams&>(pm.mp));
+}
+}  // namespace
 
 int launch_prepared_mma(const void* prepared, cudaStream_t stream) {
   const PreparedMma& pm = *static_cast<const PreparedMma*>(prepared);
@@ -734,10 +786,14 @@ int launch_prepared_mma(const void* prepared, cudaStream_t stream) {
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   switch (pm.variant) {
-    case 0: DAAM_CUDA_TRY(cudaLaunchKernelEx(&cfg, accumulate_mma_kernel<false, false>, pm.mp)); break;
-    case 1: DAAM_CUDA_TRY(cudaLaunchKernelEx(&cfg, accumulate_mma_kernel<true, false>, pm.mp)); break;
-    case 2: DAAM_CUDA_TRY(cudaLaunchKernelEx(&cfg, accumulate_mma_kernel<false, true>, pm.mp)); break;
-    default: DAAM_CUDA_TRY(cudaLaunchKernelEx(&cfg, accumulate_mma_kernel<true, true>, pm.mp)); break;
+    case 0: DAAM_CUDA_TRY((launch_variant<false, false, false>(cfg, pm))); break;
+    case 1: DAAM_CUDA_TRY((launch_variant<true, false, false>(cfg, pm))); break;
+    case 2: DAAM_CUDA_TRY((launch_variant<false, true, false>(cfg, pm))); break;
+    case 3: DAAM_CUDA_TRY((launch_variant<true, true, false>(cfg, pm))); break;
+    case 4: DAAM_CUDA_TRY((launch_variant<false, false, true>(cfg, pm))); break;
+    case 5: DAAM_CUDA_TRY((launch_variant<true, false, true>(cfg, pm))); break;
+    case 6: DAAM_CUDA_TRY((launch_variant<false, true, true>(cfg, pm))); break;
+    default: DAAM_CUDA_TRY((launch_variant<true, true, true>(cfg, pm))); break;
   }
   DAAM_CUDA_TRY(cudaGetLastError());
   count_launch();

@@ -5,6 +5,10 @@
 // logits live in registers, K^T sits in shared memory and is read as warp-wide broadcasts, so softmax needs no
 // shuffles and the accumulator update `acc[t][pixel] += p[t]` is one fully coalesced 128-byte access per warp and
 // token. Replaces daam/trace.py:276 (get_attention_scores), :219-244 (_unravel_attn) and :293-294 (update loop).
+//
+// The step-slab kernel (daam_accumulate_steps) is the same body with kStep: next to every add it stores the addend into
+// the layer's step slab, again one coalesced 128-byte access per warp and token (flushed like RED in reduce mode; in
+// load / add / store mode the add is an fma, so the stored value is the rounded product, i.e. fma(p, inv, 0)).
 #include <mutex>
 
 #include "simt_common.cuh"
@@ -12,7 +16,8 @@
 namespace daam {
 namespace {
 
-__global__ void __launch_bounds__(kTilePixels, 3) accumulate_simt_kernel(const __grid_constant__ LaunchParams P) {
+template <bool kStep>
+__device__ __forceinline__ void accumulate_simt_body(const LaunchParams& P, const StepSlabs* S) {
   extern __shared__ __align__(16) float smem[];
   // contiguous chunk of tiles per CTA: consecutive tiles share (layer, prompt, head), so K^T is staged once per run
   const int per = P.total_tiles / gridDim.x, rem = P.total_tiles % gridDim.x;
@@ -37,11 +42,15 @@ __global__ void __launch_bounds__(kTilePixels, 3) accumulate_simt_kernel(const _
 
     const int pixel = t.pixel0 + threadIdx.x;
     if (pixel < L.hw) {
-      float* a = L.acc + ((long long)(t.prompt * L.heads + t.head) * kTokens) * L.hw + pixel;
+      const long long off = ((long long)(t.prompt * L.heads + t.head) * kTokens) * L.hw + pixel;
+      float* a = L.acc + off;
       const long long hw = L.hw;
       if (P.rmw_mode == 1) {
 #pragma unroll
-        for (int j = 0; j < kTokens; ++j) atomicAdd(a + j * hw, s[j] * inv);   // result unused -> RED
+        for (int j = 0; j < kTokens; ++j) {
+          atomicAdd(a + j * hw, s[j] * inv);          // result unused -> RED
+          if constexpr (kStep) S->step[t.li][off + j * hw] = add_ftz(0.f, s[j] * inv);
+        }
       } else {
         constexpr int kChunk = 11;                    // 77 = 7 x 11 loads in flight per thread
 #pragma unroll
@@ -51,31 +60,45 @@ __global__ void __launch_bounds__(kTilePixels, 3) accumulate_simt_kernel(const _
           for (int i = 0; i < kChunk; ++i) old[i] = a[(j0 + i) * hw];
 #pragma unroll
           for (int i = 0; i < kChunk; ++i) a[(j0 + i) * hw] = fmaf(s[j0 + i], inv, old[i]);
+          if constexpr (kStep) {
+#pragma unroll
+            for (int i = 0; i < kChunk; ++i) S->step[t.li][off + (j0 + i) * hw] = fmaf(s[j0 + i], inv, 0.f);
+          }
         }
       }
     }
   }
 }
 
+__global__ void __launch_bounds__(kTilePixels, 3) accumulate_simt_kernel(const __grid_constant__ LaunchParams P) {
+  accumulate_simt_body<false>(P, nullptr);
+}
+
+__global__ void __launch_bounds__(kTilePixels, 3)
+accumulate_simt_step_kernel(const __grid_constant__ LaunchParams P, const __grid_constant__ StepSlabs S) {
+  accumulate_simt_body<true>(P, &S);
+}
+
 }  // namespace
 
-int prepare_accumulate_simt(const LaunchParams& p, const DeviceInfo& dev, int* grid_out, size_t* smem_out) {
+int prepare_accumulate_simt(const LaunchParams& p, const StepSlabs* steps, const DeviceInfo& dev, int* grid_out,
+                            size_t* smem_out) {
   int dmax = 0;
   for (int i = 0; i < p.n_layers; ++i) dmax = p.layer[i].head_dim > dmax ? p.layer[i].head_dim : dmax;
   const size_t smem = sizeof(float) * simt::tile_smem_floats(dmax);
   static std::mutex mu;
-  static size_t configured_dev[64] = {};              // the attribute is per device
+  static size_t configured_dev[2][64] = {};           // the attribute is per device (and per kernel)
+  const void* fn = steps ? (const void*)accumulate_simt_step_kernel : (const void*)accumulate_simt_kernel;
   {
     std::lock_guard<std::mutex> lock(mu);
-    size_t& configured = configured_dev[dev.device & 63];
+    size_t& configured = configured_dev[steps ? 1 : 0][dev.device & 63];
     if (smem > configured) {
-      DAAM_CUDA_TRY(cudaFuncSetAttribute(accumulate_simt_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)smem));
+      DAAM_CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
       configured = smem;
     }
   }
   int occ = 0;
-  DAAM_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, accumulate_simt_kernel, kTilePixels, smem));
+  DAAM_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, fn, kTilePixels, smem));
   if (occ < 1) occ = 1;
   int grid = dev.sm_count * occ;
   if (grid > p.total_tiles) grid = p.total_tiles;
@@ -84,8 +107,11 @@ int prepare_accumulate_simt(const LaunchParams& p, const DeviceInfo& dev, int* g
   return DAAM_OK;
 }
 
-int launch_prepared_simt(const LaunchParams& p, int grid, size_t smem, cudaStream_t stream) {
-  accumulate_simt_kernel<<<grid, kTilePixels, smem, stream>>>(p);
+int launch_prepared_simt(const LaunchParams& p, const StepSlabs* steps, int grid, size_t smem, cudaStream_t stream) {
+  if (steps)
+    accumulate_simt_step_kernel<<<grid, kTilePixels, smem, stream>>>(p, *steps);
+  else
+    accumulate_simt_kernel<<<grid, kTilePixels, smem, stream>>>(p);
   DAAM_CUDA_TRY(cudaGetLastError());
   count_launch();
   return DAAM_OK;

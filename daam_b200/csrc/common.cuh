@@ -50,6 +50,20 @@ __device__ __forceinline__ float fast_exp2(float x) {
   return y;
 }
 
+// The bulk-tensor reduce-add (cp.reduce.async.bulk .add.f32) and red.global.add.f32 flush subnormal inputs and results
+// to zero; the accumulator updates done in shared memory use the same arithmetic, so both give the same bits.
+// add_ftz(0.f, p) is the addend as such an add sees it: what the step-slab instances store.
+__device__ __forceinline__ float add_ftz(float a, float b) {
+  float r;
+  asm("add.rn.ftz.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+
+// Step slabs of one launch (daam_accumulate_steps): step[i] has the layout of layer i's accumulator.
+struct StepSlabs {
+  float* step[kMaxLayersPerLaunch];
+};
+
 // ---- error plumbing ---------------------------------------------------------------------------------------------
 void set_error(const char* fmt, ...);
 int cuda_fail(cudaError_t e, const char* what);
@@ -70,11 +84,12 @@ void count_launch(int n = 1);
 // ---- kernel launchers (one per translation unit) ----------------------------------------------------------------
 // Preparation (tensor maps, grid, shared-memory size) is split from the launch so that api.cu can cache it per
 // distinct daam_layer[] input: the steady state of a trace replays the same layer calls every denoising step.
-int prepare_accumulate_simt(const LaunchParams& p, const DeviceInfo& dev, int* grid, size_t* smem);
-int launch_prepared_simt(const LaunchParams& p, int grid, size_t smem, cudaStream_t stream);
+// `steps`: the launch's step slabs (daam_accumulate_steps, selects the step-slab kernel instances) or nullptr.
+int prepare_accumulate_simt(const LaunchParams& p, const StepSlabs* steps, const DeviceInfo& dev, int* grid, size_t* smem);
+int launch_prepared_simt(const LaunchParams& p, const StepSlabs* steps, int grid, size_t smem, cudaStream_t stream);
 void* prepared_mma_new();
 void prepared_mma_delete(void* prepared);
-int prepare_accumulate_mma(const LaunchParams& p, const DeviceInfo& dev, void* prepared);
+int prepare_accumulate_mma(const LaunchParams& p, const StepSlabs* steps, const DeviceInfo& dev, void* prepared);
 int launch_prepared_mma(const void* prepared, cudaStream_t stream);
 bool mma_supported(const LayerParams& l);
 

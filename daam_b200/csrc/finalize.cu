@@ -624,6 +624,20 @@ extern "C" int daam_finalize_per_key(const daam_key_group* groups, int32_t n_gro
   return DAAM_OK;
 }
 
+extern "C" int daam_normalize_maps(float* maps, int32_t n_maps, int32_t n_rows, int32_t x, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!maps || n_maps < 0 || n_rows <= 0 || x <= 0) { set_error("daam_normalize_maps: null pointer or bad size"); return DAAM_E_INVALID; }
+  if (n_maps > 65535) { set_error("daam_normalize_maps: %d maps > 65535", n_maps); return DAAM_E_UNSUPPORTED; }
+  if (n_maps == 0) return DAAM_OK;
+  DeviceInfo dev;
+  if (int rc = get_device_info(&dev)) return rc;
+  const int xx = x * x;
+  normalize_kernel<<<dim3((xx + 255) / 256, n_maps), 256, 0, stream>>>(maps, n_rows, xx);
+  DAAM_CUDA_TRY(cudaGetLastError());
+  count_launch();
+  return DAAM_OK;
+}
+
 extern "C" int daam_word_heat_map(const float* global_maps, int32_t n_rows, int32_t x, const int32_t* rows,
                                   int32_t n_sel, float* out, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);

@@ -23,7 +23,7 @@ import torch
 from . import _native
 from .utils import compute_token_merge_indices
 
-__all__ = ['GlobalHeatMap', 'RawHeatMapCollection', 'WordHeatMap', 'LayerSlab']
+__all__ = ['GlobalHeatMap', 'RawHeatMapCollection', 'WordHeatMap', 'LayerSlab', 'TimeHeatMaps']
 
 RawHeatMapKey = Tuple[int, int, int]  # factor, layer, head
 
@@ -50,6 +50,7 @@ class LayerSlab:
     touched: bool = False        # a key exists only once it has been updated (defaultdict semantics)
     head_offset: int = 0         # first real head behind key head 0 (non-zero only for the un-guided B=1 quirk)
     captured: bool = False       # the layer's kernel launch is part of a CUDA graph: replays update it without the hook
+    step: Optional[torch.Tensor] = None   # time-resolved traces only: what the last step added, shaped like ``acc``
 
     @property
     def n_prompts(self) -> int:
@@ -68,6 +69,7 @@ class RawHeatMapCollection:
         self.epoch = 0                        # bumped whenever a slab object is (re)allocated (descriptor caches key on it)
         self._sync = None                     # callable making pending kernel work visible to the current stream
         self._zero = None                     # callable(slabs) zeroing slabs in accumulate-stream order
+        self.time_resolved = False            # allocate a step slab next to every accumulator (trace(time_resolved=True))
 
     # -- wiring from the tracer -------------------------------------------------------------------------------------
     def bind(self, sync, zero):
@@ -83,12 +85,14 @@ class RawHeatMapCollection:
         slab = self.slabs.get(layer_idx)
         shape = (n_prompts, heads, _native.TOKENS, h * w)
         if slab is None or tuple(slab.acc.shape) != shape or slab.acc.device != torch.device(device) \
-                or slab.factor != factor:
+                or slab.factor != factor or (self.time_resolved and slab.step is None):
             if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
                 raise RuntimeError('accumulator slabs cannot be created inside a CUDA-graph capture: run one eager '
                                    'UNet step under trace() before capturing')
             acc = torch.zeros(shape, dtype=torch.float32, device=device)
-            slab = LayerSlab(layer_idx, factor, heads, h, w, acc, head_offset=head_offset)
+            # the kernel writes every element of a step slab each step: no zeroing needed
+            step = torch.empty(shape, dtype=torch.float32, device=device) if self.time_resolved else None
+            slab = LayerSlab(layer_idx, factor, heads, h, w, acc, head_offset=head_offset, step=step)
             self.slabs[layer_idx] = slab
             self.epoch += 1
         if not slab.touched:
@@ -271,3 +275,40 @@ class GlobalHeatMap:
                                  threshold, word_maps.data_ptr(), out.data_ptr(), scratch.data_ptr(), _stream_ptr(dev))
         whms = [WordHeatMap(word_maps[i], w, idx) for i, (w, (_, idx)) in enumerate(zip(words, merged))]
         return whms, (out.cpu() if to_cpu else out)
+
+
+class TimeHeatMaps:
+    """One global heat map per traced denoising step (UNet forward) of one prompt: ``heat_maps[t]`` is exactly what
+    :meth:`~daam_b200.trace.DiffusionHeatMapHooker.compute_global_heat_map` would return had only step ``t`` been
+    traced (per-key bicubic, clamp, mean over keys, ``n_tokens + 2`` rows).
+
+    The steps do not sum to the all-steps map: the clamp comes after the time sum there and per step here."""
+
+    def __init__(self, tokenizer, prompt: str, heat_maps: torch.Tensor):
+        self.tokenizer = tokenizer
+        self.prompt = prompt
+        self.heat_maps = heat_maps           # device fp32 [steps, n_rows, x, x]
+
+    def __len__(self) -> int:
+        return self.heat_maps.shape[0]
+
+    def __getitem__(self, t: int) -> GlobalHeatMap:
+        """Step ``t`` as a :class:`GlobalHeatMap` (``compute_word_heat_map``, ``expand_words``)."""
+        return GlobalHeatMap(self.tokenizer, self.prompt, self.heat_maps[t])
+
+    def word_heat_maps(self, word: str, word_idx: int = None, offset_idx: int = 0) -> torch.Tensor:
+        """``[steps, x, x]``: row ``t`` is ``self[t].compute_word_heat_map(word, word_idx, offset_idx).heatmap``."""
+        rows, _ = compute_token_merge_indices(self.tokenizer, self.prompt, word, word_idx, offset_idx)
+        maps = self.heat_maps
+        _require_cuda(maps, 'TimeHeatMaps.word_heat_maps')
+        steps, n_rows, x = maps.shape[0], maps.shape[1], maps.shape[-1]
+        for r in rows:
+            if not -n_rows <= r < n_rows:
+                raise IndexError(f'index {r} is out of bounds for dimension 0 with size {n_rows}')
+        maps = maps.detach().float().contiguous()
+        out = torch.empty((steps, x, x), dtype=torch.float32, device=maps.device)
+        with torch.cuda.device(maps.device):
+            stream = _stream_ptr(maps.device)
+            for t in range(steps):
+                _native.word_heat_map(maps[t].data_ptr(), n_rows, x, rows, out[t].data_ptr(), stream)
+        return out

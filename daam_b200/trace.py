@@ -13,6 +13,10 @@ exceptions; what differs is what runs underneath.
   (``launch='overlap'``: four CUDA calls per step); ``launch='layer'`` issues it immediately per layer.
 * ``compute_global_heat_map`` (trace.py:83-132) keeps the Python-side key filter and error messages and runs the
   bicubic-upsample / clamp / mean / normalise reduction as one kernel (``daam_finalize``).
+* ``time_resolved=True`` also answers *when* a word's attribution forms: the step launch becomes
+  ``daam_accumulate_steps`` (the kernel also stores what it adds into a second slab per layer) followed by one
+  ``daam_finalize`` per prompt over those step slabs, into that step's slot of a device history
+  (``compute_time_heat_maps``).
 
 Accumulators are fp32 regardless of the pipeline dtype (the reference accumulates in the pipeline dtype, SURVEY.md
 section 5); parity is stated against the fp32 oracle fed the same Q/K.
@@ -28,7 +32,7 @@ import torch
 import torch.nn.functional as F
 
 from . import _native, ops
-from .heatmap import GlobalHeatMap, LayerSlab, RawHeatMapCollection
+from .heatmap import GlobalHeatMap, LayerSlab, RawHeatMapCollection, TimeHeatMaps
 from .hook import AggregateHooker, ObjectHooker, UNetCrossAttentionLocator
 from .utils import cache_dir
 
@@ -40,15 +44,21 @@ class DiffusionHeatMapHooker(AggregateHooker):
 
     Extra keyword-only options (not in the reference): ``launch`` ('step' | 'overlap' | 'layer', see module docstring),
     ``batch_prompts`` (accept several prompts per generation: N independent single-prompt traces sharing each launch;
-    the reference rejects this, trace.py:172-173) and ``locate_middle_block`` (also locate the mid block without
-    enabling save/load of heads -- BASELINE config 5 "all 16+70 layers").
+    the reference rejects this, trace.py:172-173), ``locate_middle_block`` (also locate the mid block without
+    enabling save/load of heads -- BASELINE config 5 "all 16+70 layers") and ``time_resolved`` (also keep one global
+    heat map per denoising step, see :meth:`compute_time_heat_maps`).
     """
 
     def __init__(self, pipeline, low_memory: bool = False, load_heads: bool = False, save_heads: bool = False,
                  data_dir: str = None, *, launch: str = 'step', batch_prompts: bool = False,
-                 locate_middle_block: bool = False, kernel_flags: int = _native.ACC_AUTO):
+                 locate_middle_block: bool = False, kernel_flags: int = _native.ACC_AUTO, time_resolved: bool = False):
         if launch not in ('step', 'overlap', 'layer'):
             raise ValueError("launch must be 'step', 'overlap' or 'layer'")
+        if time_resolved and launch != 'step':
+            raise ValueError("time_resolved=True needs launch='step': the per-step heat map is finalized right after "
+                             "the step's launch, on the forward's own stream")
+        if time_resolved and (save_heads or load_heads):
+            raise ValueError('time_resolved=True does not support save_heads / load_heads')
         _native.load()   # fail here, loudly, if the CUDA library is missing
         self.all_heat_maps = RawHeatMapCollection()
         side = pipeline.unet.config.sample_size * pipeline.vae_scale_factor
@@ -79,6 +89,14 @@ class DiffusionHeatMapHooker(AggregateHooker):
         self._stream: Optional[torch.cuda.Stream] = None
         self._dirty = False                    # side-stream work not yet ordered before the current stream
         self.all_heat_maps.bind(self.synchronize, self._zero_slabs)
+        # time-resolved mode: the step slab of every slot of the step array, and per prompt a device history
+        # [capacity, n_rows, x, x] of per-step global heat maps (grown by doubling, restarted every generation)
+        self.time_resolved = time_resolved
+        self.all_heat_maps.time_resolved = time_resolved
+        self._step_ptrs = _native.StepPointers([0] * 64) if time_resolved else None
+        self._history: List[torch.Tensor] = []
+        self._time_steps = 0
+        self._history_rows: Optional[List[int]] = None   # n_rows of every prompt of the running generation
 
         modules = [
             UNetCrossAttentionHooker(m, self, layer_idx=idx, latent_hw=self.latent_hw, load_heads=load_heads,
@@ -199,7 +217,12 @@ class DiffusionHeatMapHooker(AggregateHooker):
                 self._packed = grown
                 self._slots = [grown.array[i] for i in range(len(grown.array))]
                 self._layer_state.clear()                  # cached slot proxies point into the old array
+                if self._step_ptrs is not None:
+                    old = list(self._step_ptrs.array)
+                    self._step_ptrs = _native.StepPointers(old + [0] * (len(grown.array) - len(old)))
             self._packed.array[pos] = desc
+            if self._step_ptrs is not None:
+                self._step_ptrs.array[pos] = slab.step.data_ptr()
             slot, own = self._slots[pos], None
         else:
             own = _native.PackedLayers([desc])             # 'layer' mode: every layer launches its own 1-element array
@@ -255,13 +278,22 @@ class DiffusionHeatMapHooker(AggregateHooker):
         try:
             capturing = torch.cuda.is_current_stream_capturing()
             if capturing:
+                if self.time_resolved:                         # drop the step: its projections live in the graph's pool
+                    self._refs, self._n_pending = [], 0
+                    raise RuntimeError('time_resolved=True cannot be captured into a CUDA graph: every step writes its '
+                                       'heat map into another history slot, which a graph replay cannot follow')
                 # CUDA-graph capture of the UNet step: the launch becomes a node of the captured stream; replays bypass the
                 # Python hook, so the layers of this launch stay live across per-generation resets
                 step = self._step_id
                 for layer_idx, st in self._layer_state.items():
                     if self._queued.get(layer_idx) == step:
                         st[4].captured = True
-            if capturing or self.launch == 'step':
+            if self.time_resolved:
+                # launch == 'step' (checked at construction): on the forward's own stream, like the branch below; then
+                # the step's global heat maps, in stream order behind it
+                _native.accumulate_steps(packed, self._step_ptrs, current, flags)
+                self._finalize_step(device, current)
+            elif capturing or self.launch == 'step':
                 # On the forward's own stream: the predecessor there is the tail of the UNet forward, never a producer of
                 # the queued Q/K, so only the accumulator updates have to wait for it (EARLY_LOADS). Stream order also
                 # makes it safe to drop the projections right after the launch.
@@ -287,6 +319,37 @@ class DiffusionHeatMapHooker(AggregateHooker):
         self._refs = []
         self._n_pending = 0
         self._step_id += 1
+
+    def _finalize_step(self, device, stream: int):
+        """Time-resolved mode, right after the step's launch on ``stream``: for every prompt, the global heat map of the
+        step slabs this step wrote -- the same reduction, key order (live-slab order) and row count as
+        :meth:`compute_global_heat_map` -- into the next slot of the prompt's history."""
+        queued = {idx for idx, step in self._queued.items() if step == self._step_id}
+        slabs = [s for s in self.all_heat_maps.live_slabs() if s.layer_idx in queued]
+        x = int(np.sqrt(self.latent_hw))
+        t = self._time_steps
+        prompts = self.last_prompts or [self.last_prompt]
+        if self._history_rows is None:
+            self._history_rows = [min(len(self.pipe.tokenizer.tokenize(p)) + 2, _native.TOKENS) for p in prompts]
+        for p in range(slabs[0].n_prompts):
+            n_rows = self._history_rows[p] if p < len(self._history_rows) else self._history_rows[0]
+            if p == len(self._history):
+                self._history.append(torch.empty((16, n_rows, x, x), dtype=torch.float32, device=device))
+            hist = self._history[p]
+            if t == hist.shape[0]:                          # grow by doubling, in stream order between two steps
+                grown = torch.empty((2 * t,) + tuple(hist.shape[1:]), dtype=torch.float32, device=device)
+                grown[:t].copy_(hist)
+                self._history[p] = hist = grown
+            groups = [_native.DaamKeyGroup(acc=s.step[p].data_ptr(), heads=s.heads, h=s.h, w=s.w,
+                                           tokens=s.step.shape[2], head_sel=-1, reserved=0) for s in slabs]
+            _native.finalize(groups, x, n_rows, False, hist[t].data_ptr(), stream)
+        self._time_steps = t + 1
+
+    def _restart_history(self):
+        """A new generation: a new per-step history (maps handed out earlier stay valid: they are other tensors)."""
+        self._history = []
+        self._time_steps = 0
+        self._history_rows = None
 
     def synchronize(self):
         """Make every accumulate issued so far visible to work enqueued on the current stream afterwards."""
@@ -343,6 +406,28 @@ class DiffusionHeatMapHooker(AggregateHooker):
             _native.finalize(groups, x, n_rows, normalize, maps.data_ptr(),
                              torch.cuda.current_stream(device).cuda_stream)
         return GlobalHeatMap(self.pipe.tokenizer, prompt, maps)
+
+    def compute_time_heat_maps(self, prompt_idx: int = 0, normalize: bool = False) -> TimeHeatMaps:
+        """One global heat map per traced denoising step (UNet forward) of the running / last generation; needs
+        ``trace(pipe, time_resolved=True)``. ``heat_maps[t]`` is what :meth:`compute_global_heat_map` would return had
+        only step ``t`` been traced, with every key and layer; ``normalize`` applies the reference's normalisation to
+        each step. Summing the steps does not give the all-steps map: there the clamp comes after the time sum.
+
+        Costs: a second fp32 slab per traced layer (as large as its accumulator) and ``steps x n_rows x x x x`` fp32 of
+        history per prompt."""
+        if not self.time_resolved:
+            raise RuntimeError('per-step heat maps need trace(pipe, time_resolved=True)')
+        self.synchronize()
+        if self._time_steps == 0 or not 0 <= prompt_idx < len(self._history):
+            raise RuntimeError('No heat maps found. Did you forget to call `with trace(...)` during generation?')
+        prompt = self.last_prompts[prompt_idx] if self.last_prompts else self.last_prompt
+        maps = self._history[prompt_idx][:self._time_steps]
+        if normalize:
+            maps = maps.clone()
+            with torch.cuda.device(maps.device):
+                _native.normalize_maps(maps.data_ptr(), maps.shape[0], maps.shape[1], maps.shape[-1],
+                                       torch.cuda.current_stream(maps.device).cuda_stream)
+        return TimeHeatMaps(self.pipe.tokenizer, prompt, maps)
 
 
     def compute_per_head_heat_maps(self, prompt=None, factors=None, normalize=False, prompt_idx: int = 0):
@@ -418,6 +503,7 @@ class PipelineHooker(ObjectHooker):
             if len(prompts) > 1 and not tr.batch_prompts:
                 raise ValueError('Only single prompt generation is supported for heat map computation.')
         hk_self.heat_maps.clear()
+        tr._restart_history()
         if len(prompts) != len(tr.last_prompts):    # slabs are laid out [prompts][images * heads]: re-derive them
             tr._layer_state.clear()
         tr.last_prompt = prompts[0]

@@ -25,7 +25,8 @@ extern "C" {
 #endif
 
 #define DAAM_ABI_VERSION 3          /* 2: + daam_attention_probs, daam_accumulate_probs, daam_finalize_per_key
-                                       3: + DAAM_ACC_EARLY_LOADS, daam_expand_words, daam_side_launcher_* */
+                                       3: + DAAM_ACC_EARLY_LOADS, daam_expand_words, daam_side_launcher_*
+                                          (later, additive: daam_accumulate_steps, daam_normalize_maps) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
 
@@ -91,6 +92,18 @@ typedef struct daam_layer {
 /* Enqueue the fused softmax(QK^T) -> unravel -> accumulate kernel over `n_layers` layer calls (any number; the
  * library packs them into as few persistent launches as possible). `layers` is host memory, read before returning. */
 int daam_accumulate(const daam_layer* layers, int32_t n_layers, uint32_t flags, void* stream);
+
+/*
+ * Time-resolved heat maps (daam_b200/trace.py, trace(..., time_resolved=True)): daam_accumulate, and also
+ *   step_acc[i][p][head][t][pixel] = the value added (flushed like the add)
+ * so that one denoising step's per-key maps exist next to the time sum. With acc == 0 beforehand, step_acc equals acc
+ * afterwards bit for bit. Every element of every step slab is written; nothing else is.
+ * step_acc: host array of n_layers device pointers, fp32, 16-byte aligned, same shape as layers[i].acc. A step slab
+ * must not overlap any accumulator or any other step slab of the call (DAAM_E_INVALID). Same flags and packing as
+ * daam_accumulate; with DAAM_ACC_EARLY_LOADS the step-slab stores, too, wait for the previous kernel.
+ */
+int daam_accumulate_steps(const daam_layer* layers, float* const* step_acc, int32_t n_layers, uint32_t flags,
+                          void* stream);
 
 /*
  * The tracer's optional side-stream launch (daam_b200/trace.py flush, launch='overlap'): the reference's hook does its
@@ -160,6 +173,13 @@ int daam_finalize(const daam_key_group* groups, int32_t n_groups, int32_t x, int
  */
 int daam_finalize_per_key(const daam_key_group* groups, int32_t n_groups, int32_t x, int32_t n_rows, int32_t normalize,
                           float* out, void* stream);
+
+/*
+ * The `normalize` step of daam_finalize on its own, in place, for n_maps independent [n_rows][x][x] heat maps stored
+ * back to back (e.g. the per-step global maps of a time-resolved trace): maps / (sum of rows 1..n_rows-2 + 1e-6) per
+ * pixel, the same arithmetic as daam_finalize(normalize = 1).
+ */
+int daam_normalize_maps(float* maps, int32_t n_maps, int32_t n_rows, int32_t x, void* stream);
 
 /*
  * Replaces GlobalHeatMap.compute_word_heat_map's tensor part (daam/heatmap.py:121-123): mean over the rows
