@@ -203,14 +203,15 @@ int build_plan(const daam_layer* layers, float* const* steps, int n_layers, uint
     }
     const int which = use_mma ? (L.dtype == DAAM_F32 ? 1 : 0) : 2;
     LaunchParams& p = packs[which];
-    // The 16-bit wgmma form reads, adds and stores whole accumulator tiles, so two layers of one launch must not share
-    // accumulator elements: a layer whose slab overlaps one already in the pack starts the next launch (stream order).
-    if (which == 0)
-      for (int m = 0; m < p.n_layers; ++m)
-        if (acc_overlap(p.layer[m], L)) {
-          if (int rc = close(0)) return rc;
-          break;
-        }
+    // Two layers of one launch must not share accumulator elements: their tiles run concurrently, and the 16-bit wgmma
+    // form and the LDST mode read, add and store them (lost updates), while RED would add in timing order (results not
+    // deterministic). A layer whose slab overlaps one already in its pack starts that pack's next launch; stream order
+    // then applies the two in call order.
+    for (int m = 0; m < p.n_layers; ++m)
+      if (acc_overlap(p.layer[m], L)) {
+        if (int rc = close(which)) return rc;
+        break;
+      }
     L.tile_begin = p.total_tiles;
     // Cost of a tile relative to the launch's other layers (SD-1.5's 40 / 80 / 160 head dims): every 64-wide K chunk is
     // one load -> (convert ->) MMA round through the two-stage ring. In the fp32 split form that chain is the whole cost

@@ -48,8 +48,8 @@ enum daam_dtype { DAAM_F32 = 0, DAAM_F16 = 1, DAAM_BF16 = 2 };
    form ignores these flags: it always adds in shared memory, into accumulator tiles loaded ahead by TMA, and stores
    them back, with the same arithmetic as RED. */
 #define DAAM_ACC_RMW_MASK   0x30u
-#define DAAM_ACC_RMW_AUTO   0x00u /* = RED on both paths (one add per element per launch, so results stay
-                                     deterministic) */
+#define DAAM_ACC_RMW_AUTO   0x00u /* = RED on both paths (one add per element per launch -- layers whose
+                                     accumulators overlap go to separate launches -- so results stay deterministic) */
 #define DAAM_ACC_RMW_LDST   0x10u /* coalesced load / add / store of the accumulator tile */
 #define DAAM_ACC_RMW_RED    0x20u /* red.global.add.f32 (SIMT) / bulk-async reduce-add from shared memory (MMA) */
 #define DAAM_ACC_NO_PDL     0x100u /* launch without programmatic dependent launch (measurement / debugging) */
@@ -90,7 +90,10 @@ typedef struct daam_layer {
 } daam_layer;
 
 /* Enqueue the fused softmax(QK^T) -> unravel -> accumulate kernel over `n_layers` layer calls (any number; the
- * library packs them into as few persistent launches as possible). `layers` is host memory, read before returning. */
+ * library packs them into as few persistent launches as possible). `layers` is host memory, read before returning.
+ * Layers may share accumulator elements (the same or overlapping slabs): such a layer starts a new launch, so on every
+ * path and in every update mode each one adds, and layers of one operand class are applied in call order. Layers of
+ * different classes (16-bit wgmma, fp32 wgmma, SIMT) go to different launches, issued class by class. */
 int daam_accumulate(const daam_layer* layers, int32_t n_layers, uint32_t flags, void* stream);
 
 /*
