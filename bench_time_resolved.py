@@ -9,7 +9,9 @@ addend into a step slab per layer) and one ``daam_finalize`` per prompt over tho
 script times both on the same resident prompt sets, rotation, blocks and medians as the value leg of ``bench.py``
 (whose workload shapes and byte counts it imports): the accumulate alone, the finalize alone, and both per step, in µs
 per step, with their algorithmic bytes. The finalize reduces all 77 rows (the longest prompt), so it reads every step
-slab once. One JSON line goes to stdout.
+slab once. A last leg times ``daam_accumulate_range`` (the accumulate of ``trace(pipe, step_ranges=[...])`` while a step
+lies in a declared range: it also adds each step's addend into a range slab per layer) on the same sets. One JSON line
+goes to stdout.
 
 ``--dump-outputs DIR`` writes the step slabs of the last timed step (``step_layerNN.npy``, float32, sampled above 64 MB
 like ``bench.py --dump-outputs``). Nothing is written anywhere else.
@@ -58,11 +60,13 @@ def main():
 
     with torch.no_grad():
         sets = bench.build_sets(layers, args.prompts, dtype, n_sets, 1234)
-        slabs, ptrs, groups = [], [], []
+        slabs, ptrs, groups, ranges, range_ptrs = [], [], [], [], []
         for _, keep in sets:
             step = [torch.empty_like(acc) for _, _, acc in keep]
             slabs.append(step)
             ptrs.append(_native.StepPointers([s.data_ptr() for s in step]))
+            ranges.append([torch.zeros_like(acc) for _, _, acc in keep])
+            range_ptrs.append(_native.StepPointers([r.data_ptr() for r in ranges[-1]]))
             groups.append([[_native.DaamKeyGroup(acc=s[p].data_ptr(), heads=s.shape[1], h=int(hw ** 0.5),
                                                  w=int(hw ** 0.5), tokens=TOKENS, head_sel=-1, reserved=0)
                             for s, (hw, _, _) in zip(step, layers)] for p in range(args.prompts)])
@@ -79,6 +83,9 @@ def main():
         def both(i):
             accumulate(i)
             finalize(i)
+
+        def accumulate_range(i):
+            ops.accumulate_range(sets[i % n_sets][0], range_ptrs[i % n_sets], 'cuda', stream, flags)
 
         def timed(fn):
             """Median over blocks of the per-step device time; each block is queued behind a spin kernel so that host
@@ -104,6 +111,7 @@ def main():
         acc_us, _ = timed(accumulate)
         fin_us, _ = timed(finalize)
         both_us, last = timed(both)
+        range_us, _ = timed(accumulate_range)
         wall = time.time() - t0
 
     esize = 4 if dtype == torch.float32 else 2
@@ -111,6 +119,7 @@ def main():
     plain_bytes = bench.algorithmic_bytes_per_step(layers, args.prompts, esize)
     acc_bytes = plain_bytes + px * 4                                              # + the step-slab write
     fin_bytes = px * 4 + args.prompts * n_rows * x * x * 4                        # step slabs read, maps written
+    range_bytes = plain_bytes + 2 * px * 4                                        # + the range-slab read and write
     peak, peak_src = bench.measured_peak()
     if args.dump_outputs:
         bench.dump_outputs(args.dump_outputs, {f'step_layer{i:02d}': s for i, s in enumerate(slabs[(last - 1) % n_sets])})
@@ -122,6 +131,9 @@ def main():
         'accumulate_steps_gbs': round(acc_bytes / (acc_us * 1e-6) / 1e9, 1),
         'finalize_gbs': round(fin_bytes / (fin_us * 1e-6) / 1e9, 1),
         'accumulate_steps_frac_of_peak': round(acc_bytes / (acc_us * 1e-6) / 1e9 / peak, 4),
+        'accumulate_range_us': round(range_us, 3), 'accumulate_range_bytes': range_bytes,
+        'accumulate_range_gbs': round(range_bytes / (range_us * 1e-6) / 1e9, 1),
+        'accumulate_range_frac_of_peak': round(range_bytes / (range_us * 1e-6) / 1e9 / peak, 4),
         'peak_gbs': peak, 'peak_source': peak_src, 'finalize_rows': n_rows, 'x': x,
         'timing': f'median of {len(bench.block_sizes(args.steps))} blocks of K={args.steps} steps (CUDA events, launches '
                   f'queued behind a spin kernel), rotating over {n_sets} prompt sets, {wall:.1f} s',

@@ -23,7 +23,7 @@ E_INVALID, E_UNSUPPORTED, E_CUDA = -1, -2, -3
 TOKENS = 77
 EXPAND_SCRATCH_FLOATS = 64   # DAAM_EXPAND_SCRATCH_FLOATS: per word
 
-EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize',
+EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize',
            'daam_finalize_per_key', 'daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
            'daam_side_launcher_create', 'daam_side_launcher_destroy',
            'daam_side_launcher_launch', 'daam_side_launcher_join', 'daam_side_launcher_idle', 'daam_abi_version',
@@ -79,6 +79,8 @@ def load() -> ctypes.CDLL:
     lib.daam_accumulate.restype = ctypes.c_int
     lib.daam_accumulate_steps.argtypes = [ctypes.POINTER(DaamLayer), ctypes.POINTER(vp), i32, u32, vp]
     lib.daam_accumulate_steps.restype = ctypes.c_int
+    lib.daam_accumulate_range.argtypes = [ctypes.POINTER(DaamLayer), ctypes.POINTER(vp), i32, u32, vp]
+    lib.daam_accumulate_range.restype = ctypes.c_int
     lib.daam_normalize_maps.argtypes = [vp, i32, i32, i32, vp]
     lib.daam_normalize_maps.restype = ctypes.c_int
     lib.daam_attention_probs.argtypes = [ctypes.POINTER(DaamLayer), vp, vp]
@@ -177,7 +179,8 @@ def accumulate(layers, stream: int, flags: int = ACC_AUTO):
 
 
 class StepPointers:
-    """A ready-made ``float* step_acc[]`` (host array of device pointers) for :func:`accumulate_steps`."""
+    """A ready-made ``float* step_acc[]`` / ``range_acc[]`` (host array of device pointers) for
+    :func:`accumulate_steps` and :func:`accumulate_range`."""
 
     def __init__(self, ptrs: Sequence[int]):
         self.array = (ctypes.c_void_p * max(len(ptrs), 1))(*ptrs)
@@ -193,6 +196,20 @@ def accumulate_steps(layers, steps, stream: int, flags: int = ACC_AUTO):
     if len(arr.array) < packed.n:
         raise ValueError(f'{len(arr.array)} step slabs for {packed.n} layers')
     rc = load().daam_accumulate_steps(packed.array, arr.array, packed.n, flags, stream)
+    if rc != 0:
+        _check(rc)
+
+
+def accumulate_range(layers, ranges, stream: int, flags: int = ACC_AUTO):
+    """``daam_accumulate_range``: ``layers`` as for :func:`accumulate`; ``ranges`` a :class:`StepPointers` or a sequence
+    of device pointers, one range slab per layer (the first ``n`` are used)."""
+    packed = layers if isinstance(layers, PackedLayers) else PackedLayers(layers)
+    if packed.n == 0:
+        return
+    arr = ranges if isinstance(ranges, StepPointers) else StepPointers(ranges)
+    if len(arr.array) < packed.n:
+        raise ValueError(f'{len(arr.array)} range slabs for {packed.n} layers')
+    rc = load().daam_accumulate_range(packed.array, arr.array, packed.n, flags, stream)
     if rc != 0:
         _check(rc)
 

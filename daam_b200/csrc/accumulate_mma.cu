@@ -38,6 +38,13 @@
 //                same bulk group. Before sS is rewritten, that thread waits for the previous group's reads.
 //   split form : red mode stages the flushed p in sP (the reduce flushes its inputs anyway) and bulk-stores sP next to
 //                the reduce; ldst mode writes p to the step slab in its coalesced load / add / store pass.
+// Range-slab instances (kSlab == kSlabAdd, daam_accumulate_range): every form also ADDS what it adds into a second slab,
+// with the arithmetic it applies to the accumulator, so that a slab zeroed before a span of steps ends up holding
+// exactly the accumulator a trace of only those steps would hold.
+//   16-bit form: sS as in the step form (p flushed, as add.rn.ftz sees it); in place of the step store, a bulk-tensor
+//                reduce-add from sS into the range slab, in the same bulk group (the reduce flushes like add.rn.ftz).
+//   split form : red mode issues a second reduce-add from sP; ldst mode loads, adds and stores the range slab in its
+//                coalesced pass, like the accumulator.
 //
 // Replaces daam/trace.py:276 (get_attention_scores), :219-244 (_unravel_attn) and :293-294 (update loop).
 #include <cuda.h>
@@ -286,10 +293,12 @@ __device__ __forceinline__ void wgmma_chunk_16bit(Frag& d, uint32_t a_src, uint3
 __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 // kChunked: some layer of the launch has head_dim > 64 (several K chunks per tile); the common single-chunk case keeps
-// its simpler loops (one load iteration per tile). kStep: also store each tile's probabilities into the step slab.
-template <bool kSplit, bool kChunked, bool kStep>
+// its simpler loops (one load iteration per tile). kSlab: also store (kSlabStore) or add (kSlabAdd) each tile's
+// probabilities into the second slab.
+template <bool kSplit, bool kChunked, int kSlab>
 __global__ void __launch_bounds__(kSplit ? kThreads : kThreads16, 1)
-accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kStep> MP) {
+accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP) {
+  constexpr bool kStep = kSlab != kSlabNone;          // a second slab (the step-form code paths, store or add)
   constexpr int kStageBytesT = kSplit ? kSplitStageBytes : kStageBytes;
   constexpr int kOperandBytes = (kSplit ? kStages + 1 : kStages) * kStageBytesT;     // stages (+ the lo buffer)
   // staged probabilities (split) / the accumulator ring (16-bit), + sS (16-bit step form)
@@ -532,8 +541,10 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kStep> MP) {
         consumer_barrier();
         if (tid == 0) {
           tma_store_2d(&MP.amap[t.li], sP_u32 + a * kPBytes, t.pixel0, (t.prompt * L.heads + t.head) * kTokens);
-          if constexpr (kStep)                         // same bulk group: the waits below cover both stores
+          if constexpr (kSlab == kSlabStore)           // same bulk group: the waits below cover both stores
             tma_store_2d(&MP.smap[t.li], sS_u32, t.pixel0, (t.prompt * L.heads + t.head) * kTokens);
+          if constexpr (kSlab == kSlabAdd)             // (and the range reduce: its reads of sS)
+            tma_reduce_add_2d(&MP.smap[t.li], sS_u32, t.pixel0, (t.prompt * L.heads + t.head) * kTokens);
           bulk_commit();
           if (i > 0) {                                 // one store of slack: the previous tile's store has read its slot
             bulk_wait_read1();
@@ -553,7 +564,7 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kStep> MP) {
       consumer_barrier();                              // ... and (ldst mode) every thread has read the previous tile
       const bool lowq = quad < 2;
       // step form, red mode: stage p as the reduce sees it (flushed), so that one buffer serves the reduce and the store
-      const bool stage_ftz = kStep && P.rmw_mode == 1;
+      const bool stage_ftz = kSlab == kSlabStore && P.rmw_mode == 1;
 #pragma unroll
       for (int jj = 0; jj < 10; ++jj) {
 #pragma unroll
@@ -574,7 +585,10 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kStep> MP) {
         consumer_barrier();
         if (tid == 0) {
           tma_reduce_add_2d(&MP.amap[t.li], sP_u32, t.pixel0, (t.prompt * L.heads + t.head) * kTokens);
-          if constexpr (kStep) tma_store_2d(&MP.smap[t.li], sP_u32, t.pixel0, (t.prompt * L.heads + t.head) * kTokens);
+          if constexpr (kSlab == kSlabStore)
+            tma_store_2d(&MP.smap[t.li], sP_u32, t.pixel0, (t.prompt * L.heads + t.head) * kTokens);
+          if constexpr (kSlab == kSlabAdd)
+            tma_reduce_add_2d(&MP.smap[t.li], sP_u32, t.pixel0, (t.prompt * L.heads + t.head) * kTokens);
           bulk_commit();
         }
         issued = true;
@@ -591,8 +605,14 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kStep> MP) {
             float4 o = *g;
             o.x += p.x; o.y += p.y; o.z += p.z; o.w += p.w;
             *g = o;
-            if constexpr (kStep)
+            if constexpr (kSlab == kSlabStore)
               reinterpret_cast<float4*>(MP.step[t.li] + (acc - L.acc) + tok * hw)[c4] = p;
+            if constexpr (kSlab == kSlabAdd) {
+              float4* r = reinterpret_cast<float4*>(MP.step[t.li] + (acc - L.acc) + tok * hw) + c4;
+              float4 ro = *r;
+              ro.x += p.x; ro.y += p.y; ro.z += p.z; ro.w += p.w;
+              *r = ro;
+            }
           }
         }
       }
@@ -708,7 +728,7 @@ std::once_flag g_attr_once[64];                       // the shared-memory attri
 struct PreparedMma {
   MmaStepParams mp;                                   // the plain instances are launched with its MmaParams part
   int grid, block, smem, variant;                     // variant: bit 0 split (fp32), bit 1 chunked (head_dim > 64),
-};                                                    // bit 2 step slabs
+};                                                    // bits 2-3 the SlabMode (1 step slabs, 2 range slabs)
 void* prepared_mma_new() { return new PreparedMma; }                 // (aligned new: CUtensorMap is alignas(64))
 void prepared_mma_delete(void* p) { delete static_cast<PreparedMma*>(p); }
 
@@ -718,7 +738,8 @@ bool mma_supported(const LayerParams& L) {
 }
 
 // Tensor maps, grid and kernel variant of one pack of layers (all fp32, or all 16-bit). `out`: prepared_mma_new().
-int prepare_accumulate_mma(const LaunchParams& p, const StepSlabs* steps, const DeviceInfo& dev, void* out) {
+int prepare_accumulate_mma(const LaunchParams& p, const StepSlabs* steps, SlabMode mode, const DeviceInfo& dev,
+                           void* out) {
   if (dev.cc_major != 9) { set_error("the wgmma kernel needs an sm_90 device (found sm_%d%d)", dev.cc_major, dev.cc_minor); return DAAM_E_UNSUPPORTED; }
   PreparedMma& pm = *static_cast<PreparedMma*>(out);
   MmaStepParams& mp = pm.mp;
@@ -731,7 +752,7 @@ int prepare_accumulate_mma(const LaunchParams& p, const StepSlabs* steps, const 
     if (int rc = make_qk_map(L.q, L.dtype, L.head_dim, L.heads, L.hw, L.n_prompts, L.qs_head, L.qs_pixel, L.qs_prompt, kTilePixels, &mp.qmap[i])) return rc;
     if (int rc = make_qk_map(L.k, L.dtype, L.head_dim, L.heads, kTokens, L.n_prompts, L.ks_head, L.ks_token, L.ks_prompt, kTokensPad, &mp.kmap[i])) return rc;
     if (int rc = make_acc_map(L.acc, L.hw, L.n_prompts * L.heads * kTokens, &mp.amap[i])) return rc;
-    if (steps) {                                      // the step slab has the accumulator's shape: same map, other base
+    if (steps) {                                      // the second slab has the accumulator's shape: same map, other base
       if (int rc = make_acc_map(steps->step[i], L.hw, L.n_prompts * L.heads * kTokens, &mp.smap[i])) return rc;
       mp.step[i] = steps->step[i];
     }
@@ -743,31 +764,36 @@ int prepare_accumulate_mma(const LaunchParams& p, const StepSlabs* steps, const 
       cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
       if (e != cudaSuccess) attr_err = e;
     };
-    set((const void*)accumulate_mma_kernel<false, false, false>, kSmemBytes);
-    set((const void*)accumulate_mma_kernel<false, true, false>, kSmemBytes);
-    set((const void*)accumulate_mma_kernel<true, false, false>, kSplitSmemBytes);
-    set((const void*)accumulate_mma_kernel<true, true, false>, kSplitSmemBytes);
-    set((const void*)accumulate_mma_kernel<false, false, true>, kStepSmemBytes);
-    set((const void*)accumulate_mma_kernel<false, true, true>, kStepSmemBytes);
-    set((const void*)accumulate_mma_kernel<true, false, true>, kSplitSmemBytes);
-    set((const void*)accumulate_mma_kernel<true, true, true>, kSplitSmemBytes);
+    set((const void*)accumulate_mma_kernel<false, false, kSlabNone>, kSmemBytes);
+    set((const void*)accumulate_mma_kernel<false, true, kSlabNone>, kSmemBytes);
+    set((const void*)accumulate_mma_kernel<true, false, kSlabNone>, kSplitSmemBytes);
+    set((const void*)accumulate_mma_kernel<true, true, kSlabNone>, kSplitSmemBytes);
+    set((const void*)accumulate_mma_kernel<false, false, kSlabStore>, kStepSmemBytes);
+    set((const void*)accumulate_mma_kernel<false, true, kSlabStore>, kStepSmemBytes);
+    set((const void*)accumulate_mma_kernel<true, false, kSlabStore>, kSplitSmemBytes);
+    set((const void*)accumulate_mma_kernel<true, true, kSlabStore>, kSplitSmemBytes);
+    set((const void*)accumulate_mma_kernel<false, false, kSlabAdd>, kStepSmemBytes);
+    set((const void*)accumulate_mma_kernel<false, true, kSlabAdd>, kStepSmemBytes);
+    set((const void*)accumulate_mma_kernel<true, false, kSlabAdd>, kSplitSmemBytes);
+    set((const void*)accumulate_mma_kernel<true, true, kSlabAdd>, kSplitSmemBytes);
   });
   DAAM_CUDA_TRY(attr_err);
   pm.grid = dev.sm_count;                             // one CTA per SM (both forms fill its shared memory)
   if (pm.grid > p.total_tiles) pm.grid = p.total_tiles;
   pm.block = split ? kThreads : kThreads16;
   pm.smem = split ? kSplitSmemBytes : (steps ? kStepSmemBytes : kSmemBytes);
-  pm.variant = (split ? 1 : 0) | (chunked ? 2 : 0) | (steps ? 4 : 0);
+  pm.variant = (split ? 1 : 0) | (chunked ? 2 : 0) | (mode << 2);
   return DAAM_OK;
 }
 
 namespace {
-template <bool kSplit, bool kChunked, bool kStep>
+template <bool kSplit, bool kChunked, int kSlab>
 cudaError_t launch_variant(const cudaLaunchConfig_t& cfg, const PreparedMma& pm) {
-  if constexpr (kStep)
-    return cudaLaunchKernelEx(&cfg, accumulate_mma_kernel<kSplit, kChunked, true>, pm.mp);
+  if constexpr (kSlab != kSlabNone)
+    return cudaLaunchKernelEx(&cfg, accumulate_mma_kernel<kSplit, kChunked, kSlab>, pm.mp);
   else
-    return cudaLaunchKernelEx(&cfg, accumulate_mma_kernel<kSplit, kChunked, false>, static_cast<const MmaParams&>(pm.mp));
+    return cudaLaunchKernelEx(&cfg, accumulate_mma_kernel<kSplit, kChunked, kSlabNone>,
+                              static_cast<const MmaParams&>(pm.mp));
 }
 }  // namespace
 
@@ -786,14 +812,18 @@ int launch_prepared_mma(const void* prepared, cudaStream_t stream) {
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   switch (pm.variant) {
-    case 0: DAAM_CUDA_TRY((launch_variant<false, false, false>(cfg, pm))); break;
-    case 1: DAAM_CUDA_TRY((launch_variant<true, false, false>(cfg, pm))); break;
-    case 2: DAAM_CUDA_TRY((launch_variant<false, true, false>(cfg, pm))); break;
-    case 3: DAAM_CUDA_TRY((launch_variant<true, true, false>(cfg, pm))); break;
-    case 4: DAAM_CUDA_TRY((launch_variant<false, false, true>(cfg, pm))); break;
-    case 5: DAAM_CUDA_TRY((launch_variant<true, false, true>(cfg, pm))); break;
-    case 6: DAAM_CUDA_TRY((launch_variant<false, true, true>(cfg, pm))); break;
-    default: DAAM_CUDA_TRY((launch_variant<true, true, true>(cfg, pm))); break;
+    case 0: DAAM_CUDA_TRY((launch_variant<false, false, kSlabNone>(cfg, pm))); break;
+    case 1: DAAM_CUDA_TRY((launch_variant<true, false, kSlabNone>(cfg, pm))); break;
+    case 2: DAAM_CUDA_TRY((launch_variant<false, true, kSlabNone>(cfg, pm))); break;
+    case 3: DAAM_CUDA_TRY((launch_variant<true, true, kSlabNone>(cfg, pm))); break;
+    case 4: DAAM_CUDA_TRY((launch_variant<false, false, kSlabStore>(cfg, pm))); break;
+    case 5: DAAM_CUDA_TRY((launch_variant<true, false, kSlabStore>(cfg, pm))); break;
+    case 6: DAAM_CUDA_TRY((launch_variant<false, true, kSlabStore>(cfg, pm))); break;
+    case 7: DAAM_CUDA_TRY((launch_variant<true, true, kSlabStore>(cfg, pm))); break;
+    case 8: DAAM_CUDA_TRY((launch_variant<false, false, kSlabAdd>(cfg, pm))); break;
+    case 9: DAAM_CUDA_TRY((launch_variant<true, false, kSlabAdd>(cfg, pm))); break;
+    case 10: DAAM_CUDA_TRY((launch_variant<false, true, kSlabAdd>(cfg, pm))); break;
+    default: DAAM_CUDA_TRY((launch_variant<true, true, kSlabAdd>(cfg, pm))); break;
   }
   DAAM_CUDA_TRY(cudaGetLastError());
   count_launch();

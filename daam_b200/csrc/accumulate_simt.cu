@@ -9,6 +9,8 @@
 // The step-slab kernel (daam_accumulate_steps) is the same body with kStep: next to every add it stores the addend into
 // the layer's step slab, again one coalesced 128-byte access per warp and token (flushed like RED in reduce mode; in
 // load / add / store mode the add is an fma, so the stored value is the rounded product, i.e. fma(p, inv, 0)).
+// The range-slab kernel (daam_accumulate_range) adds the addend into the layer's range slab with the arithmetic of the
+// accumulator update: a second RED in reduce mode, fma(p, inv, old) in load / add / store mode.
 #include <mutex>
 
 #include "simt_common.cuh"
@@ -16,7 +18,7 @@
 namespace daam {
 namespace {
 
-template <bool kStep>
+template <int kSlab>
 __device__ __forceinline__ void accumulate_simt_body(const LaunchParams& P, const StepSlabs* S) {
   extern __shared__ __align__(16) float smem[];
   // contiguous chunk of tiles per CTA: consecutive tiles share (layer, prompt, head), so K^T is staged once per run
@@ -49,7 +51,8 @@ __device__ __forceinline__ void accumulate_simt_body(const LaunchParams& P, cons
 #pragma unroll
         for (int j = 0; j < kTokens; ++j) {
           atomicAdd(a + j * hw, s[j] * inv);          // result unused -> RED
-          if constexpr (kStep) S->step[t.li][off + j * hw] = add_ftz(0.f, s[j] * inv);
+          if constexpr (kSlab == kSlabStore) S->step[t.li][off + j * hw] = add_ftz(0.f, s[j] * inv);
+          if constexpr (kSlab == kSlabAdd) atomicAdd(S->step[t.li] + off + j * hw, s[j] * inv);
         }
       } else {
         constexpr int kChunk = 11;                    // 77 = 7 x 11 loads in flight per thread
@@ -58,9 +61,17 @@ __device__ __forceinline__ void accumulate_simt_body(const LaunchParams& P, cons
           float old[kChunk];
 #pragma unroll
           for (int i = 0; i < kChunk; ++i) old[i] = a[(j0 + i) * hw];
+          if constexpr (kSlab == kSlabAdd) {
+            float* r = S->step[t.li] + off;
+            float old_r[kChunk];
+#pragma unroll
+            for (int i = 0; i < kChunk; ++i) old_r[i] = r[(j0 + i) * hw];
+#pragma unroll
+            for (int i = 0; i < kChunk; ++i) r[(j0 + i) * hw] = fmaf(s[j0 + i], inv, old_r[i]);
+          }
 #pragma unroll
           for (int i = 0; i < kChunk; ++i) a[(j0 + i) * hw] = fmaf(s[j0 + i], inv, old[i]);
-          if constexpr (kStep) {
+          if constexpr (kSlab == kSlabStore) {
 #pragma unroll
             for (int i = 0; i < kChunk; ++i) S->step[t.li][off + (j0 + i) * hw] = fmaf(s[j0 + i], inv, 0.f);
           }
@@ -71,27 +82,39 @@ __device__ __forceinline__ void accumulate_simt_body(const LaunchParams& P, cons
 }
 
 __global__ void __launch_bounds__(kTilePixels, 3) accumulate_simt_kernel(const __grid_constant__ LaunchParams P) {
-  accumulate_simt_body<false>(P, nullptr);
+  accumulate_simt_body<kSlabNone>(P, nullptr);
+}
+
+// (defined before the step kernel: in this order nvcc keeps the step kernel at its register count, 150 instead of 151)
+__global__ void __launch_bounds__(kTilePixels, 3)
+accumulate_simt_range_kernel(const __grid_constant__ LaunchParams P, const __grid_constant__ StepSlabs S) {
+  accumulate_simt_body<kSlabAdd>(P, &S);
 }
 
 __global__ void __launch_bounds__(kTilePixels, 3)
 accumulate_simt_step_kernel(const __grid_constant__ LaunchParams P, const __grid_constant__ StepSlabs S) {
-  accumulate_simt_body<true>(P, &S);
+  accumulate_simt_body<kSlabStore>(P, &S);
+}
+
+const void* simt_kernel(SlabMode mode) {
+  return mode == kSlabAdd     ? (const void*)accumulate_simt_range_kernel
+         : mode == kSlabStore ? (const void*)accumulate_simt_step_kernel
+                              : (const void*)accumulate_simt_kernel;
 }
 
 }  // namespace
 
-int prepare_accumulate_simt(const LaunchParams& p, const StepSlabs* steps, const DeviceInfo& dev, int* grid_out,
+int prepare_accumulate_simt(const LaunchParams& p, SlabMode mode, const DeviceInfo& dev, int* grid_out,
                             size_t* smem_out) {
   int dmax = 0;
   for (int i = 0; i < p.n_layers; ++i) dmax = p.layer[i].head_dim > dmax ? p.layer[i].head_dim : dmax;
   const size_t smem = sizeof(float) * simt::tile_smem_floats(dmax);
   static std::mutex mu;
-  static size_t configured_dev[2][64] = {};           // the attribute is per device (and per kernel)
-  const void* fn = steps ? (const void*)accumulate_simt_step_kernel : (const void*)accumulate_simt_kernel;
+  static size_t configured_dev[3][64] = {};           // the attribute is per device (and per kernel)
+  const void* fn = simt_kernel(mode);
   {
     std::lock_guard<std::mutex> lock(mu);
-    size_t& configured = configured_dev[steps ? 1 : 0][dev.device & 63];
+    size_t& configured = configured_dev[mode][dev.device & 63];
     if (smem > configured) {
       DAAM_CUDA_TRY(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
       configured = smem;
@@ -107,8 +130,11 @@ int prepare_accumulate_simt(const LaunchParams& p, const StepSlabs* steps, const
   return DAAM_OK;
 }
 
-int launch_prepared_simt(const LaunchParams& p, const StepSlabs* steps, int grid, size_t smem, cudaStream_t stream) {
-  if (steps)
+int launch_prepared_simt(const LaunchParams& p, const StepSlabs* steps, SlabMode mode, int grid, size_t smem,
+                         cudaStream_t stream) {
+  if (mode == kSlabAdd)
+    accumulate_simt_range_kernel<<<grid, kTilePixels, smem, stream>>>(p, *steps);
+  else if (mode == kSlabStore)
     accumulate_simt_step_kernel<<<grid, kTilePixels, smem, stream>>>(p, *steps);
   else
     accumulate_simt_kernel<<<grid, kTilePixels, smem, stream>>>(p);

@@ -92,7 +92,7 @@ namespace {
 struct PlannedLaunch {
   bool is_mma = false;
   LaunchParams simt;                     // SIMT: the parameter block itself
-  bool has_steps = false;                // SIMT: the step-slab kernel, with these slabs
+  SlabMode mode = kSlabNone;             // SIMT: the step- or range-slab kernel, with these slabs
   StepSlabs steps;
   int grid = 0;
   size_t smem = 0;
@@ -104,10 +104,10 @@ struct PlannedLaunch {
 // layer calls (same pointers: the caching allocator hands the projections the same addresses) every denoising step,
 // so plans are cached by the verbatim daam_layer[] input; a hit costs one memcmp instead of ~3 hash lookups per layer.
 struct Plan {
-  std::vector<uint8_t> key;              // the caller's daam_layer[n] bytes (+ its step_acc[n] pointers)
+  std::vector<uint8_t> key;              // the caller's daam_layer[n] bytes (+ its step_acc[n] / range_acc[n] pointers)
   uint32_t flags = 0;
   int device = -1;
-  bool with_steps = false;               // daam_accumulate_steps
+  SlabMode mode = kSlabNone;             // daam_accumulate_steps stores into the slabs, daam_accumulate_range adds
   std::vector<PlannedLaunch> launches;
   uint64_t stamp = 0;
 };
@@ -126,26 +126,29 @@ bool acc_overlap(const LayerParams& a, const LayerParams& b) {
   return spans_overlap(a.acc, slab_bytes(a), b.acc, slab_bytes(b));
 }
 
-// daam_accumulate_steps: every step slab is non-null, 16-byte aligned, and shares no byte with an accumulator or with
-// another step slab of the call (the kernels store it without reading it, in any order).
-int validate_steps(const daam_layer* layers, float* const* steps, int n_layers) {
-  if (!steps) { set_error("daam_accumulate_steps: step_acc is a null array"); return DAAM_E_INVALID; }
+// daam_accumulate_steps / daam_accumulate_range: every second slab is non-null, 16-byte aligned, and shares no byte
+// with an accumulator or with another second slab of the call (the kernels store or add it tile by tile, in any order,
+// next to the accumulator update).
+int validate_steps(const daam_layer* layers, float* const* steps, int n_layers, SlabMode mode) {
+  const char* fn = mode == kSlabAdd ? "daam_accumulate_range" : "daam_accumulate_steps";
+  const char* what = mode == kSlabAdd ? "range" : "step";
+  if (!steps) { set_error("%s: %s_acc is a null array", fn, what); return DAAM_E_INVALID; }
   std::vector<LayerParams> all((size_t)n_layers);
   for (int i = 0; i < n_layers; ++i)
     if (int rc = make_layer_params(layers[i], i, &all[i], /*need_acc=*/true)) return rc;
   for (int i = 0; i < n_layers; ++i) {
-    if (!steps[i]) { set_error("daam_accumulate_steps: layer %d has a null step slab", i); return DAAM_E_INVALID; }
-    if (reinterpret_cast<uintptr_t>(steps[i]) % 16 != 0) { set_error("daam_accumulate_steps: layer %d: the step slab is not 16-byte aligned", i); return DAAM_E_INVALID; }
+    if (!steps[i]) { set_error("%s: layer %d has a null %s slab", fn, i, what); return DAAM_E_INVALID; }
+    if (reinterpret_cast<uintptr_t>(steps[i]) % 16 != 0) { set_error("%s: layer %d: the %s slab is not 16-byte aligned", fn, i, what); return DAAM_E_INVALID; }
   }
   for (int i = 0; i < n_layers; ++i) {
     const size_t n = slab_bytes(all[i]);
     for (int j = 0; j < n_layers; ++j) {
       if (spans_overlap(steps[i], n, all[j].acc, slab_bytes(all[j]))) {
-        set_error("daam_accumulate_steps: the step slab of layer %d overlaps the accumulator of layer %d", i, j);
+        set_error("%s: the %s slab of layer %d overlaps the accumulator of layer %d", fn, what, i, j);
         return DAAM_E_INVALID;
       }
       if (j != i && spans_overlap(steps[i], n, steps[j], slab_bytes(all[j]))) {
-        set_error("daam_accumulate_steps: the step slabs of layers %d and %d overlap", i, j);
+        set_error("%s: the %s slabs of layers %d and %d overlap", fn, what, i, j);
         return DAAM_E_INVALID;
       }
     }
@@ -153,13 +156,13 @@ int validate_steps(const daam_layer* layers, float* const* steps, int n_layers) 
   return DAAM_OK;
 }
 
-int build_plan(const daam_layer* layers, float* const* steps, int n_layers, uint32_t flags, const DeviceInfo& dev,
-               Plan* plan) {
+int build_plan(const daam_layer* layers, float* const* steps, SlabMode mode, int n_layers, uint32_t flags,
+               const DeviceInfo& dev, Plan* plan) {
   const uint32_t path = flags & 3u, rmw = flags & DAAM_ACC_RMW_MASK;
   // Three packs: 16-bit layers for the wgmma kernel (TMA form), fp32 layers for its split form, and the rest for
   // the SIMT kernel. Each is closed when its parameter block is full.
   LaunchParams packs[3];                 // 0: wgmma 16-bit, 1: wgmma fp32, 2: SIMT
-  StepSlabs pack_steps[3];               // daam_accumulate_steps: the step slab of every layer of a pack
+  StepSlabs pack_steps[3];               // steps / range: the second slab of every layer of a pack
   for (LaunchParams& p : packs) {
     p.n_layers = p.total_tiles = 0;
     p.rmw_mode = (rmw == DAAM_ACC_RMW_LDST) ? 0 : 1;     // default: reduce-add
@@ -180,12 +183,12 @@ int build_plan(const daam_layer* layers, float* const* steps, int n_layers, uint
     int rc;
     if (l.is_mma) {
       l.mma.reset(prepared_mma_new());
-      rc = prepare_accumulate_mma(p, st, dev, l.mma.get());
+      rc = prepare_accumulate_mma(p, st, mode, dev, l.mma.get());
     } else {
       l.simt = p;
-      l.has_steps = st != nullptr;
+      l.mode = mode;
       if (st) l.steps = *st;
-      rc = prepare_accumulate_simt(p, st, dev, &l.grid, &l.smem);
+      rc = prepare_accumulate_simt(p, mode, dev, &l.grid, &l.smem);
     }
     p.n_layers = 0;
     p.total_tiles = 0;
@@ -238,21 +241,23 @@ int build_plan(const daam_layer* layers, float* const* steps, int n_layers, uint
 namespace daam {
 namespace {
 
-// daam_accumulate (steps == nullptr) and daam_accumulate_steps.
-int accumulate_impl(const daam_layer* layers, float* const* steps, int32_t n_layers, uint32_t flags, void* stream_) {
+// daam_accumulate (steps == nullptr, kSlabNone), daam_accumulate_steps (kSlabStore) and daam_accumulate_range
+// (kSlabAdd).
+int accumulate_impl(const daam_layer* layers, float* const* steps, SlabMode mode, int32_t n_layers, uint32_t flags,
+                    void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DeviceInfo dev;
   if (int rc = get_device_info(&dev)) return rc;
 
   static thread_local std::vector<std::unique_ptr<Plan>> plans;    // per calling thread: no locking on the hot path
   static thread_local uint64_t clock = 0;
-  const bool with_steps = steps != nullptr;
+  const bool with_steps = mode != kSlabNone;
   const size_t layer_bytes = sizeof(daam_layer) * (size_t)n_layers;
   const size_t step_bytes = with_steps ? sizeof(float*) * (size_t)n_layers : 0;
   const size_t bytes = layer_bytes + step_bytes;
   Plan* plan = nullptr;
   for (auto& c : plans)
-    if (c->key.size() == bytes && c->flags == flags && c->device == dev.device && c->with_steps == with_steps &&
+    if (c->key.size() == bytes && c->flags == flags && c->device == dev.device && c->mode == mode &&
         memcmp(c->key.data(), layers, layer_bytes) == 0 &&
         (!with_steps || memcmp(c->key.data() + layer_bytes, steps, step_bytes) == 0)) {
       plan = c.get();
@@ -260,7 +265,7 @@ int accumulate_impl(const daam_layer* layers, float* const* steps, int32_t n_lay
     }
   if (!plan) {
     if (with_steps)
-      if (int rc = validate_steps(layers, steps, n_layers)) return rc;
+      if (int rc = validate_steps(layers, steps, n_layers, mode)) return rc;
     std::unique_ptr<Plan> fresh(new Plan);
     fresh->key.assign(reinterpret_cast<const uint8_t*>(layers), reinterpret_cast<const uint8_t*>(layers) + layer_bytes);
     if (with_steps)
@@ -268,8 +273,8 @@ int accumulate_impl(const daam_layer* layers, float* const* steps, int32_t n_lay
                         reinterpret_cast<const uint8_t*>(steps) + step_bytes);
     fresh->flags = flags;
     fresh->device = dev.device;
-    fresh->with_steps = with_steps;
-    if (int rc = build_plan(layers, steps, n_layers, flags, dev, fresh.get())) return rc;     // failed plans are not cached
+    fresh->mode = mode;
+    if (int rc = build_plan(layers, steps, mode, n_layers, flags, dev, fresh.get())) return rc;     // failed plans are not cached
     if (plans.size() >= kMaxPlans) {                                                   // evict the least recently used
       size_t oldest = 0;
       for (size_t i = 1; i < plans.size(); ++i)
@@ -284,7 +289,8 @@ int accumulate_impl(const daam_layer* layers, float* const* steps, int32_t n_lay
   plan->stamp = ++clock;
   for (const PlannedLaunch& l : plan->launches) {
     const int rc = l.is_mma ? launch_prepared_mma(l.mma.get(), stream)
-                            : launch_prepared_simt(l.simt, l.has_steps ? &l.steps : nullptr, l.grid, l.smem, stream);
+                            : launch_prepared_simt(l.simt, l.mode != kSlabNone ? &l.steps : nullptr, l.mode, l.grid,
+                                                   l.smem, stream);
     if (rc) return rc;
   }
   return DAAM_OK;
@@ -296,7 +302,7 @@ int accumulate_impl(const daam_layer* layers, float* const* steps, int32_t n_lay
 extern "C" int daam_accumulate(const daam_layer* layers, int32_t n_layers, uint32_t flags, void* stream) {
   if (n_layers < 0 || (n_layers > 0 && !layers)) { set_error("daam_accumulate: bad layer array"); return DAAM_E_INVALID; }
   if (n_layers == 0) return DAAM_OK;
-  return accumulate_impl(layers, nullptr, n_layers, flags, stream);
+  return accumulate_impl(layers, nullptr, kSlabNone, n_layers, flags, stream);
 }
 
 extern "C" int daam_accumulate_steps(const daam_layer* layers, float* const* step_acc, int32_t n_layers, uint32_t flags,
@@ -304,7 +310,15 @@ extern "C" int daam_accumulate_steps(const daam_layer* layers, float* const* ste
   if (n_layers < 0 || (n_layers > 0 && !layers)) { set_error("daam_accumulate_steps: bad layer array"); return DAAM_E_INVALID; }
   if (n_layers > 0 && !step_acc) { set_error("daam_accumulate_steps: step_acc is a null array"); return DAAM_E_INVALID; }
   if (n_layers == 0) return DAAM_OK;
-  return accumulate_impl(layers, step_acc, n_layers, flags, stream);
+  return accumulate_impl(layers, step_acc, kSlabStore, n_layers, flags, stream);
+}
+
+extern "C" int daam_accumulate_range(const daam_layer* layers, float* const* range_acc, int32_t n_layers, uint32_t flags,
+                                     void* stream) {
+  if (n_layers < 0 || (n_layers > 0 && !layers)) { set_error("daam_accumulate_range: bad layer array"); return DAAM_E_INVALID; }
+  if (n_layers > 0 && !range_acc) { set_error("daam_accumulate_range: range_acc is a null array"); return DAAM_E_INVALID; }
+  if (n_layers == 0) return DAAM_OK;
+  return accumulate_impl(layers, range_acc, kSlabAdd, n_layers, flags, stream);
 }
 
 // ---- side-stream launcher ------------------------------------------------------------------------------------------

@@ -51,13 +51,16 @@ class LayerSlab:
     head_offset: int = 0         # first real head behind key head 0 (non-zero only for the un-guided B=1 quirk)
     captured: bool = False       # the layer's kernel launch is part of a CUDA graph: replays update it without the hook
     step: Optional[torch.Tensor] = None   # time-resolved traces only: what the last step added, shaped like ``acc``
+    # step-range traces only: ``ranges[i]`` is shaped like ``acc`` and holds the sum over the steps of declared range i
+    ranges: Optional[List[torch.Tensor]] = None
 
     @property
     def n_prompts(self) -> int:
         return self.acc.shape[0]
 
-    def key_view(self, head: int, prompt: int = 0) -> torch.Tensor:
-        return self.acc[prompt, head].view(self.acc.shape[2], self.h, self.w)
+    def key_view(self, head: int, prompt: int = 0, step_range: Optional[int] = None) -> torch.Tensor:
+        src = self.acc if step_range is None else self.ranges[step_range]
+        return src[prompt, head].view(src.shape[2], self.h, self.w)
 
 
 class RawHeatMapCollection:
@@ -70,6 +73,8 @@ class RawHeatMapCollection:
         self._sync = None                     # callable making pending kernel work visible to the current stream
         self._zero = None                     # callable(slabs) zeroing slabs in accumulate-stream order
         self.time_resolved = False            # allocate a step slab next to every accumulator (trace(time_resolved=True))
+        self.n_ranges = 0                     # range slabs next to every accumulator (trace(step_ranges=[...]))
+        self.range_steps: List[int] = []      # UNet forwards each range has received since the last clear()
 
     # -- wiring from the tracer -------------------------------------------------------------------------------------
     def bind(self, sync, zero):
@@ -85,14 +90,17 @@ class RawHeatMapCollection:
         slab = self.slabs.get(layer_idx)
         shape = (n_prompts, heads, _native.TOKENS, h * w)
         if slab is None or tuple(slab.acc.shape) != shape or slab.acc.device != torch.device(device) \
-                or slab.factor != factor or (self.time_resolved and slab.step is None):
+                or slab.factor != factor or (self.time_resolved and slab.step is None) \
+                or (self.n_ranges and slab.ranges is None):
             if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
                 raise RuntimeError('accumulator slabs cannot be created inside a CUDA-graph capture: run one eager '
                                    'UNet step under trace() before capturing')
             acc = torch.zeros(shape, dtype=torch.float32, device=device)
             # the kernel writes every element of a step slab each step: no zeroing needed
             step = torch.empty(shape, dtype=torch.float32, device=device) if self.time_resolved else None
-            slab = LayerSlab(layer_idx, factor, heads, h, w, acc, head_offset=head_offset, step=step)
+            ranges = [torch.zeros(shape, dtype=torch.float32, device=device) for _ in range(self.n_ranges)] \
+                if self.n_ranges else None
+            slab = LayerSlab(layer_idx, factor, heads, h, w, acc, head_offset=head_offset, step=step, ranges=ranges)
             self.slabs[layer_idx] = slab
             self.epoch += 1
         if not slab.touched:
@@ -139,11 +147,27 @@ class RawHeatMapCollection:
     def heads(self) -> Set[int]:
         return {h for s in self.live_slabs() for h in range(s.heads)}
 
-    def items(self, prompt: int = 0) -> Iterator[Tuple[RawHeatMapKey, torch.Tensor]]:
+    def items(self, prompt: int = 0, *, step_range: Optional[int] = None) -> Iterator[Tuple[RawHeatMapKey, torch.Tensor]]:
+        """``((factor, layer, head), [77, h, w])`` for every key; with ``step_range=i`` the per-key sums over the steps
+        of declared range ``i`` (``trace(pipe, step_ranges=[...])``) instead of over every step."""
+        if step_range is not None:
+            self.check_step_range(step_range)
         self._synchronize()
+        if step_range is not None and self.range_steps[step_range] == 0:
+            raise RuntimeError('No heat maps found for the given parameters.')
         for slab in self.live_slabs():
+            if step_range is not None and slab.ranges is None:
+                continue
             for head in range(slab.heads):
-                yield (slab.factor, slab.layer_idx, head), slab.key_view(head, prompt)
+                yield (slab.factor, slab.layer_idx, head), slab.key_view(head, prompt, step_range)
+
+    def check_step_range(self, step_range: int):
+        """Raises unless ``step_range`` indexes a range declared with ``trace(pipe, step_ranges=[...])``."""
+        if not self.n_ranges:
+            raise RuntimeError('step_range needs a trace declared with step_ranges, e.g. trace(pipe, '
+                               'step_ranges=[(0, 10)])')
+        if not isinstance(step_range, int) or not 0 <= step_range < self.n_ranges:
+            raise IndexError(f'step_range {step_range!r} is not one of the {self.n_ranges} declared step ranges')
 
     def __iter__(self):
         return self.items(0)
@@ -159,6 +183,9 @@ class RawHeatMapCollection:
         else:
             for slab in live:
                 slab.acc.zero_()
+                for r in slab.ranges or ():
+                    r.zero_()
+        self.range_steps = [0] * self.n_ranges
         for slab in live:                     # graph-captured layers stay live: replays bypass the Python hook
             slab.touched = slab.captured
         self._order = [i for i in self._order if self.slabs[i].captured]

@@ -12,7 +12,7 @@ import torch
 from . import _native
 
 __all__ = ['cond_half', 'make_layer_desc', 'new_accumulator', 'pack', 'accumulate', 'accumulate_steps',
-           'accumulate_layer', 'attention_probs', 'accumulate_probs']
+           'accumulate_range', 'accumulate_layer', 'attention_probs', 'accumulate_probs']
 
 _DTYPES = {torch.float32: _native.DAAM_F32, torch.float16: _native.DAAM_F16, torch.bfloat16: _native.DAAM_BF16}
 
@@ -98,6 +98,25 @@ def accumulate_steps(descs, steps, device, stream: Optional[torch.cuda.Stream] =
     else:
         with torch.cuda.device(index):
             _native.accumulate_steps(descs, steps, s.cuda_stream, flags)
+
+
+def accumulate_range(descs, ranges, device, stream: Optional[torch.cuda.Stream] = None, flags: int = _native.ACC_AUTO):
+    """:func:`accumulate`, and also add what each layer adds into its range slab, with the accumulator's arithmetic
+    (``daam_accumulate_range``). ``ranges``: one contiguous fp32 tensor per descriptor, shaped like its accumulator, or
+    a prepared :class:`_native.StepPointers`."""
+    dev = device if isinstance(device, torch.device) else torch.device(device)
+    index = dev.index if dev.index is not None else torch.cuda.current_device()
+    s = torch.cuda.current_stream(index) if stream is None else stream
+    if not isinstance(ranges, _native.StepPointers):
+        for t in ranges:
+            if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
+                raise RuntimeError('range slabs must be contiguous fp32 CUDA tensors')
+        ranges = _native.StepPointers([t.data_ptr() for t in ranges])
+    if index == torch.cuda.current_device():
+        _native.accumulate_range(descs, ranges, s.cuda_stream, flags)
+    else:
+        with torch.cuda.device(index):
+            _native.accumulate_range(descs, ranges, s.cuda_stream, flags)
 
 
 def accumulate_layer(q: torch.Tensor, k: torch.Tensor, heads: int, scale: Optional[float] = None,

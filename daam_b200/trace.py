@@ -17,6 +17,11 @@ exceptions; what differs is what runs underneath.
   ``daam_accumulate_steps`` (the kernel also stores what it adds into a second slab per layer) followed by one
   ``daam_finalize`` per prompt over those step slabs, into that step's slot of a device history
   (``compute_time_heat_maps``).
+* ``step_ranges=[(a, b), ...]`` answers what DAAM attributes during chosen spans of steps: every traced layer gets one
+  more zeroed slab per declared range, and while the UNet forward index lies in range ``i`` the step launch becomes
+  ``daam_accumulate_range``, which also adds what it adds into range ``i``'s slabs. Each range slab then is the
+  accumulator a trace of only those steps would hold, so every read (``step_range=i``) reduces it exactly as the full
+  run's accumulator is reduced.
 
 Accumulators are fp32 regardless of the pipeline dtype (the reference accumulates in the pipeline dtype, SURVEY.md
 section 5); parity is stated against the fp32 oracle fed the same Q/K.
@@ -25,7 +30,7 @@ from __future__ import annotations
 
 import math
 from pathlib import Path
-from typing import Dict, List, Optional, Type, Union
+from typing import Dict, List, Optional, Tuple, Type, Union
 
 import numpy as np
 import torch
@@ -45,15 +50,29 @@ class DiffusionHeatMapHooker(AggregateHooker):
     Extra keyword-only options (not in the reference): ``launch`` ('step' | 'overlap' | 'layer', see module docstring),
     ``batch_prompts`` (accept several prompts per generation: N independent single-prompt traces sharing each launch;
     the reference rejects this, trace.py:172-173), ``locate_middle_block`` (also locate the mid block without
-    enabling save/load of heads -- BASELINE config 5 "all 16+70 layers") and ``time_resolved`` (also keep one global
-    heat map per denoising step, see :meth:`compute_time_heat_maps`).
+    enabling save/load of heads -- BASELINE config 5 "all 16+70 layers"), ``time_resolved`` (also keep one global
+    heat map per denoising step, see :meth:`compute_time_heat_maps`) and ``step_ranges`` (a list of half-open
+    ``(start, stop)`` tuples or ``range`` objects over UNet-forward indices of a generation, counted as
+    :class:`TimeHeatMaps` counts them: also keep the per-key sums over each of those spans; read them with
+    ``step_range=i`` in :meth:`compute_global_heat_map`, :meth:`compute_per_head_heat_maps` and
+    ``all_heat_maps.items``).
     """
 
     def __init__(self, pipeline, low_memory: bool = False, load_heads: bool = False, save_heads: bool = False,
                  data_dir: str = None, *, launch: str = 'step', batch_prompts: bool = False,
-                 locate_middle_block: bool = False, kernel_flags: int = _native.ACC_AUTO, time_resolved: bool = False):
+                 locate_middle_block: bool = False, kernel_flags: int = _native.ACC_AUTO, time_resolved: bool = False,
+                 step_ranges=None):
         if launch not in ('step', 'overlap', 'layer'):
             raise ValueError("launch must be 'step', 'overlap' or 'layer'")
+        if step_ranges is not None:
+            step_ranges = _normalize_step_ranges(step_ranges)
+            if launch != 'step':
+                raise ValueError("step_ranges needs launch='step': which range a launch adds into depends on the UNet "
+                                 "forward it ends, on the forward's own stream")
+            if save_heads or load_heads:
+                raise ValueError('step_ranges does not support save_heads / load_heads')
+            if time_resolved:
+                raise ValueError('step_ranges cannot be combined with time_resolved=True')
         if time_resolved and launch != 'step':
             raise ValueError("time_resolved=True needs launch='step': the per-step heat map is finalized right after "
                              "the step's launch, on the forward's own stream")
@@ -97,6 +116,12 @@ class DiffusionHeatMapHooker(AggregateHooker):
         self._history: List[torch.Tensor] = []
         self._time_steps = 0
         self._history_rows: Optional[List[int]] = None   # n_rows of every prompt of the running generation
+        # step-range mode: per declared range, the range slab of every slot of the step array; the UNet forward index
+        self.step_ranges: Optional[List[Tuple[int, int]]] = step_ranges
+        self.all_heat_maps.n_ranges = len(step_ranges) if step_ranges else 0
+        self.all_heat_maps.range_steps = [0] * self.all_heat_maps.n_ranges
+        self._range_ptrs = [_native.StepPointers([0] * 64) for _ in step_ranges] if step_ranges else None
+        self._forward_idx = 0
 
         modules = [
             UNetCrossAttentionHooker(m, self, layer_idx=idx, latent_hw=self.latent_hw, load_heads=load_heads,
@@ -220,9 +245,15 @@ class DiffusionHeatMapHooker(AggregateHooker):
                 if self._step_ptrs is not None:
                     old = list(self._step_ptrs.array)
                     self._step_ptrs = _native.StepPointers(old + [0] * (len(grown.array) - len(old)))
+                if self._range_ptrs is not None:
+                    self._range_ptrs = [_native.StepPointers(list(r.array) + [0] * (len(grown.array) - len(r.array)))
+                                        for r in self._range_ptrs]
             self._packed.array[pos] = desc
             if self._step_ptrs is not None:
                 self._step_ptrs.array[pos] = slab.step.data_ptr()
+            if self._range_ptrs is not None:
+                for ptrs, r in zip(self._range_ptrs, slab.ranges):
+                    ptrs.array[pos] = r.data_ptr()
             slot, own = self._slots[pos], None
         else:
             own = _native.PackedLayers([desc])             # 'layer' mode: every layer launches its own 1-element array
@@ -282,6 +313,10 @@ class DiffusionHeatMapHooker(AggregateHooker):
                     self._refs, self._n_pending = [], 0
                     raise RuntimeError('time_resolved=True cannot be captured into a CUDA graph: every step writes its '
                                        'heat map into another history slot, which a graph replay cannot follow')
+                if self.step_ranges is not None:
+                    self._refs, self._n_pending = [], 0
+                    raise RuntimeError('step_ranges cannot be captured into a CUDA graph: which range slabs a step adds '
+                                       'into depends on the step index, which a graph replay cannot follow')
                 # CUDA-graph capture of the UNet step: the launch becomes a node of the captured stream; replays bypass the
                 # Python hook, so the layers of this launch stay live across per-generation resets
                 step = self._step_id
@@ -293,6 +328,15 @@ class DiffusionHeatMapHooker(AggregateHooker):
                 # the step's global heat maps, in stream order behind it
                 _native.accumulate_steps(packed, self._step_ptrs, current, flags)
                 self._finalize_step(device, current)
+            elif self.step_ranges is not None:
+                # launch == 'step' (checked at construction), on the forward's own stream as below
+                r = self._range_of(self._forward_idx)
+                if r is None:
+                    _native.accumulate(packed, current, flags)
+                else:
+                    _native.accumulate_range(packed, self._range_ptrs[r], current, flags)
+                    self.all_heat_maps.range_steps[r] += 1
+                self._forward_idx += 1
             elif capturing or self.launch == 'step':
                 # On the forward's own stream: the predecessor there is the tail of the UNet forward, never a producer of
                 # the queued Q/K, so only the accumulator updates have to wait for it (EARLY_LOADS). Stream order also
@@ -346,10 +390,24 @@ class DiffusionHeatMapHooker(AggregateHooker):
         self._time_steps = t + 1
 
     def _restart_history(self):
-        """A new generation: a new per-step history (maps handed out earlier stay valid: they are other tensors)."""
+        """A new generation: a new per-step history (maps handed out earlier stay valid: they are other tensors), and
+        the UNet forward count of the step ranges starts again (their slabs were zeroed with the accumulators)."""
         self._history = []
         self._time_steps = 0
         self._history_rows = None
+        self._forward_idx = 0
+
+    def _range_of(self, forward_idx: int) -> Optional[int]:
+        for i, (start, stop) in enumerate(self.step_ranges):
+            if start <= forward_idx < stop:
+                return i
+        return None
+
+    @property
+    def step_range_counts(self) -> List[int]:
+        """How many UNet forwards of the running / last generation each declared step range has received."""
+        self.synchronize()
+        return list(self.all_heat_maps.range_steps)
 
     def synchronize(self):
         """Make every accumulate issued so far visible to work enqueued on the current stream afterwards."""
@@ -367,30 +425,34 @@ class DiffusionHeatMapHooker(AggregateHooker):
         self.synchronize()
         for slab in slabs:
             slab.acc.zero_()
+            for r in slab.ranges or ():
+                r.zero_()
         if self._stream is not None:   # later side-stream launches must see the zeroed slabs
             self._stream.wait_stream(torch.cuda.current_stream(slabs[0].acc.device))
 
     # -- finalize -------------------------------------------------------------------------------------------------------
     def compute_global_heat_map(self, prompt=None, factors=None, head_idx=None, layer_idx=None, normalize=False,
-                                prompt_idx: int = 0) -> GlobalHeatMap:
+                                prompt_idx: int = 0, *, step_range: Optional[int] = None) -> GlobalHeatMap:
         """Aggregate across time (already summed in the slabs) and across layers/heads (trace.py:83-132).
 
         Args mirror the reference: ``factors`` restricts the spatial factors, ``head_idx`` / ``layer_idx`` restrict to one
         head / layer, ``normalize`` divides by the per-pixel sum over the real tokens. ``prompt_idx`` selects the prompt in
-        ``batch_prompts`` mode.
+        ``batch_prompts`` mode. ``step_range=i`` aggregates over the steps of declared range ``i`` only
+        (``trace(pipe, step_ranges=[...])``): the DAAM map a trace of only those steps would give.
         """
         if prompt is None:
             prompt = self.last_prompts[prompt_idx] if self.last_prompts else self.last_prompt
         factors = {0, 1, 2, 4, 8, 16, 32, 64} if factors is None else set(factors)
         x = int(np.sqrt(self.latent_hw))
+        self._check_step_range(step_range)
         self.synchronize()
         groups, keep = [], []
-        for slab in self.all_heat_maps.live_slabs():
+        for slab in self._slabs_for(step_range):
             if slab.factor not in factors or (layer_idx is not None and layer_idx != slab.layer_idx):
                 continue
             if head_idx is not None and not 0 <= head_idx < slab.heads:
                 continue
-            acc = slab.acc[prompt_idx]
+            acc = (slab.acc if step_range is None else slab.ranges[step_range])[prompt_idx]
             groups.append(_native.DaamKeyGroup(acc=acc.data_ptr(), heads=slab.heads, h=slab.h, w=slab.w,
                                                tokens=acc.shape[1], head_sel=-1 if head_idx is None else head_idx,
                                                reserved=0))
@@ -430,20 +492,23 @@ class DiffusionHeatMapHooker(AggregateHooker):
         return TimeHeatMaps(self.pipe.tokenizer, prompt, maps)
 
 
-    def compute_per_head_heat_maps(self, prompt=None, factors=None, normalize=False, prompt_idx: int = 0):
+    def compute_per_head_heat_maps(self, prompt=None, factors=None, normalize=False, prompt_idx: int = 0, *,
+                                   step_range: Optional[int] = None):
         """Every ``compute_global_heat_map(layer_idx=l, head_idx=h)`` of the reference's ``--all-heads`` sweep
         (daam/run/generate.py:239-255) in one launch. Returns ``(keys, maps)``: ``keys[i] = (factor, layer, head)`` and
-        ``maps[i]`` the ``[n_tokens + 2, x, x]`` heat map the reference computes for that single key."""
+        ``maps[i]`` the ``[n_tokens + 2, x, x]`` heat map the reference computes for that single key. ``step_range=i``:
+        over the steps of declared range ``i`` only, as in :meth:`compute_global_heat_map`."""
         if prompt is None:
             prompt = self.last_prompts[prompt_idx] if self.last_prompts else self.last_prompt
         factors = {0, 1, 2, 4, 8, 16, 32, 64} if factors is None else set(factors)
         x = int(np.sqrt(self.latent_hw))
+        self._check_step_range(step_range)
         self.synchronize()
         groups, keep, keys = [], [], []
-        for slab in self.all_heat_maps.live_slabs():
+        for slab in self._slabs_for(step_range):
             if slab.factor not in factors:
                 continue
-            acc = slab.acc[prompt_idx]
+            acc = (slab.acc if step_range is None else slab.ranges[step_range])[prompt_idx]
             groups.append(_native.DaamKeyGroup(acc=acc.data_ptr(), heads=slab.heads, h=slab.h, w=slab.w,
                                                tokens=acc.shape[1], head_sel=-1, reserved=0))
             keep.append(acc)
@@ -457,6 +522,48 @@ class DiffusionHeatMapHooker(AggregateHooker):
             _native.finalize_per_key(groups, x, n_rows, normalize, maps.data_ptr(),
                                      torch.cuda.current_stream(device).cuda_stream)
         return keys, maps
+
+    def _check_step_range(self, step_range: Optional[int]):
+        if step_range is not None:
+            self.all_heat_maps.check_step_range(step_range)
+
+    def _slabs_for(self, step_range: Optional[int]) -> List[LayerSlab]:
+        """The live slabs a read reduces; with ``step_range``, those with range slabs, after checking (synchronized)
+        that the range has received a step."""
+        slabs = self.all_heat_maps.live_slabs()
+        if step_range is None:
+            return slabs
+        if self.all_heat_maps.range_steps[step_range] == 0:
+            raise RuntimeError('No heat maps found for the given parameters.')
+        return [s for s in slabs if s.ranges is not None]
+
+
+def _normalize_step_ranges(step_ranges) -> List[Tuple[int, int]]:
+    """``trace(step_ranges=...)``: a non-empty list of half-open ``(start, stop)`` tuples or step-1 ``range`` objects
+    over UNet-forward indices, none empty or negative, no two overlapping. Returns ``[(start, stop), ...]`` in the
+    given order (the order ``step_range=i`` indexes)."""
+    if isinstance(step_ranges, (range, tuple)) or not hasattr(step_ranges, '__iter__'):
+        raise ValueError(f'step_ranges is a list of (start, stop) tuples or ranges, got {step_ranges!r}')
+    out = []
+    for r in step_ranges:
+        if isinstance(r, range):
+            if r.step != 1:
+                raise ValueError(f'step range {r!r} must have step 1')
+            start, stop = r.start, r.stop
+        elif isinstance(r, tuple) and len(r) == 2 and all(isinstance(v, int) and not isinstance(v, bool) for v in r):
+            start, stop = r
+        else:
+            raise ValueError(f'a step range is a (start, stop) tuple of ints or a range, got {r!r}')
+        if start < 0 or stop <= start:
+            raise ValueError(f'step range [{start}, {stop}) must have 0 <= start < stop')
+        out.append((start, stop))
+    if not out:
+        raise ValueError('step_ranges must declare at least one range')
+    spans = sorted(out)
+    for (a0, a1), (b0, b1) in zip(spans, spans[1:]):
+        if b0 < a1:
+            raise ValueError(f'step ranges [{a0}, {a1}) and [{b0}, {b1}) overlap')
+    return out
 
 
 class ImageProcessorHooker(ObjectHooker):

@@ -26,7 +26,8 @@ extern "C" {
 
 #define DAAM_ABI_VERSION 3          /* 2: + daam_attention_probs, daam_accumulate_probs, daam_finalize_per_key
                                        3: + DAAM_ACC_EARLY_LOADS, daam_expand_words, daam_side_launcher_*
-                                          (later, additive: daam_accumulate_steps, daam_normalize_maps) */
+                                          (later, additive: daam_accumulate_steps, daam_normalize_maps,
+                                          daam_accumulate_range) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
 
@@ -106,6 +107,18 @@ int daam_accumulate(const daam_layer* layers, int32_t n_layers, uint32_t flags, 
  * daam_accumulate; with DAAM_ACC_EARLY_LOADS the step-slab stores, too, wait for the previous kernel.
  */
 int daam_accumulate_steps(const daam_layer* layers, float* const* step_acc, int32_t n_layers, uint32_t flags,
+                          void* stream);
+
+/*
+ * Step-range heat maps (daam_b200/trace.py, trace(..., step_ranges=[...])): daam_accumulate, and also
+ *   range_acc[i][p][head][t][pixel] += the value added
+ * with the arithmetic daam_accumulate applies to acc in the same update mode (16-bit wgmma form: add.rn.ftz, as the
+ * accumulator tile; fp32 split form and SIMT: the reduce-add or load / add / store the flags select). So a range slab
+ * zeroed before a span of calls holds afterwards, bit for bit, what an accumulator that received only those calls
+ * would hold. Same validation, flags and packing as daam_accumulate_steps (range_acc: host array of n_layers device
+ * pointers, fp32, 16-byte aligned, shaped like layers[i].acc, overlapping no accumulator and no other range slab).
+ */
+int daam_accumulate_range(const daam_layer* layers, float* const* range_acc, int32_t n_layers, uint32_t flags,
                           void* stream);
 
 /*
