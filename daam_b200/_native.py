@@ -186,32 +186,30 @@ class StepPointers:
         self.array = (ctypes.c_void_p * max(len(ptrs), 1))(*ptrs)
 
 
-def accumulate_steps(layers, steps, stream: int, flags: int = ACC_AUTO):
-    """``daam_accumulate_steps``: ``layers`` as for :func:`accumulate`; ``steps`` a :class:`StepPointers` or a sequence of
-    device pointers, one step slab per layer (the first ``n`` are used)."""
+def _accumulate_second(entry: str, word: str, layers, slabs, stream: int, flags: int):
+    """``entry`` (``daam_accumulate_steps`` / ``daam_accumulate_range``) over ``layers`` and one second slab per layer;
+    ``word`` names the slabs in messages."""
     packed = layers if isinstance(layers, PackedLayers) else PackedLayers(layers)
     if packed.n == 0:
         return
-    arr = steps if isinstance(steps, StepPointers) else StepPointers(steps)
+    arr = slabs if isinstance(slabs, StepPointers) else StepPointers(slabs)
     if len(arr.array) < packed.n:
-        raise ValueError(f'{len(arr.array)} step slabs for {packed.n} layers')
-    rc = load().daam_accumulate_steps(packed.array, arr.array, packed.n, flags, stream)
+        raise ValueError(f'{len(arr.array)} {word} slabs for {packed.n} layers')
+    rc = getattr(load(), entry)(packed.array, arr.array, packed.n, flags, stream)
     if rc != 0:
         _check(rc)
+
+
+def accumulate_steps(layers, steps, stream: int, flags: int = ACC_AUTO):
+    """``daam_accumulate_steps``: ``layers`` as for :func:`accumulate`; ``steps`` a :class:`StepPointers` or a sequence of
+    device pointers, one step slab per layer (the first ``n`` are used)."""
+    _accumulate_second('daam_accumulate_steps', 'step', layers, steps, stream, flags)
 
 
 def accumulate_range(layers, ranges, stream: int, flags: int = ACC_AUTO):
     """``daam_accumulate_range``: ``layers`` as for :func:`accumulate`; ``ranges`` a :class:`StepPointers` or a sequence
     of device pointers, one range slab per layer (the first ``n`` are used)."""
-    packed = layers if isinstance(layers, PackedLayers) else PackedLayers(layers)
-    if packed.n == 0:
-        return
-    arr = ranges if isinstance(ranges, StepPointers) else StepPointers(ranges)
-    if len(arr.array) < packed.n:
-        raise ValueError(f'{len(arr.array)} range slabs for {packed.n} layers')
-    rc = load().daam_accumulate_range(packed.array, arr.array, packed.n, flags, stream)
-    if rc != 0:
-        _check(rc)
+    _accumulate_second('daam_accumulate_range', 'range', layers, ranges, stream, flags)
 
 
 def normalize_maps(maps_ptr: int, n_maps: int, n_rows: int, x: int, stream: int):

@@ -31,8 +31,9 @@
 // head_dim other than 64 (SD-1.x: 40 / 80 / 160): the contraction runs in 64-wide K chunks, one chunk per smem stage,
 // accumulated into the same registers; the last chunk is zero-filled beyond head_dim by the TMA unit.
 //
-// Step-slab instances (kStep, daam_accumulate_steps): every form also STORES what it adds into a second fp32 slab of the
-// accumulator's layout, flushed like the add, so that a caller gets one denoising step's maps next to the time sum.
+// Step-slab instances (kSlab == kSlabStore, daam_accumulate_steps): every form also STORES what it adds into a second
+// fp32 slab of the accumulator's layout, flushed like the add, so that a caller gets one denoising step's maps next to
+// the time sum.
 //   16-bit form: one more [77][128] shared block sS; the consumers write p there in the pass that adds into the ring
 //                slot, and the thread that stores the accumulator tile issues a second bulk-tensor store from sS in the
 //                same bulk group. Before sS is rewritten, that thread waits for the previous group's reads.
@@ -71,14 +72,14 @@ constexpr int kThreads16 = kConsumers + 64;           // 16-bit form: + the Q/K 
 constexpr int kBarBytes = 64;                         // split form: mbarriers
 constexpr int kBarBytes16 = 8 * 2 * (kStages + kAccStages);
 constexpr int kSmemBytes = 1024 + kStages * kStageBytes + kAccStages * kPBytes + kBarBytes16;
-constexpr int kStepSmemBytes = kSmemBytes + kPBytes;  // 16-bit form with a step slab: + the sS block (207.5 KB in all)
+constexpr int kSlabSmemBytes = kSmemBytes + kPBytes;  // 16-bit form with a second slab: + the sS block (207.5 KB)
 // split (fp32) form: a raw stage holds the fp32 tiles as [Q sub0][Q sub1][K sub0][K sub1] (sub-tile = 32 floats = one
 // 128-byte swizzle span per row); one more buffer of the same shape holds the lo terms
 constexpr int kSplitStageBytes = 2 * kStageBytes;     // 53248 = 52 x 1024
 constexpr int kSplitSmemBytes = 1024 + (kStages + 1) * kSplitStageBytes + kPBytes + kBarBytes;
 static_assert(kSmemBytes <= 232448, "16-bit form exceeds the 227 KB shared-memory limit");
 static_assert(kSplitSmemBytes <= 232448, "split form exceeds the 227 KB shared-memory limit");
-static_assert(kStepSmemBytes <= 232448, "16-bit step form exceeds the 227 KB shared-memory limit");
+static_assert(kSlabSmemBytes <= 232448, "16-bit second-slab form exceeds the 227 KB shared-memory limit");
 
 struct MmaParams {
   LaunchParams base;
@@ -86,14 +87,14 @@ struct MmaParams {
   CUtensorMap kmap[kMaxLayersPerLaunch];
   CUtensorMap amap[kMaxLayersPerLaunch];
 };
-// Parameter block of the step-slab instances (about 20 KB): the step slab of every layer as a tensor map shaped like
-// amap (bulk stores) and as a plain pointer (split form, ldst mode).
-struct MmaStepParams : MmaParams {
+// Parameter block of the second-slab instances (about 20 KB): the second slab of every layer as a tensor map shaped
+// like amap (bulk stores and reduces) and as a plain pointer (split form, ldst mode).
+struct MmaSlabParams : MmaParams {
   CUtensorMap smap[kMaxLayersPerLaunch];
-  float* step[kMaxLayersPerLaunch];
+  float* slab[kMaxLayersPerLaunch];
 };
-template <bool kStep>
-using MmaParamsT = std::conditional_t<kStep, MmaStepParams, MmaParams>;
+template <bool kSecond>
+using MmaParamsT = std::conditional_t<kSecond, MmaSlabParams, MmaParams>;
 
 // ---- PTX wrappers -------------------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -298,11 +299,11 @@ __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wa
 template <bool kSplit, bool kChunked, int kSlab>
 __global__ void __launch_bounds__(kSplit ? kThreads : kThreads16, 1)
 accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP) {
-  constexpr bool kStep = kSlab != kSlabNone;          // a second slab (the step-form code paths, store or add)
+  constexpr bool kSecond = kSlab != kSlabNone;        // a second slab (store or add)
   constexpr int kStageBytesT = kSplit ? kSplitStageBytes : kStageBytes;
   constexpr int kOperandBytes = (kSplit ? kStages + 1 : kStages) * kStageBytesT;     // stages (+ the lo buffer)
-  // staged probabilities (split) / the accumulator ring (16-bit), + sS (16-bit step form)
-  constexpr int kPTiles = kSplit ? 1 : kAccStages + (kStep ? 1 : 0);
+  // staged probabilities (split) / the accumulator ring (16-bit), + sS (16-bit form with a second slab)
+  constexpr int kPTiles = kSplit ? 1 : kAccStages + (kSecond ? 1 : 0);
   const LaunchParams& P = MP.base;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
@@ -310,7 +311,7 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP)
   uint8_t* gen = smem_raw + (base - raw);
   float* sP = reinterpret_cast<float*>(gen + kOperandBytes);
   const uint32_t sP_u32 = base + kOperandBytes;
-  float* sS = sP + kAccStages * (kTokens * kTilePixels);              // 16-bit step form: the tile's p, stored as is
+  float* sS = sP + kAccStages * (kTokens * kTilePixels);              // 16-bit second-slab form: the tile's p
   const uint32_t sS_u32 = sP_u32 + kAccStages * kPBytes;
   const uint32_t bars = sP_u32 + kPTiles * kPBytes;
   const uint32_t full0 = bars, empty0 = bars + 8 * kStages;           // Q/K ring
@@ -348,7 +349,7 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP)
     const Tile t0 = decode_tile(P, first, li0);
     if (warp != 8) {
       prefetch_tensormap(&MP.amap[t0.li]);
-      if constexpr (kStep) prefetch_tensormap(&MP.smap[t0.li]);
+      if constexpr (kSecond) prefetch_tensormap(&MP.smap[t0.li]);
     } else {
       prefetch_tensormap(&MP.qmap[t0.li]);
       prefetch_tensormap(&MP.kmap[t0.li]);
@@ -517,7 +518,7 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP)
             }
           }
         }
-        if constexpr (kStep) {                         // the previous tile's step store has finished reading sS
+        if constexpr (kSecond) {                       // the previous tile's second-slab store / reduce has read sS
           if (tid == 0 && i > 0) bulk_wait_read0();
           consumer_barrier();
         }
@@ -530,7 +531,7 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP)
               const float pa = d[4 * jj + e] * inv0, pb = d[4 * jj + 2 + e] * inv1;
               sA[col * kTilePixels + ra] = add_ftz(old[4 * jj + e], lowq ? pa : pb);
               sA[col * kTilePixels + rb] = add_ftz(old[4 * jj + 2 + e], lowq ? pb : pa);
-              if constexpr (kStep) {
+              if constexpr (kSecond) {
                 sS[col * kTilePixels + ra] = add_ftz(0.f, lowq ? pa : pb);
                 sS[col * kTilePixels + rb] = add_ftz(0.f, lowq ? pb : pa);
               }
@@ -572,7 +573,7 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP)
           const int col = 8 * jj + 2 * quad + e;
           if (col < kTokens) {
             float a = d[4 * jj + e] * inv0, b = d[4 * jj + 2 + e] * inv1;
-            if constexpr (kStep) {
+            if constexpr (kSecond) {
               if (stage_ftz) { a = add_ftz(0.f, a); b = add_ftz(0.f, b); }
             }
             sP[col * kTilePixels + (lowq ? r0 : r0 + 8)] = lowq ? a : b;
@@ -606,9 +607,9 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP)
             o.x += p.x; o.y += p.y; o.z += p.z; o.w += p.w;
             *g = o;
             if constexpr (kSlab == kSlabStore)
-              reinterpret_cast<float4*>(MP.step[t.li] + (acc - L.acc) + tok * hw)[c4] = p;
+              reinterpret_cast<float4*>(MP.slab[t.li] + (acc - L.acc) + tok * hw)[c4] = p;
             if constexpr (kSlab == kSlabAdd) {
-              float4* r = reinterpret_cast<float4*>(MP.step[t.li] + (acc - L.acc) + tok * hw) + c4;
+              float4* r = reinterpret_cast<float4*>(MP.slab[t.li] + (acc - L.acc) + tok * hw) + c4;
               float4 ro = *r;
               ro.x += p.x; ro.y += p.y; ro.z += p.z; ro.w += p.w;
               *r = ro;
@@ -720,15 +721,36 @@ int make_acc_map(float* acc, int hw, int rows, CUtensorMap* out) {
   return DAAM_OK;
 }
 
+// Every wgmma instance and its dynamic shared memory, indexed by PreparedMma::variant: bit 0 split (fp32), bit 1
+// chunked (head_dim > 64), bits 2-3 the SlabMode.
+struct MmaInstance {
+  const void* fn;
+  int smem;
+};
+const MmaInstance kMmaInstances[] = {
+    {(const void*)accumulate_mma_kernel<false, false, kSlabNone>, kSmemBytes},
+    {(const void*)accumulate_mma_kernel<true, false, kSlabNone>, kSplitSmemBytes},
+    {(const void*)accumulate_mma_kernel<false, true, kSlabNone>, kSmemBytes},
+    {(const void*)accumulate_mma_kernel<true, true, kSlabNone>, kSplitSmemBytes},
+    {(const void*)accumulate_mma_kernel<false, false, kSlabStore>, kSlabSmemBytes},
+    {(const void*)accumulate_mma_kernel<true, false, kSlabStore>, kSplitSmemBytes},
+    {(const void*)accumulate_mma_kernel<false, true, kSlabStore>, kSlabSmemBytes},
+    {(const void*)accumulate_mma_kernel<true, true, kSlabStore>, kSplitSmemBytes},
+    {(const void*)accumulate_mma_kernel<false, false, kSlabAdd>, kSlabSmemBytes},
+    {(const void*)accumulate_mma_kernel<true, false, kSlabAdd>, kSplitSmemBytes},
+    {(const void*)accumulate_mma_kernel<false, true, kSlabAdd>, kSlabSmemBytes},
+    {(const void*)accumulate_mma_kernel<true, true, kSlabAdd>, kSplitSmemBytes},
+};
+
 std::once_flag g_attr_once[64];                       // the shared-memory attribute is per device
 
 }  // namespace
 
 // Parameter block of one wgmma launch, opaque to api.cu (which caches prepared launches by their daam_layer[] input).
 struct PreparedMma {
-  MmaStepParams mp;                                   // the plain instances are launched with its MmaParams part
-  int grid, block, smem, variant;                     // variant: bit 0 split (fp32), bit 1 chunked (head_dim > 64),
-};                                                    // bits 2-3 the SlabMode (1 step slabs, 2 range slabs)
+  MmaSlabParams mp;                                   // the plain instances are launched with its MmaParams part
+  int grid, block, variant;                           // variant: index into kMmaInstances
+};
 void* prepared_mma_new() { return new PreparedMma; }                 // (aligned new: CUtensorMap is alignas(64))
 void prepared_mma_delete(void* p) { delete static_cast<PreparedMma*>(p); }
 
@@ -738,11 +760,11 @@ bool mma_supported(const LayerParams& L) {
 }
 
 // Tensor maps, grid and kernel variant of one pack of layers (all fp32, or all 16-bit). `out`: prepared_mma_new().
-int prepare_accumulate_mma(const LaunchParams& p, const StepSlabs* steps, SlabMode mode, const DeviceInfo& dev,
+int prepare_accumulate_mma(const LaunchParams& p, const SecondSlabs* slabs, SlabMode mode, const DeviceInfo& dev,
                            void* out) {
   if (dev.cc_major != 9) { set_error("the wgmma kernel needs an sm_90 device (found sm_%d%d)", dev.cc_major, dev.cc_minor); return DAAM_E_UNSUPPORTED; }
   PreparedMma& pm = *static_cast<PreparedMma*>(out);
-  MmaStepParams& mp = pm.mp;
+  MmaSlabParams& mp = pm.mp;
   mp.base = p;
   const bool split = p.n_layers > 0 && p.layer[0].dtype == DAAM_F32;     // a pack holds one operand class (api.cu)
   bool chunked = false;
@@ -752,57 +774,32 @@ int prepare_accumulate_mma(const LaunchParams& p, const StepSlabs* steps, SlabMo
     if (int rc = make_qk_map(L.q, L.dtype, L.head_dim, L.heads, L.hw, L.n_prompts, L.qs_head, L.qs_pixel, L.qs_prompt, kTilePixels, &mp.qmap[i])) return rc;
     if (int rc = make_qk_map(L.k, L.dtype, L.head_dim, L.heads, kTokens, L.n_prompts, L.ks_head, L.ks_token, L.ks_prompt, kTokensPad, &mp.kmap[i])) return rc;
     if (int rc = make_acc_map(L.acc, L.hw, L.n_prompts * L.heads * kTokens, &mp.amap[i])) return rc;
-    if (steps) {                                      // the second slab has the accumulator's shape: same map, other base
-      if (int rc = make_acc_map(steps->step[i], L.hw, L.n_prompts * L.heads * kTokens, &mp.smap[i])) return rc;
-      mp.step[i] = steps->step[i];
+    if (slabs) {                                      // the second slab has the accumulator's shape: same map, other base
+      if (int rc = make_acc_map(slabs->slab[i], L.hw, L.n_prompts * L.heads * kTokens, &mp.smap[i])) return rc;
+      mp.slab[i] = slabs->slab[i];
     }
     chunked = chunked || L.head_dim > 64;
   }
   cudaError_t attr_err = cudaSuccess;
   std::call_once(g_attr_once[dev.device & 63], [&] {
-    auto set = [&](const void* fn, int bytes) {
-      cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-      if (e != cudaSuccess) attr_err = e;
-    };
-    set((const void*)accumulate_mma_kernel<false, false, kSlabNone>, kSmemBytes);
-    set((const void*)accumulate_mma_kernel<false, true, kSlabNone>, kSmemBytes);
-    set((const void*)accumulate_mma_kernel<true, false, kSlabNone>, kSplitSmemBytes);
-    set((const void*)accumulate_mma_kernel<true, true, kSlabNone>, kSplitSmemBytes);
-    set((const void*)accumulate_mma_kernel<false, false, kSlabStore>, kStepSmemBytes);
-    set((const void*)accumulate_mma_kernel<false, true, kSlabStore>, kStepSmemBytes);
-    set((const void*)accumulate_mma_kernel<true, false, kSlabStore>, kSplitSmemBytes);
-    set((const void*)accumulate_mma_kernel<true, true, kSlabStore>, kSplitSmemBytes);
-    set((const void*)accumulate_mma_kernel<false, false, kSlabAdd>, kStepSmemBytes);
-    set((const void*)accumulate_mma_kernel<false, true, kSlabAdd>, kStepSmemBytes);
-    set((const void*)accumulate_mma_kernel<true, false, kSlabAdd>, kSplitSmemBytes);
-    set((const void*)accumulate_mma_kernel<true, true, kSlabAdd>, kSplitSmemBytes);
+    for (const MmaInstance& k : kMmaInstances)
+      if (cudaError_t e = cudaFuncSetAttribute(k.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, k.smem)) attr_err = e;
   });
   DAAM_CUDA_TRY(attr_err);
   pm.grid = dev.sm_count;                             // one CTA per SM (both forms fill its shared memory)
   if (pm.grid > p.total_tiles) pm.grid = p.total_tiles;
   pm.block = split ? kThreads : kThreads16;
-  pm.smem = split ? kSplitSmemBytes : (steps ? kStepSmemBytes : kSmemBytes);
   pm.variant = (split ? 1 : 0) | (chunked ? 2 : 0) | (mode << 2);
   return DAAM_OK;
 }
 
-namespace {
-template <bool kSplit, bool kChunked, int kSlab>
-cudaError_t launch_variant(const cudaLaunchConfig_t& cfg, const PreparedMma& pm) {
-  if constexpr (kSlab != kSlabNone)
-    return cudaLaunchKernelEx(&cfg, accumulate_mma_kernel<kSplit, kChunked, kSlab>, pm.mp);
-  else
-    return cudaLaunchKernelEx(&cfg, accumulate_mma_kernel<kSplit, kChunked, kSlabNone>,
-                              static_cast<const MmaParams&>(pm.mp));
-}
-}  // namespace
-
 int launch_prepared_mma(const void* prepared, cudaStream_t stream) {
   const PreparedMma& pm = *static_cast<const PreparedMma*>(prepared);
+  const MmaInstance& k = kMmaInstances[pm.variant];
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(pm.grid);
   cfg.blockDim = dim3(pm.block);
-  cfg.dynamicSmemBytes = pm.smem;
+  cfg.dynamicSmemBytes = k.smem;
   cfg.stream = stream;
   // Programmatic stream serialization also inside a stream capture: the launch becomes a kernel node with a programmatic
   // edge from its predecessor (CUDA >= 12.3).
@@ -811,20 +808,10 @@ int launch_prepared_mma(const void* prepared, cudaStream_t stream) {
   attr[0].val.programmaticStreamSerializationAllowed = pm.mp.base.pdl ? 1 : 0;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  switch (pm.variant) {
-    case 0: DAAM_CUDA_TRY((launch_variant<false, false, kSlabNone>(cfg, pm))); break;
-    case 1: DAAM_CUDA_TRY((launch_variant<true, false, kSlabNone>(cfg, pm))); break;
-    case 2: DAAM_CUDA_TRY((launch_variant<false, true, kSlabNone>(cfg, pm))); break;
-    case 3: DAAM_CUDA_TRY((launch_variant<true, true, kSlabNone>(cfg, pm))); break;
-    case 4: DAAM_CUDA_TRY((launch_variant<false, false, kSlabStore>(cfg, pm))); break;
-    case 5: DAAM_CUDA_TRY((launch_variant<true, false, kSlabStore>(cfg, pm))); break;
-    case 6: DAAM_CUDA_TRY((launch_variant<false, true, kSlabStore>(cfg, pm))); break;
-    case 7: DAAM_CUDA_TRY((launch_variant<true, true, kSlabStore>(cfg, pm))); break;
-    case 8: DAAM_CUDA_TRY((launch_variant<false, false, kSlabAdd>(cfg, pm))); break;
-    case 9: DAAM_CUDA_TRY((launch_variant<true, false, kSlabAdd>(cfg, pm))); break;
-    case 10: DAAM_CUDA_TRY((launch_variant<false, true, kSlabAdd>(cfg, pm))); break;
-    default: DAAM_CUDA_TRY((launch_variant<true, true, kSlabAdd>(cfg, pm))); break;
-  }
+  // the one kernel argument: the whole block for the second-slab instances, its MmaParams part for the plain ones
+  const MmaParams* plain = &pm.mp;
+  void* args[] = {(pm.variant >> 2) != kSlabNone ? (void*)&pm.mp : (void*)plain};
+  DAAM_CUDA_TRY(cudaLaunchKernelExC(&cfg, k.fn, args));
   DAAM_CUDA_TRY(cudaGetLastError());
   count_launch();
   return DAAM_OK;

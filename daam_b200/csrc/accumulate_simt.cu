@@ -6,9 +6,9 @@
 // shuffles and the accumulator update `acc[t][pixel] += p[t]` is one fully coalesced 128-byte access per warp and
 // token. Replaces daam/trace.py:276 (get_attention_scores), :219-244 (_unravel_attn) and :293-294 (update loop).
 //
-// The step-slab kernel (daam_accumulate_steps) is the same body with kStep: next to every add it stores the addend into
-// the layer's step slab, again one coalesced 128-byte access per warp and token (flushed like RED in reduce mode; in
-// load / add / store mode the add is an fma, so the stored value is the rounded product, i.e. fma(p, inv, 0)).
+// The step-slab kernel (daam_accumulate_steps) is the same body with kSlabStore: next to every add it stores the addend
+// into the layer's step slab, again one coalesced 128-byte access per warp and token (flushed like RED in reduce mode;
+// in load / add / store mode the add is an fma, so the stored value is the rounded product, i.e. fma(p, inv, 0)).
 // The range-slab kernel (daam_accumulate_range) adds the addend into the layer's range slab with the arithmetic of the
 // accumulator update: a second RED in reduce mode, fma(p, inv, old) in load / add / store mode.
 #include <mutex>
@@ -19,7 +19,7 @@ namespace daam {
 namespace {
 
 template <int kSlab>
-__device__ __forceinline__ void accumulate_simt_body(const LaunchParams& P, const StepSlabs* S) {
+__device__ __forceinline__ void accumulate_simt_body(const LaunchParams& P, const SecondSlabs* S) {
   extern __shared__ __align__(16) float smem[];
   // contiguous chunk of tiles per CTA: consecutive tiles share (layer, prompt, head), so K^T is staged once per run
   const int per = P.total_tiles / gridDim.x, rem = P.total_tiles % gridDim.x;
@@ -51,8 +51,8 @@ __device__ __forceinline__ void accumulate_simt_body(const LaunchParams& P, cons
 #pragma unroll
         for (int j = 0; j < kTokens; ++j) {
           atomicAdd(a + j * hw, s[j] * inv);          // result unused -> RED
-          if constexpr (kSlab == kSlabStore) S->step[t.li][off + j * hw] = add_ftz(0.f, s[j] * inv);
-          if constexpr (kSlab == kSlabAdd) atomicAdd(S->step[t.li] + off + j * hw, s[j] * inv);
+          if constexpr (kSlab == kSlabStore) S->slab[t.li][off + j * hw] = add_ftz(0.f, s[j] * inv);
+          if constexpr (kSlab == kSlabAdd) atomicAdd(S->slab[t.li] + off + j * hw, s[j] * inv);
         }
       } else {
         constexpr int kChunk = 11;                    // 77 = 7 x 11 loads in flight per thread
@@ -62,7 +62,7 @@ __device__ __forceinline__ void accumulate_simt_body(const LaunchParams& P, cons
 #pragma unroll
           for (int i = 0; i < kChunk; ++i) old[i] = a[(j0 + i) * hw];
           if constexpr (kSlab == kSlabAdd) {
-            float* r = S->step[t.li] + off;
+            float* r = S->slab[t.li] + off;
             float old_r[kChunk];
 #pragma unroll
             for (int i = 0; i < kChunk; ++i) old_r[i] = r[(j0 + i) * hw];
@@ -73,7 +73,7 @@ __device__ __forceinline__ void accumulate_simt_body(const LaunchParams& P, cons
           for (int i = 0; i < kChunk; ++i) a[(j0 + i) * hw] = fmaf(s[j0 + i], inv, old[i]);
           if constexpr (kSlab == kSlabStore) {
 #pragma unroll
-            for (int i = 0; i < kChunk; ++i) S->step[t.li][off + (j0 + i) * hw] = fmaf(s[j0 + i], inv, 0.f);
+            for (int i = 0; i < kChunk; ++i) S->slab[t.li][off + (j0 + i) * hw] = fmaf(s[j0 + i], inv, 0.f);
           }
         }
       }
@@ -87,20 +87,18 @@ __global__ void __launch_bounds__(kTilePixels, 3) accumulate_simt_kernel(const _
 
 // (defined before the step kernel: in this order nvcc keeps the step kernel at its register count, 150 instead of 151)
 __global__ void __launch_bounds__(kTilePixels, 3)
-accumulate_simt_range_kernel(const __grid_constant__ LaunchParams P, const __grid_constant__ StepSlabs S) {
+accumulate_simt_range_kernel(const __grid_constant__ LaunchParams P, const __grid_constant__ SecondSlabs S) {
   accumulate_simt_body<kSlabAdd>(P, &S);
 }
 
 __global__ void __launch_bounds__(kTilePixels, 3)
-accumulate_simt_step_kernel(const __grid_constant__ LaunchParams P, const __grid_constant__ StepSlabs S) {
+accumulate_simt_step_kernel(const __grid_constant__ LaunchParams P, const __grid_constant__ SecondSlabs S) {
   accumulate_simt_body<kSlabStore>(P, &S);
 }
 
-const void* simt_kernel(SlabMode mode) {
-  return mode == kSlabAdd     ? (const void*)accumulate_simt_range_kernel
-         : mode == kSlabStore ? (const void*)accumulate_simt_step_kernel
-                              : (const void*)accumulate_simt_kernel;
-}
+// The three kernels, indexed by SlabMode.
+const void* const kSimtInstances[] = {(const void*)accumulate_simt_kernel, (const void*)accumulate_simt_step_kernel,
+                                    (const void*)accumulate_simt_range_kernel};
 
 }  // namespace
 
@@ -111,7 +109,7 @@ int prepare_accumulate_simt(const LaunchParams& p, SlabMode mode, const DeviceIn
   const size_t smem = sizeof(float) * simt::tile_smem_floats(dmax);
   static std::mutex mu;
   static size_t configured_dev[3][64] = {};           // the attribute is per device (and per kernel)
-  const void* fn = simt_kernel(mode);
+  const void* fn = kSimtInstances[mode];
   {
     std::lock_guard<std::mutex> lock(mu);
     size_t& configured = configured_dev[mode][dev.device & 63];
@@ -130,15 +128,10 @@ int prepare_accumulate_simt(const LaunchParams& p, SlabMode mode, const DeviceIn
   return DAAM_OK;
 }
 
-int launch_prepared_simt(const LaunchParams& p, const StepSlabs* steps, SlabMode mode, int grid, size_t smem,
+int launch_prepared_simt(const LaunchParams& p, const SecondSlabs* slabs, SlabMode mode, int grid, size_t smem,
                          cudaStream_t stream) {
-  if (mode == kSlabAdd)
-    accumulate_simt_range_kernel<<<grid, kTilePixels, smem, stream>>>(p, *steps);
-  else if (mode == kSlabStore)
-    accumulate_simt_step_kernel<<<grid, kTilePixels, smem, stream>>>(p, *steps);
-  else
-    accumulate_simt_kernel<<<grid, kTilePixels, smem, stream>>>(p);
-  DAAM_CUDA_TRY(cudaGetLastError());
+  void* args[] = {const_cast<LaunchParams*>(&p), const_cast<SecondSlabs*>(slabs)};   // (the plain kernel reads args[0])
+  DAAM_CUDA_TRY(cudaLaunchKernel(kSimtInstances[mode], dim3(grid), dim3(kTilePixels), args, smem, stream));
   count_launch();
   return DAAM_OK;
 }

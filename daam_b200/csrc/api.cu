@@ -93,7 +93,7 @@ struct PlannedLaunch {
   bool is_mma = false;
   LaunchParams simt;                     // SIMT: the parameter block itself
   SlabMode mode = kSlabNone;             // SIMT: the step- or range-slab kernel, with these slabs
-  StepSlabs steps;
+  SecondSlabs slabs;
   int grid = 0;
   size_t smem = 0;
   struct MmaDeleter { void operator()(void* p) const { prepared_mma_delete(p); } };
@@ -126,28 +126,29 @@ bool acc_overlap(const LayerParams& a, const LayerParams& b) {
   return spans_overlap(a.acc, slab_bytes(a), b.acc, slab_bytes(b));
 }
 
-// daam_accumulate_steps / daam_accumulate_range: every second slab is non-null, 16-byte aligned, and shares no byte
-// with an accumulator or with another second slab of the call (the kernels store or add it tile by tile, in any order,
-// next to the accumulator update).
-int validate_steps(const daam_layer* layers, float* const* steps, int n_layers, SlabMode mode) {
-  const char* fn = mode == kSlabAdd ? "daam_accumulate_range" : "daam_accumulate_steps";
-  const char* what = mode == kSlabAdd ? "range" : "step";
-  if (!steps) { set_error("%s: %s_acc is a null array", fn, what); return DAAM_E_INVALID; }
+// The word the messages of daam_accumulate_steps / daam_accumulate_range use for their second slabs.
+const char* slab_word(SlabMode mode) { return mode == kSlabAdd ? "range" : "step"; }
+
+// daam_accumulate_steps / daam_accumulate_range (`fn`): every second slab is non-null, 16-byte aligned, and shares no
+// byte with an accumulator or with another second slab of the call (the kernels store or add it tile by tile, in any
+// order, next to the accumulator update).
+int validate_second_slabs(const char* fn, const daam_layer* layers, float* const* slabs, int n_layers, SlabMode mode) {
+  const char* what = slab_word(mode);
   std::vector<LayerParams> all((size_t)n_layers);
   for (int i = 0; i < n_layers; ++i)
     if (int rc = make_layer_params(layers[i], i, &all[i], /*need_acc=*/true)) return rc;
   for (int i = 0; i < n_layers; ++i) {
-    if (!steps[i]) { set_error("%s: layer %d has a null %s slab", fn, i, what); return DAAM_E_INVALID; }
-    if (reinterpret_cast<uintptr_t>(steps[i]) % 16 != 0) { set_error("%s: layer %d: the %s slab is not 16-byte aligned", fn, i, what); return DAAM_E_INVALID; }
+    if (!slabs[i]) { set_error("%s: layer %d has a null %s slab", fn, i, what); return DAAM_E_INVALID; }
+    if (reinterpret_cast<uintptr_t>(slabs[i]) % 16 != 0) { set_error("%s: layer %d: the %s slab is not 16-byte aligned", fn, i, what); return DAAM_E_INVALID; }
   }
   for (int i = 0; i < n_layers; ++i) {
     const size_t n = slab_bytes(all[i]);
     for (int j = 0; j < n_layers; ++j) {
-      if (spans_overlap(steps[i], n, all[j].acc, slab_bytes(all[j]))) {
+      if (spans_overlap(slabs[i], n, all[j].acc, slab_bytes(all[j]))) {
         set_error("%s: the %s slab of layer %d overlaps the accumulator of layer %d", fn, what, i, j);
         return DAAM_E_INVALID;
       }
-      if (j != i && spans_overlap(steps[i], n, steps[j], slab_bytes(all[j]))) {
+      if (j != i && spans_overlap(slabs[i], n, slabs[j], slab_bytes(all[j]))) {
         set_error("%s: the %s slabs of layers %d and %d overlap", fn, what, i, j);
         return DAAM_E_INVALID;
       }
@@ -156,13 +157,13 @@ int validate_steps(const daam_layer* layers, float* const* steps, int n_layers, 
   return DAAM_OK;
 }
 
-int build_plan(const daam_layer* layers, float* const* steps, SlabMode mode, int n_layers, uint32_t flags,
+int build_plan(const daam_layer* layers, float* const* slabs, SlabMode mode, int n_layers, uint32_t flags,
                const DeviceInfo& dev, Plan* plan) {
   const uint32_t path = flags & 3u, rmw = flags & DAAM_ACC_RMW_MASK;
   // Three packs: 16-bit layers for the wgmma kernel (TMA form), fp32 layers for its split form, and the rest for
   // the SIMT kernel. Each is closed when its parameter block is full.
   LaunchParams packs[3];                 // 0: wgmma 16-bit, 1: wgmma fp32, 2: SIMT
-  StepSlabs pack_steps[3];               // steps / range: the second slab of every layer of a pack
+  SecondSlabs pack_slabs[3];             // steps / range: the second slab of every layer of a pack
   for (LaunchParams& p : packs) {
     p.n_layers = p.total_tiles = 0;
     p.rmw_mode = (rmw == DAAM_ACC_RMW_LDST) ? 0 : 1;     // default: reduce-add
@@ -179,7 +180,7 @@ int build_plan(const daam_layer* layers, float* const* steps, SlabMode mode, int
     plan->launches.emplace_back();
     PlannedLaunch& l = plan->launches.back();
     l.is_mma = which != 2;
-    const StepSlabs* st = steps ? &pack_steps[which] : nullptr;
+    const SecondSlabs* st = slabs ? &pack_slabs[which] : nullptr;
     int rc;
     if (l.is_mma) {
       l.mma.reset(prepared_mma_new());
@@ -187,7 +188,7 @@ int build_plan(const daam_layer* layers, float* const* steps, SlabMode mode, int
     } else {
       l.simt = p;
       l.mode = mode;
-      if (st) l.steps = *st;
+      if (st) l.slabs = *st;
       rc = prepare_accumulate_simt(p, mode, dev, &l.grid, &l.smem);
     }
     p.n_layers = 0;
@@ -223,7 +224,7 @@ int build_plan(const daam_layer* layers, float* const* steps, SlabMode mode, int
     const int n_chunks = (L.head_dim + 63) / 64;
     L.weight = which == 1 ? n_chunks : 1 + 4 * n_chunks;
     L.weight_begin = p.total_weight;
-    if (steps) pack_steps[which].step[p.n_layers] = steps[i];
+    if (slabs) pack_slabs[which].slab[p.n_layers] = slabs[i];
     p.layer[p.n_layers++] = L;
     p.total_tiles += L.tiles_per_head * L.heads * L.n_prompts;
     p.total_weight += L.tiles_per_head * L.heads * L.n_prompts * L.weight;
@@ -241,40 +242,43 @@ int build_plan(const daam_layer* layers, float* const* steps, SlabMode mode, int
 namespace daam {
 namespace {
 
-// daam_accumulate (steps == nullptr, kSlabNone), daam_accumulate_steps (kSlabStore) and daam_accumulate_range
-// (kSlabAdd).
-int accumulate_impl(const daam_layer* layers, float* const* steps, SlabMode mode, int32_t n_layers, uint32_t flags,
-                    void* stream_) {
+// daam_accumulate (slabs == nullptr, kSlabNone), daam_accumulate_steps (kSlabStore) and daam_accumulate_range
+// (kSlabAdd), with the argument checks they share; `fn`: the entry point, as its messages name it.
+int accumulate_impl(const char* fn, const daam_layer* layers, float* const* slabs, SlabMode mode, int32_t n_layers,
+                    uint32_t flags, void* stream_) {
+  if (n_layers < 0 || (n_layers > 0 && !layers)) { set_error("%s: bad layer array", fn); return DAAM_E_INVALID; }
+  if (n_layers == 0) return DAAM_OK;
+  const bool with_slabs = mode != kSlabNone;
+  if (with_slabs && !slabs) { set_error("%s: %s_acc is a null array", fn, slab_word(mode)); return DAAM_E_INVALID; }
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DeviceInfo dev;
   if (int rc = get_device_info(&dev)) return rc;
 
   static thread_local std::vector<std::unique_ptr<Plan>> plans;    // per calling thread: no locking on the hot path
   static thread_local uint64_t clock = 0;
-  const bool with_steps = mode != kSlabNone;
   const size_t layer_bytes = sizeof(daam_layer) * (size_t)n_layers;
-  const size_t step_bytes = with_steps ? sizeof(float*) * (size_t)n_layers : 0;
-  const size_t bytes = layer_bytes + step_bytes;
+  const size_t slab_ptr_bytes = with_slabs ? sizeof(float*) * (size_t)n_layers : 0;
+  const size_t bytes = layer_bytes + slab_ptr_bytes;
   Plan* plan = nullptr;
   for (auto& c : plans)
     if (c->key.size() == bytes && c->flags == flags && c->device == dev.device && c->mode == mode &&
         memcmp(c->key.data(), layers, layer_bytes) == 0 &&
-        (!with_steps || memcmp(c->key.data() + layer_bytes, steps, step_bytes) == 0)) {
+        (!with_slabs || memcmp(c->key.data() + layer_bytes, slabs, slab_ptr_bytes) == 0)) {
       plan = c.get();
       break;
     }
   if (!plan) {
-    if (with_steps)
-      if (int rc = validate_steps(layers, steps, n_layers, mode)) return rc;
+    if (with_slabs)
+      if (int rc = validate_second_slabs(fn, layers, slabs, n_layers, mode)) return rc;
     std::unique_ptr<Plan> fresh(new Plan);
     fresh->key.assign(reinterpret_cast<const uint8_t*>(layers), reinterpret_cast<const uint8_t*>(layers) + layer_bytes);
-    if (with_steps)
-      fresh->key.insert(fresh->key.end(), reinterpret_cast<const uint8_t*>(steps),
-                        reinterpret_cast<const uint8_t*>(steps) + step_bytes);
+    if (with_slabs)
+      fresh->key.insert(fresh->key.end(), reinterpret_cast<const uint8_t*>(slabs),
+                        reinterpret_cast<const uint8_t*>(slabs) + slab_ptr_bytes);
     fresh->flags = flags;
     fresh->device = dev.device;
     fresh->mode = mode;
-    if (int rc = build_plan(layers, steps, mode, n_layers, flags, dev, fresh.get())) return rc;     // failed plans are not cached
+    if (int rc = build_plan(layers, slabs, mode, n_layers, flags, dev, fresh.get())) return rc;     // failed plans are not cached
     if (plans.size() >= kMaxPlans) {                                                   // evict the least recently used
       size_t oldest = 0;
       for (size_t i = 1; i < plans.size(); ++i)
@@ -289,7 +293,7 @@ int accumulate_impl(const daam_layer* layers, float* const* steps, SlabMode mode
   plan->stamp = ++clock;
   for (const PlannedLaunch& l : plan->launches) {
     const int rc = l.is_mma ? launch_prepared_mma(l.mma.get(), stream)
-                            : launch_prepared_simt(l.simt, l.mode != kSlabNone ? &l.steps : nullptr, l.mode, l.grid,
+                            : launch_prepared_simt(l.simt, l.mode != kSlabNone ? &l.slabs : nullptr, l.mode, l.grid,
                                                    l.smem, stream);
     if (rc) return rc;
   }
@@ -300,25 +304,17 @@ int accumulate_impl(const daam_layer* layers, float* const* steps, SlabMode mode
 }  // namespace daam
 
 extern "C" int daam_accumulate(const daam_layer* layers, int32_t n_layers, uint32_t flags, void* stream) {
-  if (n_layers < 0 || (n_layers > 0 && !layers)) { set_error("daam_accumulate: bad layer array"); return DAAM_E_INVALID; }
-  if (n_layers == 0) return DAAM_OK;
-  return accumulate_impl(layers, nullptr, kSlabNone, n_layers, flags, stream);
+  return accumulate_impl("daam_accumulate", layers, nullptr, kSlabNone, n_layers, flags, stream);
 }
 
 extern "C" int daam_accumulate_steps(const daam_layer* layers, float* const* step_acc, int32_t n_layers, uint32_t flags,
                                      void* stream) {
-  if (n_layers < 0 || (n_layers > 0 && !layers)) { set_error("daam_accumulate_steps: bad layer array"); return DAAM_E_INVALID; }
-  if (n_layers > 0 && !step_acc) { set_error("daam_accumulate_steps: step_acc is a null array"); return DAAM_E_INVALID; }
-  if (n_layers == 0) return DAAM_OK;
-  return accumulate_impl(layers, step_acc, kSlabStore, n_layers, flags, stream);
+  return accumulate_impl("daam_accumulate_steps", layers, step_acc, kSlabStore, n_layers, flags, stream);
 }
 
 extern "C" int daam_accumulate_range(const daam_layer* layers, float* const* range_acc, int32_t n_layers, uint32_t flags,
                                      void* stream) {
-  if (n_layers < 0 || (n_layers > 0 && !layers)) { set_error("daam_accumulate_range: bad layer array"); return DAAM_E_INVALID; }
-  if (n_layers > 0 && !range_acc) { set_error("daam_accumulate_range: range_acc is a null array"); return DAAM_E_INVALID; }
-  if (n_layers == 0) return DAAM_OK;
-  return accumulate_impl(layers, range_acc, kSlabAdd, n_layers, flags, stream);
+  return accumulate_impl("daam_accumulate_range", layers, range_acc, kSlabAdd, n_layers, flags, stream);
 }
 
 // ---- side-stream launcher ------------------------------------------------------------------------------------------

@@ -59,10 +59,10 @@ __device__ __forceinline__ float add_ftz(float a, float b) {
   return r;
 }
 
-// Step slabs of one launch (daam_accumulate_steps, daam_accumulate_range): step[i] has the layout of layer i's
-// accumulator.
-struct StepSlabs {
-  float* step[kMaxLayersPerLaunch];
+// Second slabs of one launch (daam_accumulate_steps: step slabs, daam_accumulate_range: range slabs): slab[i] has the
+// layout of layer i's accumulator.
+struct SecondSlabs {
+  float* slab[kMaxLayersPerLaunch];
 };
 // What the accumulate kernels do to the second slab next to the add: nothing (daam_accumulate), store the addend
 // (daam_accumulate_steps), or add it with the accumulator's arithmetic (daam_accumulate_range).
@@ -88,14 +88,14 @@ void count_launch(int n = 1);
 // ---- kernel launchers (one per translation unit) ----------------------------------------------------------------
 // Preparation (tensor maps, grid, shared-memory size) is split from the launch so that api.cu can cache it per
 // distinct daam_layer[] input: the steady state of a trace replays the same layer calls every denoising step.
-// `steps`: the launch's second slabs, nullptr exactly when `mode` is kSlabNone; `mode` selects the kernel instances
+// `slabs`: the launch's second slabs, nullptr exactly when `mode` is kSlabNone; `mode` selects the kernel instances
 // (kSlabStore: daam_accumulate_steps, kSlabAdd: daam_accumulate_range).
 int prepare_accumulate_simt(const LaunchParams& p, SlabMode mode, const DeviceInfo& dev, int* grid, size_t* smem);
-int launch_prepared_simt(const LaunchParams& p, const StepSlabs* steps, SlabMode mode, int grid, size_t smem,
+int launch_prepared_simt(const LaunchParams& p, const SecondSlabs* slabs, SlabMode mode, int grid, size_t smem,
                          cudaStream_t stream);
 void* prepared_mma_new();
 void prepared_mma_delete(void* prepared);
-int prepare_accumulate_mma(const LaunchParams& p, const StepSlabs* steps, SlabMode mode, const DeviceInfo& dev,
+int prepare_accumulate_mma(const LaunchParams& p, const SecondSlabs* slabs, SlabMode mode, const DeviceInfo& dev,
                            void* prepared);
 int launch_prepared_mma(const void* prepared, cudaStream_t stream);
 bool mma_supported(const LayerParams& l);

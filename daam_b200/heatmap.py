@@ -58,6 +58,17 @@ class LayerSlab:
     def n_prompts(self) -> int:
         return self.acc.shape[0]
 
+    @property
+    def second(self) -> List[torch.Tensor]:
+        """The slabs the accumulate launches write next to ``acc``: the step slab, the range slabs, or none."""
+        return [self.step] if self.step is not None else (self.ranges or [])
+
+    def zero_(self):
+        """Zero the accumulator and the range slabs (a step slab needs no zeroing: every step rewrites it whole)."""
+        self.acc.zero_()
+        for r in self.ranges or ():
+            r.zero_()
+
     def key_view(self, head: int, prompt: int = 0, step_range: Optional[int] = None) -> torch.Tensor:
         src = self.acc if step_range is None else self.ranges[step_range]
         return src[prompt, head].view(src.shape[2], self.h, self.w)
@@ -150,16 +161,21 @@ class RawHeatMapCollection:
     def items(self, prompt: int = 0, *, step_range: Optional[int] = None) -> Iterator[Tuple[RawHeatMapKey, torch.Tensor]]:
         """``((factor, layer, head), [77, h, w])`` for every key; with ``step_range=i`` the per-key sums over the steps
         of declared range ``i`` (``trace(pipe, step_ranges=[...])``) instead of over every step."""
+        for slab in self.read_slabs(step_range):
+            for head in range(slab.heads):
+                yield (slab.factor, slab.layer_idx, head), slab.key_view(head, prompt, step_range)
+
+    def read_slabs(self, step_range: Optional[int] = None) -> List[LayerSlab]:
+        """The slabs a read reduces, once every pending accumulate is visible: the live slabs, or with ``step_range``
+        those with range slabs, after checking the index and that the range has received a step."""
         if step_range is not None:
             self.check_step_range(step_range)
         self._synchronize()
-        if step_range is not None and self.range_steps[step_range] == 0:
+        if step_range is None:
+            return self.live_slabs()
+        if self.range_steps[step_range] == 0:
             raise RuntimeError('No heat maps found for the given parameters.')
-        for slab in self.live_slabs():
-            if step_range is not None and slab.ranges is None:
-                continue
-            for head in range(slab.heads):
-                yield (slab.factor, slab.layer_idx, head), slab.key_view(head, prompt, step_range)
+        return [s for s in self.live_slabs() if s.ranges is not None]
 
     def check_step_range(self, step_range: int):
         """Raises unless ``step_range`` indexes a range declared with ``trace(pipe, step_ranges=[...])``."""
@@ -182,9 +198,7 @@ class RawHeatMapCollection:
             self._zero(live)
         else:
             for slab in live:
-                slab.acc.zero_()
-                for r in slab.ranges or ():
-                    r.zero_()
+                slab.zero_()
         self.range_steps = [0] * self.n_ranges
         for slab in live:                     # graph-captured layers stay live: replays bypass the Python hook
             slab.touched = slab.captured

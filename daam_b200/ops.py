@@ -68,55 +68,47 @@ def pack(descs: Sequence[_native.DaamLayer]) -> _native.PackedLayers:
     return _native.PackedLayers(list(descs))
 
 
-def accumulate(descs, device, stream: Optional[torch.cuda.Stream] = None, flags: int = _native.ACC_AUTO):
-    """Enqueue the fused kernel over the given layer calls (sequence of descriptors or :func:`pack` result) on
-    ``stream`` (default: the current stream of ``device``)."""
+def _run_on(device, stream: Optional[torch.cuda.Stream], launch):
+    """``launch(stream_ptr)`` with ``device`` current, on ``stream`` (default: the current stream of ``device``)."""
     dev = device if isinstance(device, torch.device) else torch.device(device)
     index = dev.index if dev.index is not None else torch.cuda.current_device()
     s = torch.cuda.current_stream(index) if stream is None else stream
     if index == torch.cuda.current_device():
-        _native.accumulate(descs, s.cuda_stream, flags)
+        launch(s.cuda_stream)
     else:
         with torch.cuda.device(index):
-            _native.accumulate(descs, s.cuda_stream, flags)
+            launch(s.cuda_stream)
+
+
+def accumulate(descs, device, stream: Optional[torch.cuda.Stream] = None, flags: int = _native.ACC_AUTO):
+    """Enqueue the fused kernel over the given layer calls (sequence of descriptors or :func:`pack` result) on
+    ``stream`` (default: the current stream of ``device``)."""
+    _run_on(device, stream, lambda s: _native.accumulate(descs, s, flags))
+
+
+def _accumulate_second(native_fn, word: str, descs, slabs, device, stream, flags: int):
+    """``native_fn`` (:func:`_native.accumulate_steps` / :func:`_native.accumulate_range`) over ``descs`` and one second
+    slab per descriptor; ``word`` names the slabs in messages."""
+    if not isinstance(slabs, _native.StepPointers):
+        for t in slabs:
+            if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
+                raise RuntimeError(f'{word} slabs must be contiguous fp32 CUDA tensors')
+        slabs = _native.StepPointers([t.data_ptr() for t in slabs])
+    _run_on(device, stream, lambda s: native_fn(descs, slabs, s, flags))
 
 
 def accumulate_steps(descs, steps, device, stream: Optional[torch.cuda.Stream] = None, flags: int = _native.ACC_AUTO):
     """:func:`accumulate`, and also store what each layer adds into its step slab (``daam_accumulate_steps``).
     ``steps``: one contiguous fp32 tensor per descriptor, shaped like its accumulator, or a prepared
     :class:`_native.StepPointers`."""
-    dev = device if isinstance(device, torch.device) else torch.device(device)
-    index = dev.index if dev.index is not None else torch.cuda.current_device()
-    s = torch.cuda.current_stream(index) if stream is None else stream
-    if not isinstance(steps, _native.StepPointers):
-        for t in steps:
-            if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
-                raise RuntimeError('step slabs must be contiguous fp32 CUDA tensors')
-        steps = _native.StepPointers([t.data_ptr() for t in steps])
-    if index == torch.cuda.current_device():
-        _native.accumulate_steps(descs, steps, s.cuda_stream, flags)
-    else:
-        with torch.cuda.device(index):
-            _native.accumulate_steps(descs, steps, s.cuda_stream, flags)
+    _accumulate_second(_native.accumulate_steps, 'step', descs, steps, device, stream, flags)
 
 
 def accumulate_range(descs, ranges, device, stream: Optional[torch.cuda.Stream] = None, flags: int = _native.ACC_AUTO):
     """:func:`accumulate`, and also add what each layer adds into its range slab, with the accumulator's arithmetic
     (``daam_accumulate_range``). ``ranges``: one contiguous fp32 tensor per descriptor, shaped like its accumulator, or
     a prepared :class:`_native.StepPointers`."""
-    dev = device if isinstance(device, torch.device) else torch.device(device)
-    index = dev.index if dev.index is not None else torch.cuda.current_device()
-    s = torch.cuda.current_stream(index) if stream is None else stream
-    if not isinstance(ranges, _native.StepPointers):
-        for t in ranges:
-            if not (t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()):
-                raise RuntimeError('range slabs must be contiguous fp32 CUDA tensors')
-        ranges = _native.StepPointers([t.data_ptr() for t in ranges])
-    if index == torch.cuda.current_device():
-        _native.accumulate_range(descs, ranges, s.cuda_stream, flags)
-    else:
-        with torch.cuda.device(index):
-            _native.accumulate_range(descs, ranges, s.cuda_stream, flags)
+    _accumulate_second(_native.accumulate_range, 'range', descs, ranges, device, stream, flags)
 
 
 def accumulate_layer(q: torch.Tensor, k: torch.Tensor, heads: int, scale: Optional[float] = None,

@@ -64,20 +64,19 @@ class DiffusionHeatMapHooker(AggregateHooker):
                  step_ranges=None):
         if launch not in ('step', 'overlap', 'layer'):
             raise ValueError("launch must be 'step', 'overlap' or 'layer'")
+        modes = []                             # the enabled second-slab modes, and why each needs the step launch
         if step_ranges is not None:
             step_ranges = _normalize_step_ranges(step_ranges)
+            modes.append(('step_ranges', 'which range a launch adds into depends on the UNet forward it ends'))
+        if time_resolved:
+            modes.append(('time_resolved=True', "the per-step heat map is finalized right after the step's launch"))
+        for name, why in modes:
             if launch != 'step':
-                raise ValueError("step_ranges needs launch='step': which range a launch adds into depends on the UNet "
-                                 "forward it ends, on the forward's own stream")
+                raise ValueError(f"{name} needs launch='step': {why}, on the forward's own stream")
             if save_heads or load_heads:
-                raise ValueError('step_ranges does not support save_heads / load_heads')
-            if time_resolved:
-                raise ValueError('step_ranges cannot be combined with time_resolved=True')
-        if time_resolved and launch != 'step':
-            raise ValueError("time_resolved=True needs launch='step': the per-step heat map is finalized right after "
-                             "the step's launch, on the forward's own stream")
-        if time_resolved and (save_heads or load_heads):
-            raise ValueError('time_resolved=True does not support save_heads / load_heads')
+                raise ValueError(f'{name} does not support save_heads / load_heads')
+        if len(modes) > 1:
+            raise ValueError('step_ranges cannot be combined with time_resolved=True')
         _native.load()   # fail here, loudly, if the CUDA library is missing
         self.all_heat_maps = RawHeatMapCollection()
         side = pipeline.unet.config.sample_size * pipeline.vae_scale_factor
@@ -108,20 +107,22 @@ class DiffusionHeatMapHooker(AggregateHooker):
         self._stream: Optional[torch.cuda.Stream] = None
         self._dirty = False                    # side-stream work not yet ordered before the current stream
         self.all_heat_maps.bind(self.synchronize, self._zero_slabs)
-        # time-resolved mode: the step slab of every slot of the step array, and per prompt a device history
-        # [capacity, n_rows, x, x] of per-step global heat maps (grown by doubling, restarted every generation)
+        # time-resolved mode: per prompt a device history [capacity, n_rows, x, x] of per-step global heat maps (grown
+        # by doubling, restarted every generation)
         self.time_resolved = time_resolved
         self.all_heat_maps.time_resolved = time_resolved
-        self._step_ptrs = _native.StepPointers([0] * 64) if time_resolved else None
         self._history: List[torch.Tensor] = []
         self._time_steps = 0
         self._history_rows: Optional[List[int]] = None   # n_rows of every prompt of the running generation
-        # step-range mode: per declared range, the range slab of every slot of the step array; the UNet forward index
+        # step-range mode: the UNet forward index of the running generation
         self.step_ranges: Optional[List[Tuple[int, int]]] = step_ranges
         self.all_heat_maps.n_ranges = len(step_ranges) if step_ranges else 0
         self.all_heat_maps.range_steps = [0] * self.all_heat_maps.n_ranges
-        self._range_ptrs = [_native.StepPointers([0] * 64) for _ in step_ranges] if step_ranges else None
         self._forward_idx = 0
+        # the second slab of every slot of the step array (LayerSlab.second): one array of step slabs in time-resolved
+        # mode, one array of range slabs per declared range in step-range mode, none otherwise
+        self._slab_ptrs = [_native.StepPointers([0] * 64)
+                           for _ in range(1 if time_resolved else self.all_heat_maps.n_ranges)]
 
         modules = [
             UNetCrossAttentionHooker(m, self, layer_idx=idx, latent_hw=self.latent_hw, load_heads=load_heads,
@@ -221,16 +222,7 @@ class DiffusionHeatMapHooker(AggregateHooker):
             raise RuntimeError(f'layer {layer_idx}: {hw} query positions are not a square map')
         # "second half of the batch*heads axis" (trace.py:240): the conditional samples of a CFG batch
         _, n_samples, head0, n_heads = ops.cond_half(bsz, heads)
-        # Samples vs prompts: diffusers repeats every prompt num_images_per_prompt times (prompt-major), and the
-        # reference's keys then enumerate images x heads of its single prompt (the "head" index of a key runs over
-        # the whole kept axis, trace.py:240, 293-294). The slab is therefore [prompts][images * heads]; the kernel
-        # sees the same memory as [samples][heads].
-        n_real = len(self.last_prompts) if self.last_prompts else (n_samples if self.batch_prompts else 1)
-        if n_real > 1 and not self.batch_prompts:
-            raise ValueError('Only single prompt generation is supported for heat map computation.')
-        if n_samples % n_real != 0:
-            raise RuntimeError(f'layer {layer_idx}: {n_samples} conditional samples for {n_real} prompts')
-        images = n_samples // n_real
+        n_real, images = self._prompt_layout(layer_idx, n_samples)
         slab = self.all_heat_maps.slab_for(layer_idx, factor, n_real, images * n_heads, side, side, q.device, head0)
         self._epoch_seen = self.all_heat_maps.epoch        # (this call may have bumped it; the other layers' slabs stand)
         desc = ops.make_layer_desc(q, k, slab.acc.view(n_samples, n_heads, slab.acc.shape[2], hw), heads, scale)
@@ -242,18 +234,11 @@ class DiffusionHeatMapHooker(AggregateHooker):
                 self._packed = grown
                 self._slots = [grown.array[i] for i in range(len(grown.array))]
                 self._layer_state.clear()                  # cached slot proxies point into the old array
-                if self._step_ptrs is not None:
-                    old = list(self._step_ptrs.array)
-                    self._step_ptrs = _native.StepPointers(old + [0] * (len(grown.array) - len(old)))
-                if self._range_ptrs is not None:
-                    self._range_ptrs = [_native.StepPointers(list(r.array) + [0] * (len(grown.array) - len(r.array)))
-                                        for r in self._range_ptrs]
+                self._slab_ptrs = [_native.StepPointers(list(p.array) + [0] * (len(grown.array) - len(p.array)))
+                                   for p in self._slab_ptrs]
             self._packed.array[pos] = desc
-            if self._step_ptrs is not None:
-                self._step_ptrs.array[pos] = slab.step.data_ptr()
-            if self._range_ptrs is not None:
-                for ptrs, r in zip(self._range_ptrs, slab.ranges):
-                    ptrs.array[pos] = r.data_ptr()
+            for ptrs, second in zip(self._slab_ptrs, slab.second):
+                ptrs.array[pos] = second.data_ptr()
             slot, own = self._slots[pos], None
         else:
             own = _native.PackedLayers([desc])             # 'layer' mode: every layer launches its own 1-element array
@@ -265,29 +250,32 @@ class DiffusionHeatMapHooker(AggregateHooker):
         self._device = q.device
         return state, q, k
 
+    def _prompt_layout(self, layer_idx: int, n_samples: int) -> Tuple[int, int]:
+        """``(prompts, images per prompt)`` of a layer call's ``n_samples`` conditional samples.
+
+        Samples vs prompts: diffusers repeats every prompt num_images_per_prompt times (prompt-major), and the
+        reference's keys then enumerate images x heads of its single prompt (the "head" index of a key runs over the
+        whole kept axis, trace.py:240, 293-294). A slab is therefore [prompts][images * heads]; the kernel sees the same
+        memory as [samples][heads]."""
+        n_real = len(self.last_prompts) if self.last_prompts else (n_samples if self.batch_prompts else 1)
+        if n_real > 1 and not self.batch_prompts:
+            raise ValueError('Only single prompt generation is supported for heat map computation.')
+        if n_samples % n_real != 0:
+            raise RuntimeError(f'layer {layer_idx}: {n_samples} conditional samples for {n_real} prompts')
+        return n_real, n_samples // n_real
+
     def _launch_now(self, own, device):
         """``launch='layer'``: the layer's kernel right away on the current stream (the producer of Q/K may be the
         immediately preceding kernel there, so no EARLY_LOADS)."""
-        index = device.index if device.index is not None else torch.cuda.current_device()
-        stream = torch.cuda.current_stream(index).cuda_stream
-        if index == torch.cuda.current_device():
-            _native.accumulate(own, stream, self.kernel_flags)
-        else:
-            with torch.cuda.device(index):
-                _native.accumulate(own, stream, self.kernel_flags)
+        ops._run_on(device, None, lambda stream: _native.accumulate(own, stream, self.kernel_flags))
 
     def _accumulate_probs(self, layer_idx: int, factor: int, probs: torch.Tensor, bsz: int, heads: int):
         """Heat maps from materialised probabilities (save_heads / load_heads compatibility path)."""
         hw = probs.shape[1]
         side = int(math.sqrt(hw))
         _, n_samples, head0, n_heads = ops.cond_half(bsz, heads)
-        n_real = len(self.last_prompts) if self.last_prompts else (n_samples if self.batch_prompts else 1)
-        if n_real > 1 and not self.batch_prompts:
-            raise ValueError('Only single prompt generation is supported for heat map computation.')
-        if n_samples % n_real != 0:
-            raise RuntimeError(f'layer {layer_idx}: {n_samples} conditional samples for {n_real} prompts')
-        slab = self.all_heat_maps.slab_for(layer_idx, factor, n_real, (n_samples // n_real) * n_heads, side, side,
-                                           probs.device, head0)
+        n_real, images = self._prompt_layout(layer_idx, n_samples)
+        slab = self.all_heat_maps.slab_for(layer_idx, factor, n_real, images * n_heads, side, side, probs.device, head0)
         self.synchronize()
         ops.accumulate_probs(probs, slab.acc)
 
@@ -309,39 +297,36 @@ class DiffusionHeatMapHooker(AggregateHooker):
         try:
             capturing = torch.cuda.is_current_stream_capturing()
             if capturing:
-                if self.time_resolved:                         # drop the step: its projections live in the graph's pool
+                if self._slab_ptrs:                            # drop the step: its projections live in the graph's pool
                     self._refs, self._n_pending = [], 0
-                    raise RuntimeError('time_resolved=True cannot be captured into a CUDA graph: every step writes its '
-                                       'heat map into another history slot, which a graph replay cannot follow')
-                if self.step_ranges is not None:
-                    self._refs, self._n_pending = [], 0
-                    raise RuntimeError('step_ranges cannot be captured into a CUDA graph: which range slabs a step adds '
-                                       'into depends on the step index, which a graph replay cannot follow')
+                    what, why = ('time_resolved=True', 'every step writes its heat map into another history slot') \
+                        if self.time_resolved else \
+                        ('step_ranges', 'which range slabs a step adds into depends on the step index')
+                    raise RuntimeError(f'{what} cannot be captured into a CUDA graph: {why}, which a graph replay '
+                                       f'cannot follow')
                 # CUDA-graph capture of the UNet step: the launch becomes a node of the captured stream; replays bypass the
                 # Python hook, so the layers of this launch stay live across per-generation resets
                 step = self._step_id
                 for layer_idx, st in self._layer_state.items():
                     if self._queued.get(layer_idx) == step:
                         st[4].captured = True
-            if self.time_resolved:
-                # launch == 'step' (checked at construction): on the forward's own stream, like the branch below; then
-                # the step's global heat maps, in stream order behind it
-                _native.accumulate_steps(packed, self._step_ptrs, current, flags)
-                self._finalize_step(device, current)
-            elif self.step_ranges is not None:
-                # launch == 'step' (checked at construction), on the forward's own stream as below
-                r = self._range_of(self._forward_idx)
-                if r is None:
-                    _native.accumulate(packed, current, flags)
-                else:
-                    _native.accumulate_range(packed, self._range_ptrs[r], current, flags)
-                    self.all_heat_maps.range_steps[r] += 1
-                self._forward_idx += 1
-            elif capturing or self.launch == 'step':
+            if capturing or self.launch == 'step':
                 # On the forward's own stream: the predecessor there is the tail of the UNet forward, never a producer of
                 # the queued Q/K, so only the accumulator updates have to wait for it (EARLY_LOADS). Stream order also
-                # makes it safe to drop the projections right after the launch.
-                _native.accumulate(packed, current, flags)
+                # makes it safe to drop the projections right after the launch. The second-slab modes need this launch
+                # (checked at construction): time-resolved mode stores into the step slabs, then reduces them to the
+                # step's global heat maps in stream order behind it; step-range mode adds into the slabs of the range
+                # this forward lies in, if any.
+                r = self._range_of(self._forward_idx) if self.step_ranges is not None else None
+                if self.time_resolved:
+                    _native.accumulate_steps(packed, self._slab_ptrs[0], current, flags)
+                    self._finalize_step(device, current)
+                elif r is not None:
+                    _native.accumulate_range(packed, self._slab_ptrs[r], current, flags)
+                    self.all_heat_maps.range_steps[r] += 1
+                else:
+                    _native.accumulate(packed, current, flags)
+                self._forward_idx += 1
             else:
                 side = self._side_stream(device)
                 if self._launcher is None:
@@ -384,9 +369,7 @@ class DiffusionHeatMapHooker(AggregateHooker):
                 grown = torch.empty((2 * t,) + tuple(hist.shape[1:]), dtype=torch.float32, device=device)
                 grown[:t].copy_(hist)
                 self._history[p] = hist = grown
-            groups = [_native.DaamKeyGroup(acc=s.step[p].data_ptr(), heads=s.heads, h=s.h, w=s.w,
-                                           tokens=s.step.shape[2], head_sel=-1, reserved=0) for s in slabs]
-            _native.finalize(groups, x, n_rows, False, hist[t].data_ptr(), stream)
+            _native.finalize([_key_group(s.step[p], s) for s in slabs], x, n_rows, False, hist[t].data_ptr(), stream)
         self._time_steps = t + 1
 
     def _restart_history(self):
@@ -424,9 +407,7 @@ class DiffusionHeatMapHooker(AggregateHooker):
             return
         self.synchronize()
         for slab in slabs:
-            slab.acc.zero_()
-            for r in slab.ranges or ():
-                r.zero_()
+            slab.zero_()
         if self._stream is not None:   # later side-stream launches must see the zeroed slabs
             self._stream.wait_stream(torch.cuda.current_stream(slabs[0].acc.device))
 
@@ -440,29 +421,9 @@ class DiffusionHeatMapHooker(AggregateHooker):
         ``batch_prompts`` mode. ``step_range=i`` aggregates over the steps of declared range ``i`` only
         (``trace(pipe, step_ranges=[...])``): the DAAM map a trace of only those steps would give.
         """
-        if prompt is None:
-            prompt = self.last_prompts[prompt_idx] if self.last_prompts else self.last_prompt
-        factors = {0, 1, 2, 4, 8, 16, 32, 64} if factors is None else set(factors)
-        x = int(np.sqrt(self.latent_hw))
-        self._check_step_range(step_range)
-        self.synchronize()
-        groups, keep = [], []
-        for slab in self._slabs_for(step_range):
-            if slab.factor not in factors or (layer_idx is not None and layer_idx != slab.layer_idx):
-                continue
-            if head_idx is not None and not 0 <= head_idx < slab.heads:
-                continue
-            acc = (slab.acc if step_range is None else slab.ranges[step_range])[prompt_idx]
-            groups.append(_native.DaamKeyGroup(acc=acc.data_ptr(), heads=slab.heads, h=slab.h, w=slab.w,
-                                               tokens=acc.shape[1], head_sel=-1 if head_idx is None else head_idx,
-                                               reserved=0))
-            keep.append(acc)
-        if not groups:
-            if head_idx is not None or layer_idx is not None:
-                raise RuntimeError('No heat maps found for the given parameters.')
-            raise RuntimeError('No heat maps found. Did you forget to call `with trace(...)` during generation?')
-        n_rows = min(len(self.pipe.tokenizer.tokenize(prompt)) + 2, _native.TOKENS)   # 1 for SOS and 1 for padding
-        device = keep[0].device
+        prompt, x, n_rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range, layer_idx,
+                                                             head_idx)
+        device = slabs[0].acc.device
         maps = torch.empty((n_rows, x, x), dtype=torch.float32, device=device)
         with torch.cuda.device(device):
             _native.finalize(groups, x, n_rows, normalize, maps.data_ptr(),
@@ -498,44 +459,44 @@ class DiffusionHeatMapHooker(AggregateHooker):
         (daam/run/generate.py:239-255) in one launch. Returns ``(keys, maps)``: ``keys[i] = (factor, layer, head)`` and
         ``maps[i]`` the ``[n_tokens + 2, x, x]`` heat map the reference computes for that single key. ``step_range=i``:
         over the steps of declared range ``i`` only, as in :meth:`compute_global_heat_map`."""
-        if prompt is None:
-            prompt = self.last_prompts[prompt_idx] if self.last_prompts else self.last_prompt
-        factors = {0, 1, 2, 4, 8, 16, 32, 64} if factors is None else set(factors)
-        x = int(np.sqrt(self.latent_hw))
-        self._check_step_range(step_range)
-        self.synchronize()
-        groups, keep, keys = [], [], []
-        for slab in self._slabs_for(step_range):
-            if slab.factor not in factors:
-                continue
-            acc = (slab.acc if step_range is None else slab.ranges[step_range])[prompt_idx]
-            groups.append(_native.DaamKeyGroup(acc=acc.data_ptr(), heads=slab.heads, h=slab.h, w=slab.w,
-                                               tokens=acc.shape[1], head_sel=-1, reserved=0))
-            keep.append(acc)
-            keys += [(slab.factor, slab.layer_idx, head) for head in range(slab.heads)]
-        if not groups:
-            raise RuntimeError('No heat maps found. Did you forget to call `with trace(...)` during generation?')
-        n_rows = min(len(self.pipe.tokenizer.tokenize(prompt)) + 2, _native.TOKENS)
-        device = keep[0].device
+        prompt, x, n_rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range)
+        keys = [(slab.factor, slab.layer_idx, head) for slab in slabs for head in range(slab.heads)]
+        device = slabs[0].acc.device
         maps = torch.empty((len(keys), n_rows, x, x), dtype=torch.float32, device=device)
         with torch.cuda.device(device):
             _native.finalize_per_key(groups, x, n_rows, normalize, maps.data_ptr(),
                                      torch.cuda.current_stream(device).cuda_stream)
         return keys, maps
 
-    def _check_step_range(self, step_range: Optional[int]):
-        if step_range is not None:
-            self.all_heat_maps.check_step_range(step_range)
+    def _read_groups(self, prompt, factors, prompt_idx: int, step_range: Optional[int], layer_idx=None, head_idx=None):
+        """What the heat-map reads share: the prompt (default: the generation's), the map side ``x``, the row count, and
+        the key groups of prompt ``prompt_idx`` over the live slabs (with ``step_range``: over that range's slabs) that
+        pass the filters, with the slabs behind them. Raises when no slab passes."""
+        if prompt is None:
+            prompt = self.last_prompts[prompt_idx] if self.last_prompts else self.last_prompt
+        factors = {0, 1, 2, 4, 8, 16, 32, 64} if factors is None else set(factors)
+        groups, slabs = [], []
+        for slab in self.all_heat_maps.read_slabs(step_range):
+            if slab.factor not in factors or (layer_idx is not None and layer_idx != slab.layer_idx):
+                continue
+            if head_idx is not None and not 0 <= head_idx < slab.heads:
+                continue
+            acc = (slab.acc if step_range is None else slab.ranges[step_range])[prompt_idx]
+            groups.append(_key_group(acc, slab, -1 if head_idx is None else head_idx))
+            slabs.append(slab)
+        if not groups:
+            if head_idx is not None or layer_idx is not None:
+                raise RuntimeError('No heat maps found for the given parameters.')
+            raise RuntimeError('No heat maps found. Did you forget to call `with trace(...)` during generation?')
+        n_rows = min(len(self.pipe.tokenizer.tokenize(prompt)) + 2, _native.TOKENS)   # 1 for SOS and 1 for padding
+        return prompt, int(np.sqrt(self.latent_hw)), n_rows, groups, slabs
 
-    def _slabs_for(self, step_range: Optional[int]) -> List[LayerSlab]:
-        """The live slabs a read reduces; with ``step_range``, those with range slabs, after checking (synchronized)
-        that the range has received a step."""
-        slabs = self.all_heat_maps.live_slabs()
-        if step_range is None:
-            return slabs
-        if self.all_heat_maps.range_steps[step_range] == 0:
-            raise RuntimeError('No heat maps found for the given parameters.')
-        return [s for s in slabs if s.ranges is not None]
+
+def _key_group(acc: torch.Tensor, slab: LayerSlab, head_sel: int = -1) -> _native.DaamKeyGroup:
+    """The finalize input of one prompt's ``[heads, 77, hw]`` slab of ``slab``'s layer (its accumulator, step slab or a
+    range slab); ``head_sel``: one head, or -1 for all."""
+    return _native.DaamKeyGroup(acc=acc.data_ptr(), heads=slab.heads, h=slab.h, w=slab.w, tokens=acc.shape[1],
+                                head_sel=head_sel, reserved=0)
 
 
 def _normalize_step_ranges(step_ranges) -> List[Tuple[int, int]]:

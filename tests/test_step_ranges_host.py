@@ -76,13 +76,13 @@ def test_ranges_are_normalised_in_declared_order():
 def test_reads_need_the_option():
     pipe = make_pipeline(TINY_SPEC, dtype=torch.float32, device='cpu', seed=0)
     tc = trace(pipe)
-    assert tc.step_ranges is None and tc.all_heat_maps.n_ranges == 0 and tc._range_ptrs is None
+    assert tc.step_ranges is None and tc.all_heat_maps.n_ranges == 0 and tc._slab_ptrs == []
     for read in (lambda: tc.compute_global_heat_map(step_range=0), lambda: tc.compute_per_head_heat_maps(step_range=0),
                  lambda: list(tc.all_heat_maps.items(step_range=0))):
         with pytest.raises(RuntimeError, match='step_ranges'):
             read()
     tc = trace(pipe, step_ranges=[range(2, 4), (0, 2)])
-    assert tc.step_ranges == [(2, 4), (0, 2)] and tc.all_heat_maps.n_ranges == 2
+    assert tc.step_ranges == [(2, 4), (0, 2)] and tc.all_heat_maps.n_ranges == 2 and len(tc._slab_ptrs) == 2
     assert tc.step_range_counts == [0, 0]
     with pytest.raises(IndexError):
         tc.compute_global_heat_map(step_range=2)

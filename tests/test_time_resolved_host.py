@@ -37,11 +37,11 @@ def test_option_is_keyword_only_and_off_by_default():
 def test_accessor_needs_the_mode_and_a_generation():
     pipe = make_pipeline(TINY_SPEC, dtype=torch.float32, device='cpu', seed=0)
     tc = trace(pipe)
-    assert tc.all_heat_maps.time_resolved is False and tc._step_ptrs is None
+    assert tc.all_heat_maps.time_resolved is False and tc._slab_ptrs == []
     with pytest.raises(RuntimeError, match='time_resolved=True'):
         tc.compute_time_heat_maps()
     tc = trace(pipe, time_resolved=True)
-    assert tc.all_heat_maps.time_resolved is True
+    assert tc.all_heat_maps.time_resolved is True and len(tc._slab_ptrs) == 1
     with pytest.raises(RuntimeError, match='No heat maps found'):
         tc.compute_time_heat_maps()
 
