@@ -8,7 +8,7 @@ from __future__ import annotations
 
 import ctypes
 import os
-from typing import Optional, Sequence
+from typing import Optional, Sequence, Tuple
 
 LIB_NAME = 'libdaam_b200.so'
 LIB_PATH = os.path.join(os.path.dirname(os.path.abspath(__file__)), LIB_NAME)
@@ -25,6 +25,8 @@ EXPAND_SCRATCH_FLOATS = 64   # DAAM_EXPAND_SCRATCH_FLOATS: per word
 
 EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize',
            'daam_finalize_per_key', 'daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
+           'daam_finalize_rect', 'daam_finalize_per_key_rect', 'daam_normalize_maps_rect', 'daam_word_heat_map_rect',
+           'daam_expand_as_rect', 'daam_expand_words_rect',
            'daam_side_launcher_create', 'daam_side_launcher_destroy',
            'daam_side_launcher_launch', 'daam_side_launcher_join', 'daam_side_launcher_idle', 'daam_abi_version',
            'daam_last_error', 'daam_device_info', 'daam_launch_count')
@@ -98,6 +100,17 @@ def load() -> ctypes.CDLL:
     lib.daam_expand_words.argtypes = [vp, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32, i32, i32, f32,
                                       vp, vp, vp, vp]
     lib.daam_expand_words.restype = ctypes.c_int
+    # the rectangular siblings: (map_h, map_w) where the square entry points take x
+    lib.daam_finalize_rect.argtypes = [ctypes.POINTER(DaamKeyGroup), i32, i32, i32, i32, i32, vp, vp]
+    lib.daam_finalize_per_key_rect.argtypes = [ctypes.POINTER(DaamKeyGroup), i32, i32, i32, i32, i32, vp, vp]
+    lib.daam_normalize_maps_rect.argtypes = [vp, i32, i32, i32, i32, vp]
+    lib.daam_word_heat_map_rect.argtypes = [vp, i32, i32, i32, ctypes.POINTER(i32), i32, vp, vp]
+    lib.daam_expand_as_rect.argtypes = [vp, i32, i32, i32, i32, i32, i32, f32, vp, vp, vp]
+    lib.daam_expand_words_rect.argtypes = [vp, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
+                                           i32, i32, f32, vp, vp, vp, vp]
+    for name in ('daam_finalize_rect', 'daam_finalize_per_key_rect', 'daam_normalize_maps_rect',
+                 'daam_word_heat_map_rect', 'daam_expand_as_rect', 'daam_expand_words_rect'):
+        getattr(lib, name).restype = ctypes.c_int
     lib.daam_side_launcher_create.argtypes = [ctypes.POINTER(vp)]
     lib.daam_side_launcher_create.restype = ctypes.c_int
     lib.daam_side_launcher_destroy.argtypes = [vp]
@@ -212,8 +225,18 @@ def accumulate_range(layers, ranges, stream: int, flags: int = ACC_AUTO):
     _accumulate_second('daam_accumulate_range', 'range', layers, ranges, stream, flags)
 
 
-def normalize_maps(maps_ptr: int, n_maps: int, n_rows: int, x: int, stream: int):
-    _check(load().daam_normalize_maps(ctypes.c_void_p(maps_ptr), n_maps, n_rows, x, ctypes.c_void_p(stream)))
+def map_size(x) -> Tuple[int, int]:
+    """A heat-map grid given as its side ``x`` (square) or as ``(h, w)``: returns ``(h, w)``."""
+    if isinstance(x, (tuple, list)):      # (torch.Size is a tuple)
+        h, w = x
+        return int(h), int(w)
+    return int(x), int(x)
+
+
+def normalize_maps(maps_ptr: int, n_maps: int, n_rows: int, x, stream: int):
+    """``x``: the map side, or ``(h, w)``."""
+    h, w = map_size(x)
+    _check(load().daam_normalize_maps_rect(ctypes.c_void_p(maps_ptr), n_maps, n_rows, h, w, ctypes.c_void_p(stream)))
 
 
 def attention_probs(layer: DaamLayer, probs_ptr: int, stream: int):
@@ -225,38 +248,45 @@ def accumulate_probs(probs_ptr: int, dtype: int, first_row: int, n_rows: int, hw
     _check(load().daam_accumulate_probs(probs_ptr, dtype, first_row, n_rows, hw, tokens, acc_ptr, stream))
 
 
-def finalize(groups: Sequence[DaamKeyGroup], x: int, n_rows: int, normalize: bool, out_ptr: int, stream: int):
+# The finalize / word-map / expand wrappers take the map grid as its side ``x`` or as ``(h, w)`` and call the ``_rect``
+# entry points (the square ones are their (x, x) case in the library).
+def finalize(groups: Sequence[DaamKeyGroup], x, n_rows: int, normalize: bool, out_ptr: int, stream: int):
+    h, w = map_size(x)
     n = len(groups)
     arr = (DaamKeyGroup * max(n, 1))(*groups)
-    _check(load().daam_finalize(arr, n, x, n_rows, int(bool(normalize)), ctypes.c_void_p(out_ptr),
-                                ctypes.c_void_p(stream)))
-
-
-def finalize_per_key(groups: Sequence[DaamKeyGroup], x: int, n_rows: int, normalize: bool, out_ptr: int, stream: int):
-    n = len(groups)
-    arr = (DaamKeyGroup * max(n, 1))(*groups)
-    _check(load().daam_finalize_per_key(arr, n, x, n_rows, int(bool(normalize)), ctypes.c_void_p(out_ptr),
-                                        ctypes.c_void_p(stream)))
-
-
-def word_heat_map(maps_ptr: int, n_rows: int, x: int, rows: Sequence[int], out_ptr: int, stream: int):
-    arr = (ctypes.c_int32 * max(len(rows), 1))(*rows)
-    _check(load().daam_word_heat_map(ctypes.c_void_p(maps_ptr), n_rows, x, arr, len(rows), ctypes.c_void_p(out_ptr),
+    _check(load().daam_finalize_rect(arr, n, h, w, n_rows, int(bool(normalize)), ctypes.c_void_p(out_ptr),
                                      ctypes.c_void_p(stream)))
 
 
-def expand_as(map_ptr: int, x: int, out_h: int, out_w: int, absolute: bool, threshold: Optional[float], out_ptr: int,
+def finalize_per_key(groups: Sequence[DaamKeyGroup], x, n_rows: int, normalize: bool, out_ptr: int, stream: int):
+    h, w = map_size(x)
+    n = len(groups)
+    arr = (DaamKeyGroup * max(n, 1))(*groups)
+    _check(load().daam_finalize_per_key_rect(arr, n, h, w, n_rows, int(bool(normalize)), ctypes.c_void_p(out_ptr),
+                                             ctypes.c_void_p(stream)))
+
+
+def word_heat_map(maps_ptr: int, n_rows: int, x, rows: Sequence[int], out_ptr: int, stream: int):
+    h, w = map_size(x)
+    arr = (ctypes.c_int32 * max(len(rows), 1))(*rows)
+    _check(load().daam_word_heat_map_rect(ctypes.c_void_p(maps_ptr), n_rows, h, w, arr, len(rows),
+                                          ctypes.c_void_p(out_ptr), ctypes.c_void_p(stream)))
+
+
+def expand_as(map_ptr: int, x, out_h: int, out_w: int, absolute: bool, threshold: Optional[float], out_ptr: int,
               scratch_ptr: int, stream: int):
+    h, w = map_size(x)
     use_thr = bool(threshold)   # the reference's `if threshold:` (daam/heatmap.py:87)
-    _check(load().daam_expand_as(ctypes.c_void_p(map_ptr), x, out_h, out_w, int(bool(absolute)), int(use_thr),
-                                 float(threshold) if use_thr else 0.0, ctypes.c_void_p(out_ptr),
-                                 ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
+    _check(load().daam_expand_as_rect(ctypes.c_void_p(map_ptr), h, w, out_h, out_w, int(bool(absolute)), int(use_thr),
+                                      float(threshold) if use_thr else 0.0, ctypes.c_void_p(out_ptr),
+                                      ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
 
 
-def expand_words(maps_ptr: int, n_rows: int, x: int, rows_per_word: Sequence[Sequence[int]], out_h: int, out_w: int,
+def expand_words(maps_ptr: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int, out_w: int,
                  absolute: bool, threshold: Optional[float], word_maps_ptr: Optional[int], out_ptr: int, scratch_ptr: int,
                  stream: int):
     """``rows_per_word[w]``: the rows of ``maps`` word ``w`` averages (already offset for SOS)."""
+    h, w = map_size(x)
     flat = [r for rows in rows_per_word for r in rows]
     begin = [0]
     for rows in rows_per_word:
@@ -264,10 +294,11 @@ def expand_words(maps_ptr: int, n_rows: int, x: int, rows_per_word: Sequence[Seq
     rows_arr = (ctypes.c_int32 * max(len(flat), 1))(*flat)
     begin_arr = (ctypes.c_int32 * len(begin))(*begin)
     use_thr = bool(threshold)   # the reference's `if threshold:` (daam/heatmap.py:87)
-    _check(load().daam_expand_words(ctypes.c_void_p(maps_ptr), n_rows, x, rows_arr, begin_arr, len(rows_per_word), out_h,
-                                    out_w, int(bool(absolute)), int(use_thr), float(threshold) if use_thr else 0.0,
-                                    ctypes.c_void_p(word_maps_ptr) if word_maps_ptr else None,
-                                    ctypes.c_void_p(out_ptr), ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
+    _check(load().daam_expand_words_rect(ctypes.c_void_p(maps_ptr), n_rows, h, w, rows_arr, begin_arr,
+                                         len(rows_per_word), out_h, out_w, int(bool(absolute)), int(use_thr),
+                                         float(threshold) if use_thr else 0.0,
+                                         ctypes.c_void_p(word_maps_ptr) if word_maps_ptr else None,
+                                         ctypes.c_void_p(out_ptr), ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
 
 
 def device_info():

@@ -21,7 +21,7 @@ constexpr int kMaxGroups = 160;   // key groups (layer x prompt slices) per fina
 constexpr int kMaxRows = 128;     // selected rows of a word map
 
 struct FinalizeParams {
-  int n_groups, x, n_rows, n_keys;
+  int n_groups, oh, ow, n_rows, n_keys;   // output map [oh][ow]
   daam_key_group g[kMaxGroups];
 };
 
@@ -63,13 +63,13 @@ __device__ __forceinline__ float bicubic_at(const float* __restrict__ src, int w
   return v;
 }
 
-// grid: (ceil(x*x / 256), n_rows). One thread = one output element (row t, pixel o); it walks every selected key.
+// grid: (ceil(oh*ow / 256), n_rows). One thread = one output element (row t, pixel o); it walks every selected key.
 __global__ void __launch_bounds__(256) finalize_kernel(const __grid_constant__ FinalizeParams P, float* __restrict__ out) {
   const int o = blockIdx.x * blockDim.x + threadIdx.x;
   const int t = blockIdx.y;
-  const int x = P.x;
-  if (o >= x * x) return;
-  const int oy = o / x, ox = o - oy * x;
+  const int oh = P.oh, ow = P.ow;
+  if (o >= oh * ow) return;
+  const int oy = o / ow, ox = o - oy * ow;
   float sum = 0.f;
   int ch = -1, cw = -1;
   Taps ty, tx;
@@ -78,10 +78,10 @@ __global__ void __launch_bounds__(256) finalize_kernel(const __grid_constant__ F
     const int hw = G.h * G.w;
     const int h0 = G.head_sel < 0 ? 0 : G.head_sel;
     const int h1 = G.head_sel < 0 ? G.heads : G.head_sel + 1;
-    const bool same = (G.h == x && G.w == x);
+    const bool same = (G.h == oh && G.w == ow);
     if (!same && (G.h != ch || G.w != cw)) {
-      ty = make_taps(oy, G.h, x);
-      tx = make_taps(ox, G.w, x);
+      ty = make_taps(oy, G.h, oh);
+      tx = make_taps(ox, G.w, ow);
       ch = G.h; cw = G.w;
     }
     const float* base = G.acc + (long long)t * hw;
@@ -94,19 +94,21 @@ __global__ void __launch_bounds__(256) finalize_kernel(const __grid_constant__ F
       for (int head = h0; head < h1; ++head) sum += fmaxf(bicubic_at(base + head * head_stride, G.w, ty, tx), 0.f);
     }
   }
-  out[(long long)t * x * x + o] = sum / (float)P.n_keys;
+  out[(long long)t * oh * ow + o] = sum / (float)P.n_keys;
 }
 
 
 // ---- fast path: integer upsampling factors 1 / 2 / 4 -------------------------------------------------------------
-// One CTA owns one output band (BR = 8 or 4 rows x x columns) of one token row and walks the key classes (distinct
-// source resolutions) one after the other. With an integer factor F the cubic weights depend only on the output phase
-// (F distinct weight sets per axis), and the F x F outputs under one source pixel read the same 5 x 5 source window: a
-// thread owns ONE source pixel and emits its F x F outputs from one window (25 values, 9-14 FMAs per output).
+// One CTA owns one output band (BR = 8 or 4 rows x ow columns; the last band is partial when BR does not divide oh) of
+// one token row and walks the key classes (distinct (kh, kw) source sizes) one after the other. A class has one integer
+// factor F on both axes (oh = F kh, ow = F kw), so the cubic weights depend only on the output phase (F distinct weight
+// sets per axis), and the F x F outputs under one source pixel read the same 5 x 5 source window: a thread owns ONE
+// source pixel and emits its F x F outputs from one window (25 values, 9-14 FMAs per output).
 // The windows come from shared memory: the band's source rows (+2 halo rows each side, clamped at the borders) of a
-// CHUNK of keys are streamed in with 16-byte cp.async (every thread has several independent copies in flight, two
-// chunks double-buffered), so the key loop is no longer a chain of dependent global loads -- the round-1 kernel's bound
-// (34.8 us for the 175-key SD-2.1 case, 222 registers, 0.86 waves) -- and the kernel fits two CTAs per SM.
+// CHUNK of keys are streamed in with cp.async -- 16-byte units, or 8- / 4-byte units when a key row is not a multiple of
+// 4 floats (every thread has several independent copies in flight, two chunks double-buffered) -- so the key loop is no
+// longer a chain of dependent global loads -- the round-1 kernel's bound (34.8 us for the 175-key SD-2.1 case, 222
+// registers, 0.86 waves) -- and the kernel fits two CTAs per SM.
 // When a class has fewer source pixels per band than threads, the spare thread groups take every kg-th key and the
 // groups are merged through the shared-memory band in a fixed order (deterministic sums). Arithmetic per key is
 // bit-identical to bicubic_at (same taps, same weights, same order).
@@ -160,37 +162,55 @@ __device__ __forceinline__ void cp_async16(float* smem_dst, const float* gsrc) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc)
                : "memory");
 }
+// 8- and 4-byte units (key rows that are not a multiple of 4 floats); .cg takes 16-byte copies only
+__device__ __forceinline__ void cp_async8(float* smem_dst, const float* gsrc) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc)
+               : "memory");
+}
+__device__ __forceinline__ void cp_async4(float* smem_dst, const float* gsrc) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc)
+               : "memory");
+}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
 
 // Streams chunk `chunk` of a factor-2 / factor-4 class into `buf` (one commit group): the band's source rows (+2 halo rows
-// each side, border rows replicated like the clamped taps) of up to kc keys. Every thread copies one fixed 16-byte unit
-// of every keys_par-th key. Shared by the class passes and by the cross-class prefetch (next class's first chunk).
+// each side, border rows replicated like the clamped taps) of up to kc keys. Every thread copies fixed units (16, 8 or 4
+// bytes: the widest that divides a key row) of every keys_par-th key; a key with more units than threads is copied by
+// all threads, 256 units apart. Shared by the class passes and by the cross-class prefetch (next class's first chunk).
 struct ChunkGeom {
-  int region, kc, n_src, kg, VR;
-  __device__ __forceinline__ ChunkGeom(int side, int f, int br) {
+  int region, kc, n_src, kg, VR, unit;
+  __device__ __forceinline__ ChunkGeom(int kw, int f, int br) {
     const int R = br / f;                              // source rows under the band
     VR = R + 4;                                        // + 2 halo rows above and below
-    region = VR * side;                                // floats of one key's staged rows
-    n_src = R * side;                                  // source pixels under the band (<= 256, checked by the host)
+    region = VR * kw;                                  // floats of one key's staged rows
+    n_src = R * kw;                                    // source pixels under the band (<= 256, checked by the host)
     kg = 256 / n_src;                                  // thread groups that split the keys
     kc = kStageFloats / region;                        // keys per chunk, a multiple of kg so every group keeps its stride
     kc -= kc % kg;
+    unit = kw % 4 == 0 ? 4 : (kw % 2 == 0 ? 2 : 1);    // floats per cp.async
   }
 };
-__device__ __forceinline__ void issue_chunk(int side, int f, int band, int br, const float* const* keys, int nk, int chunk,
-                                            float* buf) {
-  const ChunkGeom G(side, f, br);
-  const int row_units = side / 4, key_units = G.VR * row_units;     // 16-byte units
-  const int keys_par = 256 / key_units, copy_k = (int)threadIdx.x / key_units;
+__device__ __forceinline__ void issue_chunk(int kh, int kw, int f, int band, int br, const float* const* keys, int nk,
+                                            int chunk, float* buf) {
+  const ChunkGeom G(kw, f, br);
+  const int u = G.unit, row_units = kw / u, key_units = G.VR * row_units;
+  const int keys_par = key_units <= 256 ? 256 / key_units : 1, copy_k = (int)threadIdx.x / key_units;
   const int k0 = chunk * G.kc, kn = min(G.kc, nk - k0);
   if (copy_k < keys_par) {
-    const int pos = (int)threadIdx.x - copy_k * key_units;
-    const int vr = pos / row_units, c4 = pos - vr * row_units;
-    const int src = min(max(band * (br / f) - 2 + vr, 0), side - 1) * side + 4 * c4;
-    float* dst = buf + vr * side + 4 * c4;
-    for (int k = copy_k; k < kn; k += keys_par) cp_async16(dst + k * G.region, keys[k0 + k] + src);
+    for (int pos = (int)threadIdx.x - copy_k * key_units; pos < key_units; pos += 256) {
+      const int vr = pos / row_units, c = pos - vr * row_units;
+      const int src = min(max(band * (br / f) - 2 + vr, 0), kh - 1) * kw + u * c;
+      float* dst = buf + vr * kw + u * c;
+      if (u == 4) {
+        for (int k = copy_k; k < kn; k += keys_par) cp_async16(dst + k * G.region, keys[k0 + k] + src);
+      } else if (u == 2) {
+        for (int k = copy_k; k < kn; k += keys_par) cp_async8(dst + k * G.region, keys[k0 + k] + src);
+      } else {
+        for (int k = copy_k; k < kn; k += keys_par) cp_async4(dst + k * G.region, keys[k0 + k] + src);
+      }
+    }
   }
   cp_async_commit();
 }
@@ -198,29 +218,29 @@ __device__ __forceinline__ void issue_chunk(int side, int f, int band, int br, c
 // What to prefetch while a class is being merged: the first chunk of the next factor-2 / factor-4 class (into chunk
 // buffer 1; the merge parks the key groups in buffer 0).
 struct NextClass {
-  int side, f, nk;                                     // f == 0: nothing to prefetch
+  int kh, kw, f, nk;                                   // f == 0: nothing to prefetch
   const float* const* keys;
 };
 
 // `first_buf`: the chunk buffer holding this class's chunk 0 (1 when the previous class prefetched it, else 0 and the
 // chunk is issued here).
 template <int F>
-__device__ __forceinline__ void class_pass(const FinalizeParams& P, int side, int nk, int band, int br, float* tile,
+__device__ __forceinline__ void class_pass(const FinalizeParams& P, int kh, int kw, int nk, int band, int br, float* tile,
                                            const float* const* keys, float* stage, bool prefetched, const NextClass& next) {
-  const int x = P.x;
-  const ChunkGeom G(side, F, br);
+  const int ow = P.ow;
+  const ChunkGeom G(kw, F, br);
   const int region = G.region, n_src = G.n_src, kg = G.kg, kc = G.kc;
   const int n_chunks = (nk + kc - 1) / kc;
   const int first_buf = prefetched ? 1 : 0;
-  auto issue = [&](int c) { issue_chunk(side, F, band, br, keys, nk, c, stage + ((c + first_buf) & 1) * kStageFloats); };
+  auto issue = [&](int c) { issue_chunk(kh, kw, F, band, br, keys, nk, c, stage + ((c + first_buf) & 1) * kStageFloats); };
 
   const int group = (int)threadIdx.x / n_src;
   const int s = (int)threadIdx.x - group * n_src;
   const bool live = group < kg;
-  const int ly = s / side, sx = s - ly * side;
+  const int ly = s / kw, sx = s - ly * kw;
   int ix[5];
 #pragma unroll
-  for (int j = 0; j < 5; ++j) ix[j] = min(max(sx - 2 + j, 0), side - 1);
+  for (int j = 0; j < 5; ++j) ix[j] = min(max(sx - 2 + j, 0), kw - 1);
   PhaseWeights<F> pw;
   pw.init();
   float acc[F][F];
@@ -234,7 +254,7 @@ __device__ __forceinline__ void class_pass(const FinalizeParams& P, int side, in
     if (c + 1 < n_chunks) { issue(c + 1); cp_async_wait<1>(); } else { cp_async_wait<0>(); }
     __syncthreads();                                   // chunk c has landed for every thread
     if (live) {
-      const float* buf = stage + ((c + first_buf) & 1) * kStageFloats + ly * side;
+      const float* buf = stage + ((c + first_buf) & 1) * kStageFloats + ly * kw;
       const int kn = min(kc, nk - c * kc);
       for (int k = group; k < kn; k += kg) {
         const float* src = buf + k * region;
@@ -242,23 +262,25 @@ __device__ __forceinline__ void class_pass(const FinalizeParams& P, int side, in
 #pragma unroll
         for (int i = 0; i < 5; ++i)
 #pragma unroll
-          for (int j = 0; j < 5; ++j) v[i][j] = src[i * side + ix[j]];
+          for (int j = 0; j < 5; ++j) v[i][j] = src[i * kw + ix[j]];
         add_key<F>(pw, v, acc);
       }
     }
     __syncthreads();                                   // buffer (c & 1) may be overwritten by chunk c + 2
   }
   // both chunk buffers are free now: the next class's first chunk streams into buffer 1 while this class is merged
-  if (next.f) issue_chunk(next.side, next.f, band, br, next.keys, next.nk, 0, stage + kStageFloats);
+  if (next.f) issue_chunk(next.kh, next.kw, next.f, band, br, next.keys, next.nk, 0, stage + kStageFloats);
   // merge the key groups in a fixed order (deterministic sums): every group parks its band in the (now free) first
-  // chunk buffer, then each band element is summed over the groups by one thread
-  const int band_elems = br * x;
+  // chunk buffer, then each band element is summed over the groups by one thread. Source rows past the map's last row
+  // (a partial last band) were staged from the clamped border row: their outputs land in band rows that are never
+  // written out.
+  const int band_elems = br * ow;
   if (live) {
-    float* mine = stage + group * band_elems + (ly * F) * x + sx * F;
+    float* mine = stage + group * band_elems + (ly * F) * ow + sx * F;
 #pragma unroll
     for (int py = 0; py < F; ++py)
 #pragma unroll
-      for (int px = 0; px < F; ++px) mine[py * x + px] = acc[py][px];
+      for (int px = 0; px < F; ++px) mine[py * ow + px] = acc[py][px];
   }
   __syncthreads();
   for (int i = threadIdx.x; i < band_elems; i += blockDim.x) {
@@ -269,14 +291,16 @@ __device__ __forceinline__ void class_pass(const FinalizeParams& P, int side, in
   __syncthreads();
 }
 
-// factor 1: bicubic at scale 1 is the identity, the class contributes clamp(src) -- coalesced float4 reads; when the
-// band has fewer float4s than threads, the spare thread groups take every kg-th key (merged in a fixed order)
-__device__ __forceinline__ void class_pass_identity(const FinalizeParams& P, int nk, int band, int br, float* tile,
+// factor 1: bicubic at scale 1 is the identity, the class contributes clamp(src) -- coalesced float4 reads over the
+// band's `rows` valid rows (rows * ow is a multiple of 4: ow * br is, and a partial last band ends at h * w, which the
+// host checks); when the band has fewer float4s than threads, the spare thread groups take every kg-th key (merged in a
+// fixed order)
+__device__ __forceinline__ void class_pass_identity(const FinalizeParams& P, int nk, int band, int br, int rows, float* tile,
                                                     const float* const* keys, float* stage, const NextClass& next) {
-  const int x = P.x;
+  const int ow = P.ow;
   // this pass reads its keys straight from global memory: the next class's first chunk streams in underneath it
-  if (next.f) issue_chunk(next.side, next.f, band, br, next.keys, next.nk, 0, stage + kStageFloats);
-  const int n4 = br * x / 4;
+  if (next.f) issue_chunk(next.kh, next.kw, next.f, band, br, next.keys, next.nk, 0, stage + kStageFloats);
+  const int n_el = rows * ow, n4 = n_el / 4;
   const int kg = n4 >= 256 ? 1 : 256 / n4;
   const int passes = (n4 + 255) / 256;
   for (int pass = 0; pass < passes; ++pass) {
@@ -285,7 +309,7 @@ __device__ __forceinline__ void class_pass_identity(const FinalizeParams& P, int
     const bool live = i < n4 && group < kg;
     float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
     if (live) {
-      const long long off = (long long)band * br * x + 4 * i;
+      const long long off = (long long)band * br * ow + 4 * i;
 #pragma unroll 8
       for (int k = group; k < nk; k += kg) {
         const float4 v = __ldg(reinterpret_cast<const float4*>(keys[k] + off));
@@ -301,11 +325,11 @@ __device__ __forceinline__ void class_pass_identity(const FinalizeParams& P, int
       }
       __syncthreads();
     } else {                                             // park the groups' bands, then sum them in a fixed order
-      if (live) *reinterpret_cast<float4*>(stage + group * (br * x) + 4 * i) = acc;
+      if (live) *reinterpret_cast<float4*>(stage + group * n_el + 4 * i) = acc;
       __syncthreads();
-      for (int e = threadIdx.x; e < br * x; e += blockDim.x) {
+      for (int e = threadIdx.x; e < n_el; e += blockDim.x) {
         float sum = tile[e];
-        for (int g = 0; g < kg; ++g) sum += stage[g * (br * x) + e];
+        for (int g = 0; g < kg; ++g) sum += stage[g * n_el + e];
         tile[e] = sum;
       }
       __syncthreads();
@@ -316,12 +340,12 @@ __device__ __forceinline__ void class_pass_identity(const FinalizeParams& P, int
 struct ClassList {
   int n;
   int band_rows;            // 8, or 4 when that is what fills the machine / keeps a band's source pixels within one CTA
-  int side[8];              // distinct source sides, all dividing x with factor 1, 2 or 4
+  int kh[8], kw[8];         // distinct source sizes, each (oh / F, ow / F) with F = 1, 2 or 4
   int key_begin[9];         // keys[] is ordered class by class: class c owns [key_begin[c], key_begin[c + 1])
   int key_slot[kMaxGroups]; // where group g's first selected key goes in keys[]
 };
 
-// grid: (x / band_rows bands, n_rows); dynamic smem: two chunk buffers + the band tile (band_rows * x floats)
+// grid: (ceil(oh / band_rows) bands, n_rows); dynamic smem: two chunk buffers + the band tile (band_rows * ow floats)
 __global__ void __launch_bounds__(256, 2) finalize_fast_kernel(const __grid_constant__ FinalizeParams P,
                                                                const __grid_constant__ ClassList C,
                                                                float* __restrict__ out) {
@@ -329,7 +353,8 @@ __global__ void __launch_bounds__(256, 2) finalize_fast_kernel(const __grid_cons
   __shared__ const float* keys[kMaxClassKeys];
   float* stage = dyn;                                  // 2 x kStageFloats
   float* tile = dyn + 2 * kStageFloats;
-  const int band = blockIdx.x, t = blockIdx.y, x = P.x, br = C.band_rows;
+  const int band = blockIdx.x, t = blockIdx.y, oh = P.oh, ow = P.ow, br = C.band_rows;
+  const int rows = min(br, oh - band * br);            // valid output rows of this band
   // key pointers (token row t) of every selected key, class by class; one thread per key group
   for (int g = threadIdx.x; g < P.n_groups; g += blockDim.x) {
     const daam_key_group& G = P.g[g];
@@ -338,29 +363,29 @@ __global__ void __launch_bounds__(256, 2) finalize_fast_kernel(const __grid_cons
     const long long hw = (long long)G.h * G.w;
     for (int head = h0; head < h1; ++head) keys[C.key_slot[g] + head - h0] = G.acc + ((long long)head * G.tokens + t) * hw;
   }
-  for (int i = threadIdx.x; i < br * x; i += blockDim.x) tile[i] = 0.f;
+  for (int i = threadIdx.x; i < br * ow; i += blockDim.x) tile[i] = 0.f;
   __syncthreads();
   bool prefetched = false;                             // chunk 0 of class c is already streaming into buffer 1
   for (int c = 0; c < C.n; ++c) {
-    const int side = C.side[c], f = x / side, nk = C.key_begin[c + 1] - C.key_begin[c];
+    const int kh = C.kh[c], kw = C.kw[c], f = ow / kw, nk = C.key_begin[c + 1] - C.key_begin[c];
     const float* const* ck = keys + C.key_begin[c];
-    NextClass next = {0, 0, 0, nullptr};
-    if (c + 1 < C.n && C.side[c + 1] != x)
-      next = {C.side[c + 1], x / C.side[c + 1], C.key_begin[c + 2] - C.key_begin[c + 1], keys + C.key_begin[c + 1]};
-    if (f == 1) class_pass_identity(P, nk, band, br, tile, ck, stage, next);
-    else if (f == 2) class_pass<2>(P, side, nk, band, br, tile, ck, stage, prefetched, next);
-    else class_pass<4>(P, side, nk, band, br, tile, ck, stage, prefetched, next);
+    NextClass next = {0, 0, 0, 0, nullptr};
+    if (c + 1 < C.n && C.kw[c + 1] != ow)
+      next = {C.kh[c + 1], C.kw[c + 1], ow / C.kw[c + 1], C.key_begin[c + 2] - C.key_begin[c + 1], keys + C.key_begin[c + 1]};
+    if (f == 1) class_pass_identity(P, nk, band, br, rows, tile, ck, stage, next);
+    else if (f == 2) class_pass<2>(P, kh, kw, nk, band, br, tile, ck, stage, prefetched, next);
+    else class_pass<4>(P, kh, kw, nk, band, br, tile, ck, stage, prefetched, next);
     prefetched = next.f != 0;
   }
   __syncthreads();
-  float* dst = out + (long long)t * x * x + (long long)band * br * x;
-  for (int i = threadIdx.x; i < br * x; i += blockDim.x) dst[i] = tile[i] / (float)P.n_keys;
+  float* dst = out + (long long)t * oh * ow + (long long)band * br * ow;
+  for (int i = threadIdx.x; i < rows * ow; i += blockDim.x) dst[i] = tile[i] / (float)P.n_keys;
 }
 
-// One output map per selected key (no mean): out[key][row][x][x] = clamp(bicubic(key[row])). grid: (ceil(x*x/256), n_rows,
-// n_keys); key k belongs to group g with first_key[g] <= k < first_key[g + 1].
+// One output map per selected key (no mean): out[key][row][oh][ow] = clamp(bicubic(key[row])). grid: (ceil(oh*ow/256),
+// n_rows, n_keys); key k belongs to group g with first_key[g] <= k < first_key[g + 1].
 struct PerKeyParams {
-  int n_groups, x, n_rows, n_keys;
+  int n_groups, oh, ow, n_rows, n_keys;
   int first_key[kMaxGroups + 1];
   daam_key_group g[kMaxGroups];
 };
@@ -368,8 +393,8 @@ struct PerKeyParams {
 __global__ void __launch_bounds__(256) finalize_per_key_kernel(const __grid_constant__ PerKeyParams P, float* __restrict__ out) {
   const int o = blockIdx.x * blockDim.x + threadIdx.x;
   const int t = blockIdx.y, key = blockIdx.z;
-  const int x = P.x;
-  if (o >= x * x) return;
+  const int oh = P.oh, ow = P.ow;
+  if (o >= oh * ow) return;
   int g = 0;
   while (g + 1 < P.n_groups && key >= P.first_key[g + 1]) ++g;
   const daam_key_group& G = P.g[g];
@@ -377,13 +402,13 @@ __global__ void __launch_bounds__(256) finalize_per_key_kernel(const __grid_cons
   const int hw = G.h * G.w;
   const float* src = G.acc + ((long long)head * G.tokens + t) * hw;
   float v;
-  if (G.h == x && G.w == x) {
+  if (G.h == oh && G.w == ow) {
     v = __ldg(src + o);
   } else {
-    const int oy = o / x, ox = o - oy * x;
-    v = bicubic_at(src, G.w, make_taps(oy, G.h, x), make_taps(ox, G.w, x));
+    const int oy = o / ow, ox = o - oy * ow;
+    v = bicubic_at(src, G.w, make_taps(oy, G.h, oh), make_taps(ox, G.w, ow));
   }
-  out[((long long)key * P.n_rows + t) * x * x + o] = fmaxf(v, 0.f);
+  out[((long long)key * P.n_rows + t) * oh * ow + o] = fmaxf(v, 0.f);
 }
 
 // maps / (maps[1:-1].sum(0) + 1e-6), in place (daam/trace.py:129-130)
@@ -412,10 +437,11 @@ __global__ void word_map_kernel(const float* __restrict__ maps, const __grid_con
 }
 
 // ---- fused word list -> image-size masks -------------------------------------------------------------------------
-// One cooperative launch for a LIST of words: gather-mean of the word's rows of the global map (heatmap.py:121-123) ->
-// bicubic to (out_h, out_w) -> min / max over the image -> normalise / threshold (heatmap.py:77-93). CTA = (word, chunk
-// of output pixels). The word map lives in shared memory; the min/max pass and the write pass both interpolate from it
-// (16 shared loads + 20 FMAs per pixel), so nothing but the final image is written and nothing is read back: per-chunk
+// One cooperative launch for a LIST of words: gather-mean of the word's rows of the [mh][mw] global map
+// (heatmap.py:121-123) -> bicubic to (out_h, out_w), taps mh -> out_h and mw -> out_w -> min / max over the image ->
+// normalise / threshold (heatmap.py:77-93). CTA = (word, chunk of output pixels). The word map lives in shared memory;
+// the min/max pass and the write pass both interpolate from it (16 shared loads + 20 FMAs per pixel), so nothing but
+// the final image is written and nothing is read back: per-chunk
 // partial min/max go through `scratch`, one grid-wide barrier separates the passes. With `absolute` there is no
 // min/max pass and no barrier. Deterministic (no atomics).
 constexpr int kMaxWords = 96;
@@ -423,11 +449,11 @@ constexpr int kMaxWordRows = 320;       // selected rows over all words of a lau
 constexpr int kMaxChunks = 32;          // CTAs per word; scratch holds 2 floats per (word, chunk)
 
 struct ExpandWordsParams {
-  const float* maps;                    // [n_map_rows][x][x]
-  float* word_maps;                     // optional [n_words][x][x]
+  const float* maps;                    // [n_map_rows][mh][mw]
+  float* word_maps;                     // optional [n_words][mh][mw]
   float* out;                           // [n_words][oh][ow]
   float* scratch;                       // [n_words][chunks][2]
-  int x, oh, ow, n_words, chunks, absolute, use_threshold;
+  int mh, mw, oh, ow, n_words, chunks, absolute, use_threshold;
   float threshold;
   int row_begin[kMaxWords + 1];
   int rows[kMaxWordRows];
@@ -447,10 +473,10 @@ __device__ __forceinline__ float bicubic_shared(const float* sm, int w, const Ta
 }
 
 __global__ void __launch_bounds__(256) expand_words_kernel(const __grid_constant__ ExpandWordsParams P) {
-  extern __shared__ __align__(16) float wm[];          // the word map [x][x]
+  extern __shared__ __align__(16) float wm[];          // the word map [mh][mw]
   __shared__ float red_lo[8], red_hi[8];
   const int word = blockIdx.x / P.chunks, chunk = blockIdx.x - word * P.chunks;
-  const int x = P.x, xx = x * x, n = P.oh * P.ow;
+  const int mh = P.mh, mw = P.mw, xx = mh * mw, n = P.oh * P.ow;
   const int r0 = P.row_begin[word], r1 = P.row_begin[word + 1];
   for (int i = threadIdx.x; i < xx; i += blockDim.x) {
     float s = 0.f;
@@ -467,7 +493,7 @@ __global__ void __launch_bounds__(256) expand_words_kernel(const __grid_constant
     lo = INFINITY; hi = -INFINITY;
     for (int o = begin + threadIdx.x; o < end; o += blockDim.x) {
       const int oy = o / P.ow, ox = o - oy * P.ow;
-      const float v = bicubic_shared(wm, x, make_taps(oy, x, P.oh), make_taps(ox, x, P.ow));
+      const float v = bicubic_shared(wm, mw, make_taps(oy, mh, P.oh), make_taps(ox, mw, P.ow));
       lo = fminf(lo, v); hi = fmaxf(hi, v);
     }
 #pragma unroll
@@ -496,7 +522,7 @@ __global__ void __launch_bounds__(256) expand_words_kernel(const __grid_constant
   float* dst = P.out + (long long)word * n;
   for (int o = begin + threadIdx.x; o < end; o += blockDim.x) {
     const int oy = o / P.ow, ox = o - oy * P.ow;
-    float v = bicubic_shared(wm, x, make_taps(oy, x, P.oh), make_taps(ox, x, P.ow));
+    float v = bicubic_shared(wm, mw, make_taps(oy, mh, P.oh), make_taps(ox, mw, P.ow));
     if (!P.absolute) v = (v - lo) / (hi - lo + 1e-8f);
     if (P.use_threshold) v = v > P.threshold ? 1.f : 0.f;
     dst[o] = v;
@@ -514,59 +540,62 @@ static bool force_generic_finalize() {
   return e && e[0] == '1';
 }
 
-extern "C" int daam_finalize(const daam_key_group* groups, int32_t n_groups, int32_t x, int32_t n_rows,
-                             int32_t normalize, float* out, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!groups || !out || x <= 0 || n_rows <= 0) { set_error("daam_finalize: null pointer or non-positive size"); return DAAM_E_INVALID; }
-  if (n_groups <= 0) { set_error("daam_finalize: no key selected"); return DAAM_E_INVALID; }
-  if (n_groups > kMaxGroups) { set_error("daam_finalize: %d key groups > %d", n_groups, kMaxGroups); return DAAM_E_UNSUPPORTED; }
+// One implementation behind each square / rectangular pair of entry points: the square entry point is the (x, x) case
+// and reports errors under its own name.
+static int finalize_impl(const char* name, const daam_key_group* groups, int32_t n_groups, int32_t oh, int32_t ow,
+                         int32_t n_rows, int32_t normalize, float* out, cudaStream_t stream) {
+  if (!groups || !out || oh <= 0 || ow <= 0 || n_rows <= 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
+  if (n_groups <= 0) { set_error("%s: no key selected", name); return DAAM_E_INVALID; }
+  if (n_groups > kMaxGroups) { set_error("%s: %d key groups > %d", name, n_groups, kMaxGroups); return DAAM_E_UNSUPPORTED; }
   DeviceInfo dev;
   if (int rc = get_device_info(&dev)) return rc;
   FinalizeParams p;
-  p.n_groups = n_groups; p.x = x; p.n_rows = n_rows; p.n_keys = 0;
+  p.n_groups = n_groups; p.oh = oh; p.ow = ow; p.n_rows = n_rows; p.n_keys = 0;
   for (int i = 0; i < n_groups; ++i) {
     const daam_key_group& g = groups[i];
     if (!g.acc || g.heads <= 0 || g.h <= 0 || g.w <= 0 || g.tokens < n_rows || g.head_sel >= g.heads) {
-      set_error("daam_finalize: bad key group %d (heads %d, h %d, w %d, tokens %d, head_sel %d, n_rows %d)", i, g.heads,
+      set_error("%s: bad key group %d (heads %d, h %d, w %d, tokens %d, head_sel %d, n_rows %d)", name, i, g.heads,
                 g.h, g.w, g.tokens, g.head_sel, n_rows);
       return DAAM_E_INVALID;
     }
     p.g[i] = g;
     p.n_keys += g.head_sel < 0 ? g.heads : 1;
   }
-  const int xx = x * x;
-  // fast path: every key is square with an integer factor 1 / 2 / 4 (all SD / SDXL layers that are ever traced) and
-  // 16-byte-aligned rows (cp.async / float4)
+  const int xx = oh * ow;
+  // fast path: every key has one integer factor F = 1 / 2 / 4 on both axes (all SD / SDXL layers that are ever traced)
+  // and 16-byte-aligned key bases (cp.async / float4: an aligned slab and h * w a multiple of 4). A square map keeps
+  // the rule it always had (side a multiple of 16), so its kernel choice and bits do not move.
   ClassList cls;
   cls.n = 0;
-  bool fast = x % 16 == 0 && x <= 256 && p.n_keys <= kMaxClassKeys && !force_generic_finalize();
+  bool fast = (oh != ow || oh % 16 == 0) && ow <= 256 && p.n_keys <= kMaxClassKeys && !force_generic_finalize();
   for (int i = 0; i < n_groups && fast; ++i) {
     const daam_key_group& g = groups[i];
-    if (g.h != g.w || x % g.h != 0 || (x / g.h != 1 && x / g.h != 2 && x / g.h != 4) ||
-        reinterpret_cast<uintptr_t>(g.acc) % 16 != 0) { fast = false; break; }
+    const int f = oh / g.h;
+    if (oh % g.h != 0 || ow % g.w != 0 || ow / g.w != f || (f != 1 && f != 2 && f != 4) ||
+        reinterpret_cast<uintptr_t>(g.acc) % 16 != 0 || (g.h * g.w) % 4 != 0) { fast = false; break; }
     bool seen = false;
-    for (int c = 0; c < cls.n; ++c) seen = seen || cls.side[c] == g.h;
+    for (int c = 0; c < cls.n; ++c) seen = seen || (cls.kh[c] == g.h && cls.kw[c] == g.w);
     if (!seen) {
       if (cls.n == 8) { fast = false; break; }
-      cls.side[cls.n++] = g.h;
+      cls.kh[cls.n] = g.h; cls.kw[cls.n] = g.w; ++cls.n;
     }
   }
   if (fast) {
     // 8-row bands unless that leaves the machine under-filled (< 2 CTAs per SM) or a band's source pixels of the
-    // factor-2 class would exceed one CTA's 256 threads (x > 128); forcing either height measured the same within 1 %
+    // factor-2 class would exceed one CTA's 256 threads (ow > 128); forcing either height measured the same within 1 %
     // for the 175-key SD-2.1 case
-    cls.band_rows = ((x / 8) * n_rows >= 2 * dev.sm_count && x <= 128) ? 8 : 4;
+    cls.band_rows = (((oh + 7) / 8) * n_rows >= 2 * dev.sm_count && ow <= 128) ? 8 : 4;
     int next = 0;
     for (int c = 0; c < cls.n; ++c) {                   // keys[] of the kernel: class by class, groups in call order
       cls.key_begin[c] = next;
       for (int i = 0; i < n_groups; ++i)
-        if (groups[i].h == cls.side[c]) {
+        if (groups[i].h == cls.kh[c] && groups[i].w == cls.kw[c]) {
           cls.key_slot[i] = next;
           next += groups[i].head_sel < 0 ? groups[i].heads : 1;
         }
     }
     cls.key_begin[cls.n] = next;
-    const size_t smem = (2 * kStageFloats + (size_t)cls.band_rows * x) * sizeof(float);
+    const size_t smem = (2 * kStageFloats + (size_t)cls.band_rows * ow) * sizeof(float);
     static std::once_flag attr_once[64];
     cudaError_t attr_err = cudaSuccess;
     std::call_once(attr_once[dev.device & 63], [&] {
@@ -574,7 +603,8 @@ extern "C" int daam_finalize(const daam_key_group* groups, int32_t n_groups, int
                                       (int)((2 * kStageFloats + 8 * 256) * sizeof(float)));
     });
     DAAM_CUDA_TRY(attr_err);
-    finalize_fast_kernel<<<dim3(x / cls.band_rows, n_rows), 256, smem, stream>>>(p, cls, out);
+    const int bands = (oh + cls.band_rows - 1) / cls.band_rows;
+    finalize_fast_kernel<<<dim3(bands, n_rows), 256, smem, stream>>>(p, cls, out);
   } else {
     dim3 grid((xx + 255) / 256, n_rows);
     finalize_kernel<<<grid, 256, 0, stream>>>(p, out);
@@ -589,20 +619,31 @@ extern "C" int daam_finalize(const daam_key_group* groups, int32_t n_groups, int
   return DAAM_OK;
 }
 
-extern "C" int daam_finalize_per_key(const daam_key_group* groups, int32_t n_groups, int32_t x, int32_t n_rows,
-                                     int32_t normalize, float* out, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!groups || !out || x <= 0 || n_rows <= 0) { set_error("daam_finalize_per_key: null pointer or non-positive size"); return DAAM_E_INVALID; }
-  if (n_groups <= 0) { set_error("daam_finalize_per_key: no key selected"); return DAAM_E_INVALID; }
-  if (n_groups > kMaxGroups) { set_error("daam_finalize_per_key: %d key groups > %d", n_groups, kMaxGroups); return DAAM_E_UNSUPPORTED; }
+extern "C" int daam_finalize(const daam_key_group* groups, int32_t n_groups, int32_t x, int32_t n_rows,
+                             int32_t normalize, float* out, void* stream_) {
+  return finalize_impl("daam_finalize", groups, n_groups, x, x, n_rows, normalize, out,
+                       static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int daam_finalize_rect(const daam_key_group* groups, int32_t n_groups, int32_t map_h, int32_t map_w,
+                                  int32_t n_rows, int32_t normalize, float* out, void* stream_) {
+  return finalize_impl("daam_finalize_rect", groups, n_groups, map_h, map_w, n_rows, normalize, out,
+                       static_cast<cudaStream_t>(stream_));
+}
+
+static int finalize_per_key_impl(const char* name, const daam_key_group* groups, int32_t n_groups, int32_t oh, int32_t ow,
+                                 int32_t n_rows, int32_t normalize, float* out, cudaStream_t stream) {
+  if (!groups || !out || oh <= 0 || ow <= 0 || n_rows <= 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
+  if (n_groups <= 0) { set_error("%s: no key selected", name); return DAAM_E_INVALID; }
+  if (n_groups > kMaxGroups) { set_error("%s: %d key groups > %d", name, n_groups, kMaxGroups); return DAAM_E_UNSUPPORTED; }
   DeviceInfo dev;
   if (int rc = get_device_info(&dev)) return rc;
   static thread_local PerKeyParams p;
-  p.n_groups = n_groups; p.x = x; p.n_rows = n_rows; p.n_keys = 0;
+  p.n_groups = n_groups; p.oh = oh; p.ow = ow; p.n_rows = n_rows; p.n_keys = 0;
   for (int i = 0; i < n_groups; ++i) {
     const daam_key_group& g = groups[i];
     if (!g.acc || g.heads <= 0 || g.h <= 0 || g.w <= 0 || g.tokens < n_rows || g.head_sel >= g.heads) {
-      set_error("daam_finalize_per_key: bad key group %d", i);
+      set_error("%s: bad key group %d", name, i);
       return DAAM_E_INVALID;
     }
     p.g[i] = g;
@@ -610,13 +651,13 @@ extern "C" int daam_finalize_per_key(const daam_key_group* groups, int32_t n_gro
     p.n_keys += g.head_sel < 0 ? g.heads : 1;
   }
   p.first_key[n_groups] = p.n_keys;
-  if (p.n_keys > 65535) { set_error("daam_finalize_per_key: %d keys > 65535", p.n_keys); return DAAM_E_UNSUPPORTED; }
-  const int xx = x * x;
+  if (p.n_keys > 65535) { set_error("%s: %d keys > 65535", name, p.n_keys); return DAAM_E_UNSUPPORTED; }
+  const int xx = oh * ow;
   dim3 grid((xx + 255) / 256, n_rows, p.n_keys);
   finalize_per_key_kernel<<<grid, 256, 0, stream>>>(p, out);
   DAAM_CUDA_TRY(cudaGetLastError());
   count_launch();
-  if (normalize) {   // every key's map is an independent [n_rows, x, x] block
+  if (normalize) {   // every key's map is an independent [n_rows, oh, ow] block
     normalize_kernel<<<dim3((xx + 255) / 256, p.n_keys), 256, 0, stream>>>(out, n_rows, xx);
     DAAM_CUDA_TRY(cudaGetLastError());
     count_launch();
@@ -624,25 +665,46 @@ extern "C" int daam_finalize_per_key(const daam_key_group* groups, int32_t n_gro
   return DAAM_OK;
 }
 
-extern "C" int daam_normalize_maps(float* maps, int32_t n_maps, int32_t n_rows, int32_t x, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!maps || n_maps < 0 || n_rows <= 0 || x <= 0) { set_error("daam_normalize_maps: null pointer or bad size"); return DAAM_E_INVALID; }
-  if (n_maps > 65535) { set_error("daam_normalize_maps: %d maps > 65535", n_maps); return DAAM_E_UNSUPPORTED; }
+extern "C" int daam_finalize_per_key(const daam_key_group* groups, int32_t n_groups, int32_t x, int32_t n_rows,
+                                     int32_t normalize, float* out, void* stream_) {
+  return finalize_per_key_impl("daam_finalize_per_key", groups, n_groups, x, x, n_rows, normalize, out,
+                               static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int daam_finalize_per_key_rect(const daam_key_group* groups, int32_t n_groups, int32_t map_h, int32_t map_w,
+                                          int32_t n_rows, int32_t normalize, float* out, void* stream_) {
+  return finalize_per_key_impl("daam_finalize_per_key_rect", groups, n_groups, map_h, map_w, n_rows, normalize, out,
+                               static_cast<cudaStream_t>(stream_));
+}
+
+static int normalize_maps_impl(const char* name, float* maps, int32_t n_maps, int32_t n_rows, int32_t mh, int32_t mw,
+                               cudaStream_t stream) {
+  if (!maps || n_maps < 0 || n_rows <= 0 || mh <= 0 || mw <= 0) { set_error("%s: null pointer or bad size", name); return DAAM_E_INVALID; }
+  if (n_maps > 65535) { set_error("%s: %d maps > 65535", name, n_maps); return DAAM_E_UNSUPPORTED; }
   if (n_maps == 0) return DAAM_OK;
   DeviceInfo dev;
   if (int rc = get_device_info(&dev)) return rc;
-  const int xx = x * x;
+  const int xx = mh * mw;
   normalize_kernel<<<dim3((xx + 255) / 256, n_maps), 256, 0, stream>>>(maps, n_rows, xx);
   DAAM_CUDA_TRY(cudaGetLastError());
   count_launch();
   return DAAM_OK;
 }
 
-extern "C" int daam_word_heat_map(const float* global_maps, int32_t n_rows, int32_t x, const int32_t* rows,
-                                  int32_t n_sel, float* out, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!global_maps || !rows || !out || x <= 0 || n_sel <= 0) { set_error("daam_word_heat_map: null pointer or empty selection"); return DAAM_E_INVALID; }
-  if (n_sel > kMaxRows) { set_error("daam_word_heat_map: %d rows > %d", n_sel, kMaxRows); return DAAM_E_UNSUPPORTED; }
+extern "C" int daam_normalize_maps(float* maps, int32_t n_maps, int32_t n_rows, int32_t x, void* stream_) {
+  return normalize_maps_impl("daam_normalize_maps", maps, n_maps, n_rows, x, x, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int daam_normalize_maps_rect(float* maps, int32_t n_maps, int32_t n_rows, int32_t map_h, int32_t map_w,
+                                        void* stream_) {
+  return normalize_maps_impl("daam_normalize_maps_rect", maps, n_maps, n_rows, map_h, map_w,
+                             static_cast<cudaStream_t>(stream_));
+}
+
+static int word_heat_map_impl(const char* name, const float* global_maps, int32_t n_rows, int32_t mh, int32_t mw,
+                              const int32_t* rows, int32_t n_sel, float* out, cudaStream_t stream) {
+  if (!global_maps || !rows || !out || mh <= 0 || mw <= 0 || n_sel <= 0) { set_error("%s: null pointer or empty selection", name); return DAAM_E_INVALID; }
+  if (n_sel > kMaxRows) { set_error("%s: %d rows > %d", name, n_sel, kMaxRows); return DAAM_E_UNSUPPORTED; }
   DeviceInfo dev;
   if (int rc = get_device_info(&dev)) return rc;
   RowSel sel;
@@ -650,18 +712,30 @@ extern "C" int daam_word_heat_map(const float* global_maps, int32_t n_rows, int3
   for (int i = 0; i < n_sel; ++i) {
     int r = rows[i];
     if (r < 0) r += n_rows;   // torch-style negative index
-    if (r < 0 || r >= n_rows) { set_error("daam_word_heat_map: row %d out of range [0, %d)", rows[i], n_rows); return DAAM_E_INVALID; }
+    if (r < 0 || r >= n_rows) { set_error("%s: row %d out of range [0, %d)", name, rows[i], n_rows); return DAAM_E_INVALID; }
     sel.rows[i] = r;
   }
-  const int xx = x * x;
+  const int xx = mh * mw;
   word_map_kernel<<<(xx + 255) / 256, 256, 0, stream>>>(global_maps, sel, xx, out);
   DAAM_CUDA_TRY(cudaGetLastError());
   count_launch();
   return DAAM_OK;
 }
 
+extern "C" int daam_word_heat_map(const float* global_maps, int32_t n_rows, int32_t x, const int32_t* rows,
+                                  int32_t n_sel, float* out, void* stream_) {
+  return word_heat_map_impl("daam_word_heat_map", global_maps, n_rows, x, x, rows, n_sel, out,
+                            static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int daam_word_heat_map_rect(const float* global_maps, int32_t n_rows, int32_t map_h, int32_t map_w,
+                                       const int32_t* rows, int32_t n_sel, float* out, void* stream_) {
+  return word_heat_map_impl("daam_word_heat_map_rect", global_maps, n_rows, map_h, map_w, rows, n_sel, out,
+                            static_cast<cudaStream_t>(stream_));
+}
+
 static int launch_expand_words(ExpandWordsParams& p, const DeviceInfo& dev, cudaStream_t stream) {
-  const size_t smem = (size_t)p.x * p.x * sizeof(float);
+  const size_t smem = (size_t)p.mh * p.mw * sizeof(float);
   static std::mutex mu;
   static size_t configured_dev[64] = {};
   static int blocks_per_sm[64] = {};
@@ -696,7 +770,7 @@ static int launch_expand_words(ExpandWordsParams& p, const DeviceInfo& dev, cuda
     q.n_words = batch;
     q.chunks = chunks;
     q.out = p.out + (long long)done * n;
-    q.word_maps = p.word_maps ? p.word_maps + (long long)done * p.x * p.x : nullptr;
+    q.word_maps = p.word_maps ? p.word_maps + (long long)done * p.mh * p.mw : nullptr;
     q.scratch = p.scratch + 2LL * kMaxChunks * done;
     for (int i = 0; i <= batch; ++i) q.row_begin[i] = p.row_begin[done + i];
     void* args[] = {&q};
@@ -708,41 +782,76 @@ static int launch_expand_words(ExpandWordsParams& p, const DeviceInfo& dev, cuda
   return DAAM_OK;
 }
 
-extern "C" int daam_expand_words(const float* global_maps, int32_t n_rows, int32_t x, const int32_t* rows,
-                                 const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w,
-                                 int32_t absolute, int32_t use_threshold, float threshold, float* word_maps, float* out,
-                                 float* scratch, void* stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  if (!global_maps || !rows || !row_begin || !out || !scratch || x <= 0 || out_h <= 0 || out_w <= 0 || n_rows <= 0) { set_error("daam_expand_words: null pointer or non-positive size"); return DAAM_E_INVALID; }
-  if (n_words <= 0) { set_error("daam_expand_words: empty word list"); return DAAM_E_INVALID; }
-  if (n_words > kMaxWords) { set_error("daam_expand_words: %d words > %d", n_words, kMaxWords); return DAAM_E_UNSUPPORTED; }
-  if (row_begin[0] != 0 || row_begin[n_words] > kMaxWordRows) { set_error("daam_expand_words: row_begin must start at 0 and select at most %d rows", kMaxWordRows); return DAAM_E_UNSUPPORTED; }
-  if ((size_t)x * x * sizeof(float) > 200 * 1024) { set_error("daam_expand_words: x = %d does not fit shared memory", x); return DAAM_E_UNSUPPORTED; }
+static int expand_words_impl(const char* name, const float* global_maps, int32_t n_rows, int32_t mh, int32_t mw,
+                             const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w,
+                             int32_t absolute, int32_t use_threshold, float threshold, float* word_maps, float* out,
+                             float* scratch, cudaStream_t stream) {
+  if (!global_maps || !rows || !row_begin || !out || !scratch || mh <= 0 || mw <= 0 || out_h <= 0 || out_w <= 0 || n_rows <= 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
+  if (n_words <= 0) { set_error("%s: empty word list", name); return DAAM_E_INVALID; }
+  if (n_words > kMaxWords) { set_error("%s: %d words > %d", name, n_words, kMaxWords); return DAAM_E_UNSUPPORTED; }
+  if (row_begin[0] != 0 || row_begin[n_words] > kMaxWordRows) { set_error("%s: row_begin must start at 0 and select at most %d rows", name, kMaxWordRows); return DAAM_E_UNSUPPORTED; }
+  if ((size_t)mh * mw * sizeof(float) > 200 * 1024) {
+    if (mh == mw) set_error("%s: x = %d does not fit shared memory", name, mh);
+    else set_error("%s: a %d x %d map does not fit shared memory", name, mh, mw);
+    return DAAM_E_UNSUPPORTED;
+  }
   DeviceInfo dev;
   if (int rc = get_device_info(&dev)) return rc;
   static thread_local ExpandWordsParams p;
   p.maps = global_maps; p.word_maps = word_maps; p.out = out; p.scratch = scratch;
-  p.x = x; p.oh = out_h; p.ow = out_w; p.n_words = n_words; p.chunks = 1;
+  p.mh = mh; p.mw = mw; p.oh = out_h; p.ow = out_w; p.n_words = n_words; p.chunks = 1;
   p.absolute = absolute ? 1 : 0; p.use_threshold = use_threshold ? 1 : 0; p.threshold = threshold;
   for (int w = 0; w < n_words; ++w) {
-    if (row_begin[w + 1] <= row_begin[w]) { set_error("daam_expand_words: word %d selects no row", w); return DAAM_E_INVALID; }
+    if (row_begin[w + 1] <= row_begin[w]) { set_error("%s: word %d selects no row", name, w); return DAAM_E_INVALID; }
     p.row_begin[w] = row_begin[w];
   }
   p.row_begin[n_words] = row_begin[n_words];
   for (int i = 0; i < row_begin[n_words]; ++i) {
     int r = rows[i];
     if (r < 0) r += n_rows;   // torch-style negative index
-    if (r < 0 || r >= n_rows) { set_error("daam_expand_words: row %d out of range [0, %d)", rows[i], n_rows); return DAAM_E_INVALID; }
+    if (r < 0 || r >= n_rows) { set_error("%s: row %d out of range [0, %d)", name, rows[i], n_rows); return DAAM_E_INVALID; }
     p.rows[i] = r;
   }
   return launch_expand_words(p, dev, stream);
 }
 
+extern "C" int daam_expand_words(const float* global_maps, int32_t n_rows, int32_t x, const int32_t* rows,
+                                 const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w,
+                                 int32_t absolute, int32_t use_threshold, float threshold, float* word_maps, float* out,
+                                 float* scratch, void* stream_) {
+  return expand_words_impl("daam_expand_words", global_maps, n_rows, x, x, rows, row_begin, n_words, out_h, out_w,
+                           absolute, use_threshold, threshold, word_maps, out, scratch, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int daam_expand_words_rect(const float* global_maps, int32_t n_rows, int32_t map_h, int32_t map_w,
+                                      const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h,
+                                      int32_t out_w, int32_t absolute, int32_t use_threshold, float threshold,
+                                      float* word_maps, float* out, float* scratch, void* stream_) {
+  return expand_words_impl("daam_expand_words_rect", global_maps, n_rows, map_h, map_w, rows, row_begin, n_words, out_h,
+                           out_w, absolute, use_threshold, threshold, word_maps, out, scratch,
+                           static_cast<cudaStream_t>(stream_));
+}
+
+// one word whose "rows" are the word map itself; `self` names the entry point in the null-pointer message, `inner` in
+// the checks shared with expand_words (the square pair has always reported those as daam_expand_words)
+static int expand_as_impl(const char* self, const char* inner, const float* word_map, int32_t mh, int32_t mw,
+                          int32_t out_h, int32_t out_w, int32_t absolute, int32_t use_threshold, float threshold,
+                          float* out, float* scratch, void* stream_) {
+  const int32_t rows[1] = {0}, row_begin[2] = {0, 1};
+  if (!word_map) { set_error("%s: null pointer or non-positive size", self); return DAAM_E_INVALID; }
+  return expand_words_impl(inner, word_map, 1, mh, mw, rows, row_begin, 1, out_h, out_w, absolute, use_threshold,
+                           threshold, nullptr, out, scratch, static_cast<cudaStream_t>(stream_));
+}
+
 extern "C" int daam_expand_as(const float* word_map, int32_t x, int32_t out_h, int32_t out_w, int32_t absolute,
                               int32_t use_threshold, float threshold, float* out, float* scratch, void* stream_) {
-  // one word whose "rows" are the word map itself
-  const int32_t rows[1] = {0}, row_begin[2] = {0, 1};
-  if (!word_map) { set_error("daam_expand_as: null pointer or non-positive size"); return DAAM_E_INVALID; }
-  return daam_expand_words(word_map, 1, x, rows, row_begin, 1, out_h, out_w, absolute, use_threshold, threshold, nullptr,
-                           out, scratch, stream_);
+  return expand_as_impl("daam_expand_as", "daam_expand_words", word_map, x, x, out_h, out_w, absolute, use_threshold,
+                        threshold, out, scratch, stream_);
+}
+
+extern "C" int daam_expand_as_rect(const float* word_map, int32_t map_h, int32_t map_w, int32_t out_h, int32_t out_w,
+                                   int32_t absolute, int32_t use_threshold, float threshold, float* out, float* scratch,
+                                   void* stream_) {
+  return expand_as_impl("daam_expand_as_rect", "daam_expand_as_rect", word_map, map_h, map_w, out_h, out_w, absolute,
+                        use_threshold, threshold, out, scratch, stream_);
 }

@@ -15,18 +15,17 @@ __all__ = ['compute_iou', 'compute_ioa']
 
 
 def _match_size(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
-    """evaluate.py:15-18 / 27-30: bicubic resize of ``a`` to ``b``'s shape, then ``a < 1 -> 0``, ``a >= 1 -> 1``."""
+    """evaluate.py:15-18 / 27-30: bicubic resize of ``a`` to ``b``'s shape, then ``a < 1 -> 0``, ``a >= 1 -> 1``.
+    Like the reference, only ``shape[0]`` decides whether to resize; ``a`` may be rectangular."""
     if a.shape[0] == b.shape[0]:
         return a
     if not a.is_cuda:
         raise RuntimeError('compute_iou/compute_ioa resize on CUDA tensors only (there is no CPU fallback)')
-    if a.shape[0] != a.shape[1]:
-        raise ValueError('the native resize takes square source maps')
     src = a.detach().float().contiguous()
     out = torch.empty(tuple(b.shape), dtype=torch.float32, device=a.device)
     scratch = torch.empty(2, dtype=torch.float32, device=a.device)
     with torch.cuda.device(a.device):
-        _native.expand_as(src.data_ptr(), src.shape[0], b.shape[0], b.shape[1], True, None, out.data_ptr(),
+        _native.expand_as(src.data_ptr(), tuple(src.shape), b.shape[0], b.shape[1], True, None, out.data_ptr(),
                           scratch.data_ptr(), torch.cuda.current_stream(a.device).cuda_stream)
     return (out >= 1).float()
 

@@ -1,0 +1,65 @@
+"""The heat-map geometry of one latent size: the grid the global heat maps live on, and each traced layer's key size
+``(h, w)`` and spatial factor. The tracer asks this one object for all of them.
+
+* Square latent (``H == W``, and before the first UNet forward): the reference's rule, bit for bit -- the grid is
+  ``sqrt(latent_hw)`` on both axes, a layer of ``n`` query positions has keys ``sqrt(n)`` on both axes and factor
+  ``int(sqrt(latent_hw // n))`` (daam/trace.py:32-33, 285-289), including its quirks at square sizes other than the
+  model's own (SD-2.1-base at 768 pixels: factor 0).
+* Non-square latent: with ``g = unet.config.sample_size / sqrt(latent_hw)`` (1 for SD-1.x / SD-2.x, 2 for SDXL) the grid
+  is ``(ceil(H / g), ceil(W / g))``; a layer with ``n`` query positions sits at the level ``s`` where
+  ``ceil(H / 2^s) * ceil(W / 2^s) == n`` (diffusers' stride-2 convolutions; the up path resizes to the skip's size), its
+  keys are ``[ceil(H / 2^s), ceil(W / 2^s)]`` in row-major pixel order and its factor is ``2^s // g``.
+"""
+from __future__ import annotations
+
+import math
+from typing import Optional, Tuple
+
+__all__ = ['LatentGeometry']
+
+
+class LatentGeometry:
+    """``latent_hw``: the tracer's ``latent_hw`` (4096 or 9216); ``sample_size``: ``unet.config.sample_size``;
+    ``latent_shape``: ``(H, W)`` of the sample the UNet receives, ``None`` while unknown (treated as square)."""
+
+    def __init__(self, latent_hw: int, sample_size: int, latent_shape: Optional[Tuple[int, int]] = None):
+        self.latent_hw = latent_hw
+        self.latent_shape = None if latent_shape is None else (int(latent_shape[0]), int(latent_shape[1]))
+        self.square = self.latent_shape is None or self.latent_shape[0] == self.latent_shape[1]
+        if self.square:
+            x = int(math.sqrt(latent_hw))
+            self.g = None
+            self.grid: Tuple[int, int] = (x, x)
+        else:
+            H, W = self.latent_shape
+            g = sample_size / math.sqrt(latent_hw)
+            if g not in (1, 2):
+                raise ValueError(f'heat maps of a non-square {H}x{W} latent need unet.config.sample_size / '
+                                 f'sqrt(latent_hw) = 1 (SD-1.x, SD-2.x) or 2 (SDXL); this UNet has {sample_size} / '
+                                 f'{int(math.sqrt(latent_hw))} = {g:g}')
+            self.g = int(g)
+            self.grid = (-(-H // self.g), -(-W // self.g))
+
+    @property
+    def key(self):
+        """What the layer rule depends on: equal keys give equal ``(h, w, factor)`` for every ``n``."""
+        return None if self.square else self.latent_shape
+
+    def level(self, n: int, layer_idx: int = 0) -> Tuple[Optional[int], Optional[int], int]:
+        """``(h, w, factor)`` of a layer with ``n`` query positions. Square rule: ``h = w = None`` when ``n`` is not a
+        perfect square (the caller raises if it needs them). Non-square rule: raises ``RuntimeError`` when no level
+        matches."""
+        if self.square:
+            side = int(math.sqrt(n))
+            factor = int(math.sqrt(self.latent_hw // n))
+            return (side, side, factor) if side * side == n else (None, None, factor)
+        H, W = self.latent_shape
+        s = 0
+        while True:
+            h, w = -(-H // (1 << s)), -(-W // (1 << s))
+            if h * w == n:
+                return h, w, (1 << s) // self.g
+            if h * w < n or (h == 1 and w == 1):
+                raise RuntimeError(f'layer {layer_idx}: {n} query positions match no level of the {H}x{W} latent '
+                                   f'(ceil(H / 2^s) * ceil(W / 2^s) for s = 0, 1, ...)')
+            s += 1

@@ -37,6 +37,17 @@ def _require_cuda(t: torch.Tensor, what: str):
         raise RuntimeError(f'{what}: daam_b200 computes on CUDA tensors only (there is no CPU fallback)')
 
 
+def _image_size(image, map_h: int, map_w: int) -> Tuple[int, int]:
+    """``(out_h, out_w)`` a ``[map_h, map_w]`` map expands to over ``image``. A square map keeps the reference's
+    ``size=(image.size[0], image.size[1])`` (heatmap.py:80; the same thing for the square images such maps come from);
+    a non-square map comes from a non-square image and expands to ``(image.height, image.width)``."""
+    if map_h == map_w:
+        return int(image.size[0]), int(image.size[1])
+    if hasattr(image, 'height') and hasattr(image, 'width'):
+        return int(image.height), int(image.width)
+    return int(image.size[1]), int(image.size[0])      # PIL-like ``size = (width, height)``
+
+
 @dataclass
 class LayerSlab:
     """Accumulators of one traced layer: ``acc[prompt][head]`` is the reference's ``[77, h, w]`` map of key
@@ -114,6 +125,8 @@ class RawHeatMapCollection:
             slab = LayerSlab(layer_idx, factor, heads, h, w, acc, head_offset=head_offset, step=step, ranges=ranges)
             self.slabs[layer_idx] = slab
             self.epoch += 1
+        elif (slab.h, slab.w) != (h, w):      # same pixel count, other key shape (a transposed latent): re-tag
+            slab.h, slab.w = h, w
         if not slab.touched:
             slab.touched = True
             self._order.append(layer_idx)
@@ -218,14 +231,16 @@ class WordHeatMap:
     def expand_as(self, image, absolute: bool = False, threshold: Optional[float] = None, plot: bool = False,
                   **plot_kwargs) -> torch.Tensor:
         """Bicubic-upsample to the image size, min-max normalise unless ``absolute``, optionally binarise; returns a
-        CPU tensor like heatmap.py:77-93 (including its ``size=(image.size[0], image.size[1])`` axis order)."""
+        CPU tensor like heatmap.py:77-93 (a square map keeps its ``size=(image.size[0], image.size[1])`` axis order; a
+        non-square ``[h, w]`` map expands to ``[image.height, image.width]``)."""
         _require_cuda(self.heatmap, 'WordHeatMap.expand_as')
         src = self.heatmap.detach().float().contiguous()
-        out_h, out_w = int(image.size[0]), int(image.size[1])
+        grid = tuple(src.shape[-2:])
+        out_h, out_w = _image_size(image, *grid)
         out = torch.empty((out_h, out_w), dtype=torch.float32, device=src.device)
         scratch = torch.empty(_native.EXPAND_SCRATCH_FLOATS, dtype=torch.float32, device=src.device)
         with torch.cuda.device(src.device):
-            _native.expand_as(src.data_ptr(), src.shape[-1], out_h, out_w, absolute, threshold, out.data_ptr(),
+            _native.expand_as(src.data_ptr(), grid, out_h, out_w, absolute, threshold, out.data_ptr(),
                               scratch.data_ptr(), _stream_ptr(src.device))
         im = out.cpu()          # the reference returns a CPU tensor (heatmap.py:93); GlobalHeatMap.expand_words defers this
         if plot:
@@ -260,7 +275,8 @@ class WordHeatMap:
 
 
 class GlobalHeatMap:
-    """``[n_prompt_tokens + 2, x, x]`` per-token maps plus the word lookup (heatmap.py:114-123)."""
+    """``[n_prompt_tokens + 2, xh, xw]`` per-token maps plus the word lookup (heatmap.py:114-123); ``xh == xw`` for
+    square images."""
 
     def __init__(self, tokenizer, prompt: str, heat_maps: torch.Tensor):
         self.tokenizer = tokenizer
@@ -272,14 +288,14 @@ class GlobalHeatMap:
         rows, word_idx = compute_token_merge_indices(self.tokenizer, self.prompt, word, word_idx, offset_idx)
         maps = self.heat_maps
         _require_cuda(maps, 'GlobalHeatMap.compute_word_heat_map')
-        n_rows, x = maps.shape[0], maps.shape[-1]
+        n_rows, grid = maps.shape[0], tuple(maps.shape[-2:])
         for r in rows:  # torch's advanced indexing raises IndexError on out-of-range rows
             if not -n_rows <= r < n_rows:
                 raise IndexError(f'index {r} is out of bounds for dimension 0 with size {n_rows}')
         maps = maps.detach().float().contiguous()
-        out = torch.empty((x, x), dtype=torch.float32, device=maps.device)
+        out = torch.empty(grid, dtype=torch.float32, device=maps.device)
         with torch.cuda.device(maps.device):
-            _native.word_heat_map(maps.data_ptr(), n_rows, x, rows, out.data_ptr(), _stream_ptr(maps.device))
+            _native.word_heat_map(maps.data_ptr(), n_rows, grid, rows, out.data_ptr(), _stream_ptr(maps.device))
         return WordHeatMap(out, word, word_idx)
 
     def expand_words(self, words, image, absolute: bool = False, threshold: Optional[float] = None,
@@ -289,8 +305,9 @@ class GlobalHeatMap:
         bicubic to the image size -> min/max -> normalise / threshold) and one device-to-host copy instead of four
         launches and a blocking copy per word.
 
-        Returns ``(word_heat_maps, expanded)``: a list of :class:`WordHeatMap` (device ``[x, x]`` views, same values as
-        ``compute_word_heat_map``) and ``expanded`` ``[len(words), image.size[0], image.size[1]]`` (CPU by default like
+        Returns ``(word_heat_maps, expanded)``: a list of :class:`WordHeatMap` (device ``[xh, xw]`` views, same values as
+        ``compute_word_heat_map``) and ``expanded`` ``[len(words), out_h, out_w]`` -- the image size as
+        :meth:`WordHeatMap.expand_as` orders it -- (CPU by default like
         ``expand_as``; ``to_cpu=False`` keeps it on the device until the caller needs it). ``word_idx`` may be a list
         parallel to ``words``. Raises the reference's ``ValueError`` for a word that is not in the prompt."""
         words = list(words)
@@ -298,21 +315,21 @@ class GlobalHeatMap:
         merged = [compute_token_merge_indices(self.tokenizer, self.prompt, w, i, offset_idx) for w, i in zip(words, idxs)]
         maps = self.heat_maps
         _require_cuda(maps, 'GlobalHeatMap.expand_words')
-        n_rows, x = maps.shape[0], maps.shape[-1]
+        n_rows, grid = maps.shape[0], tuple(maps.shape[-2:])
         for rows, _ in merged:
             for r in rows:
                 if not -n_rows <= r < n_rows:
                     raise IndexError(f'index {r} is out of bounds for dimension 0 with size {n_rows}')
+        out_h, out_w = _image_size(image, *grid)
         if not words:
-            return [], torch.empty((0, int(image.size[0]), int(image.size[1])))
+            return [], torch.empty((0, out_h, out_w))
         maps = maps.detach().float().contiguous()
-        out_h, out_w = int(image.size[0]), int(image.size[1])
         dev = maps.device
-        word_maps = torch.empty((len(words), x, x), dtype=torch.float32, device=dev)
+        word_maps = torch.empty((len(words),) + grid, dtype=torch.float32, device=dev)
         out = torch.empty((len(words), out_h, out_w), dtype=torch.float32, device=dev)
         scratch = torch.empty(_native.EXPAND_SCRATCH_FLOATS * len(words), dtype=torch.float32, device=dev)
         with torch.cuda.device(dev):
-            _native.expand_words(maps.data_ptr(), n_rows, x, [rows for rows, _ in merged], out_h, out_w, absolute,
+            _native.expand_words(maps.data_ptr(), n_rows, grid, [rows for rows, _ in merged], out_h, out_w, absolute,
                                  threshold, word_maps.data_ptr(), out.data_ptr(), scratch.data_ptr(), _stream_ptr(dev))
         whms = [WordHeatMap(word_maps[i], w, idx) for i, (w, (_, idx)) in enumerate(zip(words, merged))]
         return whms, (out.cpu() if to_cpu else out)
@@ -328,7 +345,7 @@ class TimeHeatMaps:
     def __init__(self, tokenizer, prompt: str, heat_maps: torch.Tensor):
         self.tokenizer = tokenizer
         self.prompt = prompt
-        self.heat_maps = heat_maps           # device fp32 [steps, n_rows, x, x]
+        self.heat_maps = heat_maps           # device fp32 [steps, n_rows, xh, xw]
 
     def __len__(self) -> int:
         return self.heat_maps.shape[0]
@@ -338,18 +355,18 @@ class TimeHeatMaps:
         return GlobalHeatMap(self.tokenizer, self.prompt, self.heat_maps[t])
 
     def word_heat_maps(self, word: str, word_idx: int = None, offset_idx: int = 0) -> torch.Tensor:
-        """``[steps, x, x]``: row ``t`` is ``self[t].compute_word_heat_map(word, word_idx, offset_idx).heatmap``."""
+        """``[steps, xh, xw]``: row ``t`` is ``self[t].compute_word_heat_map(word, word_idx, offset_idx).heatmap``."""
         rows, _ = compute_token_merge_indices(self.tokenizer, self.prompt, word, word_idx, offset_idx)
         maps = self.heat_maps
         _require_cuda(maps, 'TimeHeatMaps.word_heat_maps')
-        steps, n_rows, x = maps.shape[0], maps.shape[1], maps.shape[-1]
+        steps, n_rows, grid = maps.shape[0], maps.shape[1], tuple(maps.shape[-2:])
         for r in rows:
             if not -n_rows <= r < n_rows:
                 raise IndexError(f'index {r} is out of bounds for dimension 0 with size {n_rows}')
         maps = maps.detach().float().contiguous()
-        out = torch.empty((steps, x, x), dtype=torch.float32, device=maps.device)
+        out = torch.empty((steps,) + grid, dtype=torch.float32, device=maps.device)
         with torch.cuda.device(maps.device):
             stream = _stream_ptr(maps.device)
             for t in range(steps):
-                _native.word_heat_map(maps[t].data_ptr(), n_rows, x, rows, out[t].data_ptr(), stream)
+                _native.word_heat_map(maps[t].data_ptr(), n_rows, grid, rows, out[t].data_ptr(), stream)
         return out

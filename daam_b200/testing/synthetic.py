@@ -201,7 +201,8 @@ class _Down(nn.Module):
         self.conv = nn.Conv2d(c, c, 3, stride=2, padding=1) if full else None
 
     def forward(self, x):
-        return self.conv(x) if self.conv is not None else F.avg_pool2d(x, 2)
+        # ceil-sized like diffusers' stride-2 convolution (which the full body's conv is): odd sides round up
+        return self.conv(x) if self.conv is not None else F.avg_pool2d(x, 2, ceil_mode=True)
 
 
 class _Up(nn.Module):
@@ -209,8 +210,12 @@ class _Up(nn.Module):
         super().__init__()
         self.conv = nn.Conv2d(c, c, 3, padding=1) if full else None
 
-    def forward(self, x):
-        x = F.interpolate(x, scale_factor=2.0, mode='nearest')
+    def forward(self, x, size=None):
+        # to the next skip's size (diffusers' upsample_size), which is twice the input unless a side was odd
+        if size is None or tuple(size) == (2 * x.shape[-2], 2 * x.shape[-1]):
+            x = F.interpolate(x, scale_factor=2.0, mode='nearest')
+        else:
+            x = F.interpolate(x, size=size, mode='nearest')
         return self.conv(x) if self.conv is not None else x
 
 
@@ -262,7 +267,7 @@ class _UpBlockBase(nn.Module):
             if hasattr(self, 'attentions'):
                 x = self.attentions[i](x, ctx)
         if self.upsamplers is not None:
-            x = self.upsamplers[0](x)
+            x = self.upsamplers[0](x, tuple(skips[-1].shape[-2:]) if skips else None)
         return x
 
 
@@ -451,18 +456,17 @@ class SyntheticPipeline:
         lat.copy_((lat - 0.02 * eps).clamp_(-4, 4))
         st['stat'].copy_(eps.float().mean(dim=(1, 2, 3)))
 
-    def _state(self, n):
+    def _state(self, n, latent_h, latent_w):
         spec, dev = self.unet.spec, self.device
-        key = (n, tuple(id(m.processor) for m in self._attn))
+        key = (n, latent_h, latent_w, tuple(id(m.processor) for m in self._attn))
         st = self._graphs.get(key)
         if st is None:
             if len(self._graphs) > 4:
                 self._graphs.clear()
             st = {
                 'emb': torch.empty(2 * n, spec.tokens, spec.cross_attention_dim, dtype=self.dtype, device=dev),
-                'lat0': torch.empty(n, spec.in_channels, spec.sample_size, spec.sample_size, dtype=self.dtype, device=dev),
-                'latents': torch.empty(n, spec.in_channels, spec.sample_size, spec.sample_size, dtype=self.dtype,
-                                       device=dev),
+                'lat0': torch.empty(n, spec.in_channels, latent_h, latent_w, dtype=self.dtype, device=dev),
+                'latents': torch.empty(n, spec.in_channels, latent_h, latent_w, dtype=self.dtype, device=dev),
                 't': torch.zeros(1, dtype=torch.float32, device=dev),
                 'stat': torch.zeros(n, dtype=torch.float32, device=dev),
                 'graph': None, 'eager_steps': 0,
@@ -472,15 +476,21 @@ class SyntheticPipeline:
 
     @torch.no_grad()
     def __call__(self, prompt, num_inference_steps: int = 50, generator: Optional[torch.Generator] = None,
-                 callback=None, guidance_scale: float = 7.5):
-        self.check_inputs(prompt)
+                 callback=None, guidance_scale: float = 7.5, height: Optional[int] = None, width: Optional[int] = None):
+        """``height`` / ``width``: the image size in pixels, as diffusers takes it (default: the model's own square
+        size); the latent is ``height // 8 x width // 8``."""
+        spec = self.unet.spec
+        height = spec.sample_size * self.vae_scale_factor if height is None else height
+        width = spec.sample_size * self.vae_scale_factor if width is None else width
+        self.check_inputs(prompt, height, width)
         prompts = [prompt] if isinstance(prompt, str) else list(prompt)
-        n, spec = len(prompts), self.unet.spec
+        n = len(prompts)
+        latent_h, latent_w = height // self.vae_scale_factor, width // self.vae_scale_factor
         if generator is None:
             generator = torch.Generator().manual_seed(self.seed)
         cuda = self.device.type == 'cuda'
         emb_h = self.encode(prompts, generator).to(self.dtype)
-        lat_h = torch.randn(n, spec.in_channels, spec.sample_size, spec.sample_size, generator=generator,
+        lat_h = torch.randn(n, spec.in_channels, latent_h, latent_w, generator=generator,
                             dtype=torch.float32).to(self.dtype)
         t_h = torch.tensor([[1000.0 * (1.0 - i / max(1, num_inference_steps))] for i in range(num_inference_steps)])
         out_h = torch.empty(n, dtype=torch.float32)
@@ -488,7 +498,7 @@ class SyntheticPipeline:
             emb_h, lat_h, t_h, out_h = emb_h.pin_memory(), lat_h.pin_memory(), t_h.pin_memory(), out_h.pin_memory()
         self.h2d_bytes_per_step = emb_h.numel() * emb_h.element_size() + lat_h.numel() * lat_h.element_size() + 4
         self.d2h_bytes_per_step = n * 4
-        st = self._state(n)
+        st = self._state(n, latent_h, latent_w)
         for i in range(num_inference_steps):
             st['emb'].copy_(emb_h, non_blocking=True)            # H2D: the step's inputs
             st['lat0'].copy_(lat_h, non_blocking=True)

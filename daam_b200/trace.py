@@ -28,15 +28,14 @@ section 5); parity is stated against the fp32 oracle fed the same Q/K.
 """
 from __future__ import annotations
 
-import math
 from pathlib import Path
 from typing import Dict, List, Optional, Tuple, Type, Union
 
-import numpy as np
 import torch
 import torch.nn.functional as F
 
 from . import _native, ops
+from .geometry import LatentGeometry
 from .heatmap import GlobalHeatMap, LayerSlab, RawHeatMapCollection, TimeHeatMaps
 from .hook import AggregateHooker, ObjectHooker, UNetCrossAttentionLocator
 from .utils import cache_dir
@@ -81,6 +80,10 @@ class DiffusionHeatMapHooker(AggregateHooker):
         self.all_heat_maps = RawHeatMapCollection()
         side = pipeline.unet.config.sample_size * pipeline.vae_scale_factor
         self.latent_hw = 4096 if side in (512, 1024) else 9216   # 64x64, or 96x96 for the 768-pixel models
+        # the heat-map grid and every layer's (h, w, factor): square until the first UNet forward shows the latent
+        # (a forward pre-hook on the UNet re-derives it whenever the latent's (H, W) changes)
+        self._sample_size = pipeline.unet.config.sample_size
+        self.geometry = LatentGeometry(self.latent_hw, self._sample_size)
         self.locator = UNetCrossAttentionLocator(restrict={0} if low_memory else None,
                                                  locate_middle_block=locate_middle_block or load_heads or save_heads)
         self.last_prompt: str = ''
@@ -129,6 +132,7 @@ class DiffusionHeatMapHooker(AggregateHooker):
                                      save_heads=save_heads, data_dir=data_dir)
             for idx, m in enumerate(self.locator.locate(pipeline.unet))
         ]
+        self._attn_hookers = list(modules)
         modules.append(PipelineHooker(pipeline, self))
         if type(pipeline).__name__ == 'StableDiffusionXLPipeline' and getattr(pipeline, 'image_processor', None):
             modules.append(ImageProcessorHooker(pipeline.image_processor, self))
@@ -157,16 +161,41 @@ class DiffusionHeatMapHooker(AggregateHooker):
         super()._hook_impl()
         unet = self.pipe.unet
         self._forward_hook = None
+        self._pre_hook = None
         if self.launch != 'layer' and hasattr(unet, 'register_forward_hook'):
             # end of every UNet forward = end of the step's layer calls: issue the step launch right away
             self._forward_hook = unet.register_forward_hook(lambda *_: self.flush())
+        if hasattr(unet, 'register_forward_pre_hook'):
+            # start of every UNet forward: the latent's (H, W) decides the heat-map geometry (one shape comparison)
+            self._pre_hook = unet.register_forward_pre_hook(self._see_sample, with_kwargs=True)
 
     def _unhook_impl(self):
         self.synchronize()      # issue what is queued and order it (and the parked projections) before the caller's stream
         if getattr(self, '_forward_hook', None) is not None:
             self._forward_hook.remove()
             self._forward_hook = None
+        if getattr(self, '_pre_hook', None) is not None:
+            self._pre_hook.remove()
+            self._pre_hook = None
         super()._unhook_impl()
+
+    # -- geometry -----------------------------------------------------------------------------------------------------
+    def _see_sample(self, _module, args, kwargs):
+        """UNet forward pre-hook: the latent ``sample`` (``args[0]`` or ``kwargs['sample']``) fixes the geometry."""
+        sample = args[0] if args else kwargs.get('sample')
+        if sample is not None and tuple(sample.shape[-2:]) != self.geometry.latent_shape:
+            self.set_latent_shape(tuple(sample.shape[-2:]))
+
+    def set_latent_shape(self, shape: Tuple[int, int]):
+        """Re-derive the heat-map geometry for a latent of spatial size ``shape = (H, W)``. When the layer rule changes
+        (e.g. 512x768 after 768x512: same query counts, transposed keys) every cached layer descriptor and factor is
+        dropped, so the next call of each layer re-tags its slab with the new ``(h, w)``."""
+        geometry = LatentGeometry(self.latent_hw, self._sample_size, shape)
+        if geometry.key != self.geometry.key:
+            self._layer_state.clear()
+            for hooker in self._attn_hookers:
+                hooker._geom = None
+        self.geometry = geometry
 
     # -- kernel queue -------------------------------------------------------------------------------------------------
     def _side_stream(self, device) -> torch.cuda.Stream:
@@ -217,13 +246,13 @@ class DiffusionHeatMapHooker(AggregateHooker):
         if q.stride(-1) != 1 or k.stride(-1) != 1:
             q, k = q.contiguous(), k.contiguous()
         bsz, hw, _ = q.shape
-        side = int(math.sqrt(hw))
-        if side * side != hw:
+        h, w, _ = self.geometry.level(hw, layer_idx)
+        if h is None:
             raise RuntimeError(f'layer {layer_idx}: {hw} query positions are not a square map')
         # "second half of the batch*heads axis" (trace.py:240): the conditional samples of a CFG batch
         _, n_samples, head0, n_heads = ops.cond_half(bsz, heads)
         n_real, images = self._prompt_layout(layer_idx, n_samples)
-        slab = self.all_heat_maps.slab_for(layer_idx, factor, n_real, images * n_heads, side, side, q.device, head0)
+        slab = self.all_heat_maps.slab_for(layer_idx, factor, n_real, images * n_heads, h, w, q.device, head0)
         self._epoch_seen = self.all_heat_maps.epoch        # (this call may have bumped it; the other layers' slabs stand)
         desc = ops.make_layer_desc(q, k, slab.acc.view(n_samples, n_heads, slab.acc.shape[2], hw), heads, scale)
         if self.launch != 'layer':
@@ -271,11 +300,12 @@ class DiffusionHeatMapHooker(AggregateHooker):
 
     def _accumulate_probs(self, layer_idx: int, factor: int, probs: torch.Tensor, bsz: int, heads: int):
         """Heat maps from materialised probabilities (save_heads / load_heads compatibility path)."""
-        hw = probs.shape[1]
-        side = int(math.sqrt(hw))
+        h, w, _ = self.geometry.level(probs.shape[1], layer_idx)
+        if h is None:
+            raise RuntimeError(f'layer {layer_idx}: {probs.shape[1]} query positions are not a square map')
         _, n_samples, head0, n_heads = ops.cond_half(bsz, heads)
         n_real, images = self._prompt_layout(layer_idx, n_samples)
-        slab = self.all_heat_maps.slab_for(layer_idx, factor, n_real, images * n_heads, side, side, probs.device, head0)
+        slab = self.all_heat_maps.slab_for(layer_idx, factor, n_real, images * n_heads, h, w, probs.device, head0)
         self.synchronize()
         ops.accumulate_probs(probs, slab.acc)
 
@@ -355,7 +385,7 @@ class DiffusionHeatMapHooker(AggregateHooker):
         :meth:`compute_global_heat_map` -- into the next slot of the prompt's history."""
         queued = {idx for idx, step in self._queued.items() if step == self._step_id}
         slabs = [s for s in self.all_heat_maps.live_slabs() if s.layer_idx in queued]
-        x = int(np.sqrt(self.latent_hw))
+        grid = self.geometry.grid
         t = self._time_steps
         prompts = self.last_prompts or [self.last_prompt]
         if self._history_rows is None:
@@ -363,13 +393,13 @@ class DiffusionHeatMapHooker(AggregateHooker):
         for p in range(slabs[0].n_prompts):
             n_rows = self._history_rows[p] if p < len(self._history_rows) else self._history_rows[0]
             if p == len(self._history):
-                self._history.append(torch.empty((16, n_rows, x, x), dtype=torch.float32, device=device))
+                self._history.append(torch.empty((16, n_rows) + grid, dtype=torch.float32, device=device))
             hist = self._history[p]
             if t == hist.shape[0]:                          # grow by doubling, in stream order between two steps
                 grown = torch.empty((2 * t,) + tuple(hist.shape[1:]), dtype=torch.float32, device=device)
                 grown[:t].copy_(hist)
                 self._history[p] = hist = grown
-            _native.finalize([_key_group(s.step[p], s) for s in slabs], x, n_rows, False, hist[t].data_ptr(), stream)
+            _native.finalize([_key_group(s.step[p], s) for s in slabs], grid, n_rows, False, hist[t].data_ptr(), stream)
         self._time_steps = t + 1
 
     def _restart_history(self):
@@ -421,12 +451,12 @@ class DiffusionHeatMapHooker(AggregateHooker):
         ``batch_prompts`` mode. ``step_range=i`` aggregates over the steps of declared range ``i`` only
         (``trace(pipe, step_ranges=[...])``): the DAAM map a trace of only those steps would give.
         """
-        prompt, x, n_rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range, layer_idx,
-                                                             head_idx)
+        prompt, grid, n_rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range, layer_idx,
+                                                                head_idx)
         device = slabs[0].acc.device
-        maps = torch.empty((n_rows, x, x), dtype=torch.float32, device=device)
+        maps = torch.empty((n_rows,) + grid, dtype=torch.float32, device=device)
         with torch.cuda.device(device):
-            _native.finalize(groups, x, n_rows, normalize, maps.data_ptr(),
+            _native.finalize(groups, grid, n_rows, normalize, maps.data_ptr(),
                              torch.cuda.current_stream(device).cuda_stream)
         return GlobalHeatMap(self.pipe.tokenizer, prompt, maps)
 
@@ -436,8 +466,8 @@ class DiffusionHeatMapHooker(AggregateHooker):
         only step ``t`` been traced, with every key and layer; ``normalize`` applies the reference's normalisation to
         each step. Summing the steps does not give the all-steps map: there the clamp comes after the time sum.
 
-        Costs: a second fp32 slab per traced layer (as large as its accumulator) and ``steps x n_rows x x x x`` fp32 of
-        history per prompt."""
+        Costs: a second fp32 slab per traced layer (as large as its accumulator) and ``steps x n_rows x xh x xw`` fp32
+        of history per prompt (``heat_maps`` is ``[steps, n_rows, xh, xw]``, the grid of :attr:`geometry`)."""
         if not self.time_resolved:
             raise RuntimeError('per-step heat maps need trace(pipe, time_resolved=True)')
         self.synchronize()
@@ -448,7 +478,7 @@ class DiffusionHeatMapHooker(AggregateHooker):
         if normalize:
             maps = maps.clone()
             with torch.cuda.device(maps.device):
-                _native.normalize_maps(maps.data_ptr(), maps.shape[0], maps.shape[1], maps.shape[-1],
+                _native.normalize_maps(maps.data_ptr(), maps.shape[0], maps.shape[1], maps.shape[-2:],
                                        torch.cuda.current_stream(maps.device).cuda_stream)
         return TimeHeatMaps(self.pipe.tokenizer, prompt, maps)
 
@@ -457,19 +487,19 @@ class DiffusionHeatMapHooker(AggregateHooker):
                                    step_range: Optional[int] = None):
         """Every ``compute_global_heat_map(layer_idx=l, head_idx=h)`` of the reference's ``--all-heads`` sweep
         (daam/run/generate.py:239-255) in one launch. Returns ``(keys, maps)``: ``keys[i] = (factor, layer, head)`` and
-        ``maps[i]`` the ``[n_tokens + 2, x, x]`` heat map the reference computes for that single key. ``step_range=i``:
+        ``maps[i]`` the ``[n_tokens + 2, xh, xw]`` heat map the reference computes for that single key. ``step_range=i``:
         over the steps of declared range ``i`` only, as in :meth:`compute_global_heat_map`."""
-        prompt, x, n_rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range)
+        prompt, grid, n_rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range)
         keys = [(slab.factor, slab.layer_idx, head) for slab in slabs for head in range(slab.heads)]
         device = slabs[0].acc.device
-        maps = torch.empty((len(keys), n_rows, x, x), dtype=torch.float32, device=device)
+        maps = torch.empty((len(keys), n_rows) + grid, dtype=torch.float32, device=device)
         with torch.cuda.device(device):
-            _native.finalize_per_key(groups, x, n_rows, normalize, maps.data_ptr(),
+            _native.finalize_per_key(groups, grid, n_rows, normalize, maps.data_ptr(),
                                      torch.cuda.current_stream(device).cuda_stream)
         return keys, maps
 
     def _read_groups(self, prompt, factors, prompt_idx: int, step_range: Optional[int], layer_idx=None, head_idx=None):
-        """What the heat-map reads share: the prompt (default: the generation's), the map side ``x``, the row count, and
+        """What the heat-map reads share: the prompt (default: the generation's), the map grid ``(xh, xw)``, the row count, and
         the key groups of prompt ``prompt_idx`` over the live slabs (with ``step_range``: over that range's slabs) that
         pass the filters, with the slabs behind them. Raises when no slab passes."""
         if prompt is None:
@@ -489,7 +519,7 @@ class DiffusionHeatMapHooker(AggregateHooker):
                 raise RuntimeError('No heat maps found for the given parameters.')
             raise RuntimeError('No heat maps found. Did you forget to call `with trace(...)` during generation?')
         n_rows = min(len(self.pipe.tokenizer.tokenize(prompt)) + 2, _native.TOKENS)   # 1 for SOS and 1 for padding
-        return prompt, int(np.sqrt(self.latent_hw)), n_rows, groups, slabs
+        return prompt, self.geometry.grid, n_rows, groups, slabs
 
 
 def _key_group(acc: torch.Tensor, slab: LayerSlab, head_sel: int = -1) -> _native.DaamKeyGroup:
@@ -593,7 +623,7 @@ class UNetCrossAttentionHooker(ObjectHooker):
         self.heat_maps = parent_trace.all_heat_maps
         self.context_size = context_size
         self.layer_idx = layer_idx
-        self.latent_hw = latent_hw
+        self.latent_hw = latent_hw             # kept for the reference's signature; the factor comes from trace.geometry
         self.load_heads = load_heads
         self.save_heads = save_heads
         self.trace = parent_trace
@@ -618,7 +648,7 @@ class UNetCrossAttentionHooker(ObjectHooker):
             self._save_attn(probs)
         else:
             probs = self._load_attn().to(query.device)
-        factor = int(math.sqrt(self.latent_hw // probs.shape[1]))
+        factor = self.trace.geometry.level(probs.shape[1], self.layer_idx)[2]
         self.trace._gen_idx += 1
         if probs.shape[-1] == self.context_size and factor != 8:
             self.trace._accumulate_probs(self.layer_idx, factor, probs, bsz, heads)
@@ -646,11 +676,12 @@ class UNetCrossAttentionHooker(ObjectHooker):
 
         heads = attn.heads
         tokens = key.shape[1]
+        tr = self.trace
         geom = self._geom                                    # (n, tokens) -> factor and the trace / skip decision
         if geom is None or geom[0] != n or geom[1] != tokens:
-            factor = int(math.sqrt(self.latent_hw // n))
-            geom = self._geom = (n, tokens, factor, tokens == self.context_size and factor != 8)   # trace.py:285-289
-        tr = self.trace
+            # trace.py:285-289; the tracer's geometry gives the factor (and drops this cache when the latent changes)
+            factor = tr.geometry.level(n, self.layer_idx)[2] if tokens == self.context_size else None
+            geom = self._geom = (n, tokens, factor, tokens == self.context_size and factor != 8)
         tr._gen_idx += 1
         if geom[3]:                                          # skip if too large (trace.py:289)
             tr._enqueue(self.layer_idx, geom[2], query, key, heads, attn.scale)

@@ -182,6 +182,16 @@ int daam_finalize(const daam_key_group* groups, int32_t n_groups, int32_t x, int
                   float* out, void* stream);
 
 /*
+ * daam_finalize to a rectangular [map_h][map_w] grid (non-square images): every key is bicubic-upsampled with taps
+ * key h -> map_h and key w -> map_w, then clamp, mean and normalise as daam_finalize. out: device fp32
+ * [n_rows][map_h][map_w]. daam_finalize(x) is exactly daam_finalize_rect(x, x). Keys with one integer factor 1, 2 or 4
+ * on both axes and 16-byte-aligned bases (aligned slab, h * w a multiple of 4) run the banded fast kernel; anything
+ * else, or DAAM_FINALIZE_GENERIC=1, runs the generic gather kernel (DESIGN.md section 4.3).
+ */
+int daam_finalize_rect(const daam_key_group* groups, int32_t n_groups, int32_t map_h, int32_t map_w, int32_t n_rows,
+                       int32_t normalize, float* out, void* stream);
+
+/*
  * The reference's --all-heads sweep calls compute_global_heat_map(layer_idx=l, head_idx=h) once per (layer, head)
  * (daam/run/generate.py:239-255): each call reduces exactly one key, i.e. bicubic + clamp (+ normalise) of that key.
  * This entry point produces all of them in one launch: out [n_keys][n_rows][x][x] (device fp32), keys enumerated
@@ -191,11 +201,24 @@ int daam_finalize_per_key(const daam_key_group* groups, int32_t n_groups, int32_
                           float* out, void* stream);
 
 /*
+ * daam_finalize_per_key to a rectangular grid: out [n_keys][n_rows][map_h][map_w] (device fp32), taps key h -> map_h
+ * and key w -> map_w. daam_finalize_per_key(x) is exactly daam_finalize_per_key_rect(x, x).
+ */
+int daam_finalize_per_key_rect(const daam_key_group* groups, int32_t n_groups, int32_t map_h, int32_t map_w,
+                               int32_t n_rows, int32_t normalize, float* out, void* stream);
+
+/*
  * The `normalize` step of daam_finalize on its own, in place, for n_maps independent [n_rows][x][x] heat maps stored
  * back to back (e.g. the per-step global maps of a time-resolved trace): maps / (sum of rows 1..n_rows-2 + 1e-6) per
  * pixel, the same arithmetic as daam_finalize(normalize = 1).
  */
 int daam_normalize_maps(float* maps, int32_t n_maps, int32_t n_rows, int32_t x, void* stream);
+
+/*
+ * daam_normalize_maps for n_maps [n_rows][map_h][map_w] heat maps stored back to back. daam_normalize_maps(x) is
+ * exactly daam_normalize_maps_rect(x, x).
+ */
+int daam_normalize_maps_rect(float* maps, int32_t n_maps, int32_t n_rows, int32_t map_h, int32_t map_w, void* stream);
 
 /*
  * Replaces GlobalHeatMap.compute_word_heat_map's tensor part (daam/heatmap.py:121-123): mean over the rows
@@ -204,6 +227,13 @@ int daam_normalize_maps(float* maps, int32_t n_maps, int32_t n_rows, int32_t x, 
  */
 int daam_word_heat_map(const float* global_maps, int32_t n_rows, int32_t x, const int32_t* rows, int32_t n_sel,
                        float* out, void* stream);
+
+/*
+ * daam_word_heat_map of global_maps [n_rows][map_h][map_w] -> out [map_h][map_w]. daam_word_heat_map(x) is exactly
+ * daam_word_heat_map_rect(x, x).
+ */
+int daam_word_heat_map_rect(const float* global_maps, int32_t n_rows, int32_t map_h, int32_t map_w,
+                            const int32_t* rows, int32_t n_sel, float* out, void* stream);
 
 /*
  * Replaces WordHeatMap.expand_as's tensor part (daam/heatmap.py:77-93): bicubic upsample of word_map [x][x] to
@@ -215,6 +245,15 @@ int daam_word_heat_map(const float* global_maps, int32_t n_rows, int32_t x, cons
 #define DAAM_EXPAND_SCRATCH_FLOATS 64   /* per word: partial min/max of up to 32 pixel chunks */
 int daam_expand_as(const float* word_map, int32_t x, int32_t out_h, int32_t out_w, int32_t absolute,
                    int32_t use_threshold, float threshold, float* out, float* scratch, void* stream);
+
+/*
+ * daam_expand_as of a rectangular word_map [map_h][map_w]: taps map_h -> out_h and map_w -> out_w. Limit:
+ * map_h * map_w * 4 bytes <= 200 KB (the map lives in shared memory). daam_expand_as(x) is exactly
+ * daam_expand_as_rect(x, x).
+ */
+int daam_expand_as_rect(const float* word_map, int32_t map_h, int32_t map_w, int32_t out_h, int32_t out_w,
+                        int32_t absolute, int32_t use_threshold, float threshold, float* out, float* scratch,
+                        void* stream);
 
 /*
  * The per-word loop a user of the reference writes -- `for word in prompt: global_heat_map.compute_word_heat_map(word)
@@ -229,6 +268,16 @@ int daam_expand_as(const float* word_map, int32_t x, int32_t out_h, int32_t out_
 int daam_expand_words(const float* global_maps, int32_t n_rows, int32_t x, const int32_t* rows, const int32_t* row_begin,
                       int32_t n_words, int32_t out_h, int32_t out_w, int32_t absolute, int32_t use_threshold,
                       float threshold, float* word_maps, float* out, float* scratch, void* stream);
+
+/*
+ * daam_expand_words over rectangular global_maps [n_rows][map_h][map_w]: word maps [n_words][map_h][map_w], taps
+ * map_h -> out_h and map_w -> out_w, out [n_words][out_h][out_w]. Same limits as daam_expand_words plus map_h * map_w *
+ * 4 bytes <= 200 KB. daam_expand_words(x) is exactly daam_expand_words_rect(x, x).
+ */
+int daam_expand_words_rect(const float* global_maps, int32_t n_rows, int32_t map_h, int32_t map_w, const int32_t* rows,
+                           const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w, int32_t absolute,
+                           int32_t use_threshold, float threshold, float* word_maps, float* out, float* scratch,
+                           void* stream);
 
 /* Library / device introspection. */
 int daam_abi_version(void);
