@@ -64,7 +64,7 @@ def layer_keys(workload, sample_size, image):
 
 
 def fast_rule(keys, grid):
-    """The library's choice of finalize kernel (finalize.cu, ``finalize_impl``), restated for the report."""
+    """The library's choice of finalize kernel (finalize.cu, ``daam_finalize``), restated for the report."""
     xh, xw = grid
     if (xh == xw and xh % 16) or xw > 256 or sum(k for _, _, k in keys) > 2048:
         return 'generic'

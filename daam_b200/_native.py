@@ -18,15 +18,13 @@ ACC_AUTO, ACC_FORCE_SIMT, ACC_FORCE_MMA = 0, 1, 2
 ACC_RMW_AUTO, ACC_RMW_LDST, ACC_RMW_RED = 0x00, 0x10, 0x20
 ACC_NO_PDL = 0x100
 ACC_EARLY_LOADS = 0x200   # see include/daam_b200.h: only valid when q/k were complete before the previous kernel started
-ABI_VERSION = 3
+ABI_VERSION = 4
 E_INVALID, E_UNSUPPORTED, E_CUDA = -1, -2, -3
 TOKENS = 77
 EXPAND_SCRATCH_FLOATS = 64   # DAAM_EXPAND_SCRATCH_FLOATS: per word
 
 EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize',
            'daam_finalize_per_key', 'daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
-           'daam_finalize_rect', 'daam_finalize_per_key_rect', 'daam_normalize_maps_rect', 'daam_word_heat_map_rect',
-           'daam_expand_as_rect', 'daam_expand_words_rect',
            'daam_side_launcher_create', 'daam_side_launcher_destroy',
            'daam_side_launcher_launch', 'daam_side_launcher_join', 'daam_side_launcher_idle', 'daam_abi_version',
            'daam_last_error', 'daam_device_info', 'daam_launch_count')
@@ -83,34 +81,23 @@ def load() -> ctypes.CDLL:
     lib.daam_accumulate_steps.restype = ctypes.c_int
     lib.daam_accumulate_range.argtypes = [ctypes.POINTER(DaamLayer), ctypes.POINTER(vp), i32, u32, vp]
     lib.daam_accumulate_range.restype = ctypes.c_int
-    lib.daam_normalize_maps.argtypes = [vp, i32, i32, i32, vp]
+    lib.daam_normalize_maps.argtypes = [vp, i32, i32, i32, i32, vp]
     lib.daam_normalize_maps.restype = ctypes.c_int
     lib.daam_attention_probs.argtypes = [ctypes.POINTER(DaamLayer), vp, vp]
     lib.daam_attention_probs.restype = ctypes.c_int
     lib.daam_accumulate_probs.argtypes = [vp, i32, i32, i32, i32, i32, vp, vp]
     lib.daam_accumulate_probs.restype = ctypes.c_int
-    lib.daam_finalize.argtypes = [ctypes.POINTER(DaamKeyGroup), i32, i32, i32, i32, vp, vp]
+    lib.daam_finalize.argtypes = [ctypes.POINTER(DaamKeyGroup), i32, i32, i32, i32, i32, vp, vp]
     lib.daam_finalize.restype = ctypes.c_int
-    lib.daam_finalize_per_key.argtypes = [ctypes.POINTER(DaamKeyGroup), i32, i32, i32, i32, vp, vp]
+    lib.daam_finalize_per_key.argtypes = [ctypes.POINTER(DaamKeyGroup), i32, i32, i32, i32, i32, vp, vp]
     lib.daam_finalize_per_key.restype = ctypes.c_int
-    lib.daam_word_heat_map.argtypes = [vp, i32, i32, ctypes.POINTER(i32), i32, vp, vp]
+    lib.daam_word_heat_map.argtypes = [vp, i32, i32, i32, ctypes.POINTER(i32), i32, vp, vp]
     lib.daam_word_heat_map.restype = ctypes.c_int
-    lib.daam_expand_as.argtypes = [vp, i32, i32, i32, i32, i32, f32, vp, vp, vp]
+    lib.daam_expand_as.argtypes = [vp, i32, i32, i32, i32, i32, i32, f32, vp, vp, vp]
     lib.daam_expand_as.restype = ctypes.c_int
-    lib.daam_expand_words.argtypes = [vp, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32, i32, i32, f32,
-                                      vp, vp, vp, vp]
+    lib.daam_expand_words.argtypes = [vp, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32, i32,
+                                      i32, f32, vp, vp, vp, vp]
     lib.daam_expand_words.restype = ctypes.c_int
-    # the rectangular siblings: (map_h, map_w) where the square entry points take x
-    lib.daam_finalize_rect.argtypes = [ctypes.POINTER(DaamKeyGroup), i32, i32, i32, i32, i32, vp, vp]
-    lib.daam_finalize_per_key_rect.argtypes = [ctypes.POINTER(DaamKeyGroup), i32, i32, i32, i32, i32, vp, vp]
-    lib.daam_normalize_maps_rect.argtypes = [vp, i32, i32, i32, i32, vp]
-    lib.daam_word_heat_map_rect.argtypes = [vp, i32, i32, i32, ctypes.POINTER(i32), i32, vp, vp]
-    lib.daam_expand_as_rect.argtypes = [vp, i32, i32, i32, i32, i32, i32, f32, vp, vp, vp]
-    lib.daam_expand_words_rect.argtypes = [vp, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
-                                           i32, i32, f32, vp, vp, vp, vp]
-    for name in ('daam_finalize_rect', 'daam_finalize_per_key_rect', 'daam_normalize_maps_rect',
-                 'daam_word_heat_map_rect', 'daam_expand_as_rect', 'daam_expand_words_rect'):
-        getattr(lib, name).restype = ctypes.c_int
     lib.daam_side_launcher_create.argtypes = [ctypes.POINTER(vp)]
     lib.daam_side_launcher_create.restype = ctypes.c_int
     lib.daam_side_launcher_destroy.argtypes = [vp]
@@ -236,7 +223,7 @@ def map_size(x) -> Tuple[int, int]:
 def normalize_maps(maps_ptr: int, n_maps: int, n_rows: int, x, stream: int):
     """``x``: the map side, or ``(h, w)``."""
     h, w = map_size(x)
-    _check(load().daam_normalize_maps_rect(ctypes.c_void_p(maps_ptr), n_maps, n_rows, h, w, ctypes.c_void_p(stream)))
+    _check(load().daam_normalize_maps(ctypes.c_void_p(maps_ptr), n_maps, n_rows, h, w, ctypes.c_void_p(stream)))
 
 
 def attention_probs(layer: DaamLayer, probs_ptr: int, stream: int):
@@ -248,38 +235,38 @@ def accumulate_probs(probs_ptr: int, dtype: int, first_row: int, n_rows: int, hw
     _check(load().daam_accumulate_probs(probs_ptr, dtype, first_row, n_rows, hw, tokens, acc_ptr, stream))
 
 
-# The finalize / word-map / expand wrappers take the map grid as its side ``x`` or as ``(h, w)`` and call the ``_rect``
-# entry points (the square ones are their (x, x) case in the library).
-def finalize(groups: Sequence[DaamKeyGroup], x, n_rows: int, normalize: bool, out_ptr: int, stream: int):
+# The finalize / word-map / expand wrappers take the map grid as its side ``x`` or as ``(h, w)``.
+def _finalize(entry: str, groups: Sequence[DaamKeyGroup], x, n_rows: int, normalize: bool, out_ptr: int, stream: int):
+    """``entry``: ``daam_finalize`` or ``daam_finalize_per_key`` (same arguments)."""
     h, w = map_size(x)
     n = len(groups)
     arr = (DaamKeyGroup * max(n, 1))(*groups)
-    _check(load().daam_finalize_rect(arr, n, h, w, n_rows, int(bool(normalize)), ctypes.c_void_p(out_ptr),
-                                     ctypes.c_void_p(stream)))
+    _check(getattr(load(), entry)(arr, n, h, w, n_rows, int(bool(normalize)), ctypes.c_void_p(out_ptr),
+                                  ctypes.c_void_p(stream)))
+
+
+def finalize(groups: Sequence[DaamKeyGroup], x, n_rows: int, normalize: bool, out_ptr: int, stream: int):
+    _finalize('daam_finalize', groups, x, n_rows, normalize, out_ptr, stream)
 
 
 def finalize_per_key(groups: Sequence[DaamKeyGroup], x, n_rows: int, normalize: bool, out_ptr: int, stream: int):
-    h, w = map_size(x)
-    n = len(groups)
-    arr = (DaamKeyGroup * max(n, 1))(*groups)
-    _check(load().daam_finalize_per_key_rect(arr, n, h, w, n_rows, int(bool(normalize)), ctypes.c_void_p(out_ptr),
-                                             ctypes.c_void_p(stream)))
+    _finalize('daam_finalize_per_key', groups, x, n_rows, normalize, out_ptr, stream)
 
 
 def word_heat_map(maps_ptr: int, n_rows: int, x, rows: Sequence[int], out_ptr: int, stream: int):
     h, w = map_size(x)
     arr = (ctypes.c_int32 * max(len(rows), 1))(*rows)
-    _check(load().daam_word_heat_map_rect(ctypes.c_void_p(maps_ptr), n_rows, h, w, arr, len(rows),
-                                          ctypes.c_void_p(out_ptr), ctypes.c_void_p(stream)))
+    _check(load().daam_word_heat_map(ctypes.c_void_p(maps_ptr), n_rows, h, w, arr, len(rows), ctypes.c_void_p(out_ptr),
+                                     ctypes.c_void_p(stream)))
 
 
 def expand_as(map_ptr: int, x, out_h: int, out_w: int, absolute: bool, threshold: Optional[float], out_ptr: int,
               scratch_ptr: int, stream: int):
     h, w = map_size(x)
     use_thr = bool(threshold)   # the reference's `if threshold:` (daam/heatmap.py:87)
-    _check(load().daam_expand_as_rect(ctypes.c_void_p(map_ptr), h, w, out_h, out_w, int(bool(absolute)), int(use_thr),
-                                      float(threshold) if use_thr else 0.0, ctypes.c_void_p(out_ptr),
-                                      ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
+    _check(load().daam_expand_as(ctypes.c_void_p(map_ptr), h, w, out_h, out_w, int(bool(absolute)), int(use_thr),
+                                 float(threshold) if use_thr else 0.0, ctypes.c_void_p(out_ptr),
+                                 ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
 
 
 def expand_words(maps_ptr: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int, out_w: int,
@@ -294,11 +281,11 @@ def expand_words(maps_ptr: int, n_rows: int, x, rows_per_word: Sequence[Sequence
     rows_arr = (ctypes.c_int32 * max(len(flat), 1))(*flat)
     begin_arr = (ctypes.c_int32 * len(begin))(*begin)
     use_thr = bool(threshold)   # the reference's `if threshold:` (daam/heatmap.py:87)
-    _check(load().daam_expand_words_rect(ctypes.c_void_p(maps_ptr), n_rows, h, w, rows_arr, begin_arr,
-                                         len(rows_per_word), out_h, out_w, int(bool(absolute)), int(use_thr),
-                                         float(threshold) if use_thr else 0.0,
-                                         ctypes.c_void_p(word_maps_ptr) if word_maps_ptr else None,
-                                         ctypes.c_void_p(out_ptr), ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
+    _check(load().daam_expand_words(ctypes.c_void_p(maps_ptr), n_rows, h, w, rows_arr, begin_arr,
+                                    len(rows_per_word), out_h, out_w, int(bool(absolute)), int(use_thr),
+                                    float(threshold) if use_thr else 0.0,
+                                    ctypes.c_void_p(word_maps_ptr) if word_maps_ptr else None,
+                                    ctypes.c_void_p(out_ptr), ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
 
 
 def device_info():

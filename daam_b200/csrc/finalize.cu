@@ -540,17 +540,15 @@ static bool force_generic_finalize() {
   return e && e[0] == '1';
 }
 
-// One implementation behind each square / rectangular pair of entry points: the square entry point is the (x, x) case
-// and reports errors under its own name.
-static int finalize_impl(const char* name, const daam_key_group* groups, int32_t n_groups, int32_t oh, int32_t ow,
-                         int32_t n_rows, int32_t normalize, float* out, cudaStream_t stream) {
+// The checks daam_finalize and daam_finalize_per_key share (arguments, device, every key group); `name` is the entry
+// point that was called. *n_keys: the keys the groups select.
+static int check_key_groups(const char* name, const daam_key_group* groups, int32_t n_groups, int32_t oh, int32_t ow,
+                            int32_t n_rows, const float* out, DeviceInfo* dev, int* n_keys) {
   if (!groups || !out || oh <= 0 || ow <= 0 || n_rows <= 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
   if (n_groups <= 0) { set_error("%s: no key selected", name); return DAAM_E_INVALID; }
   if (n_groups > kMaxGroups) { set_error("%s: %d key groups > %d", name, n_groups, kMaxGroups); return DAAM_E_UNSUPPORTED; }
-  DeviceInfo dev;
-  if (int rc = get_device_info(&dev)) return rc;
-  FinalizeParams p;
-  p.n_groups = n_groups; p.oh = oh; p.ow = ow; p.n_rows = n_rows; p.n_keys = 0;
+  if (int rc = get_device_info(dev)) return rc;
+  *n_keys = 0;
   for (int i = 0; i < n_groups; ++i) {
     const daam_key_group& g = groups[i];
     if (!g.acc || g.heads <= 0 || g.h <= 0 || g.w <= 0 || g.tokens < n_rows || g.head_sel >= g.heads) {
@@ -558,9 +556,19 @@ static int finalize_impl(const char* name, const daam_key_group* groups, int32_t
                 g.h, g.w, g.tokens, g.head_sel, n_rows);
       return DAAM_E_INVALID;
     }
-    p.g[i] = g;
-    p.n_keys += g.head_sel < 0 ? g.heads : 1;
+    *n_keys += g.head_sel < 0 ? g.heads : 1;
   }
+  return DAAM_OK;
+}
+
+extern "C" int daam_finalize(const daam_key_group* groups, int32_t n_groups, int32_t oh, int32_t ow, int32_t n_rows,
+                             int32_t normalize, float* out, void* stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DeviceInfo dev;
+  FinalizeParams p;
+  if (int rc = check_key_groups("daam_finalize", groups, n_groups, oh, ow, n_rows, out, &dev, &p.n_keys)) return rc;
+  p.n_groups = n_groups; p.oh = oh; p.ow = ow; p.n_rows = n_rows;
+  for (int i = 0; i < n_groups; ++i) p.g[i] = groups[i];
   const int xx = oh * ow;
   // fast path: every key has one integer factor F = 1 / 2 / 4 on both axes (all SD / SDXL layers that are ever traced)
   // and 16-byte-aligned key bases (cp.async / float4: an aligned slab and h * w a multiple of 4). A square map keeps
@@ -619,39 +627,20 @@ static int finalize_impl(const char* name, const daam_key_group* groups, int32_t
   return DAAM_OK;
 }
 
-extern "C" int daam_finalize(const daam_key_group* groups, int32_t n_groups, int32_t x, int32_t n_rows,
-                             int32_t normalize, float* out, void* stream_) {
-  return finalize_impl("daam_finalize", groups, n_groups, x, x, n_rows, normalize, out,
-                       static_cast<cudaStream_t>(stream_));
-}
-
-extern "C" int daam_finalize_rect(const daam_key_group* groups, int32_t n_groups, int32_t map_h, int32_t map_w,
-                                  int32_t n_rows, int32_t normalize, float* out, void* stream_) {
-  return finalize_impl("daam_finalize_rect", groups, n_groups, map_h, map_w, n_rows, normalize, out,
-                       static_cast<cudaStream_t>(stream_));
-}
-
-static int finalize_per_key_impl(const char* name, const daam_key_group* groups, int32_t n_groups, int32_t oh, int32_t ow,
-                                 int32_t n_rows, int32_t normalize, float* out, cudaStream_t stream) {
-  if (!groups || !out || oh <= 0 || ow <= 0 || n_rows <= 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
-  if (n_groups <= 0) { set_error("%s: no key selected", name); return DAAM_E_INVALID; }
-  if (n_groups > kMaxGroups) { set_error("%s: %d key groups > %d", name, n_groups, kMaxGroups); return DAAM_E_UNSUPPORTED; }
+extern "C" int daam_finalize_per_key(const daam_key_group* groups, int32_t n_groups, int32_t oh, int32_t ow,
+                                     int32_t n_rows, int32_t normalize, float* out, void* stream_) {
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DeviceInfo dev;
-  if (int rc = get_device_info(&dev)) return rc;
   static thread_local PerKeyParams p;
-  p.n_groups = n_groups; p.oh = oh; p.ow = ow; p.n_rows = n_rows; p.n_keys = 0;
-  for (int i = 0; i < n_groups; ++i) {
-    const daam_key_group& g = groups[i];
-    if (!g.acc || g.heads <= 0 || g.h <= 0 || g.w <= 0 || g.tokens < n_rows || g.head_sel >= g.heads) {
-      set_error("%s: bad key group %d", name, i);
-      return DAAM_E_INVALID;
-    }
-    p.g[i] = g;
-    p.first_key[i] = p.n_keys;
-    p.n_keys += g.head_sel < 0 ? g.heads : 1;
+  if (int rc = check_key_groups("daam_finalize_per_key", groups, n_groups, oh, ow, n_rows, out, &dev, &p.n_keys)) return rc;
+  if (p.n_keys > 65535) { set_error("daam_finalize_per_key: %d keys > 65535", p.n_keys); return DAAM_E_UNSUPPORTED; }
+  p.n_groups = n_groups; p.oh = oh; p.ow = ow; p.n_rows = n_rows;
+  for (int i = 0, first = 0; i < n_groups; ++i) {
+    p.g[i] = groups[i];
+    p.first_key[i] = first;
+    first += groups[i].head_sel < 0 ? groups[i].heads : 1;
   }
   p.first_key[n_groups] = p.n_keys;
-  if (p.n_keys > 65535) { set_error("%s: %d keys > 65535", name, p.n_keys); return DAAM_E_UNSUPPORTED; }
   const int xx = oh * ow;
   dim3 grid((xx + 255) / 256, n_rows, p.n_keys);
   finalize_per_key_kernel<<<grid, 256, 0, stream>>>(p, out);
@@ -665,46 +654,23 @@ static int finalize_per_key_impl(const char* name, const daam_key_group* groups,
   return DAAM_OK;
 }
 
-extern "C" int daam_finalize_per_key(const daam_key_group* groups, int32_t n_groups, int32_t x, int32_t n_rows,
-                                     int32_t normalize, float* out, void* stream_) {
-  return finalize_per_key_impl("daam_finalize_per_key", groups, n_groups, x, x, n_rows, normalize, out,
-                               static_cast<cudaStream_t>(stream_));
-}
-
-extern "C" int daam_finalize_per_key_rect(const daam_key_group* groups, int32_t n_groups, int32_t map_h, int32_t map_w,
-                                          int32_t n_rows, int32_t normalize, float* out, void* stream_) {
-  return finalize_per_key_impl("daam_finalize_per_key_rect", groups, n_groups, map_h, map_w, n_rows, normalize, out,
-                               static_cast<cudaStream_t>(stream_));
-}
-
-static int normalize_maps_impl(const char* name, float* maps, int32_t n_maps, int32_t n_rows, int32_t mh, int32_t mw,
-                               cudaStream_t stream) {
-  if (!maps || n_maps < 0 || n_rows <= 0 || mh <= 0 || mw <= 0) { set_error("%s: null pointer or bad size", name); return DAAM_E_INVALID; }
-  if (n_maps > 65535) { set_error("%s: %d maps > 65535", name, n_maps); return DAAM_E_UNSUPPORTED; }
+extern "C" int daam_normalize_maps(float* maps, int32_t n_maps, int32_t n_rows, int32_t mh, int32_t mw, void* stream_) {
+  if (!maps || n_maps < 0 || n_rows <= 0 || mh <= 0 || mw <= 0) { set_error("daam_normalize_maps: null pointer or bad size"); return DAAM_E_INVALID; }
+  if (n_maps > 65535) { set_error("daam_normalize_maps: %d maps > 65535", n_maps); return DAAM_E_UNSUPPORTED; }
   if (n_maps == 0) return DAAM_OK;
   DeviceInfo dev;
   if (int rc = get_device_info(&dev)) return rc;
   const int xx = mh * mw;
-  normalize_kernel<<<dim3((xx + 255) / 256, n_maps), 256, 0, stream>>>(maps, n_rows, xx);
+  normalize_kernel<<<dim3((xx + 255) / 256, n_maps), 256, 0, static_cast<cudaStream_t>(stream_)>>>(maps, n_rows, xx);
   DAAM_CUDA_TRY(cudaGetLastError());
   count_launch();
   return DAAM_OK;
 }
 
-extern "C" int daam_normalize_maps(float* maps, int32_t n_maps, int32_t n_rows, int32_t x, void* stream_) {
-  return normalize_maps_impl("daam_normalize_maps", maps, n_maps, n_rows, x, x, static_cast<cudaStream_t>(stream_));
-}
-
-extern "C" int daam_normalize_maps_rect(float* maps, int32_t n_maps, int32_t n_rows, int32_t map_h, int32_t map_w,
-                                        void* stream_) {
-  return normalize_maps_impl("daam_normalize_maps_rect", maps, n_maps, n_rows, map_h, map_w,
-                             static_cast<cudaStream_t>(stream_));
-}
-
-static int word_heat_map_impl(const char* name, const float* global_maps, int32_t n_rows, int32_t mh, int32_t mw,
-                              const int32_t* rows, int32_t n_sel, float* out, cudaStream_t stream) {
-  if (!global_maps || !rows || !out || mh <= 0 || mw <= 0 || n_sel <= 0) { set_error("%s: null pointer or empty selection", name); return DAAM_E_INVALID; }
-  if (n_sel > kMaxRows) { set_error("%s: %d rows > %d", name, n_sel, kMaxRows); return DAAM_E_UNSUPPORTED; }
+extern "C" int daam_word_heat_map(const float* global_maps, int32_t n_rows, int32_t mh, int32_t mw, const int32_t* rows,
+                                  int32_t n_sel, float* out, void* stream_) {
+  if (!global_maps || !rows || !out || mh <= 0 || mw <= 0 || n_sel <= 0) { set_error("daam_word_heat_map: null pointer or empty selection"); return DAAM_E_INVALID; }
+  if (n_sel > kMaxRows) { set_error("daam_word_heat_map: %d rows > %d", n_sel, kMaxRows); return DAAM_E_UNSUPPORTED; }
   DeviceInfo dev;
   if (int rc = get_device_info(&dev)) return rc;
   RowSel sel;
@@ -712,26 +678,14 @@ static int word_heat_map_impl(const char* name, const float* global_maps, int32_
   for (int i = 0; i < n_sel; ++i) {
     int r = rows[i];
     if (r < 0) r += n_rows;   // torch-style negative index
-    if (r < 0 || r >= n_rows) { set_error("%s: row %d out of range [0, %d)", name, rows[i], n_rows); return DAAM_E_INVALID; }
+    if (r < 0 || r >= n_rows) { set_error("daam_word_heat_map: row %d out of range [0, %d)", rows[i], n_rows); return DAAM_E_INVALID; }
     sel.rows[i] = r;
   }
   const int xx = mh * mw;
-  word_map_kernel<<<(xx + 255) / 256, 256, 0, stream>>>(global_maps, sel, xx, out);
+  word_map_kernel<<<(xx + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream_)>>>(global_maps, sel, xx, out);
   DAAM_CUDA_TRY(cudaGetLastError());
   count_launch();
   return DAAM_OK;
-}
-
-extern "C" int daam_word_heat_map(const float* global_maps, int32_t n_rows, int32_t x, const int32_t* rows,
-                                  int32_t n_sel, float* out, void* stream_) {
-  return word_heat_map_impl("daam_word_heat_map", global_maps, n_rows, x, x, rows, n_sel, out,
-                            static_cast<cudaStream_t>(stream_));
-}
-
-extern "C" int daam_word_heat_map_rect(const float* global_maps, int32_t n_rows, int32_t map_h, int32_t map_w,
-                                       const int32_t* rows, int32_t n_sel, float* out, void* stream_) {
-  return word_heat_map_impl("daam_word_heat_map_rect", global_maps, n_rows, map_h, map_w, rows, n_sel, out,
-                            static_cast<cudaStream_t>(stream_));
 }
 
 static int launch_expand_words(ExpandWordsParams& p, const DeviceInfo& dev, cudaStream_t stream) {
@@ -782,19 +736,16 @@ static int launch_expand_words(ExpandWordsParams& p, const DeviceInfo& dev, cuda
   return DAAM_OK;
 }
 
+// behind daam_expand_words and daam_expand_as; `name` is the entry point that was called
 static int expand_words_impl(const char* name, const float* global_maps, int32_t n_rows, int32_t mh, int32_t mw,
                              const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w,
                              int32_t absolute, int32_t use_threshold, float threshold, float* word_maps, float* out,
-                             float* scratch, cudaStream_t stream) {
+                             float* scratch, void* stream) {
   if (!global_maps || !rows || !row_begin || !out || !scratch || mh <= 0 || mw <= 0 || out_h <= 0 || out_w <= 0 || n_rows <= 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
   if (n_words <= 0) { set_error("%s: empty word list", name); return DAAM_E_INVALID; }
   if (n_words > kMaxWords) { set_error("%s: %d words > %d", name, n_words, kMaxWords); return DAAM_E_UNSUPPORTED; }
   if (row_begin[0] != 0 || row_begin[n_words] > kMaxWordRows) { set_error("%s: row_begin must start at 0 and select at most %d rows", name, kMaxWordRows); return DAAM_E_UNSUPPORTED; }
-  if ((size_t)mh * mw * sizeof(float) > 200 * 1024) {
-    if (mh == mw) set_error("%s: x = %d does not fit shared memory", name, mh);
-    else set_error("%s: a %d x %d map does not fit shared memory", name, mh, mw);
-    return DAAM_E_UNSUPPORTED;
-  }
+  if ((size_t)mh * mw * sizeof(float) > 200 * 1024) { set_error("%s: a %d x %d map does not fit shared memory", name, mh, mw); return DAAM_E_UNSUPPORTED; }
   DeviceInfo dev;
   if (int rc = get_device_info(&dev)) return rc;
   static thread_local ExpandWordsParams p;
@@ -812,46 +763,22 @@ static int expand_words_impl(const char* name, const float* global_maps, int32_t
     if (r < 0 || r >= n_rows) { set_error("%s: row %d out of range [0, %d)", name, rows[i], n_rows); return DAAM_E_INVALID; }
     p.rows[i] = r;
   }
-  return launch_expand_words(p, dev, stream);
+  return launch_expand_words(p, dev, static_cast<cudaStream_t>(stream));
 }
 
-extern "C" int daam_expand_words(const float* global_maps, int32_t n_rows, int32_t x, const int32_t* rows,
+extern "C" int daam_expand_words(const float* global_maps, int32_t n_rows, int32_t mh, int32_t mw, const int32_t* rows,
                                  const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w,
                                  int32_t absolute, int32_t use_threshold, float threshold, float* word_maps, float* out,
-                                 float* scratch, void* stream_) {
-  return expand_words_impl("daam_expand_words", global_maps, n_rows, x, x, rows, row_begin, n_words, out_h, out_w,
-                           absolute, use_threshold, threshold, word_maps, out, scratch, static_cast<cudaStream_t>(stream_));
+                                 float* scratch, void* stream) {
+  return expand_words_impl("daam_expand_words", global_maps, n_rows, mh, mw, rows, row_begin, n_words, out_h, out_w,
+                           absolute, use_threshold, threshold, word_maps, out, scratch, stream);
 }
 
-extern "C" int daam_expand_words_rect(const float* global_maps, int32_t n_rows, int32_t map_h, int32_t map_w,
-                                      const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h,
-                                      int32_t out_w, int32_t absolute, int32_t use_threshold, float threshold,
-                                      float* word_maps, float* out, float* scratch, void* stream_) {
-  return expand_words_impl("daam_expand_words_rect", global_maps, n_rows, map_h, map_w, rows, row_begin, n_words, out_h,
-                           out_w, absolute, use_threshold, threshold, word_maps, out, scratch,
-                           static_cast<cudaStream_t>(stream_));
-}
-
-// one word whose "rows" are the word map itself; `self` names the entry point in the null-pointer message, `inner` in
-// the checks shared with expand_words (the square pair has always reported those as daam_expand_words)
-static int expand_as_impl(const char* self, const char* inner, const float* word_map, int32_t mh, int32_t mw,
-                          int32_t out_h, int32_t out_w, int32_t absolute, int32_t use_threshold, float threshold,
-                          float* out, float* scratch, void* stream_) {
+// one word whose "rows" are the word map itself
+extern "C" int daam_expand_as(const float* word_map, int32_t mh, int32_t mw, int32_t out_h, int32_t out_w,
+                              int32_t absolute, int32_t use_threshold, float threshold, float* out, float* scratch,
+                              void* stream) {
   const int32_t rows[1] = {0}, row_begin[2] = {0, 1};
-  if (!word_map) { set_error("%s: null pointer or non-positive size", self); return DAAM_E_INVALID; }
-  return expand_words_impl(inner, word_map, 1, mh, mw, rows, row_begin, 1, out_h, out_w, absolute, use_threshold,
-                           threshold, nullptr, out, scratch, static_cast<cudaStream_t>(stream_));
-}
-
-extern "C" int daam_expand_as(const float* word_map, int32_t x, int32_t out_h, int32_t out_w, int32_t absolute,
-                              int32_t use_threshold, float threshold, float* out, float* scratch, void* stream_) {
-  return expand_as_impl("daam_expand_as", "daam_expand_words", word_map, x, x, out_h, out_w, absolute, use_threshold,
-                        threshold, out, scratch, stream_);
-}
-
-extern "C" int daam_expand_as_rect(const float* word_map, int32_t map_h, int32_t map_w, int32_t out_h, int32_t out_w,
-                                   int32_t absolute, int32_t use_threshold, float threshold, float* out, float* scratch,
-                                   void* stream_) {
-  return expand_as_impl("daam_expand_as_rect", "daam_expand_as_rect", word_map, map_h, map_w, out_h, out_w, absolute,
-                        use_threshold, threshold, out, scratch, stream_);
+  return expand_words_impl("daam_expand_as", word_map, 1, mh, mw, rows, row_begin, 1, out_h, out_w, absolute,
+                           use_threshold, threshold, nullptr, out, scratch, stream);
 }

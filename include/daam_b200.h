@@ -24,10 +24,11 @@
 extern "C" {
 #endif
 
-#define DAAM_ABI_VERSION 3          /* 2: + daam_attention_probs, daam_accumulate_probs, daam_finalize_per_key
+#define DAAM_ABI_VERSION 4          /* 2: + daam_attention_probs, daam_accumulate_probs, daam_finalize_per_key
                                        3: + DAAM_ACC_EARLY_LOADS, daam_expand_words, daam_side_launcher_*
                                           (later, additive: daam_accumulate_steps, daam_normalize_maps,
-                                          daam_accumulate_range) */
+                                          daam_accumulate_range)
+                                       4: the finalize family takes (map_h, map_w); the _rect names are gone */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
 
@@ -173,111 +174,72 @@ typedef struct daam_key_group {
 
 /*
  * Replaces DiffusionHeatMapHooker.compute_global_heat_map (daam/trace.py:83-132) after its Python-side key filter:
- * per selected key bicubic upsample (align_corners=False, A=-0.75, no antialias) to (x, x), clamp(min=0), mean over
- * the keys, keep rows [0, n_rows), and if `normalize` divide by (sum of rows 1..n_rows-2 + 1e-6) per pixel.
- * out: device fp32 [n_rows][x][x]. `groups` is host memory. Fails with DAAM_E_INVALID when no key is selected (the
- * host turns that into the reference's "No heat maps found" RuntimeError, trace.py:120-124).
+ * per selected key bicubic upsample (align_corners=False, A=-0.75, no antialias) to the [map_h][map_w] grid, taps key
+ * h -> map_h and key w -> map_w, clamp(min=0), mean over the keys, keep rows [0, n_rows), and if `normalize` divide by
+ * (sum of rows 1..n_rows-2 + 1e-6) per pixel. out: device fp32 [n_rows][map_h][map_w]. `groups` is host memory, at most
+ * 160 groups. Fails with DAAM_E_INVALID when no key is selected (the host turns that into the reference's "No heat maps
+ * found" RuntimeError, trace.py:120-124).
+ * The banded fast kernel runs when every key has one integer factor 1, 2 or 4 on both axes and a 16-byte-aligned base
+ * (aligned slab, h * w a multiple of 4), map_w <= 256, there are at most 8 key sizes and 2048 keys, and, for a square
+ * map only, side % 16 == 0; anything else, or DAAM_FINALIZE_GENERIC=1, runs the generic gather kernel (DESIGN.md
+ * section 4.3).
  */
-int daam_finalize(const daam_key_group* groups, int32_t n_groups, int32_t x, int32_t n_rows, int32_t normalize,
-                  float* out, void* stream);
-
-/*
- * daam_finalize to a rectangular [map_h][map_w] grid (non-square images): every key is bicubic-upsampled with taps
- * key h -> map_h and key w -> map_w, then clamp, mean and normalise as daam_finalize. out: device fp32
- * [n_rows][map_h][map_w]. daam_finalize(x) is exactly daam_finalize_rect(x, x). Keys with one integer factor 1, 2 or 4
- * on both axes and 16-byte-aligned bases (aligned slab, h * w a multiple of 4) run the banded fast kernel; anything
- * else, or DAAM_FINALIZE_GENERIC=1, runs the generic gather kernel (DESIGN.md section 4.3).
- */
-int daam_finalize_rect(const daam_key_group* groups, int32_t n_groups, int32_t map_h, int32_t map_w, int32_t n_rows,
-                       int32_t normalize, float* out, void* stream);
+int daam_finalize(const daam_key_group* groups, int32_t n_groups, int32_t map_h, int32_t map_w, int32_t n_rows,
+                  int32_t normalize, float* out, void* stream);
 
 /*
  * The reference's --all-heads sweep calls compute_global_heat_map(layer_idx=l, head_idx=h) once per (layer, head)
  * (daam/run/generate.py:239-255): each call reduces exactly one key, i.e. bicubic + clamp (+ normalise) of that key.
- * This entry point produces all of them in one launch: out [n_keys][n_rows][x][x] (device fp32), keys enumerated
- * group by group, head by head, in the order given.
+ * This entry point produces all of them in one launch: out [n_keys][n_rows][map_h][map_w] (device fp32), taps key
+ * h -> map_h and key w -> map_w, keys enumerated group by group, head by head, in the order given. Limits: 160 groups,
+ * 65535 keys.
  */
-int daam_finalize_per_key(const daam_key_group* groups, int32_t n_groups, int32_t x, int32_t n_rows, int32_t normalize,
-                          float* out, void* stream);
+int daam_finalize_per_key(const daam_key_group* groups, int32_t n_groups, int32_t map_h, int32_t map_w, int32_t n_rows,
+                          int32_t normalize, float* out, void* stream);
 
 /*
- * daam_finalize_per_key to a rectangular grid: out [n_keys][n_rows][map_h][map_w] (device fp32), taps key h -> map_h
- * and key w -> map_w. daam_finalize_per_key(x) is exactly daam_finalize_per_key_rect(x, x).
+ * The `normalize` step of daam_finalize on its own, in place, for n_maps <= 65535 independent [n_rows][map_h][map_w]
+ * heat maps stored back to back (e.g. the per-step global maps of a time-resolved trace): maps / (sum of rows
+ * 1..n_rows-2 + 1e-6) per pixel, the same arithmetic as daam_finalize(normalize = 1).
  */
-int daam_finalize_per_key_rect(const daam_key_group* groups, int32_t n_groups, int32_t map_h, int32_t map_w,
-                               int32_t n_rows, int32_t normalize, float* out, void* stream);
-
-/*
- * The `normalize` step of daam_finalize on its own, in place, for n_maps independent [n_rows][x][x] heat maps stored
- * back to back (e.g. the per-step global maps of a time-resolved trace): maps / (sum of rows 1..n_rows-2 + 1e-6) per
- * pixel, the same arithmetic as daam_finalize(normalize = 1).
- */
-int daam_normalize_maps(float* maps, int32_t n_maps, int32_t n_rows, int32_t x, void* stream);
-
-/*
- * daam_normalize_maps for n_maps [n_rows][map_h][map_w] heat maps stored back to back. daam_normalize_maps(x) is
- * exactly daam_normalize_maps_rect(x, x).
- */
-int daam_normalize_maps_rect(float* maps, int32_t n_maps, int32_t n_rows, int32_t map_h, int32_t map_w, void* stream);
+int daam_normalize_maps(float* maps, int32_t n_maps, int32_t n_rows, int32_t map_h, int32_t map_w, void* stream);
 
 /*
  * Replaces GlobalHeatMap.compute_word_heat_map's tensor part (daam/heatmap.py:121-123): mean over the rows
- * `rows[0..n_sel)` (host array, already offset by +1 for SOS as daam/utils.py:91 does) of global_maps [n_rows][x][x]
- * -> out [x][x] (both device fp32).
+ * `rows[0..n_sel)` (host array, n_sel <= 128, already offset by +1 for SOS as daam/utils.py:91 does) of global_maps
+ * [n_rows][map_h][map_w] -> out [map_h][map_w] (both device fp32).
  */
-int daam_word_heat_map(const float* global_maps, int32_t n_rows, int32_t x, const int32_t* rows, int32_t n_sel,
-                       float* out, void* stream);
+int daam_word_heat_map(const float* global_maps, int32_t n_rows, int32_t map_h, int32_t map_w, const int32_t* rows,
+                       int32_t n_sel, float* out, void* stream);
 
 /*
- * daam_word_heat_map of global_maps [n_rows][map_h][map_w] -> out [map_h][map_w]. daam_word_heat_map(x) is exactly
- * daam_word_heat_map_rect(x, x).
- */
-int daam_word_heat_map_rect(const float* global_maps, int32_t n_rows, int32_t map_h, int32_t map_w,
-                            const int32_t* rows, int32_t n_sel, float* out, void* stream);
-
-/*
- * Replaces WordHeatMap.expand_as's tensor part (daam/heatmap.py:77-93): bicubic upsample of word_map [x][x] to
- * [out_h][out_w], then unless `absolute` (im - min) / (max - min + 1e-8), then if `use_threshold` binarise
- * (im > threshold) (the reference's `if threshold:` -- Python truthiness -- is resolved by the host).
- * out: device fp32 [out_h][out_w]; scratch: device, >= DAAM_EXPAND_SCRATCH_FLOATS floats, owned by the caller.
- * One launch (the n_words = 1 case of daam_expand_words).
+ * Replaces WordHeatMap.expand_as's tensor part (daam/heatmap.py:77-93): bicubic upsample of word_map [map_h][map_w] to
+ * [out_h][out_w], taps map_h -> out_h and map_w -> out_w, then unless `absolute` (im - min) / (max - min + 1e-8), then
+ * if `use_threshold` binarise (im > threshold) (the reference's `if threshold:` -- Python truthiness -- is resolved by
+ * the host). out: device fp32 [out_h][out_w]; scratch: device, >= DAAM_EXPAND_SCRATCH_FLOATS floats, owned by the
+ * caller. Limit: map_h * map_w * 4 bytes <= 200 KB (the map lives in shared memory). One launch (the n_words = 1 case
+ * of daam_expand_words).
  */
 #define DAAM_EXPAND_SCRATCH_FLOATS 64   /* per word: partial min/max of up to 32 pixel chunks */
-int daam_expand_as(const float* word_map, int32_t x, int32_t out_h, int32_t out_w, int32_t absolute,
+int daam_expand_as(const float* word_map, int32_t map_h, int32_t map_w, int32_t out_h, int32_t out_w, int32_t absolute,
                    int32_t use_threshold, float threshold, float* out, float* scratch, void* stream);
-
-/*
- * daam_expand_as of a rectangular word_map [map_h][map_w]: taps map_h -> out_h and map_w -> out_w. Limit:
- * map_h * map_w * 4 bytes <= 200 KB (the map lives in shared memory). daam_expand_as(x) is exactly
- * daam_expand_as_rect(x, x).
- */
-int daam_expand_as_rect(const float* word_map, int32_t map_h, int32_t map_w, int32_t out_h, int32_t out_w,
-                        int32_t absolute, int32_t use_threshold, float threshold, float* out, float* scratch,
-                        void* stream);
 
 /*
  * The per-word loop a user of the reference writes -- `for word in prompt: global_heat_map.compute_word_heat_map(word)
  * .expand_as(image)` (daam/heatmap.py:121-123 then :77-93; e.g. daam/run/generate.py, the README example) -- for a LIST
  * of words in one cooperative launch: word w averages rows[row_begin[w] .. row_begin[w+1]) of global_maps
- * [n_rows][x][x] (rows already offset by +1 for SOS, daam/utils.py:91), the [x][x] mean is bicubic-upsampled to
- * [out_h][out_w], min-max normalised unless `absolute`, binarised if `use_threshold`.
- * out: device fp32 [n_words][out_h][out_w]; word_maps: optional device fp32 [n_words][x][x] (the word heat maps
+ * [n_rows][map_h][map_w] (rows already offset by +1 for SOS, daam/utils.py:91), the [map_h][map_w] mean is
+ * bicubic-upsampled to [out_h][out_w] (taps map_h -> out_h and map_w -> out_w), min-max normalised unless `absolute`,
+ * binarised if `use_threshold`.
+ * out: device fp32 [n_words][out_h][out_w]; word_maps: optional device fp32 [n_words][map_h][map_w] (the word heat maps
  * themselves, NULL to skip); scratch: device, >= DAAM_EXPAND_SCRATCH_FLOATS * n_words floats; rows / row_begin: host.
- * Limits: n_words <= 96, row_begin[n_words] <= 320. Nothing is copied to the host: the caller reads `out` back once.
+ * Limits: n_words <= 96, row_begin[n_words] <= 320, map_h * map_w * 4 bytes <= 200 KB. Nothing is copied to the host:
+ * the caller reads `out` back once.
  */
-int daam_expand_words(const float* global_maps, int32_t n_rows, int32_t x, const int32_t* rows, const int32_t* row_begin,
-                      int32_t n_words, int32_t out_h, int32_t out_w, int32_t absolute, int32_t use_threshold,
-                      float threshold, float* word_maps, float* out, float* scratch, void* stream);
-
-/*
- * daam_expand_words over rectangular global_maps [n_rows][map_h][map_w]: word maps [n_words][map_h][map_w], taps
- * map_h -> out_h and map_w -> out_w, out [n_words][out_h][out_w]. Same limits as daam_expand_words plus map_h * map_w *
- * 4 bytes <= 200 KB. daam_expand_words(x) is exactly daam_expand_words_rect(x, x).
- */
-int daam_expand_words_rect(const float* global_maps, int32_t n_rows, int32_t map_h, int32_t map_w, const int32_t* rows,
-                           const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w, int32_t absolute,
-                           int32_t use_threshold, float threshold, float* word_maps, float* out, float* scratch,
-                           void* stream);
+int daam_expand_words(const float* global_maps, int32_t n_rows, int32_t map_h, int32_t map_w, const int32_t* rows,
+                      const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w, int32_t absolute,
+                      int32_t use_threshold, float threshold, float* word_maps, float* out, float* scratch,
+                      void* stream);
 
 /* Library / device introspection. */
 int daam_abi_version(void);

@@ -32,10 +32,13 @@ def test_header_and_binding_agree():
     assert declared_functions() == sorted(_native.EXPORTS)
 
 
-def test_every_declared_symbol_is_exported(lib):
+def test_every_declared_symbol_is_exported_at_abi_4(lib):
     for name in declared_functions():
         assert hasattr(lib, name), f'{name} declared in include/daam_b200.h but not exported'
-    assert _native.abi_version() == _native.ABI_VERSION == 3
+    assert _native.abi_version() == _native.ABI_VERSION == 4
+    for name in ('daam_finalize', 'daam_finalize_per_key', 'daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as',
+                 'daam_expand_words'):   # one entry point per operation, no `_rect` twin
+        assert not hasattr(lib, name + '_rect'), f'{name}_rect is still exported'
 
 
 def test_struct_layout_matches_the_header():

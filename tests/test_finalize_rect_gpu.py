@@ -1,10 +1,8 @@
-"""The rectangular finalize / word-map / expand entry points (``daam_*_rect``) against float64 torch: every key as
-``B_y @ key @ B_x^T`` with ``bicubic64(kh, xh)`` / ``bicubic64(kw, xw)``, then clamp, mean and normalise, within the
-finalize tolerances of ``test_production_sizes_gpu.py``. Fast and generic kernels, the grids of SD-2.1 at 512x768 /
+"""The finalize / word-map / expand entry points on rectangular ``(map_h, map_w)`` grids against float64 torch: every
+key as ``B_y @ key @ B_x^T`` with ``bicubic64(kh, xh)`` / ``bicubic64(kw, xw)``, then clamp, mean and normalise, within
+the finalize tolerances of ``test_production_sizes_gpu.py``. Fast and generic kernels, the grids of SD-2.1 at 512x768 /
 768x512 and SDXL at 1216x832 / 1344x768 / 1152x896 (26-wide key rows), a 13-wide key row, an odd grid that falls back,
-and square calls through the ``_rect`` entry points bit-equal to the square ones."""
-import ctypes
-
+and the refusals, which name the entry point that was called."""
 import pytest
 import torch
 
@@ -161,68 +159,15 @@ def test_word_maps_and_expand_words_rect(grid, out_hw):
             assert torch.equal(single, out[i]), f'{what}: expand_as differs from expand_words'
 
 
-def _lib():
-    return _native.load()
-
-
-def test_square_calls_through_rect_are_bit_equal(monkeypatch):
-    """Every square entry point against its ``_rect`` sibling at (x, x): same bits (one implementation)."""
-    lib = _lib()
-    g = torch.Generator(device=DEV).manual_seed(9)
-    x, n_rows = 64, 40
-    stacks = [torch.exp(torch.randn(h, 77, s, s, generator=g, device=DEV)) for s, h in ((64, 5), (32, 10), (16, 20))]
-    groups = _groups(stacks)
-    arr = (_native.DaamKeyGroup * len(groups))(*groups)
-    stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    for generic in (False, True):
-        monkeypatch.setenv('DAAM_FINALIZE_GENERIC', '1' if generic else '0')
-        for normalize in (0, 1):
-            a, b = torch.empty(n_rows, x, x, device=DEV), torch.empty(n_rows, x, x, device=DEV)
-            assert lib.daam_finalize(arr, len(groups), x, n_rows, normalize, ctypes.c_void_p(a.data_ptr()), stream) == 0
-            assert lib.daam_finalize_rect(arr, len(groups), x, x, n_rows, normalize, ctypes.c_void_p(b.data_ptr()),
-                                          stream) == 0
-            torch.cuda.synchronize()
-            assert torch.equal(_bits(a), _bits(b))
-    a, b = torch.empty(35, n_rows, x, x, device=DEV), torch.empty(35, n_rows, x, x, device=DEV)
-    assert lib.daam_finalize_per_key(arr, len(groups), x, n_rows, 1, ctypes.c_void_p(a.data_ptr()), stream) == 0
-    assert lib.daam_finalize_per_key_rect(arr, len(groups), x, x, n_rows, 1, ctypes.c_void_p(b.data_ptr()), stream) == 0
-    torch.cuda.synchronize()
-    assert torch.equal(_bits(a), _bits(b))
-    maps = torch.rand(3, n_rows, x, x, generator=g, device=DEV)
-    a, b = maps.clone(), maps.clone()
-    assert lib.daam_normalize_maps(ctypes.c_void_p(a.data_ptr()), 3, n_rows, x, stream) == 0
-    assert lib.daam_normalize_maps_rect(ctypes.c_void_p(b.data_ptr()), 3, n_rows, x, x, stream) == 0
-    rows = (ctypes.c_int32 * 2)(2, 3)
-    begin = (ctypes.c_int32 * 3)(0, 1, 2)
-    wa, wb = torch.empty(x, x, device=DEV), torch.empty(x, x, device=DEV)
-    assert lib.daam_word_heat_map(ctypes.c_void_p(maps.data_ptr()), n_rows, x, rows, 2, ctypes.c_void_p(wa.data_ptr()),
-                                  stream) == 0
-    assert lib.daam_word_heat_map_rect(ctypes.c_void_p(maps.data_ptr()), n_rows, x, x, rows, 2,
-                                       ctypes.c_void_p(wb.data_ptr()), stream) == 0
-    ea, eb = torch.empty(2, 512, 512, device=DEV), torch.empty(2, 512, 512, device=DEV)
-    scratch = torch.empty(4 * _native.EXPAND_SCRATCH_FLOATS, device=DEV)
-    sp = ctypes.c_void_p(scratch.data_ptr())
-    assert lib.daam_expand_words(ctypes.c_void_p(maps.data_ptr()), n_rows, x, rows, begin, 2, 512, 512, 0, 0,
-                                 ctypes.c_float(0.0), None, ctypes.c_void_p(ea.data_ptr()), sp, stream) == 0
-    assert lib.daam_expand_words_rect(ctypes.c_void_p(maps.data_ptr()), n_rows, x, x, rows, begin, 2, 512, 512, 0, 0,
-                                      ctypes.c_float(0.0), None, ctypes.c_void_p(eb.data_ptr()), sp, stream) == 0
-    xa, xb = torch.empty(512, 512, device=DEV), torch.empty(512, 512, device=DEV)
-    assert lib.daam_expand_as(ctypes.c_void_p(wa.data_ptr()), x, 512, 512, 0, 1, ctypes.c_float(0.4),
-                              ctypes.c_void_p(xa.data_ptr()), sp, stream) == 0
-    assert lib.daam_expand_as_rect(ctypes.c_void_p(wa.data_ptr()), x, x, 512, 512, 0, 1, ctypes.c_float(0.4),
-                                   ctypes.c_void_p(xb.data_ptr()), sp, stream) == 0
-    torch.cuda.synchronize()
-    for u, v in ((a, b), (wa, wb), (ea, eb), (xa, xb)):
-        assert torch.equal(_bits(u), _bits(v))
-
-
-def test_rect_refusals():
+def test_refusals_name_the_entry_point_called():
     stream = torch.cuda.current_stream().cuda_stream
     maps = torch.zeros(3, 300, 200, device=DEV)
     out = torch.empty(2, 8, 8, device=DEV)
     scratch = torch.empty(64, device=DEV)
-    with pytest.raises(_native.NativeError, match='daam_expand_words_rect: a 300 x 200 map does not fit shared memory'):
+    with pytest.raises(_native.NativeError, match='daam_expand_words: a 300 x 200 map does not fit shared memory'):
         _native.expand_words(maps.data_ptr(), 3, (300, 200), [[1]], 8, 8, False, None, None, out.data_ptr(),
                              scratch.data_ptr(), stream)
-    with pytest.raises(_native.NativeError, match='daam_finalize_rect: null pointer or non-positive size'):
+    with pytest.raises(_native.NativeError, match='daam_expand_as: a 300 x 200 map does not fit shared memory'):
+        _native.expand_as(maps.data_ptr(), (300, 200), 8, 8, False, None, out.data_ptr(), scratch.data_ptr(), stream)
+    with pytest.raises(_native.NativeError, match='daam_finalize: null pointer or non-positive size'):
         _native.finalize(_groups([torch.zeros(1, 77, 4, 4, device=DEV)]), (0, 4), 2, False, out.data_ptr(), stream)
