@@ -12,8 +12,11 @@
 //              block in by TMA, up to kAccStages tiles ahead, and one bulk-tensor store writes it back. The accumulator
 //              is read from HBM well before the tile needs it, and the SM never waits for an L2 read-modify-write.
 // Warp roles: 0-7 consumers (two warpgroups: MMA + softmax + accumulate), 8 Q/K TMA producer (one elected thread) that
-// runs up to two K chunks ahead through a two-stage ring, 9 accumulator loader (one elected thread). Persistent: every
-// CTA walks a contiguous chunk of the launch's tiles, one CTA per SM (the rings fill its shared memory).
+// runs up to two K chunks ahead through a two-stage ring, 9 accumulator loader (one elected thread). Persistent, one CTA
+// per SM (the rings fill its shared memory): in the single-chunk 16-bit instances CTA b takes tiles b, b + grid, ...,
+// so the tiles in flight at any moment are consecutive (whole accumulator rows and the heads of a Q row move together);
+// the others walk contiguous chunks of the launch's tiles. Accumulator loads and stores carry an L2 evict_first hint:
+// each block is read and written once per launch, and the hint keeps them from pushing out the Q/K lines below.
 //
 // fp32 projections (the reference's default dtype for SD-1.x/2.x, daam/run/generate.py:205) take the same kernel in
 // "split" form. Tensor cores have no fp32 operand type and a plain tf32 product would drop 13 mantissa bits, so every
@@ -62,6 +65,7 @@ namespace {
 
 constexpr int kStages = 2;                            // Q/K chunk ring
 constexpr int kAccStages = 3;                         // 16-bit form: accumulator tile ring
+constexpr int kPrefetchTiles = 6;                     // 16-bit form, early loads: tiles whose Q/K go to L2 before the wait
 constexpr int kQBytes = kTilePixels * 128;            // 128 rows x 128 B (64 x 16-bit, or 32 x fp32: one swizzle span)
 constexpr int kKBytes = kTokensPad * 128;             // 80 rows x 128 B
 constexpr int kStageBytes = kQBytes + kKBytes;        // 26624 = 26 x 1024 (keeps every tile 1024-byte aligned)
@@ -146,12 +150,6 @@ __device__ __forceinline__ void tma_load_4d(const CUtensorMap* map, uint32_t bar
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
-__device__ __forceinline__ void tma_load_2d(const CUtensorMap* map, uint32_t bar, uint32_t dst, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1)
-      : "memory");
-}
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
                    reinterpret_cast<uint64_t>(map)),
@@ -162,6 +160,37 @@ __device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* map, uint32
   asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
                    reinterpret_cast<uint64_t>(map)),
                "r"(src), "r"(c0), "r"(c1)
+               : "memory");
+}
+// L2 eviction-priority policies for the .L2::cache_hint forms below
+__device__ __forceinline__ uint64_t l2_evict_last() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+__device__ __forceinline__ uint64_t l2_evict_first() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
+// The box a tma_load_4d with the same coordinates would fetch, into L2 only (no shared memory, no barrier)
+__device__ __forceinline__ void tma_prefetch_4d(const CUtensorMap* map, int c0, int c1, int c2, int c3, uint64_t pol) {
+  asm volatile("cp.async.bulk.prefetch.tensor.4d.L2.global.tile.L2::cache_hint [%0, {%1, %2, %3, %4}], %5;"
+               ::"l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "l"(pol)
+               : "memory");
+}
+__device__ __forceinline__ void tma_load_2d_hint(const CUtensorMap* map, uint32_t bar, uint32_t dst, int c0, int c1,
+                                                 uint64_t pol) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4}], "
+      "[%2], %5;"
+      ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(bar), "r"(c0), "r"(c1), "l"(pol)
+      : "memory");
+}
+__device__ __forceinline__ void tma_store_2d_hint(const CUtensorMap* map, uint32_t src, int c0, int c1, uint64_t pol) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3}], [%1], %4;" ::"l"(
+                   reinterpret_cast<uint64_t>(map)),
+               "r"(src), "r"(c0), "r"(c1), "l"(pol)
                : "memory");
 }
 __device__ __forceinline__ void prefetch_tensormap(const CUtensorMap* map) {
@@ -318,8 +347,12 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP)
   const uint32_t afull0 = bars + 16 * kStages, aempty0 = afull0 + 8 * kAccStages;   // accumulator ring (16-bit form)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  int first, count;
-  if constexpr (!kChunked) {                           // equal tiles: contiguous ranges of per / per + 1 tiles
+  int first, count, stride = 1;                        // the CTA's tiles: first + i * stride, i < count (increasing)
+  if constexpr (!kChunked && !kSplit) {               // equal tiles, interleaved: the grid works on consecutive tiles
+    first = blockIdx.x;
+    stride = gridDim.x;
+    count = (P.total_tiles - (int)blockIdx.x + stride - 1) / stride;
+  } else if constexpr (!kChunked) {                    // equal tiles: contiguous ranges of per / per + 1 tiles
     const int per = P.total_tiles / gridDim.x, rem = P.total_tiles % gridDim.x;
     first = blockIdx.x * per + min((int)blockIdx.x, rem);
     count = per + ((int)blockIdx.x < rem ? 1 : 0);
@@ -360,7 +393,9 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP)
   // previous kernel on the stream. By default nothing below starts before that kernel has completed and flushed.
   // With `early_loads` (the caller vouches that Q/K were complete before the previous kernel started, DAAM_ACC_EARLY_LOADS)
   // only the accumulator traffic waits (16-bit form: the accumulator loader's first load; split form: the first
-  // reduce): Q/K loads, MMAs and the first tiles' softmax overlap the previous kernel's tail.
+  // reduce): Q/K loads, MMAs and the first tiles' softmax overlap the previous kernel's tail. The same promise makes
+  // the 16-bit producer's L2 prefetch of its next tiles' Q/K legal before the wait: the previous kernel only writes
+  // accumulators, so those bytes are final, and a prefetch reads nothing into shared memory that could go stale.
   // Our own dependents may be scheduled as soon as every CTA of this grid is past this point.
   if (!P.early_loads) griddep_wait();
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
@@ -370,14 +405,15 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP)
     if constexpr (!kSplit) {
       if (lane == 0 && count > 0) {
         if (P.early_loads) griddep_wait();           // everything the previous kernel added is complete and visible
+        const uint64_t pol = l2_evict_first();
         int li = 0;
         for (int i = 0; i < count; ++i) {
-          const Tile t = decode_tile(P, first + i, li);
+          const Tile t = decode_tile(P, first + i * stride, li);
           const int a = i % kAccStages;
           mbar_wait(aempty0 + 8 * a, ((uint32_t)(i / kAccStages) & 1u) ^ 1u);     // its previous tile's store has read it
           mbar_expect_tx(afull0 + 8 * a, kPBytes);   // (a partial tile's out-of-range pixels land as zeros)
-          tma_load_2d(&MP.amap[t.li], afull0 + 8 * a, sP_u32 + a * kPBytes, t.pixel0,
-                      (t.prompt * P.layer[t.li].heads + t.head) * kTokens);
+          tma_load_2d_hint(&MP.amap[t.li], afull0 + 8 * a, sP_u32 + a * kPBytes, t.pixel0,
+                           (t.prompt * P.layer[t.li].heads + t.head) * kTokens, pol);
         }
       }
     }
@@ -386,7 +422,26 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP)
     if (lane == 0) {
       int li = 0, j = 0;
       for (int i = 0; i < count; ++i) {
-        const Tile t = decode_tile(P, first + i, li);
+        if (!kSplit && P.early_loads && i == (kChunked ? 1 : kStages)) {
+          // the first tiles' stages are loaded; before waiting for a free stage (and, on a CTA that starts early, for
+          // the previous launch), pull the Q boxes of the next kPrefetchTiles tiles and the K box of every new head
+          // into L2 at evict_last priority, with the coordinates of the loads that will read them
+          const uint64_t pol = l2_evict_last();
+          const int end = min(count, i + kPrefetchTiles);
+          int pli = 0;
+          Tile prev = decode_tile(P, first + (i - 1) * stride, pli);         // its K is loaded already
+          for (int p = i; p < end; ++p) {
+            const Tile u = decode_tile(P, first + p * stride, pli);
+            const bool new_head = u.li != prev.li || u.prompt != prev.prompt || u.head != prev.head;
+            const int nc = kChunked ? (P.layer[u.li].head_dim + 63) >> 6 : 1;
+            for (int c = 0; c < nc; ++c) {
+              tma_prefetch_4d(&MP.qmap[u.li], 64 * c, u.head, u.pixel0, u.prompt, pol);
+              if (new_head) tma_prefetch_4d(&MP.kmap[u.li], 64 * c, u.head, 0, u.prompt, pol);
+            }
+            prev = u;
+          }
+        }
+        const Tile t = decode_tile(P, first + i * stride, li);
         const int n_chunks = kChunked ? (P.layer[t.li].head_dim + 63) >> 6 : 1;
         for (int c = 0; c < n_chunks; ++c, ++j) {      // one load iteration = one 64-wide K chunk of one tile
           const int s = j % kStages;
@@ -418,7 +473,7 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP)
     int li = 0, j = 0;
     bool issued = false;
     for (int i = 0; i < count; ++i) {
-      const Tile t = decode_tile(P, first + i, li);
+      const Tile t = decode_tile(P, first + i * stride, li);
       const LayerParams& L = P.layer[t.li];
       const int n_chunks = kChunked ? (L.head_dim + 63) >> 6 : 1;
       Frag d;
@@ -541,7 +596,8 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP)
         fence_proxy_async();                           // generic-proxy writes -> visible to the bulk-async proxy
         consumer_barrier();
         if (tid == 0) {
-          tma_store_2d(&MP.amap[t.li], sP_u32 + a * kPBytes, t.pixel0, (t.prompt * L.heads + t.head) * kTokens);
+          tma_store_2d_hint(&MP.amap[t.li], sP_u32 + a * kPBytes, t.pixel0, (t.prompt * L.heads + t.head) * kTokens,
+                            l2_evict_first());
           if constexpr (kSlab == kSlabStore)           // same bulk group: the waits below cover both stores
             tma_store_2d(&MP.smap[t.li], sS_u32, t.pixel0, (t.prompt * L.heads + t.head) * kTokens);
           if constexpr (kSlab == kSlabAdd)             // (and the range reduce: its reads of sS)
