@@ -810,9 +810,12 @@ struct PreparedMma {
 void* prepared_mma_new() { return new PreparedMma; }                 // (aligned new: CUtensorMap is alignas(64))
 void prepared_mma_delete(void* p) { delete static_cast<PreparedMma*>(p); }
 
+// hw % 4 == 0: the accumulator / second-slab tensor maps (make_acc_map) need a row pitch of hw * 4 bytes that is a
+// multiple of 16, and the split form's load / add / store epilogue moves float4 columns. Other layers (odd-sized keys
+// such as 19 x 25) take the SIMT kernel, which updates the accumulator one element at a time.
 bool mma_supported(const LayerParams& L) {
   return L.head_dim % 8 == 0 && L.head_dim <= DAAM_MAX_HEAD_DIM && L.vec_ok && L.qs_head > 0 && L.qs_pixel > 0 &&
-         L.ks_head > 0 && L.ks_token > 0;
+         L.ks_head > 0 && L.ks_token > 0 && L.hw % 4 == 0;
 }
 
 // Tensor maps, grid and kernel variant of one pack of layers (all fp32, or all 16-bit). `out`: prepared_mma_new().

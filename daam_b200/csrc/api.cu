@@ -58,7 +58,6 @@ int make_layer_params(const daam_layer& in, int index, LayerParams* out, bool ne
   if (in.tokens != kTokens) { set_error("daam_accumulate: layer %d: tokens = %d, only %d is traced (daam/trace.py:289)", index, in.tokens, kTokens); return DAAM_E_UNSUPPORTED; }
   if (in.head_dim <= 0 || in.head_dim % 8 != 0 || in.head_dim > DAAM_MAX_HEAD_DIM) { set_error("daam_accumulate: layer %d: head_dim = %d must be a multiple of 8 in (0, %d]", index, in.head_dim, DAAM_MAX_HEAD_DIM); return DAAM_E_UNSUPPORTED; }
   if (in.n_prompts <= 0 || in.heads <= 0 || in.hw <= 0) { set_error("daam_accumulate: layer %d: non-positive n_prompts/heads/hw", index); return DAAM_E_INVALID; }
-  if (in.hw % 4 != 0) { set_error("daam_accumulate: layer %d: hw = %d must be a multiple of 4", index, in.hw); return DAAM_E_UNSUPPORTED; }
   if (need_acc && reinterpret_cast<uintptr_t>(in.acc) % 16 != 0) { set_error("daam_accumulate: layer %d: acc is not 16-byte aligned", index); return DAAM_E_INVALID; }
   if (!(in.scale > 0.f)) { set_error("daam_accumulate: layer %d: scale must be positive", index); return DAAM_E_INVALID; }
   LayerParams& L = *out;
@@ -201,8 +200,8 @@ int build_plan(const daam_layer* layers, float* const* slabs, SlabMode mode, int
     if (int rc = make_layer_params(layers[i], i, &L, /*need_acc=*/true)) return rc;
     const bool use_mma = path != DAAM_ACC_FORCE_SIMT && dev.cc_major == 9 && mma_supported(L);
     if (path == DAAM_ACC_FORCE_MMA && !use_mma) {
-      set_error("daam_accumulate: layer %d cannot take the wgmma path (dtype %d, head_dim %d, alignment %d, sm_%d%d)", i,
-                L.dtype, L.head_dim, L.vec_ok, dev.cc_major, dev.cc_minor);
+      set_error("daam_accumulate: layer %d cannot take the wgmma path (dtype %d, head_dim %d, alignment %d, hw = %d, "
+                "sm_%d%d)", i, L.dtype, L.head_dim, L.vec_ok, L.hw, dev.cc_major, dev.cc_minor);
       return DAAM_E_UNSUPPORTED;
     }
     const int which = use_mma ? (L.dtype == DAAM_F32 ? 1 : 0) : 2;

@@ -28,7 +28,8 @@ extern "C" {
                                        3: + DAAM_ACC_EARLY_LOADS, daam_expand_words, daam_side_launcher_*
                                           (later, additive: daam_accumulate_steps, daam_normalize_maps,
                                           daam_accumulate_range)
-                                       4: the finalize family takes (map_h, map_w); the _rect names are gone */
+                                       4: the finalize family takes (map_h, map_w); the _rect names are gone
+                                          (later, additive: layers with hw not a multiple of 4 are accepted) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
 
@@ -42,8 +43,8 @@ enum daam_status {
 enum daam_dtype { DAAM_F32 = 0, DAAM_F16 = 1, DAAM_BF16 = 2 };
 
 /* daam_accumulate flags */
-#define DAAM_ACC_AUTO        0u  /* wgmma path whenever rows are 16-byte aligned (any dtype, head_dim % 8 == 0),
-                                    SIMT fp32 path otherwise */
+#define DAAM_ACC_AUTO        0u  /* wgmma path whenever rows are 16-byte aligned (any dtype, head_dim % 8 == 0) and
+                                    hw % 4 == 0, SIMT fp32 path otherwise */
 #define DAAM_ACC_FORCE_SIMT  1u  /* always the SIMT fp32 ("warp dot") kernel */
 #define DAAM_ACC_FORCE_MMA   2u  /* wgmma kernel or DAAM_E_UNSUPPORTED */
 /* Accumulator update of the SIMT kernel and of the wgmma kernel's fp32 form. The wgmma kernel's 16-bit (fp16 / bf16)
@@ -85,7 +86,8 @@ typedef struct daam_layer {
   float* acc;                /* device; fp32 [n_prompts][heads][tokens][hw], 16-byte aligned */
   int64_t q_stride_prompt, q_stride_pixel, q_stride_head;   /* in elements; the head_dim axis is contiguous */
   int64_t k_stride_prompt, k_stride_token, k_stride_head;
-  int32_t n_prompts, heads, hw, tokens, head_dim;
+  int32_t n_prompts, heads, hw, tokens, head_dim;   /* hw: any positive pixel count; the wgmma path needs hw % 4 == 0
+                                                       (DAAM_ACC_AUTO sends other layers to the SIMT kernel) */
   int32_t dtype;             /* enum daam_dtype of q and k */
   float scale;               /* attn.scale = head_dim ** -0.5 */
   int32_t reserved;

@@ -17,6 +17,9 @@ Fixtures
                      map, normalised map, filtered maps, per-key sums (rows a1-a9 end to end).
   pipeline_tiny96.npz the same for the 96x96-latent geometry of the 768-pixel models (latent_hw 9216, trace.py:32-33):
                      (96, 96) global maps from keys at 96^2 / 48^2 / 24^2.
+  pipeline_tiny600.npz the generation of pipeline_tiny.npz at 600x600 pixels (``python -m oracle.make_golden
+                     pipeline_offgrid``): keys at 75^2 / 38^2 / 19^2 (factors 0 / 1 / 3), bicubic down-sampling of the
+                     75^2 keys onto the 64 x 64 grid.
   perkey.npz         the reference's --all-heads sweep (daam/run/generate.py:239-255) over finalize.npz's keys:
                      ``compute_global_heat_map(layer_idx=l, head_idx=h)`` for every key, plain and normalised.
   vs_reference.npz   the rest of what tests/test_oracle_vs_reference.py compares with: exact fingerprints of the
@@ -147,6 +150,30 @@ def make_pipeline96_fixture(daam):
     print('pipeline96', len(keys), {k: tuple(v.shape) for k, v in out.items()})
 
 
+def make_pipeline_offgrid_fixture(daam):
+    """The generation of pipeline_tiny.npz at 600x600 pixels: a 75x75 latent off the 64-pixel grid, whose traced layers
+    have 75^2 / 38^2 / 19^2 query positions (factors 0 / 1 / 3 under the reference's rule) and odd pixel counts."""
+    pipe = make_pipeline(TINY_SPEC, dtype=torch.float32, seed=3)
+    with daam.trace(pipe) as tc:
+        pipe(PROMPT, num_inference_steps=2, generator=torch.Generator().manual_seed(11), height=600, width=600)
+        keys = [k for k, _ in tc.all_heat_maps]
+        sums = np.array([float(v.double().sum()) for _, v in tc.all_heat_maps])
+        absmax = np.array([float(v.abs().max()) for _, v in tc.all_heat_maps])
+        out = {
+            'global': tc.compute_global_heat_map().heat_maps.numpy(),
+            'global_norm': tc.compute_global_heat_map(normalize=True).heat_maps.numpy(),
+            'factors_0': tc.compute_global_heat_map(factors=[0]).heat_maps.numpy(),
+            'factors_3': tc.compute_global_heat_map(factors=[3]).heat_maps.numpy(),
+            'layer9_head0': tc.compute_global_heat_map(layer_idx=9, head_idx=0).heat_maps.numpy(),
+            'word_ball': tc.compute_global_heat_map().compute_word_heat_map('ball').heatmap.numpy(),
+        }
+        names = list(tc.layer_names)
+    np.savez_compressed(os.path.join(OUT, 'pipeline_tiny600.npz'), prompt=PROMPT, steps=2, unet_seed=3, gen_seed=11,
+                        height=600, width=600, keys=np.array(keys), key_sums=sums, key_absmax=absmax,
+                        layer_names=np.array(names), **out)
+    print('pipeline600', len(keys), {k: tuple(v.shape) for k, v in out.items()})
+
+
 def make_perkey_fixture(daam):
     """Every (layer, head) map of the all-heads sweep, from the keys stored in finalize.npz."""
     fx = np.load(os.path.join(OUT, 'finalize.npz'), allow_pickle=False)
@@ -244,10 +271,14 @@ def main():
     if sys.argv[1:] == ['vs_reference']:
         make_vs_reference_fixture(daam)
         return
+    if sys.argv[1:] == ['pipeline_offgrid']:
+        make_pipeline_offgrid_fixture(daam)
+        return
     make_layers(daam)
     make_finalize(daam)
     make_pipeline_fixture(daam)
     make_pipeline96_fixture(daam)
+    make_pipeline_offgrid_fixture(daam)
     make_perkey_fixture(daam)
     make_vs_reference_fixture(daam)
 
