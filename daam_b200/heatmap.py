@@ -6,6 +6,7 @@ Mirror of the reference's L2 (``daam/heatmap.py``) for the hot-path rows of SURV
   iteration over ``((factor, layer, head), tensor[77, h, w])``, ``clear``), but backed by one fp32 device slab per traced
   layer, laid out ``[prompts][heads][77][h*w]``: the slab *is* the reference's per-key tensors (each key a contiguous
   view), and it is what ``daam_accumulate`` adds into, so nothing is copied or re-laid-out between kernel and API.
+  A trace with ``negative=True`` keeps the unconditional half of the CFG batch in the same slab, below it.
 * :class:`GlobalHeatMap` (heatmap.py:114-142) / :class:`WordHeatMap` (heatmap.py:56-96) -- ``compute_word_heat_map``
   and ``expand_as`` run the native kernels (``daam_word_heat_map``, ``daam_expand_as``).
 
@@ -64,6 +65,11 @@ class LayerSlab:
     step: Optional[torch.Tensor] = None   # time-resolved traces only: what the last step added, shaped like ``acc``
     # step-range traces only: ``ranges[i]`` is shaped like ``acc`` and holds the sum over the steps of declared range i
     ranges: Optional[List[torch.Tensor]] = None
+    # negative traces only: ``storage`` [2 * n_prompts, heads, 77, h*w] is what the layer's descriptor covers, the CFG
+    # batch in its order; ``neg = storage[:n_prompts]`` (the unconditional half) and ``acc = storage[n_prompts:]``. The
+    # step and range slabs then have ``storage``'s height too.
+    storage: Optional[torch.Tensor] = None
+    neg: Optional[torch.Tensor] = None
 
     @property
     def n_prompts(self) -> int:
@@ -76,12 +82,27 @@ class LayerSlab:
 
     def zero_(self):
         """Zero the accumulator and the range slabs (a step slab needs no zeroing: every step rewrites it whole)."""
-        self.acc.zero_()
+        (self.acc if self.storage is None else self.storage).zero_()
         for r in self.ranges or ():
             r.zero_()
 
-    def key_view(self, head: int, prompt: int = 0, step_range: Optional[int] = None) -> torch.Tensor:
-        src = self.acc if step_range is None else self.ranges[step_range]
+    def half(self, t: torch.Tensor, negative: bool = False) -> torch.Tensor:
+        """The ``[n_prompts, heads, 77, h*w]`` half of a step or range slab that belongs to ``acc`` (or with
+        ``negative`` to ``neg``); the slab itself when the trace keeps no negative half."""
+        if self.storage is None:
+            return t
+        n = self.n_prompts
+        return t[:n] if negative else t[n:]
+
+    def source(self, step_range: Optional[int] = None, negative: bool = False) -> torch.Tensor:
+        """What a read reduces: ``acc`` or ``neg``, or the matching half of range slab ``step_range``."""
+        if step_range is None:
+            return self.neg if negative else self.acc
+        return self.half(self.ranges[step_range], negative)
+
+    def key_view(self, head: int, prompt: int = 0, step_range: Optional[int] = None,
+                 negative: bool = False) -> torch.Tensor:
+        src = self.source(step_range, negative)
         return src[prompt, head].view(src.shape[2], self.h, self.w)
 
 
@@ -97,6 +118,7 @@ class RawHeatMapCollection:
         self.time_resolved = False            # allocate a step slab next to every accumulator (trace(time_resolved=True))
         self.n_ranges = 0                     # range slabs next to every accumulator (trace(step_ranges=[...]))
         self.range_steps: List[int] = []      # UNet forwards each range has received since the last clear()
+        self.negative = False                 # slabs also hold the unconditional half (trace(negative=True))
 
     # -- wiring from the tracer -------------------------------------------------------------------------------------
     def bind(self, sync, zero):
@@ -113,16 +135,19 @@ class RawHeatMapCollection:
         shape = (n_prompts, heads, _native.TOKENS, h * w)
         if slab is None or tuple(slab.acc.shape) != shape or slab.acc.device != torch.device(device) \
                 or slab.factor != factor or (self.time_resolved and slab.step is None) \
-                or (self.n_ranges and slab.ranges is None):
+                or (self.n_ranges and slab.ranges is None) or (self.negative and slab.neg is None):
             if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
                 raise RuntimeError('accumulator slabs cannot be created inside a CUDA-graph capture: run one eager '
                                    'UNet step under trace() before capturing')
-            acc = torch.zeros(shape, dtype=torch.float32, device=device)
+            full = (2 * n_prompts,) + shape[1:] if self.negative else shape
+            storage = torch.zeros(full, dtype=torch.float32, device=device)
             # the kernel writes every element of a step slab each step: no zeroing needed
-            step = torch.empty(shape, dtype=torch.float32, device=device) if self.time_resolved else None
-            ranges = [torch.zeros(shape, dtype=torch.float32, device=device) for _ in range(self.n_ranges)] \
+            step = torch.empty(full, dtype=torch.float32, device=device) if self.time_resolved else None
+            ranges = [torch.zeros(full, dtype=torch.float32, device=device) for _ in range(self.n_ranges)] \
                 if self.n_ranges else None
-            slab = LayerSlab(layer_idx, factor, heads, h, w, acc, head_offset=head_offset, step=step, ranges=ranges)
+            halves = dict(acc=storage[n_prompts:], storage=storage, neg=storage[:n_prompts]) if self.negative \
+                else dict(acc=storage)
+            slab = LayerSlab(layer_idx, factor, heads, h, w, head_offset=head_offset, step=step, ranges=ranges, **halves)
             self.slabs[layer_idx] = slab
             self.epoch += 1
         elif (slab.h, slab.w) != (h, w):      # same pixel count, other key shape (a transposed latent): re-tag
@@ -171,24 +196,37 @@ class RawHeatMapCollection:
     def heads(self) -> Set[int]:
         return {h for s in self.live_slabs() for h in range(s.heads)}
 
-    def items(self, prompt: int = 0, *, step_range: Optional[int] = None) -> Iterator[Tuple[RawHeatMapKey, torch.Tensor]]:
+    def items(self, prompt: int = 0, *, step_range: Optional[int] = None,
+              negative: bool = False) -> Iterator[Tuple[RawHeatMapKey, torch.Tensor]]:
         """``((factor, layer, head), [77, h, w])`` for every key; with ``step_range=i`` the per-key sums over the steps
-        of declared range ``i`` (``trace(pipe, step_ranges=[...])``) instead of over every step."""
-        for slab in self.read_slabs(step_range):
+        of declared range ``i`` (``trace(pipe, step_ranges=[...])``) instead of over every step; with ``negative`` those
+        of the unconditional half of the CFG batch (``trace(pipe, negative=True)``)."""
+        for slab in self.read_slabs(step_range, negative):
             for head in range(slab.heads):
-                yield (slab.factor, slab.layer_idx, head), slab.key_view(head, prompt, step_range)
+                yield (slab.factor, slab.layer_idx, head), slab.key_view(head, prompt, step_range, negative)
 
-    def read_slabs(self, step_range: Optional[int] = None) -> List[LayerSlab]:
+    def read_slabs(self, step_range: Optional[int] = None, negative: bool = False) -> List[LayerSlab]:
         """The slabs a read reduces, once every pending accumulate is visible: the live slabs, or with ``step_range``
-        those with range slabs, after checking the index and that the range has received a step."""
+        those with range slabs, after checking the index and that the range has received a step; with ``negative``
+        only those that keep the unconditional half."""
         if step_range is not None:
             self.check_step_range(step_range)
+        if negative:
+            self.check_negative()
         self._synchronize()
+        slabs = self.live_slabs()
+        if negative:
+            slabs = [s for s in slabs if s.neg is not None]
         if step_range is None:
-            return self.live_slabs()
+            return slabs
         if self.range_steps[step_range] == 0:
             raise RuntimeError('No heat maps found for the given parameters.')
-        return [s for s in self.live_slabs() if s.ranges is not None]
+        return [s for s in slabs if s.ranges is not None]
+
+    def check_negative(self):
+        """Raises unless the slabs keep the unconditional half (``trace(pipe, negative=True)``)."""
+        if not self.negative:
+            raise RuntimeError('negative heat maps need a trace declared with trace(pipe, negative=True)')
 
     def check_step_range(self, step_range: int):
         """Raises unless ``step_range`` indexes a range declared with ``trace(pipe, step_ranges=[...])``."""

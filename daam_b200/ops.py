@@ -35,10 +35,12 @@ def new_accumulator(n_prompts: int, heads: int, hw: int, device) -> torch.Tensor
     return torch.zeros((n_prompts, heads, _native.TOKENS, hw), dtype=torch.float32, device=device)
 
 
-def make_layer_desc(q: torch.Tensor, k: torch.Tensor, acc: torch.Tensor, heads: int, scale: float
-                    ) -> _native.DaamLayer:
+def make_layer_desc(q: torch.Tensor, k: torch.Tensor, acc: torch.Tensor, heads: int, scale: float, *,
+                    whole_batch: bool = False) -> _native.DaamLayer:
     """``q [B, hw, heads*d]`` / ``k [B, 77, heads*d]`` as ``to_q`` / ``to_k`` emit them (last axis contiguous) and the
-    fp32 accumulator ``[n_prompts, n_heads, 77, hw]`` of the kept slice -> one ``daam_layer``."""
+    fp32 accumulator ``[n_prompts, n_heads, 77, hw]`` of the kept slice -> one ``daam_layer``. ``whole_batch``: the
+    descriptor covers every sample from sample 0 -- both halves of a CFG batch, the unconditional one first -- and
+    ``acc`` is ``[B, heads, 77, hw]``."""
     if not (q.is_cuda and k.is_cuda and acc.is_cuda):
         raise RuntimeError('daam_b200 computes on CUDA tensors only (there is no CPU fallback)')
     if q.dtype not in _DTYPES or k.dtype != q.dtype:
@@ -47,7 +49,7 @@ def make_layer_desc(q: torch.Tensor, k: torch.Tensor, acc: torch.Tensor, heads: 
         raise RuntimeError('the channel axis of q and k must be contiguous')
     bsz, hw, chan = q.shape
     d = chan // heads
-    first, n_prompts, head0, n_heads = cond_half(bsz, heads)
+    first, n_prompts, head0, n_heads = (0, bsz, 0, heads) if whole_batch else cond_half(bsz, heads)
     if tuple(acc.shape) != (n_prompts, n_heads, _native.TOKENS, hw) or acc.dtype != torch.float32 \
             or not acc.is_contiguous():
         raise RuntimeError(f'accumulator must be contiguous fp32 {(n_prompts, n_heads, _native.TOKENS, hw)}, '
@@ -150,15 +152,16 @@ def attention_probs(q: torch.Tensor, k: torch.Tensor, heads: int, scale: Optiona
     return probs
 
 
-def accumulate_probs(probs: torch.Tensor, acc: torch.Tensor):
+def accumulate_probs(probs: torch.Tensor, acc: torch.Tensor, *, whole_batch: bool = False):
     """``acc[r][t][pixel] += probs[first + r][pixel][t]`` with ``first = rows // 2``: the reference's "second half of
     the batch*heads axis" (daam/trace.py:240) applied to supplied probabilities (``load_heads``, trace.py:281-294).
-    ``acc``: fp32 ``[n_prompts, n_heads, 77, hw]`` (its leading two axes flatten to the kept rows)."""
+    ``acc``: fp32 ``[n_prompts, n_heads, 77, hw]`` (its leading two axes flatten to the kept rows). ``whole_batch``:
+    ``first = 0``, every row is kept (both halves of a CFG batch)."""
     if not (probs.is_cuda and acc.is_cuda):
         raise RuntimeError('daam_b200 computes on CUDA tensors only (there is no CPU fallback)')
     probs = probs.contiguous()
     rows, hw, tokens = probs.shape
-    first = rows // 2
+    first = 0 if whole_batch else rows // 2
     kept = rows - first
     if acc.dtype != torch.float32 or not acc.is_contiguous() or acc.numel() != kept * tokens * hw:
         raise RuntimeError(f'accumulator must be contiguous fp32 with {kept} x {tokens} x {hw} elements')

@@ -437,9 +437,12 @@ class SyntheticPipeline:
         self._graphs = {}
         self._attn = [m for m in self.unet.modules() if isinstance(m, SyntheticAttention)]
 
-    def check_inputs(self, prompt, *args, **kwargs):
+    def check_inputs(self, prompt, height=None, width=None, callback_steps=None, negative_prompt=None, *args, **kwargs):
+        """diffusers' SD ``check_inputs`` parameter order, so that callers bind ``negative_prompt`` as they do there."""
         if not isinstance(prompt, (str, list)):
             raise ValueError('`prompt` has to be of type `str` or `list`')
+        if negative_prompt is not None and not isinstance(negative_prompt, (str, list)):
+            raise ValueError('`negative_prompt` has to be of type `str` or `list`')
 
     def encode(self, prompts: List[str], generator: torch.Generator):
         """Synthetic text encoder: seeded gaussian embeddings, [uncond x N, cond x N] like diffusers' CFG concat."""
@@ -476,13 +479,18 @@ class SyntheticPipeline:
 
     @torch.no_grad()
     def __call__(self, prompt, num_inference_steps: int = 50, generator: Optional[torch.Generator] = None,
-                 callback=None, guidance_scale: float = 7.5, height: Optional[int] = None, width: Optional[int] = None):
+                 callback=None, guidance_scale: float = 7.5, height: Optional[int] = None, width: Optional[int] = None,
+                 negative_prompt=None):
         """``height`` / ``width``: the image size in pixels, as diffusers takes it (default: the model's own square
-        size); the latent is ``height // 8 x width // 8``."""
+        size); the latent is ``height // 8 x width // 8``. ``negative_prompt`` reaches ``check_inputs`` positionally, in
+        diffusers' SD order; the synthetic encoder ignores all text, so it changes no embedding or random draw."""
         spec = self.unet.spec
         height = spec.sample_size * self.vae_scale_factor if height is None else height
         width = spec.sample_size * self.vae_scale_factor if width is None else width
-        self.check_inputs(prompt, height, width)
+        if negative_prompt is None:
+            self.check_inputs(prompt, height, width)
+        else:
+            self.check_inputs(prompt, height, width, None, negative_prompt)
         prompts = [prompt] if isinstance(prompt, str) else list(prompt)
         n = len(prompts)
         latent_h, latent_w = height // self.vae_scale_factor, width // self.vae_scale_factor

@@ -22,12 +22,17 @@ exceptions; what differs is what runs underneath.
   ``daam_accumulate_range``, which also adds what it adds into range ``i``'s slabs. Each range slab then is the
   accumulator a trace of only those steps would hold, so every read (``step_range=i``) reduces it exactly as the full
   run's accumulator is reduced.
+* ``negative=True`` also keeps the map of the unconditional half of the CFG batch: the model attending to the negative
+  prompt (or the empty one). Every layer's slab is twice as tall, ``[uncond x N, cond x N]`` like the batch, and its
+  one descriptor covers the whole batch from sample 0, so the launches stay as they are with twice the tiles. Every read
+  takes ``negative=True`` and then reduces the lower half against the negative text.
 
 Accumulators are fp32 regardless of the pipeline dtype (the reference accumulates in the pipeline dtype, SURVEY.md
 section 5); parity is stated against the fp32 oracle fed the same Q/K.
 """
 from __future__ import annotations
 
+import inspect
 from pathlib import Path
 from typing import Dict, List, Optional, Tuple, Type, Union
 
@@ -54,13 +59,14 @@ class DiffusionHeatMapHooker(AggregateHooker):
     ``(start, stop)`` tuples or ``range`` objects over UNet-forward indices of a generation, counted as
     :class:`TimeHeatMaps` counts them: also keep the per-key sums over each of those spans; read them with
     ``step_range=i`` in :meth:`compute_global_heat_map`, :meth:`compute_per_head_heat_maps` and
-    ``all_heat_maps.items``).
+    ``all_heat_maps.items``) and ``negative`` (also keep the maps of the unconditional half of the guidance batch, the
+    negative prompt's; read them with ``negative=True`` in every read).
     """
 
     def __init__(self, pipeline, low_memory: bool = False, load_heads: bool = False, save_heads: bool = False,
                  data_dir: str = None, *, launch: str = 'step', batch_prompts: bool = False,
                  locate_middle_block: bool = False, kernel_flags: int = _native.ACC_AUTO, time_resolved: bool = False,
-                 step_ranges=None):
+                 step_ranges=None, negative: bool = False):
         if launch not in ('step', 'overlap', 'layer'):
             raise ValueError("launch must be 'step', 'overlap' or 'layer'")
         modes = []                             # the enabled second-slab modes, and why each needs the step launch
@@ -88,6 +94,9 @@ class DiffusionHeatMapHooker(AggregateHooker):
                                                  locate_middle_block=locate_middle_block or load_heads or save_heads)
         self.last_prompt: str = ''
         self.last_prompts: List[str] = []
+        self.last_negative_prompts: List[str] = []   # negative=True: the negative text of every prompt ('' for none)
+        self.negative = negative
+        self.all_heat_maps.negative = negative
         self.last_image = None
         self.time_idx = 0
         self._gen_idx = 0
@@ -111,12 +120,12 @@ class DiffusionHeatMapHooker(AggregateHooker):
         self._dirty = False                    # side-stream work not yet ordered before the current stream
         self.all_heat_maps.bind(self.synchronize, self._zero_slabs)
         # time-resolved mode: per prompt a device history [capacity, n_rows, x, x] of per-step global heat maps (grown
-        # by doubling, restarted every generation)
+        # by doubling, restarted every generation), keyed by `negative` (the negative histories exist with the mode only)
         self.time_resolved = time_resolved
         self.all_heat_maps.time_resolved = time_resolved
-        self._history: List[torch.Tensor] = []
+        self._history: Dict[bool, List[torch.Tensor]] = {False: [], True: []}
         self._time_steps = 0
-        self._history_rows: Optional[List[int]] = None   # n_rows of every prompt of the running generation
+        self._history_rows: Optional[Dict[bool, List[int]]] = None   # n_rows of every prompt of the running generation
         # step-range mode: the UNet forward index of the running generation
         self.step_ranges: Optional[List[Tuple[int, int]]] = step_ranges
         self.all_heat_maps.n_ranges = len(step_ranges) if step_ranges else 0
@@ -148,12 +157,14 @@ class DiffusionHeatMapHooker(AggregateHooker):
         return self.locator.layer_names
 
     def to_experiment(self, path, seed=None, id='.', subtype='.', **compute_kwargs):
-        """Exports the last generation call to a serializable generation experiment (trace.py:68-81)."""
+        """Exports the last generation call to a serializable generation experiment (trace.py:68-81). With
+        ``negative=True`` it records the negative map and the text it belongs to."""
         from .experiment import GenerationExperiment
+        heat_map = self.compute_global_heat_map(**compute_kwargs)
         return GenerationExperiment(
             self.last_image,
-            self.compute_global_heat_map(**compute_kwargs).heat_maps,
-            self.last_prompt,
+            heat_map.heat_maps,
+            heat_map.prompt if compute_kwargs.get('negative') else self.last_prompt,
             seed=seed, id=id, subtype=subtype, path=path, tokenizer=self.pipe.tokenizer,
         )
 
@@ -249,12 +260,17 @@ class DiffusionHeatMapHooker(AggregateHooker):
         h, w, _ = self.geometry.level(hw, layer_idx)
         if h is None:
             raise RuntimeError(f'layer {layer_idx}: {hw} query positions are not a square map')
+        self._check_guidance(layer_idx, bsz)
         # "second half of the batch*heads axis" (trace.py:240): the conditional samples of a CFG batch
         _, n_samples, head0, n_heads = ops.cond_half(bsz, heads)
         n_real, images = self._prompt_layout(layer_idx, n_samples)
         slab = self.all_heat_maps.slab_for(layer_idx, factor, n_real, images * n_heads, h, w, q.device, head0)
         self._epoch_seen = self.all_heat_maps.epoch        # (this call may have bumped it; the other layers' slabs stand)
-        desc = ops.make_layer_desc(q, k, slab.acc.view(n_samples, n_heads, slab.acc.shape[2], hw), heads, scale)
+        if self.negative:                                  # one descriptor over the whole batch, into the whole slab
+            desc = ops.make_layer_desc(q, k, slab.storage.view(bsz, n_heads, slab.acc.shape[2], hw), heads, scale,
+                                       whole_batch=True)
+        else:
+            desc = ops.make_layer_desc(q, k, slab.acc.view(n_samples, n_heads, slab.acc.shape[2], hw), heads, scale)
         if self.launch != 'layer':
             if pos >= len(self._slots):                    # grow the step array (SDXL: 70 layers)
                 grown = _native.PackedLayers([_native.DaamLayer()] * (2 * len(self._slots)))
@@ -293,6 +309,12 @@ class DiffusionHeatMapHooker(AggregateHooker):
             raise RuntimeError(f'layer {layer_idx}: {n_samples} conditional samples for {n_real} prompts')
         return n_real, n_samples // n_real
 
+    def _check_guidance(self, layer_idx: int, bsz: int):
+        """``negative=True`` keeps the unconditional half of a CFG batch: a batch without one is an error."""
+        if self.negative and bsz % 2:
+            raise RuntimeError(f'layer {layer_idx}: negative=True needs classifier-free guidance, but a batch of {bsz} '
+                               f'is not a CFG pair batch [uncond x N, cond x N]')
+
     def _launch_now(self, own, device):
         """``launch='layer'``: the layer's kernel right away on the current stream (the producer of Q/K may be the
         immediately preceding kernel there, so no EARLY_LOADS)."""
@@ -303,11 +325,15 @@ class DiffusionHeatMapHooker(AggregateHooker):
         h, w, _ = self.geometry.level(probs.shape[1], layer_idx)
         if h is None:
             raise RuntimeError(f'layer {layer_idx}: {probs.shape[1]} query positions are not a square map')
+        self._check_guidance(layer_idx, bsz)
         _, n_samples, head0, n_heads = ops.cond_half(bsz, heads)
         n_real, images = self._prompt_layout(layer_idx, n_samples)
         slab = self.all_heat_maps.slab_for(layer_idx, factor, n_real, images * n_heads, h, w, probs.device, head0)
         self.synchronize()
-        ops.accumulate_probs(probs, slab.acc)
+        if self.negative:                                  # rows [0, N*H) into neg, the rest into acc, in one launch
+            ops.accumulate_probs(probs, slab.storage, whole_batch=True)
+        else:
+            ops.accumulate_probs(probs, slab.acc)
 
     def flush(self):
         """Issue the queued layer calls as one persistent launch (per pack of 32 layers)."""
@@ -382,30 +408,44 @@ class DiffusionHeatMapHooker(AggregateHooker):
     def _finalize_step(self, device, stream: int):
         """Time-resolved mode, right after the step's launch on ``stream``: for every prompt, the global heat map of the
         step slabs this step wrote -- the same reduction, key order (live-slab order) and row count as
-        :meth:`compute_global_heat_map` -- into the next slot of the prompt's history."""
+        :meth:`compute_global_heat_map` -- into the next slot of the prompt's history. With ``negative=True`` the same
+        again over the unconditional halves of the step slabs, into the negative histories."""
         queued = {idx for idx, step in self._queued.items() if step == self._step_id}
         slabs = [s for s in self.all_heat_maps.live_slabs() if s.layer_idx in queued]
         grid = self.geometry.grid
         t = self._time_steps
-        prompts = self.last_prompts or [self.last_prompt]
+        halves = (False, True) if self.negative else (False,)
         if self._history_rows is None:
-            self._history_rows = [min(len(self.pipe.tokenizer.tokenize(p)) + 2, _native.TOKENS) for p in prompts]
-        for p in range(slabs[0].n_prompts):
-            n_rows = self._history_rows[p] if p < len(self._history_rows) else self._history_rows[0]
-            if p == len(self._history):
-                self._history.append(torch.empty((16, n_rows) + grid, dtype=torch.float32, device=device))
-            hist = self._history[p]
-            if t == hist.shape[0]:                          # grow by doubling, in stream order between two steps
-                grown = torch.empty((2 * t,) + tuple(hist.shape[1:]), dtype=torch.float32, device=device)
-                grown[:t].copy_(hist)
-                self._history[p] = hist = grown
-            _native.finalize([_key_group(s.step[p], s) for s in slabs], grid, n_rows, False, hist[t].data_ptr(), stream)
+            self._history_rows = {negative: [self._n_rows(text) for text in self._texts(negative)]
+                                  for negative in halves}
+        for negative in halves:
+            rows, history = self._history_rows[negative], self._history[negative]
+            for p in range(slabs[0].n_prompts):
+                n_rows = rows[p] if p < len(rows) else rows[0]
+                if p == len(history):
+                    history.append(torch.empty((16, n_rows) + grid, dtype=torch.float32, device=device))
+                hist = history[p]
+                if t == hist.shape[0]:                      # grow by doubling, in stream order between two steps
+                    grown = torch.empty((2 * t,) + tuple(hist.shape[1:]), dtype=torch.float32, device=device)
+                    grown[:t].copy_(hist)
+                    history[p] = hist = grown
+                _native.finalize([_key_group(s.half(s.step, negative)[p], s) for s in slabs], grid, n_rows, False,
+                                 hist[t].data_ptr(), stream)
         self._time_steps = t + 1
+
+    def _texts(self, negative: bool = False) -> List[str]:
+        """The text of every prompt of the running / last generation, or with ``negative`` its negative text."""
+        if negative:
+            return self.last_negative_prompts or ['']
+        return self.last_prompts or [self.last_prompt]
+
+    def _n_rows(self, text: str) -> int:
+        return min(len(self.pipe.tokenizer.tokenize(text)) + 2, _native.TOKENS)   # 1 for SOS and 1 for padding
 
     def _restart_history(self):
         """A new generation: a new per-step history (maps handed out earlier stay valid: they are other tensors), and
         the UNet forward count of the step ranges starts again (their slabs were zeroed with the accumulators)."""
-        self._history = []
+        self._history = {False: [], True: []}
         self._time_steps = 0
         self._history_rows = None
         self._forward_idx = 0
@@ -443,16 +483,19 @@ class DiffusionHeatMapHooker(AggregateHooker):
 
     # -- finalize -------------------------------------------------------------------------------------------------------
     def compute_global_heat_map(self, prompt=None, factors=None, head_idx=None, layer_idx=None, normalize=False,
-                                prompt_idx: int = 0, *, step_range: Optional[int] = None) -> GlobalHeatMap:
+                                prompt_idx: int = 0, *, step_range: Optional[int] = None,
+                                negative: bool = False) -> GlobalHeatMap:
         """Aggregate across time (already summed in the slabs) and across layers/heads (trace.py:83-132).
 
         Args mirror the reference: ``factors`` restricts the spatial factors, ``head_idx`` / ``layer_idx`` restrict to one
         head / layer, ``normalize`` divides by the per-pixel sum over the real tokens. ``prompt_idx`` selects the prompt in
         ``batch_prompts`` mode. ``step_range=i`` aggregates over the steps of declared range ``i`` only
-        (``trace(pipe, step_ranges=[...])``): the DAAM map a trace of only those steps would give.
+        (``trace(pipe, step_ranges=[...])``): the DAAM map a trace of only those steps would give. ``negative=True``
+        (``trace(pipe, negative=True)``): the map of the unconditional half of the batch, whose text (and so row count
+        and word lookup) is the prompt's negative prompt unless ``prompt`` is given.
         """
         prompt, grid, n_rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range, layer_idx,
-                                                                head_idx)
+                                                                head_idx, negative)
         device = slabs[0].acc.device
         maps = torch.empty((n_rows,) + grid, dtype=torch.float32, device=device)
         with torch.cuda.device(device):
@@ -460,21 +503,27 @@ class DiffusionHeatMapHooker(AggregateHooker):
                              torch.cuda.current_stream(device).cuda_stream)
         return GlobalHeatMap(self.pipe.tokenizer, prompt, maps)
 
-    def compute_time_heat_maps(self, prompt_idx: int = 0, normalize: bool = False) -> TimeHeatMaps:
+    def compute_time_heat_maps(self, prompt_idx: int = 0, normalize: bool = False, *,
+                               negative: bool = False) -> TimeHeatMaps:
         """One global heat map per traced denoising step (UNet forward) of the running / last generation; needs
         ``trace(pipe, time_resolved=True)``. ``heat_maps[t]`` is what :meth:`compute_global_heat_map` would return had
         only step ``t`` been traced, with every key and layer; ``normalize`` applies the reference's normalisation to
         each step. Summing the steps does not give the all-steps map: there the clamp comes after the time sum.
+        ``negative=True``: the same for the unconditional half, against the negative text.
 
         Costs: a second fp32 slab per traced layer (as large as its accumulator) and ``steps x n_rows x xh x xw`` fp32
         of history per prompt (``heat_maps`` is ``[steps, n_rows, xh, xw]``, the grid of :attr:`geometry`)."""
         if not self.time_resolved:
             raise RuntimeError('per-step heat maps need trace(pipe, time_resolved=True)')
+        if negative:
+            self.all_heat_maps.check_negative()
         self.synchronize()
-        if self._time_steps == 0 or not 0 <= prompt_idx < len(self._history):
+        history = self._history[negative]
+        if self._time_steps == 0 or not 0 <= prompt_idx < len(history):
             raise RuntimeError('No heat maps found. Did you forget to call `with trace(...)` during generation?')
-        prompt = self.last_prompts[prompt_idx] if self.last_prompts else self.last_prompt
-        maps = self._history[prompt_idx][:self._time_steps]
+        texts = self._texts(negative)
+        prompt = texts[prompt_idx] if prompt_idx < len(texts) else texts[0]
+        maps = history[prompt_idx][:self._time_steps]
         if normalize:
             maps = maps.clone()
             with torch.cuda.device(maps.device):
@@ -484,12 +533,13 @@ class DiffusionHeatMapHooker(AggregateHooker):
 
 
     def compute_per_head_heat_maps(self, prompt=None, factors=None, normalize=False, prompt_idx: int = 0, *,
-                                   step_range: Optional[int] = None):
+                                   step_range: Optional[int] = None, negative: bool = False):
         """Every ``compute_global_heat_map(layer_idx=l, head_idx=h)`` of the reference's ``--all-heads`` sweep
         (daam/run/generate.py:239-255) in one launch. Returns ``(keys, maps)``: ``keys[i] = (factor, layer, head)`` and
-        ``maps[i]`` the ``[n_tokens + 2, xh, xw]`` heat map the reference computes for that single key. ``step_range=i``:
-        over the steps of declared range ``i`` only, as in :meth:`compute_global_heat_map`."""
-        prompt, grid, n_rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range)
+        ``maps[i]`` the ``[n_tokens + 2, xh, xw]`` heat map the reference computes for that single key. ``step_range=i``
+        and ``negative=True`` select the slabs as in :meth:`compute_global_heat_map`."""
+        prompt, grid, n_rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range,
+                                                                negative=negative)
         keys = [(slab.factor, slab.layer_idx, head) for slab in slabs for head in range(slab.heads)]
         device = slabs[0].acc.device
         maps = torch.empty((len(keys), n_rows) + grid, dtype=torch.float32, device=device)
@@ -498,28 +548,34 @@ class DiffusionHeatMapHooker(AggregateHooker):
                                      torch.cuda.current_stream(device).cuda_stream)
         return keys, maps
 
-    def _read_groups(self, prompt, factors, prompt_idx: int, step_range: Optional[int], layer_idx=None, head_idx=None):
-        """What the heat-map reads share: the prompt (default: the generation's), the map grid ``(xh, xw)``, the row count, and
-        the key groups of prompt ``prompt_idx`` over the live slabs (with ``step_range``: over that range's slabs) that
-        pass the filters, with the slabs behind them. Raises when no slab passes."""
+    def _read_groups(self, prompt, factors, prompt_idx: int, step_range: Optional[int], layer_idx=None, head_idx=None,
+                     negative: bool = False):
+        """What the heat-map reads share: the prompt (default: the generation's, or with ``negative`` its negative
+        text), the map grid ``(xh, xw)``, the row count, and the key groups of prompt ``prompt_idx`` over the live slabs
+        (with ``step_range``: over that range's slabs; with ``negative``: their unconditional halves) that pass the
+        filters, with the slabs behind them. Raises when no slab passes."""
+        if negative:
+            self.all_heat_maps.check_negative()
         if prompt is None:
-            prompt = self.last_prompts[prompt_idx] if self.last_prompts else self.last_prompt
+            if negative:
+                prompt = self.last_negative_prompts[prompt_idx] if self.last_negative_prompts else ''
+            else:
+                prompt = self.last_prompts[prompt_idx] if self.last_prompts else self.last_prompt
         factors = {0, 1, 2, 4, 8, 16, 32, 64} if factors is None else set(factors)
         groups, slabs = [], []
-        for slab in self.all_heat_maps.read_slabs(step_range):
+        for slab in self.all_heat_maps.read_slabs(step_range, negative):
             if slab.factor not in factors or (layer_idx is not None and layer_idx != slab.layer_idx):
                 continue
             if head_idx is not None and not 0 <= head_idx < slab.heads:
                 continue
-            acc = (slab.acc if step_range is None else slab.ranges[step_range])[prompt_idx]
+            acc = slab.source(step_range, negative)[prompt_idx]
             groups.append(_key_group(acc, slab, -1 if head_idx is None else head_idx))
             slabs.append(slab)
         if not groups:
             if head_idx is not None or layer_idx is not None:
                 raise RuntimeError('No heat maps found for the given parameters.')
             raise RuntimeError('No heat maps found. Did you forget to call `with trace(...)` during generation?')
-        n_rows = min(len(self.pipe.tokenizer.tokenize(prompt)) + 2, _native.TOKENS)   # 1 for SOS and 1 for padding
-        return prompt, self.geometry.grid, n_rows, groups, slabs
+        return prompt, self.geometry.grid, self._n_rows(prompt), groups, slabs
 
 
 def _key_group(acc: torch.Tensor, slab: LayerSlab, head_sel: int = -1) -> _native.DaamKeyGroup:
@@ -600,13 +656,31 @@ class PipelineHooker(ObjectHooker):
             prompts = list(prompt)
             if len(prompts) > 1 and not tr.batch_prompts:
                 raise ValueError('Only single prompt generation is supported for heat map computation.')
+        negatives = hk_self._negative_prompts(prompt, args, kwargs, len(prompts)) if tr.negative else []
         hk_self.heat_maps.clear()
         tr._restart_history()
         if len(prompts) != len(tr.last_prompts):    # slabs are laid out [prompts][images * heads]: re-derive them
             tr._layer_state.clear()
         tr.last_prompt = prompts[0]
         tr.last_prompts = prompts
+        tr.last_negative_prompts = negatives
         return hk_self.monkey_super('check_inputs', prompt, *args, **kwargs)
+
+    def _negative_prompts(hk_self, prompt, args, kwargs, n: int) -> List[str]:
+        """The negative text of each of the ``n`` prompts, from the ``negative_prompt`` argument of the
+        ``check_inputs`` call: bound by name to the wrapped method's signature, because pipelines pass it positionally
+        at different places (diffusers' SD: ``(prompt, height, width, callback_steps, negative_prompt, ...)``; SDXL has
+        ``prompt_2`` before it). None or absent is the empty prompt, which is what the pipeline encodes then."""
+        bound = inspect.signature(hk_self._replaced['check_inputs']).bind(prompt, *args, **kwargs)
+        negative = bound.arguments.get('negative_prompt', kwargs.get('negative_prompt'))
+        if negative is None:
+            return [''] * n
+        if isinstance(negative, str):
+            return [negative] * n
+        negatives = list(negative)
+        if len(negatives) != n:
+            raise ValueError(f'negative_prompt has {len(negatives)} entries for {n} prompts')
+        return negatives
 
     def _hook_impl(self):
         self.monkey_patch('run_safety_checker', self._hooked_run_safety_checker, strict=False)  # absent in SDXL
