@@ -22,9 +22,16 @@ ABI_VERSION = 4
 E_INVALID, E_UNSUPPORTED, E_CUDA = -1, -2, -3
 TOKENS = 77
 EXPAND_SCRATCH_FLOATS = 64   # DAAM_EXPAND_SCRATCH_FLOATS: per word
+MAX_SEGMENT_WORDS = 96       # daam_segment_words: labels 1..96 plus background 0 fit a byte
+
+
+def segment_scratch_floats(n_maps: int, n_words: int) -> int:
+    """``DAAM_SEGMENT_SCRATCH_FLOATS(n_maps, n_words)``."""
+    return 64 * n_maps * n_words
 
 EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize',
            'daam_finalize_per_key', 'daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
+           'daam_segment_words',
            'daam_side_launcher_create', 'daam_side_launcher_destroy',
            'daam_side_launcher_launch', 'daam_side_launcher_join', 'daam_side_launcher_idle', 'daam_abi_version',
            'daam_last_error', 'daam_device_info', 'daam_launch_count')
@@ -98,6 +105,9 @@ def load() -> ctypes.CDLL:
     lib.daam_expand_words.argtypes = [vp, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32, i32,
                                       i32, f32, vp, vp, vp, vp]
     lib.daam_expand_words.restype = ctypes.c_int
+    lib.daam_segment_words.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
+                                       i32, i32, f32, vp, vp, vp, vp, vp]
+    lib.daam_segment_words.restype = ctypes.c_int
     lib.daam_side_launcher_create.argtypes = [ctypes.POINTER(vp)]
     lib.daam_side_launcher_create.restype = ctypes.c_int
     lib.daam_side_launcher_destroy.argtypes = [vp]
@@ -274,18 +284,37 @@ def expand_words(maps_ptr: int, n_rows: int, x, rows_per_word: Sequence[Sequence
                  stream: int):
     """``rows_per_word[w]``: the rows of ``maps`` word ``w`` averages (already offset for SOS)."""
     h, w = map_size(x)
-    flat = [r for rows in rows_per_word for r in rows]
-    begin = [0]
-    for rows in rows_per_word:
-        begin.append(begin[-1] + len(rows))
-    rows_arr = (ctypes.c_int32 * max(len(flat), 1))(*flat)
-    begin_arr = (ctypes.c_int32 * len(begin))(*begin)
+    rows_arr, begin_arr = _row_lists(rows_per_word)
     use_thr = bool(threshold)   # the reference's `if threshold:` (daam/heatmap.py:87)
     _check(load().daam_expand_words(ctypes.c_void_p(maps_ptr), n_rows, h, w, rows_arr, begin_arr,
                                     len(rows_per_word), out_h, out_w, int(bool(absolute)), int(use_thr),
                                     float(threshold) if use_thr else 0.0,
                                     ctypes.c_void_p(word_maps_ptr) if word_maps_ptr else None,
                                     ctypes.c_void_p(out_ptr), ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
+
+
+def _row_lists(rows_per_word: Sequence[Sequence[int]]):
+    """``(rows, row_begin)`` host arrays of a word list: word ``w`` owns ``rows[row_begin[w] .. row_begin[w + 1])``."""
+    flat = [r for rows in rows_per_word for r in rows]
+    begin = [0]
+    for rows in rows_per_word:
+        begin.append(begin[-1] + len(rows))
+    return (ctypes.c_int32 * max(len(flat), 1))(*flat), (ctypes.c_int32 * len(begin))(*begin)
+
+
+def segment_words(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int,
+                  out_w: int, absolute: bool, threshold: Optional[float], word_maps_ptr: int, labels_ptr: int,
+                  scores_ptr: int, scratch_ptr: int, stream: int):
+    """``daam_segment_words`` over ``n_maps`` maps ``[n_rows, h, w]`` back to back; ``rows_per_word`` as for
+    :func:`expand_words`."""
+    h, w = map_size(x)
+    rows_arr, begin_arr = _row_lists(rows_per_word)
+    use_thr = bool(threshold)   # the reference's `if threshold:` (daam/heatmap.py:87), as expand_words resolves it
+    _check(load().daam_segment_words(ctypes.c_void_p(maps_ptr), n_maps, n_rows, h, w, rows_arr, begin_arr,
+                                     len(rows_per_word), out_h, out_w, int(bool(absolute)), int(use_thr),
+                                     float(threshold) if use_thr else 0.0, ctypes.c_void_p(word_maps_ptr),
+                                     ctypes.c_void_p(labels_ptr), ctypes.c_void_p(scores_ptr),
+                                     ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
 
 
 def device_info():

@@ -10,6 +10,7 @@
 #include <math.h>
 #include <stdlib.h>
 
+#include <algorithm>
 #include <mutex>
 
 #include "common.cuh"
@@ -472,6 +473,17 @@ __device__ __forceinline__ float bicubic_shared(const float* sm, int w, const Ta
   return v;
 }
 
+// The word map at pixel i: the mean of rows[r0 .. r1) of maps [*][xx] (heatmap.py:121-123). Shared by the expand and
+// segment kernels, so that their word maps are the same bits.
+__device__ __forceinline__ float word_mean(const float* __restrict__ maps, const int* rows, int r0, int r1, int xx, int i) {
+  float s = 0.f;
+  for (int r = r0; r < r1; ++r) s += __ldg(maps + (long long)rows[r] * xx + i);
+  return s / (float)(r1 - r0);
+}
+
+// expand_as's min-max normalisation (heatmap.py:88-89)
+__device__ __forceinline__ float minmax_normalize(float v, float lo, float hi) { return (v - lo) / (hi - lo + 1e-8f); }
+
 __global__ void __launch_bounds__(256) expand_words_kernel(const __grid_constant__ ExpandWordsParams P) {
   extern __shared__ __align__(16) float wm[];          // the word map [mh][mw]
   __shared__ float red_lo[8], red_hi[8];
@@ -479,9 +491,7 @@ __global__ void __launch_bounds__(256) expand_words_kernel(const __grid_constant
   const int mh = P.mh, mw = P.mw, xx = mh * mw, n = P.oh * P.ow;
   const int r0 = P.row_begin[word], r1 = P.row_begin[word + 1];
   for (int i = threadIdx.x; i < xx; i += blockDim.x) {
-    float s = 0.f;
-    for (int r = r0; r < r1; ++r) s += __ldg(P.maps + (long long)P.rows[r] * xx + i);
-    s = s / (float)(r1 - r0);
+    const float s = word_mean(P.maps, P.rows, r0, r1, xx, i);
     wm[i] = s;
     if (chunk == 0 && P.word_maps) P.word_maps[(long long)word * xx + i] = s;
   }
@@ -523,9 +533,140 @@ __global__ void __launch_bounds__(256) expand_words_kernel(const __grid_constant
   for (int o = begin + threadIdx.x; o < end; o += blockDim.x) {
     const int oy = o / P.ow, ox = o - oy * P.ow;
     float v = bicubic_shared(wm, mw, make_taps(oy, mh, P.oh), make_taps(ox, mw, P.ow));
-    if (!P.absolute) v = (v - lo) / (hi - lo + 1e-8f);
+    if (!P.absolute) v = minmax_normalize(v, lo, hi);
     if (P.use_threshold) v = v > P.threshold ? 1.f : 0.f;
     dst[o] = v;
+  }
+}
+
+// ---- word segmentation: a per-pixel word label for a word list --------------------------------------------------
+// labels[p] = 1 + argmax_w m[w][p] (lowest w on ties), or 0 where use_threshold and the max is not > threshold;
+// scores[p] = max_w m[w][p], with m[w] what expand_words_kernel writes for word w without threshold. For n_maps global
+// maps back to back (one, or every step of a time-resolved history) in two launches whatever n_maps and n_words:
+//  1. segment_minmax_kernel, CTA = (map, word, chunk of output pixels): the word map (word_mean) goes to `word_maps`
+//     and, unless `absolute`, the chunk's min / max of the interpolated map to `scratch`;
+//  2. segment_label_kernel, CTA = (output tile, map): every word's min / max is reduced from its chunks, the source
+//     window under the tile of a pass of words is staged in shared memory from `word_maps`, and each pixel keeps the
+//     running max / argmax in registers while the words are interpolated.
+// Same taps, bicubic_shared, word_mean and minmax_normalize as expand_words_kernel: the scores are its values. The
+// [n_words][out_h][out_w] stack is never written. Deterministic (no atomics).
+constexpr int kSegTileH = 16, kSegTileW = 64;      // output tile of one label CTA
+constexpr int kSegPix = kSegTileH * kSegTileW / 256;   // output pixels per thread
+constexpr int kSegStageFloats = 12288;              // staged windows per pass when they fit (48 KB)
+
+struct SegmentParams {
+  const float* maps;                    // [n_maps][n_map_rows][mh][mw]
+  float* word_maps;                     // [n_maps][n_words][mh][mw]
+  unsigned char* labels;                // [n_maps][oh][ow]
+  float* scores;                        // [n_maps][oh][ow]
+  float* scratch;                       // [n_maps][n_words][chunks][2]
+  long long map_stride;                 // n_map_rows * mh * mw
+  int mh, mw, oh, ow, n_words, chunks, absolute, use_threshold;
+  float threshold;
+  int words_per_pass;                   // words whose windows are staged at once
+  int row_begin[kMaxWords + 1];
+  int rows[kMaxWordRows];
+};
+
+// grid: n_maps * n_words * chunks; dynamic smem: the word map [mh][mw]
+__global__ void __launch_bounds__(256) segment_minmax_kernel(const __grid_constant__ SegmentParams P) {
+  extern __shared__ __align__(16) float wm[];
+  __shared__ float red_lo[8], red_hi[8];
+  const int chunk = blockIdx.x % P.chunks, mword = blockIdx.x / P.chunks;   // mword = map * n_words + word
+  const int word = mword % P.n_words, map = mword / P.n_words;
+  const int mh = P.mh, mw = P.mw, xx = mh * mw, n = P.oh * P.ow;
+  const int r0 = P.row_begin[word], r1 = P.row_begin[word + 1];
+  const float* maps = P.maps + (long long)map * P.map_stride;
+  float* word_map = P.word_maps + (long long)mword * xx;
+  for (int i = threadIdx.x; i < xx; i += blockDim.x) {
+    const float s = word_mean(maps, P.rows, r0, r1, xx, i);
+    wm[i] = s;
+    if (chunk == 0) word_map[i] = s;
+  }
+  if (P.absolute) return;
+  __syncthreads();
+  const int per = (n + P.chunks - 1) / P.chunks;
+  const int begin = chunk * per, end = min(n, begin + per);
+  float lo = INFINITY, hi = -INFINITY;
+  for (int o = begin + threadIdx.x; o < end; o += blockDim.x) {
+    const int oy = o / P.ow, ox = o - oy * P.ow;
+    const float v = bicubic_shared(wm, mw, make_taps(oy, mh, P.oh), make_taps(ox, mw, P.ow));
+    lo = fminf(lo, v); hi = fmaxf(hi, v);
+  }
+#pragma unroll
+  for (int s = 16; s > 0; s >>= 1) {
+    lo = fminf(lo, __shfl_xor_sync(0xffffffffu, lo, s));
+    hi = fmaxf(hi, __shfl_xor_sync(0xffffffffu, hi, s));
+  }
+  if ((threadIdx.x & 31) == 0) { red_lo[threadIdx.x >> 5] = lo; red_hi[threadIdx.x >> 5] = hi; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int i = 1; i < (int)blockDim.x / 32; ++i) { lo = fminf(lo, red_lo[i]); hi = fmaxf(hi, red_hi[i]); }
+    float* slot = P.scratch + 2 * ((long long)mword * P.chunks + chunk);
+    slot[0] = lo; slot[1] = hi;
+  }
+}
+
+// grid: (tiles of kSegTileH x kSegTileW output pixels, n_maps); dynamic smem: words_per_pass source windows
+__global__ void __launch_bounds__(256) segment_label_kernel(const __grid_constant__ SegmentParams P) {
+  extern __shared__ __align__(16) float win[];
+  __shared__ float s_lo[kMaxWords], s_hi[kMaxWords];
+  const int map = blockIdx.y, mh = P.mh, mw = P.mw, oh = P.oh, ow = P.ow, n_words = P.n_words;
+  const int tiles_x = (ow + kSegTileW - 1) / kSegTileW;
+  const int y0 = (blockIdx.x / tiles_x) * kSegTileH, x0 = (blockIdx.x % tiles_x) * kSegTileW;
+  const int th = min(kSegTileH, oh - y0), tw = min(kSegTileW, ow - x0);
+  // the source rows / columns the tile's taps read: taps move monotonically with the output index
+  const int wy = make_taps(y0, mh, oh).idx[0], wx = make_taps(x0, mw, ow).idx[0];
+  const int wh = make_taps(y0 + th - 1, mh, oh).idx[3] - wy + 1, ww = make_taps(x0 + tw - 1, mw, ow).idx[3] - wx + 1;
+  const int wn = wh * ww;
+  if (!P.absolute) {
+    for (int w = threadIdx.x; w < n_words; w += blockDim.x) {   // chunks in a fixed order
+      const float* slots = P.scratch + 2 * ((long long)map * n_words + w) * P.chunks;
+      float lo = INFINITY, hi = -INFINITY;
+      for (int c = 0; c < P.chunks; ++c) { lo = fminf(lo, slots[2 * c]); hi = fmaxf(hi, slots[2 * c + 1]); }
+      s_lo[w] = lo; s_hi[w] = hi;
+    }
+  }
+  const float* word_maps = P.word_maps + (long long)map * n_words * mh * mw;
+  float best[kSegPix];
+  int arg[kSegPix];
+#pragma unroll
+  for (int k = 0; k < kSegPix; ++k) { best[k] = -INFINITY; arg[k] = 0; }
+  for (int w0 = 0; w0 < n_words; w0 += P.words_per_pass) {
+    const int nw = min(P.words_per_pass, n_words - w0);
+    __syncthreads();                                   // the previous pass has read its windows
+    for (int i = threadIdx.x; i < nw * wn; i += blockDim.x) {
+      const int wi = i / wn, r = i - wi * wn, y = r / ww, x = r - y * ww;
+      win[i] = __ldg(word_maps + ((long long)(w0 + wi) * mh + wy + y) * mw + wx + x);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < kSegPix; ++k) {
+      const int p = threadIdx.x + 256 * k;
+      if (p < th * tw) {
+        const int py = p / tw;
+        Taps ty = make_taps(y0 + py, mh, oh), tx = make_taps(x0 + p - py * tw, mw, ow);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) { ty.idx[j] -= wy; tx.idx[j] -= wx; }
+        for (int wi = 0; wi < nw; ++wi) {
+          const int w = w0 + wi;
+          float v = bicubic_shared(win + wi * wn, ww, ty, tx);
+          if (!P.absolute) v = minmax_normalize(v, s_lo[w], s_hi[w]);
+          if (w == 0 || v > best[k]) { best[k] = v; arg[k] = w; }   // strict: the lowest word wins a tie
+        }
+      }
+    }
+  }
+  const long long base = (long long)map * oh * ow;
+#pragma unroll
+  for (int k = 0; k < kSegPix; ++k) {
+    const int p = threadIdx.x + 256 * k;
+    if (p < th * tw) {
+      const int py = p / tw;
+      const long long o = base + (long long)(y0 + py) * ow + x0 + p - py * tw;
+      P.scores[o] = best[k];
+      P.labels[o] = (!P.use_threshold || best[k] > P.threshold) ? (unsigned char)(arg[k] + 1) : (unsigned char)0;
+    }
   }
 }
 
@@ -772,6 +913,69 @@ extern "C" int daam_expand_words(const float* global_maps, int32_t n_rows, int32
                                  float* scratch, void* stream) {
   return expand_words_impl("daam_expand_words", global_maps, n_rows, mh, mw, rows, row_begin, n_words, out_h, out_w,
                            absolute, use_threshold, threshold, word_maps, out, scratch, stream);
+}
+
+extern "C" int daam_segment_words(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t mh, int32_t mw,
+                                  const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h,
+                                  int32_t out_w, int32_t absolute, int32_t use_threshold, float threshold,
+                                  float* word_maps, uint8_t* labels, float* scores, float* scratch, void* stream_) {
+  const char* name = "daam_segment_words";
+  if (!global_maps || !rows || !row_begin || !word_maps || !labels || !scores || !scratch || n_maps <= 0 || mh <= 0 ||
+      mw <= 0 || out_h <= 0 || out_w <= 0 || n_rows <= 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
+  if (n_words <= 0) { set_error("%s: empty word list", name); return DAAM_E_INVALID; }
+  if (n_words > kMaxWords) { set_error("%s: %d words > %d", name, n_words, kMaxWords); return DAAM_E_UNSUPPORTED; }
+  if (row_begin[0] != 0 || row_begin[n_words] > kMaxWordRows) { set_error("%s: row_begin must start at 0 and select at most %d rows", name, kMaxWordRows); return DAAM_E_UNSUPPORTED; }
+  if ((size_t)mh * mw * sizeof(float) > 200 * 1024) { set_error("%s: a %d x %d map does not fit shared memory", name, mh, mw); return DAAM_E_UNSUPPORTED; }
+  if (n_maps > 65535) { set_error("%s: %d maps > 65535", name, n_maps); return DAAM_E_UNSUPPORTED; }
+  if ((long long)out_h * out_w > (1LL << 30)) { set_error("%s: a %d x %d output is more than 2^30 pixels", name, out_h, out_w); return DAAM_E_UNSUPPORTED; }
+  DeviceInfo dev;
+  if (int rc = get_device_info(&dev)) return rc;
+  static thread_local SegmentParams p;
+  for (int w = 0; w < n_words; ++w) {
+    if (row_begin[w + 1] <= row_begin[w]) { set_error("%s: word %d selects no row", name, w); return DAAM_E_INVALID; }
+    p.row_begin[w] = row_begin[w];
+  }
+  p.row_begin[n_words] = row_begin[n_words];
+  for (int i = 0; i < row_begin[n_words]; ++i) {
+    int r = rows[i];
+    if (r < 0) r += n_rows;   // torch-style negative index
+    if (r < 0 || r >= n_rows) { set_error("%s: row %d out of range [0, %d)", name, rows[i], n_rows); return DAAM_E_INVALID; }
+    p.rows[i] = r;
+  }
+  p.maps = global_maps; p.word_maps = word_maps; p.labels = labels; p.scores = scores; p.scratch = scratch;
+  p.map_stride = (long long)n_rows * mh * mw;
+  p.mh = mh; p.mw = mw; p.oh = out_h; p.ow = out_w; p.n_words = n_words;
+  p.absolute = absolute ? 1 : 0; p.use_threshold = use_threshold ? 1 : 0; p.threshold = threshold;
+  // launch 1: enough (map, word, chunk) CTAs for a few waves, at most kMaxChunks per word and one per 256 pixels
+  const long long n = (long long)out_h * out_w, mwords = (long long)n_maps * n_words;
+  long long chunks = (4LL * dev.sm_count + mwords - 1) / mwords;
+  if (chunks > kMaxChunks) chunks = kMaxChunks;
+  if (chunks > (n + 255) / 256) chunks = (n + 255) / 256;
+  if (chunks < 1 || p.absolute) chunks = 1;
+  p.chunks = (int)chunks;
+  // launch 2: a tile's source window is at most ceil(tile * map / out) + 4 rows (columns), and no more than the map
+  const int win_h = std::min<int>(mh, (int)ceil((double)kSegTileH * mh / out_h) + 5);
+  const int win_w = std::min<int>(mw, (int)ceil((double)kSegTileW * mw / out_w) + 5);
+  const int win = win_h * win_w;
+  p.words_per_pass = std::max(1, std::min(n_words, kSegStageFloats / win));
+  const size_t smem1 = (size_t)mh * mw * sizeof(float), smem2 = (size_t)p.words_per_pass * win * sizeof(float);
+  static std::once_flag attr_once[64];
+  cudaError_t attr_err = cudaSuccess;
+  std::call_once(attr_once[dev.device & 63], [&] {
+    attr_err = cudaFuncSetAttribute(segment_minmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    if (attr_err == cudaSuccess)
+      attr_err = cudaFuncSetAttribute(segment_label_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+  });
+  DAAM_CUDA_TRY(attr_err);
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  segment_minmax_kernel<<<(unsigned)(mwords * chunks), 256, smem1, stream>>>(p);
+  DAAM_CUDA_TRY(cudaGetLastError());
+  count_launch();
+  const int tiles = ((out_h + kSegTileH - 1) / kSegTileH) * ((out_w + kSegTileW - 1) / kSegTileW);
+  segment_label_kernel<<<dim3(tiles, n_maps), 256, smem2, stream>>>(p);
+  DAAM_CUDA_TRY(cudaGetLastError());
+  count_launch();
+  return DAAM_OK;
 }
 
 // one word whose "rows" are the word map itself

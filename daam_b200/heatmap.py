@@ -349,15 +349,10 @@ class GlobalHeatMap:
         ``expand_as``; ``to_cpu=False`` keeps it on the device until the caller needs it). ``word_idx`` may be a list
         parallel to ``words``. Raises the reference's ``ValueError`` for a word that is not in the prompt."""
         words = list(words)
-        idxs = list(word_idx) if isinstance(word_idx, (list, tuple)) else [word_idx] * len(words)
-        merged = [compute_token_merge_indices(self.tokenizer, self.prompt, w, i, offset_idx) for w, i in zip(words, idxs)]
         maps = self.heat_maps
+        merged = _word_rows(self.tokenizer, self.prompt, words, word_idx, offset_idx, maps.shape[0])
         _require_cuda(maps, 'GlobalHeatMap.expand_words')
         n_rows, grid = maps.shape[0], tuple(maps.shape[-2:])
-        for rows, _ in merged:
-            for r in rows:
-                if not -n_rows <= r < n_rows:
-                    raise IndexError(f'index {r} is out of bounds for dimension 0 with size {n_rows}')
         out_h, out_w = _image_size(image, *grid)
         if not words:
             return [], torch.empty((0, out_h, out_w))
@@ -371,6 +366,67 @@ class GlobalHeatMap:
                                  threshold, word_maps.data_ptr(), out.data_ptr(), scratch.data_ptr(), _stream_ptr(dev))
         whms = [WordHeatMap(word_maps[i], w, idx) for i, (w, (_, idx)) in enumerate(zip(words, merged))]
         return whms, (out.cpu() if to_cpu else out)
+
+    def segment(self, words, image, absolute: bool = False, threshold: Optional[float] = None, word_idx=None,
+                offset_idx: int = 0, to_cpu: bool = True):
+        """A word label per image pixel: which word of ``words`` owns it, or background. With ``m`` the
+        ``[len(words), H, W]`` that ``expand_words(words, image, absolute, word_idx=word_idx, offset_idx=offset_idx)``
+        returns (no threshold), ``scores = m.max(0).values`` and ``labels = m.argmax(0) + 1`` (the first word on ties),
+        set to 0 (background) where ``threshold`` is in effect (Python truthiness, as in ``expand_words``) and
+        ``scores > threshold`` fails -- the reference's segmentation rule (``daam/evaluate.py``, tau = 0.4) over a word
+        list. Two fused launches; the ``[len(words), H, W]`` stack is never materialised.
+
+        Returns ``(word_heat_maps, labels, scores)``: the list of :class:`WordHeatMap` that ``expand_words`` returns,
+        ``labels`` uint8 and ``scores`` fp32, both ``(H, W)`` ordered as ``expand_words`` orders the image size (CPU by
+        default, ``to_cpu=False`` keeps them on the device). At most 96 words; repeated words tie and the first wins.
+        An empty list gives all-background labels and -inf scores (the max of nothing). Raises the reference's
+        ``ValueError`` for a word that is not in the prompt."""
+        words = list(words)
+        word_maps, merged, labels, scores = _segment(self.tokenizer, self.prompt, self.heat_maps[None], words, image,
+                                                     absolute, threshold, word_idx, offset_idx, to_cpu,
+                                                     'GlobalHeatMap.segment')
+        whms = [WordHeatMap(word_maps[0, i], w, idx) for i, (w, (_, idx)) in enumerate(zip(words, merged))]
+        return whms, labels[0], scores[0]
+
+
+def _word_rows(tokenizer, prompt: str, words: List[str], word_idx, offset_idx: int, n_rows: int):
+    """``compute_token_merge_indices`` of every word (``word_idx`` may be a list parallel to ``words``), with the
+    row range checked the way torch's advanced indexing would."""
+    idxs = list(word_idx) if isinstance(word_idx, (list, tuple)) else [word_idx] * len(words)
+    merged = [compute_token_merge_indices(tokenizer, prompt, w, i, offset_idx) for w, i in zip(words, idxs)]
+    for rows, _ in merged:
+        for r in rows:
+            if not -n_rows <= r < n_rows:
+                raise IndexError(f'index {r} is out of bounds for dimension 0 with size {n_rows}')
+    return merged
+
+
+def _segment(tokenizer, prompt: str, maps: torch.Tensor, words, image, absolute, threshold, word_idx, offset_idx: int,
+             to_cpu: bool, what: str):
+    """``daam_segment_words`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(word_maps, merged, labels,
+    scores)``: the device word heat maps ``[n_maps, len(words), xh, xw]``, ``compute_token_merge_indices`` of every
+    word, and ``labels`` / ``scores`` ``[n_maps, H, W]``."""
+    n_maps, n_rows, grid = maps.shape[0], maps.shape[1], tuple(maps.shape[-2:])
+    merged = _word_rows(tokenizer, prompt, words, word_idx, offset_idx, n_rows)
+    _require_cuda(maps, what)
+    out_h, out_w = _image_size(image, *grid)
+    dev = maps.device
+    word_maps = torch.empty((n_maps, len(words)) + grid, dtype=torch.float32, device=dev)
+    if not words or n_maps == 0:
+        labels = torch.zeros((n_maps, out_h, out_w), dtype=torch.uint8, device=dev)
+        scores = torch.full((n_maps, out_h, out_w), float('-inf'), device=dev)
+        return word_maps, merged, (labels.cpu() if to_cpu else labels), (scores.cpu() if to_cpu else scores)
+    maps = maps.detach().float().contiguous()
+    labels = torch.empty((n_maps, out_h, out_w), dtype=torch.uint8, device=dev)
+    scores = torch.empty((n_maps, out_h, out_w), dtype=torch.float32, device=dev)
+    scratch = torch.empty(_native.segment_scratch_floats(n_maps, len(words)), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _native.segment_words(maps.data_ptr(), n_maps, n_rows, grid, [rows for rows, _ in merged], out_h, out_w,
+                              absolute, threshold, word_maps.data_ptr(), labels.data_ptr(), scores.data_ptr(),
+                              scratch.data_ptr(), _stream_ptr(dev))
+    if to_cpu:
+        labels, scores = labels.cpu(), scores.cpu()
+    return word_maps, merged, labels, scores
 
 
 class TimeHeatMaps:
@@ -408,3 +464,14 @@ class TimeHeatMaps:
             for t in range(steps):
                 _native.word_heat_map(maps[t].data_ptr(), n_rows, grid, rows, out[t].data_ptr(), stream)
         return out
+
+    def segment(self, words, image, absolute: bool = False, threshold: Optional[float] = None, word_idx=None,
+                offset_idx: int = 0, to_cpu: bool = True):
+        """:meth:`GlobalHeatMap.segment` for every step in one call (two launches whatever the step count): returns
+        ``(word_maps, labels, scores)`` with ``word_maps`` the device ``[steps, len(words), xh, xw]`` word heat maps and
+        ``labels`` / ``scores`` ``[steps, H, W]``; row ``t`` equals ``self[t].segment(...)`` bit for bit (min / max
+        normalisation per step and word)."""
+        word_maps, _, labels, scores = _segment(self.tokenizer, self.prompt, self.heat_maps, list(words), image,
+                                                absolute, threshold, word_idx, offset_idx, to_cpu,
+                                                'TimeHeatMaps.segment')
+        return word_maps, labels, scores

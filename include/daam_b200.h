@@ -29,7 +29,8 @@ extern "C" {
                                           (later, additive: daam_accumulate_steps, daam_normalize_maps,
                                           daam_accumulate_range)
                                        4: the finalize family takes (map_h, map_w); the _rect names are gone
-                                          (later, additive: layers with hw not a multiple of 4 are accepted) */
+                                          (later, additive: layers with hw not a multiple of 4 are accepted;
+                                          daam_segment_words) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
 
@@ -242,6 +243,27 @@ int daam_expand_words(const float* global_maps, int32_t n_rows, int32_t map_h, i
                       const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w, int32_t absolute,
                       int32_t use_threshold, float threshold, float* word_maps, float* out, float* scratch,
                       void* stream);
+
+/*
+ * Word segmentation: one label per pixel for a word list, on each of n_maps global maps stored back to back
+ * (global_maps [n_maps][n_rows][map_h][map_w]; e.g. every step of a time-resolved history). With m[w] what
+ * daam_expand_words writes for word w without threshold (same rows / row_begin, host arrays shared by all maps):
+ *   scores[i][p] = max_w m[w][p]                                  (bit-identical to daam_expand_words' values)
+ *   labels[i][p] = 1 + argmax_w m[w][p], the lowest w on ties; 0 (background) where use_threshold and
+ *                  !(scores[i][p] > threshold)
+ * min / max run per (map, word). word_maps: device fp32 [n_maps][n_words][map_h][map_w] (required: the second kernel
+ * reads them); labels: device uint8 [n_maps][out_h][out_w]; scores: device fp32 [n_maps][out_h][out_w]; scratch:
+ * device, >= DAAM_SEGMENT_SCRATCH_FLOATS(n_maps, n_words) floats. Two launches whatever n_maps and n_words; the
+ * [n_words][out_h][out_w] stack is never written. Deterministic.
+ * Limits (DAAM_E_UNSUPPORTED): n_words <= 96 (labels 1..96 plus background fit a byte), row_begin[n_words] <= 320,
+ * map_h * map_w * 4 bytes <= 200 KB, n_maps <= 65535, out_h * out_w <= 2^30. Any output size, smaller than the map
+ * included. DAAM_E_INVALID: null pointer, non-positive size, empty word list, a word without rows, a row out of range.
+ */
+#define DAAM_SEGMENT_SCRATCH_FLOATS(n_maps, n_words) (64 * (n_maps) * (n_words))
+int daam_segment_words(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t map_h, int32_t map_w,
+                       const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w,
+                       int32_t absolute, int32_t use_threshold, float threshold, float* word_maps, uint8_t* labels,
+                       float* scores, float* scratch, void* stream);
 
 /* Library / device introspection. */
 int daam_abi_version(void);
