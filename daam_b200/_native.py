@@ -30,7 +30,7 @@ def segment_scratch_floats(n_maps: int, n_words: int) -> int:
     return 64 * n_maps * n_words
 
 EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize',
-           'daam_finalize_per_key', 'daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
+           'daam_finalize_maps', 'daam_finalize_per_key','daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
            'daam_segment_words',
            'daam_side_launcher_create', 'daam_side_launcher_destroy',
            'daam_side_launcher_launch', 'daam_side_launcher_join', 'daam_side_launcher_idle', 'daam_abi_version',
@@ -50,11 +50,24 @@ class DaamLayer(ctypes.Structure):
 
 
 class DaamKeyGroup(ctypes.Structure):
-    """``struct daam_key_group`` (include/daam_b200.h)."""
+    """``struct daam_key_group`` (include/daam_b200.h). ``n_blocks`` is read by ``daam_finalize_maps`` only; its old
+    name ``reserved`` still works."""
     _fields_ = [
         ('acc', ctypes.c_void_p), ('heads', ctypes.c_int32), ('h', ctypes.c_int32), ('w', ctypes.c_int32),
-        ('tokens', ctypes.c_int32), ('head_sel', ctypes.c_int32), ('reserved', ctypes.c_int32),
+        ('tokens', ctypes.c_int32), ('head_sel', ctypes.c_int32), ('n_blocks', ctypes.c_int32),
     ]
+    reserved = property(lambda self: self.n_blocks, lambda self, v: setattr(self, 'n_blocks', v))
+
+
+class DaamMapSel(ctypes.Structure):
+    """``struct daam_map_sel`` (include/daam_b200.h): one output map of ``daam_finalize_maps``."""
+    _fields_ = [
+        ('block_begin', ctypes.c_int32), ('block_count', ctypes.c_int32), ('n_rows', ctypes.c_int32),
+        ('reserved', ctypes.c_int32), ('out', ctypes.c_void_p),
+    ]
+
+
+FINALIZE_MAX_MAPS = 64   # DAAM_FINALIZE_MAX_MAPS: maps per daam_finalize_maps call
 
 
 class NativeError(RuntimeError):
@@ -96,6 +109,9 @@ def load() -> ctypes.CDLL:
     lib.daam_accumulate_probs.restype = ctypes.c_int
     lib.daam_finalize.argtypes = [ctypes.POINTER(DaamKeyGroup), i32, i32, i32, i32, i32, vp, vp]
     lib.daam_finalize.restype = ctypes.c_int
+    lib.daam_finalize_maps.argtypes = [ctypes.POINTER(DaamKeyGroup), i32, ctypes.POINTER(DaamMapSel), i32, i32, i32,
+                                       i32, vp]
+    lib.daam_finalize_maps.restype = ctypes.c_int
     lib.daam_finalize_per_key.argtypes = [ctypes.POINTER(DaamKeyGroup), i32, i32, i32, i32, i32, vp, vp]
     lib.daam_finalize_per_key.restype = ctypes.c_int
     lib.daam_word_heat_map.argtypes = [vp, i32, i32, i32, ctypes.POINTER(i32), i32, vp, vp]
@@ -257,6 +273,19 @@ def _finalize(entry: str, groups: Sequence[DaamKeyGroup], x, n_rows: int, normal
 
 def finalize(groups: Sequence[DaamKeyGroup], x, n_rows: int, normalize: bool, out_ptr: int, stream: int):
     _finalize('daam_finalize', groups, x, n_rows, normalize, out_ptr, stream)
+
+
+def finalize_maps(groups: Sequence[DaamKeyGroup], maps: Sequence[DaamMapSel], x, normalize: bool, stream: int):
+    """``daam_finalize_maps``: ``groups`` with ``n_blocks`` set, one :class:`DaamMapSel` per output map. More than
+    :data:`FINALIZE_MAX_MAPS` maps go out in several calls, which changes no map's bits."""
+    h, w = map_size(x)
+    n = len(groups)
+    arr = (DaamKeyGroup * max(n, 1))(*groups)
+    lib = load()
+    for i in range(0, max(len(maps), 1), FINALIZE_MAX_MAPS):
+        part = maps[i:i + FINALIZE_MAX_MAPS]
+        sel = (DaamMapSel * max(len(part), 1))(*part)
+        _check(lib.daam_finalize_maps(arr, n, sel, len(part), h, w, int(bool(normalize)), ctypes.c_void_p(stream)))
 
 
 def finalize_per_key(groups: Sequence[DaamKeyGroup], x, n_rows: int, normalize: bool, out_ptr: int, stream: int):

@@ -20,10 +20,20 @@ namespace {
 
 constexpr int kMaxGroups = 160;   // key groups (layer x prompt slices) per finalize launch
 constexpr int kMaxRows = 128;     // selected rows of a word map
+constexpr int kMaxMaps = DAAM_FINALIZE_MAX_MAPS;   // output maps per finalize launch
+
+// One output map of a finalize launch: blocks [block_begin, block_begin + block_count) of every group, i.e. the keys
+// of the expanded group list `for g: for b: {acc_g + b * heads_g * tokens_g * h_g * w_g, heads_g, head_sel_g}`.
+struct MapSel {
+  float* out;                             // [n_rows][oh][ow]
+  int block_begin, block_count, n_rows, n_keys;
+  int band_rows;                          // fast kernel only: 8 or 4 (daam_finalize's rule for this map's n_rows)
+};
 
 struct FinalizeParams {
-  int n_groups, oh, ow, n_rows, n_keys;   // output map [oh][ow]
+  int n_groups, oh, ow, n_maps;           // output maps [oh][ow]
   daam_key_group g[kMaxGroups];
+  MapSel map[kMaxMaps];                   // blockIdx.z selects the map
 };
 
 struct Taps {
@@ -64,12 +74,14 @@ __device__ __forceinline__ float bicubic_at(const float* __restrict__ src, int w
   return v;
 }
 
-// grid: (ceil(oh*ow / 256), n_rows). One thread = one output element (row t, pixel o); it walks every selected key.
-__global__ void __launch_bounds__(256) finalize_kernel(const __grid_constant__ FinalizeParams P, float* __restrict__ out) {
+// grid: (ceil(oh*ow / 256), max n_rows, n_maps). One thread = one output element (map, row t, pixel o); it walks every
+// selected key: group by group, block by block, head by head.
+__global__ void __launch_bounds__(256) finalize_kernel(const __grid_constant__ FinalizeParams P) {
   const int o = blockIdx.x * blockDim.x + threadIdx.x;
   const int t = blockIdx.y;
   const int oh = P.oh, ow = P.ow;
-  if (o >= oh * ow) return;
+  const MapSel& M = P.map[blockIdx.z];
+  if (o >= oh * ow || t >= M.n_rows) return;
   const int oy = o / ow, ox = o - oy * ow;
   float sum = 0.f;
   int ch = -1, cw = -1;
@@ -85,17 +97,19 @@ __global__ void __launch_bounds__(256) finalize_kernel(const __grid_constant__ F
       tx = make_taps(ox, G.w, ow);
       ch = G.h; cw = G.w;
     }
-    const float* base = G.acc + (long long)t * hw;
     const long long head_stride = (long long)G.tokens * hw;
-    if (same) {   // scale 1: the cubic weights are exactly (0, 1, 0, 0)
+    for (int b = M.block_begin; b < M.block_begin + M.block_count; ++b) {
+      const float* base = G.acc + (long long)b * G.heads * head_stride + (long long)t * hw;
+      if (same) {   // scale 1: the cubic weights are exactly (0, 1, 0, 0)
 #pragma unroll 4
-      for (int head = h0; head < h1; ++head) sum += fmaxf(__ldg(base + head * head_stride + o), 0.f);
-    } else {
+        for (int head = h0; head < h1; ++head) sum += fmaxf(__ldg(base + head * head_stride + o), 0.f);
+      } else {
 #pragma unroll 2
-      for (int head = h0; head < h1; ++head) sum += fmaxf(bicubic_at(base + head * head_stride, G.w, ty, tx), 0.f);
+        for (int head = h0; head < h1; ++head) sum += fmaxf(bicubic_at(base + head * head_stride, G.w, ty, tx), 0.f);
+      }
     }
   }
-  out[(long long)t * oh * ow + o] = sum / (float)P.n_keys;
+  M.out[(long long)t * oh * ow + o] = sum / (float)M.n_keys;
 }
 
 
@@ -340,47 +354,54 @@ __device__ __forceinline__ void class_pass_identity(const FinalizeParams& P, int
 
 struct ClassList {
   int n;
-  int band_rows;            // 8, or 4 when that is what fills the machine / keeps a band's source pixels within one CTA
   int kh[8], kw[8];         // distinct source sizes, each (oh / F, ow / F) with F = 1, 2 or 4
-  int key_begin[9];         // keys[] is ordered class by class: class c owns [key_begin[c], key_begin[c + 1])
-  int key_slot[kMaxGroups]; // where group g's first selected key goes in keys[]
+  // per block: keys[] is ordered class by class, and class c owns [key_begin[c], key_begin[c + 1]) times the map's
+  // block count; group g's keys start at key_slot[g] times the block count, block by block, head by head
+  int key_begin[9];
+  int key_slot[kMaxGroups];
 };
 
-// grid: (ceil(oh / band_rows) bands, n_rows); dynamic smem: two chunk buffers + the band tile (band_rows * ow floats)
+// grid: (ceil(oh / 4) bands, max n_rows, n_maps); a CTA past its map's bands or rows returns at once. Dynamic smem: two
+// chunk buffers + the band tile (the largest band_rows of the launch * ow floats)
 __global__ void __launch_bounds__(256, 2) finalize_fast_kernel(const __grid_constant__ FinalizeParams P,
-                                                               const __grid_constant__ ClassList C,
-                                                               float* __restrict__ out) {
+                                                               const __grid_constant__ ClassList C) {
   extern __shared__ __align__(16) float dyn[];
   __shared__ const float* keys[kMaxClassKeys];
   float* stage = dyn;                                  // 2 x kStageFloats
   float* tile = dyn + 2 * kStageFloats;
-  const int band = blockIdx.x, t = blockIdx.y, oh = P.oh, ow = P.ow, br = C.band_rows;
+  const MapSel& M = P.map[blockIdx.z];
+  const int band = blockIdx.x, t = blockIdx.y, oh = P.oh, ow = P.ow, br = M.band_rows, nb = M.block_count;
+  if (t >= M.n_rows || band * br >= oh) return;
   const int rows = min(br, oh - band * br);            // valid output rows of this band
   // key pointers (token row t) of every selected key, class by class; one thread per key group
   for (int g = threadIdx.x; g < P.n_groups; g += blockDim.x) {
     const daam_key_group& G = P.g[g];
-    const int h0 = G.head_sel < 0 ? 0 : G.head_sel;
-    const int h1 = G.head_sel < 0 ? G.heads : G.head_sel + 1;
+    const int per_block = G.head_sel < 0 ? G.heads : 1;
     const long long hw = (long long)G.h * G.w;
-    for (int head = h0; head < h1; ++head) keys[C.key_slot[g] + head - h0] = G.acc + ((long long)head * G.tokens + t) * hw;
+    const float** dst = keys + C.key_slot[g] * nb;
+    // key j of the group: head (block_begin * heads + j) of all heads, or head_sel of block block_begin + j
+    const long long first = G.head_sel < 0 ? (long long)M.block_begin * G.heads : (long long)M.block_begin * G.heads + G.head_sel;
+    const long long step = G.head_sel < 0 ? 1 : G.heads;
+    for (int j = 0; j < per_block * nb; ++j) dst[j] = G.acc + ((first + j * step) * G.tokens + t) * hw;
   }
   for (int i = threadIdx.x; i < br * ow; i += blockDim.x) tile[i] = 0.f;
   __syncthreads();
   bool prefetched = false;                             // chunk 0 of class c is already streaming into buffer 1
   for (int c = 0; c < C.n; ++c) {
-    const int kh = C.kh[c], kw = C.kw[c], f = ow / kw, nk = C.key_begin[c + 1] - C.key_begin[c];
-    const float* const* ck = keys + C.key_begin[c];
+    const int kh = C.kh[c], kw = C.kw[c], f = ow / kw, nk = (C.key_begin[c + 1] - C.key_begin[c]) * nb;
+    const float* const* ck = keys + C.key_begin[c] * nb;
     NextClass next = {0, 0, 0, 0, nullptr};
     if (c + 1 < C.n && C.kw[c + 1] != ow)
-      next = {C.kh[c + 1], C.kw[c + 1], ow / C.kw[c + 1], C.key_begin[c + 2] - C.key_begin[c + 1], keys + C.key_begin[c + 1]};
+      next = {C.kh[c + 1], C.kw[c + 1], ow / C.kw[c + 1], (C.key_begin[c + 2] - C.key_begin[c + 1]) * nb,
+              keys + C.key_begin[c + 1] * nb};
     if (f == 1) class_pass_identity(P, nk, band, br, rows, tile, ck, stage, next);
     else if (f == 2) class_pass<2>(P, kh, kw, nk, band, br, tile, ck, stage, prefetched, next);
     else class_pass<4>(P, kh, kw, nk, band, br, tile, ck, stage, prefetched, next);
     prefetched = next.f != 0;
   }
   __syncthreads();
-  float* dst = out + (long long)t * oh * ow + (long long)band * br * ow;
-  for (int i = threadIdx.x; i < rows * ow; i += blockDim.x) dst[i] = tile[i] / (float)P.n_keys;
+  float* dst = M.out + (long long)t * oh * ow + (long long)band * br * ow;
+  for (int i = threadIdx.x; i < rows * ow; i += blockDim.x) dst[i] = tile[i] / (float)M.n_keys;
 }
 
 // One output map per selected key (no mean): out[key][row][oh][ow] = clamp(bicubic(key[row])). grid: (ceil(oh*ow/256),
@@ -412,15 +433,31 @@ __global__ void __launch_bounds__(256) finalize_per_key_kernel(const __grid_cons
   out[((long long)key * P.n_rows + t) * oh * ow + o] = fmaxf(v, 0.f);
 }
 
-// maps / (maps[1:-1].sum(0) + 1e-6), in place (daam/trace.py:129-130)
-__global__ void normalize_kernel(float* __restrict__ maps, int n_rows, int xx) {
-  const int o = blockIdx.x * blockDim.x + threadIdx.x;
-  if (o >= xx) return;
-  maps += (long long)blockIdx.y * n_rows * xx;      // blockIdx.y: independent map stacks (per-key finalize)
+// maps / (maps[1:-1].sum(0) + 1e-6), in place (daam/trace.py:129-130), at pixel o of one [n_rows][xx] map
+__device__ __forceinline__ void normalize_pixel(float* __restrict__ maps, int n_rows, int xx, int o) {
   float s = 0.f;
   for (int t = 1; t < n_rows - 1; ++t) s += maps[(long long)t * xx + o];
   s += 1e-6f;
   for (int t = 0; t < n_rows; ++t) maps[(long long)t * xx + o] = maps[(long long)t * xx + o] / s;
+}
+
+__global__ void normalize_kernel(float* __restrict__ maps, int n_rows, int xx) {
+  const int o = blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= xx) return;
+  // blockIdx.y: independent map stacks (per-key finalize)
+  normalize_pixel(maps + (long long)blockIdx.y * n_rows * xx, n_rows, xx, o);
+}
+
+// the finalize launches' normalisation: blockIdx.y selects the map, each with its own output and row count
+struct MapOuts {
+  float* out[kMaxMaps];
+  int n_rows[kMaxMaps];
+};
+
+__global__ void normalize_maps_kernel(const __grid_constant__ MapOuts P, int xx) {
+  const int o = blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= xx) return;
+  normalize_pixel(P.out[blockIdx.y], P.n_rows[blockIdx.y], xx, o);
 }
 
 struct RowSel {
@@ -702,38 +739,36 @@ static int check_key_groups(const char* name, const daam_key_group* groups, int3
   return DAAM_OK;
 }
 
-extern "C" int daam_finalize(const daam_key_group* groups, int32_t n_groups, int32_t oh, int32_t ow, int32_t n_rows,
-                             int32_t normalize, float* out, void* stream_) {
-  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  DeviceInfo dev;
-  FinalizeParams p;
-  if (int rc = check_key_groups("daam_finalize", groups, n_groups, oh, ow, n_rows, out, &dev, &p.n_keys)) return rc;
-  p.n_groups = n_groups; p.oh = oh; p.ow = ow; p.n_rows = n_rows;
+// daam_finalize and daam_finalize_maps, after validation: `maps` are MapSel with out, blocks and n_rows set, and every
+// map is reduced exactly as daam_finalize reduces the map's expanded group list. The kernel choice and the band height
+// are daam_finalize's rule applied per map, so the maps of one call take at most two launches (fast and generic, one
+// per kind present) plus one normalisation launch.
+static int launch_finalize(const daam_key_group* groups, int32_t n_groups, int32_t oh, int32_t ow, MapSel* maps,
+                           int n_maps, int keys_per_block, int32_t normalize, const DeviceInfo& dev, cudaStream_t stream) {
+  static thread_local FinalizeParams p;
+  p.n_groups = n_groups; p.oh = oh; p.ow = ow;
   for (int i = 0; i < n_groups; ++i) p.g[i] = groups[i];
   const int xx = oh * ow;
   // fast path: every key has one integer factor F = 1 / 2 / 4 on both axes (all SD / SDXL layers that are ever traced)
-  // and 16-byte-aligned key bases (cp.async / float4: an aligned slab and h * w a multiple of 4). A square map keeps
-  // the rule it always had (side a multiple of 16), so its kernel choice and bits do not move.
+  // and 16-byte-aligned key bases (cp.async / float4: an aligned slab and h * w a multiple of 4, which keeps every block
+  // of a group aligned too). A square map keeps the rule it always had (side a multiple of 16), so its kernel choice
+  // and bits do not move. The map's key count (at most kMaxClassKeys) is checked per map below.
   ClassList cls;
   cls.n = 0;
-  bool fast = (oh != ow || oh % 16 == 0) && ow <= 256 && p.n_keys <= kMaxClassKeys && !force_generic_finalize();
-  for (int i = 0; i < n_groups && fast; ++i) {
+  bool fast_groups = (oh != ow || oh % 16 == 0) && ow <= 256 && !force_generic_finalize();
+  for (int i = 0; i < n_groups && fast_groups; ++i) {
     const daam_key_group& g = groups[i];
     const int f = oh / g.h;
     if (oh % g.h != 0 || ow % g.w != 0 || ow / g.w != f || (f != 1 && f != 2 && f != 4) ||
-        reinterpret_cast<uintptr_t>(g.acc) % 16 != 0 || (g.h * g.w) % 4 != 0) { fast = false; break; }
+        reinterpret_cast<uintptr_t>(g.acc) % 16 != 0 || (g.h * g.w) % 4 != 0) { fast_groups = false; break; }
     bool seen = false;
     for (int c = 0; c < cls.n; ++c) seen = seen || (cls.kh[c] == g.h && cls.kw[c] == g.w);
     if (!seen) {
-      if (cls.n == 8) { fast = false; break; }
+      if (cls.n == 8) { fast_groups = false; break; }
       cls.kh[cls.n] = g.h; cls.kw[cls.n] = g.w; ++cls.n;
     }
   }
-  if (fast) {
-    // 8-row bands unless that leaves the machine under-filled (< 2 CTAs per SM) or a band's source pixels of the
-    // factor-2 class would exceed one CTA's 256 threads (ow > 128); forcing either height measured the same within 1 %
-    // for the 175-key SD-2.1 case
-    cls.band_rows = (((oh + 7) / 8) * n_rows >= 2 * dev.sm_count && ow <= 128) ? 8 : 4;
+  if (fast_groups) {
     int next = 0;
     for (int c = 0; c < cls.n; ++c) {                   // keys[] of the kernel: class by class, groups in call order
       cls.key_begin[c] = next;
@@ -744,28 +779,94 @@ extern "C" int daam_finalize(const daam_key_group* groups, int32_t n_groups, int
         }
     }
     cls.key_begin[cls.n] = next;
-    const size_t smem = (2 * kStageFloats + (size_t)cls.band_rows * ow) * sizeof(float);
-    static std::once_flag attr_once[64];
-    cudaError_t attr_err = cudaSuccess;
-    std::call_once(attr_once[dev.device & 63], [&] {
-      attr_err = cudaFuncSetAttribute(finalize_fast_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      (int)((2 * kStageFloats + 8 * 256) * sizeof(float)));
-    });
-    DAAM_CUDA_TRY(attr_err);
-    const int bands = (oh + cls.band_rows - 1) / cls.band_rows;
-    finalize_fast_kernel<<<dim3(bands, n_rows), 256, smem, stream>>>(p, cls, out);
-  } else {
-    dim3 grid((xx + 255) / 256, n_rows);
-    finalize_kernel<<<grid, 256, 0, stream>>>(p, out);
   }
-  DAAM_CUDA_TRY(cudaGetLastError());
-  count_launch();
+  for (int pass = 0; pass < 2; ++pass) {                 // pass 0: the maps on the fast kernel, pass 1: the others
+    int n = 0, max_rows = 0, max_br = 4;
+    for (int m = 0; m < n_maps; ++m) {
+      MapSel s = maps[m];
+      s.n_keys = keys_per_block * s.block_count;
+      if ((fast_groups && s.n_keys <= kMaxClassKeys) != (pass == 0)) continue;
+      // 8-row bands unless that leaves the machine under-filled (< 2 CTAs per SM) or a band's source pixels of the
+      // factor-2 class would exceed one CTA's 256 threads (ow > 128); forcing either height measured the same within
+      // 1 % for the 175-key SD-2.1 case
+      s.band_rows = (((oh + 7) / 8) * s.n_rows >= 2 * dev.sm_count && ow <= 128) ? 8 : 4;
+      max_rows = std::max(max_rows, s.n_rows);
+      max_br = std::max(max_br, s.band_rows);
+      p.map[n++] = s;
+    }
+    if (n == 0) continue;
+    p.n_maps = n;
+    if (pass == 0) {
+      int bands = 0;
+      for (int m = 0; m < n; ++m) bands = std::max(bands, (oh + p.map[m].band_rows - 1) / p.map[m].band_rows);
+      const size_t smem = (2 * kStageFloats + (size_t)max_br * ow) * sizeof(float);
+      static std::once_flag attr_once[64];
+      cudaError_t attr_err = cudaSuccess;
+      std::call_once(attr_once[dev.device & 63], [&] {
+        attr_err = cudaFuncSetAttribute(finalize_fast_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        (int)((2 * kStageFloats + 8 * 256) * sizeof(float)));
+      });
+      DAAM_CUDA_TRY(attr_err);
+      finalize_fast_kernel<<<dim3(bands, max_rows, n), 256, smem, stream>>>(p, cls);
+    } else {
+      finalize_kernel<<<dim3((xx + 255) / 256, max_rows, n), 256, 0, stream>>>(p);
+    }
+    DAAM_CUDA_TRY(cudaGetLastError());
+    count_launch();
+  }
   if (normalize) {
-    normalize_kernel<<<(xx + 255) / 256, 256, 0, stream>>>(out, n_rows, xx);
+    MapOuts outs;
+    for (int m = 0; m < n_maps; ++m) { outs.out[m] = maps[m].out; outs.n_rows[m] = maps[m].n_rows; }
+    normalize_maps_kernel<<<dim3((xx + 255) / 256, n_maps), 256, 0, stream>>>(outs, xx);
     DAAM_CUDA_TRY(cudaGetLastError());
     count_launch();
   }
   return DAAM_OK;
+}
+
+extern "C" int daam_finalize(const daam_key_group* groups, int32_t n_groups, int32_t oh, int32_t ow, int32_t n_rows,
+                             int32_t normalize, float* out, void* stream_) {
+  DeviceInfo dev;
+  int n_keys;
+  if (int rc = check_key_groups("daam_finalize", groups, n_groups, oh, ow, n_rows, out, &dev, &n_keys)) return rc;
+  MapSel map = {out, 0, 1, n_rows, 0, 0};             // block 0 of every group: the groups as given
+  return launch_finalize(groups, n_groups, oh, ow, &map, 1, n_keys, normalize, dev, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int daam_finalize_maps(const daam_key_group* groups, int32_t n_groups, const daam_map_sel* maps,
+                                  int32_t n_maps, int32_t oh, int32_t ow, int32_t normalize, void* stream_) {
+  const char* name = "daam_finalize_maps";
+  if (!maps || n_maps <= 0) { set_error("%s: no output map", name); return DAAM_E_INVALID; }
+  if (n_maps > kMaxMaps) { set_error("%s: %d maps > %d", name, n_maps, kMaxMaps); return DAAM_E_UNSUPPORTED; }
+  MapSel sel[kMaxMaps];
+  int max_rows = 0;
+  for (int m = 0; m < n_maps; ++m) {
+    const daam_map_sel& s = maps[m];
+    if (!s.out || s.n_rows <= 0 || s.block_begin < 0 || s.block_count <= 0) {
+      set_error("%s: bad map %d (out %p, n_rows %d, blocks [%d, +%d))", name, m, (void*)s.out, s.n_rows, s.block_begin,
+                s.block_count);
+      return DAAM_E_INVALID;
+    }
+    sel[m] = {s.out, s.block_begin, s.block_count, s.n_rows, 0, 0};
+    max_rows = std::max(max_rows, s.n_rows);
+  }
+  DeviceInfo dev;
+  int keys_per_block;
+  if (int rc = check_key_groups(name, groups, n_groups, oh, ow, max_rows, maps[0].out, &dev, &keys_per_block)) return rc;
+  for (int i = 0; i < n_groups; ++i)
+    for (int m = 0; m < n_maps; ++m)
+      if ((long long)maps[m].block_begin + maps[m].block_count > groups[i].n_blocks) {
+        set_error("%s: map %d reads blocks [%d, %lld) but key group %d holds %d", name, m, maps[m].block_begin,
+                  (long long)maps[m].block_begin + maps[m].block_count, i, groups[i].n_blocks);
+        return DAAM_E_INVALID;
+      }
+  for (int m = 0; m < n_maps; ++m)
+    if ((long long)keys_per_block * maps[m].block_count > (1 << 30)) {
+      set_error("%s: map %d selects more than 2^30 keys", name, m);
+      return DAAM_E_UNSUPPORTED;
+    }
+  return launch_finalize(groups, n_groups, oh, ow, sel, n_maps, keys_per_block, normalize, dev,
+                         static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int daam_finalize_per_key(const daam_key_group* groups, int32_t n_groups, int32_t oh, int32_t ow,

@@ -24,7 +24,8 @@ import torch
 from . import _native
 from .utils import compute_token_merge_indices
 
-__all__ = ['GlobalHeatMap', 'RawHeatMapCollection', 'WordHeatMap', 'LayerSlab', 'TimeHeatMaps']
+__all__ = ['GlobalHeatMap', 'RawHeatMapCollection', 'WordHeatMap', 'LayerSlab', 'GlobalHeatMapStack', 'TimeHeatMaps',
+           'ImageHeatMaps']
 
 RawHeatMapKey = Tuple[int, int, int]  # factor, layer, head
 
@@ -70,10 +71,17 @@ class LayerSlab:
     # step and range slabs then have ``storage``'s height too.
     storage: Optional[torch.Tensor] = None
     neg: Optional[torch.Tensor] = None
+    # images per prompt: a prompt's ``heads`` keys are ``images`` runs of ``heads_per_image`` heads, image-major (key
+    # head ``i * heads_per_image + h`` is head h of image i); 1 for slabs that ``RawHeatMapCollection.update`` creates
+    images: int = 1
 
     @property
     def n_prompts(self) -> int:
         return self.acc.shape[0]
+
+    @property
+    def heads_per_image(self) -> int:
+        return self.heads // self.images
 
     @property
     def second(self) -> List[torch.Tensor]:
@@ -129,8 +137,9 @@ class RawHeatMapCollection:
             self._sync()
 
     def slab_for(self, layer_idx: int, factor: int, n_prompts: int, heads: int, h: int, w: int, device,
-                 head_offset: int = 0) -> LayerSlab:
-        """Returns (allocating or re-shaping on demand) the zero-initialised slab of a layer and marks it live."""
+                 head_offset: int = 0, images: int = 1) -> LayerSlab:
+        """Returns (allocating or re-shaping on demand) the zero-initialised slab of a layer and marks it live.
+        ``heads`` counts every image's heads of one prompt (``images`` runs of ``heads // images``)."""
         slab = self.slabs.get(layer_idx)
         shape = (n_prompts, heads, _native.TOKENS, h * w)
         if slab is None or tuple(slab.acc.shape) != shape or slab.acc.device != torch.device(device) \
@@ -147,11 +156,13 @@ class RawHeatMapCollection:
                 if self.n_ranges else None
             halves = dict(acc=storage[n_prompts:], storage=storage, neg=storage[:n_prompts]) if self.negative \
                 else dict(acc=storage)
-            slab = LayerSlab(layer_idx, factor, heads, h, w, head_offset=head_offset, step=step, ranges=ranges, **halves)
+            slab = LayerSlab(layer_idx, factor, heads, h, w, head_offset=head_offset, step=step, ranges=ranges,
+                             images=images, **halves)
             self.slabs[layer_idx] = slab
             self.epoch += 1
         elif (slab.h, slab.w) != (h, w):      # same pixel count, other key shape (a transposed latent): re-tag
             slab.h, slab.w = h, w
+        slab.images = images                  # (same key count, other split into images: only the tag changes)
         if not slab.touched:
             slab.touched = True
             self._order.append(layer_idx)
@@ -429,30 +440,28 @@ def _segment(tokenizer, prompt: str, maps: torch.Tensor, words, image, absolute,
     return word_maps, merged, labels, scores
 
 
-class TimeHeatMaps:
-    """One global heat map per traced denoising step (UNet forward) of one prompt: ``heat_maps[t]`` is exactly what
-    :meth:`~daam_b200.trace.DiffusionHeatMapHooker.compute_global_heat_map` would return had only step ``t`` been
-    traced (per-key bicubic, clamp, mean over keys, ``n_tokens + 2`` rows).
-
-    The steps do not sum to the all-steps map: the clamp comes after the time sum there and per step here."""
+class GlobalHeatMapStack:
+    """Global heat maps of one prompt's text stacked along a first axis: ``heat_maps[t]`` is one
+    ``[n_rows, xh, xw]`` map. Base of :class:`TimeHeatMaps` (one map per step) and :class:`ImageHeatMaps` (one per
+    image)."""
 
     def __init__(self, tokenizer, prompt: str, heat_maps: torch.Tensor):
         self.tokenizer = tokenizer
         self.prompt = prompt
-        self.heat_maps = heat_maps           # device fp32 [steps, n_rows, xh, xw]
+        self.heat_maps = heat_maps           # device fp32 [maps, n_rows, xh, xw]
 
     def __len__(self) -> int:
         return self.heat_maps.shape[0]
 
     def __getitem__(self, t: int) -> GlobalHeatMap:
-        """Step ``t`` as a :class:`GlobalHeatMap` (``compute_word_heat_map``, ``expand_words``)."""
+        """Map ``t`` as a :class:`GlobalHeatMap` (``compute_word_heat_map``, ``expand_words``)."""
         return GlobalHeatMap(self.tokenizer, self.prompt, self.heat_maps[t])
 
     def word_heat_maps(self, word: str, word_idx: int = None, offset_idx: int = 0) -> torch.Tensor:
-        """``[steps, xh, xw]``: row ``t`` is ``self[t].compute_word_heat_map(word, word_idx, offset_idx).heatmap``."""
+        """``[maps, xh, xw]``: row ``t`` is ``self[t].compute_word_heat_map(word, word_idx, offset_idx).heatmap``."""
         rows, _ = compute_token_merge_indices(self.tokenizer, self.prompt, word, word_idx, offset_idx)
         maps = self.heat_maps
-        _require_cuda(maps, 'TimeHeatMaps.word_heat_maps')
+        _require_cuda(maps, f'{type(self).__name__}.word_heat_maps')
         steps, n_rows, grid = maps.shape[0], maps.shape[1], tuple(maps.shape[-2:])
         for r in rows:
             if not -n_rows <= r < n_rows:
@@ -467,11 +476,27 @@ class TimeHeatMaps:
 
     def segment(self, words, image, absolute: bool = False, threshold: Optional[float] = None, word_idx=None,
                 offset_idx: int = 0, to_cpu: bool = True):
-        """:meth:`GlobalHeatMap.segment` for every step in one call (two launches whatever the step count): returns
-        ``(word_maps, labels, scores)`` with ``word_maps`` the device ``[steps, len(words), xh, xw]`` word heat maps and
-        ``labels`` / ``scores`` ``[steps, H, W]``; row ``t`` equals ``self[t].segment(...)`` bit for bit (min / max
-        normalisation per step and word)."""
+        """:meth:`GlobalHeatMap.segment` for every map in one call (two launches whatever the map count): returns
+        ``(word_maps, labels, scores)`` with ``word_maps`` the device ``[maps, len(words), xh, xw]`` word heat maps and
+        ``labels`` / ``scores`` ``[maps, H, W]``; row ``t`` equals ``self[t].segment(...)`` bit for bit (min / max
+        normalisation per map and word)."""
         word_maps, _, labels, scores = _segment(self.tokenizer, self.prompt, self.heat_maps, list(words), image,
                                                 absolute, threshold, word_idx, offset_idx, to_cpu,
-                                                'TimeHeatMaps.segment')
+                                                f'{type(self).__name__}.segment')
         return word_maps, labels, scores
+
+
+class TimeHeatMaps(GlobalHeatMapStack):
+    """One global heat map per traced denoising step (UNet forward) of one prompt: ``heat_maps[t]`` is exactly what
+    :meth:`~daam_b200.trace.DiffusionHeatMapHooker.compute_global_heat_map` would return had only step ``t`` been
+    traced (per-key bicubic, clamp, mean over keys, ``n_tokens + 2`` rows). ``heat_maps`` is ``[steps, n_rows, xh,
+    xw]``; ``word_heat_maps`` and ``segment`` work over every step.
+
+    The steps do not sum to the all-steps map: the clamp comes after the time sum there and per step here."""
+
+
+class ImageHeatMaps(GlobalHeatMapStack):
+    """One global heat map per image of one prompt (``num_images_per_prompt``): ``heat_maps[i]`` is exactly
+    :meth:`~daam_b200.trace.DiffusionHeatMapHooker.compute_global_heat_map` with ``image_idx=i``, the DAAM map over
+    image ``i``'s keys only. ``heat_maps`` is ``[images, n_rows, xh, xw]``; ``word_heat_maps`` and ``segment`` work over
+    every image."""

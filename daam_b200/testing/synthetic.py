@@ -480,10 +480,13 @@ class SyntheticPipeline:
     @torch.no_grad()
     def __call__(self, prompt, num_inference_steps: int = 50, generator: Optional[torch.Generator] = None,
                  callback=None, guidance_scale: float = 7.5, height: Optional[int] = None, width: Optional[int] = None,
-                 negative_prompt=None):
+                 negative_prompt=None, num_images_per_prompt: int = 1):
         """``height`` / ``width``: the image size in pixels, as diffusers takes it (default: the model's own square
         size); the latent is ``height // 8 x width // 8``. ``negative_prompt`` reaches ``check_inputs`` positionally, in
-        diffusers' SD order; the synthetic encoder ignores all text, so it changes no embedding or random draw."""
+        diffusers' SD order; the synthetic encoder ignores all text, so it changes no embedding or random draw.
+        ``num_images_per_prompt``: like diffusers, every prompt's embeddings are repeated prompt-major (the batch is
+        ``[uncond x N x n, cond x N x n]``) and one latent is drawn per image; with 1 the draws are those of a call
+        without it."""
         spec = self.unet.spec
         height = spec.sample_size * self.vae_scale_factor if height is None else height
         width = spec.sample_size * self.vae_scale_factor if width is None else width
@@ -492,12 +495,15 @@ class SyntheticPipeline:
         else:
             self.check_inputs(prompt, height, width, None, negative_prompt)
         prompts = [prompt] if isinstance(prompt, str) else list(prompt)
-        n = len(prompts)
         latent_h, latent_w = height // self.vae_scale_factor, width // self.vae_scale_factor
         if generator is None:
             generator = torch.Generator().manual_seed(self.seed)
         cuda = self.device.type == 'cuda'
         emb_h = self.encode(prompts, generator).to(self.dtype)
+        if num_images_per_prompt != 1:                        # [2, N, ...] -> [2, N * n, ...], each prompt n times
+            emb_h = emb_h.view(2, len(prompts), *emb_h.shape[1:]).repeat_interleave(num_images_per_prompt, dim=1) \
+                .reshape(-1, *emb_h.shape[1:])
+        n = len(prompts) * num_images_per_prompt
         lat_h = torch.randn(n, spec.in_channels, latent_h, latent_w, generator=generator,
                             dtype=torch.float32).to(self.dtype)
         t_h = torch.tensor([[1000.0 * (1.0 - i / max(1, num_inference_steps))] for i in range(num_inference_steps)])

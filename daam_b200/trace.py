@@ -41,7 +41,7 @@ import torch.nn.functional as F
 
 from . import _native, ops
 from .geometry import LatentGeometry
-from .heatmap import GlobalHeatMap, LayerSlab, RawHeatMapCollection, TimeHeatMaps
+from .heatmap import GlobalHeatMap, ImageHeatMaps, LayerSlab, RawHeatMapCollection, TimeHeatMaps
 from .hook import AggregateHooker, ObjectHooker, UNetCrossAttentionLocator
 from .utils import cache_dir
 
@@ -98,6 +98,7 @@ class DiffusionHeatMapHooker(AggregateHooker):
         self.negative = negative
         self.all_heat_maps.negative = negative
         self.last_image = None
+        self.last_images: list = []   # every image of the last generation, prompt-major (``out.images[p * n + i]``)
         self.time_idx = 0
         self._gen_idx = 0
         self.launch = launch
@@ -119,11 +120,13 @@ class DiffusionHeatMapHooker(AggregateHooker):
         self._stream: Optional[torch.cuda.Stream] = None
         self._dirty = False                    # side-stream work not yet ordered before the current stream
         self.all_heat_maps.bind(self.synchronize, self._zero_slabs)
-        # time-resolved mode: per prompt a device history [capacity, n_rows, x, x] of per-step global heat maps (grown
-        # by doubling, restarted every generation), keyed by `negative` (the negative histories exist with the mode only)
+        # time-resolved mode: device histories [capacity, n_rows, xh, xw] of per-step global heat maps (grown by
+        # doubling, restarted every generation), keyed by `negative` (the negative histories exist with the mode only)
+        # and then by (prompt, None) for a prompt's map over all its images, or by (prompt, image) for one image's map
+        # (kept only when a generation has several images per prompt)
         self.time_resolved = time_resolved
         self.all_heat_maps.time_resolved = time_resolved
-        self._history: Dict[bool, List[torch.Tensor]] = {False: [], True: []}
+        self._history: Dict[bool, Dict[Tuple[int, Optional[int]], torch.Tensor]] = {False: {}, True: {}}
         self._time_steps = 0
         self._history_rows: Optional[Dict[bool, List[int]]] = None   # n_rows of every prompt of the running generation
         # step-range mode: the UNet forward index of the running generation
@@ -158,11 +161,16 @@ class DiffusionHeatMapHooker(AggregateHooker):
 
     def to_experiment(self, path, seed=None, id='.', subtype='.', **compute_kwargs):
         """Exports the last generation call to a serializable generation experiment (trace.py:68-81). With
-        ``negative=True`` it records the negative map and the text it belongs to."""
+        ``negative=True`` it records the negative map and the text it belongs to; with ``image_idx=i`` image ``i``'s map
+        and image ``i`` of the prompt (``prompt_idx``)."""
         from .experiment import GenerationExperiment
         heat_map = self.compute_global_heat_map(**compute_kwargs)
+        image = self.last_image
+        if compute_kwargs.get('image_idx') is not None:
+            per_prompt = len(self.last_images) // max(1, len(self._texts()))
+            image = self.last_images[compute_kwargs.get('prompt_idx', 0) * per_prompt + compute_kwargs['image_idx']]
         return GenerationExperiment(
-            self.last_image,
+            image,
             heat_map.heat_maps,
             heat_map.prompt if compute_kwargs.get('negative') else self.last_prompt,
             seed=seed, id=id, subtype=subtype, path=path, tokenizer=self.pipe.tokenizer,
@@ -264,7 +272,7 @@ class DiffusionHeatMapHooker(AggregateHooker):
         # "second half of the batch*heads axis" (trace.py:240): the conditional samples of a CFG batch
         _, n_samples, head0, n_heads = ops.cond_half(bsz, heads)
         n_real, images = self._prompt_layout(layer_idx, n_samples)
-        slab = self.all_heat_maps.slab_for(layer_idx, factor, n_real, images * n_heads, h, w, q.device, head0)
+        slab = self.all_heat_maps.slab_for(layer_idx, factor, n_real, images * n_heads, h, w, q.device, head0, images)
         self._epoch_seen = self.all_heat_maps.epoch        # (this call may have bumped it; the other layers' slabs stand)
         if self.negative:                                  # one descriptor over the whole batch, into the whole slab
             desc = ops.make_layer_desc(q, k, slab.storage.view(bsz, n_heads, slab.acc.shape[2], hw), heads, scale,
@@ -328,7 +336,8 @@ class DiffusionHeatMapHooker(AggregateHooker):
         self._check_guidance(layer_idx, bsz)
         _, n_samples, head0, n_heads = ops.cond_half(bsz, heads)
         n_real, images = self._prompt_layout(layer_idx, n_samples)
-        slab = self.all_heat_maps.slab_for(layer_idx, factor, n_real, images * n_heads, h, w, probs.device, head0)
+        slab = self.all_heat_maps.slab_for(layer_idx, factor, n_real, images * n_heads, h, w, probs.device, head0,
+                                           images)
         self.synchronize()
         if self.negative:                                  # rows [0, N*H) into neg, the rest into acc, in one launch
             ops.accumulate_probs(probs, slab.storage, whole_batch=True)
@@ -406,10 +415,12 @@ class DiffusionHeatMapHooker(AggregateHooker):
         self._step_id += 1
 
     def _finalize_step(self, device, stream: int):
-        """Time-resolved mode, right after the step's launch on ``stream``: for every prompt, the global heat map of the
-        step slabs this step wrote -- the same reduction, key order (live-slab order) and row count as
-        :meth:`compute_global_heat_map` -- into the next slot of the prompt's history. With ``negative=True`` the same
-        again over the unconditional halves of the step slabs, into the negative histories."""
+        """Time-resolved mode, right after the step's launch on ``stream``: ONE ``daam_finalize_maps`` launch writes,
+        for every prompt, the global heat map of the step slabs this step wrote -- the same reduction, key order
+        (live-slab order) and row count as :meth:`compute_global_heat_map` -- into the next slot of the prompt's
+        history; with several images per prompt also every image's map (``image_idx``) into that image's history; and
+        with ``negative=True`` the same again over the unconditional halves of the step slabs, into the negative
+        histories."""
         queued = {idx for idx, step in self._queued.items() if step == self._step_id}
         slabs = [s for s in self.all_heat_maps.live_slabs() if s.layer_idx in queued]
         grid = self.geometry.grid
@@ -418,19 +429,20 @@ class DiffusionHeatMapHooker(AggregateHooker):
         if self._history_rows is None:
             self._history_rows = {negative: [self._n_rows(text) for text in self._texts(negative)]
                                   for negative in halves}
+        n_prompts, images = slabs[0].n_prompts, slabs[0].images
+        maps = []
         for negative in halves:
             rows, history = self._history_rows[negative], self._history[negative]
-            for p in range(slabs[0].n_prompts):
+            first = n_prompts if self.negative and not negative else 0    # step slabs: [uncond x N, cond x N]
+            for p in range(n_prompts):
                 n_rows = rows[p] if p < len(rows) else rows[0]
-                if p == len(history):
-                    history.append(torch.empty((16, n_rows) + grid, dtype=torch.float32, device=device))
-                hist = history[p]
-                if t == hist.shape[0]:                      # grow by doubling, in stream order between two steps
-                    grown = torch.empty((2 * t,) + tuple(hist.shape[1:]), dtype=torch.float32, device=device)
-                    grown[:t].copy_(hist)
-                    history[p] = hist = grown
-                _native.finalize([_key_group(s.half(s.step, negative)[p], s) for s in slabs], grid, n_rows, False,
-                                 hist[t].data_ptr(), stream)
+                block = (first + p) * images
+                for image, begin, count in [(None, block, images)] + \
+                        ([(i, block + i, 1) for i in range(images)] if images > 1 else []):
+                    hist = _history_slot(history, (p, image), n_rows, grid, t, device)
+                    maps.append(_native.DaamMapSel(block_begin=begin, block_count=count, n_rows=n_rows,
+                                                   out=hist[t].data_ptr()))
+        _native.finalize_maps([_block_group(s.step, s) for s in slabs], maps, grid, False, stream)
         self._time_steps = t + 1
 
     def _texts(self, negative: bool = False) -> List[str]:
@@ -445,7 +457,7 @@ class DiffusionHeatMapHooker(AggregateHooker):
     def _restart_history(self):
         """A new generation: a new per-step history (maps handed out earlier stay valid: they are other tensors), and
         the UNet forward count of the step ranges starts again (their slabs were zeroed with the accumulators)."""
-        self._history = {False: [], True: []}
+        self._history = {False: {}, True: {}}
         self._time_steps = 0
         self._history_rows = None
         self._forward_idx = 0
@@ -483,8 +495,8 @@ class DiffusionHeatMapHooker(AggregateHooker):
 
     # -- finalize -------------------------------------------------------------------------------------------------------
     def compute_global_heat_map(self, prompt=None, factors=None, head_idx=None, layer_idx=None, normalize=False,
-                                prompt_idx: int = 0, *, step_range: Optional[int] = None,
-                                negative: bool = False) -> GlobalHeatMap:
+                                prompt_idx: int = 0, *, step_range: Optional[int] = None, negative: bool = False,
+                                image_idx: Optional[int] = None) -> GlobalHeatMap:
         """Aggregate across time (already summed in the slabs) and across layers/heads (trace.py:83-132).
 
         Args mirror the reference: ``factors`` restricts the spatial factors, ``head_idx`` / ``layer_idx`` restrict to one
@@ -493,9 +505,13 @@ class DiffusionHeatMapHooker(AggregateHooker):
         (``trace(pipe, step_ranges=[...])``): the DAAM map a trace of only those steps would give. ``negative=True``
         (``trace(pipe, negative=True)``): the map of the unconditional half of the batch, whose text (and so row count
         and word lookup) is the prompt's negative prompt unless ``prompt`` is given.
+
+        With several images per prompt (``num_images_per_prompt``) the map is, as in the reference, the mean over every
+        image's keys, and ``head_idx`` indexes images x heads. ``image_idx=i`` keeps image ``i``'s keys only (``head_idx``
+        then counts that image's heads); an un-guided batch has only the kept images (see ``ops.cond_half``).
         """
         prompt, grid, n_rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range, layer_idx,
-                                                                head_idx, negative)
+                                                                head_idx, negative, image_idx)
         device = slabs[0].acc.device
         maps = torch.empty((n_rows,) + grid, dtype=torch.float32, device=device)
         with torch.cuda.device(device):
@@ -503,27 +519,53 @@ class DiffusionHeatMapHooker(AggregateHooker):
                              torch.cuda.current_stream(device).cuda_stream)
         return GlobalHeatMap(self.pipe.tokenizer, prompt, maps)
 
+    def compute_image_heat_maps(self, prompt_idx: int = 0, factors=None, layer_idx=None, head_idx=None,
+                                normalize: bool = False, *, step_range: Optional[int] = None,
+                                negative: bool = False) -> ImageHeatMaps:
+        """Every image's map of prompt ``prompt_idx`` in one launch (``daam_finalize_maps``): ``heat_maps[i]`` is
+        ``compute_global_heat_map(image_idx=i, ...)`` with the same arguments, bit for bit (``head_idx`` counts one
+        image's heads). Returns an :class:`ImageHeatMaps` ``[images, n_rows, xh, xw]``."""
+        prompt, grid, n_rows, _, slabs = self._read_groups(None, factors, prompt_idx, step_range, layer_idx, head_idx,
+                                                           negative, 0)
+        images, n_prompts = slabs[0].images, slabs[0].n_prompts
+        if not 0 <= prompt_idx < n_prompts:
+            raise IndexError(f'prompt_idx {prompt_idx} is out of range for {n_prompts} prompt(s)')
+        groups = [_block_group(s.source(step_range, negative), s, -1 if head_idx is None else head_idx) for s in slabs]
+        device = slabs[0].acc.device
+        out = torch.empty((images, n_rows) + grid, dtype=torch.float32, device=device)
+        maps = [_native.DaamMapSel(block_begin=prompt_idx * images + i, block_count=1, n_rows=n_rows,
+                                   out=out[i].data_ptr()) for i in range(images)]
+        with torch.cuda.device(device):
+            _native.finalize_maps(groups, maps, grid, normalize, torch.cuda.current_stream(device).cuda_stream)
+        return ImageHeatMaps(self.pipe.tokenizer, prompt, out)
+
     def compute_time_heat_maps(self, prompt_idx: int = 0, normalize: bool = False, *,
-                               negative: bool = False) -> TimeHeatMaps:
+                               negative: bool = False, image_idx: Optional[int] = None) -> TimeHeatMaps:
         """One global heat map per traced denoising step (UNet forward) of the running / last generation; needs
         ``trace(pipe, time_resolved=True)``. ``heat_maps[t]`` is what :meth:`compute_global_heat_map` would return had
         only step ``t`` been traced, with every key and layer; ``normalize`` applies the reference's normalisation to
         each step. Summing the steps does not give the all-steps map: there the clamp comes after the time sum.
-        ``negative=True``: the same for the unconditional half, against the negative text.
+        ``negative=True``: the same for the unconditional half, against the negative text. ``image_idx=i``: image
+        ``i``'s map after every step (``compute_global_heat_map(image_idx=i)`` of a trace of that step only).
 
         Costs: a second fp32 slab per traced layer (as large as its accumulator) and ``steps x n_rows x xh x xw`` fp32
-        of history per prompt (``heat_maps`` is ``[steps, n_rows, xh, xw]``, the grid of :attr:`geometry`)."""
+        of history per prompt (``heat_maps`` is ``[steps, n_rows, xh, xw]``, the grid of :attr:`geometry`), and as much
+        again per image when a generation has several images per prompt."""
         if not self.time_resolved:
             raise RuntimeError('per-step heat maps need trace(pipe, time_resolved=True)')
         if negative:
             self.all_heat_maps.check_negative()
         self.synchronize()
         history = self._history[negative]
-        if self._time_steps == 0 or not 0 <= prompt_idx < len(history):
+        if self._time_steps == 0 or (prompt_idx, None) not in history:
             raise RuntimeError('No heat maps found. Did you forget to call `with trace(...)` during generation?')
+        if image_idx is not None:
+            _check_image_idx(image_idx, max(1, sum(1 for p, i in history if p == prompt_idx and i is not None)))
         texts = self._texts(negative)
         prompt = texts[prompt_idx] if prompt_idx < len(texts) else texts[0]
-        maps = history[prompt_idx][:self._time_steps]
+        # one image per prompt: its map is the prompt's map (same keys, same order)
+        key = (prompt_idx, image_idx) if (prompt_idx, image_idx) in history else (prompt_idx, None)
+        maps = history[key][:self._time_steps]
         if normalize:
             maps = maps.clone()
             with torch.cuda.device(maps.device):
@@ -533,14 +575,16 @@ class DiffusionHeatMapHooker(AggregateHooker):
 
 
     def compute_per_head_heat_maps(self, prompt=None, factors=None, normalize=False, prompt_idx: int = 0, *,
-                                   step_range: Optional[int] = None, negative: bool = False):
+                                   step_range: Optional[int] = None, negative: bool = False,
+                                   image_idx: Optional[int] = None):
         """Every ``compute_global_heat_map(layer_idx=l, head_idx=h)`` of the reference's ``--all-heads`` sweep
         (daam/run/generate.py:239-255) in one launch. Returns ``(keys, maps)``: ``keys[i] = (factor, layer, head)`` and
         ``maps[i]`` the ``[n_tokens + 2, xh, xw]`` heat map the reference computes for that single key. ``step_range=i``
-        and ``negative=True`` select the slabs as in :meth:`compute_global_heat_map`."""
+        and ``negative=True`` select the slabs as in :meth:`compute_global_heat_map`; ``image_idx=i`` keeps image
+        ``i``'s keys, whose ``head`` then counts that image's heads."""
         prompt, grid, n_rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range,
-                                                                negative=negative)
-        keys = [(slab.factor, slab.layer_idx, head) for slab in slabs for head in range(slab.heads)]
+                                                                negative=negative, image_idx=image_idx)
+        keys = [(slab.factor, slab.layer_idx, head) for slab, g in zip(slabs, groups) for head in range(g.heads)]
         device = slabs[0].acc.device
         maps = torch.empty((len(keys), n_rows) + grid, dtype=torch.float32, device=device)
         with torch.cuda.device(device):
@@ -549,11 +593,12 @@ class DiffusionHeatMapHooker(AggregateHooker):
         return keys, maps
 
     def _read_groups(self, prompt, factors, prompt_idx: int, step_range: Optional[int], layer_idx=None, head_idx=None,
-                     negative: bool = False):
+                     negative: bool = False, image_idx: Optional[int] = None):
         """What the heat-map reads share: the prompt (default: the generation's, or with ``negative`` its negative
         text), the map grid ``(xh, xw)``, the row count, and the key groups of prompt ``prompt_idx`` over the live slabs
         (with ``step_range``: over that range's slabs; with ``negative``: their unconditional halves) that pass the
-        filters, with the slabs behind them. Raises when no slab passes."""
+        filters, with the slabs behind them; with ``image_idx`` the groups hold image ``image_idx``'s heads only, and
+        ``head_idx`` counts those. Raises when no slab passes, and ``IndexError`` for a bad ``image_idx``."""
         if negative:
             self.all_heat_maps.check_negative()
         if prompt is None:
@@ -562,14 +607,27 @@ class DiffusionHeatMapHooker(AggregateHooker):
             else:
                 prompt = self.last_prompts[prompt_idx] if self.last_prompts else self.last_prompt
         factors = {0, 1, 2, 4, 8, 16, 32, 64} if factors is None else set(factors)
+        read = self.all_heat_maps.read_slabs(step_range, negative)
+        if image_idx is not None and read:
+            images = {s.images for s in read}
+            if len(images) > 1:
+                raise RuntimeError(f'image_idx needs every traced layer to hold the same images per prompt, got '
+                                   f'{sorted(images)}')
+            _check_image_idx(image_idx, images.pop())
         groups, slabs = [], []
-        for slab in self.all_heat_maps.read_slabs(step_range, negative):
+        for slab in read:
             if slab.factor not in factors or (layer_idx is not None and layer_idx != slab.layer_idx):
                 continue
-            if head_idx is not None and not 0 <= head_idx < slab.heads:
+            heads = slab.heads if image_idx is None else slab.heads_per_image
+            if head_idx is not None and not 0 <= head_idx < heads:
                 continue
-            acc = slab.source(step_range, negative)[prompt_idx]
-            groups.append(_key_group(acc, slab, -1 if head_idx is None else head_idx))
+            src = slab.source(step_range, negative)
+            if image_idx is None:
+                groups.append(_key_group(src[prompt_idx], slab, -1 if head_idx is None else head_idx))
+            else:                                          # image i: heads [i * H, (i + 1) * H) of the prompt
+                groups.append(_native.DaamKeyGroup(acc=src[prompt_idx, image_idx * heads].data_ptr(), heads=heads,
+                                                   h=slab.h, w=slab.w, tokens=src.shape[2],
+                                                   head_sel=-1 if head_idx is None else head_idx, n_blocks=1))
             slabs.append(slab)
         if not groups:
             if head_idx is not None or layer_idx is not None:
@@ -582,7 +640,33 @@ def _key_group(acc: torch.Tensor, slab: LayerSlab, head_sel: int = -1) -> _nativ
     """The finalize input of one prompt's ``[heads, 77, hw]`` slab of ``slab``'s layer (its accumulator, step slab or a
     range slab); ``head_sel``: one head, or -1 for all."""
     return _native.DaamKeyGroup(acc=acc.data_ptr(), heads=slab.heads, h=slab.h, w=slab.w, tokens=acc.shape[1],
-                                head_sel=head_sel, reserved=0)
+                                head_sel=head_sel, n_blocks=0)
+
+
+def _block_group(src: torch.Tensor, slab: LayerSlab, head_sel: int = -1) -> _native.DaamKeyGroup:
+    """The ``daam_finalize_maps`` input of a whole ``[prompts, images * heads, 77, hw]`` slab ``src`` of ``slab``'s layer
+    (accumulator, step, range or negative slab): one block per (prompt, image), block ``p * images + i``; ``head_sel``
+    one head within each image, or -1 for all."""
+    return _native.DaamKeyGroup(acc=src.data_ptr(), heads=slab.heads_per_image, h=slab.h, w=slab.w, tokens=src.shape[2],
+                                head_sel=head_sel, n_blocks=src.shape[0] * slab.images)
+
+
+def _check_image_idx(image_idx, images: int):
+    if not isinstance(image_idx, int) or isinstance(image_idx, bool) or not 0 <= image_idx < images:
+        raise IndexError(f'image_idx {image_idx!r} is out of range for {images} image(s) per prompt')
+
+
+def _history_slot(history: dict, key, n_rows: int, grid, t: int, device) -> torch.Tensor:
+    """The time-resolved history ``history[key]`` ``[capacity, n_rows, xh, xw]`` with room for step ``t``: created
+    with 16 slots, grown by doubling (in stream order between two steps)."""
+    hist = history.get(key)
+    if hist is None:
+        hist = history[key] = torch.empty((16, n_rows) + tuple(grid), dtype=torch.float32, device=device)
+    if t == hist.shape[0]:
+        grown = torch.empty((2 * t,) + tuple(hist.shape[1:]), dtype=torch.float32, device=device)
+        grown[:t].copy_(hist)
+        history[key] = hist = grown
+    return hist
 
 
 def _normalize_step_ranges(step_ranges) -> List[Tuple[int, int]]:
@@ -614,7 +698,8 @@ def _normalize_step_ranges(step_ranges) -> List[Tuple[int, int]]:
 
 
 class ImageProcessorHooker(ObjectHooker):
-    """Remembers the first post-processed image of an SDXL pipeline (trace.py:135-147)."""
+    """Remembers the first post-processed image of an SDXL pipeline (trace.py:135-147), and all of them in
+    ``last_images``."""
 
     def __init__(self, processor, parent_trace: 'trace'):
         super().__init__(processor)
@@ -623,6 +708,7 @@ class ImageProcessorHooker(ObjectHooker):
     def _hooked_postprocess(hk_self, _, *args, **kwargs):
         images = hk_self.monkey_super('postprocess', *args, **kwargs)
         hk_self.parent_trace.last_image = images[0]
+        hk_self.parent_trace.last_images = list(images)
         return images
 
     def _hook_impl(self):
@@ -630,7 +716,8 @@ class ImageProcessorHooker(ObjectHooker):
 
 
 class PipelineHooker(ObjectHooker):
-    """Per-generation reset + prompt capture at ``check_inputs``; image capture at the safety checker (trace.py:150-186)."""
+    """Per-generation reset + prompt capture at ``check_inputs``; image capture at the safety checker (trace.py:150-186):
+    ``last_image`` is the last image, as in the reference, and ``last_images`` all of them."""
 
     def __init__(self, pipeline, parent_trace: 'trace'):
         super().__init__(pipeline)
@@ -646,6 +733,7 @@ class PipelineHooker(ObjectHooker):
         else:
             images = self.numpy_to_pil(image)
         hk_self.parent_trace.last_image = images[len(images) - 1]
+        hk_self.parent_trace.last_images = list(images)      # prompt-major, as the pipeline returns them
         return image, has_nsfw
 
     def _hooked_check_inputs(hk_self, _, prompt: Union[str, List[str]], *args, **kwargs):

@@ -30,7 +30,8 @@ extern "C" {
                                           daam_accumulate_range)
                                        4: the finalize family takes (map_h, map_w); the _rect names are gone
                                           (later, additive: layers with hw not a multiple of 4 are accepted;
-                                          daam_segment_words) */
+                                          daam_segment_words, daam_finalize_maps; daam_key_group.reserved is
+                                          n_blocks) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
 
@@ -167,12 +168,15 @@ int daam_accumulate_probs(const void* probs, int32_t dtype, int32_t first_row, i
 /*
  * All (or one) heads of one traced layer: `acc` points at [heads][tokens][h*w] fp32 (one prompt's slice of the
  * accumulator daam_accumulate fills). head_sel = -1 selects every head, otherwise one head index.
+ * daam_finalize_maps reads a group as `n_blocks` such blocks back to back ([n_blocks][heads][tokens][h*w] from acc:
+ * e.g. a whole slab [prompts][images * heads] with `heads` the heads per image) and head_sel applies inside each block;
+ * the other entry points ignore n_blocks (it was `reserved`, callers set it to 0).
  */
 typedef struct daam_key_group {
   const float* acc;          /* device */
   int32_t heads, h, w, tokens;
   int32_t head_sel;
-  int32_t reserved;
+  int32_t n_blocks;
 } daam_key_group;
 
 /*
@@ -189,6 +193,28 @@ typedef struct daam_key_group {
  */
 int daam_finalize(const daam_key_group* groups, int32_t n_groups, int32_t map_h, int32_t map_w, int32_t n_rows,
                   int32_t normalize, float* out, void* stream);
+
+/*
+ * Several daam_finalize maps over one group list in one launch (e.g. every image's map of a prompt, or every map a
+ * time-resolved step writes). Each group is read as n_blocks blocks (see daam_key_group); map m reduces blocks
+ * [block_begin, block_begin + block_count) of EVERY group, and is bit for bit what daam_finalize gives for the expanded
+ * group list `for g: for b in those blocks: {acc_g + b * heads_g * tokens_g * h_g * w_g, heads_g, head_sel_g}` with
+ * maps[m].n_rows and maps[m].out (same key order, kernel choice and band height; with head_sel = -1 that is one group
+ * per layer with heads_g * block_count heads). `normalize` applies per map over its own rows. `groups` and `maps` are
+ * host memory. One launch per kind of kernel the maps take (fast / generic: one when every map is alike, which is the
+ * case whenever their key counts are on the same side of 2048) plus one normalisation launch.
+ * Limits: n_groups <= 160 and n_maps <= DAAM_FINALIZE_MAX_MAPS (DAAM_E_UNSUPPORTED). DAAM_E_INVALID: what
+ * daam_finalize refuses, no map, a map without output, rows or blocks, a negative block_begin, or a block range past
+ * a group's n_blocks.
+ */
+#define DAAM_FINALIZE_MAX_MAPS 64
+typedef struct daam_map_sel {
+  int32_t block_begin, block_count;   /* blocks [block_begin, block_begin + block_count) of every group */
+  int32_t n_rows, reserved;           /* rows [0, n_rows) of the map; reserved: 0 */
+  float* out;                         /* device fp32 [n_rows][map_h][map_w] */
+} daam_map_sel;
+int daam_finalize_maps(const daam_key_group* groups, int32_t n_groups, const daam_map_sel* maps, int32_t n_maps,
+                       int32_t map_h, int32_t map_w, int32_t normalize, void* stream);
 
 /*
  * The reference's --all-heads sweep calls compute_global_heat_map(layer_idx=l, head_idx=h) once per (layer, head)
