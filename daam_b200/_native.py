@@ -21,6 +21,7 @@ ACC_EARLY_LOADS = 0x200   # see include/daam_b200.h: only valid when q/k were co
 ABI_VERSION = 4
 E_INVALID, E_UNSUPPORTED, E_CUDA = -1, -2, -3
 TOKENS = 77
+CONTEXT_TOKENS = (77, 154, 231)   # daam_accumulate: one to three 77-token chunks (DAAM_MAX_TOKENS = 231)
 EXPAND_SCRATCH_FLOATS = 64   # DAAM_EXPAND_SCRATCH_FLOATS: per word
 MAX_SEGMENT_WORDS = 96       # daam_segment_words: labels 1..96 plus background 0 fit a byte
 

@@ -50,6 +50,14 @@
 //   split form : red mode issues a second reduce-add from sP; ldst mode loads, adds and stores the range slab in its
 //                coalesced pass, like the accumulator.
 //
+// Long-context instances (kC = 2 or 3 chunks of 77 tokens: 154- / 231-token contexts, 16-bit form, plain slab mode):
+// a stage holds the Q box and kC K boxes [80 x 64], loaded at token rows 77c of the same 4-D map (token extent = the
+// context); columns 77-79 of a box hold the next chunk's first tokens (or TMA zeros after the last one), which the
+// column masks exclude exactly as they exclude the zero rows of a 77-token box. The consumers issue kC sets of
+// wgmma.m64n80k16 into kC fragments, take max and sum over all of them, then add chunk c's probabilities into one ring
+// slot per chunk (accumulator rows (p H + h) 77 kC + 77 c): a tile consumes kC consecutive slots of the same 3-slot
+// ring, each with the single-chunk epilogue.
+//
 // Replaces daam/trace.py:276 (get_attention_scores), :219-244 (_unravel_attn) and :293-294 (update loop).
 #include <cuda.h>
 
@@ -84,6 +92,11 @@ constexpr int kSplitSmemBytes = 1024 + (kStages + 1) * kSplitStageBytes + kPByte
 static_assert(kSmemBytes <= 232448, "16-bit form exceeds the 227 KB shared-memory limit");
 static_assert(kSplitSmemBytes <= 232448, "split form exceeds the 227 KB shared-memory limit");
 static_assert(kSlabSmemBytes <= 232448, "16-bit second-slab form exceeds the 227 KB shared-memory limit");
+// 16-bit long-context form: kC K boxes per stage (kC = 3: 2 x 46 KB of stages + 3 x 38.5 KB of ring, 208.6 KB)
+constexpr int long_smem_bytes(int chunks) {
+  return 1024 + kStages * (kQBytes + chunks * kKBytes) + kAccStages * kPBytes + kBarBytes16;
+}
+static_assert(long_smem_bytes(3) <= 232448, "16-bit long-context form exceeds the 227 KB shared-memory limit");
 
 struct MmaParams {
   LaunchParams base;
@@ -319,17 +332,31 @@ __device__ __forceinline__ void wgmma_chunk_16bit(Frag& d, uint32_t a_src, uint3
   wgmma_commit();
   wgmma_wait0();
 }
+// The same over the kC K boxes of a long-context stage (box c at k_src + c * kKBytes), into kC fragments, one group.
+template <bool kBf16, int kC>
+__device__ __forceinline__ void wgmma_chunk_16bit_long(Frag (&d)[kC], uint32_t a_src, uint32_t k_src) {
+  wgmma_fence();
+#pragma unroll
+  for (int c = 0; c < kC; ++c)
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      wgmma_16bit<kBf16>(d[c], wgmma_desc_sw128(a_src + 32 * k), wgmma_desc_sw128(k_src + c * kKBytes + 32 * k));
+  wgmma_commit();
+  wgmma_wait0();
+}
 
 __device__ __forceinline__ void griddep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
 // kChunked: some layer of the launch has head_dim > 64 (several K chunks per tile); the common single-chunk case keeps
 // its simpler loops (one load iteration per tile). kSlab: also store (kSlabStore) or add (kSlabAdd) each tile's
-// probabilities into the second slab.
-template <bool kSplit, bool kChunked, int kSlab>
+// probabilities into the second slab. kC: 77-token chunks of the context (1, or 2 / 3 in the long-context instances).
+template <bool kSplit, bool kChunked, int kSlab, int kC = 1>
 __global__ void __launch_bounds__(kSplit ? kThreads : kThreads16, 1)
 accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP) {
+  static_assert(kC == 1 || (!kSplit && kSlab == kSlabNone), "long contexts: 16-bit form, plain slab mode only");
   constexpr bool kSecond = kSlab != kSlabNone;        // a second slab (store or add)
-  constexpr int kStageBytesT = kSplit ? kSplitStageBytes : kStageBytes;
+  constexpr int kCtx = kC * kTokens;                  // context rows: the accumulator's token extent
+  constexpr int kStageBytesT = kSplit ? kSplitStageBytes : kQBytes + kC * kKBytes;
   constexpr int kOperandBytes = (kSplit ? kStages + 1 : kStages) * kStageBytesT;     // stages (+ the lo buffer)
   // staged probabilities (split) / the accumulator ring (16-bit), + sS (16-bit form with a second slab)
   constexpr int kPTiles = kSplit ? 1 : kAccStages + (kSecond ? 1 : 0);
@@ -409,11 +436,15 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP)
         int li = 0;
         for (int i = 0; i < count; ++i) {
           const Tile t = decode_tile(P, first + i * stride, li);
-          const int a = i % kAccStages;
-          mbar_wait(aempty0 + 8 * a, ((uint32_t)(i / kAccStages) & 1u) ^ 1u);     // its previous tile's store has read it
-          mbar_expect_tx(afull0 + 8 * a, kPBytes);   // (a partial tile's out-of-range pixels land as zeros)
-          tma_load_2d_hint(&MP.amap[t.li], afull0 + 8 * a, sP_u32 + a * kPBytes, t.pixel0,
-                           (t.prompt * P.layer[t.li].heads + t.head) * kTokens, pol);
+#pragma unroll
+          for (int c = 0; c < kC; ++c) {             // one ring slot per 77-token chunk of the tile
+            const int n = i * kC + c;
+            const int a = n % kAccStages;
+            mbar_wait(aempty0 + 8 * a, ((uint32_t)(n / kAccStages) & 1u) ^ 1u);   // its previous tile's store has read it
+            mbar_expect_tx(afull0 + 8 * a, kPBytes);   // (a partial tile's out-of-range pixels land as zeros)
+            tma_load_2d_hint(&MP.amap[t.li], afull0 + 8 * a, sP_u32 + a * kPBytes, t.pixel0,
+                             (t.prompt * P.layer[t.li].heads + t.head) * kCtx + c * kTokens, pol);
+          }
         }
       }
     }
@@ -436,7 +467,9 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP)
             const int nc = kChunked ? (P.layer[u.li].head_dim + 63) >> 6 : 1;
             for (int c = 0; c < nc; ++c) {
               tma_prefetch_4d(&MP.qmap[u.li], 64 * c, u.head, u.pixel0, u.prompt, pol);
-              if (new_head) tma_prefetch_4d(&MP.kmap[u.li], 64 * c, u.head, 0, u.prompt, pol);
+              if (new_head)
+#pragma unroll
+                for (int kc = 0; kc < kC; ++kc) tma_prefetch_4d(&MP.kmap[u.li], 64 * c, u.head, kc * kTokens, u.prompt, pol);
             }
             prev = u;
           }
@@ -457,9 +490,11 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP)
             tma_load_4d(&MP.kmap[t.li], full0 + 8 * s, k_dst + kKBytes, 64 * c + 32, t.head, 0, t.prompt);
           } else {
             const uint32_t k_dst = q_dst + kQBytes;
-            mbar_expect_tx(full0 + 8 * s, kStageBytes);
+            mbar_expect_tx(full0 + 8 * s, kStageBytesT);
             tma_load_4d(&MP.qmap[t.li], full0 + 8 * s, q_dst, 64 * c, t.head, t.pixel0, t.prompt);
-            tma_load_4d(&MP.kmap[t.li], full0 + 8 * s, k_dst, 64 * c, t.head, 0, t.prompt);
+#pragma unroll
+            for (int kc = 0; kc < kC; ++kc)            // K box kc: token rows 77 kc .. 77 kc + 79
+              tma_load_4d(&MP.kmap[t.li], full0 + 8 * s, k_dst + kc * kKBytes, 64 * c, t.head, kc * kTokens, t.prompt);
           }
         }
       }
@@ -476,14 +511,18 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP)
       const Tile t = decode_tile(P, first + i * stride, li);
       const LayerParams& L = P.layer[t.li];
       const int n_chunks = kChunked ? (L.head_dim + 63) >> 6 : 1;
-      Frag d;
+      Frag dd[kC];                                     // the logits of 77-token chunk c in dd[c]
+      Frag& d = dd[0];
 #pragma unroll
-      for (int e = 0; e < 40; ++e) d[e] = 0.f;
+      for (int kc = 0; kc < kC; ++kc)
+#pragma unroll
+        for (int e = 0; e < 40; ++e) dd[kc][e] = 0.f;
       for (int c = 0; c < n_chunks; ++c, ++j) {
         const int s = j % kStages;
         mbar_wait(full0 + 8 * s, (uint32_t)(j / kStages) & 1u);        // the chunk's operand tiles have landed
         const uint32_t q_src = base + s * kStageBytesT;
-        frag_fence(d);
+#pragma unroll
+        for (int kc = 0; kc < kC; ++kc) frag_fence(dd[kc]);
         if constexpr (kSplit) {
           uint8_t* stage = gen + s * kStageBytesT;
           uint8_t* lo = gen + kStages * kStageBytesT;
@@ -509,24 +548,35 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP)
         } else {
           // K 16 = 32 bytes along the swizzled row; columns beyond head_dim are zero-filled by TMA
           const uint32_t a_src = q_src + wg * 64 * 128, k_src = q_src + kQBytes;
-          if (L.dtype == DAAM_BF16)
-            wgmma_chunk_16bit<true>(d, a_src, k_src);
-          else
-            wgmma_chunk_16bit<false>(d, a_src, k_src);
+          if constexpr (kC == 1) {
+            if (L.dtype == DAAM_BF16)
+              wgmma_chunk_16bit<true>(d, a_src, k_src);
+            else
+              wgmma_chunk_16bit<false>(d, a_src, k_src);
+          } else {
+            if (L.dtype == DAAM_BF16)
+              wgmma_chunk_16bit_long<true, kC>(dd, a_src, k_src);
+            else
+              wgmma_chunk_16bit_long<false, kC>(dd, a_src, k_src);
+          }
         }
-        frag_fence(d);
+#pragma unroll
+        for (int kc = 0; kc < kC; ++kc) frag_fence(dd[kc]);
         __syncwarp();
         if (lane == 0) mbar_arrive(empty0 + 8 * s);    // this warp is done with the stage
       }
 
       // softmax over the 77 live columns of rows r0 (d[4j], d[4j+1]) and r0 + 8 (d[4j+2], d[4j+3]); columns 77..79
-      // (zero-filled token rows) sit in j = 9 of quads 2 (odd column) and 3
+      // (zero-filled token rows) sit in j = 9 of quads 2 (odd column) and 3. Long contexts: the same over every chunk's
+      // fragment (there columns 77..79 hold the next chunk's first tokens, masked alike).
       float m0 = d[0], m1 = d[2];
+#pragma unroll
+      for (int kc = 0; kc < kC; ++kc)
 #pragma unroll
       for (int jj = 0; jj < 10; ++jj) {
         const bool l0 = jj < 9 || quad <= 2, l1 = jj < 9 || quad < 2;   // column 8jj+2q (+1) < 77
-        if (l0) { m0 = fmaxf(m0, d[4 * jj]); m1 = fmaxf(m1, d[4 * jj + 2]); }
-        if (l1) { m0 = fmaxf(m0, d[4 * jj + 1]); m1 = fmaxf(m1, d[4 * jj + 3]); }
+        if (l0) { m0 = fmaxf(m0, dd[kc][4 * jj]); m1 = fmaxf(m1, dd[kc][4 * jj + 2]); }
+        if (l1) { m0 = fmaxf(m0, dd[kc][4 * jj + 1]); m1 = fmaxf(m1, dd[kc][4 * jj + 3]); }
       }
       m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 1));
       m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 2));
@@ -535,14 +585,17 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP)
       const float sc = L.scale_log2e, mc0 = m0 * sc, mc1 = m1 * sc;
       float sum0 = 0.f, sum1 = 0.f;
 #pragma unroll
+      for (int kc = 0; kc < kC; ++kc)
+#pragma unroll
       for (int jj = 0; jj < 10; ++jj) {
         const bool l0 = jj < 9 || quad <= 2, l1 = jj < 9 || quad < 2;
-        d[4 * jj] = l0 ? fast_exp2(fmaf(d[4 * jj], sc, -mc0)) : 0.f;
-        d[4 * jj + 2] = l0 ? fast_exp2(fmaf(d[4 * jj + 2], sc, -mc1)) : 0.f;
-        d[4 * jj + 1] = l1 ? fast_exp2(fmaf(d[4 * jj + 1], sc, -mc0)) : 0.f;
-        d[4 * jj + 3] = l1 ? fast_exp2(fmaf(d[4 * jj + 3], sc, -mc1)) : 0.f;
-        sum0 += d[4 * jj] + d[4 * jj + 1];
-        sum1 += d[4 * jj + 2] + d[4 * jj + 3];
+        float* f = dd[kc];
+        f[4 * jj] = l0 ? fast_exp2(fmaf(f[4 * jj], sc, -mc0)) : 0.f;
+        f[4 * jj + 2] = l0 ? fast_exp2(fmaf(f[4 * jj + 2], sc, -mc1)) : 0.f;
+        f[4 * jj + 1] = l1 ? fast_exp2(fmaf(f[4 * jj + 1], sc, -mc0)) : 0.f;
+        f[4 * jj + 3] = l1 ? fast_exp2(fmaf(f[4 * jj + 3], sc, -mc1)) : 0.f;
+        sum0 += f[4 * jj] + f[4 * jj + 1];
+        sum1 += f[4 * jj + 2] + f[4 * jj + 3];
       }
       sum0 += __shfl_xor_sync(0xffffffffu, sum0, 1);
       sum0 += __shfl_xor_sync(0xffffffffu, sum0, 2);
@@ -555,12 +608,15 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP)
         // store (clipped to the map for a partial tile). Quads 0-1 update row r0 while quads 2-3 update row r0 + 8 (and
         // then the other way round), so one access touches 16 banks instead of 8. All old values are loaded before the
         // first store: the compiler cannot tell the two rows apart and would otherwise serialise every load behind the
-        // previous store.
-        const int a = i % kAccStages;
+        // previous store. Long contexts: chunk kc of the tile goes through ring slot n = i kC + kc, with this epilogue.
+#pragma unroll
+        for (int kc = 0; kc < kC; ++kc) {
+        const int n = i * kC + kc;
+        const int a = n % kAccStages;
         float* sA = sP + a * (kTokens * kTilePixels);
         const bool lowq = quad < 2;
         const int ra = lowq ? r0 : r0 + 8, rb = lowq ? r0 + 8 : r0;
-        mbar_wait(afull0 + 8 * a, (uint32_t)(i / kAccStages) & 1u);
+        mbar_wait(afull0 + 8 * a, (uint32_t)(n / kAccStages) & 1u);
         float old[40];
 #pragma unroll
         for (int jj = 0; jj < 10; ++jj) {
@@ -577,13 +633,14 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP)
           if (tid == 0 && i > 0) bulk_wait_read0();
           consumer_barrier();
         }
+        const float* f = dd[kc];
 #pragma unroll
         for (int jj = 0; jj < 10; ++jj) {
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             const int col = 8 * jj + 2 * quad + e;
             if (col < kTokens) {
-              const float pa = d[4 * jj + e] * inv0, pb = d[4 * jj + 2 + e] * inv1;
+              const float pa = f[4 * jj + e] * inv0, pb = f[4 * jj + 2 + e] * inv1;
               sA[col * kTilePixels + ra] = add_ftz(old[4 * jj + e], lowq ? pa : pb);
               sA[col * kTilePixels + rb] = add_ftz(old[4 * jj + 2 + e], lowq ? pb : pa);
               if constexpr (kSecond) {
@@ -596,17 +653,18 @@ accumulate_mma_kernel(const __grid_constant__ MmaParamsT<kSlab != kSlabNone> MP)
         fence_proxy_async();                           // generic-proxy writes -> visible to the bulk-async proxy
         consumer_barrier();
         if (tid == 0) {
-          tma_store_2d_hint(&MP.amap[t.li], sP_u32 + a * kPBytes, t.pixel0, (t.prompt * L.heads + t.head) * kTokens,
-                            l2_evict_first());
+          tma_store_2d_hint(&MP.amap[t.li], sP_u32 + a * kPBytes, t.pixel0,
+                            (t.prompt * L.heads + t.head) * kCtx + kc * kTokens, l2_evict_first());
           if constexpr (kSlab == kSlabStore)           // same bulk group: the waits below cover both stores
             tma_store_2d(&MP.smap[t.li], sS_u32, t.pixel0, (t.prompt * L.heads + t.head) * kTokens);
           if constexpr (kSlab == kSlabAdd)             // (and the range reduce: its reads of sS)
             tma_reduce_add_2d(&MP.smap[t.li], sS_u32, t.pixel0, (t.prompt * L.heads + t.head) * kTokens);
           bulk_commit();
-          if (i > 0) {                                 // one store of slack: the previous tile's store has read its slot
+          if (n > 0) {                                 // one store of slack: the previous tile's store has read its slot
             bulk_wait_read1();
-            mbar_arrive(aempty0 + 8 * ((i - 1) % kAccStages));
+            mbar_arrive(aempty0 + 8 * ((n - 1) % kAccStages));
           }
+        }
         }
         continue;
       }
@@ -796,7 +854,13 @@ const MmaInstance kMmaInstances[] = {
     {(const void*)accumulate_mma_kernel<true, false, kSlabAdd>, kSplitSmemBytes},
     {(const void*)accumulate_mma_kernel<false, true, kSlabAdd>, kSlabSmemBytes},
     {(const void*)accumulate_mma_kernel<true, true, kSlabAdd>, kSplitSmemBytes},
+    // long contexts (16-bit, plain slab mode), from kLongVariant0: bit 0 chunked, bit 1 three 77-token chunks (else two)
+    {(const void*)accumulate_mma_kernel<false, false, kSlabNone, 2>, long_smem_bytes(2)},
+    {(const void*)accumulate_mma_kernel<false, true, kSlabNone, 2>, long_smem_bytes(2)},
+    {(const void*)accumulate_mma_kernel<false, false, kSlabNone, 3>, long_smem_bytes(3)},
+    {(const void*)accumulate_mma_kernel<false, true, kSlabNone, 3>, long_smem_bytes(3)},
 };
+constexpr int kLongVariant0 = 12;
 
 std::once_flag g_attr_once[64];                       // the shared-memory attribute is per device
 
@@ -806,6 +870,7 @@ std::once_flag g_attr_once[64];                       // the shared-memory attri
 struct PreparedMma {
   MmaSlabParams mp;                                   // the plain instances are launched with its MmaParams part
   int grid, block, variant;                           // variant: index into kMmaInstances
+  bool second;                                        // a second-slab instance (takes the whole MmaSlabParams)
 };
 void* prepared_mma_new() { return new PreparedMma; }                 // (aligned new: CUtensorMap is alignas(64))
 void prepared_mma_delete(void* p) { delete static_cast<PreparedMma*>(p); }
@@ -826,13 +891,20 @@ int prepare_accumulate_mma(const LaunchParams& p, const SecondSlabs* slabs, Slab
   MmaSlabParams& mp = pm.mp;
   mp.base = p;
   const bool split = p.n_layers > 0 && p.layer[0].dtype == DAAM_F32;     // a pack holds one operand class (api.cu)
+  const int ctx = p.n_layers > 0 ? p.layer[0].tokens : kTokens;          // ... and one context length
+  if ((ctx != kTokens && ctx != 2 * kTokens && ctx != 3 * kTokens) || (ctx != kTokens && (split || slabs))) {
+    set_error("the wgmma kernel takes %d-token contexts, or 154 / 231 tokens for 16-bit layers without a second slab "
+              "(got %d)", kTokens, ctx);
+    return DAAM_E_UNSUPPORTED;
+  }
   bool chunked = false;
   for (int i = 0; i < p.n_layers; ++i) {
     const LayerParams& L = p.layer[i];
     if ((L.dtype == DAAM_F32) != split) { set_error("mixed fp32 / 16-bit layers in one wgmma pack"); return DAAM_E_INVALID; }
+    if (L.tokens != ctx) { set_error("mixed context lengths in one wgmma pack"); return DAAM_E_INVALID; }
     if (int rc = make_qk_map(L.q, L.dtype, L.head_dim, L.heads, L.hw, L.n_prompts, L.qs_head, L.qs_pixel, L.qs_prompt, kTilePixels, &mp.qmap[i])) return rc;
-    if (int rc = make_qk_map(L.k, L.dtype, L.head_dim, L.heads, kTokens, L.n_prompts, L.ks_head, L.ks_token, L.ks_prompt, kTokensPad, &mp.kmap[i])) return rc;
-    if (int rc = make_acc_map(L.acc, L.hw, L.n_prompts * L.heads * kTokens, &mp.amap[i])) return rc;
+    if (int rc = make_qk_map(L.k, L.dtype, L.head_dim, L.heads, ctx, L.n_prompts, L.ks_head, L.ks_token, L.ks_prompt, kTokensPad, &mp.kmap[i])) return rc;
+    if (int rc = make_acc_map(L.acc, L.hw, L.n_prompts * L.heads * ctx, &mp.amap[i])) return rc;
     if (slabs) {                                      // the second slab has the accumulator's shape: same map, other base
       if (int rc = make_acc_map(slabs->slab[i], L.hw, L.n_prompts * L.heads * kTokens, &mp.smap[i])) return rc;
       mp.slab[i] = slabs->slab[i];
@@ -848,7 +920,9 @@ int prepare_accumulate_mma(const LaunchParams& p, const SecondSlabs* slabs, Slab
   pm.grid = dev.sm_count;                             // one CTA per SM (both forms fill its shared memory)
   if (pm.grid > p.total_tiles) pm.grid = p.total_tiles;
   pm.block = split ? kThreads : kThreads16;
-  pm.variant = (split ? 1 : 0) | (chunked ? 2 : 0) | (mode << 2);
+  pm.variant = ctx == kTokens ? (split ? 1 : 0) | (chunked ? 2 : 0) | (mode << 2)
+                              : kLongVariant0 + (chunked ? 1 : 0) + (ctx == 3 * kTokens ? 2 : 0);
+  pm.second = mode != kSlabNone;
   return DAAM_OK;
 }
 
@@ -869,7 +943,7 @@ int launch_prepared_mma(const void* prepared, cudaStream_t stream) {
   cfg.numAttrs = 1;
   // the one kernel argument: the whole block for the second-slab instances, its MmaParams part for the plain ones
   const MmaParams* plain = &pm.mp;
-  void* args[] = {(pm.variant >> 2) != kSlabNone ? (void*)&pm.mp : (void*)plain};
+  void* args[] = {pm.second ? (void*)&pm.mp : (void*)plain};
   DAAM_CUDA_TRY(cudaLaunchKernelExC(&cfg, k.fn, args));
   DAAM_CUDA_TRY(cudaGetLastError());
   count_launch();

@@ -55,7 +55,7 @@ int make_layer_params(const daam_layer& in, int index, LayerParams* out, bool ne
 int make_layer_params(const daam_layer& in, int index, LayerParams* out, bool need_acc) {
   if (!in.q || !in.k || (need_acc && !in.acc)) { set_error("daam_accumulate: layer %d has a null pointer", index); return DAAM_E_INVALID; }
   if (in.dtype != DAAM_F32 && in.dtype != DAAM_F16 && in.dtype != DAAM_BF16) { set_error("daam_accumulate: layer %d: unknown dtype %d", index, in.dtype); return DAAM_E_INVALID; }
-  if (in.tokens != kTokens) { set_error("daam_accumulate: layer %d: tokens = %d, only %d is traced (daam/trace.py:289)", index, in.tokens, kTokens); return DAAM_E_UNSUPPORTED; }
+  if (in.tokens != kTokens && in.tokens != 2 * kTokens && in.tokens != 3 * kTokens) { set_error("daam_accumulate: layer %d: tokens = %d, only %d, %d or %d (one to three %d-token CLIP chunks) are traced", index, in.tokens, kTokens, 2 * kTokens, 3 * kTokens, kTokens); return DAAM_E_UNSUPPORTED; }
   if (in.head_dim <= 0 || in.head_dim % 8 != 0 || in.head_dim > DAAM_MAX_HEAD_DIM) { set_error("daam_accumulate: layer %d: head_dim = %d must be a multiple of 8 in (0, %d]", index, in.head_dim, DAAM_MAX_HEAD_DIM); return DAAM_E_UNSUPPORTED; }
   if (in.n_prompts <= 0 || in.heads <= 0 || in.hw <= 0) { set_error("daam_accumulate: layer %d: non-positive n_prompts/heads/hw", index); return DAAM_E_INVALID; }
   if (need_acc && reinterpret_cast<uintptr_t>(in.acc) % 16 != 0) { set_error("daam_accumulate: layer %d: acc is not 16-byte aligned", index); return DAAM_E_INVALID; }
@@ -76,7 +76,7 @@ int make_layer_params(const daam_layer& in, int index, LayerParams* out, bool ne
   L.vec_ok = reinterpret_cast<uintptr_t>(in.q) % 16 == 0 && reinterpret_cast<uintptr_t>(in.k) % 16 == 0 &&
              aligned(in.q_stride_prompt) && aligned(in.q_stride_pixel) && aligned(in.q_stride_head) &&
              aligned(in.k_stride_prompt) && aligned(in.k_stride_token) && aligned(in.k_stride_head);
-  L.pad_ = 0;
+  L.tokens = in.tokens;
   return DAAM_OK;
 }
 
@@ -87,9 +87,10 @@ using namespace daam;
 namespace daam {
 namespace {
 
-// One kernel launch of a plan: a pack of layers for the wgmma kernel (prepared block, opaque) or the SIMT kernel.
+// One kernel launch of a plan: a pack of layers for the wgmma kernel (prepared block, opaque) or a SIMT kernel.
 struct PlannedLaunch {
   bool is_mma = false;
+  bool simt_long = false;                // SIMT: the long-context kernel (154- / 231-token layers)
   LaunchParams simt;                     // SIMT: the parameter block itself
   SlabMode mode = kSlabNone;             // SIMT: the step- or range-slab kernel, with these slabs
   SecondSlabs slabs;
@@ -112,8 +113,8 @@ struct Plan {
 };
 constexpr size_t kMaxPlans = 32;
 
-// Whether the accumulator slabs [n_prompts][heads][77][hw] (fp32) of two layers share bytes.
-size_t slab_bytes(const LayerParams& l) { return (size_t)l.n_prompts * l.heads * kTokens * l.hw * sizeof(float); }
+// Bytes of a layer's accumulator slab [n_prompts][heads][tokens][hw] (fp32).
+size_t slab_bytes(const LayerParams& l) { return (size_t)l.n_prompts * l.heads * l.tokens * l.hw * sizeof(float); }
 
 // Whether [a, a + na) and [b, b + nb) share bytes.
 bool spans_overlap(const void* a, size_t na, const void* b, size_t nb) {
@@ -134,8 +135,10 @@ const char* slab_word(SlabMode mode) { return mode == kSlabAdd ? "range" : "step
 int validate_second_slabs(const char* fn, const daam_layer* layers, float* const* slabs, int n_layers, SlabMode mode) {
   const char* what = slab_word(mode);
   std::vector<LayerParams> all((size_t)n_layers);
-  for (int i = 0; i < n_layers; ++i)
+  for (int i = 0; i < n_layers; ++i) {
     if (int rc = make_layer_params(layers[i], i, &all[i], /*need_acc=*/true)) return rc;
+    if (all[i].tokens != kTokens) { set_error("%s: layer %d: tokens = %d, the %s slabs take %d-token contexts only", fn, i, all[i].tokens, what, kTokens); return DAAM_E_UNSUPPORTED; }
+  }
   for (int i = 0; i < n_layers; ++i) {
     if (!slabs[i]) { set_error("%s: layer %d has a null %s slab", fn, i, what); return DAAM_E_INVALID; }
     if (reinterpret_cast<uintptr_t>(slabs[i]) % 16 != 0) { set_error("%s: layer %d: the %s slab is not 16-byte aligned", fn, i, what); return DAAM_E_INVALID; }
@@ -159,10 +162,14 @@ int validate_second_slabs(const char* fn, const daam_layer* layers, float* const
 int build_plan(const daam_layer* layers, float* const* slabs, SlabMode mode, int n_layers, uint32_t flags,
                const DeviceInfo& dev, Plan* plan) {
   const uint32_t path = flags & 3u, rmw = flags & DAAM_ACC_RMW_MASK;
-  // Three packs: 16-bit layers for the wgmma kernel (TMA form), fp32 layers for its split form, and the rest for
-  // the SIMT kernel. Each is closed when its parameter block is full.
-  LaunchParams packs[3];                 // 0: wgmma 16-bit, 1: wgmma fp32, 2: SIMT
-  SecondSlabs pack_slabs[3];             // steps / range: the second slab of every layer of a pack
+  // Three packs of 77-token layers: 16-bit layers for the wgmma kernel (TMA form), fp32 layers for its split form, and
+  // the rest for the SIMT kernel. Long contexts (154 / 231 tokens) take four more, one per context length and kernel:
+  // a long-context layer never shares a launch with a layer of another length or class. Each pack is closed when its
+  // parameter block is full.
+  constexpr int kPacks = 7;
+  LaunchParams packs[kPacks];            // 0: wgmma 16-bit, 1: wgmma fp32, 2: SIMT; 3 / 4: wgmma 16-bit at 154 / 231
+  SecondSlabs pack_slabs[kPacks];        // tokens; 5 / 6: long-context SIMT at 154 / 231 tokens
+                                         // steps / range: the second slab of every layer of a pack
   for (LaunchParams& p : packs) {
     p.n_layers = p.total_tiles = 0;
     p.rmw_mode = (rmw == DAAM_ACC_RMW_LDST) ? 0 : 1;     // default: reduce-add
@@ -178,12 +185,16 @@ int build_plan(const daam_layer* layers, float* const* slabs, SlabMode mode, int
     if (p.n_layers == 0) return DAAM_OK;
     plan->launches.emplace_back();
     PlannedLaunch& l = plan->launches.back();
-    l.is_mma = which != 2;
+    l.is_mma = which != 2 && which < 5;
+    l.simt_long = which >= 5;
     const SecondSlabs* st = slabs ? &pack_slabs[which] : nullptr;
     int rc;
     if (l.is_mma) {
       l.mma.reset(prepared_mma_new());
       rc = prepare_accumulate_mma(p, st, mode, dev, l.mma.get());
+    } else if (l.simt_long) {
+      l.simt = p;
+      rc = prepare_accumulate_simt_long(p, dev, &l.grid, &l.smem);
     } else {
       l.simt = p;
       l.mode = mode;
@@ -198,13 +209,16 @@ int build_plan(const daam_layer* layers, float* const* slabs, SlabMode mode, int
   for (int i = 0; i < n_layers; ++i) {
     LayerParams L;
     if (int rc = make_layer_params(layers[i], i, &L, /*need_acc=*/true)) return rc;
-    const bool use_mma = path != DAAM_ACC_FORCE_SIMT && dev.cc_major == 9 && mma_supported(L);
+    const int ctx_chunks = L.tokens / kTokens;          // 1, or 2 / 3 for a long context
+    // (the wgmma kernel's fp32 split form has no long-context instances: such layers take the SIMT kernel)
+    const bool use_mma = path != DAAM_ACC_FORCE_SIMT && dev.cc_major == 9 && mma_supported(L) &&
+                         (ctx_chunks == 1 || L.dtype != DAAM_F32);
     if (path == DAAM_ACC_FORCE_MMA && !use_mma) {
       set_error("daam_accumulate: layer %d cannot take the wgmma path (dtype %d, head_dim %d, alignment %d, hw = %d, "
-                "sm_%d%d)", i, L.dtype, L.head_dim, L.vec_ok, L.hw, dev.cc_major, dev.cc_minor);
+                "tokens = %d, sm_%d%d)", i, L.dtype, L.head_dim, L.vec_ok, L.hw, L.tokens, dev.cc_major, dev.cc_minor);
       return DAAM_E_UNSUPPORTED;
     }
-    const int which = use_mma ? (L.dtype == DAAM_F32 ? 1 : 0) : 2;
+    const int which = ctx_chunks > 1 ? (use_mma ? 1 : 3) + ctx_chunks : use_mma ? (L.dtype == DAAM_F32 ? 1 : 0) : 2;
     LaunchParams& p = packs[which];
     // Two layers of one launch must not share accumulator elements: their tiles run concurrently, and the 16-bit wgmma
     // form and the LDST mode read, add and store them (lost updates), while RED would add in timing order (results not
@@ -230,7 +244,7 @@ int build_plan(const daam_layer* layers, float* const* slabs, SlabMode mode, int
     if (p.n_layers == kMaxLayersPerLaunch)
       if (int rc = close(which)) return rc;
   }
-  for (int which = 0; which < 3; ++which)
+  for (int which = 0; which < kPacks; ++which)
     if (int rc = close(which)) return rc;
   return DAAM_OK;
 }
@@ -291,9 +305,10 @@ int accumulate_impl(const char* fn, const daam_layer* layers, float* const* slab
   }
   plan->stamp = ++clock;
   for (const PlannedLaunch& l : plan->launches) {
-    const int rc = l.is_mma ? launch_prepared_mma(l.mma.get(), stream)
-                            : launch_prepared_simt(l.simt, l.mode != kSlabNone ? &l.slabs : nullptr, l.mode, l.grid,
-                                                   l.smem, stream);
+    const int rc = l.is_mma      ? launch_prepared_mma(l.mma.get(), stream)
+                   : l.simt_long ? launch_prepared_simt_long(l.simt, l.grid, l.smem, stream)
+                                 : launch_prepared_simt(l.simt, l.mode != kSlabNone ? &l.slabs : nullptr, l.mode,
+                                                        l.grid, l.smem, stream);
     if (rc) return rc;
   }
   return DAAM_OK;

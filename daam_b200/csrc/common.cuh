@@ -30,7 +30,7 @@ struct LayerParams {
   int vec_ok;               // 1: q/k rows are 16-byte aligned -> vector loads
   int weight;               // relative cost of one tile of this layer (wgmma kernel, K-chunked launches)
   int weight_begin;         // exclusive prefix of tiles x weight over the launch's layers
-  int pad_;
+  int tokens;               // context rows: 77, or 154 / 231 (long-context instances); the accumulator's token extent
 };
 
 struct LaunchParams {
@@ -93,6 +93,9 @@ void count_launch(int n = 1);
 int prepare_accumulate_simt(const LaunchParams& p, SlabMode mode, const DeviceInfo& dev, int* grid, size_t* smem);
 int launch_prepared_simt(const LaunchParams& p, const SecondSlabs* slabs, SlabMode mode, int grid, size_t smem,
                          cudaStream_t stream);
+// The SIMT kernel of 154- / 231-token contexts (accumulate_simt_long.cu): every layer of `p` has the same context length.
+int prepare_accumulate_simt_long(const LaunchParams& p, const DeviceInfo& dev, int* grid, size_t* smem);
+int launch_prepared_simt_long(const LaunchParams& p, int grid, size_t smem, cudaStream_t stream);
 void* prepared_mma_new();
 void prepared_mma_delete(void* prepared);
 int prepare_accumulate_mma(const LaunchParams& p, const SecondSlabs* slabs, SlabMode mode, const DeviceInfo& dev,

@@ -104,6 +104,7 @@ extern "C" int daam_attention_probs(const daam_layer* layer, void* probs, void* 
   if (int rc = get_device_info(&dev)) return rc;
   static thread_local LaunchParams p;
   if (int rc = make_layer_params(*layer, 0, &p.layer[0], /*need_acc=*/false)) return rc;
+  if (layer->tokens != kTokens) { set_error("daam_attention_probs: tokens = %d, only %d-token contexts are materialised (the save_heads file format)", layer->tokens, kTokens); return DAAM_E_UNSUPPORTED; }
   p.n_layers = 1;
   p.layer[0].tile_begin = 0;
   p.total_tiles = p.layer[0].tiles_per_head * p.layer[0].heads * p.layer[0].n_prompts;
@@ -137,7 +138,7 @@ extern "C" int daam_accumulate_probs(const void* probs, int32_t dtype, int32_t f
                                      int32_t tokens, float* acc, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!probs || !acc || first_row < 0 || n_rows <= 0 || hw <= 0) { set_error("daam_accumulate_probs: null pointer or bad size"); return DAAM_E_INVALID; }
-  if (tokens != kTokens) { set_error("daam_accumulate_probs: tokens = %d, only %d is traced (daam/trace.py:289)", tokens, kTokens); return DAAM_E_UNSUPPORTED; }
+  if (tokens != kTokens) { set_error("daam_accumulate_probs: tokens = %d, only %d-token probabilities are accumulated (the load_heads file format)", tokens, kTokens); return DAAM_E_UNSUPPORTED; }
   if (dtype != DAAM_F32 && dtype != DAAM_F16 && dtype != DAAM_BF16) { set_error("daam_accumulate_probs: unknown dtype %d", dtype); return DAAM_E_INVALID; }
   DeviceInfo dev;
   if (int rc = get_device_info(&dev)) return rc;

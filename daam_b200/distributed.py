@@ -35,7 +35,8 @@ def gather_heat_maps(local_maps: Sequence[torch.Tensor], n_total: int, x, group=
                      tokens: int = TOKENS, device=None) -> Optional[torch.Tensor]:
     """All-gathers per-prompt global heat maps. ``local_maps[j]`` belongs to prompt ``rank + j * world``; returns
     ``[n_total, tokens, xh, xw]`` (rows beyond a prompt's length are zero) on every rank. ``x``: the map side, or
-    ``(xh, xw)`` for non-square images.
+    ``(xh, xw)`` for non-square images. Compact maps of a ``long_prompts`` trace with ``c``-chunk contexts have up to
+    ``75 c + 2`` rows: pass ``tokens=75 * c + 2``.
 
     ``device``: where the exchange buffers live. Default: the device of ``local_maps``; a rank that owns no prompt
     (``n_total < world``, or an uneven shard) has no map to infer it from and then uses the current CUDA device under

@@ -80,6 +80,11 @@ class LayerSlab:
         return self.acc.shape[0]
 
     @property
+    def tokens(self) -> int:
+        """Context rows of every key: 77, or 154 / 231 in a ``long_prompts`` trace."""
+        return self.acc.shape[2]
+
+    @property
     def heads_per_image(self) -> int:
         return self.heads // self.images
 
@@ -137,11 +142,14 @@ class RawHeatMapCollection:
             self._sync()
 
     def slab_for(self, layer_idx: int, factor: int, n_prompts: int, heads: int, h: int, w: int, device,
-                 head_offset: int = 0, images: int = 1) -> LayerSlab:
+                 head_offset: int = 0, images: int = 1, tokens: int = _native.TOKENS) -> LayerSlab:
         """Returns (allocating or re-shaping on demand) the zero-initialised slab of a layer and marks it live.
-        ``heads`` counts every image's heads of one prompt (``images`` runs of ``heads // images``)."""
+        ``heads`` counts every image's heads of one prompt (``images`` runs of ``heads // images``); ``tokens`` is the
+        context length (77, or 154 / 231 in a ``long_prompts`` trace): every context row is accumulated."""
+        if tokens not in _native.CONTEXT_TOKENS:
+            raise ValueError(f'a slab holds a context of {_native.CONTEXT_TOKENS} tokens, not {tokens}')
         slab = self.slabs.get(layer_idx)
-        shape = (n_prompts, heads, _native.TOKENS, h * w)
+        shape = (n_prompts, heads, tokens, h * w)
         if slab is None or tuple(slab.acc.shape) != shape or slab.acc.device != torch.device(device) \
                 or slab.factor != factor or (self.time_resolved and slab.step is None) \
                 or (self.n_ranges and slab.ranges is None) or (self.negative and slab.neg is None):

@@ -31,16 +31,17 @@ def cond_half(bsz: int, heads: int) -> Tuple[int, int, int, int]:
     raise RuntimeError(f'a batch of {bsz} is neither a CFG pair batch nor a single sample')
 
 
-def new_accumulator(n_prompts: int, heads: int, hw: int, device) -> torch.Tensor:
-    return torch.zeros((n_prompts, heads, _native.TOKENS, hw), dtype=torch.float32, device=device)
+def new_accumulator(n_prompts: int, heads: int, hw: int, device, tokens: int = _native.TOKENS) -> torch.Tensor:
+    return torch.zeros((n_prompts, heads, tokens, hw), dtype=torch.float32, device=device)
 
 
 def make_layer_desc(q: torch.Tensor, k: torch.Tensor, acc: torch.Tensor, heads: int, scale: float, *,
                     whole_batch: bool = False) -> _native.DaamLayer:
-    """``q [B, hw, heads*d]`` / ``k [B, 77, heads*d]`` as ``to_q`` / ``to_k`` emit them (last axis contiguous) and the
-    fp32 accumulator ``[n_prompts, n_heads, 77, hw]`` of the kept slice -> one ``daam_layer``. ``whole_batch``: the
-    descriptor covers every sample from sample 0 -- both halves of a CFG batch, the unconditional one first -- and
-    ``acc`` is ``[B, heads, 77, hw]``."""
+    """``q [B, hw, heads*d]`` / ``k [B, T, heads*d]`` as ``to_q`` / ``to_k`` emit them (last axis contiguous) and the
+    fp32 accumulator ``[n_prompts, n_heads, T, hw]`` of the kept slice -> one ``daam_layer``. ``T`` is the context
+    length: 77, or 154 / 231 for a long context (``_native.CONTEXT_TOKENS``). ``whole_batch``: the descriptor covers
+    every sample from sample 0 -- both halves of a CFG batch, the unconditional one first -- and ``acc`` is
+    ``[B, heads, T, hw]``."""
     if not (q.is_cuda and k.is_cuda and acc.is_cuda):
         raise RuntimeError('daam_b200 computes on CUDA tensors only (there is no CPU fallback)')
     if q.dtype not in _DTYPES or k.dtype != q.dtype:
@@ -50,9 +51,10 @@ def make_layer_desc(q: torch.Tensor, k: torch.Tensor, acc: torch.Tensor, heads: 
     bsz, hw, chan = q.shape
     d = chan // heads
     first, n_prompts, head0, n_heads = (0, bsz, 0, heads) if whole_batch else cond_half(bsz, heads)
-    if tuple(acc.shape) != (n_prompts, n_heads, _native.TOKENS, hw) or acc.dtype != torch.float32 \
+    tokens = k.shape[1] if k.shape[1] in _native.CONTEXT_TOKENS else _native.TOKENS
+    if tuple(acc.shape) != (n_prompts, n_heads, tokens, hw) or acc.dtype != torch.float32 \
             or not acc.is_contiguous():
-        raise RuntimeError(f'accumulator must be contiguous fp32 {(n_prompts, n_heads, _native.TOKENS, hw)}, '
+        raise RuntimeError(f'accumulator must be contiguous fp32 {(n_prompts, n_heads, tokens, hw)}, '
                            f'got {acc.dtype} {tuple(acc.shape)}')
     es = q.element_size()
     return _native.DaamLayer(
@@ -119,7 +121,8 @@ def accumulate_layer(q: torch.Tensor, k: torch.Tensor, heads: int, scale: Option
     bsz, hw, chan = q.shape
     _, n_prompts, _, n_heads = cond_half(bsz, heads)
     if acc is None:
-        acc = new_accumulator(n_prompts, n_heads, hw, q.device)
+        acc = new_accumulator(n_prompts, n_heads, hw, q.device,
+                              k.shape[1] if k.shape[1] in _native.CONTEXT_TOKENS else _native.TOKENS)
     if scale is None:
         scale = (chan // heads) ** -0.5
     accumulate([make_layer_desc(q, k, acc, heads, scale)], q.device, flags=flags)

@@ -437,9 +437,15 @@ class SyntheticPipeline:
         self._graphs = {}
         self._attn = [m for m in self.unet.modules() if isinstance(m, SyntheticAttention)]
 
-    def check_inputs(self, prompt, height=None, width=None, callback_steps=None, negative_prompt=None, *args, **kwargs):
-        """diffusers' SD ``check_inputs`` parameter order, so that callers bind ``negative_prompt`` as they do there."""
-        if not isinstance(prompt, (str, list)):
+    def check_inputs(self, prompt, height=None, width=None, callback_steps=None, negative_prompt=None,
+                     prompt_embeds=None, negative_prompt_embeds=None, *args, **kwargs):
+        """diffusers' SD ``check_inputs`` parameter order, so that callers bind ``negative_prompt`` and
+        ``prompt_embeds`` as they do there."""
+        if prompt is None and prompt_embeds is None:
+            raise ValueError('Provide either `prompt` or `prompt_embeds`')
+        if prompt is not None and prompt_embeds is not None:
+            raise ValueError('Cannot forward both `prompt` and `prompt_embeds`')
+        if prompt is not None and not isinstance(prompt, (str, list)):
             raise ValueError('`prompt` has to be of type `str` or `list`')
         if negative_prompt is not None and not isinstance(negative_prompt, (str, list)):
             raise ValueError('`negative_prompt` has to be of type `str` or `list`')
@@ -459,15 +465,15 @@ class SyntheticPipeline:
         lat.copy_((lat - 0.02 * eps).clamp_(-4, 4))
         st['stat'].copy_(eps.float().mean(dim=(1, 2, 3)))
 
-    def _state(self, n, latent_h, latent_w):
+    def _state(self, n, latent_h, latent_w, tokens):
         spec, dev = self.unet.spec, self.device
-        key = (n, latent_h, latent_w, tuple(id(m.processor) for m in self._attn))
+        key = (n, latent_h, latent_w, tuple(id(m.processor) for m in self._attn), tokens)
         st = self._graphs.get(key)
         if st is None:
             if len(self._graphs) > 4:
                 self._graphs.clear()
             st = {
-                'emb': torch.empty(2 * n, spec.tokens, spec.cross_attention_dim, dtype=self.dtype, device=dev),
+                'emb': torch.empty(2 * n, tokens, spec.cross_attention_dim, dtype=self.dtype, device=dev),
                 'lat0': torch.empty(n, spec.in_channels, latent_h, latent_w, dtype=self.dtype, device=dev),
                 'latents': torch.empty(n, spec.in_channels, latent_h, latent_w, dtype=self.dtype, device=dev),
                 't': torch.zeros(1, dtype=torch.float32, device=dev),
@@ -478,28 +484,43 @@ class SyntheticPipeline:
         return st
 
     @torch.no_grad()
-    def __call__(self, prompt, num_inference_steps: int = 50, generator: Optional[torch.Generator] = None,
+    def __call__(self, prompt=None, num_inference_steps: int = 50, generator: Optional[torch.Generator] = None,
                  callback=None, guidance_scale: float = 7.5, height: Optional[int] = None, width: Optional[int] = None,
-                 negative_prompt=None, num_images_per_prompt: int = 1):
+                 negative_prompt=None, num_images_per_prompt: int = 1, prompt_embeds: Optional[torch.Tensor] = None,
+                 negative_prompt_embeds: Optional[torch.Tensor] = None):
         """``height`` / ``width``: the image size in pixels, as diffusers takes it (default: the model's own square
         size); the latent is ``height // 8 x width // 8``. ``negative_prompt`` reaches ``check_inputs`` positionally, in
         diffusers' SD order; the synthetic encoder ignores all text, so it changes no embedding or random draw.
         ``num_images_per_prompt``: like diffusers, every prompt's embeddings are repeated prompt-major (the batch is
         ``[uncond x N x n, cond x N x n]``) and one latent is drawn per image; with 1 the draws are those of a call
-        without it."""
+        without it. ``prompt_embeds`` / ``negative_prompt_embeds`` ``[N, T, C]`` (``prompt=None``; e.g. ``T`` = 154
+        or 231 for chunked long-prompt embeddings): the cond and uncond halves of the batch as given (zeros for a missing
+        uncond half) instead of the synthetic encoder's draw; ``check_inputs`` gets ``prompt=None`` and them by name."""
         spec = self.unet.spec
         height = spec.sample_size * self.vae_scale_factor if height is None else height
         width = spec.sample_size * self.vae_scale_factor if width is None else width
-        if negative_prompt is None:
+        if prompt_embeds is not None:
+            self.check_inputs(prompt, height, width, None, negative_prompt, prompt_embeds=prompt_embeds,
+                              negative_prompt_embeds=negative_prompt_embeds)
+        elif negative_prompt is None:
             self.check_inputs(prompt, height, width)
         else:
             self.check_inputs(prompt, height, width, None, negative_prompt)
-        prompts = [prompt] if isinstance(prompt, str) else list(prompt)
+        if prompt_embeds is not None:
+            prompts = [None] * prompt_embeds.shape[0]
+        else:
+            prompts = [prompt] if isinstance(prompt, str) else list(prompt)
         latent_h, latent_w = height // self.vae_scale_factor, width // self.vae_scale_factor
         if generator is None:
             generator = torch.Generator().manual_seed(self.seed)
         cuda = self.device.type == 'cuda'
-        emb_h = self.encode(prompts, generator).to(self.dtype)
+        if prompt_embeds is not None:
+            cond = prompt_embeds.detach().float().cpu()
+            uncond = torch.zeros_like(cond) if negative_prompt_embeds is None \
+                else negative_prompt_embeds.detach().float().cpu()
+            emb_h = torch.cat([uncond, cond]).to(self.dtype)
+        else:
+            emb_h = self.encode(prompts, generator).to(self.dtype)
         if num_images_per_prompt != 1:                        # [2, N, ...] -> [2, N * n, ...], each prompt n times
             emb_h = emb_h.view(2, len(prompts), *emb_h.shape[1:]).repeat_interleave(num_images_per_prompt, dim=1) \
                 .reshape(-1, *emb_h.shape[1:])
@@ -512,7 +533,7 @@ class SyntheticPipeline:
             emb_h, lat_h, t_h, out_h = emb_h.pin_memory(), lat_h.pin_memory(), t_h.pin_memory(), out_h.pin_memory()
         self.h2d_bytes_per_step = emb_h.numel() * emb_h.element_size() + lat_h.numel() * lat_h.element_size() + 4
         self.d2h_bytes_per_step = n * 4
-        st = self._state(n, latent_h, latent_w)
+        st = self._state(n, latent_h, latent_w, emb_h.shape[1])
         for i in range(num_inference_steps):
             st['emb'].copy_(emb_h, non_blocking=True)            # H2D: the step's inputs
             st['lat0'].copy_(lat_h, non_blocking=True)

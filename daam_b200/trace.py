@@ -43,7 +43,7 @@ from . import _native, ops
 from .geometry import LatentGeometry
 from .heatmap import GlobalHeatMap, ImageHeatMaps, LayerSlab, RawHeatMapCollection, TimeHeatMaps
 from .hook import AggregateHooker, ObjectHooker, UNetCrossAttentionLocator
-from .utils import cache_dir
+from .utils import cache_dir, context_rows
 
 __all__ = ['trace', 'DiffusionHeatMapHooker', 'GlobalHeatMap', 'UNetCrossAttentionHooker', 'PipelineHooker',
            'ImageProcessorHooker']
@@ -59,16 +59,25 @@ class DiffusionHeatMapHooker(AggregateHooker):
     ``(start, stop)`` tuples or ``range`` objects over UNet-forward indices of a generation, counted as
     :class:`TimeHeatMaps` counts them: also keep the per-key sums over each of those spans; read them with
     ``step_range=i`` in :meth:`compute_global_heat_map`, :meth:`compute_per_head_heat_maps` and
-    ``all_heat_maps.items``) and ``negative`` (also keep the maps of the unconditional half of the guidance batch, the
-    negative prompt's; read them with ``negative=True`` in every read).
+    ``all_heat_maps.items``), ``negative`` (also keep the maps of the unconditional half of the guidance batch, the
+    negative prompt's; read them with ``negative=True`` in every read) and ``long_prompts`` (also trace contexts of 154
+    and 231 tokens, two or three CLIP chunks such as chunked ``prompt_embeds`` give: every context row is accumulated,
+    and every read returns the compact ``n_tokens + 2`` rows that :func:`~daam_b200.utils.context_rows` names; any
+    other context length raises at the layer call; not with ``time_resolved``, ``step_ranges``, ``save_heads`` or
+    ``load_heads``).
     """
 
     def __init__(self, pipeline, low_memory: bool = False, load_heads: bool = False, save_heads: bool = False,
                  data_dir: str = None, *, launch: str = 'step', batch_prompts: bool = False,
                  locate_middle_block: bool = False, kernel_flags: int = _native.ACC_AUTO, time_resolved: bool = False,
-                 step_ranges=None, negative: bool = False):
+                 step_ranges=None, negative: bool = False, long_prompts: bool = False):
         if launch not in ('step', 'overlap', 'layer'):
             raise ValueError("launch must be 'step', 'overlap' or 'layer'")
+        if long_prompts:
+            for name, on in (('time_resolved=True', time_resolved), ('step_ranges', step_ranges is not None),
+                             ('save_heads', save_heads), ('load_heads', load_heads)):
+                if on:
+                    raise ValueError(f'long_prompts=True does not support {name}: it traces 77-token contexts only')
         modes = []                             # the enabled second-slab modes, and why each needs the step launch
         if step_ranges is not None:
             step_ranges = _normalize_step_ranges(step_ranges)
@@ -97,6 +106,7 @@ class DiffusionHeatMapHooker(AggregateHooker):
         self.last_negative_prompts: List[str] = []   # negative=True: the negative text of every prompt ('' for none)
         self.negative = negative
         self.all_heat_maps.negative = negative
+        self.long_prompts = long_prompts
         self.last_image = None
         self.last_images: list = []   # every image of the last generation, prompt-major (``out.images[p * n + i]``)
         self.time_idx = 0
@@ -272,7 +282,8 @@ class DiffusionHeatMapHooker(AggregateHooker):
         # "second half of the batch*heads axis" (trace.py:240): the conditional samples of a CFG batch
         _, n_samples, head0, n_heads = ops.cond_half(bsz, heads)
         n_real, images = self._prompt_layout(layer_idx, n_samples)
-        slab = self.all_heat_maps.slab_for(layer_idx, factor, n_real, images * n_heads, h, w, q.device, head0, images)
+        slab = self.all_heat_maps.slab_for(layer_idx, factor, n_real, images * n_heads, h, w, q.device, head0, images,
+                                           k.shape[1])
         self._epoch_seen = self.all_heat_maps.epoch        # (this call may have bumped it; the other layers' slabs stand)
         if self.negative:                                  # one descriptor over the whole batch, into the whole slab
             desc = ops.make_layer_desc(q, k, slab.storage.view(bsz, n_heads, slab.acc.shape[2], hw), heads, scale,
@@ -510,34 +521,38 @@ class DiffusionHeatMapHooker(AggregateHooker):
         image's keys, and ``head_idx`` indexes images x heads. ``image_idx=i`` keeps image ``i``'s keys only (``head_idx``
         then counts that image's heads); an un-guided batch has only the kept images (see ``ops.cond_half``).
         """
-        prompt, grid, n_rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range, layer_idx,
-                                                                head_idx, negative, image_idx)
+        prompt, grid, rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range, layer_idx,
+                                                              head_idx, negative, image_idx)
         device = slabs[0].acc.device
-        maps = torch.empty((n_rows,) + grid, dtype=torch.float32, device=device)
+        n_fin = _finalized_rows(rows)
+        maps = torch.empty((n_fin,) + grid, dtype=torch.float32, device=device)
         with torch.cuda.device(device):
-            _native.finalize(groups, grid, n_rows, normalize, maps.data_ptr(),
+            _native.finalize(groups, grid, n_fin, normalize and n_fin == len(rows), maps.data_ptr(),
                              torch.cuda.current_stream(device).cuda_stream)
-        return GlobalHeatMap(self.pipe.tokenizer, prompt, maps)
+        return GlobalHeatMap(self.pipe.tokenizer, prompt, _compact(maps, rows, normalize))
 
     def compute_image_heat_maps(self, prompt_idx: int = 0, factors=None, layer_idx=None, head_idx=None,
                                 normalize: bool = False, *, step_range: Optional[int] = None,
-                                negative: bool = False) -> ImageHeatMaps:
+                                negative: bool = False, prompt: Optional[str] = None) -> ImageHeatMaps:
         """Every image's map of prompt ``prompt_idx`` in one launch (``daam_finalize_maps``): ``heat_maps[i]`` is
         ``compute_global_heat_map(image_idx=i, ...)`` with the same arguments, bit for bit (``head_idx`` counts one
-        image's heads). Returns an :class:`ImageHeatMaps` ``[images, n_rows, xh, xw]``."""
-        prompt, grid, n_rows, _, slabs = self._read_groups(None, factors, prompt_idx, step_range, layer_idx, head_idx,
-                                                           negative, 0)
+        image's heads). ``prompt``: the text, when it is not the generation's (e.g. one driven by ``prompt_embeds``).
+        Returns an :class:`ImageHeatMaps` ``[images, n_rows, xh, xw]``."""
+        prompt, grid, rows, _, slabs = self._read_groups(prompt, factors, prompt_idx, step_range, layer_idx, head_idx,
+                                                         negative, 0)
         images, n_prompts = slabs[0].images, slabs[0].n_prompts
         if not 0 <= prompt_idx < n_prompts:
             raise IndexError(f'prompt_idx {prompt_idx} is out of range for {n_prompts} prompt(s)')
         groups = [_block_group(s.source(step_range, negative), s, -1 if head_idx is None else head_idx) for s in slabs]
         device = slabs[0].acc.device
-        out = torch.empty((images, n_rows) + grid, dtype=torch.float32, device=device)
-        maps = [_native.DaamMapSel(block_begin=prompt_idx * images + i, block_count=1, n_rows=n_rows,
+        n_fin = _finalized_rows(rows)
+        out = torch.empty((images, n_fin) + grid, dtype=torch.float32, device=device)
+        maps = [_native.DaamMapSel(block_begin=prompt_idx * images + i, block_count=1, n_rows=n_fin,
                                    out=out[i].data_ptr()) for i in range(images)]
         with torch.cuda.device(device):
-            _native.finalize_maps(groups, maps, grid, normalize, torch.cuda.current_stream(device).cuda_stream)
-        return ImageHeatMaps(self.pipe.tokenizer, prompt, out)
+            _native.finalize_maps(groups, maps, grid, normalize and n_fin == len(rows),
+                                  torch.cuda.current_stream(device).cuda_stream)
+        return ImageHeatMaps(self.pipe.tokenizer, prompt, _compact(out, rows, normalize))
 
     def compute_time_heat_maps(self, prompt_idx: int = 0, normalize: bool = False, *,
                                negative: bool = False, image_idx: Optional[int] = None) -> TimeHeatMaps:
@@ -582,23 +597,26 @@ class DiffusionHeatMapHooker(AggregateHooker):
         ``maps[i]`` the ``[n_tokens + 2, xh, xw]`` heat map the reference computes for that single key. ``step_range=i``
         and ``negative=True`` select the slabs as in :meth:`compute_global_heat_map`; ``image_idx=i`` keeps image
         ``i``'s keys, whose ``head`` then counts that image's heads."""
-        prompt, grid, n_rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range,
-                                                                negative=negative, image_idx=image_idx)
+        prompt, grid, rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range,
+                                                              negative=negative, image_idx=image_idx)
         keys = [(slab.factor, slab.layer_idx, head) for slab, g in zip(slabs, groups) for head in range(g.heads)]
         device = slabs[0].acc.device
-        maps = torch.empty((len(keys), n_rows) + grid, dtype=torch.float32, device=device)
+        n_fin = _finalized_rows(rows)
+        maps = torch.empty((len(keys), n_fin) + grid, dtype=torch.float32, device=device)
         with torch.cuda.device(device):
-            _native.finalize_per_key(groups, grid, n_rows, normalize, maps.data_ptr(),
+            _native.finalize_per_key(groups, grid, n_fin, normalize and n_fin == len(rows), maps.data_ptr(),
                                      torch.cuda.current_stream(device).cuda_stream)
-        return keys, maps
+        return keys, _compact(maps, rows, normalize)
 
     def _read_groups(self, prompt, factors, prompt_idx: int, step_range: Optional[int], layer_idx=None, head_idx=None,
                      negative: bool = False, image_idx: Optional[int] = None):
         """What the heat-map reads share: the prompt (default: the generation's, or with ``negative`` its negative
-        text), the map grid ``(xh, xw)``, the row count, and the key groups of prompt ``prompt_idx`` over the live slabs
-        (with ``step_range``: over that range's slabs; with ``negative``: their unconditional halves) that pass the
-        filters, with the slabs behind them; with ``image_idx`` the groups hold image ``image_idx``'s heads only, and
-        ``head_idx`` counts those. Raises when no slab passes, and ``IndexError`` for a bad ``image_idx``."""
+        text), the map grid ``(xh, xw)``, the context rows the map reads (``utils.context_rows``: ``[0, n_tokens + 2)``
+        for a 77-token context), and the key groups of prompt ``prompt_idx`` over the live slabs (with ``step_range``:
+        over that range's slabs; with ``negative``: their unconditional halves) that pass the filters, with the slabs
+        behind them; with ``image_idx`` the groups hold image ``image_idx``'s heads only, and ``head_idx`` counts those.
+        Raises when no slab passes, ``IndexError`` for a bad ``image_idx`` and ``ValueError`` when the generation was
+        driven by embeddings and no ``prompt`` text is given."""
         if negative:
             self.all_heat_maps.check_negative()
         if prompt is None:
@@ -606,6 +624,9 @@ class DiffusionHeatMapHooker(AggregateHooker):
                 prompt = self.last_negative_prompts[prompt_idx] if self.last_negative_prompts else ''
             else:
                 prompt = self.last_prompts[prompt_idx] if self.last_prompts else self.last_prompt
+            if prompt is None:
+                raise ValueError(f'the generation was driven by {"negative_" if negative else ""}prompt_embeds, so '
+                                 f'its text is unknown: pass the text it encodes as prompt=...')
         factors = {0, 1, 2, 4, 8, 16, 32, 64} if factors is None else set(factors)
         read = self.all_heat_maps.read_slabs(step_range, negative)
         if image_idx is not None and read:
@@ -633,7 +654,36 @@ class DiffusionHeatMapHooker(AggregateHooker):
             if head_idx is not None or layer_idx is not None:
                 raise RuntimeError('No heat maps found for the given parameters.')
             raise RuntimeError('No heat maps found. Did you forget to call `with trace(...)` during generation?')
-        return prompt, self.geometry.grid, self._n_rows(prompt), groups, slabs
+        tokens = {s.tokens for s in slabs}
+        if len(tokens) > 1:
+            raise RuntimeError(f'the traced layers hold contexts of {sorted(tokens)} tokens: one read reduces one '
+                               f'context length')
+        return prompt, self.geometry.grid, context_rows(len(self.pipe.tokenizer.tokenize(prompt)), tokens.pop()), \
+            groups, slabs
+
+
+def _finalized_rows(rows: List[int]) -> int:
+    """The leading context rows a read finalizes: through its EOS row, ``rows[-1]``. For a 77-token context that is
+    ``len(rows)``, the reference's truncation, and the finalize kernels return the map itself."""
+    return rows[-1] + 1
+
+
+def _compact(maps: torch.Tensor, rows: List[int], normalize: bool) -> torch.Tensor:
+    """The compact map of a long context from the finalized prefix ``maps`` ``[..., rows[-1] + 1, xh, xw]``: its
+    ``rows`` gathered on the device in order (SOS, every prompt token, EOS), then with ``normalize`` divided by the sum
+    of compact rows ``1 .. n`` plus 1e-6 (``daam_normalize_maps``: the reference's ``rows[1:-1]`` rule on the compact
+    map). When the rows are the prefix itself (every 77-token read, and a long context whose prompt fits its first
+    chunk) the finalize call has normalised already and ``maps`` is returned as it is."""
+    if maps.shape[-3] == len(rows):
+        return maps
+    index = torch.tensor(rows, dtype=torch.long).to(maps.device)
+    out = maps.index_select(maps.dim() - 3, index)
+    if normalize:
+        grid = tuple(out.shape[-2:])
+        with torch.cuda.device(out.device):
+            _native.normalize_maps(out.data_ptr(), out.numel() // (len(rows) * grid[0] * grid[1]), len(rows), grid,
+                                   torch.cuda.current_stream(out.device).cuda_stream)
+    return out
 
 
 def _key_group(acc: torch.Tensor, slab: LayerSlab, head_sel: int = -1) -> _native.DaamKeyGroup:
@@ -736,9 +786,18 @@ class PipelineHooker(ObjectHooker):
         hk_self.parent_trace.last_images = list(images)      # prompt-major, as the pipeline returns them
         return image, has_nsfw
 
-    def _hooked_check_inputs(hk_self, _, prompt: Union[str, List[str]], *args, **kwargs):
+    def _hooked_check_inputs(hk_self, _, prompt: Union[str, List[str], None], *args, **kwargs):
         tr = hk_self.parent_trace
-        if isinstance(prompt, str):
+        if prompt is None:
+            # a generation driven by prompt_embeds (e.g. chunked long-prompt embeddings): the prompt count comes from
+            # them, and no text is recorded (a read then needs prompt=...)
+            prompts = [None] * hk_self._embeds_count(prompt, args, kwargs)
+            if len(prompts) > 1 and not tr.batch_prompts:
+                raise ValueError('Only single prompt generation is supported for heat map computation.')
+            if tr.time_resolved:
+                raise ValueError('time_resolved=True needs the prompt text (the per-step heat map has one row per '
+                                 'token): a generation driven by prompt_embeds alone cannot be traced with it')
+        elif isinstance(prompt, str):
             prompts = [prompt]
         else:
             prompts = list(prompt)
@@ -753,6 +812,13 @@ class PipelineHooker(ObjectHooker):
         tr.last_prompts = prompts
         tr.last_negative_prompts = negatives
         return hk_self.monkey_super('check_inputs', prompt, *args, **kwargs)
+
+    def _embeds_count(hk_self, prompt, args, kwargs) -> int:
+        """The number of prompts of a ``check_inputs`` call without text: the batch of its ``prompt_embeds`` argument
+        ``[N, T, C]``, bound by name like ``negative_prompt`` (1 when absent)."""
+        bound = inspect.signature(hk_self._replaced['check_inputs']).bind(prompt, *args, **kwargs)
+        embeds = bound.arguments.get('prompt_embeds', kwargs.get('prompt_embeds'))
+        return int(embeds.shape[0]) if embeds is not None else 1
 
     def _negative_prompts(hk_self, prompt, args, kwargs, n: int) -> List[str]:
         """The negative text of each of the ``n`` prompts, from the ``negative_prompt`` argument of the
@@ -842,8 +908,17 @@ class UNetCrossAttentionHooker(ObjectHooker):
         geom = self._geom                                    # (n, tokens) -> factor and the trace / skip decision
         if geom is None or geom[0] != n or geom[1] != tokens:
             # trace.py:285-289; the tracer's geometry gives the factor (and drops this cache when the latent changes)
-            factor = tr.geometry.level(n, self.layer_idx)[2] if tokens == self.context_size else None
-            geom = self._geom = (n, tokens, factor, tokens == self.context_size and factor != 8)
+            traced = tokens == self.context_size
+            if tr.long_prompts and not traced:
+                if tokens not in _native.CONTEXT_TOKENS:
+                    raise ValueError(f'layer {self.layer_idx}: a context of {tokens} tokens cannot be traced; '
+                                     f'long_prompts=True traces {", ".join(map(str, _native.CONTEXT_TOKENS))} tokens '
+                                     f'(1-3 CLIP chunks of 77)')
+                traced = True
+            if geom is not None and geom[1] != tokens:     # another context length: re-derive the layer's slab
+                tr._layer_state.pop(self.layer_idx, None)
+            factor = tr.geometry.level(n, self.layer_idx)[2] if traced else None
+            geom = self._geom = (n, tokens, factor, traced and factor != 8)
         tr._gen_idx += 1
         if geom[3]:                                          # skip if too large (trace.py:289)
             tr._enqueue(self.layer_idx, geom[2], query, key, heads, attn.scale)

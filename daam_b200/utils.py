@@ -12,7 +12,7 @@ from typing import List, Optional, Tuple, TypeVar
 import numpy as np
 import torch
 
-__all__ = ['set_seed', 'compute_token_merge_indices', 'cache_dir', 'auto_device', 'auto_autocast']
+__all__ = ['set_seed', 'compute_token_merge_indices', 'cache_dir', 'auto_device', 'auto_autocast', 'context_rows']
 
 T = TypeVar('T')
 
@@ -51,6 +51,26 @@ def cache_dir() -> Path:
     if os.name == 'posix':
         return Path(os.environ.get('XDG_CACHE_HOME', os.path.expanduser('~/.cache')), 'daam')
     return Path(os.environ.get('LOCALAPPDATA') or os.path.expanduser('~\\AppData\\Local'), 'daam')
+
+
+CHUNK_TOKENS = 77          # one CLIP window: BOS, 75 prompt tokens, EOS
+CHUNK_PROMPT_TOKENS = 75
+
+
+def context_rows(n_tokens: int, tokens: int = CHUNK_TOKENS) -> List[int]:
+    """The context rows a heat map of a ``n_tokens``-token prompt reads from a ``tokens``-row context (77, 154 or 231:
+    one to three CLIP chunks), in the order of its rows: the SOS row 0, the row of every prompt token, the EOS row.
+
+    A context of ``c`` chunks is ``c x 77`` rows, chunk ``i`` being BOS, prompt tokens ``75i .. 75i + 74``, EOS, padding
+    (the layout of compel and of the long-prompt-weighting pipelines). Prompt token ``j`` sits at row
+    ``77 (j // 75) + 1 + j % 75`` and the EOS row follows the last token. ``n_tokens`` is capped at ``75 c``; for one
+    chunk the rows are ``[0, n_tokens + 2)``, the reference's truncation to 77."""
+    chunks = tokens // CHUNK_TOKENS
+    if tokens not in (CHUNK_TOKENS, 2 * CHUNK_TOKENS, 3 * CHUNK_TOKENS):
+        raise ValueError(f'a context of {tokens} tokens is not 1-3 chunks of {CHUNK_TOKENS}')
+    n = max(0, min(int(n_tokens), CHUNK_PROMPT_TOKENS * chunks))
+    rows = [CHUNK_TOKENS * (j // CHUNK_PROMPT_TOKENS) + 1 + j % CHUNK_PROMPT_TOKENS for j in range(n)]
+    return [0] + rows + [rows[-1] + 1 if rows else 1]
 
 
 def _pieces(tokenizer, text: str) -> List[str]:

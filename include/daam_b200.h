@@ -31,14 +31,16 @@ extern "C" {
                                        4: the finalize family takes (map_h, map_w); the _rect names are gone
                                           (later, additive: layers with hw not a multiple of 4 are accepted;
                                           daam_segment_words, daam_finalize_maps; daam_key_group.reserved is
-                                          n_blocks) */
+                                          n_blocks; daam_accumulate takes 154- and 231-token contexts) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
+#define DAAM_MAX_TOKENS 231     /* daam_accumulate: long contexts of 2 or 3 CLIP chunks of 77 tokens (154, 231) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
 
 enum daam_status {
   DAAM_OK = 0,
   DAAM_E_INVALID = -1,          /* bad argument (shape, alignment, null pointer) */
-  DAAM_E_UNSUPPORTED = -2,      /* tokens != 77, head_dim not a multiple of 8 or > DAAM_MAX_HEAD_DIM, ... */
+  DAAM_E_UNSUPPORTED = -2,      /* tokens not 77 / 154 / 231 (77 only outside daam_accumulate), head_dim not a
+                                   multiple of 8 or > DAAM_MAX_HEAD_DIM, ... */
   DAAM_E_CUDA = -3              /* a CUDA runtime call failed (including: no device) */
 };
 
@@ -81,6 +83,12 @@ enum daam_dtype { DAAM_F32 = 0, DAAM_F16 = 1, DAAM_BF16 = 2 };
  * `acc` is fp32, contiguous [n_prompts][heads][tokens][hw]: acc[p][head] is exactly the reference's per-key
  * [77, h, w] heat map for key (factor, layer, head). n_prompts > 1 is the batched mode (independent single-prompt
  * traces run in one launch); the reference itself is single-prompt (trace.py:172-173).
+ *
+ * Long contexts (daam_accumulate only): tokens may be 77, 154 or 231 (one to three CLIP chunks of 77 tokens, e.g.
+ * chunked prompt embeddings); the softmax runs over all `tokens` columns and every row is accumulated. Any other count
+ * is DAAM_E_UNSUPPORTED. 16-bit layers the wgmma path takes run its long-context instances; fp32 layers and the rest
+ * run a two-pass SIMT kernel. A long-context layer never shares a launch with a layer of another context length.
+ * daam_accumulate_steps, daam_accumulate_range, daam_attention_probs and daam_accumulate_probs take 77 tokens only.
  */
 typedef struct daam_layer {
   const void* q;             /* device; element (prompt 0, pixel 0, head 0, dim 0) of the CONDITIONAL half */
