@@ -795,6 +795,7 @@ int make_qk_map(const void* ptr, int dtype, int head_dim, int heads, int rows, i
   if (!enc) { set_error("cuTensorMapEncodeTiled is not available from this driver"); return DAAM_E_CUDA; }
   const cuuint64_t es = dtype == DAAM_F32 ? 4 : 2;
   const cuuint64_t dims[4] = {(cuuint64_t)head_dim, (cuuint64_t)heads, (cuuint64_t)rows, (cuuint64_t)prompts};
+  // (a stride <= 0 only reaches here for an axis of extent 1, which the map never steps along: mma_supported)
   auto bytes = [es](long long s) { return (cuuint64_t)(s > 0 ? s : 8) * es; };
   const cuuint64_t strides[3] = {bytes(s_head), bytes(s_row), bytes(s_prompt)};
   const cuuint32_t box[4] = {(cuuint32_t)(128 / es), 1, (cuuint32_t)box_rows, 1};
@@ -878,9 +879,13 @@ void prepared_mma_delete(void* p) { delete static_cast<PreparedMma*>(p); }
 // hw % 4 == 0: the accumulator / second-slab tensor maps (make_acc_map) need a row pitch of hw * 4 bytes that is a
 // multiple of 16, and the split form's load / add / store epilogue moves float4 columns. Other layers (odd-sized keys
 // such as 19 x 25) take the SIMT kernel, which updates the accumulator one element at a time.
+// Strides: a tensor map takes positive byte strides only, so every stride make_qk_map encodes must be positive. The
+// prompt stride is one of them once there are two or more prompts: a zero stride (a sample broadcast with expand()) or
+// a negative one (samples stored in reverse) takes the SIMT kernel, which indexes any int64 stride.
 bool mma_supported(const LayerParams& L) {
+  const bool prompts_ok = L.n_prompts == 1 || (L.qs_prompt > 0 && L.ks_prompt > 0);
   return L.head_dim % 8 == 0 && L.head_dim <= DAAM_MAX_HEAD_DIM && L.vec_ok && L.qs_head > 0 && L.qs_pixel > 0 &&
-         L.ks_head > 0 && L.ks_token > 0 && L.hw % 4 == 0;
+         L.ks_head > 0 && L.ks_token > 0 && prompts_ok && L.hw % 4 == 0;
 }
 
 // Tensor maps, grid and kernel variant of one pack of layers (all fp32, or all 16-bit). `out`: prepared_mma_new().

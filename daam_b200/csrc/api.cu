@@ -215,7 +215,8 @@ int build_plan(const daam_layer* layers, float* const* slabs, SlabMode mode, int
                          (ctx_chunks == 1 || L.dtype != DAAM_F32);
     if (path == DAAM_ACC_FORCE_MMA && !use_mma) {
       set_error("daam_accumulate: layer %d cannot take the wgmma path (dtype %d, head_dim %d, alignment %d, hw = %d, "
-                "tokens = %d, sm_%d%d)", i, L.dtype, L.head_dim, L.vec_ok, L.hw, L.tokens, dev.cc_major, dev.cc_minor);
+                "tokens = %d, %d prompts with prompt strides q %lld / k %lld, sm_%d%d)", i, L.dtype, L.head_dim,
+                L.vec_ok, L.hw, L.tokens, L.n_prompts, L.qs_prompt, L.ks_prompt, dev.cc_major, dev.cc_minor);
       return DAAM_E_UNSUPPORTED;
     }
     const int which = ctx_chunks > 1 ? (use_mma ? 1 : 3) + ctx_chunks : use_mma ? (L.dtype == DAAM_F32 ? 1 : 0) : 2;

@@ -31,7 +31,8 @@ extern "C" {
                                        4: the finalize family takes (map_h, map_w); the _rect names are gone
                                           (later, additive: layers with hw not a multiple of 4 are accepted;
                                           daam_segment_words, daam_finalize_maps; daam_key_group.reserved is
-                                          n_blocks; daam_accumulate takes 154- and 231-token contexts) */
+                                          n_blocks; daam_accumulate takes 154- and 231-token contexts; layers with
+                                          several prompts and a prompt stride <= 0 take the SIMT kernel) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_TOKENS 231     /* daam_accumulate: long contexts of 2 or 3 CLIP chunks of 77 tokens (154, 231) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
@@ -47,8 +48,9 @@ enum daam_status {
 enum daam_dtype { DAAM_F32 = 0, DAAM_F16 = 1, DAAM_BF16 = 2 };
 
 /* daam_accumulate flags */
-#define DAAM_ACC_AUTO        0u  /* wgmma path whenever rows are 16-byte aligned (any dtype, head_dim % 8 == 0) and
-                                    hw % 4 == 0, SIMT fp32 path otherwise */
+#define DAAM_ACC_AUTO        0u  /* wgmma path whenever rows are 16-byte aligned (any dtype, head_dim % 8 == 0),
+                                    hw % 4 == 0, the head and pixel / token strides are positive and, with
+                                    n_prompts > 1, so are both prompt strides; SIMT fp32 path otherwise */
 #define DAAM_ACC_FORCE_SIMT  1u  /* always the SIMT fp32 ("warp dot") kernel */
 #define DAAM_ACC_FORCE_MMA   2u  /* wgmma kernel or DAAM_E_UNSUPPORTED */
 /* Accumulator update of the SIMT kernel and of the wgmma kernel's fp32 form. The wgmma kernel's 16-bit (fp16 / bf16)
@@ -95,7 +97,15 @@ typedef struct daam_layer {
   const void* k;             /* device; element (prompt 0, token 0, head 0, dim 0) of the conditional half */
   float* acc;                /* device; fp32 [n_prompts][heads][tokens][hw], 16-byte aligned */
   int64_t q_stride_prompt, q_stride_pixel, q_stride_head;   /* in elements; the head_dim axis is contiguous */
-  int64_t k_stride_prompt, k_stride_token, k_stride_head;
+  int64_t k_stride_prompt, k_stride_token, k_stride_head;   /* Any int64 value, in any order: head-major
+                                                               ([B, H, N, d]), padded heads, fused projections
+                                                               (qkv / kv buffers), padding between samples. A zero
+                                                               prompt stride repeats sample 0 (expand()), a negative
+                                                               one walks back from it; with n_prompts > 1 such a
+                                                               layer takes the SIMT kernel (DAAM_ACC_AUTO) and
+                                                               DAAM_ACC_FORCE_MMA refuses it (DAAM_E_UNSUPPORTED).
+                                                               The wgmma path needs every other stride positive and
+                                                               a multiple of 16 bytes. */
   int32_t n_prompts, heads, hw, tokens, head_dim;   /* hw: any positive pixel count; the wgmma path needs hw % 4 == 0
                                                        (DAAM_ACC_AUTO sends other layers to the SIMT kernel) */
   int32_t dtype;             /* enum daam_dtype of q and k */
