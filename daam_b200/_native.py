@@ -30,9 +30,17 @@ def segment_scratch_floats(n_maps: int, n_words: int) -> int:
     """``DAAM_SEGMENT_SCRATCH_FLOATS(n_maps, n_words)``."""
     return 64 * n_maps * n_words
 
+MAX_REGIONS = 63             # DAAM_REGION_MAX_REGIONS: regions per daam_region_overlap call
+
+
+def region_scratch_floats(n_maps: int, n_words: int, n_regions: int, out_h: int, out_w: int) -> int:
+    """``DAAM_REGION_SCRATCH_FLOATS(n_maps, n_words, n_regions, out_h, out_w)``."""
+    return n_maps * n_words * (64 + (n_regions + 1) * ((out_h + 15) // 16) * ((out_w + 63) // 64))
+
+
 EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize',
            'daam_finalize_maps', 'daam_finalize_per_key','daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
-           'daam_segment_words',
+           'daam_segment_words', 'daam_region_overlap',
            'daam_side_launcher_create', 'daam_side_launcher_destroy',
            'daam_side_launcher_launch', 'daam_side_launcher_join', 'daam_side_launcher_idle', 'daam_abi_version',
            'daam_last_error', 'daam_device_info', 'daam_launch_count')
@@ -125,6 +133,9 @@ def load() -> ctypes.CDLL:
     lib.daam_segment_words.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
                                        i32, i32, f32, vp, vp, vp, vp, vp]
     lib.daam_segment_words.restype = ctypes.c_int
+    lib.daam_region_overlap.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
+                                        i32, i32, f32, vp, vp, i32, vp, vp, vp, vp]
+    lib.daam_region_overlap.restype = ctypes.c_int
     lib.daam_side_launcher_create.argtypes = [ctypes.POINTER(vp)]
     lib.daam_side_launcher_create.restype = ctypes.c_int
     lib.daam_side_launcher_destroy.argtypes = [vp]
@@ -345,6 +356,22 @@ def segment_words(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Seq
                                      float(threshold) if use_thr else 0.0, ctypes.c_void_p(word_maps_ptr),
                                      ctypes.c_void_p(labels_ptr), ctypes.c_void_p(scores_ptr),
                                      ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
+
+
+def region_overlap(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int,
+                   out_w: int, absolute: bool, threshold: Optional[float], word_maps_ptr: int, regions_ptr: int,
+                   n_regions: int, intersection_ptr: int, word_area_ptr: int, scratch_ptr: int, stream: int):
+    """``daam_region_overlap`` over ``n_maps`` maps ``[n_rows, h, w]`` back to back and ``n_regions`` uint8 regions
+    ``[out_h, out_w]``; ``rows_per_word`` as for :func:`expand_words`."""
+    h, w = map_size(x)
+    rows_arr, begin_arr = _row_lists(rows_per_word)
+    use_thr = bool(threshold)   # the reference's `if threshold:` (daam/heatmap.py:87), as expand_words resolves it
+    _check(load().daam_region_overlap(ctypes.c_void_p(maps_ptr), n_maps, n_rows, h, w, rows_arr, begin_arr,
+                                      len(rows_per_word), out_h, out_w, int(bool(absolute)), int(use_thr),
+                                      float(threshold) if use_thr else 0.0, ctypes.c_void_p(word_maps_ptr),
+                                      ctypes.c_void_p(regions_ptr), n_regions, ctypes.c_void_p(intersection_ptr),
+                                      ctypes.c_void_p(word_area_ptr), ctypes.c_void_p(scratch_ptr),
+                                      ctypes.c_void_p(stream)))
 
 
 def device_info():

@@ -707,6 +707,192 @@ __global__ void __launch_bounds__(256) segment_label_kernel(const __grid_constan
   }
 }
 
+// ---- word-region overlap: sums of a word list's expanded maps over binary image regions -------------------------
+// With m[w] what expand_words_kernel writes for word w (0/1 when use_threshold) and R[r] = (regions[r] != 0):
+//   intersection[map][r][w] = sum_p R[r](p) m[w](p),   word_area[map][w] = sum_p m[w](p)
+// in three launches whatever n_maps, n_words and n_regions:
+//  1. segment_minmax_kernel (unchanged): word maps and per-chunk min / max partials;
+//  2. region_tile_kernel, CTA = (16 x 64 output tile, map): stages the source windows of a pass of words as
+//     segment_label_kernel does, computes m[w] per pixel with the same taps, bicubic_shared, minmax_normalize and
+//     threshold compare as expand_words_kernel, and reduces every (word, slot) over the tile in a fixed order -- slot 0
+//     is the word's area, slot 1 + r its sum inside region r -- into one partial per tile;
+//  3. region_reduce_kernel: one warp per (map, word, slot) sums the tiles' partials in a fixed order.
+// The [n_words][out_h][out_w] stack is never written; no atomics, so the sums are the same bits on every call. With a
+// threshold every value is 0 or 1 and every partial an integer below 2^24, so the sums are exact counts.
+constexpr int kMaxRegions = DAAM_REGION_MAX_REGIONS;   // 63 + the area slot: 64 slots per word, two groups of 32
+constexpr int kRegionSlots = kMaxRegions + 1;
+
+struct RegionParams {
+  SegmentParams s;                      // maps, word_maps, scratch (min / max partials), sizes, rows, words_per_pass
+  const unsigned char* regions;         // [n_regions][oh][ow]
+  float* partials;                      // [n_maps][n_words][n_regions + 1][tiles]
+  int n_regions, tiles;
+};
+
+// Lane l returns the warp's sum of s[l]. Five halving exchange rounds (31 shuffles for 32 values); the order of every
+// add is fixed.
+// One round: lanes with bit H set keep s[H .. 2H), the others s[0 .. H); each sends the other half to lane ^ H. The
+// round count is a template argument so that every index is a constant and s[] stays in registers.
+template <int H>
+__device__ __forceinline__ void reduce_scatter_round(float (&s)[32], int lane) {
+  const bool upper = (lane & H) != 0;
+#pragma unroll
+  for (int i = 0; i < H; ++i) {
+    const float send = upper ? s[i] : s[i + H];
+    const float keep = upper ? s[i + H] : s[i];
+    s[i] = keep + __shfl_xor_sync(0xffffffffu, send, H);
+  }
+}
+
+__device__ __forceinline__ float warp_reduce_scatter32(float (&s)[32]) {
+  const int lane = threadIdx.x & 31;
+  reduce_scatter_round<16>(s, lane);
+  reduce_scatter_round<8>(s, lane);
+  reduce_scatter_round<4>(s, lane);
+  reduce_scatter_round<2>(s, lane);
+  reduce_scatter_round<1>(s, lane);
+  return s[0];
+}
+
+// grid: (tiles of kSegTileH x kSegTileW output pixels, n_maps); dynamic smem: words_per_pass source windows
+__global__ void __launch_bounds__(256) region_tile_kernel(const __grid_constant__ RegionParams R) {
+  extern __shared__ __align__(16) float win[];
+  __shared__ float s_lo[kMaxWords], s_hi[kMaxWords];
+  __shared__ float red[2][8][kRegionSlots];          // per-warp sums of a word, double-buffered across words
+  __shared__ int tyi[4][kSegTileH], txi[4][kSegTileW];   // the tile's taps, relative to the staged window
+  __shared__ float tyw[4][kSegTileH], txw[4][kSegTileW];
+  const SegmentParams& P = R.s;
+  const int map = blockIdx.y, mh = P.mh, mw = P.mw, oh = P.oh, ow = P.ow, n_words = P.n_words;
+  const int tiles_x = (ow + kSegTileW - 1) / kSegTileW;
+  const int y0 = (blockIdx.x / tiles_x) * kSegTileH, x0 = (blockIdx.x % tiles_x) * kSegTileW;
+  const int th = min(kSegTileH, oh - y0), tw = min(kSegTileW, ow - x0);
+  const int wy = make_taps(y0, mh, oh).idx[0], wx = make_taps(x0, mw, ow).idx[0];
+  const int wh = make_taps(y0 + th - 1, mh, oh).idx[3] - wy + 1, ww = make_taps(x0 + tw - 1, mw, ow).idx[3] - wx + 1;
+  const int wn = wh * ww;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int n_slots = R.n_regions + 1;
+  if (!P.absolute) {
+    for (int w = threadIdx.x; w < n_words; w += blockDim.x) {   // chunks in a fixed order
+      const float* slots = P.scratch + 2 * ((long long)map * n_words + w) * P.chunks;
+      float lo = INFINITY, hi = -INFINITY;
+      for (int c = 0; c < P.chunks; ++c) { lo = fminf(lo, slots[2 * c]); hi = fmaxf(hi, slots[2 * c + 1]); }
+      s_lo[w] = lo; s_hi[w] = hi;
+    }
+  }
+  if (threadIdx.x < th) {
+    const Taps t = make_taps(y0 + threadIdx.x, mh, oh);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) { tyi[j][threadIdx.x] = t.idx[j] - wy; tyw[j][threadIdx.x] = t.w[j]; }
+  } else if (threadIdx.x >= kSegTileH && threadIdx.x < kSegTileH + tw) {
+    const int x = threadIdx.x - kSegTileH;
+    const Taps t = make_taps(x0 + x, mw, ow);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) { txi[j][x] = t.idx[j] - wx; txw[j][x] = t.w[j]; }
+  }
+  // slot bits of the thread's pixels: bit j of mask[g][k] says pixel k counts towards slot 32 g + j (slot 0: every
+  // pixel of the tile, slot 1 + r: the pixels inside region r); each region byte is read once
+  const long long n = (long long)oh * ow;
+  unsigned mask[2][kSegPix];
+#pragma unroll
+  for (int k = 0; k < kSegPix; ++k) {
+    const int p = threadIdx.x + 256 * k;
+    mask[0][k] = 0u; mask[1][k] = 0u;
+    if (p < th * tw) {
+      const int py = p / tw;
+      const unsigned char* reg = R.regions + (long long)(y0 + py) * ow + x0 + p - py * tw;
+      unsigned m0 = 1u, m1 = 0u;
+      for (int r = 0; r < R.n_regions; ++r) {
+        const unsigned bit = __ldg(reg + r * n) != 0 ? 1u : 0u;
+        if (r < 31) m0 |= bit << (r + 1); else m1 |= bit << (r - 31);
+      }
+      mask[0][k] = m0; mask[1][k] = m1;
+    }
+  }
+  const float* word_maps = P.word_maps + (long long)map * n_words * mh * mw;
+  float* partials = R.partials + (long long)map * n_words * n_slots * R.tiles + blockIdx.x;
+  for (int w0 = 0; w0 < n_words; w0 += P.words_per_pass) {
+    const int nw = min(P.words_per_pass, n_words - w0);
+    __syncthreads();                                   // the previous pass has read its windows (and the taps are set)
+    for (int i = threadIdx.x; i < nw * wn; i += blockDim.x) {
+      const int wi = i / wn, r = i - wi * wn, y = r / ww, x = r - y * ww;
+      win[i] = __ldg(word_maps + ((long long)(w0 + wi) * mh + wy + y) * mw + wx + x);
+    }
+    __syncthreads();
+    for (int wi = 0; wi < nw; ++wi) {
+      const int w = w0 + wi;
+      float v[kSegPix];
+#pragma unroll
+      for (int k = 0; k < kSegPix; ++k) {
+        const int p = threadIdx.x + 256 * k;
+        v[k] = 0.f;
+        if (p < th * tw) {
+          const int py = p / tw, px = p - py * tw;
+          Taps ty, tx;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            ty.idx[j] = tyi[j][py]; ty.w[j] = tyw[j][py]; tx.idx[j] = txi[j][px]; tx.w[j] = txw[j][px];
+          }
+          float x = bicubic_shared(win + wi * wn, ww, ty, tx);
+          if (!P.absolute) x = minmax_normalize(x, s_lo[w], s_hi[w]);
+          if (P.use_threshold) x = x > P.threshold ? 1.f : 0.f;
+          v[k] = x;
+        }
+      }
+      float (*buf)[kRegionSlots] = red[w & 1];
+#pragma unroll
+      for (int g = 0; g < 2; ++g) {
+        if (g * 32 < n_slots) {
+          float s[32];
+#pragma unroll
+          for (int j = 0; j < 32; ++j) {
+            float a = 0.f;
+#pragma unroll
+            for (int k = 0; k < kSegPix; ++k) a += (mask[g][k] >> j) & 1u ? v[k] : 0.f;
+            s[j] = a;
+          }
+          buf[warp][32 * g + lane] = warp_reduce_scatter32(s);
+        }
+      }
+      // one barrier per word: red[w & 1] is rewritten two words later, after every warp has passed the next barrier
+      __syncthreads();
+      if (warp == (w & 7)) {
+        for (int slot = lane; slot < n_slots; slot += 32) {
+          float a = 0.f;
+#pragma unroll
+          for (int i = 0; i < 8; ++i) a += buf[i][slot];
+          partials[((long long)w * n_slots + slot) * R.tiles] = a;
+        }
+      }
+    }
+  }
+}
+
+// grid: ceil(n_out / 8), 256 threads; one warp per output o = (map * n_words + word) * (n_regions + 1) + slot sums
+// the tiles' partials (lane-strided, then a butterfly) in a fixed order
+__global__ void __launch_bounds__(256) region_reduce_kernel(const float* __restrict__ partials, long long n_out,
+                                                            int tiles, int n_words, int n_regions,
+                                                            float* __restrict__ intersection, float* __restrict__ area) {
+  const long long o = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (o >= n_out) return;                              // whole warps
+  const int lane = threadIdx.x & 31;
+  const float* src = partials + o * tiles;
+  float s = 0.f;
+  for (int t = lane; t < tiles; t += 32) s += __ldg(src + t);
+#pragma unroll
+  for (int h = 16; h > 0; h >>= 1) s += __shfl_xor_sync(0xffffffffu, s, h);
+  if (lane == 0) {
+    const int n_slots = n_regions + 1;
+    const int slot = (int)(o % n_slots);
+    const long long mword = o / n_slots;               // map * n_words + word
+    if (slot == 0) {
+      area[mword] = s;
+    } else {
+      const long long map = mword / n_words, word = mword - map * n_words;
+      intersection[(map * n_regions + slot - 1) * n_words + word] = s;
+    }
+  }
+}
+
 }  // namespace
 }  // namespace daam
 
@@ -1016,22 +1202,20 @@ extern "C" int daam_expand_words(const float* global_maps, int32_t n_rows, int32
                            absolute, use_threshold, threshold, word_maps, out, scratch, stream);
 }
 
-extern "C" int daam_segment_words(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t mh, int32_t mw,
-                                  const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h,
-                                  int32_t out_w, int32_t absolute, int32_t use_threshold, float threshold,
-                                  float* word_maps, uint8_t* labels, float* scores, float* scratch, void* stream_) {
-  const char* name = "daam_segment_words";
-  if (!global_maps || !rows || !row_begin || !word_maps || !labels || !scores || !scratch || n_maps <= 0 || mh <= 0 ||
-      mw <= 0 || out_h <= 0 || out_w <= 0 || n_rows <= 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
+// What daam_segment_words and daam_region_overlap share once their own pointers are checked: the word-list, map and
+// size checks, `p` (all but labels / scores) and the shared memory of both launches (`*smem1`: one word map for
+// segment_minmax_kernel, `*smem2`: words_per_pass staged source windows for the tile kernel). Launches nothing.
+static int segment_prepare(const char* name, const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t mh,
+                           int32_t mw, const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h,
+                           int32_t out_w, int32_t absolute, int32_t use_threshold, float threshold, float* word_maps,
+                           float* scratch, SegmentParams& p, DeviceInfo* dev, size_t* smem1, size_t* smem2) {
   if (n_words <= 0) { set_error("%s: empty word list", name); return DAAM_E_INVALID; }
   if (n_words > kMaxWords) { set_error("%s: %d words > %d", name, n_words, kMaxWords); return DAAM_E_UNSUPPORTED; }
   if (row_begin[0] != 0 || row_begin[n_words] > kMaxWordRows) { set_error("%s: row_begin must start at 0 and select at most %d rows", name, kMaxWordRows); return DAAM_E_UNSUPPORTED; }
   if ((size_t)mh * mw * sizeof(float) > 200 * 1024) { set_error("%s: a %d x %d map does not fit shared memory", name, mh, mw); return DAAM_E_UNSUPPORTED; }
   if (n_maps > 65535) { set_error("%s: %d maps > 65535", name, n_maps); return DAAM_E_UNSUPPORTED; }
   if ((long long)out_h * out_w > (1LL << 30)) { set_error("%s: a %d x %d output is more than 2^30 pixels", name, out_h, out_w); return DAAM_E_UNSUPPORTED; }
-  DeviceInfo dev;
-  if (int rc = get_device_info(&dev)) return rc;
-  static thread_local SegmentParams p;
+  if (int rc = get_device_info(dev)) return rc;
   for (int w = 0; w < n_words; ++w) {
     if (row_begin[w + 1] <= row_begin[w]) { set_error("%s: word %d selects no row", name, w); return DAAM_E_INVALID; }
     p.row_begin[w] = row_begin[w];
@@ -1043,13 +1227,13 @@ extern "C" int daam_segment_words(const float* global_maps, int32_t n_maps, int3
     if (r < 0 || r >= n_rows) { set_error("%s: row %d out of range [0, %d)", name, rows[i], n_rows); return DAAM_E_INVALID; }
     p.rows[i] = r;
   }
-  p.maps = global_maps; p.word_maps = word_maps; p.labels = labels; p.scores = scores; p.scratch = scratch;
+  p.maps = global_maps; p.word_maps = word_maps; p.labels = nullptr; p.scores = nullptr; p.scratch = scratch;
   p.map_stride = (long long)n_rows * mh * mw;
   p.mh = mh; p.mw = mw; p.oh = out_h; p.ow = out_w; p.n_words = n_words;
   p.absolute = absolute ? 1 : 0; p.use_threshold = use_threshold ? 1 : 0; p.threshold = threshold;
   // launch 1: enough (map, word, chunk) CTAs for a few waves, at most kMaxChunks per word and one per 256 pixels
   const long long n = (long long)out_h * out_w, mwords = (long long)n_maps * n_words;
-  long long chunks = (4LL * dev.sm_count + mwords - 1) / mwords;
+  long long chunks = (4LL * dev->sm_count + mwords - 1) / mwords;
   if (chunks > kMaxChunks) chunks = kMaxChunks;
   if (chunks > (n + 255) / 256) chunks = (n + 255) / 256;
   if (chunks < 1 || p.absolute) chunks = 1;
@@ -1059,21 +1243,77 @@ extern "C" int daam_segment_words(const float* global_maps, int32_t n_maps, int3
   const int win_w = std::min<int>(mw, (int)ceil((double)kSegTileW * mw / out_w) + 5);
   const int win = win_h * win_w;
   p.words_per_pass = std::max(1, std::min(n_words, kSegStageFloats / win));
-  const size_t smem1 = (size_t)mh * mw * sizeof(float), smem2 = (size_t)p.words_per_pass * win * sizeof(float);
+  *smem1 = (size_t)mh * mw * sizeof(float);
+  *smem2 = (size_t)p.words_per_pass * win * sizeof(float);
   static std::once_flag attr_once[64];
   cudaError_t attr_err = cudaSuccess;
-  std::call_once(attr_once[dev.device & 63], [&] {
+  std::call_once(attr_once[dev->device & 63], [&] {
     attr_err = cudaFuncSetAttribute(segment_minmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     if (attr_err == cudaSuccess)
       attr_err = cudaFuncSetAttribute(segment_label_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    if (attr_err == cudaSuccess)
+      attr_err = cudaFuncSetAttribute(region_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   });
   DAAM_CUDA_TRY(attr_err);
-  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  segment_minmax_kernel<<<(unsigned)(mwords * chunks), 256, smem1, stream>>>(p);
+  return DAAM_OK;
+}
+
+static int launch_segment_minmax(const SegmentParams& p, int n_maps, size_t smem1, cudaStream_t stream) {
+  segment_minmax_kernel<<<(unsigned)((long long)n_maps * p.n_words * p.chunks), 256, smem1, stream>>>(p);
   DAAM_CUDA_TRY(cudaGetLastError());
   count_launch();
+  return DAAM_OK;
+}
+
+extern "C" int daam_segment_words(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t mh, int32_t mw,
+                                  const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h,
+                                  int32_t out_w, int32_t absolute, int32_t use_threshold, float threshold,
+                                  float* word_maps, uint8_t* labels, float* scores, float* scratch, void* stream_) {
+  const char* name = "daam_segment_words";
+  if (!global_maps || !rows || !row_begin || !word_maps || !labels || !scores || !scratch || n_maps <= 0 || mh <= 0 ||
+      mw <= 0 || out_h <= 0 || out_w <= 0 || n_rows <= 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
+  static thread_local SegmentParams p;
+  DeviceInfo dev;
+  size_t smem1, smem2;
+  if (int rc = segment_prepare(name, global_maps, n_maps, n_rows, mh, mw, rows, row_begin, n_words, out_h, out_w,
+                               absolute, use_threshold, threshold, word_maps, scratch, p, &dev, &smem1, &smem2)) return rc;
+  p.labels = labels; p.scores = scores;
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (int rc = launch_segment_minmax(p, n_maps, smem1, stream)) return rc;
   const int tiles = ((out_h + kSegTileH - 1) / kSegTileH) * ((out_w + kSegTileW - 1) / kSegTileW);
   segment_label_kernel<<<dim3(tiles, n_maps), 256, smem2, stream>>>(p);
+  DAAM_CUDA_TRY(cudaGetLastError());
+  count_launch();
+  return DAAM_OK;
+}
+
+extern "C" int daam_region_overlap(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t mh, int32_t mw,
+                                   const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h,
+                                   int32_t out_w, int32_t absolute, int32_t use_threshold, float threshold,
+                                   float* word_maps, const uint8_t* regions, int32_t n_regions, float* intersection,
+                                   float* word_area, float* scratch, void* stream_) {
+  const char* name = "daam_region_overlap";
+  if (!global_maps || !rows || !row_begin || !word_maps || !regions || !intersection || !word_area || !scratch ||
+      n_maps <= 0 || mh <= 0 || mw <= 0 || out_h <= 0 || out_w <= 0 || n_rows <= 0 || n_regions <= 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
+  if (n_regions > kMaxRegions) { set_error("%s: %d regions > %d", name, n_regions, kMaxRegions); return DAAM_E_UNSUPPORTED; }
+  // fp32 partial sums of 0/1 values stay exact integers up to 2^24
+  if ((long long)out_h * out_w > (1LL << 24)) { set_error("%s: a %d x %d output is more than 2^24 pixels", name, out_h, out_w); return DAAM_E_UNSUPPORTED; }
+  static thread_local RegionParams p;
+  DeviceInfo dev;
+  size_t smem1, smem2;
+  if (int rc = segment_prepare(name, global_maps, n_maps, n_rows, mh, mw, rows, row_begin, n_words, out_h, out_w,
+                               absolute, use_threshold, threshold, word_maps, scratch, p.s, &dev, &smem1, &smem2)) return rc;
+  const int tiles = ((out_h + kSegTileH - 1) / kSegTileH) * ((out_w + kSegTileW - 1) / kSegTileW);
+  p.regions = regions; p.n_regions = n_regions; p.tiles = tiles;
+  p.partials = scratch + 64LL * n_maps * n_words;     // after segment_minmax_kernel's min / max partials
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (int rc = launch_segment_minmax(p.s, n_maps, smem1, stream)) return rc;
+  region_tile_kernel<<<dim3(tiles, n_maps), 256, smem2, stream>>>(p);
+  DAAM_CUDA_TRY(cudaGetLastError());
+  count_launch();
+  const long long n_out = (long long)n_maps * n_words * (n_regions + 1);
+  region_reduce_kernel<<<(unsigned)((n_out + 7) / 8), 256, 0, stream>>>(p.partials, n_out, tiles, n_words, n_regions,
+                                                                        intersection, word_area);
   DAAM_CUDA_TRY(cudaGetLastError());
   count_launch();
   return DAAM_OK;

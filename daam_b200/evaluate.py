@@ -4,6 +4,12 @@ Only ``compute_iou`` / ``compute_ioa`` are mirrored -- the part of SURVEY.md sec
 When the two masks differ in size the reference bicubically resizes the first to the second and binarises it at 1;
 that resize runs on the native ``daam_expand_as`` kernel (absolute mode). The COCO evaluators (``UnsupervisedEvaluator``,
 ``MeanEvaluator``, PNG mask loading) are out of scope.
+
+These functions score one (mask, region) pair per call, each ending in a blocking ``.item()``. To score a word list
+against several regions, or every step of a history, use :meth:`GlobalHeatMap.region_overlap
+<daam_b200.heatmap.GlobalHeatMap.region_overlap>` / :meth:`GlobalHeatMapStack.region_overlap
+<daam_b200.heatmap.GlobalHeatMapStack.region_overlap>`: three fused launches for every (map, region, word), whose
+``iou()`` / ``ioa()`` equal ``compute_iou`` / ``compute_ioa`` of each thresholded mask and binary region bit for bit.
 """
 from __future__ import annotations
 

@@ -25,7 +25,7 @@ from . import _native
 from .utils import compute_token_merge_indices
 
 __all__ = ['GlobalHeatMap', 'RawHeatMapCollection', 'WordHeatMap', 'LayerSlab', 'GlobalHeatMapStack', 'TimeHeatMaps',
-           'ImageHeatMaps']
+           'ImageHeatMaps', 'RegionOverlap']
 
 RawHeatMapKey = Tuple[int, int, int]  # factor, layer, head
 
@@ -407,6 +407,29 @@ class GlobalHeatMap:
         whms = [WordHeatMap(word_maps[0, i], w, idx) for i, (w, (_, idx)) in enumerate(zip(words, merged))]
         return whms, labels[0], scores[0]
 
+    def region_overlap(self, words, image, regions: torch.Tensor, absolute: bool = False,
+                       threshold: Optional[float] = None, word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
+        """How much of each word's expanded map lies inside each image region: the sums behind the reference's
+        ``compute_iou`` / ``compute_ioa`` (``daam/evaluate.py``) for every (word, region) pair at once. With ``m`` the
+        ``[len(words), H, W]`` that ``expand_words(words, image, absolute, threshold, word_idx, offset_idx)`` returns
+        (0/1 masks when ``threshold`` is in effect) and ``regions`` a device ``bool`` / ``uint8`` ``[R, H, W]`` or
+        ``[H, W]`` tensor at that size (nonzero is inside), the :class:`RegionOverlap` holds
+        ``intersection[r, w] = (m[w] * (regions[r] != 0)).sum()``, ``word_area[w] = m[w].sum()`` and
+        ``region_area[r]``; its ``iou()`` / ``ioa()`` equal ``compute_iou`` / ``compute_ioa`` of every pair, bit for bit,
+        when the threshold is in effect. Three fused launches; the ``[len(words), H, W]`` stack is never materialised.
+
+        Returns ``(word_heat_maps, overlap)``: the list of :class:`WordHeatMap` that :meth:`segment` returns and the
+        :class:`RegionOverlap` (CPU by default, ``to_cpu=False`` keeps it on the device). A ``[H, W]`` region is one
+        region: the region axis stays, of length 1. At most 96 words, 63 regions and 2**24 image pixels. An empty word
+        list or region set launches nothing, returns no word heat maps and measures no word (a word axis of length 0).
+        Raises the reference's ``ValueError`` for a word that is not in the prompt."""
+        words = list(words)
+        word_maps, merged, overlap = _region_overlap(self.tokenizer, self.prompt, self.heat_maps[None], words, image,
+                                                     regions, absolute, threshold, word_idx, offset_idx, to_cpu,
+                                                     'GlobalHeatMap.region_overlap')
+        whms = [WordHeatMap(word_maps[0, i], w, idx) for i, (w, (_, idx)) in enumerate(zip(words, merged))]
+        return whms, RegionOverlap(overlap.intersection[0], overlap.word_area[0], overlap.region_area)
+
 
 def _word_rows(tokenizer, prompt: str, words: List[str], word_idx, offset_idx: int, n_rows: int):
     """``compute_token_merge_indices`` of every word (``word_idx`` may be a list parallel to ``words``), with the
@@ -446,6 +469,80 @@ def _segment(tokenizer, prompt: str, maps: torch.Tensor, words, image, absolute,
     if to_cpu:
         labels, scores = labels.cpu(), scores.cpu()
     return word_maps, merged, labels, scores
+
+
+@dataclass
+class RegionOverlap:
+    """Sums of word maps over image regions (:meth:`GlobalHeatMap.region_overlap`): ``intersection`` ``[..., R, W]``
+    (``sum_p region[r](p) * m[w](p)``), ``word_area`` ``[..., W]`` (``sum_p m[w](p)``) and ``region_area`` ``[R]``
+    (pixels inside each region), fp32. ``...`` is the map axis of a :class:`GlobalHeatMapStack`, absent for one map.
+    The scores are the reference's formulas (``daam/evaluate.py``) in the same fp32 operation order."""
+    intersection: torch.Tensor
+    word_area: torch.Tensor
+    region_area: torch.Tensor
+
+    def iou(self) -> torch.Tensor:
+        """``I / (A_w + A_r - I + 1e-8)``: ``compute_iou(mask, region)`` of every pair."""
+        i = self.intersection
+        return i / (self.word_area.unsqueeze(-2) + self.region_area.unsqueeze(-1) - i + 1e-8)
+
+    def ioa(self) -> torch.Tensor:
+        """``I / (A_w + 1e-8)``: ``compute_ioa(mask, region)`` of every pair, the intersection over the word's area."""
+        return self.intersection / (self.word_area.unsqueeze(-2) + 1e-8)
+
+    def region_mean(self) -> torch.Tensor:
+        """``I / (A_r + 1e-8)``: without a threshold the mean of the word's expanded map inside the region, with one the
+        fraction of the region the word's mask covers."""
+        return self.intersection / (self.region_area.unsqueeze(-1) + 1e-8)
+
+
+def _region_overlap(tokenizer, prompt: str, maps: torch.Tensor, words, image, regions, absolute, threshold, word_idx,
+                    offset_idx: int, to_cpu: bool, what: str):
+    """``daam_region_overlap`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(word_maps, merged, overlap)``: the
+    device word heat maps ``[n_maps, len(words), xh, xw]``, ``compute_token_merge_indices`` of every word, and the
+    :class:`RegionOverlap` with a leading map axis."""
+    n_maps, n_rows, grid = maps.shape[0], maps.shape[1], tuple(maps.shape[-2:])
+    merged = _word_rows(tokenizer, prompt, words, word_idx, offset_idx, n_rows)
+    _require_cuda(maps, what)
+    out_h, out_w = _image_size(image, *grid)
+    if not isinstance(regions, torch.Tensor):
+        raise TypeError(f'{what}: regions must be a torch.Tensor, not {type(regions).__name__}')
+    if regions.dtype not in (torch.bool, torch.uint8):
+        raise TypeError(f'{what}: regions must be bool or uint8, not {regions.dtype}')
+    if regions.dim() == 2:
+        regions = regions[None]
+    if regions.dim() != 3 or tuple(regions.shape[1:]) != (out_h, out_w):
+        raise ValueError(f'{what}: regions of shape {tuple(regions.shape)} do not match the expanded maps\' '
+                         f'(R, {out_h}, {out_w}) (a [{out_h}, {out_w}] region or a stack of them)')
+    _require_cuda(regions, what)
+    dev = maps.device
+    if regions.device != dev:
+        raise ValueError(f'{what}: regions are on {regions.device}, the heat maps on {dev}')
+    n_regions = regions.shape[0]
+    if not words or n_regions == 0 or n_maps == 0:
+        ov = RegionOverlap(torch.zeros((n_maps, n_regions, 0), device=dev), torch.zeros((n_maps, 0), device=dev),
+                           torch.zeros((n_regions,), device=dev))
+        word_maps = torch.empty((n_maps, 0) + grid, dtype=torch.float32, device=dev)
+        return word_maps, [], (_to_cpu(ov) if to_cpu else ov)
+    maps = maps.detach().float().contiguous()
+    region_bytes = regions.detach().contiguous().view(torch.uint8)
+    word_maps = torch.empty((n_maps, len(words)) + grid, dtype=torch.float32, device=dev)
+    inter = torch.empty((n_maps, n_regions, len(words)), dtype=torch.float32, device=dev)
+    area = torch.empty((n_maps, len(words)), dtype=torch.float32, device=dev)
+    scratch = torch.empty(_native.region_scratch_floats(n_maps, len(words), n_regions, out_h, out_w),
+                          dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _native.region_overlap(maps.data_ptr(), n_maps, n_rows, grid, [rows for rows, _ in merged], out_h, out_w,
+                               absolute, threshold, word_maps.data_ptr(), region_bytes.data_ptr(), n_regions,
+                               inter.data_ptr(), area.data_ptr(), scratch.data_ptr(), _stream_ptr(dev))
+    # exact pixel counts (at most 2**24 pixels): what ``region.float().sum()`` gives in compute_iou
+    region_area = (region_bytes != 0).sum((-1, -2)).float()
+    ov = RegionOverlap(inter, area, region_area)
+    return word_maps, merged, (_to_cpu(ov) if to_cpu else ov)
+
+
+def _to_cpu(ov: RegionOverlap) -> RegionOverlap:
+    return RegionOverlap(ov.intersection.cpu(), ov.word_area.cpu(), ov.region_area.cpu())
 
 
 class GlobalHeatMapStack:
@@ -492,6 +589,18 @@ class GlobalHeatMapStack:
                                                 absolute, threshold, word_idx, offset_idx, to_cpu,
                                                 f'{type(self).__name__}.segment')
         return word_maps, labels, scores
+
+    def region_overlap(self, words, image, regions: torch.Tensor, absolute: bool = False,
+                       threshold: Optional[float] = None, word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
+        """:meth:`GlobalHeatMap.region_overlap` for every map in one call (three launches whatever the map count):
+        returns ``(word_maps, overlap)`` with ``word_maps`` the device ``[maps, len(words), xh, xw]`` word heat maps and
+        ``overlap`` a :class:`RegionOverlap` with a leading map axis (``intersection`` ``[maps, R, W]``, ``word_area``
+        ``[maps, W]``); row ``t`` equals ``self[t].region_overlap(...)`` bit for bit (min / max normalisation per map
+        and word). E.g. ``overlap.iou()[:, 0, 0]`` is word 0's IoU with region 0 at every step of a history."""
+        word_maps, _, overlap = _region_overlap(self.tokenizer, self.prompt, self.heat_maps, list(words), image,
+                                                regions, absolute, threshold, word_idx, offset_idx, to_cpu,
+                                                f'{type(self).__name__}.region_overlap')
+        return word_maps, overlap
 
 
 class TimeHeatMaps(GlobalHeatMapStack):

@@ -32,7 +32,8 @@ extern "C" {
                                           (later, additive: layers with hw not a multiple of 4 are accepted;
                                           daam_segment_words, daam_finalize_maps; daam_key_group.reserved is
                                           n_blocks; daam_accumulate takes 154- and 231-token contexts; layers with
-                                          several prompts and a prompt stride <= 0 take the SIMT kernel) */
+                                          several prompts and a prompt stride <= 0 take the SIMT kernel;
+                                          daam_region_overlap) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_TOKENS 231     /* daam_accumulate: long contexts of 2 or 3 CLIP chunks of 77 tokens (154, 231) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
@@ -308,6 +309,31 @@ int daam_segment_words(const float* global_maps, int32_t n_maps, int32_t n_rows,
                        const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w,
                        int32_t absolute, int32_t use_threshold, float threshold, float* word_maps, uint8_t* labels,
                        float* scores, float* scratch, void* stream);
+
+/*
+ * Word-region overlap: how much of each word's expanded map lies inside each of n_regions binary image regions, on
+ * each of n_maps global maps stored back to back -- the sums behind the reference's evaluation (daam/evaluate.py:14-35:
+ * compute_iou / compute_ioa of every (word mask, region) pair). With m[w] what daam_expand_words writes for word w with
+ * the same arguments (0/1 when use_threshold) and R[r](p) = (regions[r][p] != 0):
+ *   intersection[i][r][w] = sum_p R[r](p) * m[w](p)          (fp32 [n_maps][n_regions][n_words])
+ *   word_area[i][w]       = sum_p m[w](p)                    (fp32 [n_maps][n_words])
+ * Arguments as daam_segment_words, plus regions: device uint8 [n_regions][out_h][out_w], shared by every map (any
+ * nonzero byte is inside). scratch: device, >= DAAM_REGION_SCRATCH_FLOATS(n_maps, n_words, n_regions, out_h, out_w)
+ * floats. Three launches whatever n_maps, n_words and n_regions; the [n_words][out_h][out_w] stack is never written.
+ * The sums run in a fixed order without atomics, so repeated calls give the same bits; with use_threshold every
+ * sum is an exact pixel count.
+ * Limits (DAAM_E_UNSUPPORTED): n_words <= 96, row_begin[n_words] <= 320, n_regions <= 63 (DAAM_REGION_MAX_REGIONS),
+ * map_h * map_w * 4 bytes <= 200 KB, n_maps <= 65535, out_h * out_w <= 2^24 (counts stay exact in fp32). DAAM_E_INVALID:
+ * null pointer, non-positive size (n_regions included), empty word list, a word without rows, a row out of range.
+ */
+#define DAAM_REGION_MAX_REGIONS 63
+#define DAAM_REGION_SCRATCH_FLOATS(n_maps, n_words, n_regions, out_h, out_w)                                        \
+  ((int64_t)(n_maps) * (n_words) * (64 + ((int64_t)(n_regions) + 1) * (((out_h) + 15) / 16) * (((out_w) + 63) / 64)))
+int daam_region_overlap(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t map_h, int32_t map_w,
+                        const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w,
+                        int32_t absolute, int32_t use_threshold, float threshold, float* word_maps,
+                        const uint8_t* regions, int32_t n_regions, float* intersection, float* word_area, float* scratch,
+                        void* stream);
 
 /* Library / device introspection. */
 int daam_abi_version(void);
