@@ -38,9 +38,14 @@ def region_scratch_floats(n_maps: int, n_words: int, n_regions: int, out_h: int,
     return n_maps * n_words * (64 + (n_regions + 1) * ((out_h + 15) // 16) * ((out_w + 63) // 64))
 
 
+def overlay_frames_bytes(n_maps: int, n_words: int, out_h: int, out_w: int) -> int:
+    """``DAAM_OVERLAY_FRAMES_BYTES(n_maps, n_words, out_h, out_w)``: the frames rounded up to whole 4-byte words."""
+    return (n_maps * n_words * out_h * out_w * 3 + 3) // 4 * 4
+
+
 EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize',
            'daam_finalize_maps', 'daam_finalize_per_key','daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
-           'daam_segment_words', 'daam_region_overlap',
+           'daam_segment_words', 'daam_region_overlap', 'daam_overlay_words', 'daam_jet_colormap',
            'daam_side_launcher_create', 'daam_side_launcher_destroy',
            'daam_side_launcher_launch', 'daam_side_launcher_join', 'daam_side_launcher_idle', 'daam_abi_version',
            'daam_last_error', 'daam_device_info', 'daam_launch_count')
@@ -136,6 +141,11 @@ def load() -> ctypes.CDLL:
     lib.daam_region_overlap.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
                                         i32, i32, f32, vp, vp, i32, vp, vp, vp, vp]
     lib.daam_region_overlap.restype = ctypes.c_int
+    lib.daam_overlay_words.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
+                                       i32, i32, f32, i32, vp, vp, i64, vp, vp, vp]
+    lib.daam_overlay_words.restype = ctypes.c_int
+    lib.daam_jet_colormap.argtypes = [vp]
+    lib.daam_jet_colormap.restype = ctypes.c_int
     lib.daam_side_launcher_create.argtypes = [ctypes.POINTER(vp)]
     lib.daam_side_launcher_create.restype = ctypes.c_int
     lib.daam_side_launcher_destroy.argtypes = [vp]
@@ -372,6 +382,30 @@ def region_overlap(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Se
                                       ctypes.c_void_p(regions_ptr), n_regions, ctypes.c_void_p(intersection_ptr),
                                       ctypes.c_void_p(word_area_ptr), ctypes.c_void_p(scratch_ptr),
                                       ctypes.c_void_p(stream)))
+
+
+def overlay_words(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int,
+                  out_w: int, absolute: bool, threshold: Optional[float], color_normalize: bool, word_maps_ptr: int,
+                  image_ptr: int, image_map_stride: int, frames_ptr: int, scratch_ptr: int, stream: int):
+    """``daam_overlay_words`` over ``n_maps`` maps ``[n_rows, h, w]`` back to back; ``image_ptr`` uint8 ``[out_h, out_w,
+    3]``, map ``i``'s at ``image_ptr + i * image_map_stride`` bytes (0: one image for all); ``frames_ptr`` a buffer of
+    :func:`overlay_frames_bytes` bytes; ``rows_per_word`` as for :func:`expand_words`."""
+    h, w = map_size(x)
+    rows_arr, begin_arr = _row_lists(rows_per_word)
+    use_thr = bool(threshold)   # the reference's `if threshold:` (daam/heatmap.py:87), as expand_words resolves it
+    _check(load().daam_overlay_words(ctypes.c_void_p(maps_ptr), n_maps, n_rows, h, w, rows_arr, begin_arr,
+                                     len(rows_per_word), out_h, out_w, int(bool(absolute)), int(use_thr),
+                                     float(threshold) if use_thr else 0.0, int(bool(color_normalize)),
+                                     ctypes.c_void_p(word_maps_ptr), ctypes.c_void_p(image_ptr), image_map_stride,
+                                     ctypes.c_void_p(frames_ptr), ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
+
+
+def jet_colormap():
+    """``daam_jet_colormap``: the fp32 ``[256, 3]`` colour table the overlay kernel reads, as a CPU tensor."""
+    import torch
+    out = torch.empty((256, 3), dtype=torch.float32)
+    _check(load().daam_jet_colormap(ctypes.c_void_p(out.data_ptr())))
+    return out
 
 
 def device_info():

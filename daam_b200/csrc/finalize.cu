@@ -893,6 +893,222 @@ __global__ void __launch_bounds__(256) region_reduce_kernel(const float* __restr
   }
 }
 
+// ---- heat-map overlays: the jet-coloured word map blended onto the image -----------------------------------------
+// The reference's plot_overlay (heatmap.py:20-53, 66-75) as pixels: with m[w] what expand_words_kernel writes for word
+// w, for every byte of frames [n_maps][n_words][oh][ow][3]:
+//   c = color_normalize ? (hi == lo ? 0 : (m - lo) / (hi - lo)) : clamp(m, 0, 1)   (lo / hi: min / max of m[w])
+//   k = min(int(c * 256), 255)                                                      (matplotlib's Colormap, N = 256)
+//   a = clamp(m, 0, 1)                                                              (the image drawn with alpha 1 - a)
+//   out = uint8(clamp(rne((1 - a) * image + a * jet[k]), 0, 255))                   (every operation rounded in fp32)
+// in two launches whatever n_maps and n_words:
+//  1. segment_minmax_kernel (unchanged): word maps and the per-chunk min / max of the interpolated map v;
+//  2. overlay_kernel, CTA = (16 x 64 output tile, map): stages the source windows of a pass of words as
+//     segment_label_kernel does, computes m[w] with the same taps, bicubic_shared, minmax_normalize and threshold
+//     compare as expand_words_kernel, and writes every word's RGB bytes through shared memory in aligned 4- and 16-byte
+//     stores. v -> m is monotone non-decreasing in fp32 (subtract, divide by a positive constant, `>` threshold), so
+//     lo / hi of m are m at the min / max of v: no pass over m.
+// The [n_words][out_h][out_w] stack is never written. A 4-byte word of frames belongs to the CTA that owns its first
+// byte; when it reaches past the tile row, that CTA computes the one next pixel in memory order (the next tile, row,
+// word or map) from the global word maps, with the same arithmetic.
+
+// matplotlib's `jet` segment data (_cm.py): piecewise linear through (x, y) in each channel
+struct JetSegments { int n; double x[6], y[6]; };
+constexpr JetSegments kJet[3] = {
+    {5, {0., 0.35, 0.66, 0.89, 1.}, {0., 0., 1., 1., 0.5}},
+    {6, {0., 0.125, 0.375, 0.64, 0.91, 1.}, {0., 0., 1., 1., 0., 0.}},
+    {5, {0., 0.11, 0.34, 0.65, 1.}, {0.5, 1., 1., 0., 0.}},
+};
+
+constexpr double jet_channel(int ch, double x) {
+  const JetSegments& s = kJet[ch];
+  int i = 0;
+  while (i + 2 < s.n && x > s.x[i + 1]) ++i;
+  const double t = (x - s.x[i]) / (s.x[i + 1] - s.x[i]);
+  const double d = (s.y[i + 1] - s.y[i]) * t;
+  return s.y[i] + d;
+}
+
+struct JetTable { float v[256 * 3]; };
+constexpr JetTable make_jet_table() {
+  JetTable t{};
+  for (int k = 0; k < 256; ++k)
+    for (int ch = 0; ch < 3; ++ch) t.v[3 * k + ch] = (float)(255.0 * jet_channel(ch, k / 255.0));
+  return t;
+}
+constexpr JetTable kJetTable = make_jet_table();
+static_assert(kJetTable.v[0] == 0.f && kJetTable.v[1] == 0.f && kJetTable.v[2] == 127.5f, "jet(0) = (0, 0, 0.5)");
+static_assert(kJetTable.v[765] == 127.5f && kJetTable.v[766] == 0.f && kJetTable.v[767] == 0.f, "jet(1) = (0.5, 0, 0)");
+
+// L[k][ch] = fp32(255 * jet_ch(k / 255)): the one copy of the table; daam_jet_colormap reads it back
+__constant__ JetTable c_jet = kJetTable;
+
+constexpr int kOverlayRowBytes = 16 + 3 * kSegTileW + 16;   // a tile row's bytes from its 16-byte aligned base, + 1 pixel
+
+struct OverlayParams {
+  SegmentParams s;                      // maps, word_maps, scratch, sizes, rows, words_per_pass; s.absolute: no min / max
+  const unsigned char* image;           // [oh][ow][3], map i at image + i * image_map_stride
+  long long image_map_stride;           // bytes; 0: one image for every map
+  unsigned char* frames;                // [n_maps][n_words][oh][ow][3], 4-byte aligned, padded to a 4-byte multiple
+  int absolute, color_normalize, n_maps;
+};
+
+// min / max of the interpolated map v of (map, word), reduced from segment_minmax_kernel's chunks
+__device__ __forceinline__ void overlay_v_bounds(const SegmentParams& P, int map, int w, float& lo, float& hi) {
+  lo = 0.f; hi = 0.f;
+  if (P.absolute) return;                              // no min / max was computed: neither is needed
+  const float* slots = P.scratch + 2 * ((long long)map * P.n_words + w) * P.chunks;
+  lo = INFINITY; hi = -INFINITY;
+  for (int c = 0; c < P.chunks; ++c) { lo = fminf(lo, slots[2 * c]); hi = fmaxf(hi, slots[2 * c + 1]); }
+}
+
+// v -> m as expand_words_kernel does it
+__device__ __forceinline__ float overlay_m(const OverlayParams& O, float v, float vlo, float vhi) {
+  if (!O.absolute) v = minmax_normalize(v, vlo, vhi);
+  if (O.s.use_threshold) v = v > O.s.threshold ? 1.f : 0.f;
+  return v;
+}
+
+// one pixel's three bytes from m, the word's lo / hi of m, the image pixel and the staged table
+__device__ __forceinline__ void overlay_rgb(float m, float lo, float hi, int color_normalize, const unsigned char* im,
+                                            const float* lut, unsigned char* out) {
+  float c;
+  if (color_normalize) c = hi == lo ? 0.f : __fdiv_rn(__fsub_rn(m, lo), __fsub_rn(hi, lo));
+  else c = fminf(fmaxf(m, 0.f), 1.f);
+  const int k = min((int)__fmul_rn(c, 256.f), 255);
+  const float a = fminf(fmaxf(m, 0.f), 1.f), na = __fsub_rn(1.f, a);
+#pragma unroll
+  for (int ch = 0; ch < 3; ++ch) {
+    const float v = __fadd_rn(__fmul_rn(na, (float)im[ch]), __fmul_rn(a, lut[3 * k + ch]));
+    out[ch] = (unsigned char)min(max(__float2int_rn(v), 0), 255);
+  }
+}
+
+// The bytes of output pixel (oy, ox) of (map, word), computed from the global word map: the same taps and
+// bicubic_shared over the whole map as the tile path over its staged window. Zeros past the last map.
+__device__ void overlay_pixel_global(const OverlayParams& O, const float* lut, int map, int w, int oy, int ox,
+                                     unsigned char* out) {
+  const SegmentParams& P = O.s;
+  if (map >= O.n_maps) { out[0] = out[1] = out[2] = 0; return; }
+  float vlo, vhi;
+  overlay_v_bounds(P, map, w, vlo, vhi);
+  const float lo = overlay_m(O, vlo, vlo, vhi), hi = overlay_m(O, vhi, vlo, vhi);
+  const float* wm = P.word_maps + ((long long)map * P.n_words + w) * P.mh * P.mw;
+  const float v = bicubic_shared(wm, P.mw, make_taps(oy, P.mh, P.oh), make_taps(ox, P.mw, P.ow));
+  const unsigned char* im = O.image + map * O.image_map_stride + ((long long)oy * P.ow + ox) * 3;
+  const unsigned char px[3] = {__ldg(im), __ldg(im + 1), __ldg(im + 2)};
+  overlay_rgb(overlay_m(O, v, vlo, vhi), lo, hi, O.color_normalize, px, lut, out);
+}
+
+// grid: (tiles of kSegTileH x kSegTileW output pixels, n_maps); dynamic smem: words_per_pass source windows
+__global__ void __launch_bounds__(256) overlay_kernel(const __grid_constant__ OverlayParams O) {
+  extern __shared__ __align__(16) float win[];
+  __shared__ float s_vlo[kMaxWords], s_vhi[kMaxWords], s_lo[kMaxWords], s_hi[kMaxWords];
+  __shared__ int tyi[4][kSegTileH], txi[4][kSegTileW];   // the tile's taps, relative to the staged window
+  __shared__ float tyw[4][kSegTileH], txw[4][kSegTileW];
+  __shared__ float lut[256 * 3];
+  __shared__ unsigned char img[kSegTileH * kSegTileW * 3];
+  __shared__ __align__(16) unsigned char rows[2][kSegTileH][kOverlayRowBytes];   // double-buffered across words
+  const SegmentParams& P = O.s;
+  const int map = blockIdx.y, mh = P.mh, mw = P.mw, oh = P.oh, ow = P.ow, n_words = P.n_words;
+  const int tiles_x = (ow + kSegTileW - 1) / kSegTileW;
+  const int y0 = (blockIdx.x / tiles_x) * kSegTileH, x0 = (blockIdx.x % tiles_x) * kSegTileW;
+  const int th = min(kSegTileH, oh - y0), tw = min(kSegTileW, ow - x0);
+  const int wy = make_taps(y0, mh, oh).idx[0], wx = make_taps(x0, mw, ow).idx[0];
+  const int wh = make_taps(y0 + th - 1, mh, oh).idx[3] - wy + 1, ww = make_taps(x0 + tw - 1, mw, ow).idx[3] - wx + 1;
+  const int wn = wh * ww;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int w = threadIdx.x; w < n_words; w += blockDim.x) {
+    float vlo, vhi;
+    overlay_v_bounds(P, map, w, vlo, vhi);
+    s_vlo[w] = vlo; s_vhi[w] = vhi;
+    s_lo[w] = overlay_m(O, vlo, vlo, vhi); s_hi[w] = overlay_m(O, vhi, vlo, vhi);
+  }
+  for (int i = threadIdx.x; i < 256 * 3; i += blockDim.x) lut[i] = c_jet.v[i];
+  if (threadIdx.x < th) {
+    const Taps t = make_taps(y0 + threadIdx.x, mh, oh);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) { tyi[j][threadIdx.x] = t.idx[j] - wy; tyw[j][threadIdx.x] = t.w[j]; }
+  } else if (threadIdx.x >= kSegTileH && threadIdx.x < kSegTileH + tw) {
+    const int x = threadIdx.x - kSegTileH;
+    const Taps t = make_taps(x0 + x, mw, ow);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) { txi[j][x] = t.idx[j] - wx; txw[j][x] = t.w[j]; }
+  }
+  // the tile's image bytes, read once for every word
+  const unsigned char* image = O.image + map * O.image_map_stride;
+  for (int i = threadIdx.x; i < th * tw * 3; i += blockDim.x) {
+    const int r = i / (tw * 3), b = i - r * tw * 3;
+    img[i] = __ldg(image + ((long long)(y0 + r) * ow + x0) * 3 + b);
+  }
+  const float* word_maps = P.word_maps + (long long)map * n_words * mh * mw;
+  const unsigned long long frames = (unsigned long long)O.frames;   // byte addresses: the alignment of the stores
+  for (int w0 = 0; w0 < n_words; w0 += P.words_per_pass) {
+    const int nw = min(P.words_per_pass, n_words - w0);
+    __syncthreads();                                   // the previous pass has read its windows (and the tables are set)
+    for (int i = threadIdx.x; i < nw * wn; i += blockDim.x) {
+      const int wi = i / wn, r = i - wi * wn, y = r / ww, x = r - y * ww;
+      win[i] = __ldg(word_maps + ((long long)(w0 + wi) * mh + wy + y) * mw + wx + x);
+    }
+    __syncthreads();
+    for (int wi = 0; wi < nw; ++wi) {
+      const int w = w0 + wi;
+      const float vlo = s_vlo[w], vhi = s_vhi[w], lo = s_lo[w], hi = s_hi[w];
+      // row py of the tile starts at byte g0(py) of frames; rows[w & 1][py][g0 & 15] holds that byte
+      const long long row0 = (((long long)map * n_words + w) * oh + y0) * ow + x0;
+#pragma unroll
+      for (int k = 0; k < kSegPix; ++k) {
+        const int p = threadIdx.x + 256 * k;
+        if (p < th * tw) {
+          const int py = p / tw, px = p - py * tw;
+          Taps ty, tx;
+#pragma unroll
+          for (int j = 0; j < 4; ++j) {
+            ty.idx[j] = tyi[j][py]; ty.w[j] = tyw[j][py]; tx.idx[j] = txi[j][px]; tx.w[j] = txw[j][px];
+          }
+          const float m = overlay_m(O, bicubic_shared(win + wi * wn, ww, ty, tx), vlo, vhi);
+          const unsigned shift = (unsigned)((frames + 3 * (row0 + (long long)py * ow)) & 15);
+          overlay_rgb(m, lo, hi, O.color_normalize, img + 3 * p, lut, &rows[w & 1][py][shift + 3 * px]);
+        }
+      }
+      // a row whose last 4-byte word reaches past it: the next pixel in memory order
+      if (threadIdx.x < th) {
+        const int py = threadIdx.x;
+        const unsigned long long g1 = frames + 3 * (row0 + (long long)py * ow + tw);
+        if (g1 & 3) {
+          int nm = map, nwd = w, ny = y0 + py, nx = x0 + tw;
+          if (nx == ow) { nx = 0; ++ny; }
+          if (ny == oh) { ny = 0; ++nwd; }
+          if (nwd == n_words) { nwd = 0; ++nm; }
+          const unsigned shift = (unsigned)((g1 - 3 * tw) & 15);
+          overlay_pixel_global(O, lut, nm, nwd, ny, nx, &rows[w & 1][py][shift + 3 * tw]);
+        }
+      }
+      // one barrier per word: rows[w & 1] is rewritten two words later, after every warp has passed the next barrier
+      __syncthreads();
+      for (int py = warp; py < th; py += 8) {
+        const unsigned long long g0 = frames + 3 * (row0 + (long long)py * ow), g1 = g0 + 3 * tw;
+        const unsigned long long base = g0 & ~15ull, a0 = (g0 + 3) & ~3ull, a1 = (g1 + 3) & ~3ull;
+        // the owned words [a0, a1): 4-byte words up to a 16-byte boundary, 16-byte stores, 4-byte words
+        const unsigned long long b0 = min((a0 + 15) & ~15ull, a1), b1 = max(b0, a1 & ~15ull);
+        const int n_head = (int)((b0 - a0) >> 2), n_body = (int)((b1 - b0) >> 4), n_tail = (int)((a1 - b1) >> 2);
+        const unsigned char* src = rows[w & 1][py];
+        for (int j = lane; j < n_head + n_body + n_tail; j += 32) {
+          if (j < n_head) {
+            const unsigned long long a = a0 + 4 * j;
+            *reinterpret_cast<unsigned*>(O.frames + (a - frames)) = *reinterpret_cast<const unsigned*>(src + (a - base));
+          } else if (j < n_head + n_body) {
+            const unsigned long long a = b0 + 16 * (j - n_head);
+            *reinterpret_cast<uint4*>(O.frames + (a - frames)) = *reinterpret_cast<const uint4*>(src + (a - base));
+          } else {
+            const unsigned long long a = b1 + 4 * (j - n_head - n_body);
+            *reinterpret_cast<unsigned*>(O.frames + (a - frames)) = *reinterpret_cast<const unsigned*>(src + (a - base));
+          }
+        }
+      }
+    }
+  }
+}
+
 }  // namespace
 }  // namespace daam
 
@@ -1202,7 +1418,7 @@ extern "C" int daam_expand_words(const float* global_maps, int32_t n_rows, int32
                            absolute, use_threshold, threshold, word_maps, out, scratch, stream);
 }
 
-// What daam_segment_words and daam_region_overlap share once their own pointers are checked: the word-list, map and
+// What daam_segment_words, daam_region_overlap and daam_overlay_words share once their own pointers are checked: the word-list, map and
 // size checks, `p` (all but labels / scores) and the shared memory of both launches (`*smem1`: one word map for
 // segment_minmax_kernel, `*smem2`: words_per_pass staged source windows for the tile kernel). Launches nothing.
 static int segment_prepare(const char* name, const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t mh,
@@ -1253,6 +1469,8 @@ static int segment_prepare(const char* name, const float* global_maps, int32_t n
       attr_err = cudaFuncSetAttribute(segment_label_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
     if (attr_err == cudaSuccess)
       attr_err = cudaFuncSetAttribute(region_tile_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+    if (attr_err == cudaSuccess)
+      attr_err = cudaFuncSetAttribute(overlay_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
   });
   DAAM_CUDA_TRY(attr_err);
   return DAAM_OK;
@@ -1316,6 +1534,39 @@ extern "C" int daam_region_overlap(const float* global_maps, int32_t n_maps, int
                                                                         intersection, word_area);
   DAAM_CUDA_TRY(cudaGetLastError());
   count_launch();
+  return DAAM_OK;
+}
+
+extern "C" int daam_overlay_words(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t mh, int32_t mw,
+                                  const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h,
+                                  int32_t out_w, int32_t absolute, int32_t use_threshold, float threshold,
+                                  int32_t color_normalize, float* word_maps, const uint8_t* image,
+                                  int64_t image_map_stride, uint8_t* frames, float* scratch, void* stream_) {
+  const char* name = "daam_overlay_words";
+  if (!global_maps || !rows || !row_begin || !word_maps || !image || !frames || !scratch || n_maps <= 0 || mh <= 0 ||
+      mw <= 0 || out_h <= 0 || out_w <= 0 || n_rows <= 0 || image_map_stride < 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
+  if ((uintptr_t)frames & 3) { set_error("%s: frames must be 4-byte aligned", name); return DAAM_E_INVALID; }
+  static thread_local OverlayParams p;
+  DeviceInfo dev;
+  size_t smem1, smem2;
+  // segment_minmax_kernel computes the min / max of v unless neither the normalisation nor the colour scale needs it
+  const int skip_minmax = absolute && !color_normalize;
+  if (int rc = segment_prepare(name, global_maps, n_maps, n_rows, mh, mw, rows, row_begin, n_words, out_h, out_w,
+                               skip_minmax, use_threshold, threshold, word_maps, scratch, p.s, &dev, &smem1, &smem2)) return rc;
+  p.image = image; p.image_map_stride = image_map_stride; p.frames = frames;
+  p.absolute = absolute ? 1 : 0; p.color_normalize = color_normalize ? 1 : 0; p.n_maps = n_maps;
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (int rc = launch_segment_minmax(p.s, n_maps, smem1, stream)) return rc;
+  const int tiles = ((out_h + kSegTileH - 1) / kSegTileH) * ((out_w + kSegTileW - 1) / kSegTileW);
+  overlay_kernel<<<dim3(tiles, n_maps), 256, smem2, stream>>>(p);
+  DAAM_CUDA_TRY(cudaGetLastError());
+  count_launch();
+  return DAAM_OK;
+}
+
+extern "C" int daam_jet_colormap(float* out) {
+  if (!out) { set_error("daam_jet_colormap: null pointer"); return DAAM_E_INVALID; }
+  DAAM_CUDA_TRY(cudaMemcpyFromSymbol(out, c_jet, sizeof(JetTable)));
   return DAAM_OK;
 }
 

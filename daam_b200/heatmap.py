@@ -17,6 +17,7 @@ from __future__ import annotations
 
 from dataclasses import dataclass
 from functools import lru_cache
+from types import SimpleNamespace
 from typing import Dict, Iterator, List, Optional, Set, Tuple
 
 import torch
@@ -430,6 +431,28 @@ class GlobalHeatMap:
         whms = [WordHeatMap(word_maps[0, i], w, idx) for i, (w, (_, idx)) in enumerate(zip(words, merged))]
         return whms, RegionOverlap(overlap.intersection[0], overlap.word_area[0], overlap.region_area)
 
+    def overlay_words(self, words, image, absolute: bool = False, threshold: Optional[float] = None,
+                      color_normalize: bool = True, word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
+        """The reference's ``plot_overlay`` (heatmap.py:20-53, 66-75) as pixels, for a word list: each word's expanded
+        map coloured with matplotlib's ``jet`` (autoscaled to the map's min / max with ``color_normalize``, else
+        clipped to [0, 1]) under the image drawn with alpha ``1 - heat``. With ``m`` the ``[len(words), H, W]`` that
+        ``expand_words(words, image, absolute, threshold, word_idx, offset_idx)`` returns, frame ``w`` is, per pixel and
+        channel, ``uint8(round((1 - a) * image + a * L[k]))`` with ``a = clamp(m[w], 0, 1)``, ``L`` the 256-entry table
+        of :func:`jet_colormap` and ``k`` the colour index of ``m[w]`` (every operation rounded in fp32). Two fused
+        launches; the ``[len(words), H, W]`` fp32 stack is never materialised.
+
+        ``image``: a PIL image (converted to RGB), or a numpy / torch ``uint8`` ``[H, W, 3]`` array (a torch one on the
+        CPU or on the heat map's device), ``(H, W)`` the size ``expand_words`` gives. Returns ``(word_heat_maps,
+        frames)``: the list of :class:`WordHeatMap` that :meth:`segment` returns and ``frames`` uint8 ``[len(words), H,
+        W, 3]`` (CPU by default, ``to_cpu=False`` keeps them on the device). At most 96 words; an empty list launches
+        nothing. Raises the reference's ``ValueError`` for a word that is not in the prompt."""
+        words = list(words)
+        word_maps, merged, frames = _overlay(self.tokenizer, self.prompt, self.heat_maps[None], words, image, absolute,
+                                             threshold, color_normalize, word_idx, offset_idx, to_cpu,
+                                             'GlobalHeatMap.overlay_words', stack=False)
+        whms = [WordHeatMap(word_maps[0, i], w, idx) for i, (w, (_, idx)) in enumerate(zip(words, merged))]
+        return whms, frames[0]
+
 
 def _word_rows(tokenizer, prompt: str, words: List[str], word_idx, offset_idx: int, n_rows: int):
     """``compute_token_merge_indices`` of every word (``word_idx`` may be a list parallel to ``words``), with the
@@ -545,6 +568,71 @@ def _to_cpu(ov: RegionOverlap) -> RegionOverlap:
     return RegionOverlap(ov.intersection.cpu(), ov.word_area.cpu(), ov.region_area.cpu())
 
 
+def jet_colormap() -> torch.Tensor:
+    """The fp32 ``[256, 3]`` table the overlay kernel colours with: ``L[k] = 255 * jet(k / 255)``, matplotlib's ``jet``
+    segment data evaluated in float64 and rounded once to fp32 (``L[0] = (0, 0, 127.5)``, ``L[255] = (127.5, 0, 0)``)."""
+    return _native.jet_colormap()
+
+
+def _overlay_image(image, n_maps: int, grid, dev, what: str, stack: bool):
+    """``(image, out_h, out_w, per_map)``: ``image`` as a uint8 ``[H, W, 3]`` or, for a stack, ``[n_maps, H, W, 3]``
+    tensor (not yet on the device), and the size the maps expand to over it."""
+    if isinstance(image, torch.Tensor):
+        arr = image
+    elif hasattr(image, 'convert') and hasattr(image, 'size'):           # PIL
+        import numpy as np
+        arr = torch.from_numpy(np.array(image.convert('RGB')))
+    elif hasattr(image, '__array_interface__'):                          # numpy
+        import numpy as np
+        arr = torch.from_numpy(np.ascontiguousarray(image))
+    else:
+        raise TypeError(f'{what}: image must be a PIL image or a uint8 [H, W, 3] numpy / torch array, not '
+                        f'{type(image).__name__}')
+    if arr.dtype != torch.uint8:
+        raise TypeError(f'{what}: image must be uint8, not {arr.dtype}')
+    if arr.device.type != 'cpu' and arr.device != dev:
+        raise ValueError(f'{what}: image is on {arr.device}, the heat maps on {dev}')
+    per_map = stack and arr.dim() == 4
+    if arr.dim() not in ((3, 4) if stack else (3,)) or (per_map and arr.shape[0] != n_maps):
+        want = f'[{n_maps}, H, W, 3] or [H, W, 3]' if stack else '[H, W, 3]'
+        raise ValueError(f'{what}: an image of shape {tuple(arr.shape)} is not {want}')
+    h, w = int(arr.shape[-3]), int(arr.shape[-2])
+    out_h, out_w = _image_size(SimpleNamespace(size=(w, h), height=h, width=w), *grid)
+    if tuple(arr.shape[-3:]) != (out_h, out_w, 3):
+        raise ValueError(f'{what}: an image of shape {tuple(arr.shape)} does not match the expanded maps\' '
+                         f'({out_h}, {out_w}, 3)' + (' (a square map keeps the reference\'s (size[0], size[1]) order, '
+                                                      'which transposes a non-square image)' if h != w else ''))
+    return arr, out_h, out_w, per_map
+
+
+def _overlay(tokenizer, prompt: str, maps: torch.Tensor, words, image, absolute, threshold, color_normalize, word_idx,
+             offset_idx: int, to_cpu: bool, what: str, stack: bool):
+    """``daam_overlay_words`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(word_maps, merged, frames)``: the
+    device word heat maps ``[n_maps, len(words), xh, xw]``, ``compute_token_merge_indices`` of every word, and
+    ``frames`` uint8 ``[n_maps, len(words), H, W, 3]``."""
+    n_maps, n_rows, grid = maps.shape[0], maps.shape[1], tuple(maps.shape[-2:])
+    merged = _word_rows(tokenizer, prompt, words, word_idx, offset_idx, n_rows)
+    _require_cuda(maps, what)
+    dev = maps.device
+    image, out_h, out_w, per_map = _overlay_image(image, n_maps, grid, dev, what, stack)
+    shape = (n_maps, len(words), out_h, out_w, 3)
+    word_maps = torch.empty((n_maps, len(words)) + grid, dtype=torch.float32, device=dev)
+    if not words or n_maps == 0:
+        frames = torch.empty(shape, dtype=torch.uint8, device='cpu' if to_cpu else dev)
+        return word_maps, merged, frames
+    image = image.to(dev).contiguous()                   # one copy to the device
+    maps = maps.detach().float().contiguous()
+    # the kernel writes whole 4-byte words: the frames are a view of a buffer rounded up to them
+    buf = torch.empty(_native.overlay_frames_bytes(*shape[:4]), dtype=torch.uint8, device=dev)
+    frames = buf[:n_maps * len(words) * out_h * out_w * 3].view(shape)
+    scratch = torch.empty(_native.segment_scratch_floats(n_maps, len(words)), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _native.overlay_words(maps.data_ptr(), n_maps, n_rows, grid, [rows for rows, _ in merged], out_h, out_w,
+                              absolute, threshold, color_normalize, word_maps.data_ptr(), image.data_ptr(),
+                              out_h * out_w * 3 if per_map else 0, buf.data_ptr(), scratch.data_ptr(), _stream_ptr(dev))
+    return word_maps, merged, (frames.cpu() if to_cpu else frames)
+
+
 class GlobalHeatMapStack:
     """Global heat maps of one prompt's text stacked along a first axis: ``heat_maps[t]`` is one
     ``[n_rows, xh, xw]`` map. Base of :class:`TimeHeatMaps` (one map per step) and :class:`ImageHeatMaps` (one per
@@ -601,6 +689,19 @@ class GlobalHeatMapStack:
                                                 regions, absolute, threshold, word_idx, offset_idx, to_cpu,
                                                 f'{type(self).__name__}.region_overlap')
         return word_maps, overlap
+
+    def overlay_words(self, words, image, absolute: bool = False, threshold: Optional[float] = None,
+                      color_normalize: bool = True, word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
+        """:meth:`GlobalHeatMap.overlay_words` for every map in one call (two launches whatever the map count): returns
+        ``(word_maps, frames)`` with ``word_maps`` the device ``[maps, len(words), xh, xw]`` word heat maps and
+        ``frames`` uint8 ``[maps, len(words), H, W, 3]``; row ``t`` equals ``self[t].overlay_words(...)`` byte for byte
+        (colour scale per map and word). ``image`` is one image for every map, or a uint8 ``[maps, H, W, 3]`` array
+        with one per map (e.g. the images of ``compute_image_heat_maps()``). ``frames[:, w]`` is word ``w`` forming over
+        a history, frame by frame."""
+        word_maps, _, frames = _overlay(self.tokenizer, self.prompt, self.heat_maps, list(words), image, absolute,
+                                        threshold, color_normalize, word_idx, offset_idx, to_cpu,
+                                        f'{type(self).__name__}.overlay_words', stack=True)
+        return word_maps, frames
 
 
 class TimeHeatMaps(GlobalHeatMapStack):

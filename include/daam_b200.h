@@ -33,7 +33,7 @@ extern "C" {
                                           daam_segment_words, daam_finalize_maps; daam_key_group.reserved is
                                           n_blocks; daam_accumulate takes 154- and 231-token contexts; layers with
                                           several prompts and a prompt stride <= 0 take the SIMT kernel;
-                                          daam_region_overlap) */
+                                          daam_region_overlap; daam_overlay_words, daam_jet_colormap) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_TOKENS 231     /* daam_accumulate: long contexts of 2 or 3 CLIP chunks of 77 tokens (154, 231) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
@@ -334,6 +334,39 @@ int daam_region_overlap(const float* global_maps, int32_t n_maps, int32_t n_rows
                         int32_t absolute, int32_t use_threshold, float threshold, float* word_maps,
                         const uint8_t* regions, int32_t n_regions, float* intersection, float* word_area, float* scratch,
                         void* stream);
+
+/*
+ * Heat-map overlays: the reference's plot_overlay (daam/heatmap.py:20-53, :66-75 -- the word map coloured with
+ * matplotlib's `jet` under the image drawn with alpha 1 - heat) as RGB pixels, for a word list on each of n_maps global
+ * maps stored back to back. With m[w] what daam_expand_words writes for word w with the same arguments, for every map,
+ * word, pixel and channel:
+ *   c   = color_normalize ? (hi == lo ? 0 : (m - lo) / (hi - lo)) : min(max(m, 0), 1)   (lo, hi: min / max of m[w])
+ *   k   = min(int(c * 256), 255)                              (matplotlib's Colormap with N = 256)
+ *   a   = min(max(m, 0), 1)
+ *   out = uint8(clamp(rne((1 - a) * image + a * L[k]), 0, 255))   (each operation rounded in fp32, no fused multiply-add)
+ * with L the table daam_jet_colormap returns.
+ * Arguments as daam_segment_words, plus color_normalize; image: device uint8 [out_h][out_w][3], map i's image at
+ * image + i * image_map_stride bytes (0: one image for every map); frames: device uint8
+ * [n_maps][n_words][out_h][out_w][3], 4-byte aligned, in a buffer of DAAM_OVERLAY_FRAMES_BYTES(...) bytes (the frames
+ * rounded up to whole 4-byte words: the bytes past them are overwritten); scratch: device, >=
+ * DAAM_SEGMENT_SCRATCH_FLOATS(n_maps, n_words) floats. Two launches whatever n_maps and n_words; the
+ * [n_words][out_h][out_w] fp32 stack is never written. Deterministic.
+ * Limits (DAAM_E_UNSUPPORTED): as daam_segment_words. DAAM_E_INVALID: as daam_segment_words, plus a negative
+ * image_map_stride or frames not 4-byte aligned.
+ */
+#define DAAM_OVERLAY_FRAMES_BYTES(n_maps, n_words, out_h, out_w)                                                      \
+  (((int64_t)(n_maps) * (n_words) * (out_h) * (out_w) * 3 + 3) / 4 * 4)
+int daam_overlay_words(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t map_h, int32_t map_w,
+                       const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w,
+                       int32_t absolute, int32_t use_threshold, float threshold, int32_t color_normalize,
+                       float* word_maps, const uint8_t* image, int64_t image_map_stride, uint8_t* frames,
+                       float* scratch, void* stream);
+
+/*
+ * The 256 x 3 colour table daam_overlay_words reads: L[k][ch] = fp32(255 * jet_ch(k / 255)), jet_ch evaluated in
+ * float64, piecewise linear through matplotlib's `jet` segment points. out: host fp32 [256][3].
+ */
+int daam_jet_colormap(float* out);
 
 /* Library / device introspection. */
 int daam_abi_version(void);
