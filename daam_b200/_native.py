@@ -330,58 +330,51 @@ def expand_as(map_ptr: int, x, out_h: int, out_w: int, absolute: bool, threshold
                                  ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
 
 
-def expand_words(maps_ptr: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int, out_w: int,
-                 absolute: bool, threshold: Optional[float], word_maps_ptr: Optional[int], out_ptr: int, scratch_ptr: int,
-                 stream: int):
-    """``rows_per_word[w]``: the rows of ``maps`` word ``w`` averages (already offset for SOS)."""
+def _word_list(x, rows_per_word: Sequence[Sequence[int]], out_h: int, out_w: int, absolute: bool,
+               threshold: Optional[float]):
+    """The arguments every word-list entry point takes after its map and row counts: ``h, w, rows, row_begin, n_words,
+    out_h, out_w, absolute, use_threshold, threshold``. ``rows_per_word[w]``: the rows word ``w`` averages (already
+    offset for SOS); word ``w`` owns ``rows[row_begin[w] .. row_begin[w + 1])``."""
     h, w = map_size(x)
-    rows_arr, begin_arr = _row_lists(rows_per_word)
-    use_thr = bool(threshold)   # the reference's `if threshold:` (daam/heatmap.py:87)
-    _check(load().daam_expand_words(ctypes.c_void_p(maps_ptr), n_rows, h, w, rows_arr, begin_arr,
-                                    len(rows_per_word), out_h, out_w, int(bool(absolute)), int(use_thr),
-                                    float(threshold) if use_thr else 0.0,
-                                    ctypes.c_void_p(word_maps_ptr) if word_maps_ptr else None,
-                                    ctypes.c_void_p(out_ptr), ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
-
-
-def _row_lists(rows_per_word: Sequence[Sequence[int]]):
-    """``(rows, row_begin)`` host arrays of a word list: word ``w`` owns ``rows[row_begin[w] .. row_begin[w + 1])``."""
     flat = [r for rows in rows_per_word for r in rows]
     begin = [0]
     for rows in rows_per_word:
         begin.append(begin[-1] + len(rows))
-    return (ctypes.c_int32 * max(len(flat), 1))(*flat), (ctypes.c_int32 * len(begin))(*begin)
+    use_thr = bool(threshold)   # the reference's `if threshold:` (daam/heatmap.py:87)
+    return (h, w, (ctypes.c_int32 * max(len(flat), 1))(*flat), (ctypes.c_int32 * len(begin))(*begin), len(rows_per_word),
+            out_h, out_w, int(bool(absolute)), int(use_thr), float(threshold) if use_thr else 0.0)
+
+
+def expand_words(maps_ptr: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int, out_w: int,
+                 absolute: bool, threshold: Optional[float], word_maps_ptr: Optional[int], out_ptr: int, scratch_ptr: int,
+                 stream: int):
+    """``daam_expand_words``; ``rows_per_word`` as for :func:`_word_list`."""
+    _check(load().daam_expand_words(ctypes.c_void_p(maps_ptr), n_rows,
+                                    *_word_list(x, rows_per_word, out_h, out_w, absolute, threshold),
+                                    ctypes.c_void_p(word_maps_ptr) if word_maps_ptr else None,
+                                    ctypes.c_void_p(out_ptr), ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
 
 
 def segment_words(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int,
                   out_w: int, absolute: bool, threshold: Optional[float], word_maps_ptr: int, labels_ptr: int,
                   scores_ptr: int, scratch_ptr: int, stream: int):
-    """``daam_segment_words`` over ``n_maps`` maps ``[n_rows, h, w]`` back to back; ``rows_per_word`` as for
-    :func:`expand_words`."""
-    h, w = map_size(x)
-    rows_arr, begin_arr = _row_lists(rows_per_word)
-    use_thr = bool(threshold)   # the reference's `if threshold:` (daam/heatmap.py:87), as expand_words resolves it
-    _check(load().daam_segment_words(ctypes.c_void_p(maps_ptr), n_maps, n_rows, h, w, rows_arr, begin_arr,
-                                     len(rows_per_word), out_h, out_w, int(bool(absolute)), int(use_thr),
-                                     float(threshold) if use_thr else 0.0, ctypes.c_void_p(word_maps_ptr),
-                                     ctypes.c_void_p(labels_ptr), ctypes.c_void_p(scores_ptr),
-                                     ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
+    """``daam_segment_words`` over ``n_maps`` maps ``[n_rows, h, w]`` back to back."""
+    _check(load().daam_segment_words(ctypes.c_void_p(maps_ptr), n_maps, n_rows,
+                                     *_word_list(x, rows_per_word, out_h, out_w, absolute, threshold),
+                                     ctypes.c_void_p(word_maps_ptr), ctypes.c_void_p(labels_ptr),
+                                     ctypes.c_void_p(scores_ptr), ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
 
 
 def region_overlap(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int,
                    out_w: int, absolute: bool, threshold: Optional[float], word_maps_ptr: int, regions_ptr: int,
                    n_regions: int, intersection_ptr: int, word_area_ptr: int, scratch_ptr: int, stream: int):
     """``daam_region_overlap`` over ``n_maps`` maps ``[n_rows, h, w]`` back to back and ``n_regions`` uint8 regions
-    ``[out_h, out_w]``; ``rows_per_word`` as for :func:`expand_words`."""
-    h, w = map_size(x)
-    rows_arr, begin_arr = _row_lists(rows_per_word)
-    use_thr = bool(threshold)   # the reference's `if threshold:` (daam/heatmap.py:87), as expand_words resolves it
-    _check(load().daam_region_overlap(ctypes.c_void_p(maps_ptr), n_maps, n_rows, h, w, rows_arr, begin_arr,
-                                      len(rows_per_word), out_h, out_w, int(bool(absolute)), int(use_thr),
-                                      float(threshold) if use_thr else 0.0, ctypes.c_void_p(word_maps_ptr),
-                                      ctypes.c_void_p(regions_ptr), n_regions, ctypes.c_void_p(intersection_ptr),
-                                      ctypes.c_void_p(word_area_ptr), ctypes.c_void_p(scratch_ptr),
-                                      ctypes.c_void_p(stream)))
+    ``[out_h, out_w]``."""
+    _check(load().daam_region_overlap(ctypes.c_void_p(maps_ptr), n_maps, n_rows,
+                                      *_word_list(x, rows_per_word, out_h, out_w, absolute, threshold),
+                                      ctypes.c_void_p(word_maps_ptr), ctypes.c_void_p(regions_ptr), n_regions,
+                                      ctypes.c_void_p(intersection_ptr), ctypes.c_void_p(word_area_ptr),
+                                      ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
 
 
 def overlay_words(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int,
@@ -389,15 +382,12 @@ def overlay_words(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Seq
                   image_ptr: int, image_map_stride: int, frames_ptr: int, scratch_ptr: int, stream: int):
     """``daam_overlay_words`` over ``n_maps`` maps ``[n_rows, h, w]`` back to back; ``image_ptr`` uint8 ``[out_h, out_w,
     3]``, map ``i``'s at ``image_ptr + i * image_map_stride`` bytes (0: one image for all); ``frames_ptr`` a buffer of
-    :func:`overlay_frames_bytes` bytes; ``rows_per_word`` as for :func:`expand_words`."""
-    h, w = map_size(x)
-    rows_arr, begin_arr = _row_lists(rows_per_word)
-    use_thr = bool(threshold)   # the reference's `if threshold:` (daam/heatmap.py:87), as expand_words resolves it
-    _check(load().daam_overlay_words(ctypes.c_void_p(maps_ptr), n_maps, n_rows, h, w, rows_arr, begin_arr,
-                                     len(rows_per_word), out_h, out_w, int(bool(absolute)), int(use_thr),
-                                     float(threshold) if use_thr else 0.0, int(bool(color_normalize)),
-                                     ctypes.c_void_p(word_maps_ptr), ctypes.c_void_p(image_ptr), image_map_stride,
-                                     ctypes.c_void_p(frames_ptr), ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
+    :func:`overlay_frames_bytes` bytes."""
+    _check(load().daam_overlay_words(ctypes.c_void_p(maps_ptr), n_maps, n_rows,
+                                     *_word_list(x, rows_per_word, out_h, out_w, absolute, threshold),
+                                     int(bool(color_normalize)), ctypes.c_void_p(word_maps_ptr),
+                                     ctypes.c_void_p(image_ptr), image_map_stride, ctypes.c_void_p(frames_ptr),
+                                     ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
 
 
 def jet_colormap():

@@ -1,0 +1,895 @@
+// Word-list kernels: a word's heat map (the mean of its rows of a global map), and one pipeline that takes a list of
+// words from the global map to image-size results without writing the [n_words][out_h][out_w] stack of expanded maps.
+//
+// Replaces GlobalHeatMap.compute_word_heat_map (daam/heatmap.py:121-123) and WordHeatMap.expand_as
+// (daam/heatmap.py:77-93) over a word list. Every consumer runs the same steps:
+//  1. word map: the gather-mean of the word's rows (word_mean) into shared memory;
+//  2. min / max of the bicubic-interpolated word map v over the image, per chunk of output pixels, then over the
+//     chunks in a fixed order (word_bounds in the tile kernels);
+//  3. the tile kernels stage the source window under a 16 x 64 output tile for a pass of words;
+//  4. per pixel: interpolate (bicubic.cuh), normalise and threshold: m = word_value(v), what expand_as returns.
+// The consumers differ only in what they do with m:
+//  - expand_words_kernel writes it (one cooperative launch, steps 1, 2 and 4 in one kernel);
+//  - segment_label_kernel keeps each pixel's max / argmax over the words;
+//  - region_tile_kernel sums it over binary image regions (then region_reduce_kernel);
+//  - overlay_kernel blends its jet colour onto the image.
+// The tile kernels run after segment_minmax_kernel (steps 1 and 2, the word maps and min / max partials to global
+// memory); region_tile_kernel and overlay_kernel share the tile helpers (block_tile, word_bounds, stage_windows, tap
+// tables). expand_words_kernel, segment_minmax_kernel and segment_label_kernel keep their steps inline: written with
+// the helpers, nvcc scheduled them differently and they measured slower. Every consumer's m is expand_words_kernel's
+// value bit for bit. Deterministic: no atomics.
+#include <cooperative_groups.h>
+#include <math.h>
+
+#include <algorithm>
+#include <mutex>
+
+#include "bicubic.cuh"
+#include "common.cuh"
+
+namespace daam {
+namespace {
+
+constexpr int kMaxRows = 128;                       // selected rows of daam_word_heat_map
+constexpr int kMaxWords = 96;
+constexpr int kMaxWordRows = 320;                   // selected rows over all words of a launch
+constexpr int kMaxChunks = 32;                      // min / max CTAs per word; scratch holds 2 floats per (word, chunk)
+constexpr int kMaxSmem = 200 * 1024;                // dynamic shared memory: a word map, or a tile kernel's windows
+constexpr int kSegTileH = 16, kSegTileW = 64;       // output tile of one tile-kernel CTA
+constexpr int kSegPix = kSegTileH * kSegTileW / 256;   // output pixels per thread
+constexpr int kSegStageFloats = 12288;              // staged windows per pass when they fit (48 KB)
+
+// The word map at pixel i: the mean of rows[r0 .. r1) of maps [*][xx] (heatmap.py:121-123). Every word map of this
+// file is built with it, so that they are the same bits.
+__device__ __forceinline__ float word_mean(const float* __restrict__ maps, const int* rows, int r0, int r1, int xx, int i) {
+  float s = 0.f;
+  for (int r = r0; r < r1; ++r) s += __ldg(maps + (long long)rows[r] * xx + i);
+  return s / (float)(r1 - r0);
+}
+
+struct RowSel {
+  int n;
+  int rows[kMaxRows];
+};
+
+__global__ void word_map_kernel(const float* __restrict__ maps, const __grid_constant__ RowSel sel, int xx,
+                                float* __restrict__ out) {
+  const int o = blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= xx) return;
+  out[o] = word_mean(maps, sel.rows, 0, sel.n, xx, o);
+}
+
+// What every word-list kernel reads; each kernel's params add its outputs.
+struct WordListParams {
+  const float* maps;                    // [n_maps][n_map_rows][mh][mw]
+  float* word_maps;                     // [n_maps][n_words][mh][mw] (optional for expand_words_kernel)
+  float* scratch;                       // min / max partials [n_maps][n_words][chunks][2]
+  long long map_stride;                 // n_map_rows * mh * mw
+  int mh, mw, oh, ow, n_words, chunks, absolute, use_threshold;
+  float threshold;
+  int words_per_pass;                   // tile kernels: words whose windows are staged at once
+  int minmax;                           // the min / max partials are computed and read
+  int row_begin[kMaxWords + 1];
+  int rows[kMaxWordRows];
+};
+
+// v at output pixel (oy, ox), from a whole word map
+__device__ __forceinline__ float word_map_at(const WordListParams& P, const float* wm, int oy, int ox) {
+  return bicubic_shared(wm, P.mw, make_taps(oy, P.mh, P.oh), make_taps(ox, P.mw, P.ow));
+}
+
+// expand_as's min-max normalisation (heatmap.py:88-89)
+__device__ __forceinline__ float minmax_normalize(float v, float lo, float hi) { return (v - lo) / (hi - lo + 1e-8f); }
+
+// v -> m, for a word whose v has min / max lo / hi
+__device__ __forceinline__ float word_value(const WordListParams& P, float v, float lo, float hi) {
+  if (!P.absolute) v = minmax_normalize(v, lo, hi);
+  if (P.use_threshold) v = v > P.threshold ? 1.f : 0.f;
+  return v;
+}
+
+// ---- expand: the word list's m written out ----------------------------------------------------------------------
+// CTA = (word, chunk of output pixels). The word map lives in shared memory; the min/max pass and the write pass both
+// interpolate from it (16 shared loads + 20 FMAs per pixel), so nothing but the final image is written and nothing is
+// read back. The chunks' min / max go through `scratch` across one grid-wide barrier; with `absolute` there is no
+// min/max pass and no barrier.
+struct ExpandParams {
+  WordListParams s;                     // one map
+  float* out;                           // [n_words][oh][ow]
+};
+
+__global__ void __launch_bounds__(256) expand_words_kernel(const __grid_constant__ ExpandParams E) {
+  const WordListParams& P = E.s;
+  extern __shared__ __align__(16) float wm[];          // the word map [mh][mw]
+  __shared__ float red_lo[8], red_hi[8];
+  const int word = blockIdx.x / P.chunks, chunk = blockIdx.x - word * P.chunks;
+  const int mh = P.mh, mw = P.mw, xx = mh * mw, n = P.oh * P.ow;
+  const int r0 = P.row_begin[word], r1 = P.row_begin[word + 1];
+  for (int i = threadIdx.x; i < xx; i += blockDim.x) {
+    const float s = word_mean(P.maps, P.rows, r0, r1, xx, i);
+    wm[i] = s;
+    if (chunk == 0 && P.word_maps) P.word_maps[(long long)word * xx + i] = s;
+  }
+  __syncthreads();
+  const int per = (n + P.chunks - 1) / P.chunks;
+  const int begin = chunk * per, end = min(n, begin + per);
+  float lo = 0.f, hi = 0.f;
+  if (!P.absolute) {
+    lo = INFINITY; hi = -INFINITY;
+    for (int o = begin + threadIdx.x; o < end; o += blockDim.x) {
+      const int oy = o / P.ow, ox = o - oy * P.ow;
+      const float v = bicubic_shared(wm, mw, make_taps(oy, mh, P.oh), make_taps(ox, mw, P.ow));
+      lo = fminf(lo, v); hi = fmaxf(hi, v);
+    }
+#pragma unroll
+    for (int s = 16; s > 0; s >>= 1) {
+      lo = fminf(lo, __shfl_xor_sync(0xffffffffu, lo, s));
+      hi = fmaxf(hi, __shfl_xor_sync(0xffffffffu, hi, s));
+    }
+    if ((threadIdx.x & 31) == 0) { red_lo[threadIdx.x >> 5] = lo; red_hi[threadIdx.x >> 5] = hi; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      for (int i = 1; i < (int)blockDim.x / 32; ++i) { lo = fminf(lo, red_lo[i]); hi = fmaxf(hi, red_hi[i]); }
+      float* slot = P.scratch + 2 * ((long long)word * P.chunks + chunk);
+      slot[0] = lo; slot[1] = hi;
+      __threadfence();
+    }
+    cooperative_groups::this_grid().sync();
+    if (threadIdx.x == 0) {
+      lo = INFINITY; hi = -INFINITY;
+      const volatile float* slots = P.scratch + 2 * (long long)word * P.chunks;
+      for (int c = 0; c < P.chunks; ++c) { lo = fminf(lo, slots[2 * c]); hi = fmaxf(hi, slots[2 * c + 1]); }
+      red_lo[0] = lo; red_hi[0] = hi;
+    }
+    __syncthreads();
+    lo = red_lo[0]; hi = red_hi[0];
+  }
+  float* dst = E.out + (long long)word * n;
+  for (int o = begin + threadIdx.x; o < end; o += blockDim.x) {
+    const int oy = o / P.ow, ox = o - oy * P.ow;
+    dst[o] = word_value(P, word_map_at(P, wm, oy, ox), lo, hi);
+  }
+}
+
+// ---- the tile kernels' first launch and the helpers they share ------------------------------------------------
+// grid: n_maps * n_words * chunks, CTA = (map, word, chunk of output pixels); dynamic smem: the word map [mh][mw].
+// Chunk 0 writes the word map; with `minmax` every chunk writes its min / max of v to `scratch`.
+__global__ void __launch_bounds__(256) segment_minmax_kernel(const __grid_constant__ WordListParams P) {
+  extern __shared__ __align__(16) float wm[];
+  __shared__ float red_lo[8], red_hi[8];
+  const int chunk = blockIdx.x % P.chunks, mword = blockIdx.x / P.chunks;   // mword = map * n_words + word
+  const int word = mword % P.n_words, map = mword / P.n_words;
+  const int mh = P.mh, mw = P.mw, xx = mh * mw, n = P.oh * P.ow;
+  const int r0 = P.row_begin[word], r1 = P.row_begin[word + 1];
+  const float* maps = P.maps + (long long)map * P.map_stride;
+  float* word_map = P.word_maps + (long long)mword * xx;
+  for (int i = threadIdx.x; i < xx; i += blockDim.x) {
+    const float s = word_mean(maps, P.rows, r0, r1, xx, i);
+    wm[i] = s;
+    if (chunk == 0) word_map[i] = s;
+  }
+  if (!P.minmax) return;
+  __syncthreads();
+  const int per = (n + P.chunks - 1) / P.chunks;
+  const int begin = chunk * per, end = min(n, begin + per);
+  float lo = INFINITY, hi = -INFINITY;
+  for (int o = begin + threadIdx.x; o < end; o += blockDim.x) {
+    const int oy = o / P.ow, ox = o - oy * P.ow;
+    const float v = bicubic_shared(wm, mw, make_taps(oy, mh, P.oh), make_taps(ox, mw, P.ow));
+    lo = fminf(lo, v); hi = fmaxf(hi, v);
+  }
+#pragma unroll
+  for (int s = 16; s > 0; s >>= 1) {
+    lo = fminf(lo, __shfl_xor_sync(0xffffffffu, lo, s));
+    hi = fmaxf(hi, __shfl_xor_sync(0xffffffffu, hi, s));
+  }
+  if ((threadIdx.x & 31) == 0) { red_lo[threadIdx.x >> 5] = lo; red_hi[threadIdx.x >> 5] = hi; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int i = 1; i < (int)blockDim.x / 32; ++i) { lo = fminf(lo, red_lo[i]); hi = fmaxf(hi, red_hi[i]); }
+    float* slot = P.scratch + 2 * ((long long)mword * P.chunks + chunk);
+    slot[0] = lo; slot[1] = hi;
+  }
+}
+
+// A tile kernel's CTA: output rows [y0, y0 + th) and columns [x0, x0 + tw) of map blockIdx.y, and the source window
+// [wy, wy + wh) x [wx, wx + ww) (wn floats) its taps read: taps move monotonically with the output index
+struct Tile {
+  int y0, x0, th, tw, wy, wx, wh, ww, wn;
+};
+
+__device__ __forceinline__ Tile block_tile(const WordListParams& P) {
+  const int tiles_x = (P.ow + kSegTileW - 1) / kSegTileW;
+  Tile t;
+  t.y0 = (blockIdx.x / tiles_x) * kSegTileH; t.x0 = (blockIdx.x % tiles_x) * kSegTileW;
+  t.th = min(kSegTileH, P.oh - t.y0); t.tw = min(kSegTileW, P.ow - t.x0);
+  t.wy = make_taps(t.y0, P.mh, P.oh).idx[0]; t.wx = make_taps(t.x0, P.mw, P.ow).idx[0];
+  t.wh = make_taps(t.y0 + t.th - 1, P.mh, P.oh).idx[3] - t.wy + 1;
+  t.ww = make_taps(t.x0 + t.tw - 1, P.mw, P.ow).idx[3] - t.wx + 1;
+  t.wn = t.wh * t.ww;
+  return t;
+}
+
+// min / max of v of (map, word w), reduced from segment_minmax_kernel's chunks in a fixed order; 0 / 0 without minmax
+__device__ __forceinline__ void word_bounds(const WordListParams& P, int map, int w, float& lo, float& hi) {
+  lo = 0.f; hi = 0.f;
+  if (!P.minmax) return;
+  const float* slots = P.scratch + 2 * ((long long)map * P.n_words + w) * P.chunks;
+  lo = INFINITY; hi = -INFINITY;
+  for (int c = 0; c < P.chunks; ++c) { lo = fminf(lo, slots[2 * c]); hi = fmaxf(hi, slots[2 * c + 1]); }
+}
+
+// The source windows of words [w0, w0 + nw) of `word_maps` (one map's) into `win`, one after the other. Barriers on
+// both sides: the previous pass has read `win`, and every thread sees this one.
+__device__ __forceinline__ void stage_windows(const WordListParams& P, const Tile& T, const float* word_maps, int w0,
+                                              int nw, float* win) {
+  __syncthreads();
+  for (int i = threadIdx.x; i < nw * T.wn; i += blockDim.x) {
+    const int wi = i / T.wn, r = i - wi * T.wn, y = r / T.ww, x = r - y * T.ww;
+    win[i] = __ldg(word_maps + ((long long)(w0 + wi) * P.mh + T.wy + y) * P.mw + T.wx + x);
+  }
+  __syncthreads();
+}
+
+// The tile's taps per output row and column, relative to the staged window: filled once per CTA (visible after the
+// first stage_windows), read back per pixel by tile_taps
+struct TapTables {
+  int yi[4][kSegTileH], xi[4][kSegTileW];
+  float yw[4][kSegTileH], xw[4][kSegTileW];
+};
+
+__device__ __forceinline__ void fill_tap_tables(const WordListParams& P, const Tile& T, TapTables& tt) {
+  if (threadIdx.x < T.th) {
+    const Taps t = make_taps(T.y0 + threadIdx.x, P.mh, P.oh);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) { tt.yi[j][threadIdx.x] = t.idx[j] - T.wy; tt.yw[j][threadIdx.x] = t.w[j]; }
+  } else if (threadIdx.x >= kSegTileH && threadIdx.x < kSegTileH + T.tw) {
+    const int x = threadIdx.x - kSegTileH;
+    const Taps t = make_taps(T.x0 + x, P.mw, P.ow);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) { tt.xi[j][x] = t.idx[j] - T.wx; tt.xw[j][x] = t.w[j]; }
+  }
+}
+
+__device__ __forceinline__ void tile_taps(const TapTables& tt, int py, int px, Taps& ty, Taps& tx) {
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    ty.idx[j] = tt.yi[j][py]; ty.w[j] = tt.yw[j][py]; tx.idx[j] = tt.xi[j][px]; tx.w[j] = tt.xw[j][px];
+  }
+}
+
+// ---- segmentation: a per-pixel word label -----------------------------------------------------------------------
+// labels[p] = 1 + argmax_w m[w][p] (lowest w on ties), or 0 where use_threshold and the max is not > threshold;
+// scores[p] = max_w m[w][p], with m[w] taken without threshold. Each pixel keeps the running max / argmax in registers
+// while the words are interpolated; its taps are computed per pixel.
+struct SegmentParams {
+  WordListParams s;
+  unsigned char* labels;                // [n_maps][oh][ow]
+  float* scores;                        // [n_maps][oh][ow]
+};
+
+// grid: (tiles of kSegTileH x kSegTileW output pixels, n_maps); dynamic smem: words_per_pass source windows
+__global__ void __launch_bounds__(256) segment_label_kernel(const __grid_constant__ SegmentParams S) {
+  const WordListParams& P = S.s;
+  extern __shared__ __align__(16) float win[];
+  __shared__ float s_lo[kMaxWords], s_hi[kMaxWords];
+  const int map = blockIdx.y, mh = P.mh, mw = P.mw, oh = P.oh, ow = P.ow, n_words = P.n_words;
+  const int tiles_x = (ow + kSegTileW - 1) / kSegTileW;
+  const int y0 = (blockIdx.x / tiles_x) * kSegTileH, x0 = (blockIdx.x % tiles_x) * kSegTileW;
+  const int th = min(kSegTileH, oh - y0), tw = min(kSegTileW, ow - x0);
+  // the source rows / columns the tile's taps read: taps move monotonically with the output index
+  const int wy = make_taps(y0, mh, oh).idx[0], wx = make_taps(x0, mw, ow).idx[0];
+  const int wh = make_taps(y0 + th - 1, mh, oh).idx[3] - wy + 1, ww = make_taps(x0 + tw - 1, mw, ow).idx[3] - wx + 1;
+  const int wn = wh * ww;
+  if (!P.absolute) {
+    for (int w = threadIdx.x; w < n_words; w += blockDim.x) {   // chunks in a fixed order
+      const float* slots = P.scratch + 2 * ((long long)map * n_words + w) * P.chunks;
+      float lo = INFINITY, hi = -INFINITY;
+      for (int c = 0; c < P.chunks; ++c) { lo = fminf(lo, slots[2 * c]); hi = fmaxf(hi, slots[2 * c + 1]); }
+      s_lo[w] = lo; s_hi[w] = hi;
+    }
+  }
+  const float* word_maps = P.word_maps + (long long)map * n_words * mh * mw;
+  float best[kSegPix];
+  int arg[kSegPix];
+#pragma unroll
+  for (int k = 0; k < kSegPix; ++k) { best[k] = -INFINITY; arg[k] = 0; }
+  for (int w0 = 0; w0 < n_words; w0 += P.words_per_pass) {
+    const int nw = min(P.words_per_pass, n_words - w0);
+    __syncthreads();                                   // the previous pass has read its windows
+    for (int i = threadIdx.x; i < nw * wn; i += blockDim.x) {
+      const int wi = i / wn, r = i - wi * wn, y = r / ww, x = r - y * ww;
+      win[i] = __ldg(word_maps + ((long long)(w0 + wi) * mh + wy + y) * mw + wx + x);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < kSegPix; ++k) {
+      const int p = threadIdx.x + 256 * k;
+      if (p < th * tw) {
+        const int py = p / tw;
+        Taps ty = make_taps(y0 + py, mh, oh), tx = make_taps(x0 + p - py * tw, mw, ow);
+#pragma unroll
+        for (int j = 0; j < 4; ++j) { ty.idx[j] -= wy; tx.idx[j] -= wx; }
+        for (int wi = 0; wi < nw; ++wi) {
+          const int w = w0 + wi;
+          float v = bicubic_shared(win + wi * wn, ww, ty, tx);
+          if (!P.absolute) v = minmax_normalize(v, s_lo[w], s_hi[w]);
+          if (w == 0 || v > best[k]) { best[k] = v; arg[k] = w; }   // strict: the lowest word wins a tie
+        }
+      }
+    }
+  }
+  const long long base = (long long)map * oh * ow;
+#pragma unroll
+  for (int k = 0; k < kSegPix; ++k) {
+    const int p = threadIdx.x + 256 * k;
+    if (p < th * tw) {
+      const int py = p / tw;
+      const long long o = base + (long long)(y0 + py) * ow + x0 + p - py * tw;
+      S.scores[o] = best[k];
+      S.labels[o] = (!P.use_threshold || best[k] > P.threshold) ? (unsigned char)(arg[k] + 1) : (unsigned char)0;
+    }
+  }
+}
+
+// ---- word-region overlap: sums of m over binary image regions ---------------------------------------------------
+// With R[r] = (regions[r] != 0):
+//   intersection[map][r][w] = sum_p R[r](p) m[w](p),   word_area[map][w] = sum_p m[w](p)
+// region_tile_kernel reduces every (word, slot) over its tile in a fixed order -- slot 0 is the word's area, slot 1 + r
+// its sum inside region r -- into one partial per tile; region_reduce_kernel sums the tiles' partials in a fixed order.
+// With a threshold every value is 0 or 1 and every partial an integer below 2^24, so the sums are exact counts.
+constexpr int kMaxRegions = DAAM_REGION_MAX_REGIONS;   // 63 + the area slot: 64 slots per word, two groups of 32
+constexpr int kRegionSlots = kMaxRegions + 1;
+
+struct RegionParams {
+  WordListParams s;
+  const unsigned char* regions;         // [n_regions][oh][ow]
+  float* partials;                      // [n_maps][n_words][n_regions + 1][tiles]
+  int n_regions, tiles;
+};
+
+// Lane l returns the warp's sum of s[l]. Five halving exchange rounds (31 shuffles for 32 values); the order of every
+// add is fixed.
+// One round: lanes with bit H set keep s[H .. 2H), the others s[0 .. H); each sends the other half to lane ^ H. The
+// round count is a template argument so that every index is a constant and s[] stays in registers.
+template <int H>
+__device__ __forceinline__ void reduce_scatter_round(float (&s)[32], int lane) {
+  const bool upper = (lane & H) != 0;
+#pragma unroll
+  for (int i = 0; i < H; ++i) {
+    const float send = upper ? s[i] : s[i + H];
+    const float keep = upper ? s[i + H] : s[i];
+    s[i] = keep + __shfl_xor_sync(0xffffffffu, send, H);
+  }
+}
+
+__device__ __forceinline__ float warp_reduce_scatter32(float (&s)[32]) {
+  const int lane = threadIdx.x & 31;
+  reduce_scatter_round<16>(s, lane);
+  reduce_scatter_round<8>(s, lane);
+  reduce_scatter_round<4>(s, lane);
+  reduce_scatter_round<2>(s, lane);
+  reduce_scatter_round<1>(s, lane);
+  return s[0];
+}
+
+// grid: (tiles of kSegTileH x kSegTileW output pixels, n_maps); dynamic smem: words_per_pass source windows
+__global__ void __launch_bounds__(256) region_tile_kernel(const __grid_constant__ RegionParams R) {
+  extern __shared__ __align__(16) float win[];
+  __shared__ float s_lo[kMaxWords], s_hi[kMaxWords];
+  __shared__ float red[2][8][kRegionSlots];          // per-warp sums of a word, double-buffered across words
+  __shared__ TapTables taps;
+  const WordListParams& P = R.s;
+  const int map = blockIdx.y, oh = P.oh, ow = P.ow, n_words = P.n_words;
+  const Tile T = block_tile(P);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int n_slots = R.n_regions + 1;
+  for (int w = threadIdx.x; w < n_words; w += blockDim.x) word_bounds(P, map, w, s_lo[w], s_hi[w]);
+  fill_tap_tables(P, T, taps);
+  // slot bits of the thread's pixels: bit j of mask[g][k] says pixel k counts towards slot 32 g + j (slot 0: every
+  // pixel of the tile, slot 1 + r: the pixels inside region r); each region byte is read once
+  const long long n = (long long)oh * ow;
+  unsigned mask[2][kSegPix];
+#pragma unroll
+  for (int k = 0; k < kSegPix; ++k) {
+    const int p = threadIdx.x + 256 * k;
+    mask[0][k] = 0u; mask[1][k] = 0u;
+    if (p < T.th * T.tw) {
+      const int py = p / T.tw;
+      const unsigned char* reg = R.regions + (long long)(T.y0 + py) * ow + T.x0 + p - py * T.tw;
+      unsigned m0 = 1u, m1 = 0u;
+      for (int r = 0; r < R.n_regions; ++r) {
+        const unsigned bit = __ldg(reg + r * n) != 0 ? 1u : 0u;
+        if (r < 31) m0 |= bit << (r + 1); else m1 |= bit << (r - 31);
+      }
+      mask[0][k] = m0; mask[1][k] = m1;
+    }
+  }
+  const float* word_maps = P.word_maps + (long long)map * n_words * P.mh * P.mw;
+  float* partials = R.partials + (long long)map * n_words * n_slots * R.tiles + blockIdx.x;
+  for (int w0 = 0; w0 < n_words; w0 += P.words_per_pass) {
+    const int nw = min(P.words_per_pass, n_words - w0);
+    stage_windows(P, T, word_maps, w0, nw, win);
+    for (int wi = 0; wi < nw; ++wi) {
+      const int w = w0 + wi;
+      float v[kSegPix];
+#pragma unroll
+      for (int k = 0; k < kSegPix; ++k) {
+        const int p = threadIdx.x + 256 * k;
+        v[k] = 0.f;
+        if (p < T.th * T.tw) {
+          const int py = p / T.tw;
+          Taps ty, tx;
+          tile_taps(taps, py, p - py * T.tw, ty, tx);
+          v[k] = word_value(P, bicubic_shared(win + wi * T.wn, T.ww, ty, tx), s_lo[w], s_hi[w]);
+        }
+      }
+      float (*buf)[kRegionSlots] = red[w & 1];
+#pragma unroll
+      for (int g = 0; g < 2; ++g) {
+        if (g * 32 < n_slots) {
+          float s[32];
+#pragma unroll
+          for (int j = 0; j < 32; ++j) {
+            float a = 0.f;
+#pragma unroll
+            for (int k = 0; k < kSegPix; ++k) a += (mask[g][k] >> j) & 1u ? v[k] : 0.f;
+            s[j] = a;
+          }
+          buf[warp][32 * g + lane] = warp_reduce_scatter32(s);
+        }
+      }
+      // one barrier per word: red[w & 1] is rewritten two words later, after every warp has passed the next barrier
+      __syncthreads();
+      if (warp == (w & 7)) {
+        for (int slot = lane; slot < n_slots; slot += 32) {
+          float a = 0.f;
+#pragma unroll
+          for (int i = 0; i < 8; ++i) a += buf[i][slot];
+          partials[((long long)w * n_slots + slot) * R.tiles] = a;
+        }
+      }
+    }
+  }
+}
+
+// grid: ceil(n_out / 8), 256 threads; one warp per output o = (map * n_words + word) * (n_regions + 1) + slot sums
+// the tiles' partials (lane-strided, then a butterfly) in a fixed order
+__global__ void __launch_bounds__(256) region_reduce_kernel(const float* __restrict__ partials, long long n_out,
+                                                            int tiles, int n_words, int n_regions,
+                                                            float* __restrict__ intersection, float* __restrict__ area) {
+  const long long o = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (o >= n_out) return;                              // whole warps
+  const int lane = threadIdx.x & 31;
+  const float* src = partials + o * tiles;
+  float s = 0.f;
+  for (int t = lane; t < tiles; t += 32) s += __ldg(src + t);
+#pragma unroll
+  for (int h = 16; h > 0; h >>= 1) s += __shfl_xor_sync(0xffffffffu, s, h);
+  if (lane == 0) {
+    const int n_slots = n_regions + 1;
+    const int slot = (int)(o % n_slots);
+    const long long mword = o / n_slots;               // map * n_words + word
+    if (slot == 0) {
+      area[mword] = s;
+    } else {
+      const long long map = mword / n_words, word = mword - map * n_words;
+      intersection[(map * n_regions + slot - 1) * n_words + word] = s;
+    }
+  }
+}
+
+// ---- heat-map overlays: the jet-coloured m blended onto the image -----------------------------------------------
+// The reference's plot_overlay (heatmap.py:20-53, 66-75) as pixels: for every byte of frames [n_maps][n_words][oh][ow][3]:
+//   c = color_normalize ? (hi == lo ? 0 : (m - lo) / (hi - lo)) : clamp(m, 0, 1)   (lo / hi: min / max of m[w])
+//   k = min(int(c * 256), 255)                                                      (matplotlib's Colormap, N = 256)
+//   a = clamp(m, 0, 1)                                                              (the image drawn with alpha 1 - a)
+//   out = uint8(clamp(rne((1 - a) * image + a * jet[k]), 0, 255))                   (every operation rounded in fp32)
+// v -> m is monotone non-decreasing in fp32 (subtract, divide by a positive constant, `>` threshold), so lo / hi of m
+// are m at the min / max of v: no pass over m. Every word's RGB bytes go through shared memory to aligned 4- and
+// 16-byte stores. A 4-byte word of frames belongs to the CTA that owns its first byte; when it reaches past the tile
+// row, that CTA computes the one next pixel in memory order (the next tile, row, word or map) from the global word
+// maps, with the same arithmetic.
+
+// matplotlib's `jet` segment data (_cm.py): piecewise linear through (x, y) in each channel
+struct JetSegments { int n; double x[6], y[6]; };
+constexpr JetSegments kJet[3] = {
+    {5, {0., 0.35, 0.66, 0.89, 1.}, {0., 0., 1., 1., 0.5}},
+    {6, {0., 0.125, 0.375, 0.64, 0.91, 1.}, {0., 0., 1., 1., 0., 0.}},
+    {5, {0., 0.11, 0.34, 0.65, 1.}, {0.5, 1., 1., 0., 0.}},
+};
+
+constexpr double jet_channel(int ch, double x) {
+  const JetSegments& s = kJet[ch];
+  int i = 0;
+  while (i + 2 < s.n && x > s.x[i + 1]) ++i;
+  const double t = (x - s.x[i]) / (s.x[i + 1] - s.x[i]);
+  const double d = (s.y[i + 1] - s.y[i]) * t;
+  return s.y[i] + d;
+}
+
+struct JetTable { float v[256 * 3]; };
+constexpr JetTable make_jet_table() {
+  JetTable t{};
+  for (int k = 0; k < 256; ++k)
+    for (int ch = 0; ch < 3; ++ch) t.v[3 * k + ch] = (float)(255.0 * jet_channel(ch, k / 255.0));
+  return t;
+}
+constexpr JetTable kJetTable = make_jet_table();
+static_assert(kJetTable.v[0] == 0.f && kJetTable.v[1] == 0.f && kJetTable.v[2] == 127.5f, "jet(0) = (0, 0, 0.5)");
+static_assert(kJetTable.v[765] == 127.5f && kJetTable.v[766] == 0.f && kJetTable.v[767] == 0.f, "jet(1) = (0.5, 0, 0)");
+
+// L[k][ch] = fp32(255 * jet_ch(k / 255)): the one copy of the table; daam_jet_colormap reads it back
+__constant__ JetTable c_jet = kJetTable;
+
+constexpr int kOverlayRowBytes = 16 + 3 * kSegTileW + 16;   // a tile row's bytes from its 16-byte aligned base, + 1 pixel
+
+struct OverlayParams {
+  WordListParams s;                     // minmax also when only color_normalize needs it
+  const unsigned char* image;           // [oh][ow][3], map i at image + i * image_map_stride
+  long long image_map_stride;           // bytes; 0: one image for every map
+  unsigned char* frames;                // [n_maps][n_words][oh][ow][3], 4-byte aligned, padded to a 4-byte multiple
+  int color_normalize, n_maps;
+};
+
+// one pixel's three bytes from m, the word's lo / hi of m, the image pixel and the staged table
+__device__ __forceinline__ void overlay_rgb(float m, float lo, float hi, int color_normalize, const unsigned char* im,
+                                            const float* lut, unsigned char* out) {
+  float c;
+  if (color_normalize) c = hi == lo ? 0.f : __fdiv_rn(__fsub_rn(m, lo), __fsub_rn(hi, lo));
+  else c = fminf(fmaxf(m, 0.f), 1.f);
+  const int k = min((int)__fmul_rn(c, 256.f), 255);
+  const float a = fminf(fmaxf(m, 0.f), 1.f), na = __fsub_rn(1.f, a);
+#pragma unroll
+  for (int ch = 0; ch < 3; ++ch) {
+    const float v = __fadd_rn(__fmul_rn(na, (float)im[ch]), __fmul_rn(a, lut[3 * k + ch]));
+    out[ch] = (unsigned char)min(max(__float2int_rn(v), 0), 255);
+  }
+}
+
+// The bytes of output pixel (oy, ox) of (map, word), computed from the global word map: the same taps and
+// bicubic_shared over the whole map as the tile path over its staged window. Zeros past the last map.
+__device__ void overlay_pixel_global(const OverlayParams& O, const float* lut, int map, int w, int oy, int ox,
+                                     unsigned char* out) {
+  const WordListParams& P = O.s;
+  if (map >= O.n_maps) { out[0] = out[1] = out[2] = 0; return; }
+  float vlo, vhi;
+  word_bounds(P, map, w, vlo, vhi);
+  const float lo = word_value(P, vlo, vlo, vhi), hi = word_value(P, vhi, vlo, vhi);
+  const float v = word_map_at(P, P.word_maps + ((long long)map * P.n_words + w) * P.mh * P.mw, oy, ox);
+  const unsigned char* im = O.image + map * O.image_map_stride + ((long long)oy * P.ow + ox) * 3;
+  const unsigned char px[3] = {__ldg(im), __ldg(im + 1), __ldg(im + 2)};
+  overlay_rgb(word_value(P, v, vlo, vhi), lo, hi, O.color_normalize, px, lut, out);
+}
+
+// grid: (tiles of kSegTileH x kSegTileW output pixels, n_maps); dynamic smem: words_per_pass source windows
+__global__ void __launch_bounds__(256) overlay_kernel(const __grid_constant__ OverlayParams O) {
+  extern __shared__ __align__(16) float win[];
+  __shared__ float s_vlo[kMaxWords], s_vhi[kMaxWords], s_lo[kMaxWords], s_hi[kMaxWords];
+  __shared__ TapTables taps;
+  __shared__ float lut[256 * 3];
+  __shared__ unsigned char img[kSegTileH * kSegTileW * 3];
+  __shared__ __align__(16) unsigned char rows[2][kSegTileH][kOverlayRowBytes];   // double-buffered across words
+  const WordListParams& P = O.s;
+  const int map = blockIdx.y, oh = P.oh, ow = P.ow, n_words = P.n_words;
+  const Tile T = block_tile(P);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  for (int w = threadIdx.x; w < n_words; w += blockDim.x) {
+    float vlo, vhi;
+    word_bounds(P, map, w, vlo, vhi);
+    s_vlo[w] = vlo; s_vhi[w] = vhi;
+    s_lo[w] = word_value(P, vlo, vlo, vhi); s_hi[w] = word_value(P, vhi, vlo, vhi);
+  }
+  for (int i = threadIdx.x; i < 256 * 3; i += blockDim.x) lut[i] = c_jet.v[i];
+  fill_tap_tables(P, T, taps);
+  // the tile's image bytes, read once for every word
+  const unsigned char* image = O.image + map * O.image_map_stride;
+  for (int i = threadIdx.x; i < T.th * T.tw * 3; i += blockDim.x) {
+    const int r = i / (T.tw * 3), b = i - r * T.tw * 3;
+    img[i] = __ldg(image + ((long long)(T.y0 + r) * ow + T.x0) * 3 + b);
+  }
+  const float* word_maps = P.word_maps + (long long)map * n_words * P.mh * P.mw;
+  const unsigned long long frames = (unsigned long long)O.frames;   // byte addresses: the alignment of the stores
+  for (int w0 = 0; w0 < n_words; w0 += P.words_per_pass) {
+    const int nw = min(P.words_per_pass, n_words - w0);
+    stage_windows(P, T, word_maps, w0, nw, win);
+    for (int wi = 0; wi < nw; ++wi) {
+      const int w = w0 + wi;
+      const float vlo = s_vlo[w], vhi = s_vhi[w], lo = s_lo[w], hi = s_hi[w];
+      // row py of the tile starts at byte g0(py) of frames; rows[w & 1][py][g0 & 15] holds that byte
+      const long long row0 = (((long long)map * n_words + w) * oh + T.y0) * ow + T.x0;
+#pragma unroll
+      for (int k = 0; k < kSegPix; ++k) {
+        const int p = threadIdx.x + 256 * k;
+        if (p < T.th * T.tw) {
+          const int py = p / T.tw, px = p - py * T.tw;
+          Taps ty, tx;
+          tile_taps(taps, py, px, ty, tx);
+          const float m = word_value(P, bicubic_shared(win + wi * T.wn, T.ww, ty, tx), vlo, vhi);
+          const unsigned shift = (unsigned)((frames + 3 * (row0 + (long long)py * ow)) & 15);
+          overlay_rgb(m, lo, hi, O.color_normalize, img + 3 * p, lut, &rows[w & 1][py][shift + 3 * px]);
+        }
+      }
+      // a row whose last 4-byte word reaches past it: the next pixel in memory order
+      if (threadIdx.x < T.th) {
+        const int py = threadIdx.x;
+        const unsigned long long g1 = frames + 3 * (row0 + (long long)py * ow + T.tw);
+        if (g1 & 3) {
+          int nm = map, nwd = w, ny = T.y0 + py, nx = T.x0 + T.tw;
+          if (nx == ow) { nx = 0; ++ny; }
+          if (ny == oh) { ny = 0; ++nwd; }
+          if (nwd == n_words) { nwd = 0; ++nm; }
+          const unsigned shift = (unsigned)((g1 - 3 * T.tw) & 15);
+          overlay_pixel_global(O, lut, nm, nwd, ny, nx, &rows[w & 1][py][shift + 3 * T.tw]);
+        }
+      }
+      // one barrier per word: rows[w & 1] is rewritten two words later, after every warp has passed the next barrier
+      __syncthreads();
+      for (int py = warp; py < T.th; py += 8) {
+        const unsigned long long g0 = frames + 3 * (row0 + (long long)py * ow), g1 = g0 + 3 * T.tw;
+        const unsigned long long base = g0 & ~15ull, a0 = (g0 + 3) & ~3ull, a1 = (g1 + 3) & ~3ull;
+        // the owned words [a0, a1): 4-byte words up to a 16-byte boundary, 16-byte stores, 4-byte words
+        const unsigned long long b0 = min((a0 + 15) & ~15ull, a1), b1 = max(b0, a1 & ~15ull);
+        const int n_head = (int)((b0 - a0) >> 2), n_body = (int)((b1 - b0) >> 4), n_tail = (int)((a1 - b1) >> 2);
+        const unsigned char* src = rows[w & 1][py];
+        for (int j = lane; j < n_head + n_body + n_tail; j += 32) {
+          if (j < n_head) {
+            const unsigned long long a = a0 + 4 * j;
+            *reinterpret_cast<unsigned*>(O.frames + (a - frames)) = *reinterpret_cast<const unsigned*>(src + (a - base));
+          } else if (j < n_head + n_body) {
+            const unsigned long long a = b0 + 16 * (j - n_head);
+            *reinterpret_cast<uint4*>(O.frames + (a - frames)) = *reinterpret_cast<const uint4*>(src + (a - base));
+          } else {
+            const unsigned long long a = b1 + 4 * (j - n_head - n_body);
+            *reinterpret_cast<unsigned*>(O.frames + (a - frames)) = *reinterpret_cast<const unsigned*>(src + (a - base));
+          }
+        }
+      }
+    }
+  }
+}
+
+}  // namespace
+}  // namespace daam
+
+using namespace daam;
+
+extern "C" int daam_word_heat_map(const float* global_maps, int32_t n_rows, int32_t mh, int32_t mw, const int32_t* rows,
+                                  int32_t n_sel, float* out, void* stream_) {
+  if (!global_maps || !rows || !out || mh <= 0 || mw <= 0 || n_sel <= 0) { set_error("daam_word_heat_map: null pointer or empty selection"); return DAAM_E_INVALID; }
+  if (n_sel > kMaxRows) { set_error("daam_word_heat_map: %d rows > %d", n_sel, kMaxRows); return DAAM_E_UNSUPPORTED; }
+  DeviceInfo dev;
+  if (int rc = get_device_info(&dev)) return rc;
+  RowSel sel;
+  sel.n = n_sel;
+  for (int i = 0; i < n_sel; ++i) {
+    int r = rows[i];
+    if (r < 0) r += n_rows;   // torch-style negative index
+    if (r < 0 || r >= n_rows) { set_error("daam_word_heat_map: row %d out of range [0, %d)", rows[i], n_rows); return DAAM_E_INVALID; }
+    sel.rows[i] = r;
+  }
+  const int xx = mh * mw;
+  word_map_kernel<<<(xx + 255) / 256, 256, 0, static_cast<cudaStream_t>(stream_)>>>(global_maps, sel, xx, out);
+  DAAM_CUDA_TRY(cudaGetLastError());
+  count_launch();
+  return DAAM_OK;
+}
+
+// The word-list checks every word-list entry point makes once its own pointers and sizes are checked, in the order
+// they are reported, then `p` from the arguments (one chunk). `tiled`: the tile entry points' limits of 65535 maps
+// and 2^30 output pixels, checked before the device is queried.
+static int word_list_prepare(const char* name, const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t mh,
+                             int32_t mw, const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h,
+                             int32_t out_w, int32_t absolute, bool minmax, int32_t use_threshold, float threshold,
+                             float* word_maps, float* scratch, bool tiled, WordListParams& p, DeviceInfo* dev) {
+  if (n_words <= 0) { set_error("%s: empty word list", name); return DAAM_E_INVALID; }
+  if (n_words > kMaxWords) { set_error("%s: %d words > %d", name, n_words, kMaxWords); return DAAM_E_UNSUPPORTED; }
+  if (row_begin[0] != 0 || row_begin[n_words] > kMaxWordRows) { set_error("%s: row_begin must start at 0 and select at most %d rows", name, kMaxWordRows); return DAAM_E_UNSUPPORTED; }
+  if ((size_t)mh * mw * sizeof(float) > kMaxSmem) { set_error("%s: a %d x %d map does not fit shared memory", name, mh, mw); return DAAM_E_UNSUPPORTED; }
+  if (tiled && n_maps > 65535) { set_error("%s: %d maps > 65535", name, n_maps); return DAAM_E_UNSUPPORTED; }
+  if (tiled && (long long)out_h * out_w > (1LL << 30)) { set_error("%s: a %d x %d output is more than 2^30 pixels", name, out_h, out_w); return DAAM_E_UNSUPPORTED; }
+  if (int rc = get_device_info(dev)) return rc;
+  for (int w = 0; w < n_words; ++w) {
+    if (row_begin[w + 1] <= row_begin[w]) { set_error("%s: word %d selects no row", name, w); return DAAM_E_INVALID; }
+    p.row_begin[w] = row_begin[w];
+  }
+  p.row_begin[n_words] = row_begin[n_words];
+  for (int i = 0; i < row_begin[n_words]; ++i) {
+    int r = rows[i];
+    if (r < 0) r += n_rows;   // torch-style negative index
+    if (r < 0 || r >= n_rows) { set_error("%s: row %d out of range [0, %d)", name, rows[i], n_rows); return DAAM_E_INVALID; }
+    p.rows[i] = r;
+  }
+  p.maps = global_maps; p.word_maps = word_maps; p.scratch = scratch;
+  p.map_stride = (long long)n_rows * mh * mw;
+  p.mh = mh; p.mw = mw; p.oh = out_h; p.ow = out_w; p.n_words = n_words; p.chunks = 1; p.words_per_pass = 1;
+  p.absolute = absolute ? 1 : 0; p.use_threshold = use_threshold ? 1 : 0; p.threshold = threshold;
+  p.minmax = minmax ? 1 : 0;
+  return DAAM_OK;
+}
+
+static int launch_expand_words(ExpandParams& p, const DeviceInfo& dev, cudaStream_t stream) {
+  const size_t smem = (size_t)p.s.mh * p.s.mw * sizeof(float);
+  static std::mutex mu;
+  static size_t configured_dev[64] = {};
+  static int blocks_per_sm[64] = {};
+  int per_sm;
+  {
+    std::lock_guard<std::mutex> lock(mu);
+    size_t& configured = configured_dev[dev.device & 63];
+    if (smem > configured) {
+      if (smem > 48 * 1024)
+        DAAM_CUDA_TRY(cudaFuncSetAttribute(expand_words_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      configured = smem;
+      blocks_per_sm[dev.device & 63] = 0;
+    }
+    if (blocks_per_sm[dev.device & 63] == 0) {
+      int occ = 0;
+      DAAM_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, expand_words_kernel, 256, configured));
+      blocks_per_sm[dev.device & 63] = occ < 1 ? 1 : occ;
+    }
+    per_sm = blocks_per_sm[dev.device & 63];
+  }
+  const int capacity = per_sm * dev.sm_count;          // a cooperative grid must be co-resident
+  const int n = p.s.oh * p.s.ow;
+  int done = 0;
+  const int total = p.s.n_words;
+  ExpandParams q = p;
+  while (done < total) {                                // more words than the device holds at once: several launches
+    const int batch = total - done < capacity ? total - done : capacity;
+    int chunks = capacity / batch;
+    if (chunks > kMaxChunks) chunks = kMaxChunks;
+    if (chunks > (n + 255) / 256) chunks = (n + 255) / 256;
+    if (chunks < 1) chunks = 1;
+    q.s.n_words = batch;
+    q.s.chunks = chunks;
+    q.out = p.out + (long long)done * n;
+    q.s.word_maps = p.s.word_maps ? p.s.word_maps + (long long)done * p.s.mh * p.s.mw : nullptr;
+    q.s.scratch = p.s.scratch + 2LL * kMaxChunks * done;
+    for (int i = 0; i <= batch; ++i) q.s.row_begin[i] = p.s.row_begin[done + i];
+    void* args[] = {&q};
+    DAAM_CUDA_TRY(cudaLaunchCooperativeKernel((const void*)expand_words_kernel, dim3(batch * chunks), dim3(256), args, smem,
+                                              stream));
+    count_launch();
+    done += batch;
+  }
+  return DAAM_OK;
+}
+
+// behind daam_expand_words and daam_expand_as; `name` is the entry point that was called
+static int expand_words_impl(const char* name, const float* global_maps, int32_t n_rows, int32_t mh, int32_t mw,
+                             const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w,
+                             int32_t absolute, int32_t use_threshold, float threshold, float* word_maps, float* out,
+                             float* scratch, void* stream) {
+  if (!global_maps || !rows || !row_begin || !out || !scratch || mh <= 0 || mw <= 0 || out_h <= 0 || out_w <= 0 || n_rows <= 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
+  static thread_local ExpandParams p;
+  DeviceInfo dev;
+  if (int rc = word_list_prepare(name, global_maps, 1, n_rows, mh, mw, rows, row_begin, n_words, out_h, out_w, absolute,
+                                 !absolute, use_threshold, threshold, word_maps, scratch, false, p.s, &dev)) return rc;
+  p.out = out;
+  return launch_expand_words(p, dev, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int daam_expand_words(const float* global_maps, int32_t n_rows, int32_t mh, int32_t mw, const int32_t* rows,
+                                 const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w,
+                                 int32_t absolute, int32_t use_threshold, float threshold, float* word_maps, float* out,
+                                 float* scratch, void* stream) {
+  return expand_words_impl("daam_expand_words", global_maps, n_rows, mh, mw, rows, row_begin, n_words, out_h, out_w,
+                           absolute, use_threshold, threshold, word_maps, out, scratch, stream);
+}
+
+// one word whose "rows" are the word map itself
+extern "C" int daam_expand_as(const float* word_map, int32_t mh, int32_t mw, int32_t out_h, int32_t out_w,
+                              int32_t absolute, int32_t use_threshold, float threshold, float* out, float* scratch,
+                              void* stream) {
+  const int32_t rows[1] = {0}, row_begin[2] = {0, 1};
+  return expand_words_impl("daam_expand_as", word_map, 1, mh, mw, rows, row_begin, 1, out_h, out_w, absolute,
+                           use_threshold, threshold, nullptr, out, scratch, stream);
+}
+
+static int tile_count(const WordListParams& p) {
+  return ((p.oh + kSegTileH - 1) / kSegTileH) * ((p.ow + kSegTileW - 1) / kSegTileW);
+}
+
+// The tile entry points' launches after word_list_prepare: segment_minmax_kernel over (map, word, chunk), then
+// `kernel` over (tile, map). Sets k.s.chunks and k.s.words_per_pass.
+template <class Params>
+static int launch_tiles(void (*kernel)(Params), Params& k, int n_maps, const DeviceInfo& dev, cudaStream_t stream) {
+  WordListParams& p = k.s;
+  // launch 1: enough (map, word, chunk) CTAs for a few waves, at most kMaxChunks per word and one per 256 pixels
+  const long long n = (long long)p.oh * p.ow, mwords = (long long)n_maps * p.n_words;
+  long long chunks = (4LL * dev.sm_count + mwords - 1) / mwords;
+  if (chunks > kMaxChunks) chunks = kMaxChunks;
+  if (chunks > (n + 255) / 256) chunks = (n + 255) / 256;
+  if (chunks < 1 || !p.minmax) chunks = 1;
+  p.chunks = (int)chunks;
+  // launch 2: a tile's source window is at most ceil(tile * map / out) + 4 rows (columns), and no more than the map
+  const int win_h = std::min<int>(p.mh, (int)ceil((double)kSegTileH * p.mh / p.oh) + 5);
+  const int win_w = std::min<int>(p.mw, (int)ceil((double)kSegTileW * p.mw / p.ow) + 5);
+  const int win = win_h * win_w;
+  p.words_per_pass = std::max(1, std::min(p.n_words, kSegStageFloats / win));
+  static std::once_flag attr_once[64];
+  cudaError_t attr_err = cudaSuccess;
+  std::call_once(attr_once[dev.device & 63], [&] {
+    const void* kernels[] = {(const void*)segment_minmax_kernel, (const void*)segment_label_kernel,
+                             (const void*)region_tile_kernel, (const void*)overlay_kernel};
+    for (const void* f : kernels)
+      if (attr_err == cudaSuccess) attr_err = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
+  });
+  DAAM_CUDA_TRY(attr_err);
+  segment_minmax_kernel<<<(unsigned)(mwords * p.chunks), 256, (size_t)p.mh * p.mw * sizeof(float), stream>>>(p);
+  DAAM_CUDA_TRY(cudaGetLastError());
+  count_launch();
+  kernel<<<dim3(tile_count(p), n_maps), 256, (size_t)p.words_per_pass * win * sizeof(float), stream>>>(k);
+  DAAM_CUDA_TRY(cudaGetLastError());
+  count_launch();
+  return DAAM_OK;
+}
+
+extern "C" int daam_segment_words(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t mh, int32_t mw,
+                                  const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h,
+                                  int32_t out_w, int32_t absolute, int32_t use_threshold, float threshold,
+                                  float* word_maps, uint8_t* labels, float* scores, float* scratch, void* stream_) {
+  const char* name = "daam_segment_words";
+  if (!global_maps || !rows || !row_begin || !word_maps || !labels || !scores || !scratch || n_maps <= 0 || mh <= 0 ||
+      mw <= 0 || out_h <= 0 || out_w <= 0 || n_rows <= 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
+  static thread_local SegmentParams p;
+  DeviceInfo dev;
+  if (int rc = word_list_prepare(name, global_maps, n_maps, n_rows, mh, mw, rows, row_begin, n_words, out_h, out_w,
+                                 absolute, !absolute, use_threshold, threshold, word_maps, scratch, true, p.s, &dev)) return rc;
+  p.labels = labels; p.scores = scores;
+  return launch_tiles(segment_label_kernel, p, n_maps, dev, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int daam_region_overlap(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t mh, int32_t mw,
+                                   const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h,
+                                   int32_t out_w, int32_t absolute, int32_t use_threshold, float threshold,
+                                   float* word_maps, const uint8_t* regions, int32_t n_regions, float* intersection,
+                                   float* word_area, float* scratch, void* stream_) {
+  const char* name = "daam_region_overlap";
+  if (!global_maps || !rows || !row_begin || !word_maps || !regions || !intersection || !word_area || !scratch ||
+      n_maps <= 0 || mh <= 0 || mw <= 0 || out_h <= 0 || out_w <= 0 || n_rows <= 0 || n_regions <= 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
+  if (n_regions > kMaxRegions) { set_error("%s: %d regions > %d", name, n_regions, kMaxRegions); return DAAM_E_UNSUPPORTED; }
+  // fp32 partial sums of 0/1 values stay exact integers up to 2^24
+  if ((long long)out_h * out_w > (1LL << 24)) { set_error("%s: a %d x %d output is more than 2^24 pixels", name, out_h, out_w); return DAAM_E_UNSUPPORTED; }
+  static thread_local RegionParams p;
+  DeviceInfo dev;
+  if (int rc = word_list_prepare(name, global_maps, n_maps, n_rows, mh, mw, rows, row_begin, n_words, out_h, out_w,
+                                 absolute, !absolute, use_threshold, threshold, word_maps, scratch, true, p.s, &dev)) return rc;
+  p.regions = regions; p.n_regions = n_regions; p.tiles = tile_count(p.s);
+  p.partials = scratch + 64LL * n_maps * n_words;     // after segment_minmax_kernel's min / max partials
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (int rc = launch_tiles(region_tile_kernel, p, n_maps, dev, stream)) return rc;
+  const long long n_out = (long long)n_maps * n_words * (n_regions + 1);
+  region_reduce_kernel<<<(unsigned)((n_out + 7) / 8), 256, 0, stream>>>(p.partials, n_out, p.tiles, n_words, n_regions,
+                                                                        intersection, word_area);
+  DAAM_CUDA_TRY(cudaGetLastError());
+  count_launch();
+  return DAAM_OK;
+}
+
+extern "C" int daam_overlay_words(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t mh, int32_t mw,
+                                  const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h,
+                                  int32_t out_w, int32_t absolute, int32_t use_threshold, float threshold,
+                                  int32_t color_normalize, float* word_maps, const uint8_t* image,
+                                  int64_t image_map_stride, uint8_t* frames, float* scratch, void* stream_) {
+  const char* name = "daam_overlay_words";
+  if (!global_maps || !rows || !row_begin || !word_maps || !image || !frames || !scratch || n_maps <= 0 || mh <= 0 ||
+      mw <= 0 || out_h <= 0 || out_w <= 0 || n_rows <= 0 || image_map_stride < 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
+  if ((uintptr_t)frames & 3) { set_error("%s: frames must be 4-byte aligned", name); return DAAM_E_INVALID; }
+  static thread_local OverlayParams p;
+  DeviceInfo dev;
+  // the min / max of v is computed when the normalisation or the colour scale needs it
+  if (int rc = word_list_prepare(name, global_maps, n_maps, n_rows, mh, mw, rows, row_begin, n_words, out_h, out_w,
+                                 absolute, !absolute || color_normalize, use_threshold, threshold, word_maps, scratch,
+                                 true, p.s, &dev)) return rc;
+  p.image = image; p.image_map_stride = image_map_stride; p.frames = frames;
+  p.color_normalize = color_normalize ? 1 : 0; p.n_maps = n_maps;
+  return launch_tiles(overlay_kernel, p, n_maps, dev, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int daam_jet_colormap(float* out) {
+  if (!out) { set_error("daam_jet_colormap: null pointer"); return DAAM_E_INVALID; }
+  DAAM_CUDA_TRY(cudaMemcpyFromSymbol(out, c_jet, sizeof(JetTable)));
+  return DAAM_OK;
+}

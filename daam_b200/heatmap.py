@@ -347,9 +347,7 @@ class GlobalHeatMap:
         maps = self.heat_maps
         _require_cuda(maps, 'GlobalHeatMap.compute_word_heat_map')
         n_rows, grid = maps.shape[0], tuple(maps.shape[-2:])
-        for r in rows:  # torch's advanced indexing raises IndexError on out-of-range rows
-            if not -n_rows <= r < n_rows:
-                raise IndexError(f'index {r} is out of bounds for dimension 0 with size {n_rows}')
+        _check_rows(rows, n_rows)
         maps = maps.detach().float().contiguous()
         out = torch.empty(grid, dtype=torch.float32, device=maps.device)
         with torch.cuda.device(maps.device):
@@ -369,23 +367,17 @@ class GlobalHeatMap:
         ``expand_as``; ``to_cpu=False`` keeps it on the device until the caller needs it). ``word_idx`` may be a list
         parallel to ``words``. Raises the reference's ``ValueError`` for a word that is not in the prompt."""
         words = list(words)
-        maps = self.heat_maps
-        merged = _word_rows(self.tokenizer, self.prompt, words, word_idx, offset_idx, maps.shape[0])
-        _require_cuda(maps, 'GlobalHeatMap.expand_words')
-        n_rows, grid = maps.shape[0], tuple(maps.shape[-2:])
-        out_h, out_w = _image_size(image, *grid)
+        wl = _WordList(self.tokenizer, self.prompt, self.heat_maps[None], words, word_idx, offset_idx,
+                       'GlobalHeatMap.expand_words')
+        out_h, out_w = _image_size(image, *wl.grid)
         if not words:
             return [], torch.empty((0, out_h, out_w))
-        maps = maps.detach().float().contiguous()
-        dev = maps.device
-        word_maps = torch.empty((len(words),) + grid, dtype=torch.float32, device=dev)
-        out = torch.empty((len(words), out_h, out_w), dtype=torch.float32, device=dev)
-        scratch = torch.empty(_native.EXPAND_SCRATCH_FLOATS * len(words), dtype=torch.float32, device=dev)
-        with torch.cuda.device(dev):
-            _native.expand_words(maps.data_ptr(), n_rows, grid, [rows for rows, _ in merged], out_h, out_w, absolute,
-                                 threshold, word_maps.data_ptr(), out.data_ptr(), scratch.data_ptr(), _stream_ptr(dev))
-        whms = [WordHeatMap(word_maps[i], w, idx) for i, (w, (_, idx)) in enumerate(zip(words, merged))]
-        return whms, (out.cpu() if to_cpu else out)
+        out = torch.empty((len(words), out_h, out_w), dtype=torch.float32, device=wl.dev)
+        scratch = wl.scratch(_native.EXPAND_SCRATCH_FLOATS * len(words))
+        with torch.cuda.device(wl.dev):
+            _native.expand_words(wl.maps.data_ptr(), wl.n_rows, wl.grid, wl.rows, out_h, out_w, absolute, threshold,
+                                 wl.word_maps.data_ptr(), out.data_ptr(), scratch.data_ptr(), _stream_ptr(wl.dev))
+        return _word_heat_maps(wl.word_maps[0], words, wl.merged), (out.cpu() if to_cpu else out)
 
     def segment(self, words, image, absolute: bool = False, threshold: Optional[float] = None, word_idx=None,
                 offset_idx: int = 0, to_cpu: bool = True):
@@ -405,8 +397,7 @@ class GlobalHeatMap:
         word_maps, merged, labels, scores = _segment(self.tokenizer, self.prompt, self.heat_maps[None], words, image,
                                                      absolute, threshold, word_idx, offset_idx, to_cpu,
                                                      'GlobalHeatMap.segment')
-        whms = [WordHeatMap(word_maps[0, i], w, idx) for i, (w, (_, idx)) in enumerate(zip(words, merged))]
-        return whms, labels[0], scores[0]
+        return _word_heat_maps(word_maps[0], words, merged), labels[0], scores[0]
 
     def region_overlap(self, words, image, regions: torch.Tensor, absolute: bool = False,
                        threshold: Optional[float] = None, word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
@@ -428,8 +419,8 @@ class GlobalHeatMap:
         word_maps, merged, overlap = _region_overlap(self.tokenizer, self.prompt, self.heat_maps[None], words, image,
                                                      regions, absolute, threshold, word_idx, offset_idx, to_cpu,
                                                      'GlobalHeatMap.region_overlap')
-        whms = [WordHeatMap(word_maps[0, i], w, idx) for i, (w, (_, idx)) in enumerate(zip(words, merged))]
-        return whms, RegionOverlap(overlap.intersection[0], overlap.word_area[0], overlap.region_area)
+        return (_word_heat_maps(word_maps[0], words, merged),
+                RegionOverlap(overlap.intersection[0], overlap.word_area[0], overlap.region_area))
 
     def overlay_words(self, words, image, absolute: bool = False, threshold: Optional[float] = None,
                       color_normalize: bool = True, word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
@@ -450,20 +441,43 @@ class GlobalHeatMap:
         word_maps, merged, frames = _overlay(self.tokenizer, self.prompt, self.heat_maps[None], words, image, absolute,
                                              threshold, color_normalize, word_idx, offset_idx, to_cpu,
                                              'GlobalHeatMap.overlay_words', stack=False)
-        whms = [WordHeatMap(word_maps[0, i], w, idx) for i, (w, (_, idx)) in enumerate(zip(words, merged))]
-        return whms, frames[0]
+        return _word_heat_maps(word_maps[0], words, merged), frames[0]
 
 
-def _word_rows(tokenizer, prompt: str, words: List[str], word_idx, offset_idx: int, n_rows: int):
-    """``compute_token_merge_indices`` of every word (``word_idx`` may be a list parallel to ``words``), with the
-    row range checked the way torch's advanced indexing would."""
-    idxs = list(word_idx) if isinstance(word_idx, (list, tuple)) else [word_idx] * len(words)
-    merged = [compute_token_merge_indices(tokenizer, prompt, w, i, offset_idx) for w, i in zip(words, idxs)]
-    for rows, _ in merged:
-        for r in rows:
-            if not -n_rows <= r < n_rows:
-                raise IndexError(f'index {r} is out of bounds for dimension 0 with size {n_rows}')
-    return merged
+def _check_rows(rows, n_rows: int):
+    """Raises the ``IndexError`` torch's advanced indexing raises on a row out of ``[-n_rows, n_rows)``."""
+    for r in rows:
+        if not -n_rows <= r < n_rows:
+            raise IndexError(f'index {r} is out of bounds for dimension 0 with size {n_rows}')
+
+
+def _word_heat_maps(word_maps: torch.Tensor, words, merged) -> List[WordHeatMap]:
+    """One :class:`WordHeatMap` per word: ``word_maps[i]`` (device ``[xh, xw]``) with the word and its index."""
+    return [WordHeatMap(word_maps[i], w, idx) for i, (w, (_, idx)) in enumerate(zip(words, merged))]
+
+
+class _WordList:
+    """What the fused word-list ops over ``maps`` ``[n_maps, n_rows, xh, xw]`` share before they launch, in the order
+    they raise: ``compute_token_merge_indices`` of every word (``word_idx`` may be a list parallel to ``words``; the
+    reference's ``ValueError`` for a word not in the prompt, then the row range as torch's advanced indexing checks
+    it), then the CUDA check. Holds the contiguous fp32 maps and the device word heat maps ``[n_maps, len(words), xh,
+    xw]`` the launch writes."""
+
+    def __init__(self, tokenizer, prompt: str, maps: torch.Tensor, words: List[str], word_idx, offset_idx: int,
+                 what: str):
+        self.n_maps, self.n_rows, self.grid = maps.shape[0], maps.shape[1], tuple(maps.shape[-2:])
+        idxs = list(word_idx) if isinstance(word_idx, (list, tuple)) else [word_idx] * len(words)
+        self.merged = [compute_token_merge_indices(tokenizer, prompt, w, i, offset_idx) for w, i in zip(words, idxs)]
+        for rows, _ in self.merged:
+            _check_rows(rows, self.n_rows)
+        self.rows = [rows for rows, _ in self.merged]
+        _require_cuda(maps, what)
+        self.dev = maps.device
+        self.maps = maps.detach().float().contiguous()
+        self.word_maps = torch.empty((self.n_maps, len(words)) + self.grid, dtype=torch.float32, device=self.dev)
+
+    def scratch(self, n_floats: int) -> torch.Tensor:
+        return torch.empty(n_floats, dtype=torch.float32, device=self.dev)
 
 
 def _segment(tokenizer, prompt: str, maps: torch.Tensor, words, image, absolute, threshold, word_idx, offset_idx: int,
@@ -471,27 +485,23 @@ def _segment(tokenizer, prompt: str, maps: torch.Tensor, words, image, absolute,
     """``daam_segment_words`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(word_maps, merged, labels,
     scores)``: the device word heat maps ``[n_maps, len(words), xh, xw]``, ``compute_token_merge_indices`` of every
     word, and ``labels`` / ``scores`` ``[n_maps, H, W]``."""
-    n_maps, n_rows, grid = maps.shape[0], maps.shape[1], tuple(maps.shape[-2:])
-    merged = _word_rows(tokenizer, prompt, words, word_idx, offset_idx, n_rows)
-    _require_cuda(maps, what)
-    out_h, out_w = _image_size(image, *grid)
-    dev = maps.device
-    word_maps = torch.empty((n_maps, len(words)) + grid, dtype=torch.float32, device=dev)
+    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, what)
+    n_maps, dev = wl.n_maps, wl.dev
+    out_h, out_w = _image_size(image, *wl.grid)
     if not words or n_maps == 0:
         labels = torch.zeros((n_maps, out_h, out_w), dtype=torch.uint8, device=dev)
         scores = torch.full((n_maps, out_h, out_w), float('-inf'), device=dev)
-        return word_maps, merged, (labels.cpu() if to_cpu else labels), (scores.cpu() if to_cpu else scores)
-    maps = maps.detach().float().contiguous()
+        return wl.word_maps, wl.merged, (labels.cpu() if to_cpu else labels), (scores.cpu() if to_cpu else scores)
     labels = torch.empty((n_maps, out_h, out_w), dtype=torch.uint8, device=dev)
     scores = torch.empty((n_maps, out_h, out_w), dtype=torch.float32, device=dev)
-    scratch = torch.empty(_native.segment_scratch_floats(n_maps, len(words)), dtype=torch.float32, device=dev)
+    scratch = wl.scratch(_native.segment_scratch_floats(n_maps, len(words)))
     with torch.cuda.device(dev):
-        _native.segment_words(maps.data_ptr(), n_maps, n_rows, grid, [rows for rows, _ in merged], out_h, out_w,
-                              absolute, threshold, word_maps.data_ptr(), labels.data_ptr(), scores.data_ptr(),
+        _native.segment_words(wl.maps.data_ptr(), n_maps, wl.n_rows, wl.grid, wl.rows, out_h, out_w, absolute,
+                              threshold, wl.word_maps.data_ptr(), labels.data_ptr(), scores.data_ptr(),
                               scratch.data_ptr(), _stream_ptr(dev))
     if to_cpu:
         labels, scores = labels.cpu(), scores.cpu()
-    return word_maps, merged, labels, scores
+    return wl.word_maps, wl.merged, labels, scores
 
 
 @dataclass
@@ -524,9 +534,8 @@ def _region_overlap(tokenizer, prompt: str, maps: torch.Tensor, words, image, re
     """``daam_region_overlap`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(word_maps, merged, overlap)``: the
     device word heat maps ``[n_maps, len(words), xh, xw]``, ``compute_token_merge_indices`` of every word, and the
     :class:`RegionOverlap` with a leading map axis."""
-    n_maps, n_rows, grid = maps.shape[0], maps.shape[1], tuple(maps.shape[-2:])
-    merged = _word_rows(tokenizer, prompt, words, word_idx, offset_idx, n_rows)
-    _require_cuda(maps, what)
+    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, what)
+    n_maps, grid, dev = wl.n_maps, wl.grid, wl.dev
     out_h, out_w = _image_size(image, *grid)
     if not isinstance(regions, torch.Tensor):
         raise TypeError(f'{what}: regions must be a torch.Tensor, not {type(regions).__name__}')
@@ -538,7 +547,6 @@ def _region_overlap(tokenizer, prompt: str, maps: torch.Tensor, words, image, re
         raise ValueError(f'{what}: regions of shape {tuple(regions.shape)} do not match the expanded maps\' '
                          f'(R, {out_h}, {out_w}) (a [{out_h}, {out_w}] region or a stack of them)')
     _require_cuda(regions, what)
-    dev = maps.device
     if regions.device != dev:
         raise ValueError(f'{what}: regions are on {regions.device}, the heat maps on {dev}')
     n_regions = regions.shape[0]
@@ -547,21 +555,18 @@ def _region_overlap(tokenizer, prompt: str, maps: torch.Tensor, words, image, re
                            torch.zeros((n_regions,), device=dev))
         word_maps = torch.empty((n_maps, 0) + grid, dtype=torch.float32, device=dev)
         return word_maps, [], (_to_cpu(ov) if to_cpu else ov)
-    maps = maps.detach().float().contiguous()
     region_bytes = regions.detach().contiguous().view(torch.uint8)
-    word_maps = torch.empty((n_maps, len(words)) + grid, dtype=torch.float32, device=dev)
     inter = torch.empty((n_maps, n_regions, len(words)), dtype=torch.float32, device=dev)
     area = torch.empty((n_maps, len(words)), dtype=torch.float32, device=dev)
-    scratch = torch.empty(_native.region_scratch_floats(n_maps, len(words), n_regions, out_h, out_w),
-                          dtype=torch.float32, device=dev)
+    scratch = wl.scratch(_native.region_scratch_floats(n_maps, len(words), n_regions, out_h, out_w))
     with torch.cuda.device(dev):
-        _native.region_overlap(maps.data_ptr(), n_maps, n_rows, grid, [rows for rows, _ in merged], out_h, out_w,
-                               absolute, threshold, word_maps.data_ptr(), region_bytes.data_ptr(), n_regions,
-                               inter.data_ptr(), area.data_ptr(), scratch.data_ptr(), _stream_ptr(dev))
+        _native.region_overlap(wl.maps.data_ptr(), n_maps, wl.n_rows, grid, wl.rows, out_h, out_w, absolute, threshold,
+                               wl.word_maps.data_ptr(), region_bytes.data_ptr(), n_regions, inter.data_ptr(),
+                               area.data_ptr(), scratch.data_ptr(), _stream_ptr(dev))
     # exact pixel counts (at most 2**24 pixels): what ``region.float().sum()`` gives in compute_iou
     region_area = (region_bytes != 0).sum((-1, -2)).float()
     ov = RegionOverlap(inter, area, region_area)
-    return word_maps, merged, (_to_cpu(ov) if to_cpu else ov)
+    return wl.word_maps, wl.merged, (_to_cpu(ov) if to_cpu else ov)
 
 
 def _to_cpu(ov: RegionOverlap) -> RegionOverlap:
@@ -610,27 +615,23 @@ def _overlay(tokenizer, prompt: str, maps: torch.Tensor, words, image, absolute,
     """``daam_overlay_words`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(word_maps, merged, frames)``: the
     device word heat maps ``[n_maps, len(words), xh, xw]``, ``compute_token_merge_indices`` of every word, and
     ``frames`` uint8 ``[n_maps, len(words), H, W, 3]``."""
-    n_maps, n_rows, grid = maps.shape[0], maps.shape[1], tuple(maps.shape[-2:])
-    merged = _word_rows(tokenizer, prompt, words, word_idx, offset_idx, n_rows)
-    _require_cuda(maps, what)
-    dev = maps.device
-    image, out_h, out_w, per_map = _overlay_image(image, n_maps, grid, dev, what, stack)
+    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, what)
+    n_maps, dev = wl.n_maps, wl.dev
+    image, out_h, out_w, per_map = _overlay_image(image, n_maps, wl.grid, dev, what, stack)
     shape = (n_maps, len(words), out_h, out_w, 3)
-    word_maps = torch.empty((n_maps, len(words)) + grid, dtype=torch.float32, device=dev)
     if not words or n_maps == 0:
         frames = torch.empty(shape, dtype=torch.uint8, device='cpu' if to_cpu else dev)
-        return word_maps, merged, frames
+        return wl.word_maps, wl.merged, frames
     image = image.to(dev).contiguous()                   # one copy to the device
-    maps = maps.detach().float().contiguous()
     # the kernel writes whole 4-byte words: the frames are a view of a buffer rounded up to them
     buf = torch.empty(_native.overlay_frames_bytes(*shape[:4]), dtype=torch.uint8, device=dev)
     frames = buf[:n_maps * len(words) * out_h * out_w * 3].view(shape)
-    scratch = torch.empty(_native.segment_scratch_floats(n_maps, len(words)), dtype=torch.float32, device=dev)
+    scratch = wl.scratch(_native.segment_scratch_floats(n_maps, len(words)))
     with torch.cuda.device(dev):
-        _native.overlay_words(maps.data_ptr(), n_maps, n_rows, grid, [rows for rows, _ in merged], out_h, out_w,
-                              absolute, threshold, color_normalize, word_maps.data_ptr(), image.data_ptr(),
+        _native.overlay_words(wl.maps.data_ptr(), n_maps, wl.n_rows, wl.grid, wl.rows, out_h, out_w, absolute, threshold,
+                              color_normalize, wl.word_maps.data_ptr(), image.data_ptr(),
                               out_h * out_w * 3 if per_map else 0, buf.data_ptr(), scratch.data_ptr(), _stream_ptr(dev))
-    return word_maps, merged, (frames.cpu() if to_cpu else frames)
+    return wl.word_maps, wl.merged, (frames.cpu() if to_cpu else frames)
 
 
 class GlobalHeatMapStack:
@@ -656,9 +657,7 @@ class GlobalHeatMapStack:
         maps = self.heat_maps
         _require_cuda(maps, f'{type(self).__name__}.word_heat_maps')
         steps, n_rows, grid = maps.shape[0], maps.shape[1], tuple(maps.shape[-2:])
-        for r in rows:
-            if not -n_rows <= r < n_rows:
-                raise IndexError(f'index {r} is out of bounds for dimension 0 with size {n_rows}')
+        _check_rows(rows, n_rows)
         maps = maps.detach().float().contiguous()
         out = torch.empty((steps,) + grid, dtype=torch.float32, device=maps.device)
         with torch.cuda.device(maps.device):
