@@ -44,7 +44,7 @@ def overlay_frames_bytes(n_maps: int, n_words: int, out_h: int, out_w: int) -> i
 
 
 EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize',
-           'daam_finalize_maps', 'daam_finalize_per_key','daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
+           'daam_finalize_maps', 'daam_finalize_parts', 'daam_finalize_per_key','daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
            'daam_segment_words', 'daam_region_overlap', 'daam_overlay_words', 'daam_jet_colormap',
            'daam_side_launcher_create', 'daam_side_launcher_destroy',
            'daam_side_launcher_launch', 'daam_side_launcher_join', 'daam_side_launcher_idle', 'daam_abi_version',
@@ -81,7 +81,15 @@ class DaamMapSel(ctypes.Structure):
     ]
 
 
-FINALIZE_MAX_MAPS = 64   # DAAM_FINALIZE_MAX_MAPS: maps per daam_finalize_maps call
+class DaamMapPart(ctypes.Structure):
+    """``struct daam_map_part`` (include/daam_b200.h): one output map of ``daam_finalize_parts``."""
+    _fields_ = [
+        ('group_begin', ctypes.c_int32), ('group_count', ctypes.c_int32), ('n_rows', ctypes.c_int32),
+        ('reserved', ctypes.c_int32), ('out', ctypes.c_void_p),
+    ]
+
+
+FINALIZE_MAX_MAPS = 64   # DAAM_FINALIZE_MAX_MAPS: maps per daam_finalize_maps / daam_finalize_parts call
 
 
 class NativeError(RuntimeError):
@@ -126,6 +134,9 @@ def load() -> ctypes.CDLL:
     lib.daam_finalize_maps.argtypes = [ctypes.POINTER(DaamKeyGroup), i32, ctypes.POINTER(DaamMapSel), i32, i32, i32,
                                        i32, vp]
     lib.daam_finalize_maps.restype = ctypes.c_int
+    lib.daam_finalize_parts.argtypes = [ctypes.POINTER(DaamKeyGroup), i32, ctypes.POINTER(DaamMapPart), i32, i32, i32,
+                                        i32, vp]
+    lib.daam_finalize_parts.restype = ctypes.c_int
     lib.daam_finalize_per_key.argtypes = [ctypes.POINTER(DaamKeyGroup), i32, i32, i32, i32, i32, vp, vp]
     lib.daam_finalize_per_key.restype = ctypes.c_int
     lib.daam_word_heat_map.argtypes = [vp, i32, i32, i32, ctypes.POINTER(i32), i32, vp, vp]
@@ -308,6 +319,27 @@ def finalize_maps(groups: Sequence[DaamKeyGroup], maps: Sequence[DaamMapSel], x,
         part = maps[i:i + FINALIZE_MAX_MAPS]
         sel = (DaamMapSel * max(len(part), 1))(*part)
         _check(lib.daam_finalize_maps(arr, n, sel, len(part), h, w, int(bool(normalize)), ctypes.c_void_p(stream)))
+
+
+def finalize_parts(groups: Sequence[DaamKeyGroup], parts: Sequence[DaamMapPart], x, normalize: bool, stream: int):
+    """``daam_finalize_parts``: one :class:`DaamMapPart` per output map, each a range of ``groups``. More than
+    :data:`FINALIZE_MAX_MAPS` maps go out in several calls, which changes no map's bits. A part that is no range of
+    ``groups``, or has no rows or output, is a ``ValueError`` before anything is loaded or launched."""
+    h, w = map_size(x)
+    n = len(groups)
+    if not parts:
+        raise ValueError('finalize_parts: no output map')
+    for i, part in enumerate(parts):
+        if part.group_begin < 0 or part.group_count <= 0 or part.group_begin + part.group_count > n:
+            raise ValueError(f'finalize_parts: map {i} reads groups [{part.group_begin}, +{part.group_count}) of {n}')
+        if part.n_rows <= 0 or not part.out:
+            raise ValueError(f'finalize_parts: map {i} has no rows or no output')
+    arr = (DaamKeyGroup * n)(*groups)
+    lib = load()
+    for i in range(0, len(parts), FINALIZE_MAX_MAPS):
+        chunk = parts[i:i + FINALIZE_MAX_MAPS]
+        sel = (DaamMapPart * len(chunk))(*chunk)
+        _check(lib.daam_finalize_parts(arr, n, sel, len(chunk), h, w, int(bool(normalize)), ctypes.c_void_p(stream)))
 
 
 def finalize_per_key(groups: Sequence[DaamKeyGroup], x, n_rows: int, normalize: bool, out_ptr: int, stream: int):

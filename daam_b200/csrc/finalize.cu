@@ -17,17 +17,37 @@ namespace {
 constexpr int kMaxGroups = 160;   // key groups (layer x prompt slices) per finalize launch
 constexpr int kMaxMaps = DAAM_FINALIZE_MAX_MAPS;   // output maps per finalize launch
 
-// One output map of a finalize launch: blocks [block_begin, block_begin + block_count) of every group, i.e. the keys
-// of the expanded group list `for g: for b: {acc_g + b * heads_g * tokens_g * h_g * w_g, heads_g, head_sel_g}`.
+// One output map of a finalize launch: blocks [block_begin, block_begin + block_count) of the groups [group_begin,
+// group_begin + group_count), i.e. the keys of the expanded group list `for g: for b: {acc_g + b * heads_g * tokens_g *
+// h_g * w_g, heads_g, head_sel_g}`. daam_finalize_maps selects blocks of every group, daam_finalize_parts groups.
 struct MapSel {
   float* out;                             // [n_rows][oh][ow]
   int block_begin, block_count, n_rows, n_keys;
   int band_rows;                          // fast kernel only: 8 or 4 (daam_finalize's rule for this map's n_rows)
+  int group_begin, group_count;
+  // Fast kernel only (n_classes 0: the map takes the generic kernel): the map's OWN key classes. A fast key has one
+  // integer factor 1 / 2 / 4 on both axes, so a class is a source size (kh, kw) = (oh / F, ow / F) and a map has at most
+  // three, kept in the order its groups first show them. Per block: keys[] is ordered class by class, class c owns
+  // [key_begin[c], key_begin[c + 1]) times the map's block count, and a group g of class c starts at (key_slot0[c] +
+  // FinalizeParams::class_keys_before[g]) times the block count, block by block, head by head.
+  int n_classes;
+  int kh[3], kw[3];
+  int key_begin[4];
+  int key_slot0[3];                       // key_begin[c] less the class's keys in the groups before group_begin
 };
+
+MapSel make_map(float* out, int block_begin, int block_count, int n_rows, int group_begin, int group_count) {
+  MapSel s = {};
+  s.out = out; s.block_begin = block_begin; s.block_count = block_count; s.n_rows = n_rows;
+  s.group_begin = group_begin; s.group_count = group_count;
+  return s;
+}
 
 struct FinalizeParams {
   int n_groups, oh, ow, n_maps;           // output maps [oh][ow]
   daam_key_group g[kMaxGroups];
+  // fast kernel only: keys per block of the groups before g that have g's size (the same for every map of the launch)
+  int class_keys_before[kMaxGroups];
   MapSel map[kMaxMaps];                   // blockIdx.z selects the map
 };
 
@@ -43,7 +63,7 @@ __global__ void __launch_bounds__(256) finalize_kernel(const __grid_constant__ F
   float sum = 0.f;
   int ch = -1, cw = -1;
   Taps ty, tx;
-  for (int g = 0; g < P.n_groups; ++g) {
+  for (int g = M.group_begin; g < M.group_begin + M.group_count; ++g) {
     const daam_key_group& G = P.g[g];
     const int hw = G.h * G.w;
     const int h0 = G.head_sel < 0 ? 0 : G.head_sel;
@@ -309,19 +329,9 @@ __device__ __forceinline__ void class_pass_identity(const FinalizeParams& P, int
   }
 }
 
-struct ClassList {
-  int n;
-  int kh[8], kw[8];         // distinct source sizes, each (oh / F, ow / F) with F = 1, 2 or 4
-  // per block: keys[] is ordered class by class, and class c owns [key_begin[c], key_begin[c + 1]) times the map's
-  // block count; group g's keys start at key_slot[g] times the block count, block by block, head by head
-  int key_begin[9];
-  int key_slot[kMaxGroups];
-};
-
 // grid: (ceil(oh / 4) bands, max n_rows, n_maps); a CTA past its map's bands or rows returns at once. Dynamic smem: two
 // chunk buffers + the band tile (the largest band_rows of the launch * ow floats)
-__global__ void __launch_bounds__(256, 2) finalize_fast_kernel(const __grid_constant__ FinalizeParams P,
-                                                               const __grid_constant__ ClassList C) {
+__global__ void __launch_bounds__(256, 2) finalize_fast_kernel(const __grid_constant__ FinalizeParams P) {
   extern __shared__ __align__(16) float dyn[];
   __shared__ const float* keys[kMaxClassKeys];
   float* stage = dyn;                                  // 2 x kStageFloats
@@ -330,12 +340,13 @@ __global__ void __launch_bounds__(256, 2) finalize_fast_kernel(const __grid_cons
   const int band = blockIdx.x, t = blockIdx.y, oh = P.oh, ow = P.ow, br = M.band_rows, nb = M.block_count;
   if (t >= M.n_rows || band * br >= oh) return;
   const int rows = min(br, oh - band * br);            // valid output rows of this band
-  // key pointers (token row t) of every selected key, class by class; one thread per key group
-  for (int g = threadIdx.x; g < P.n_groups; g += blockDim.x) {
+  // key pointers (token row t) of every selected key, class by class; one thread per key group of the map
+  for (int g = M.group_begin + threadIdx.x; g < M.group_begin + M.group_count; g += blockDim.x) {
     const daam_key_group& G = P.g[g];
     const int per_block = G.head_sel < 0 ? G.heads : 1;
     const long long hw = (long long)G.h * G.w;
-    const float** dst = keys + C.key_slot[g] * nb;
+    const int slot0 = G.w == M.kw[0] ? M.key_slot0[0] : (G.w == M.kw[1] ? M.key_slot0[1] : M.key_slot0[2]);
+    const float** dst = keys + (slot0 + P.class_keys_before[g]) * nb;
     // key j of the group: head (block_begin * heads + j) of all heads, or head_sel of block block_begin + j
     const long long first = G.head_sel < 0 ? (long long)M.block_begin * G.heads : (long long)M.block_begin * G.heads + G.head_sel;
     const long long step = G.head_sel < 0 ? 1 : G.heads;
@@ -344,13 +355,13 @@ __global__ void __launch_bounds__(256, 2) finalize_fast_kernel(const __grid_cons
   for (int i = threadIdx.x; i < br * ow; i += blockDim.x) tile[i] = 0.f;
   __syncthreads();
   bool prefetched = false;                             // chunk 0 of class c is already streaming into buffer 1
-  for (int c = 0; c < C.n; ++c) {
-    const int kh = C.kh[c], kw = C.kw[c], f = ow / kw, nk = (C.key_begin[c + 1] - C.key_begin[c]) * nb;
-    const float* const* ck = keys + C.key_begin[c] * nb;
+  for (int c = 0; c < M.n_classes; ++c) {                // the map's own classes: maps of one launch differ in them
+    const int kh = M.kh[c], kw = M.kw[c], f = ow / kw, nk = (M.key_begin[c + 1] - M.key_begin[c]) * nb;
+    const float* const* ck = keys + M.key_begin[c] * nb;
     NextClass next = {0, 0, 0, 0, nullptr};
-    if (c + 1 < C.n && C.kw[c + 1] != ow)
-      next = {C.kh[c + 1], C.kw[c + 1], ow / C.kw[c + 1], (C.key_begin[c + 2] - C.key_begin[c + 1]) * nb,
-              keys + C.key_begin[c + 1] * nb};
+    if (c + 1 < M.n_classes && M.kw[c + 1] != ow)
+      next = {M.kh[c + 1], M.kw[c + 1], ow / M.kw[c + 1], (M.key_begin[c + 2] - M.key_begin[c + 1]) * nb,
+              keys + M.key_begin[c + 1] * nb};
     if (f == 1) class_pass_identity(P, nk, band, br, rows, tile, ck, stage, next);
     else if (f == 2) class_pass<2>(P, kh, kw, nk, band, br, tile, ck, stage, prefetched, next);
     else class_pass<4>(P, kh, kw, nk, band, br, tile, ck, stage, prefetched, next);
@@ -449,53 +460,67 @@ static int check_key_groups(const char* name, const daam_key_group* groups, int3
   return DAAM_OK;
 }
 
-// daam_finalize and daam_finalize_maps, after validation: `maps` are MapSel with out, blocks and n_rows set, and every
-// map is reduced exactly as daam_finalize reduces the map's expanded group list. The kernel choice and the band height
-// are daam_finalize's rule applied per map, so the maps of one call take at most two launches (fast and generic, one
-// per kind present) plus one normalisation launch.
-static int launch_finalize(const daam_key_group* groups, int32_t n_groups, int32_t oh, int32_t ow, MapSel* maps,
-                           int n_maps, int keys_per_block, int32_t normalize, const DeviceInfo& dev, cudaStream_t stream) {
+// daam_finalize, daam_finalize_maps and daam_finalize_parts, after validation: `maps` are MapSel with out, blocks,
+// groups and n_rows set, and every map is reduced exactly as daam_finalize reduces the map's expanded group list. The
+// kernel choice and the band height are daam_finalize's rule applied per map, to the map's own groups, so the maps of
+// one call take at most two launches (fast and generic, one per kind present) plus one normalisation launch.
+static int launch_finalize(const char* name, const daam_key_group* groups, int32_t n_groups, int32_t oh, int32_t ow,
+                           MapSel* maps, int n_maps, int32_t normalize, const DeviceInfo& dev, cudaStream_t stream) {
   static thread_local FinalizeParams p;
   p.n_groups = n_groups; p.oh = oh; p.ow = ow;
   for (int i = 0; i < n_groups; ++i) p.g[i] = groups[i];
   const int xx = oh * ow;
-  // fast path: every key has one integer factor F = 1 / 2 / 4 on both axes (all SD / SDXL layers that are ever traced)
-  // and 16-byte-aligned key bases (cp.async / float4: an aligned slab and h * w a multiple of 4, which keeps every block
-  // of a group aligned too). A square map keeps the rule it always had (side a multiple of 16), so its kernel choice
-  // and bits do not move. The map's key count (at most kMaxClassKeys) is checked per map below.
-  ClassList cls;
-  cls.n = 0;
-  bool fast_groups = (oh != ow || oh % 16 == 0) && ow <= 256 && !force_generic_finalize();
-  for (int i = 0; i < n_groups && fast_groups; ++i) {
+  // fast path: every key of the map has one integer factor F = 1 / 2 / 4 on both axes (all SD / SDXL layers that are
+  // ever traced) and a 16-byte-aligned key base (cp.async / float4: an aligned slab and h * w a multiple of 4, which
+  // keeps every block of a group aligned too). A square map keeps the rule it always had (side a multiple of 16), so its
+  // kernel choice and bits do not move. Such keys have one of three sizes, (oh / F, ow / F), so the limit of 8 key sizes
+  // a map may show can never bind. The map's key count (at most kMaxClassKeys) is checked per map below.
+  const bool fast_grid = (oh != ow || oh % 16 == 0) && ow <= 256 && !force_generic_finalize();
+  int factor[kMaxGroups];                                // of a group the fast kernel can read, else 0
+  int seen[5] = {0, 0, 0, 0, 0};                         // keys per block so far of the class with factor F
+  for (int i = 0; i < n_groups; ++i) {
     const daam_key_group& g = groups[i];
     const int f = oh / g.h;
-    if (oh % g.h != 0 || ow % g.w != 0 || ow / g.w != f || (f != 1 && f != 2 && f != 4) ||
-        reinterpret_cast<uintptr_t>(g.acc) % 16 != 0 || (g.h * g.w) % 4 != 0) { fast_groups = false; break; }
-    bool seen = false;
-    for (int c = 0; c < cls.n; ++c) seen = seen || (cls.kh[c] == g.h && cls.kw[c] == g.w);
-    if (!seen) {
-      if (cls.n == 8) { fast_groups = false; break; }
-      cls.kh[cls.n] = g.h; cls.kw[cls.n] = g.w; ++cls.n;
-    }
+    const bool ok = fast_grid && oh % g.h == 0 && ow % g.w == 0 && ow / g.w == f && (f == 1 || f == 2 || f == 4) &&
+                    reinterpret_cast<uintptr_t>(g.acc) % 16 == 0 && (g.h * g.w) % 4 == 0;
+    factor[i] = ok ? f : 0;
+    p.class_keys_before[i] = seen[factor[i]];
+    seen[factor[i]] += g.head_sel < 0 ? g.heads : 1;
   }
-  if (fast_groups) {
-    int next = 0;
-    for (int c = 0; c < cls.n; ++c) {                   // keys[] of the kernel: class by class, groups in call order
-      cls.key_begin[c] = next;
-      for (int i = 0; i < n_groups; ++i)
-        if (groups[i].h == cls.kh[c] && groups[i].w == cls.kw[c]) {
-          cls.key_slot[i] = next;
-          next += groups[i].head_sel < 0 ? groups[i].heads : 1;
-        }
+  for (int m = 0; m < n_maps; ++m) {                     // the map's keys and, if it can take the fast kernel, classes
+    MapSel& s = maps[m];
+    long long per_block = 0;
+    int keys_of[5] = {0, 0, 0, 0, 0}, nc = 0;            // nc: the map's classes so far, -1 once a group is not fast
+    for (int i = s.group_begin; i < s.group_begin + s.group_count; ++i) {
+      const int k = groups[i].head_sel < 0 ? groups[i].heads : 1, f = factor[i];
+      per_block += k;
+      if (f == 0 || nc < 0) { nc = -1; continue; }
+      if (keys_of[f] == 0) {                             // first seen: the class's keys before the map, for key_slot0
+        s.kh[nc] = groups[i].h; s.kw[nc] = groups[i].w;
+        s.key_slot0[nc++] = p.class_keys_before[i];
+      }
+      keys_of[f] += k;
     }
-    cls.key_begin[cls.n] = next;
+    if (per_block * s.block_count > (1 << 30)) {
+      set_error("%s: map %d selects more than 2^30 keys", name, m);
+      return DAAM_E_UNSUPPORTED;
+    }
+    s.n_keys = (int)per_block * s.block_count;
+    if (s.n_keys > kMaxClassKeys) nc = -1;
+    s.n_classes = std::max(nc, 0);
+    for (int c = 0, next = 0; c < s.n_classes; ++c) {    // keys[] of the kernel: class by class, groups in call order
+      s.key_begin[c] = next;
+      s.key_slot0[c] = next - s.key_slot0[c];
+      next += keys_of[oh / s.kh[c]];
+      s.key_begin[c + 1] = next;
+    }
+    for (int c = s.n_classes; c < 3; ++c) s.kh[c] = s.kw[c] = 0;
   }
   for (int pass = 0; pass < 2; ++pass) {                 // pass 0: the maps on the fast kernel, pass 1: the others
     int n = 0, max_rows = 0, max_br = 4;
     for (int m = 0; m < n_maps; ++m) {
       MapSel s = maps[m];
-      s.n_keys = keys_per_block * s.block_count;
-      if ((fast_groups && s.n_keys <= kMaxClassKeys) != (pass == 0)) continue;
+      if ((s.n_classes > 0) != (pass == 0)) continue;
       // 8-row bands unless that leaves the machine under-filled (< 2 CTAs per SM) or a band's source pixels of the
       // factor-2 class would exceed one CTA's 256 threads (ow > 128); forcing either height measured the same within
       // 1 % for the 175-key SD-2.1 case
@@ -517,7 +542,7 @@ static int launch_finalize(const daam_key_group* groups, int32_t n_groups, int32
                                         (int)((2 * kStageFloats + 8 * 256) * sizeof(float)));
       });
       DAAM_CUDA_TRY(attr_err);
-      finalize_fast_kernel<<<dim3(bands, max_rows, n), 256, smem, stream>>>(p, cls);
+      finalize_fast_kernel<<<dim3(bands, max_rows, n), 256, smem, stream>>>(p);
     } else {
       finalize_kernel<<<dim3((xx + 255) / 256, max_rows, n), 256, 0, stream>>>(p);
     }
@@ -539,8 +564,9 @@ extern "C" int daam_finalize(const daam_key_group* groups, int32_t n_groups, int
   DeviceInfo dev;
   int n_keys;
   if (int rc = check_key_groups("daam_finalize", groups, n_groups, oh, ow, n_rows, out, &dev, &n_keys)) return rc;
-  MapSel map = {out, 0, 1, n_rows, 0, 0};             // block 0 of every group: the groups as given
-  return launch_finalize(groups, n_groups, oh, ow, &map, 1, n_keys, normalize, dev, static_cast<cudaStream_t>(stream_));
+  MapSel map = make_map(out, 0, 1, n_rows, 0, n_groups);   // block 0 of every group: the groups as given
+  return launch_finalize("daam_finalize", groups, n_groups, oh, ow, &map, 1, normalize, dev,
+                         static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int daam_finalize_maps(const daam_key_group* groups, int32_t n_groups, const daam_map_sel* maps,
@@ -557,7 +583,7 @@ extern "C" int daam_finalize_maps(const daam_key_group* groups, int32_t n_groups
                 s.block_count);
       return DAAM_E_INVALID;
     }
-    sel[m] = {s.out, s.block_begin, s.block_count, s.n_rows, 0, 0};
+    sel[m] = make_map(s.out, s.block_begin, s.block_count, s.n_rows, 0, n_groups);
     max_rows = std::max(max_rows, s.n_rows);
   }
   DeviceInfo dev;
@@ -570,13 +596,36 @@ extern "C" int daam_finalize_maps(const daam_key_group* groups, int32_t n_groups
                   (long long)maps[m].block_begin + maps[m].block_count, i, groups[i].n_blocks);
         return DAAM_E_INVALID;
       }
+  return launch_finalize(name, groups, n_groups, oh, ow, sel, n_maps, normalize, dev, static_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int daam_finalize_parts(const daam_key_group* groups, int32_t n_groups, const daam_map_part* maps,
+                                   int32_t n_maps, int32_t oh, int32_t ow, int32_t normalize, void* stream_) {
+  const char* name = "daam_finalize_parts";
+  if (!maps || n_maps <= 0) { set_error("%s: no output map", name); return DAAM_E_INVALID; }
+  if (n_maps > kMaxMaps) { set_error("%s: %d maps > %d", name, n_maps, kMaxMaps); return DAAM_E_UNSUPPORTED; }
+  auto bad_map = [&](int m) {
+    set_error("%s: bad map %d (out %p, n_rows %d, groups [%d, +%d) of %d)", name, m, (void*)maps[m].out, maps[m].n_rows,
+              maps[m].group_begin, maps[m].group_count, n_groups);
+    return DAAM_E_INVALID;
+  };
   for (int m = 0; m < n_maps; ++m)
-    if ((long long)keys_per_block * maps[m].block_count > (1 << 30)) {
-      set_error("%s: map %d selects more than 2^30 keys", name, m);
-      return DAAM_E_UNSUPPORTED;
-    }
-  return launch_finalize(groups, n_groups, oh, ow, sel, n_maps, keys_per_block, normalize, dev,
-                         static_cast<cudaStream_t>(stream_));
+    if (!maps[m].out || maps[m].n_rows <= 0 || maps[m].group_begin < 0 || maps[m].group_count <= 0) return bad_map(m);
+  DeviceInfo dev;
+  int n_keys;                                            // every group is checked, read by a map or not
+  if (int rc = check_key_groups(name, groups, n_groups, oh, ow, 1, maps[0].out, &dev, &n_keys)) return rc;
+  MapSel sel[kMaxMaps];
+  for (int m = 0; m < n_maps; ++m) {
+    const daam_map_part& s = maps[m];
+    if ((long long)s.group_begin + s.group_count > n_groups) return bad_map(m);
+    for (int i = s.group_begin; i < s.group_begin + s.group_count; ++i)
+      if (groups[i].tokens < s.n_rows) {
+        set_error("%s: map %d reads %d rows but key group %d holds %d", name, m, s.n_rows, i, groups[i].tokens);
+        return DAAM_E_INVALID;
+      }
+    sel[m] = make_map(s.out, 0, 1, s.n_rows, s.group_begin, s.group_count);
+  }
+  return launch_finalize(name, groups, n_groups, oh, ow, sel, n_maps, normalize, dev, static_cast<cudaStream_t>(stream_));
 }
 
 extern "C" int daam_finalize_per_key(const daam_key_group* groups, int32_t n_groups, int32_t oh, int32_t ow,

@@ -26,7 +26,7 @@ from . import _native
 from .utils import compute_token_merge_indices
 
 __all__ = ['GlobalHeatMap', 'RawHeatMapCollection', 'WordHeatMap', 'LayerSlab', 'GlobalHeatMapStack', 'TimeHeatMaps',
-           'ImageHeatMaps', 'RegionOverlap']
+           'ImageHeatMaps', 'LayerHeatMaps', 'FactorHeatMaps', 'HeadHeatMaps', 'RegionOverlap']
 
 RawHeatMapKey = Tuple[int, int, int]  # factor, layer, head
 
@@ -636,8 +636,9 @@ def _overlay(tokenizer, prompt: str, maps: torch.Tensor, words, image, absolute,
 
 class GlobalHeatMapStack:
     """Global heat maps of one prompt's text stacked along a first axis: ``heat_maps[t]`` is one
-    ``[n_rows, xh, xw]`` map. Base of :class:`TimeHeatMaps` (one map per step) and :class:`ImageHeatMaps` (one per
-    image)."""
+    ``[n_rows, xh, xw]`` map. Base of :class:`TimeHeatMaps` (one map per step), :class:`ImageHeatMaps` (one per
+    image), :class:`LayerHeatMaps`, :class:`FactorHeatMaps` and :class:`HeadHeatMaps` (one per layer, resolution or
+    head)."""
 
     def __init__(self, tokenizer, prompt: str, heat_maps: torch.Tensor):
         self.tokenizer = tokenizer
@@ -717,3 +718,46 @@ class ImageHeatMaps(GlobalHeatMapStack):
     :meth:`~daam_b200.trace.DiffusionHeatMapHooker.compute_global_heat_map` with ``image_idx=i``, the DAAM map over
     image ``i``'s keys only. ``heat_maps`` is ``[images, n_rows, xh, xw]``; ``word_heat_maps`` and ``segment`` work over
     every image."""
+
+
+def _labels(stack: GlobalHeatMapStack, **labels) -> None:
+    """Attach one label list per keyword to ``stack``, each with one entry per map."""
+    for name, values in labels.items():
+        values = list(values)
+        if len(values) != len(stack):
+            raise ValueError(f'{type(stack).__name__}: {len(values)} {name} for {len(stack)} maps')
+        setattr(stack, name, values)
+
+
+class LayerHeatMaps(GlobalHeatMapStack):
+    """One global heat map per traced UNet layer: ``heat_maps[i]`` is exactly
+    :meth:`~daam_b200.trace.DiffusionHeatMapHooker.compute_global_heat_map` with ``layer_idx=layers[i]``, the DAAM map
+    over that layer's heads only. ``layers[i]``, ``names[i]`` (the module path, ``trace.layer_names``) and
+    ``factors[i]`` label map ``i``; ``heat_maps`` is ``[layers, n_rows, xh, xw]``, and the word-list calls work over
+    every layer: e.g. ``layers[region_overlap(...)[1].iou()[:, 0, 0].argmax()]`` is the layer that localises word 0
+    best."""
+
+    def __init__(self, tokenizer, prompt: str, heat_maps: torch.Tensor, layers, names, factors):
+        super().__init__(tokenizer, prompt, heat_maps)
+        _labels(self, layers=layers, names=names, factors=factors)
+
+
+class FactorHeatMaps(GlobalHeatMapStack):
+    """One global heat map per traced resolution: ``heat_maps[j]`` is exactly
+    :meth:`~daam_b200.trace.DiffusionHeatMapHooker.compute_global_heat_map` with ``factors={factors[j]}``;
+    ``factors`` ascends (1 is the finest layer size). ``heat_maps`` is ``[factors, n_rows, xh, xw]``."""
+
+    def __init__(self, tokenizer, prompt: str, heat_maps: torch.Tensor, factors):
+        super().__init__(tokenizer, prompt, heat_maps)
+        _labels(self, factors=factors)
+
+
+class HeadHeatMaps(GlobalHeatMapStack):
+    """One heat map per key: ``heat_maps[i]`` is the map of
+    :meth:`~daam_b200.trace.DiffusionHeatMapHooker.compute_global_heat_map` with ``layer_idx`` and ``head_idx`` of
+    ``keys[i] = (factor, layer, head)``, the reference's ``--all-heads`` sweep. ``heat_maps`` is ``[keys, n_rows, xh,
+    xw]``."""
+
+    def __init__(self, tokenizer, prompt: str, heat_maps: torch.Tensor, keys):
+        super().__init__(tokenizer, prompt, heat_maps)
+        _labels(self, keys=keys)

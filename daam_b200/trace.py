@@ -41,7 +41,8 @@ import torch.nn.functional as F
 
 from . import _native, ops
 from .geometry import LatentGeometry
-from .heatmap import GlobalHeatMap, ImageHeatMaps, LayerSlab, RawHeatMapCollection, TimeHeatMaps
+from .heatmap import (FactorHeatMaps, GlobalHeatMap, HeadHeatMaps, ImageHeatMaps, LayerHeatMaps, LayerSlab,
+                      RawHeatMapCollection, TimeHeatMaps)
 from .hook import AggregateHooker, ObjectHooker, UNetCrossAttentionLocator
 from .utils import cache_dir, context_rows
 
@@ -597,6 +598,10 @@ class DiffusionHeatMapHooker(AggregateHooker):
         ``maps[i]`` the ``[n_tokens + 2, xh, xw]`` heat map the reference computes for that single key. ``step_range=i``
         and ``negative=True`` select the slabs as in :meth:`compute_global_heat_map`; ``image_idx=i`` keeps image
         ``i``'s keys, whose ``head`` then counts that image's heads."""
+        return self._per_head(prompt, factors, normalize, prompt_idx, step_range, negative, image_idx)[1:]
+
+    def _per_head(self, prompt, factors, normalize, prompt_idx, step_range, negative, image_idx):
+        """``(prompt, keys, maps)`` of :meth:`compute_per_head_heat_maps`."""
         prompt, grid, rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range,
                                                               negative=negative, image_idx=image_idx)
         keys = [(slab.factor, slab.layer_idx, head) for slab, g in zip(slabs, groups) for head in range(g.heads)]
@@ -606,7 +611,57 @@ class DiffusionHeatMapHooker(AggregateHooker):
         with torch.cuda.device(device):
             _native.finalize_per_key(groups, grid, n_fin, normalize and n_fin == len(rows), maps.data_ptr(),
                                      torch.cuda.current_stream(device).cuda_stream)
-        return keys, _compact(maps, rows, normalize)
+        return prompt, keys, _compact(maps, rows, normalize)
+
+    def compute_head_heat_maps(self, prompt=None, factors=None, normalize=False, prompt_idx: int = 0, *,
+                               step_range: Optional[int] = None, negative: bool = False,
+                               image_idx: Optional[int] = None) -> HeadHeatMaps:
+        """:meth:`compute_per_head_heat_maps` as a stack the word-list calls work on: a :class:`HeadHeatMaps` whose
+        ``keys[i] = (factor, layer, head)`` labels ``heat_maps[i]``. The stack takes ``keys x rows x xh x xw x 4`` bytes
+        (SD-2.1, 175 keys, 12 rows, 64 x 64: 34 MB; the 1100 keys of SDXL's 60 layers: 216 MB); ``factors`` and ``image_idx`` narrow
+        it."""
+        prompt, keys, maps = self._per_head(prompt, factors, normalize, prompt_idx, step_range, negative, image_idx)
+        return HeadHeatMaps(self.pipe.tokenizer, prompt, maps, keys)
+
+    def compute_layer_heat_maps(self, prompt=None, factors=None, head_idx=None, normalize=False, prompt_idx: int = 0, *,
+                                step_range: Optional[int] = None, negative: bool = False,
+                                image_idx: Optional[int] = None) -> LayerHeatMaps:
+        """Every traced layer's map in one launch (``daam_finalize_parts``): ``heat_maps[i]`` is
+        ``compute_global_heat_map(layer_idx=layers[i], ...)`` with the same arguments, bit for bit. One map per layer
+        that passes the filters (``head_idx``: the layers that have that head), in the order the layers were traced.
+        Returns a :class:`LayerHeatMaps` ``[layers, n_rows, xh, xw]``."""
+        prompt, grid, rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range, None, head_idx,
+                                                              negative, image_idx)
+        maps = self._finalize_parts(groups, [(i, 1) for i in range(len(groups))], grid, rows, normalize, slabs)
+        names = self.layer_names
+        return LayerHeatMaps(self.pipe.tokenizer, prompt, maps, [s.layer_idx for s in slabs],
+                             [names[s.layer_idx] if s.layer_idx < len(names) else None for s in slabs],
+                             [s.factor for s in slabs])
+
+    def compute_factor_heat_maps(self, prompt=None, factors=None, head_idx=None, layer_idx=None, normalize=False,
+                                 prompt_idx: int = 0, *, step_range: Optional[int] = None, negative: bool = False,
+                                 image_idx: Optional[int] = None) -> FactorHeatMaps:
+        """Every traced resolution's map in one launch (``daam_finalize_parts``): ``heat_maps[j]`` is
+        ``compute_global_heat_map(factors={stack.factors[j]}, ...)`` with the same arguments, bit for bit; ``factors``
+        keeps some of them. Returns a :class:`FactorHeatMaps` ``[factors, n_rows, xh, xw]``, factors ascending."""
+        prompt, grid, rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range, layer_idx,
+                                                              head_idx, negative, image_idx)
+        order, found, parts = _factor_parts([s.factor for s in slabs])
+        maps = self._finalize_parts([groups[i] for i in order], parts, grid, rows, normalize, slabs)
+        return FactorHeatMaps(self.pipe.tokenizer, prompt, maps, found)
+
+    def _finalize_parts(self, groups, parts, grid, rows, normalize, slabs) -> torch.Tensor:
+        """One ``daam_finalize_parts`` over ``groups``: map ``m`` reduces groups ``[begin, begin + count)`` of
+        ``parts[m] = (begin, count)`` as a read of those groups alone does. Returns ``[len(parts), len(rows), xh, xw]``."""
+        device = slabs[0].acc.device
+        n_fin = _finalized_rows(rows)
+        out = torch.empty((len(parts), n_fin) + grid, dtype=torch.float32, device=device)
+        sel = [_native.DaamMapPart(group_begin=begin, group_count=count, n_rows=n_fin, out=out[m].data_ptr())
+               for m, (begin, count) in enumerate(parts)]
+        with torch.cuda.device(device):
+            _native.finalize_parts(groups, sel, grid, normalize and n_fin == len(rows),
+                                   torch.cuda.current_stream(device).cuda_stream)
+        return _compact(out, rows, normalize)
 
     def _read_groups(self, prompt, factors, prompt_idx: int, step_range: Optional[int], layer_idx=None, head_idx=None,
                      negative: bool = False, image_idx: Optional[int] = None):
@@ -660,6 +715,21 @@ class DiffusionHeatMapHooker(AggregateHooker):
                                f'context length')
         return prompt, self.geometry.grid, context_rows(len(self.pipe.tokenizer.tokenize(prompt)), tokens.pop()), \
             groups, slabs
+
+
+def _factor_parts(factors: List[int]) -> Tuple[List[int], List[int], List[Tuple[int, int]]]:
+    """The groups of a read, whose factors are ``factors``, partitioned by factor: ``(order, found, parts)`` with
+    ``order`` the stable sort of the group indices by factor (each factor's groups contiguous, in the order a read of
+    that factor alone passes them), ``found`` the distinct factors ascending and ``parts[j] = (begin, count)`` the run
+    of ``found[j]`` in ``order``."""
+    order = sorted(range(len(factors)), key=lambda i: factors[i])
+    found, parts = [], []
+    for pos, i in enumerate(order):
+        if not found or found[-1] != factors[i]:
+            found.append(factors[i])
+            parts.append((pos, 0))
+        parts[-1] = (parts[-1][0], parts[-1][1] + 1)
+    return order, found, parts
 
 
 def _finalized_rows(rows: List[int]) -> int:

@@ -33,7 +33,8 @@ extern "C" {
                                           daam_segment_words, daam_finalize_maps; daam_key_group.reserved is
                                           n_blocks; daam_accumulate takes 154- and 231-token contexts; layers with
                                           several prompts and a prompt stride <= 0 take the SIMT kernel;
-                                          daam_region_overlap; daam_overlay_words, daam_jet_colormap) */
+                                          daam_region_overlap; daam_overlay_words, daam_jet_colormap;
+                                          daam_finalize_parts) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_TOKENS 231     /* daam_accumulate: long contexts of 2 or 3 CLIP chunks of 77 tokens (154, 231) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
@@ -234,6 +235,28 @@ typedef struct daam_map_sel {
 } daam_map_sel;
 int daam_finalize_maps(const daam_key_group* groups, int32_t n_groups, const daam_map_sel* maps, int32_t n_maps,
                        int32_t map_h, int32_t map_w, int32_t normalize, void* stream);
+
+/*
+ * Several daam_finalize maps over SUBSETS of one group list in one launch (e.g. one map per UNet layer, or one per
+ * resolution): map m reduces groups [group_begin, group_begin + group_count) of the call's list and is bit for bit what
+ *   daam_finalize(groups + group_begin, group_count, map_h, map_w, n_rows, normalize, out, stream)
+ * writes: same key order, kernel choice and band height. The kernel choice is daam_finalize's rule applied to the map's
+ * own groups: only their factors, base alignment and key count (2048) decide, so a map whose groups the banded kernel
+ * cannot read goes to the generic kernel while its neighbours stay on the fast one. Ranges may overlap, leave groups
+ * unused, or cover every group, so the all-layers map and the per-layer maps can come out of one call. n_blocks is
+ * ignored, as in daam_finalize. `groups` and `maps` are host memory. One launch per kind of kernel the maps take plus
+ * one normalisation launch.
+ * Limits: n_groups <= 160 and n_maps <= DAAM_FINALIZE_MAX_MAPS (DAAM_E_UNSUPPORTED). DAAM_E_INVALID: what daam_finalize
+ * refuses (a group with fewer tokens than a map that reads it has rows included), no map, a map without output, rows or
+ * groups, a negative group_begin, or a group range past n_groups.
+ */
+typedef struct daam_map_part {
+  int32_t group_begin, group_count;   /* groups [group_begin, group_begin + group_count) of the call's list */
+  int32_t n_rows, reserved;           /* rows [0, n_rows) of the map; reserved: 0 */
+  float* out;                         /* device fp32 [n_rows][map_h][map_w] */
+} daam_map_part;
+int daam_finalize_parts(const daam_key_group* groups, int32_t n_groups, const daam_map_part* maps, int32_t n_maps,
+                        int32_t map_h, int32_t map_w, int32_t normalize, void* stream);
 
 /*
  * The reference's --all-heads sweep calls compute_global_heat_map(layer_idx=l, head_idx=h) once per (layer, head)
