@@ -57,6 +57,14 @@ def upsample64(keys: torch.Tensor, x: int) -> torch.Tensor:
     return by @ keys.double() @ bx.T
 
 
+def up64(keys: torch.Tensor, grid: Tuple[int, int]) -> torch.Tensor:
+    """``[..., h, w]`` -> ``[..., grid[0], grid[1]]``: ``B_y @ key @ B_x^T`` in float64, each axis with its own
+    bicubic matrix (rectangular maps and keys)."""
+    by = bicubic64(keys.shape[-2], grid[0], keys.device)
+    bx = bicubic64(keys.shape[-1], grid[1], keys.device)
+    return by @ keys.double() @ bx.T
+
+
 def _normalize(maps: torch.Tensor) -> torch.Tensor:
     """maps / (sum of rows 1..-2 + 1e-6) per pixel (daam/trace.py:129-130) over the row axis -3."""
     return maps / (maps[..., 1:-1, :, :].sum(dim=-3, keepdim=True) + 1e-6)
@@ -106,6 +114,15 @@ def finalize_tolerance(stacks: Sequence[torch.Tensor], n_keys: int, x: int) -> T
     norm = max(float(bicubic64(s.shape[-1], x, 'cpu').abs().sum(dim=1).max()) for s in stacks)
     vmax = max(float(s.abs().max()) for s in stacks)
     return max(1e-4, (n_keys + 1) * FP32_EPS), 32 * FP32_EPS * norm * norm * vmax
+
+
+def rect_tolerance(stacks: Sequence[torch.Tensor], n_keys: int, grid: Tuple[int, int]) -> Tuple[float, float]:
+    """:func:`finalize_tolerance` with the 1-norms of both axes' bicubic matrices (keys and maps that are not square):
+    ``stacks`` are ``[..., h, w]`` key stacks, ``grid`` the map's ``(h, w)``."""
+    norm = max(float(bicubic64(t.shape[-2], grid[0], 'cpu').abs().sum(dim=1).max()) *
+               float(bicubic64(t.shape[-1], grid[1], 'cpu').abs().sum(dim=1).max()) for t in stacks)
+    vmax = max(float(t.abs().max()) for t in stacks)
+    return max(1e-4, (n_keys + 1) * FP32_EPS), 32 * FP32_EPS * norm * vmax
 
 
 def normalized_tolerance(raw: torch.Tensor, rtol: float, atol: float) -> torch.Tensor:

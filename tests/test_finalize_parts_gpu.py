@@ -113,7 +113,10 @@ def test_a_generic_map_between_fast_maps():
 
 
 def test_off_grid_parts():
-    """SD-2.1 at 600x800: a 75 x 100 map over 75x100 / 38x50 / 19x25 layers (non-integer factors): all generic."""
+    """SD-2.1 at 600x800: a 75 x 100 map over 75x100 / 38x50 / 19x25 layers. Every map that reads a 38x50 or 19x25
+    layer (non-integer factors) takes the generic kernel; the 75x100 layers alone, parts (0, 1) and (4, 1), take the
+    fast one with a partial last band of 3 rows (tests/test_finalize_geometry_gpu.py checks such maps against
+    float64)."""
     layers = [((75, 100), 5), ((38, 50), 10), ((19, 25), 20), ((38, 50), 10), ((75, 100), 5)]
     stacks = _stacks(layers, seed=600)
     for normalize in (False, True):

@@ -21,7 +21,7 @@ from daam_b200 import _native, ops, trace
 from daam_b200.geometry import LatentGeometry
 from daam_b200.testing.synthetic import SD21_SPEC, SDXL_SPEC, TINY_SPEC, UNetSpec, make_pipeline
 from tests.reference64 import (ACC_DIMS, FP32_EPS, MAP_DIMS, assert_close64, bicubic64, layer_maps64,
-                               normalized_tolerance)
+                               normalized_tolerance, rect_tolerance, up64)
 from tests.util import golden, rel_err
 
 pytestmark = pytest.mark.gpu
@@ -237,20 +237,6 @@ def _groups(stacks, head_sel=None):
                                  head_sel=-1 if head_sel is None else head_sel, reserved=0) for t in stacks]
 
 
-def _up64(keys, grid):
-    by = bicubic64(keys.shape[-2], grid[0], keys.device)
-    bx = bicubic64(keys.shape[-1], grid[1], keys.device)
-    return by @ keys.double() @ bx.T
-
-
-def _tolerance(stacks, n_keys, grid):
-    """``finalize_tolerance`` with the 1-norms of both axes' bicubic matrices (the keys here are not square)."""
-    norm = max(float(bicubic64(t.shape[-2], grid[0], 'cpu').abs().sum(dim=1).max()) *
-               float(bicubic64(t.shape[-1], grid[1], 'cpu').abs().sum(dim=1).max()) for t in stacks)
-    vmax = max(float(t.abs().max()) for t in stacks)
-    return max(1e-4, (n_keys + 1) * FP32_EPS), 32 * FP32_EPS * norm * vmax
-
-
 def _finalize(monkeypatch, groups, grid, n_rows, normalize, generic, per_key=0):
     monkeypatch.setenv('DAAM_FINALIZE_GENERIC', '1' if generic else '0')
     out = torch.empty(((per_key,) if per_key else ()) + (n_rows,) + grid, device=DEV)
@@ -274,11 +260,11 @@ def test_finalize_odd_keys_against_float64(monkeypatch, grid, n_rows):
         total, n = None, 0
         for t in stacks:
             sel = t[:, :n_rows] if head_sel is None else t[head_sel:head_sel + 1, :n_rows]
-            part = _up64(sel, grid).clamp_(min=0.0).sum(dim=0)
+            part = up64(sel, grid).clamp_(min=0.0).sum(dim=0)
             total = part if total is None else total + part
             n += sel.shape[0]
         ref = total / n
-        rtol, atol = _tolerance(stacks, n, grid)
+        rtol, atol = rect_tolerance(stacks, n, grid)
         if normalize:
             atol = normalized_tolerance(ref, rtol, atol)
             ref, rtol = _norm64(ref), 0.0
@@ -295,9 +281,9 @@ def test_finalize_odd_keys_against_float64(monkeypatch, grid, n_rows):
         assert torch.equal(bits(out), bits(generic)), f'per-key {grid}: odd keys did not take the generic kernel'
         first = 0
         for t in stacks:
-            raw = _up64(t[:, :n_rows], grid).clamp_(min=0.0)
+            raw = up64(t[:, :n_rows], grid).clamp_(min=0.0)
             for h in range(t.shape[0]):
-                rtol, atol = _tolerance([t[h:h + 1]], 1, grid)
+                rtol, atol = rect_tolerance([t[h:h + 1]], 1, grid)
                 ref = raw[h]
                 if normalize:
                     atol = normalized_tolerance(ref, rtol, atol)
@@ -351,7 +337,7 @@ def _global64(keys, grid, n_rows, factors=None, layer_idx=None, head_idx=None, n
         if factor not in factors or (layer_idx is not None and layer != layer_idx):
             continue
         sel = m[:, :n_rows] if head_idx is None else m[head_idx:head_idx + 1, :n_rows]
-        part = _up64(sel, grid).clamp_(min=0.0).sum(dim=0)
+        part = up64(sel, grid).clamp_(min=0.0).sum(dim=0)
         total = part if total is None else total + part
         n += sel.shape[0]
     out = total / n
@@ -427,7 +413,7 @@ def test_traced_offgrid_maps_against_float64(spec, hw, dtype):
         assert tuple(masks.shape) == (2,) + hw
         assert torch.allclose(masks[0], mask, atol=1e-6)
         for i, (word, row) in enumerate((('dog', 2), ('ball', 6))):
-            ref = _up64(hm.heat_maps[row][None].double(), hw)[0]
+            ref = up64(hm.heat_maps[row][None].double(), hw)[0]
             span = float(ref.max() - ref.min())
             ref = (ref - ref.min()) / (span + 1e-8)
             assert_close64(masks[i], ref, 0.0, _expand_tolerance(hm.heat_maps[row], hw, span), f'expand_words {word}')
@@ -435,7 +421,7 @@ def test_traced_offgrid_maps_against_float64(spec, hw, dtype):
         assert len(per_head_keys) == per_head.shape[0] > 0
         for (factor, layer, head), got in zip(per_head_keys, per_head):
             assert factor in DEFAULT_FACTORS
-            ref = _up64(keys[layer][1][head, :n_rows], geo.grid).clamp_(min=0.0)
+            ref = up64(keys[layer][1][head, :n_rows], geo.grid).clamp_(min=0.0)
             assert_close64(got, ref, RTOL, ATOL * steps, f'per-head {(factor, layer, head)}', MAP_DIMS)
 
 
