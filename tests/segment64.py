@@ -3,7 +3,8 @@ under. ``tests/test_segment_host.py`` pins :func:`segment64` to the oracle's ``p
 followed by an argmax; ``tests/test_segment_gpu.py`` compares the kernel's labels with it."""
 import torch
 
-from tests.reference64 import FP32_EPS, bicubic64
+from tests.reference64 import bicubic64
+from tests.words64 import expand64, expand_bound
 
 
 def segment64(maps, rows_per_word, hw, absolute, threshold):
@@ -25,24 +26,10 @@ def segment64(maps, rows_per_word, hw, absolute, threshold):
 
 
 def label_bound(words, by, bx, rows_per_word, absolute):
-    """Per-word bound on |fp32 normalised value - float64 value|, from the error analysis, not from observed errors:
-
-    * word map: a mean of ``k`` fp32 rows, relative error below ``(k + 1) 2^-24``;
-    * interpolation: a 16-tap stencil in fp32, error below ``32 2^-24 N_y N_x max|W|`` (``N`` the largest row 1-norm of
-      the bicubic matrix of each axis, as in ``finalize_tolerance``), plus the word map's error times ``N_y N_x``;
-    * normalisation: with ``E`` that bound for v, lo and hi (lo and hi are values of v) and ``D = hi - lo + 1e-8``,
-      ``|d((v - lo) / D)| <= 2E / D + 2E / D + 3 2^-24`` (the quotient is at most 1).
-    Absolute maps keep ``E``."""
-    ny = float(by.abs().sum(1).max())
-    nx = float(bx.abs().sum(1).max())
-    out = []
-    for w, rows in zip(words, rows_per_word):
-        vmax = float(w.abs().max())
-        e = 32 * FP32_EPS * ny * nx * vmax + (len(rows) + 1) * FP32_EPS * vmax * ny * nx
-        if absolute:
-            out.append(e)
-        else:
-            up = by @ w @ bx.T
-            d = float(up.max() - up.min()) + 1e-8
-            out.append(4 * e / d + 3 * FP32_EPS)
-    return max(out)
+    """Per pixel, a bound on |fp32 value - float64 value| of every word: :func:`tests.words64.expand_bound` (the fp32
+    row mean, the 16-tap stencil, the fp32 source coordinate of ``make_taps`` and, unless ``absolute``, the min-max
+    normalisation) for each word at the pixel, the largest over the words. ``words``: the float64 word maps of
+    non-negative global maps."""
+    out_hw = (by.shape[0], bx.shape[0])
+    bound = expand_bound(words, out_hw, absolute, [len(r) for r in rows_per_word], exp=expand64(words, out_hw, True))
+    return bound.amax(0)

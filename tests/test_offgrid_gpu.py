@@ -23,6 +23,7 @@ from daam_b200.testing.synthetic import SD21_SPEC, SDXL_SPEC, TINY_SPEC, UNetSpe
 from tests.reference64 import (ACC_DIMS, FP32_EPS, MAP_DIMS, assert_close64, bicubic64, layer_maps64,
                                normalized_tolerance, rect_tolerance, up64)
 from tests.util import golden, rel_err
+from tests.words64 import expand_bound
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
@@ -344,15 +345,11 @@ def _global64(keys, grid, n_rows, factors=None, layer_idx=None, head_idx=None, n
     return out / (out[1:-1].sum(dim=0, keepdim=True) + 1e-6) if normalize else out
 
 
-def _expand_tolerance(word_map, out_hw, span):
-    """Absolute bound of a min-max normalised fp32 up-sample (``expand_as``) at a non-integer ratio, whose cubic weights
-    are rounded to fp32: each value errs by less than ``32 * 2^-24 * N^2 * max |v|`` (``finalize_tolerance``'s stencil
-    bound, ``N`` the bicubic matrices' largest row 1-norm), the min and the max by as much again, and ``span`` (the
-    exact max - min) divides them; plus the rounding of the subtraction and the division."""
-    ny = float(bicubic64(word_map.shape[-2], out_hw[0], 'cpu').abs().sum(dim=1).max())
-    nx = float(bicubic64(word_map.shape[-1], out_hw[1], 'cpu').abs().sum(dim=1).max())
-    t = 32 * FP32_EPS * ny * nx * float(word_map.abs().max())
-    return 2 * t / span + 4 * FP32_EPS
+def _expand_tolerance(word_map, out_hw):
+    """Per-element bound of a min-max normalised fp32 up-sample (``expand_as``) of the fp32 ``word_map`` (one row, so
+    its word map is exact) against float64: :func:`tests.words64.expand_bound`, which covers the stencil's rounding,
+    the fp32 source coordinate at ratios that are not powers of two, and the normalisation."""
+    return expand_bound(word_map.double()[None], out_hw, absolute=False)[0]
 
 
 def _image(h, w):
@@ -416,7 +413,8 @@ def test_traced_offgrid_maps_against_float64(spec, hw, dtype):
             ref = up64(hm.heat_maps[row][None].double(), hw)[0]
             span = float(ref.max() - ref.min())
             ref = (ref - ref.min()) / (span + 1e-8)
-            assert_close64(masks[i], ref, 0.0, _expand_tolerance(hm.heat_maps[row], hw, span), f'expand_words {word}')
+            assert_close64(masks[i], ref, 0.0, _expand_tolerance(hm.heat_maps[row], hw).to(masks.device),
+                           f'expand_words {word}')
         per_head_keys, per_head = tc.compute_per_head_heat_maps()
         assert len(per_head_keys) == per_head.shape[0] > 0
         for (factor, layer, head), got in zip(per_head_keys, per_head):
