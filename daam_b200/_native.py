@@ -38,6 +38,15 @@ def region_scratch_floats(n_maps: int, n_words: int, n_regions: int, out_h: int,
     return n_maps * n_words * (64 + (n_regions + 1) * ((out_h + 15) // 16) * ((out_w + 63) // 64))
 
 
+WORD_OVERLAP_CTAS = 256      # DAAM_WORD_OVERLAP_CTAS: daam_word_overlap's CTAs per map
+
+
+def word_overlap_scratch_floats(n_maps: int, n_words: int, out_h: int, out_w: int) -> int:
+    """``DAAM_WORD_OVERLAP_SCRATCH_FLOATS(n_maps, n_words, out_h, out_w)``."""
+    tiles = ((out_h + 15) // 16) * ((out_w + 63) // 64)
+    return n_maps * (n_words * 64 + (n_words * (n_words + 3) // 2) * min(tiles, WORD_OVERLAP_CTAS))
+
+
 def overlay_frames_bytes(n_maps: int, n_words: int, out_h: int, out_w: int) -> int:
     """``DAAM_OVERLAY_FRAMES_BYTES(n_maps, n_words, out_h, out_w)``: the frames rounded up to whole 4-byte words."""
     return (n_maps * n_words * out_h * out_w * 3 + 3) // 4 * 4
@@ -45,7 +54,7 @@ def overlay_frames_bytes(n_maps: int, n_words: int, out_h: int, out_w: int) -> i
 
 EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize',
            'daam_finalize_maps', 'daam_finalize_parts', 'daam_finalize_per_key','daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
-           'daam_segment_words', 'daam_region_overlap', 'daam_overlay_words', 'daam_jet_colormap',
+           'daam_segment_words', 'daam_region_overlap', 'daam_word_overlap', 'daam_overlay_words', 'daam_jet_colormap',
            'daam_side_launcher_create', 'daam_side_launcher_destroy',
            'daam_side_launcher_launch', 'daam_side_launcher_join', 'daam_side_launcher_idle', 'daam_abi_version',
            'daam_last_error', 'daam_device_info', 'daam_launch_count')
@@ -152,6 +161,9 @@ def load() -> ctypes.CDLL:
     lib.daam_region_overlap.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
                                         i32, i32, f32, vp, vp, i32, vp, vp, vp, vp]
     lib.daam_region_overlap.restype = ctypes.c_int
+    lib.daam_word_overlap.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
+                                      i32, i32, f32, vp, vp, vp, vp, vp]
+    lib.daam_word_overlap.restype = ctypes.c_int
     lib.daam_overlay_words.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
                                        i32, i32, f32, i32, vp, vp, i64, vp, vp, vp]
     lib.daam_overlay_words.restype = ctypes.c_int
@@ -407,6 +419,17 @@ def region_overlap(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Se
                                       ctypes.c_void_p(word_maps_ptr), ctypes.c_void_p(regions_ptr), n_regions,
                                       ctypes.c_void_p(intersection_ptr), ctypes.c_void_p(word_area_ptr),
                                       ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
+
+
+def word_overlap(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int,
+                 out_w: int, absolute: bool, threshold: Optional[float], word_maps_ptr: int, intersection_ptr: int,
+                 word_area_ptr: int, scratch_ptr: int, stream: int):
+    """``daam_word_overlap`` over ``n_maps`` maps ``[n_rows, h, w]`` back to back: ``intersection`` ``[n_maps, n_words,
+    n_words]``, ``word_area`` ``[n_maps, n_words]``."""
+    _check(load().daam_word_overlap(ctypes.c_void_p(maps_ptr), n_maps, n_rows,
+                                    *_word_list(x, rows_per_word, out_h, out_w, absolute, threshold),
+                                    ctypes.c_void_p(word_maps_ptr), ctypes.c_void_p(intersection_ptr),
+                                    ctypes.c_void_p(word_area_ptr), ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
 
 
 def overlay_words(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int,

@@ -12,11 +12,12 @@
 //  - expand_words_kernel writes it (one cooperative launch, steps 1, 2 and 4 in one kernel);
 //  - segment_label_kernel keeps each pixel's max / argmax over the words;
 //  - region_tile_kernel sums it over binary image regions (then region_reduce_kernel);
-//  - overlay_kernel blends its jet colour onto the image.
+//  - overlay_kernel blends its jet colour onto the image;
+//  - word_pair_tile_kernel sums m[a] * m[b] over every pair of words (then word_pair_reduce_kernel).
 // The tile kernels run after segment_minmax_kernel (steps 1 and 2, the word maps and min / max partials to global
-// memory); region_tile_kernel and overlay_kernel share the tile helpers (block_tile, word_bounds, stage_windows, tap
-// tables). expand_words_kernel, segment_minmax_kernel and segment_label_kernel keep their steps inline: written with
-// the helpers, nvcc scheduled them differently and they measured slower. Every consumer's m is expand_words_kernel's
+// memory); region_tile_kernel, overlay_kernel and word_pair_tile_kernel share the tile helpers (block_tile / tile_at,
+// word_bounds, stage_windows, tap tables). expand_words_kernel, segment_minmax_kernel and segment_label_kernel keep
+// their steps inline: written with the helpers, nvcc scheduled them differently and they measured slower. Every consumer's m is expand_words_kernel's
 // value bit for bit. Deterministic: no atomics.
 #include <cooperative_groups.h>
 #include <math.h>
@@ -198,10 +199,10 @@ struct Tile {
   int y0, x0, th, tw, wy, wx, wh, ww, wn;
 };
 
-__device__ __forceinline__ Tile block_tile(const WordListParams& P) {
+__device__ __forceinline__ Tile tile_at(const WordListParams& P, unsigned tile) {
   const int tiles_x = (P.ow + kSegTileW - 1) / kSegTileW;
   Tile t;
-  t.y0 = (blockIdx.x / tiles_x) * kSegTileH; t.x0 = (blockIdx.x % tiles_x) * kSegTileW;
+  t.y0 = (tile / tiles_x) * kSegTileH; t.x0 = (tile % tiles_x) * kSegTileW;
   t.th = min(kSegTileH, P.oh - t.y0); t.tw = min(kSegTileW, P.ow - t.x0);
   t.wy = make_taps(t.y0, P.mh, P.oh).idx[0]; t.wx = make_taps(t.x0, P.mw, P.ow).idx[0];
   t.wh = make_taps(t.y0 + t.th - 1, P.mh, P.oh).idx[3] - t.wy + 1;
@@ -209,6 +210,8 @@ __device__ __forceinline__ Tile block_tile(const WordListParams& P) {
   t.wn = t.wh * t.ww;
   return t;
 }
+
+__device__ __forceinline__ Tile block_tile(const WordListParams& P) { return tile_at(P, blockIdx.x); }
 
 // min / max of v of (map, word w), reduced from segment_minmax_kernel's chunks in a fixed order; 0 / 0 without minmax
 __device__ __forceinline__ void word_bounds(const WordListParams& P, int map, int w, float& lo, float& hi) {
@@ -475,6 +478,181 @@ __global__ void __launch_bounds__(256) region_reduce_kernel(const float* __restr
     } else {
       const long long map = mword / n_words, word = mword - map * n_words;
       intersection[(map * n_regions + slot - 1) * n_words + word] = s;
+    }
+  }
+}
+
+// ---- word-pair overlap: sums of m[a] * m[b] over the image --------------------------------------------------------
+//   intersection[map][a][b] = intersection[map][b][a] = sum_p m[a](p) m[b](p),   word_area[map][a] = sum_p m[a](p)
+// Slots: the n_words (n_words + 1) / 2 pairs a <= b row by row, then the n_words areas. CTA c of a map reduces tiles
+// c, c + ctas, ... (ctas = min(tiles, kPairCtas): the same for every map count, so that a map's sums do not depend on
+// the other maps of the call) into one partial per slot, kept in shared memory and owned by one thread (with a threshold) or one
+// warp (without); word_pair_reduce_kernel sums the CTAs' partials in a fixed order and writes each pair twice.
+//  - with a threshold every m is 0 or 1: each word's tile mask is 32 ballot words, and a pair's count is the popcount
+//    of their AND. The counts are integers, so the sums are exact.
+//  - without: the m of every word over 256 of the tile's pixels at a time go to shared memory; a warp's lanes take 8
+//    of those pixels each per slot, in pixel order, then a butterfly.
+constexpr int kPairChunk = 256;                     // pixels per step without a threshold: one per thread
+constexpr int kPairMaskStride = 33;                 // a word's 32 ballot words, padded: the words' masks on other banks
+constexpr int kPairCtas = DAAM_WORD_OVERLAP_CTAS;   // CTAs per map, at most one per tile
+
+struct PairParams {
+  WordListParams s;                     // words_per_pass 0: windows are not staged, m is read from the word maps
+  float* partials;                      // [n_maps][slots][ctas]
+  int tiles, ctas;                      // tiles of a map; CTAs per map
+};
+
+__host__ __device__ __forceinline__ int pair_count(int n_words) { return n_words * (n_words + 1) / 2; }
+
+// pair slot s < pair_count(n_words) -> words a <= b
+__host__ __device__ __forceinline__ void pair_words(int s, int n_words, int& a, int& b) {
+  a = 0;
+  while (s >= n_words - a) { s -= n_words - a; ++a; }
+  b = a + s;
+}
+
+// the dynamic shared memory word_pair_tile_kernel keeps before its windows, in floats: the pair table (two bytes a
+// pair), the slots' partials, and the masks or the values of a chunk
+__host__ __device__ __forceinline__ int pair_smem_floats(int n_words, int use_threshold) {
+  const int pairs = pair_count(n_words);
+  return (pairs + 1) / 2 + pairs + n_words + n_words * (use_threshold ? kPairMaskStride : kPairChunk);
+}
+
+// grid: (ctas, n_maps); dynamic smem: pair_smem_floats, then words_per_pass source windows
+__global__ void __launch_bounds__(256) word_pair_tile_kernel(const __grid_constant__ PairParams Q) {
+  extern __shared__ __align__(16) float smem[];
+  __shared__ float s_lo[kMaxWords], s_hi[kMaxWords];
+  __shared__ TapTables taps;
+  const WordListParams& P = Q.s;
+  const int map = blockIdx.y, n_words = P.n_words, mh = P.mh, mw = P.mw;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int pairs = pair_count(n_words), n_slots = pairs + n_words;
+  unsigned short* pair_ab = reinterpret_cast<unsigned short*>(smem);          // a << 8 | b
+  float* acc = smem + (pairs + 1) / 2;                                        // [n_slots]
+  unsigned* counts = reinterpret_cast<unsigned*>(acc);                        // acc, with a threshold
+  unsigned* masks = reinterpret_cast<unsigned*>(acc + n_slots);               // [n_words][kPairMaskStride]
+  float* vals = acc + n_slots;                                                // [n_words][kPairChunk]
+  float* win = smem + pair_smem_floats(n_words, P.use_threshold);
+  for (int w = threadIdx.x; w < n_words; w += blockDim.x) word_bounds(P, map, w, s_lo[w], s_hi[w]);
+  for (int s = threadIdx.x; s < pairs; s += blockDim.x) {
+    int a, b;
+    pair_words(s, n_words, a, b);
+    pair_ab[s] = (unsigned short)(a << 8 | b);
+  }
+  for (int s = threadIdx.x; s < n_slots; s += blockDim.x) acc[s] = 0.f;     // also counts = 0
+  const float* word_maps = P.word_maps + (long long)map * n_words * mh * mw;
+  const bool staged = P.words_per_pass > 0;
+  const int per_pass = staged ? P.words_per_pass : n_words;
+  for (int tile = blockIdx.x; tile < Q.tiles; tile += Q.ctas) {
+    const Tile T = tile_at(P, tile);
+    const int n_pix = T.th * T.tw;
+    __syncthreads();                                   // the previous tile has read the tap tables and buffers
+    fill_tap_tables(P, T, taps);
+    if (!staged) __syncthreads();                      // (stage_windows' barriers publish them otherwise)
+    // m of word w (window wi of the pass) at tile pixel p < n_pix
+    auto value = [&](int w, int wi, int p) {
+      const int py = p / T.tw;
+      Taps ty, tx;
+      tile_taps(taps, py, p - py * T.tw, ty, tx);
+      float v;
+      if (staged) {
+        v = bicubic_shared(win + wi * T.wn, T.ww, ty, tx);
+      } else {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) { ty.idx[j] += T.wy; tx.idx[j] += T.wx; }
+        v = bicubic_at(word_maps + (long long)w * mh * mw, mw, ty, tx);
+      }
+      return word_value(P, v, s_lo[w], s_hi[w]);
+    };
+    if (P.use_threshold) {
+      for (int w0 = 0; w0 < n_words; w0 += per_pass) {
+        const int nw = min(per_pass, n_words - w0);
+        if (staged) stage_windows(P, T, word_maps, w0, nw, win);
+        for (int wi = 0; wi < nw; ++wi) {
+#pragma unroll
+          for (int k = 0; k < kSegPix; ++k) {
+            const int p = threadIdx.x + 256 * k;
+            const unsigned bits = __ballot_sync(0xffffffffu, p < n_pix && value(w0 + wi, wi, p) != 0.f);
+            if (lane == 0) masks[(w0 + wi) * kPairMaskStride + 8 * k + warp] = bits;
+          }
+        }
+      }
+      __syncthreads();
+      for (int s = threadIdx.x; s < n_slots; s += blockDim.x) {
+        unsigned c = 0;
+        if (s < pairs) {
+          const unsigned* ma = masks + (pair_ab[s] >> 8) * kPairMaskStride;
+          const unsigned* mb = masks + (pair_ab[s] & 255) * kPairMaskStride;
+#pragma unroll 8
+          for (int j = 0; j < 32; ++j) c += __popc(ma[j] & mb[j]);
+        } else {
+          const unsigned* ma = masks + (s - pairs) * kPairMaskStride;
+#pragma unroll 8
+          for (int j = 0; j < 32; ++j) c += __popc(ma[j]);
+        }
+        counts[s] += c;
+      }
+    } else {
+      const bool restage = staged && per_pass < n_words;   // one pass: the windows stay for every chunk
+      for (int c0 = 0; c0 < n_pix; c0 += kPairChunk) {
+        const int p = c0 + threadIdx.x;
+        for (int w0 = 0; w0 < n_words; w0 += per_pass) {
+          const int nw = min(per_pass, n_words - w0);
+          if (staged && (c0 == 0 || restage)) stage_windows(P, T, word_maps, w0, nw, win);
+          for (int wi = 0; wi < nw; ++wi) vals[(w0 + wi) * kPairChunk + threadIdx.x] = p < n_pix ? value(w0 + wi, wi, p) : 0.f;
+        }
+        __syncthreads();
+        for (int s = warp; s < n_slots; s += 8) {
+          float x = 0.f;
+          if (s < pairs) {
+            const float* va = vals + (pair_ab[s] >> 8) * kPairChunk + lane;
+            const float* vb = vals + (pair_ab[s] & 255) * kPairChunk + lane;
+#pragma unroll
+            for (int i = 0; i < kPairChunk / 32; ++i) x = fmaf(va[32 * i], vb[32 * i], x);
+          } else {
+            const float* va = vals + (s - pairs) * kPairChunk + lane;
+#pragma unroll
+            for (int i = 0; i < kPairChunk / 32; ++i) x += va[32 * i];
+          }
+#pragma unroll
+          for (int h = 16; h > 0; h >>= 1) x += __shfl_xor_sync(0xffffffffu, x, h);
+          if (lane == 0) acc[s] += x;
+        }
+        __syncthreads();                                 // the next chunk rewrites vals
+      }
+    }
+  }
+  __syncthreads();
+  float* partials = Q.partials + (long long)map * n_slots * Q.ctas + blockIdx.x;
+  for (int s = threadIdx.x; s < n_slots; s += blockDim.x)
+    partials[(long long)s * Q.ctas] = P.use_threshold ? (float)counts[s] : acc[s];
+}
+
+// grid: ceil(n_out / 8), 256 threads; one warp per output o = map * slots + slot sums the CTAs' partials (lane-strided,
+// then a butterfly) in a fixed order; a pair's sum goes to both of its intersection elements
+__global__ void __launch_bounds__(256) word_pair_reduce_kernel(const float* __restrict__ partials, long long n_out,
+                                                               int ctas, int n_words, float* __restrict__ intersection,
+                                                               float* __restrict__ area) {
+  const long long o = (long long)blockIdx.x * 8 + (threadIdx.x >> 5);
+  if (o >= n_out) return;                              // whole warps
+  const int lane = threadIdx.x & 31;
+  const float* src = partials + o * ctas;
+  float s = 0.f;
+  for (int c = lane; c < ctas; c += 32) s += __ldg(src + c);
+#pragma unroll
+  for (int h = 16; h > 0; h >>= 1) s += __shfl_xor_sync(0xffffffffu, s, h);
+  if (lane == 0) {
+    const int pairs = pair_count(n_words), n_slots = pairs + n_words;
+    const long long map = o / n_slots;
+    const int slot = (int)(o - map * n_slots);
+    if (slot < pairs) {
+      int a, b;
+      pair_words(slot, n_words, a, b);
+      float* out = intersection + map * n_words * n_words;
+      out[a * n_words + b] = s;
+      out[b * n_words + a] = s;
+    } else {
+      area[map * n_words + slot - pairs] = s;
     }
   }
 }
@@ -792,9 +970,13 @@ static int tile_count(const WordListParams& p) {
 }
 
 // The tile entry points' launches after word_list_prepare: segment_minmax_kernel over (map, word, chunk), then
-// `kernel` over (tile, map). Sets k.s.chunks and k.s.words_per_pass.
+// `kernel` over (tile, map), or over (CTA, map) with `ctas` CTAs per map. `smem_before`: the bytes of dynamic shared
+// memory the kernel keeps before its windows; such a kernel stages as many words' windows as fit beside them (it
+// stages them again per pixel chunk when they take several passes). Sets k.s.chunks and k.s.words_per_pass;
+// words_per_pass 0 (only with smem_before): not one window fits, and the kernel reads the word maps instead.
 template <class Params>
-static int launch_tiles(void (*kernel)(Params), Params& k, int n_maps, const DeviceInfo& dev, cudaStream_t stream) {
+static int launch_tiles(void (*kernel)(Params), Params& k, int n_maps, const DeviceInfo& dev, cudaStream_t stream,
+                        int ctas = 0, size_t smem_before = 0) {
   WordListParams& p = k.s;
   // launch 1: enough (map, word, chunk) CTAs for a few waves, at most kMaxChunks per word and one per 256 pixels
   const long long n = (long long)p.oh * p.ow, mwords = (long long)n_maps * p.n_words;
@@ -807,12 +989,17 @@ static int launch_tiles(void (*kernel)(Params), Params& k, int n_maps, const Dev
   const int win_h = std::min<int>(p.mh, (int)ceil((double)kSegTileH * p.mh / p.oh) + 5);
   const int win_w = std::min<int>(p.mw, (int)ceil((double)kSegTileW * p.mw / p.ow) + 5);
   const int win = win_h * win_w;
-  p.words_per_pass = std::max(1, std::min(p.n_words, kSegStageFloats / win));
+  if (smem_before)
+    p.words_per_pass = (int)std::min<size_t>(p.n_words, (kMaxSmem - smem_before) / (win * sizeof(float)));
+  else
+    p.words_per_pass = std::max(1, std::min(p.n_words, kSegStageFloats / win));
+  const size_t smem = smem_before + (size_t)p.words_per_pass * win * sizeof(float);
   static std::once_flag attr_once[64];
   cudaError_t attr_err = cudaSuccess;
   std::call_once(attr_once[dev.device & 63], [&] {
     const void* kernels[] = {(const void*)segment_minmax_kernel, (const void*)segment_label_kernel,
-                             (const void*)region_tile_kernel, (const void*)overlay_kernel};
+                             (const void*)region_tile_kernel, (const void*)overlay_kernel,
+                             (const void*)word_pair_tile_kernel};
     for (const void* f : kernels)
       if (attr_err == cudaSuccess) attr_err = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
   });
@@ -820,7 +1007,7 @@ static int launch_tiles(void (*kernel)(Params), Params& k, int n_maps, const Dev
   segment_minmax_kernel<<<(unsigned)(mwords * p.chunks), 256, (size_t)p.mh * p.mw * sizeof(float), stream>>>(p);
   DAAM_CUDA_TRY(cudaGetLastError());
   count_launch();
-  kernel<<<dim3(tile_count(p), n_maps), 256, (size_t)p.words_per_pass * win * sizeof(float), stream>>>(k);
+  kernel<<<dim3(ctas ? ctas : tile_count(p), n_maps), 256, smem, stream>>>(k);
   DAAM_CUDA_TRY(cudaGetLastError());
   count_launch();
   return DAAM_OK;
@@ -863,6 +1050,34 @@ extern "C" int daam_region_overlap(const float* global_maps, int32_t n_maps, int
   const long long n_out = (long long)n_maps * n_words * (n_regions + 1);
   region_reduce_kernel<<<(unsigned)((n_out + 7) / 8), 256, 0, stream>>>(p.partials, n_out, p.tiles, n_words, n_regions,
                                                                         intersection, word_area);
+  DAAM_CUDA_TRY(cudaGetLastError());
+  count_launch();
+  return DAAM_OK;
+}
+
+extern "C" int daam_word_overlap(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t mh, int32_t mw,
+                                 const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h,
+                                 int32_t out_w, int32_t absolute, int32_t use_threshold, float threshold,
+                                 float* word_maps, float* intersection, float* word_area, float* scratch,
+                                 void* stream_) {
+  const char* name = "daam_word_overlap";
+  if (!global_maps || !rows || !row_begin || !word_maps || !intersection || !word_area || !scratch || n_maps <= 0 ||
+      mh <= 0 || mw <= 0 || out_h <= 0 || out_w <= 0 || n_rows <= 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
+  // fp32 partial sums of 0/1 values stay exact integers up to 2^24
+  if ((long long)out_h * out_w > (1LL << 24)) { set_error("%s: a %d x %d output is more than 2^24 pixels", name, out_h, out_w); return DAAM_E_UNSUPPORTED; }
+  static thread_local PairParams p;
+  DeviceInfo dev;
+  if (int rc = word_list_prepare(name, global_maps, n_maps, n_rows, mh, mw, rows, row_begin, n_words, out_h, out_w,
+                                 absolute, !absolute, use_threshold, threshold, word_maps, scratch, true, p.s, &dev)) return rc;
+  p.tiles = tile_count(p.s);
+  p.ctas = std::min(p.tiles, kPairCtas);
+  p.partials = scratch + 64LL * n_maps * n_words;     // after segment_minmax_kernel's min / max partials
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (int rc = launch_tiles(word_pair_tile_kernel, p, n_maps, dev, stream, p.ctas,
+                            (size_t)pair_smem_floats(n_words, p.s.use_threshold) * sizeof(float))) return rc;
+  const long long n_out = (long long)n_maps * (pair_count(n_words) + n_words);
+  word_pair_reduce_kernel<<<(unsigned)((n_out + 7) / 8), 256, 0, stream>>>(p.partials, n_out, p.ctas, n_words,
+                                                                           intersection, word_area);
   DAAM_CUDA_TRY(cudaGetLastError());
   count_launch();
   return DAAM_OK;

@@ -18,7 +18,7 @@ from __future__ import annotations
 from dataclasses import dataclass
 from functools import lru_cache
 from types import SimpleNamespace
-from typing import Dict, Iterator, List, Optional, Set, Tuple
+from typing import Dict, Iterator, List, Optional, Set, Tuple, Union
 
 import torch
 
@@ -26,7 +26,7 @@ from . import _native
 from .utils import compute_token_merge_indices
 
 __all__ = ['GlobalHeatMap', 'RawHeatMapCollection', 'WordHeatMap', 'LayerSlab', 'GlobalHeatMapStack', 'TimeHeatMaps',
-           'ImageHeatMaps', 'LayerHeatMaps', 'FactorHeatMaps', 'HeadHeatMaps', 'RegionOverlap']
+           'ImageHeatMaps', 'LayerHeatMaps', 'FactorHeatMaps', 'HeadHeatMaps', 'RegionOverlap', 'WordOverlap', 'RelationOverlap']
 
 RawHeatMapKey = Tuple[int, int, int]  # factor, layer, head
 
@@ -422,6 +422,44 @@ class GlobalHeatMap:
         return (_word_heat_maps(word_maps[0], words, merged),
                 RegionOverlap(overlap.intersection[0], overlap.word_area[0], overlap.region_area))
 
+    def word_overlap(self, words, image=None, absolute: bool = False, threshold: Optional[float] = None,
+                     word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
+        """How much each word's expanded map overlaps every other word's: the sums behind ``compute_iou`` /
+        ``compute_ioa`` (``daam/evaluate.py``) and ``WordHeatMap.compute_ioa`` for every pair of ``words`` at once. With
+        ``m`` the ``[len(words), H, W]`` that ``expand_words(words, image, absolute, threshold, word_idx, offset_idx)``
+        returns (0/1 masks when ``threshold`` is in effect), the :class:`WordOverlap` holds ``intersection[a, b] =
+        (m[a] * m[b]).sum()`` (symmetric bit for bit) and ``word_area[a] = m[a].sum()``; its ``iou()`` / ``ioa()`` equal
+        ``compute_iou`` / ``compute_ioa`` of every pair of masks, bit for bit, when the threshold is in effect.
+        ``image=None`` sums over the heat-map grid itself, where ``m`` is the word heat map (normalised unless
+        ``absolute``): ``word_overlap(words, absolute=True, threshold=0.15)`` is the DAAM paper's head / dependent
+        recipe. Three fused launches; the ``[len(words), H, W]`` stack is never materialised.
+
+        Returns ``(word_heat_maps, overlap)``: the list of :class:`WordHeatMap` that :meth:`segment` returns and the
+        :class:`WordOverlap` (CPU by default, ``to_cpu=False`` keeps it on the device). At most 96 words and 2**24
+        pixels. An empty word list launches nothing and returns empty axes. Raises the reference's ``ValueError`` for a
+        word that is not in the prompt."""
+        words = list(words)
+        word_maps, merged, overlap = _word_overlap(self.tokenizer, self.prompt, self.heat_maps[None], words, image,
+                                                   absolute, threshold, word_idx, offset_idx, to_cpu,
+                                                   'GlobalHeatMap.word_overlap')
+        return (_word_heat_maps(word_maps[0], words, merged),
+                WordOverlap(overlap.intersection[0], overlap.word_area[0]))
+
+    def relation_overlap(self, relations, image=None, absolute: bool = False, threshold: Optional[float] = None,
+                         offset_idx: int = 0, to_cpu: bool = True) -> 'RelationOverlap':
+        """The overlap of head and dependent of every relation of a parse -- what the reference's
+        ``dependency_relations()`` pairs up, scored the way the DAAM paper's visuosyntactic analysis scores it, for a
+        parse from any parser. ``relations``: ``(head, dep, rel)`` triples whose endpoints are words (``str``, looked up
+        like ``compute_word_heat_map(word)``, every occurrence merged) or prompt token indices (``int``, as
+        ``word_idx``). An edge with a word that is not in the prompt is skipped, as the reference does. The distinct
+        endpoints go through one :meth:`word_overlap` call (at most 96); the returned :class:`RelationOverlap` gathers
+        ``iou``, ``iod = ioa()[dep, head]`` and ``ioh = ioa()[head, dep]`` per kept edge. ``relation_overlap(relations,
+        absolute=True, threshold=0.15)`` reproduces the paper's per-edge iou / iod / ioh."""
+        rel = _relation_overlap(self.tokenizer, self.prompt, self.heat_maps[None], relations, image, absolute, threshold,
+                                offset_idx, to_cpu, 'GlobalHeatMap.relation_overlap')
+        ov = WordOverlap(rel.overlap.intersection[0], rel.overlap.word_area[0])
+        return RelationOverlap(rel.relations, rel.kept, rel.words, ov, rel.iou[0], rel.iod[0], rel.ioh[0])
+
     def overlay_words(self, words, image, absolute: bool = False, threshold: Optional[float] = None,
                       color_normalize: bool = True, word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
         """The reference's ``plot_overlay`` (heatmap.py:20-53, 66-75) as pixels, for a word list: each word's expanded
@@ -569,8 +607,108 @@ def _region_overlap(tokenizer, prompt: str, maps: torch.Tensor, words, image, re
     return wl.word_maps, wl.merged, (_to_cpu(ov) if to_cpu else ov)
 
 
-def _to_cpu(ov: RegionOverlap) -> RegionOverlap:
+def _to_cpu(ov):
+    """A :class:`RegionOverlap` or :class:`WordOverlap` with every tensor copied to the host."""
+    if isinstance(ov, WordOverlap):
+        return WordOverlap(ov.intersection.cpu(), ov.word_area.cpu())
     return RegionOverlap(ov.intersection.cpu(), ov.word_area.cpu(), ov.region_area.cpu())
+
+
+@dataclass
+class WordOverlap:
+    """Sums of products of word maps (:meth:`GlobalHeatMap.word_overlap`): ``intersection`` ``[..., W, W]``
+    (``sum_p m[a](p) * m[b](p)``, symmetric) and ``word_area`` ``[..., W]`` (``sum_p m[a](p)``), fp32. ``...`` is the
+    map axis of a :class:`GlobalHeatMapStack`, absent for one map. The scores are the reference's formulas
+    (``daam/evaluate.py``) in the same fp32 operation order."""
+    intersection: torch.Tensor
+    word_area: torch.Tensor
+
+    def iou(self) -> torch.Tensor:
+        """``[a, b] = I / (A[a] + A[b] - I + 1e-8)``: ``compute_iou(mask_a, mask_b)`` of every pair (and the DAAM
+        notebook's ``iou``, exact while ``A[a] + A[b]`` is below 2**24), symmetric."""
+        i, a = self.intersection, self.word_area
+        return i / (a.unsqueeze(-1) + a.unsqueeze(-2) - i + 1e-8)
+
+    def ioa(self) -> torch.Tensor:
+        """``[a, b] = I / (A[a] + 1e-8)``: ``compute_ioa(mask_a, mask_b)``, the share of word ``a`` inside word ``b``
+        (0 for an empty word, as the DAAM notebook's ``ioa``)."""
+        return self.intersection / (self.word_area.unsqueeze(-1) + 1e-8)
+
+
+@dataclass
+class RelationOverlap:
+    """Head / dependent overlap of the relations of a parse (:meth:`GlobalHeatMap.relation_overlap`): the kept
+    ``relations`` ``(head, dep, rel)`` and their indices ``kept`` in the input, the distinct endpoints ``words`` (as
+    given) and their :class:`WordOverlap`, and per kept edge ``iou``, ``iod`` (the share of the dependent inside the
+    head) and ``ioh`` (the share of the head inside the dependent), each ``[..., E]``."""
+    relations: List[Tuple]
+    kept: List[int]
+    words: List[Union[str, int]]
+    overlap: 'WordOverlap'
+    iou: torch.Tensor
+    iod: torch.Tensor
+    ioh: torch.Tensor
+
+
+def _word_overlap(tokenizer, prompt: str, maps: torch.Tensor, words, image, absolute, threshold, word_idx,
+                  offset_idx: int, to_cpu: bool, what: str):
+    """``daam_word_overlap`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(word_maps, merged, overlap)``: the
+    device word heat maps ``[n_maps, len(words), xh, xw]``, ``compute_token_merge_indices`` of every word, and the
+    :class:`WordOverlap` with a leading map axis. ``image=None``: the sums run over the heat-map grid."""
+    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, what)
+    n_maps, grid, dev = wl.n_maps, wl.grid, wl.dev
+    out_h, out_w = grid if image is None else _image_size(image, *grid)
+    n = len(words)
+    if not words or n_maps == 0:
+        ov = WordOverlap(torch.zeros((n_maps, n, n), device=dev), torch.zeros((n_maps, n), device=dev))
+        return wl.word_maps, wl.merged, (_to_cpu(ov) if to_cpu else ov)
+    inter = torch.empty((n_maps, n, n), dtype=torch.float32, device=dev)
+    area = torch.empty((n_maps, n), dtype=torch.float32, device=dev)
+    scratch = wl.scratch(_native.word_overlap_scratch_floats(n_maps, n, out_h, out_w))
+    with torch.cuda.device(dev):
+        _native.word_overlap(wl.maps.data_ptr(), n_maps, wl.n_rows, grid, wl.rows, out_h, out_w, absolute, threshold,
+                             wl.word_maps.data_ptr(), inter.data_ptr(), area.data_ptr(), scratch.data_ptr(),
+                             _stream_ptr(dev))
+    ov = WordOverlap(inter, area)
+    return wl.word_maps, wl.merged, (_to_cpu(ov) if to_cpu else ov)
+
+
+def _relation_overlap(tokenizer, prompt: str, maps: torch.Tensor, relations, image, absolute, threshold,
+                      offset_idx: int, to_cpu: bool, what: str) -> RelationOverlap:
+    """``relation_overlap`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: the distinct endpoints of the edges whose words
+    are in the prompt -- one endpoint per row set, so a word given twice, in another case, or as its token index is
+    measured once -- then one ``_word_overlap`` call and a gather; every tensor has a leading map axis."""
+    kept_edges, kept, words, word_idx, ends = [], [], [], [], []
+    slot: Dict[Tuple[int, ...], int] = {}
+    for e, edge in enumerate(relations):
+        head, dep, _ = edge
+        try:
+            pair = [compute_token_merge_indices(tokenizer, prompt, x, None, offset_idx)[0]
+                    if isinstance(x, str) else [int(x) + 1] for x in (head, dep)]
+        except ValueError:          # a word not in the prompt: the reference's ``except ValueError: pass``
+            continue
+        idx = []
+        for x, rows in zip((head, dep), pair):
+            key = tuple(rows)
+            if key not in slot:
+                slot[key] = len(words)
+                words.append(x)
+                word_idx.append(None if isinstance(x, str) else int(x))
+            idx.append(slot[key])
+        kept_edges.append(tuple(edge))
+        kept.append(e)
+        ends.append(idx)
+    if len(words) > _native.MAX_SEGMENT_WORDS:
+        raise ValueError(f'{what}: {len(words)} distinct endpoints > {_native.MAX_SEGMENT_WORDS}, the word limit of '
+                         f'one word_overlap call')
+    labels = [x if isinstance(x, str) else str(x) for x in words]
+    _, _, ov = _word_overlap(tokenizer, prompt, maps, labels, image, absolute, threshold, word_idx, offset_idx, to_cpu,
+                             what)
+    dev = ov.intersection.device
+    h = torch.tensor([i for i, _ in ends], dtype=torch.long, device=dev)
+    d = torch.tensor([j for _, j in ends], dtype=torch.long, device=dev)
+    iou, ioa = ov.iou(), ov.ioa()
+    return RelationOverlap(kept_edges, kept, words, ov, iou[..., h, d], ioa[..., d, h], ioa[..., h, d])
 
 
 def jet_colormap() -> torch.Tensor:
@@ -689,6 +827,25 @@ class GlobalHeatMapStack:
                                                 regions, absolute, threshold, word_idx, offset_idx, to_cpu,
                                                 f'{type(self).__name__}.region_overlap')
         return word_maps, overlap
+
+    def word_overlap(self, words, image=None, absolute: bool = False, threshold: Optional[float] = None,
+                     word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
+        """:meth:`GlobalHeatMap.word_overlap` for every map in one call (three launches whatever the map count):
+        returns ``(word_maps, overlap)`` with ``word_maps`` the device ``[maps, len(words), xh, xw]`` word heat maps and
+        ``overlap`` a :class:`WordOverlap` with a leading map axis (``intersection`` ``[maps, W, W]``, ``word_area``
+        ``[maps, W]``); row ``t`` equals ``self[t].word_overlap(...)`` bit for bit (min / max normalisation per map and
+        word). E.g. ``overlap.iou()[:, i, j]`` is the IoU of words ``i`` and ``j`` at every step of a history."""
+        word_maps, _, overlap = _word_overlap(self.tokenizer, self.prompt, self.heat_maps, list(words), image, absolute,
+                                              threshold, word_idx, offset_idx, to_cpu,
+                                              f'{type(self).__name__}.word_overlap')
+        return word_maps, overlap
+
+    def relation_overlap(self, relations, image=None, absolute: bool = False, threshold: Optional[float] = None,
+                         offset_idx: int = 0, to_cpu: bool = True) -> 'RelationOverlap':
+        """:meth:`GlobalHeatMap.relation_overlap` for every map in one :meth:`word_overlap` call: ``iou``, ``iod`` and
+        ``ioh`` are ``[maps, E]``, row ``t`` equal to ``self[t].relation_overlap(...)``'s bit for bit."""
+        return _relation_overlap(self.tokenizer, self.prompt, self.heat_maps, relations, image, absolute, threshold,
+                                 offset_idx, to_cpu, f'{type(self).__name__}.relation_overlap')
 
     def overlay_words(self, words, image, absolute: bool = False, threshold: Optional[float] = None,
                       color_normalize: bool = True, word_idx=None, offset_idx: int = 0, to_cpu: bool = True):

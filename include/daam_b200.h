@@ -34,7 +34,7 @@ extern "C" {
                                           n_blocks; daam_accumulate takes 154- and 231-token contexts; layers with
                                           several prompts and a prompt stride <= 0 take the SIMT kernel;
                                           daam_region_overlap; daam_overlay_words, daam_jet_colormap;
-                                          daam_finalize_parts) */
+                                          daam_finalize_parts; daam_word_overlap) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_TOKENS 231     /* daam_accumulate: long contexts of 2 or 3 CLIP chunks of 77 tokens (154, 231) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
@@ -357,6 +357,36 @@ int daam_region_overlap(const float* global_maps, int32_t n_maps, int32_t n_rows
                         int32_t absolute, int32_t use_threshold, float threshold, float* word_maps,
                         const uint8_t* regions, int32_t n_regions, float* intersection, float* word_area, float* scratch,
                         void* stream);
+
+/*
+ * Word-pair overlap: how much each word's expanded map overlaps every other word's, on each of n_maps global maps
+ * stored back to back -- the sums behind the DAAM paper's head / dependent analysis (the reference's
+ * WordHeatMap.compute_ioa, daam/heatmap.py:95-96, and compute_iou / compute_ioa of every pair of word masks). With m[w]
+ * what daam_expand_words writes for word w with the same arguments (0/1 when use_threshold):
+ *   intersection[i][a][b] = sum_p m[a](p) * m[b](p)           (fp32 [n_maps][n_words][n_words])
+ *   word_area[i][a]       = sum_p m[a](p)                     (fp32 [n_maps][n_words])
+ * Each pair a <= b is summed once and written to [a][b] and [b][a], so the matrix is symmetric bit for bit; with
+ * use_threshold the diagonal equals word_area. out_h x out_w = map_h x map_w sums over the heat-map grid itself
+ * (there the bicubic taps are the identity, so m is the word heat map). Arguments as daam_segment_words; scratch:
+ * device, >= DAAM_WORD_OVERLAP_SCRATCH_FLOATS(n_maps, n_words, out_h, out_w) floats: per map 64 n_words plus
+ * n_words (n_words + 3) / 2 partials for each of min(tiles, DAAM_WORD_OVERLAP_CTAS) CTAs (tiles of 16 x 64 output
+ * pixels), e.g. 47 KB at 8 words and 4.9 MB at 96 words for a 512 x 512 or larger image. A map's sums are the same bits
+ * whatever n_maps. Three launches whatever n_maps and n_words; the [n_words][out_h][out_w] stack is never written. The sums run
+ * in a fixed order without atomics, so repeated calls give the same bits; with use_threshold every sum is an exact
+ * pixel count.
+ * Limits (DAAM_E_UNSUPPORTED): n_words <= 96, row_begin[n_words] <= 320, map_h * map_w * 4 bytes <= 200 KB,
+ * n_maps <= 65535, out_h * out_w <= 2^24 (counts stay exact in fp32). DAAM_E_INVALID: null pointer, non-positive size,
+ * empty word list, a word without rows, a row out of range.
+ */
+#define DAAM_WORD_OVERLAP_CTAS 256   /* CTAs per map, at most one per 16 x 64 output tile */
+#define DAAM_WORD_OVERLAP_SCRATCH_FLOATS(n_maps, n_words, out_h, out_w)                                               \
+  ((int64_t)(n_maps) * ((n_words) * 64 + ((n_words) * ((n_words) + 3) / 2) *                                         \
+       ((((out_h) + 15) / 16) * (((out_w) + 63) / 64) < DAAM_WORD_OVERLAP_CTAS                                       \
+            ? (((out_h) + 15) / 16) * (((out_w) + 63) / 64) : DAAM_WORD_OVERLAP_CTAS)))
+int daam_word_overlap(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t map_h, int32_t map_w,
+                      const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w,
+                      int32_t absolute, int32_t use_threshold, float threshold, float* word_maps,
+                      float* intersection, float* word_area, float* scratch, void* stream);
 
 /*
  * Heat-map overlays: the reference's plot_overlay (daam/heatmap.py:20-53, :66-75 -- the word map coloured with
