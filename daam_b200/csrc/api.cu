@@ -1,5 +1,6 @@
 // C ABI entry points of libdaam_b200.so (include/daam_b200.h): argument validation, packing of layer calls into
-// persistent launches, error strings. The kernels live in accumulate_simt.cu, accumulate_mma.cu and finalize.cu.
+// persistent launches, error strings. The kernels live in accumulate_simt.cu, accumulate_mma.cu, finalize.cu, words.cu
+// and probs.cu.
 #include <atomic>
 #include <cstdarg>
 #include <cstdio>
@@ -90,7 +91,6 @@ namespace {
 // One kernel launch of a plan: a pack of layers for the wgmma kernel (prepared block, opaque) or a SIMT kernel.
 struct PlannedLaunch {
   bool is_mma = false;
-  bool simt_long = false;                // SIMT: the long-context kernel (154- / 231-token layers)
   LaunchParams simt;                     // SIMT: the parameter block itself
   SlabMode mode = kSlabNone;             // SIMT: the step- or range-slab kernel, with these slabs
   SecondSlabs slabs;
@@ -186,15 +186,11 @@ int build_plan(const daam_layer* layers, float* const* slabs, SlabMode mode, int
     plan->launches.emplace_back();
     PlannedLaunch& l = plan->launches.back();
     l.is_mma = which != 2 && which < 5;
-    l.simt_long = which >= 5;
     const SecondSlabs* st = slabs ? &pack_slabs[which] : nullptr;
     int rc;
     if (l.is_mma) {
       l.mma.reset(prepared_mma_new());
       rc = prepare_accumulate_mma(p, st, mode, dev, l.mma.get());
-    } else if (l.simt_long) {
-      l.simt = p;
-      rc = prepare_accumulate_simt_long(p, dev, &l.grid, &l.smem);
     } else {
       l.simt = p;
       l.mode = mode;
@@ -306,10 +302,9 @@ int accumulate_impl(const char* fn, const daam_layer* layers, float* const* slab
   }
   plan->stamp = ++clock;
   for (const PlannedLaunch& l : plan->launches) {
-    const int rc = l.is_mma      ? launch_prepared_mma(l.mma.get(), stream)
-                   : l.simt_long ? launch_prepared_simt_long(l.simt, l.grid, l.smem, stream)
-                                 : launch_prepared_simt(l.simt, l.mode != kSlabNone ? &l.slabs : nullptr, l.mode,
-                                                        l.grid, l.smem, stream);
+    const int rc = l.is_mma ? launch_prepared_mma(l.mma.get(), stream)
+                            : launch_prepared_simt(l.simt, l.mode != kSlabNone ? &l.slabs : nullptr, l.mode, l.grid,
+                                                   l.smem, stream);
     if (rc) return rc;
   }
   return DAAM_OK;

@@ -90,12 +90,10 @@ void count_launch(int n = 1);
 // distinct daam_layer[] input: the steady state of a trace replays the same layer calls every denoising step.
 // `slabs`: the launch's second slabs, nullptr exactly when `mode` is kSlabNone; `mode` selects the kernel instances
 // (kSlabStore: daam_accumulate_steps, kSlabAdd: daam_accumulate_range).
+// SIMT: every layer of `p` has one context length; 154- / 231-token contexts take the long-context kernel and no slabs.
 int prepare_accumulate_simt(const LaunchParams& p, SlabMode mode, const DeviceInfo& dev, int* grid, size_t* smem);
 int launch_prepared_simt(const LaunchParams& p, const SecondSlabs* slabs, SlabMode mode, int grid, size_t smem,
                          cudaStream_t stream);
-// The SIMT kernel of 154- / 231-token contexts (accumulate_simt_long.cu): every layer of `p` has the same context length.
-int prepare_accumulate_simt_long(const LaunchParams& p, const DeviceInfo& dev, int* grid, size_t* smem);
-int launch_prepared_simt_long(const LaunchParams& p, int grid, size_t smem, cudaStream_t stream);
 void* prepared_mma_new();
 void prepared_mma_delete(void* prepared);
 int prepare_accumulate_mma(const LaunchParams& p, const SecondSlabs* slabs, SlabMode mode, const DeviceInfo& dev,

@@ -6,8 +6,6 @@
 //    accumulate_simt.cu; the 128 x 77 block of a tile is contiguous in P and written out coalesced through shared memory.
 //  * accumulate_probs_kernel -- heat-map accumulation from supplied probabilities (load_heads, trace.py:281-294):
 //    acc[r][token][pixel] += P[first_row + r][pixel][token]  (= _unravel_attn + update).
-#include <mutex>
-
 #include "simt_common.cuh"
 
 namespace daam {
@@ -31,11 +29,9 @@ __device__ __forceinline__ void write_tile(const float* sp, T* out, int n) {
 __global__ void __launch_bounds__(kTilePixels, 3) attention_probs_kernel(const __grid_constant__ LaunchParams P,
                                                                          void* __restrict__ probs) {
   extern __shared__ __align__(16) float smem[];
-  const int per = P.total_tiles / gridDim.x, rem = P.total_tiles % gridDim.x;
-  const int first = blockIdx.x * per + min((int)blockIdx.x, rem);
-  const int count = per + ((int)blockIdx.x < rem ? 1 : 0);
+  const simt::TileSpan span = simt::cta_tiles(P.total_tiles);
   int li = 0, last_run = -1;
-  for (int tile = first; tile < first + count; ++tile) {
+  for (int tile = span.first; tile < span.first + span.count; ++tile) {
     const simt::TileRef t = simt::decode_tile(P, tile, li);
     const LayerParams& L = P.layer[t.li];
     float* ks = smem;
@@ -44,7 +40,7 @@ __global__ void __launch_bounds__(kTilePixels, 3) attention_probs_kernel(const _
     const bool load_k = t.run != last_run;
     last_run = t.run;
     __syncthreads();
-    simt::stage_any(L, t, ks, qs, load_k);
+    simt::stage_any(L, t, 0, ks, qs, load_k, /*load_q=*/true);
     __syncthreads();
     float s[kTokensPad];
     const float inv = simt::pixel_softmax(L, ks, qs, s);
@@ -116,16 +112,7 @@ extern "C" int daam_attention_probs(const daam_layer* layer, void* probs, void* 
   const size_t need = (size_t)p.layer[0].head_dim * kTokensPad + (size_t)kTilePixels * kTokens;   // K^T + staged P
   if (need > floats) floats = need;
   const size_t smem = floats * sizeof(float);
-  static std::mutex mu;
-  static size_t configured_dev[64] = {};              // the attribute is per device
-  {
-    std::lock_guard<std::mutex> lock(mu);
-    size_t& configured = configured_dev[dev.device & 63];
-    if (smem > configured) {
-      DAAM_CUDA_TRY(cudaFuncSetAttribute(attention_probs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      configured = smem;
-    }
-  }
+  if (int rc = simt::reserve_dynamic_smem((const void*)attention_probs_kernel, dev.device, smem)) return rc;
   int grid = dev.sm_count * 3;
   if (grid > p.total_tiles) grid = p.total_tiles;
   attention_probs_kernel<<<grid, kTilePixels, smem, stream>>>(p, probs);

@@ -1,5 +1,6 @@
-// Device code shared by the SIMT kernels (accumulate_simt.cu, probs.cu): 16-byte staged loads of the K^T / Q tiles
-// into shared memory and the one-thread-per-pixel logits + softmax.
+// Code shared by the SIMT kernels (accumulate_simt.cu, probs.cu): each CTA's contiguous range of tiles, 16-byte staged
+// loads of the K^T / Q tiles into shared memory, the one-thread-per-pixel logits + softmax, and the host-side
+// shared-memory attribute of the kernels.
 #pragma once
 
 #include "common.cuh"
@@ -37,13 +38,26 @@ template <> struct Vec<__nv_bfloat16> {
   static __device__ __forceinline__ float one(const __nv_bfloat16* p) { return __bfloat162float(__ldg(p)); }
 };
 
-// Stage K^T (ks[dim][token], tokens padded to 80 with zeros) and the Q tile (qs[pixel][dim], row stride d+1: odd,
-// hence bank-conflict free for the per-thread row walk) into shared memory with coalesced 16-byte global loads.
+// This CTA's share of the launch's tiles, [first, first + count): contiguous, so consecutive tiles share (layer, prompt,
+// head) and K^T is staged once per run.
+struct TileSpan {
+  int first, count;
+};
+__device__ __forceinline__ TileSpan cta_tiles(int total_tiles) {
+  const int per = total_tiles / gridDim.x, rem = total_tiles % gridDim.x;
+  const int first = blockIdx.x * per + min((int)blockIdx.x, rem);
+  return {first, per + ((int)blockIdx.x < rem ? 1 : 0)};
+}
+
+// Stage K^T of context rows [77 chunk, 77 chunk + 77) (ks[dim][token], tokens padded to 80 with zeros) and the Q tile
+// (qs[pixel][dim], row stride d+1: odd, hence bank-conflict free for the per-thread row walk) into shared memory with
+// coalesced 16-byte global loads.
 template <typename T>
-__device__ __forceinline__ void stage_tile(const LayerParams& L, int prompt, int head, int pixel0, float* ks,
-                                           float* qs, bool load_k) {
+__device__ __forceinline__ void stage_tile(const LayerParams& L, int prompt, int head, int pixel0, int chunk, float* ks,
+                                           float* qs, bool load_k, bool load_q) {
   const int d = L.head_dim;
-  const T* kbase = static_cast<const T*>(L.k) + prompt * L.ks_prompt + head * L.ks_head;
+  const T* kbase = static_cast<const T*>(L.k) + prompt * L.ks_prompt + head * L.ks_head +
+                   (long long)chunk * kTokens * L.ks_token;
   const T* qbase = static_cast<const T*>(L.q) + prompt * L.qs_prompt + head * L.qs_head;
   constexpr int V = Vec<T>::kElems;
   const int qstride = d + 1;
@@ -61,7 +75,7 @@ __device__ __forceinline__ void stage_tile(const LayerParams& L, int prompt, int
 #pragma unroll
       for (int i = 0; i < V; ++i) ks[(v * V + i) * kTokensPad + t] = f[i];
     }
-    for (int c = threadIdx.x; c < kTilePixels * vec_per_row; c += blockDim.x) {
+    for (int c = threadIdx.x; load_q && c < kTilePixels * vec_per_row; c += blockDim.x) {
       const int r = c / vec_per_row, v = c - r * vec_per_row;
       float f[V];
       if (pixel0 + r < L.hw) {
@@ -78,7 +92,7 @@ __device__ __forceinline__ void stage_tile(const LayerParams& L, int prompt, int
       const int t = c / d, e = c - t * d;
       ks[e * kTokensPad + t] = t < kTokens ? Vec<T>::one(kbase + t * L.ks_token + e) : 0.f;
     }
-    for (int c = threadIdx.x; c < kTilePixels * d; c += blockDim.x) {
+    for (int c = threadIdx.x; load_q && c < kTilePixels * d; c += blockDim.x) {
       const int r = c / d, e = c - r * d;
       qs[r * qstride + e] = pixel0 + r < L.hw ? Vec<T>::one(qbase + (long long)(pixel0 + r) * L.qs_pixel + e) : 0.f;
     }
@@ -105,15 +119,15 @@ __device__ __forceinline__ TileRef decode_tile(const LaunchParams& P, int tile, 
   return t;
 }
 
-__device__ __forceinline__ void stage_any(const LayerParams& L, const TileRef& t, float* ks, float* qs, bool load_k) {
-  if (L.dtype == DAAM_F32) stage_tile<float>(L, t.prompt, t.head, t.pixel0, ks, qs, load_k);
-  else if (L.dtype == DAAM_F16) stage_tile<__half>(L, t.prompt, t.head, t.pixel0, ks, qs, load_k);
-  else stage_tile<__nv_bfloat16>(L, t.prompt, t.head, t.pixel0, ks, qs, load_k);
+__device__ __forceinline__ void stage_any(const LayerParams& L, const TileRef& t, int chunk, float* ks, float* qs,
+                                          bool load_k, bool load_q) {
+  if (L.dtype == DAAM_F32) stage_tile<float>(L, t.prompt, t.head, t.pixel0, chunk, ks, qs, load_k, load_q);
+  else if (L.dtype == DAAM_F16) stage_tile<__half>(L, t.prompt, t.head, t.pixel0, chunk, ks, qs, load_k, load_q);
+  else stage_tile<__nv_bfloat16>(L, t.prompt, t.head, t.pixel0, chunk, ks, qs, load_k, load_q);
 }
 
-// This thread's pixel: 77 un-normalised probabilities exp2(scale*log2e*(s - max)) in s[0..76]; returns 1 / sum.
-__device__ __forceinline__ float pixel_softmax(const LayerParams& L, const float* ks, const float* qs, float* s) {
-  const int d = L.head_dim;
+// This thread's pixel: the raw logits <q, k> of the staged tokens in s[0..79] (columns 77..79 are padding).
+__device__ __forceinline__ void pixel_logits(int d, const float* ks, const float* qs, float* s) {
 #pragma unroll
   for (int t = 0; t < kTokensPad; ++t) s[t] = 0.f;
   const float* qrow = qs + threadIdx.x * (d + 1);
@@ -130,6 +144,11 @@ __device__ __forceinline__ float pixel_softmax(const LayerParams& L, const float
       s[4 * j + 3] = fmaf(qv, kv.w, s[4 * j + 3]);
     }
   }
+}
+
+// This thread's pixel: 77 un-normalised probabilities exp2(scale*log2e*(s - max)) in s[0..76]; returns 1 / sum.
+__device__ __forceinline__ float pixel_softmax(const LayerParams& L, const float* ks, const float* qs, float* s) {
+  pixel_logits(L.head_dim, ks, qs, s);
   // softmax over the 77 real tokens (columns 77..79 are padding and never read)
   float m = s[0];
 #pragma unroll
@@ -142,6 +161,10 @@ __device__ __forceinline__ float pixel_softmax(const LayerParams& L, const float
 }
 
 inline size_t tile_smem_floats(int head_dim) { return (size_t)head_dim * kTokensPad + (size_t)kTilePixels * (head_dim + 1); }
+
+// Raises `kernel`'s dynamic shared-memory limit on the current device (`device`) to at least `smem` bytes; the attribute
+// is per kernel and device, and each (kernel, device) pair is set once per size it grows to.
+int reserve_dynamic_smem(const void* kernel, int device, size_t smem);
 
 }  // namespace simt
 }  // namespace daam
