@@ -47,6 +47,15 @@ def word_overlap_scratch_floats(n_maps: int, n_words: int, out_h: int, out_w: in
     return n_maps * (n_words * 64 + (n_words * (n_words + 3) // 2) * min(tiles, WORD_OVERLAP_CTAS))
 
 
+WORD_INSTANCES_MAX = 64      # DAAM_WORD_INSTANCES_MAX: max_instances of daam_word_instances
+
+
+def word_instances_plane_bytes(out_h: int, out_w: int) -> int:
+    """``DAAM_WORD_INSTANCES_PLANE_BYTES(out_h, out_w)``: the scratch bytes daam_word_instances takes per (map, word)
+    plane."""
+    return 8 * out_h * out_w + 48 * ((out_h + 1) // 2) * ((out_w + 1) // 2) + 260
+
+
 def overlay_frames_bytes(n_maps: int, n_words: int, out_h: int, out_w: int) -> int:
     """``DAAM_OVERLAY_FRAMES_BYTES(n_maps, n_words, out_h, out_w)``: the frames rounded up to whole 4-byte words."""
     return (n_maps * n_words * out_h * out_w * 3 + 3) // 4 * 4
@@ -54,7 +63,7 @@ def overlay_frames_bytes(n_maps: int, n_words: int, out_h: int, out_w: int) -> i
 
 EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize',
            'daam_finalize_maps', 'daam_finalize_parts', 'daam_finalize_per_key','daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
-           'daam_segment_words', 'daam_region_overlap', 'daam_word_overlap', 'daam_overlay_words', 'daam_jet_colormap',
+           'daam_segment_words', 'daam_region_overlap', 'daam_word_overlap', 'daam_word_instances', 'daam_overlay_words', 'daam_jet_colormap',
            'daam_side_launcher_create', 'daam_side_launcher_destroy',
            'daam_side_launcher_launch', 'daam_side_launcher_join', 'daam_side_launcher_idle', 'daam_abi_version',
            'daam_last_error', 'daam_device_info', 'daam_launch_count')
@@ -164,6 +173,9 @@ def load() -> ctypes.CDLL:
     lib.daam_word_overlap.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
                                       i32, i32, f32, vp, vp, vp, vp, vp]
     lib.daam_word_overlap.restype = ctypes.c_int
+    lib.daam_word_instances.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32,
+                                        i32, i32, f32, i32, vp, vp, vp, vp, vp, vp, vp, vp, i64, vp]
+    lib.daam_word_instances.restype = ctypes.c_int
     lib.daam_overlay_words.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
                                        i32, i32, f32, i32, vp, vp, i64, vp, vp, vp]
     lib.daam_overlay_words.restype = ctypes.c_int
@@ -430,6 +442,22 @@ def word_overlap(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequ
                                     *_word_list(x, rows_per_word, out_h, out_w, absolute, threshold),
                                     ctypes.c_void_p(word_maps_ptr), ctypes.c_void_p(intersection_ptr),
                                     ctypes.c_void_p(word_area_ptr), ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
+
+
+def word_instances(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int,
+                   out_w: int, absolute: bool, threshold: float, max_instances: int, word_maps_ptr: int, count_ptr: int,
+                   area_ptr: int, box_ptr: int, sum_yx_ptr: int, peak_ptr: int, peak_yx_ptr: int, scratch_ptr: int,
+                   scratch_bytes: int, stream: int):
+    """``daam_word_instances`` over ``n_maps`` maps ``[n_rows, h, w]`` back to back: ``count`` int32 ``[n_maps,
+    n_words]``, then per kept instance ``area`` int32, ``box`` int32 ``[4]``, ``sum_yx`` int64 ``[2]``, ``peak`` fp32 and
+    ``peak_yx`` int32 ``[2]`` (``[n_maps, n_words, max_instances, ...]``); ``scratch_bytes`` of scratch, at least
+    :func:`word_instances_plane_bytes`. The threshold is always in effect."""
+    h, w, rows, begin, n_words = _word_list(x, rows_per_word, out_h, out_w, absolute, threshold)[:5]
+    vp = ctypes.c_void_p
+    _check(load().daam_word_instances(vp(maps_ptr), n_maps, n_rows, h, w, rows, begin, n_words, out_h, out_w,
+                                      int(bool(absolute)), float(threshold), max_instances, vp(word_maps_ptr),
+                                      vp(count_ptr), vp(area_ptr), vp(box_ptr), vp(sum_yx_ptr), vp(peak_ptr),
+                                      vp(peak_yx_ptr), vp(scratch_ptr), scratch_bytes, vp(stream)))
 
 
 def overlay_words(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int,

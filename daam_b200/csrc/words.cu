@@ -13,12 +13,14 @@
 //  - segment_label_kernel keeps each pixel's max / argmax over the words;
 //  - region_tile_kernel sums it over binary image regions (then region_reduce_kernel);
 //  - overlay_kernel blends its jet colour onto the image;
-//  - word_pair_tile_kernel sums m[a] * m[b] over every pair of words (then word_pair_reduce_kernel).
+//  - word_pair_tile_kernel sums m[a] * m[b] over every pair of words (then word_pair_reduce_kernel);
+//  - instance_mask_kernel writes it without threshold for components.cu, which labels the mask m > threshold.
 // The tile kernels run after segment_minmax_kernel (steps 1 and 2, the word maps and min / max partials to global
-// memory); region_tile_kernel, overlay_kernel and word_pair_tile_kernel share the tile helpers (block_tile / tile_at,
-// word_bounds, stage_windows, tap tables). expand_words_kernel, segment_minmax_kernel and segment_label_kernel keep
+// memory); region_tile_kernel, overlay_kernel, word_pair_tile_kernel and instance_mask_kernel share the tile helpers
+// (block_tile / tile_at, word_bounds, stage_windows, tap tables). expand_words_kernel, segment_minmax_kernel and segment_label_kernel keep
 // their steps inline: written with the helpers, nvcc scheduled them differently and they measured slower. Every consumer's m is expand_words_kernel's
-// value bit for bit. Deterministic: no atomics.
+// value bit for bit. Deterministic: no atomics here (components.cu's are integer atomics, whose results do not depend
+// on their order).
 #include <cooperative_groups.h>
 #include <math.h>
 
@@ -27,6 +29,7 @@
 
 #include "bicubic.cuh"
 #include "common.cuh"
+#include "components.cuh"
 
 namespace daam {
 namespace {
@@ -827,6 +830,46 @@ __global__ void __launch_bounds__(256) overlay_kernel(const __grid_constant__ Ov
   }
 }
 
+// ---- word instances: m without threshold, for the connected components of m > threshold ---------------------------
+// Writes every pixel's m (use_threshold 0: what daam_expand_words writes without threshold) to a plane per (map, word);
+// components.cu labels the plane's mask m > threshold and reduces its components.
+struct InstanceMaskParams {
+  WordListParams s;
+  float* pre;                           // [n_maps][n_words][oh][ow]
+};
+
+// grid: (tiles of kSegTileH x kSegTileW output pixels, n_maps); dynamic smem: words_per_pass source windows
+__global__ void __launch_bounds__(256) instance_mask_kernel(const __grid_constant__ InstanceMaskParams I) {
+  extern __shared__ __align__(16) float win[];
+  __shared__ float s_lo[kMaxWords], s_hi[kMaxWords];
+  __shared__ TapTables taps;
+  const WordListParams& P = I.s;
+  const int map = blockIdx.y, ow = P.ow, n_words = P.n_words;
+  const Tile T = block_tile(P);
+  for (int w = threadIdx.x; w < n_words; w += blockDim.x) word_bounds(P, map, w, s_lo[w], s_hi[w]);
+  fill_tap_tables(P, T, taps);
+  const float* word_maps = P.word_maps + (long long)map * n_words * P.mh * P.mw;
+  const long long n = (long long)P.oh * ow;
+  for (int w0 = 0; w0 < n_words; w0 += P.words_per_pass) {
+    const int nw = min(P.words_per_pass, n_words - w0);
+    stage_windows(P, T, word_maps, w0, nw, win);
+    for (int wi = 0; wi < nw; ++wi) {
+      const int w = w0 + wi;
+      float* dst = I.pre + ((long long)map * n_words + w) * n + (long long)T.y0 * ow + T.x0;
+#pragma unroll
+      for (int k = 0; k < kSegPix; ++k) {
+        const int p = threadIdx.x + 256 * k;
+        if (p < T.th * T.tw) {
+          const int py = p / T.tw, px = p - py * T.tw;
+          Taps ty, tx;
+          tile_taps(taps, py, px, ty, tx);
+          dst[(long long)py * ow + px] = word_value(P, bicubic_shared(win + wi * T.wn, T.ww, ty, tx), s_lo[w], s_hi[w]);
+        }
+      }
+    }
+  }
+}
+
 }  // namespace
 }  // namespace daam
 
@@ -999,7 +1042,7 @@ static int launch_tiles(void (*kernel)(Params), Params& k, int n_maps, const Dev
   std::call_once(attr_once[dev.device & 63], [&] {
     const void* kernels[] = {(const void*)segment_minmax_kernel, (const void*)segment_label_kernel,
                              (const void*)region_tile_kernel, (const void*)overlay_kernel,
-                             (const void*)word_pair_tile_kernel};
+                             (const void*)word_pair_tile_kernel, (const void*)instance_mask_kernel};
     for (const void* f : kernels)
       if (attr_err == cudaSuccess) attr_err = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
   });
@@ -1106,5 +1149,53 @@ extern "C" int daam_overlay_words(const float* global_maps, int32_t n_maps, int3
 extern "C" int daam_jet_colormap(float* out) {
   if (!out) { set_error("daam_jet_colormap: null pointer"); return DAAM_E_INVALID; }
   DAAM_CUDA_TRY(cudaMemcpyFromSymbol(out, c_jet, sizeof(JetTable)));
+  return DAAM_OK;
+}
+
+extern "C" int daam_word_instances(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t mh, int32_t mw,
+                                   const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h,
+                                   int32_t out_w, int32_t absolute, float threshold, int32_t max_instances,
+                                   float* word_maps, int32_t* count, int32_t* area, int32_t* box, int64_t* sum_yx,
+                                   float* peak, int32_t* peak_yx, void* scratch, int64_t scratch_bytes, void* stream_) {
+  const char* name = "daam_word_instances";
+  if (!global_maps || !rows || !row_begin || !word_maps || !count || !area || !box || !sum_yx || !peak || !peak_yx ||
+      !scratch || n_maps <= 0 || mh <= 0 || mw <= 0 || out_h <= 0 || out_w <= 0 || n_rows <= 0 || max_instances <= 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
+  if (max_instances > kMaxInstances) { set_error("%s: max_instances %d > %d", name, max_instances, kMaxInstances); return DAAM_E_UNSUPPORTED; }
+  if ((long long)out_h * out_w > (1LL << 24)) { set_error("%s: a %d x %d output is more than 2^24 pixels", name, out_h, out_w); return DAAM_E_UNSUPPORTED; }
+  const long long plane_bytes = instance_plane_bytes(out_h, out_w);
+  if (scratch_bytes < plane_bytes) { set_error("%s: %lld scratch bytes < %lld, one %d x %d plane", name, (long long)scratch_bytes, plane_bytes, out_h, out_w); return DAAM_E_INVALID; }
+  static thread_local InstanceMaskParams p, q;
+  DeviceInfo dev;
+  if (int rc = word_list_prepare(name, global_maps, n_maps, n_rows, mh, mw, rows, row_begin, n_words, out_h, out_w,
+                                 absolute, !absolute, 0, 0.f, word_maps, nullptr, true, p.s, &dev)) return rc;
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  // a round: whole maps while a map's planes fit the scratch, else the words of one map in groups
+  const int cap = (int)std::min<long long>(scratch_bytes / plane_bytes, 65535);
+  const int maps_per_round = std::max(1, cap / n_words), words_per_round = std::min(cap, (int)n_words);
+  for (int map0 = 0; map0 < n_maps; map0 += maps_per_round) {
+    const int nm = std::min(maps_per_round, n_maps - map0);
+    for (int w0 = 0; w0 < n_words; w0 += words_per_round) {
+      const int nw = std::min(words_per_round, n_words - w0);
+      q = p;
+      q.s.maps = global_maps + map0 * p.s.map_stride;
+      q.s.n_words = nw;
+      for (int i = 0; i <= nw; ++i) q.s.row_begin[i] = p.s.row_begin[w0 + i];
+      const long long plane0 = (long long)map0 * n_words + w0;
+      q.s.word_maps = word_maps + plane0 * mh * mw;
+      InstancePlanes c;
+      instance_planes_in(scratch, nm * nw, out_h, out_w, c);
+      q.s.scratch = c.minmax;
+      q.pre = c.pre;
+      if (int rc = launch_tiles(instance_mask_kernel, q, nm, dev, stream)) return rc;
+      c.k = max_instances; c.threshold = threshold;
+      c.count = count + plane0;
+      c.out_area = area + plane0 * max_instances;
+      c.out_box = box + plane0 * max_instances * 4;
+      c.out_sum = reinterpret_cast<long long*>(sum_yx) + plane0 * max_instances * 2;
+      c.out_peak = peak + plane0 * max_instances;
+      c.out_peak_yx = peak_yx + plane0 * max_instances * 2;
+      if (int rc = launch_components(c, stream)) return rc;
+    }
+  }
   return DAAM_OK;
 }

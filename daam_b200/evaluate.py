@@ -13,7 +13,10 @@ against several regions, or every step of a history, use :meth:`GlobalHeatMap.re
 To score every pair of words against each other (``WordHeatMap.compute_ioa``, the DAAM paper's head / dependent
 overlap), use :meth:`GlobalHeatMap.word_overlap <daam_b200.heatmap.GlobalHeatMap.word_overlap>` or, for the relations
 of a parse, :meth:`GlobalHeatMap.relation_overlap <daam_b200.heatmap.GlobalHeatMap.relation_overlap>`, on one map or a
-stack: three fused launches for every pair, with the same bit-for-bit equality for thresholded masks.
+stack: three fused launches for every pair, with the same bit-for-bit equality for thresholded masks. For the boxes,
+counts and centroids of each word's thresholded mask (the localisation protocol: the largest connected component's
+box against a ground-truth box), use :meth:`GlobalHeatMap.word_instances <daam_b200.heatmap.GlobalHeatMap.word_instances>`
+and ``WordInstances.box_iou``, on one map or a stack.
 """
 from __future__ import annotations
 

@@ -26,7 +26,7 @@ from . import _native
 from .utils import compute_token_merge_indices
 
 __all__ = ['GlobalHeatMap', 'RawHeatMapCollection', 'WordHeatMap', 'LayerSlab', 'GlobalHeatMapStack', 'TimeHeatMaps',
-           'ImageHeatMaps', 'LayerHeatMaps', 'FactorHeatMaps', 'HeadHeatMaps', 'RegionOverlap', 'WordOverlap', 'RelationOverlap']
+           'ImageHeatMaps', 'LayerHeatMaps', 'FactorHeatMaps', 'HeadHeatMaps', 'RegionOverlap', 'WordOverlap', 'RelationOverlap', 'WordInstances']
 
 RawHeatMapKey = Tuple[int, int, int]  # factor, layer, head
 
@@ -460,6 +460,29 @@ class GlobalHeatMap:
         ov = WordOverlap(rel.overlap.intersection[0], rel.overlap.word_area[0])
         return RelationOverlap(rel.relations, rel.kept, rel.words, ov, rel.iou[0], rel.iod[0], rel.ioh[0])
 
+    def word_instances(self, words, image, threshold: float, absolute: bool = False, max_instances: int = 16,
+                       word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
+        """Where each word is and how many blobs it makes: the 8-connected components of each word's mask. The mask is
+        what ``expand_words(words, image, absolute, threshold, word_idx, offset_idx)`` returns, ``pre > threshold`` with
+        ``pre`` the expanded map without threshold; its components are those of ``scipy.ndimage.label(mask,
+        structure=np.ones((3, 3)))``. The :class:`WordInstances` holds each word's component ``count`` and, for its
+        ``max_instances`` largest components (ties to the one whose first pixel comes first in raster order), their
+        ``area``, half-open ``box`` ``(y0, x0, y1, x1)``, exact index sums ``sum_yx``, ``peak`` of ``pre`` and the first
+        pixel ``peak_yx`` where it is reached. ``largest_box()`` is the box of the weakly supervised localisation
+        protocol; ``box_iou(gt_boxes)`` scores it. Fused on the device: the ``[len(words), H, W]`` stack never leaves
+        it, and the results are the same bits on every call.
+
+        Returns ``(word_heat_maps, instances)``: the list of :class:`WordHeatMap` that :meth:`segment` returns and the
+        :class:`WordInstances` (CPU by default, ``to_cpu=False`` keeps it on the device). ``threshold`` must be truthy
+        (a ``ValueError`` otherwise: without a mask there are no components); ``1 <= max_instances <= 64``; at most 96
+        words and 2**24 image pixels. An empty word list launches nothing and returns empty axes. Raises the
+        reference's ``ValueError`` for a word that is not in the prompt."""
+        words = list(words)
+        word_maps, merged, inst = _word_instances(self.tokenizer, self.prompt, self.heat_maps[None], words, image,
+                                                  threshold, absolute, max_instances, word_idx, offset_idx, to_cpu,
+                                                  'GlobalHeatMap.word_instances')
+        return _word_heat_maps(word_maps[0], words, merged), inst.map(0)
+
     def overlay_words(self, words, image, absolute: bool = False, threshold: Optional[float] = None,
                       color_normalize: bool = True, word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
         """The reference's ``plot_overlay`` (heatmap.py:20-53, 66-75) as pixels, for a word list: each word's expanded
@@ -711,6 +734,98 @@ def _relation_overlap(tokenizer, prompt: str, maps: torch.Tensor, relations, ima
     return RelationOverlap(kept_edges, kept, words, ov, iou[..., h, d], ioa[..., d, h], ioa[..., h, d])
 
 
+# Scratch of one word_instances call: as many (map, word) planes as fit are labelled per round, so memory does not grow
+# with the number of maps (a 50-step, 24-word SDXL history would take about 25 GB at once).
+WORD_INSTANCES_SCRATCH_BYTES = 256 << 20
+
+
+@dataclass
+class WordInstances:
+    """Connected components of word masks (:meth:`GlobalHeatMap.word_instances`), the largest ``K`` per word, sorted by
+    area (largest first, ties to the first pixel in raster order): ``count`` int32 ``[..., W]`` (every component, not
+    capped at ``K``), ``area`` int32 ``[..., W, K]``, ``box`` int32 ``[..., W, K, 4]`` (``(y0, x0, y1, x1)``, half-open),
+    ``sum_yx`` int64 ``[..., W, K, 2]`` (sums of the row and column indices of the pixels), ``peak`` fp32 ``[..., W, K]``
+    (the max of the expanded map over the component) and ``peak_yx`` int32 ``[..., W, K, 2]`` (the first pixel where it
+    is reached). Slots past ``count`` are 0. ``...`` is the map axis of a :class:`GlobalHeatMapStack`, absent for one
+    map. The helpers are plain torch on the fields' device."""
+    count: torch.Tensor
+    area: torch.Tensor
+    box: torch.Tensor
+    sum_yx: torch.Tensor
+    peak: torch.Tensor
+    peak_yx: torch.Tensor
+
+    def map(self, i: int) -> 'WordInstances':
+        """The instances of map ``i`` of a stack."""
+        return WordInstances(*(getattr(self, f)[i] for f in _INSTANCE_FIELDS))
+
+    def cpu(self) -> 'WordInstances':
+        return WordInstances(*(getattr(self, f).cpu() for f in _INSTANCE_FIELDS))
+
+    def centroid(self) -> torch.Tensor:
+        """float64 ``[..., W, K, 2]``: ``sum_yx / area``, the mean row and column of each instance; NaN for empty
+        slots."""
+        area = self.area.double().unsqueeze(-1)
+        return torch.where(area > 0, self.sum_yx.double() / area.clamp(min=1), torch.full_like(area, float('nan')))
+
+    def largest_box(self) -> torch.Tensor:
+        """int32 ``[..., W, 4]``: the box of each word's largest instance (zeros for a word with none)."""
+        return self.box[..., 0, :]
+
+    def box_iou(self, boxes) -> torch.Tensor:
+        """float64 ``[..., W, B]``: IoU of each word's largest box against half-open ``(y0, x0, y1, x1)`` boxes ``[B,
+        4]`` (e.g. ground-truth boxes), 0 for a word without an instance."""
+        lb = self.largest_box().double().unsqueeze(-2)                     # [..., W, 1, 4]
+        gt = torch.as_tensor(boxes, dtype=torch.float64, device=lb.device).reshape(-1, 4)
+        ih = (torch.minimum(lb[..., 2], gt[:, 2]) - torch.maximum(lb[..., 0], gt[:, 0])).clamp(min=0)
+        iw = (torch.minimum(lb[..., 3], gt[:, 3]) - torch.maximum(lb[..., 1], gt[:, 1])).clamp(min=0)
+        inter = ih * iw
+        a = (lb[..., 2] - lb[..., 0]) * (lb[..., 3] - lb[..., 1])
+        b = (gt[:, 2] - gt[:, 0]) * (gt[:, 3] - gt[:, 1])
+        union = a + b - inter
+        has = (self.area[..., 0] > 0).unsqueeze(-1)
+        return torch.where(has & (union > 0), inter / union.clamp(min=1e-300), torch.zeros_like(inter))
+
+
+_INSTANCE_FIELDS = ('count', 'area', 'box', 'sum_yx', 'peak', 'peak_yx')
+
+
+def _word_instances(tokenizer, prompt: str, maps: torch.Tensor, words, image, threshold, absolute, max_instances: int,
+                    word_idx, offset_idx: int, to_cpu: bool, what: str):
+    """``daam_word_instances`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(word_maps, merged, instances)``: the
+    device word heat maps ``[n_maps, len(words), xh, xw]``, ``compute_token_merge_indices`` of every word, and the
+    :class:`WordInstances` with a leading map axis. Scratch: :data:`WORD_INSTANCES_SCRATCH_BYTES`, clipped to the planes
+    the call has, at least one plane."""
+    if not threshold:
+        raise ValueError(f'{what}: threshold must be set (truthy), not {threshold!r}: the instances are the connected '
+                         f'components of the mask expand_words(..., threshold) returns')
+    if isinstance(max_instances, bool) or not isinstance(max_instances, int) \
+            or not 1 <= max_instances <= _native.WORD_INSTANCES_MAX:
+        raise ValueError(f'{what}: max_instances must be an int in [1, {_native.WORD_INSTANCES_MAX}], not '
+                         f'{max_instances!r}')
+    if len(words) > _native.MAX_SEGMENT_WORDS:
+        raise ValueError(f'{what}: {len(words)} words > {_native.MAX_SEGMENT_WORDS}, the word limit of one call')
+    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, what)
+    n_maps, grid, dev = wl.n_maps, wl.grid, wl.dev
+    out_h, out_w = _image_size(image, *grid)
+    n, k = len(words), max_instances
+    new = torch.empty if words and n_maps else torch.zeros     # the kernels write every slot
+    i32 = dict(dtype=torch.int32, device=dev)
+    inst = WordInstances(new((n_maps, n), **i32), new((n_maps, n, k), **i32), new((n_maps, n, k, 4), **i32),
+                         new((n_maps, n, k, 2), dtype=torch.int64, device=dev),
+                         new((n_maps, n, k), dtype=torch.float32, device=dev), new((n_maps, n, k, 2), **i32))
+    if words and n_maps:
+        plane = _native.word_instances_plane_bytes(out_h, out_w)
+        n_bytes = max(plane, min(WORD_INSTANCES_SCRATCH_BYTES, plane * n_maps * n))
+        scratch = torch.empty(n_bytes, dtype=torch.uint8, device=dev)
+        with torch.cuda.device(dev):
+            _native.word_instances(wl.maps.data_ptr(), n_maps, wl.n_rows, grid, wl.rows, out_h, out_w, absolute,
+                                   threshold, k, wl.word_maps.data_ptr(),
+                                   *(getattr(inst, f).data_ptr() for f in _INSTANCE_FIELDS), scratch.data_ptr(),
+                                   n_bytes, _stream_ptr(dev))
+    return wl.word_maps, wl.merged, (inst.cpu() if to_cpu else inst)
+
+
 def jet_colormap() -> torch.Tensor:
     """The fp32 ``[256, 3]`` table the overlay kernel colours with: ``L[k] = 255 * jet(k / 255)``, matplotlib's ``jet``
     segment data evaluated in float64 and rounded once to fp32 (``L[0] = (0, 0, 127.5)``, ``L[255] = (127.5, 0, 0)``)."""
@@ -846,6 +961,19 @@ class GlobalHeatMapStack:
         ``ioh`` are ``[maps, E]``, row ``t`` equal to ``self[t].relation_overlap(...)``'s bit for bit."""
         return _relation_overlap(self.tokenizer, self.prompt, self.heat_maps, relations, image, absolute, threshold,
                                  offset_idx, to_cpu, f'{type(self).__name__}.relation_overlap')
+
+    def word_instances(self, words, image, threshold: float, absolute: bool = False, max_instances: int = 16,
+                       word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
+        """:meth:`GlobalHeatMap.word_instances` for every map in one call: returns ``(word_maps, instances)`` with
+        ``word_maps`` the device ``[maps, len(words), xh, xw]`` word heat maps and ``instances`` a
+        :class:`WordInstances` with a leading map axis (``count`` ``[maps, W]``, ``area`` ``[maps, W, K]``, ...); row
+        ``t`` equals ``self[t].word_instances(...)`` bit for bit (min / max normalisation per map and word). E.g.
+        ``instances.count[:, 0]`` is how many blobs word 0 makes at every step of a history. Scratch stays within a
+        fixed budget whatever the map count: the planes are labelled in rounds."""
+        word_maps, _, inst = _word_instances(self.tokenizer, self.prompt, self.heat_maps, list(words), image, threshold,
+                                             absolute, max_instances, word_idx, offset_idx, to_cpu,
+                                             f'{type(self).__name__}.word_instances')
+        return word_maps, inst
 
     def overlay_words(self, words, image, absolute: bool = False, threshold: Optional[float] = None,
                       color_normalize: bool = True, word_idx=None, offset_idx: int = 0, to_cpu: bool = True):

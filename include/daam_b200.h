@@ -34,7 +34,8 @@ extern "C" {
                                           n_blocks; daam_accumulate takes 154- and 231-token contexts; layers with
                                           several prompts and a prompt stride <= 0 take the SIMT kernel;
                                           daam_region_overlap; daam_overlay_words, daam_jet_colormap;
-                                          daam_finalize_parts; daam_word_overlap) */
+                                          daam_finalize_parts; daam_word_overlap;
+                                          daam_word_instances) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_TOKENS 231     /* daam_accumulate: long contexts of 2 or 3 CLIP chunks of 77 tokens (154, 231) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
@@ -387,6 +388,36 @@ int daam_word_overlap(const float* global_maps, int32_t n_maps, int32_t n_rows, 
                       const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w,
                       int32_t absolute, int32_t use_threshold, float threshold, float* word_maps,
                       float* intersection, float* word_area, float* scratch, void* stream);
+
+/*
+ * Word instances: the 8-connected components of each word's mask, on each of n_maps global maps stored back to back
+ * -- where a word is and how many blobs it makes (the weakly supervised localisation protocol: threshold the map, take
+ * the largest component, score its box). With pre[w] what daam_expand_words writes for word w without threshold
+ * (same rows / row_begin / absolute), the mask is pre[w] > threshold: what daam_expand_words writes with it. For plane
+ * (i, w) and its components sorted by area, largest first, ties to the component whose first pixel comes first in
+ * raster order (scipy.ndimage.label's order), instance j < K = max_instances:
+ *   count[i][w]              number of components, all of them                            int32 [n_maps][n_words]
+ *   area[i][w][j]            pixels                                                       int32 [...][K]
+ *   box[i][w][j]             (y0, x0, y1, x1), half-open: scipy.ndimage.find_objects      int32 [...][K][4]
+ *   sum_yx[i][w][j]          sums of the row and of the column indices of its pixels      int64 [...][K][2]
+ *   peak[i][w][j]            max of pre over the component                                fp32  [...][K]
+ *   peak_yx[i][w][j]         the first pixel in raster order where pre == peak            int32 [...][K][2]
+ * Slots j >= count are 0 in every field. Arguments as daam_word_overlap without use_threshold (the threshold is always
+ * in effect); outputs on the device. scratch: device, 8-byte aligned; as many (map, word) planes are labelled per round
+ * as scratch_bytes holds at DAAM_WORD_INSTANCES_PLANE_BYTES(out_h, out_w) each (about 20 bytes a pixel), whole maps
+ * while a map's planes fit, and the call loops over the rounds: seven launches a round. The results are the same bits
+ * whatever the scratch, and on every call (integer atomics only).
+ * Limits (DAAM_E_UNSUPPORTED): those of daam_word_overlap, and max_instances <= 64 (DAAM_WORD_INSTANCES_MAX).
+ * DAAM_E_INVALID: as daam_word_overlap, plus max_instances <= 0 and scratch_bytes below one plane.
+ */
+#define DAAM_WORD_INSTANCES_MAX 64
+#define DAAM_WORD_INSTANCES_PLANE_BYTES(out_h, out_w)                                                                 \
+  (8 * (int64_t)(out_h) * (out_w) + 48 * (int64_t)(((out_h) + 1) / 2) * (((out_w) + 1) / 2) + 260)
+int daam_word_instances(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t map_h, int32_t map_w,
+                        const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w,
+                        int32_t absolute, float threshold, int32_t max_instances, float* word_maps, int32_t* count,
+                        int32_t* area, int32_t* box, int64_t* sum_yx, float* peak, int32_t* peak_yx, void* scratch,
+                        int64_t scratch_bytes, void* stream);
 
 /*
  * Heat-map overlays: the reference's plot_overlay (daam/heatmap.py:20-53, :66-75 -- the word map coloured with
