@@ -451,13 +451,13 @@ def word_instances(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Se
     """``daam_word_instances`` over ``n_maps`` maps ``[n_rows, h, w]`` back to back: ``count`` int32 ``[n_maps,
     n_words]``, then per kept instance ``area`` int32, ``box`` int32 ``[4]``, ``sum_yx`` int64 ``[2]``, ``peak`` fp32 and
     ``peak_yx`` int32 ``[2]`` (``[n_maps, n_words, max_instances, ...]``); ``scratch_bytes`` of scratch, at least
-    :func:`word_instances_plane_bytes`. The threshold is always in effect."""
-    h, w, rows, begin, n_words = _word_list(x, rows_per_word, out_h, out_w, absolute, threshold)[:5]
+    :func:`word_instances_plane_bytes`. The threshold is always in effect: the call takes no ``use_threshold``."""
     vp = ctypes.c_void_p
-    _check(load().daam_word_instances(vp(maps_ptr), n_maps, n_rows, h, w, rows, begin, n_words, out_h, out_w,
-                                      int(bool(absolute)), float(threshold), max_instances, vp(word_maps_ptr),
-                                      vp(count_ptr), vp(area_ptr), vp(box_ptr), vp(sum_yx_ptr), vp(peak_ptr),
-                                      vp(peak_yx_ptr), vp(scratch_ptr), scratch_bytes, vp(stream)))
+    _check(load().daam_word_instances(vp(maps_ptr), n_maps, n_rows,
+                                      *_word_list(x, rows_per_word, out_h, out_w, absolute, threshold)[:-2],
+                                      float(threshold), max_instances, vp(word_maps_ptr), vp(count_ptr), vp(area_ptr),
+                                      vp(box_ptr), vp(sum_yx_ptr), vp(peak_ptr), vp(peak_yx_ptr), vp(scratch_ptr),
+                                      scratch_bytes, vp(stream)))
 
 
 def overlay_words(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int,

@@ -343,15 +343,8 @@ class GlobalHeatMap:
         self.compute_word_heat_map = lru_cache(maxsize=50)(self.compute_word_heat_map)
 
     def compute_word_heat_map(self, word: str, word_idx: int = None, offset_idx: int = 0) -> WordHeatMap:
-        rows, word_idx = compute_token_merge_indices(self.tokenizer, self.prompt, word, word_idx, offset_idx)
-        maps = self.heat_maps
-        _require_cuda(maps, 'GlobalHeatMap.compute_word_heat_map')
-        n_rows, grid = maps.shape[0], tuple(maps.shape[-2:])
-        _check_rows(rows, n_rows)
-        maps = maps.detach().float().contiguous()
-        out = torch.empty(grid, dtype=torch.float32, device=maps.device)
-        with torch.cuda.device(maps.device):
-            _native.word_heat_map(maps.data_ptr(), n_rows, grid, rows, out.data_ptr(), _stream_ptr(maps.device))
+        out, word_idx = _word_heat_map(self.tokenizer, self.prompt, self.heat_maps, word, word_idx, offset_idx,
+                                       'GlobalHeatMap.compute_word_heat_map')
         return WordHeatMap(out, word, word_idx)
 
     def expand_words(self, words, image, absolute: bool = False, threshold: Optional[float] = None,
@@ -366,18 +359,18 @@ class GlobalHeatMap:
         :meth:`WordHeatMap.expand_as` orders it -- (CPU by default like
         ``expand_as``; ``to_cpu=False`` keeps it on the device until the caller needs it). ``word_idx`` may be a list
         parallel to ``words``. Raises the reference's ``ValueError`` for a word that is not in the prompt."""
-        words = list(words)
-        wl = _WordList(self.tokenizer, self.prompt, self.heat_maps[None], words, word_idx, offset_idx,
-                       'GlobalHeatMap.expand_words')
-        out_h, out_w = _image_size(image, *wl.grid)
-        if not words:
-            return [], torch.empty((0, out_h, out_w))
-        out = torch.empty((len(words), out_h, out_w), dtype=torch.float32, device=wl.dev)
-        scratch = wl.scratch(_native.EXPAND_SCRATCH_FLOATS * len(words))
-        with torch.cuda.device(wl.dev):
-            _native.expand_words(wl.maps.data_ptr(), wl.n_rows, wl.grid, wl.rows, out_h, out_w, absolute, threshold,
-                                 wl.word_maps.data_ptr(), out.data_ptr(), scratch.data_ptr(), _stream_ptr(wl.dev))
-        return _word_heat_maps(wl.word_maps[0], words, wl.merged), (out.cpu() if to_cpu else out)
+        wl = _WordList(self.tokenizer, self.prompt, self.heat_maps[None], words, word_idx, offset_idx, image, absolute,
+                       threshold, to_cpu, 'GlobalHeatMap.expand_words')
+        if wl.empty:
+            return [], torch.empty((0, wl.out_h, wl.out_w))
+        out = torch.empty((len(wl.words), wl.out_h, wl.out_w), dtype=torch.float32, device=wl.dev)
+        scratch = wl.scratch(_native.EXPAND_SCRATCH_FLOATS * len(wl.words))
+        with torch.cuda.device(wl.dev):      # daam_expand_words takes one map and no map count
+            _native.expand_words(wl.maps.data_ptr(), wl.n_rows, wl.grid, wl.rows, wl.out_h, wl.out_w, absolute,
+                                 threshold, wl.word_maps.data_ptr(), out.data_ptr(), scratch.data_ptr(),
+                                 _stream_ptr(wl.dev))
+        _, out = wl.done(out)
+        return wl.word_heat_maps(0), out
 
     def segment(self, words, image, absolute: bool = False, threshold: Optional[float] = None, word_idx=None,
                 offset_idx: int = 0, to_cpu: bool = True):
@@ -393,11 +386,9 @@ class GlobalHeatMap:
         default, ``to_cpu=False`` keeps them on the device). At most 96 words; repeated words tie and the first wins.
         An empty list gives all-background labels and -inf scores (the max of nothing). Raises the reference's
         ``ValueError`` for a word that is not in the prompt."""
-        words = list(words)
-        word_maps, merged, labels, scores = _segment(self.tokenizer, self.prompt, self.heat_maps[None], words, image,
-                                                     absolute, threshold, word_idx, offset_idx, to_cpu,
-                                                     'GlobalHeatMap.segment')
-        return _word_heat_maps(word_maps[0], words, merged), labels[0], scores[0]
+        wl, labels, scores = _segment(self.tokenizer, self.prompt, self.heat_maps[None], words, image, absolute,
+                                      threshold, word_idx, offset_idx, to_cpu, 'GlobalHeatMap.segment')
+        return wl.word_heat_maps(0), labels[0], scores[0]
 
     def region_overlap(self, words, image, regions: torch.Tensor, absolute: bool = False,
                        threshold: Optional[float] = None, word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
@@ -415,12 +406,9 @@ class GlobalHeatMap:
         region: the region axis stays, of length 1. At most 96 words, 63 regions and 2**24 image pixels. An empty word
         list or region set launches nothing, returns no word heat maps and measures no word (a word axis of length 0).
         Raises the reference's ``ValueError`` for a word that is not in the prompt."""
-        words = list(words)
-        word_maps, merged, overlap = _region_overlap(self.tokenizer, self.prompt, self.heat_maps[None], words, image,
-                                                     regions, absolute, threshold, word_idx, offset_idx, to_cpu,
-                                                     'GlobalHeatMap.region_overlap')
-        return (_word_heat_maps(word_maps[0], words, merged),
-                RegionOverlap(overlap.intersection[0], overlap.word_area[0], overlap.region_area))
+        wl, overlap = _region_overlap(self.tokenizer, self.prompt, self.heat_maps[None], words, image, regions,
+                                      absolute, threshold, word_idx, offset_idx, to_cpu, 'GlobalHeatMap.region_overlap')
+        return wl.word_heat_maps(0), overlap.map(0)
 
     def word_overlap(self, words, image=None, absolute: bool = False, threshold: Optional[float] = None,
                      word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
@@ -438,12 +426,9 @@ class GlobalHeatMap:
         :class:`WordOverlap` (CPU by default, ``to_cpu=False`` keeps it on the device). At most 96 words and 2**24
         pixels. An empty word list launches nothing and returns empty axes. Raises the reference's ``ValueError`` for a
         word that is not in the prompt."""
-        words = list(words)
-        word_maps, merged, overlap = _word_overlap(self.tokenizer, self.prompt, self.heat_maps[None], words, image,
-                                                   absolute, threshold, word_idx, offset_idx, to_cpu,
-                                                   'GlobalHeatMap.word_overlap')
-        return (_word_heat_maps(word_maps[0], words, merged),
-                WordOverlap(overlap.intersection[0], overlap.word_area[0]))
+        wl, overlap = _word_overlap(self.tokenizer, self.prompt, self.heat_maps[None], words, image, absolute,
+                                    threshold, word_idx, offset_idx, to_cpu, 'GlobalHeatMap.word_overlap')
+        return wl.word_heat_maps(0), overlap.map(0)
 
     def relation_overlap(self, relations, image=None, absolute: bool = False, threshold: Optional[float] = None,
                          offset_idx: int = 0, to_cpu: bool = True) -> 'RelationOverlap':
@@ -455,10 +440,8 @@ class GlobalHeatMap:
         endpoints go through one :meth:`word_overlap` call (at most 96); the returned :class:`RelationOverlap` gathers
         ``iou``, ``iod = ioa()[dep, head]`` and ``ioh = ioa()[head, dep]`` per kept edge. ``relation_overlap(relations,
         absolute=True, threshold=0.15)`` reproduces the paper's per-edge iou / iod / ioh."""
-        rel = _relation_overlap(self.tokenizer, self.prompt, self.heat_maps[None], relations, image, absolute, threshold,
-                                offset_idx, to_cpu, 'GlobalHeatMap.relation_overlap')
-        ov = WordOverlap(rel.overlap.intersection[0], rel.overlap.word_area[0])
-        return RelationOverlap(rel.relations, rel.kept, rel.words, ov, rel.iou[0], rel.iod[0], rel.ioh[0])
+        return _relation_overlap(self.tokenizer, self.prompt, self.heat_maps[None], relations, image, absolute,
+                                 threshold, offset_idx, to_cpu, 'GlobalHeatMap.relation_overlap').map(0)
 
     def word_instances(self, words, image, threshold: float, absolute: bool = False, max_instances: int = 16,
                        word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
@@ -477,11 +460,9 @@ class GlobalHeatMap:
         (a ``ValueError`` otherwise: without a mask there are no components); ``1 <= max_instances <= 64``; at most 96
         words and 2**24 image pixels. An empty word list launches nothing and returns empty axes. Raises the
         reference's ``ValueError`` for a word that is not in the prompt."""
-        words = list(words)
-        word_maps, merged, inst = _word_instances(self.tokenizer, self.prompt, self.heat_maps[None], words, image,
-                                                  threshold, absolute, max_instances, word_idx, offset_idx, to_cpu,
-                                                  'GlobalHeatMap.word_instances')
-        return _word_heat_maps(word_maps[0], words, merged), inst.map(0)
+        wl, inst = _word_instances(self.tokenizer, self.prompt, self.heat_maps[None], words, image, threshold, absolute,
+                                   max_instances, word_idx, offset_idx, to_cpu, 'GlobalHeatMap.word_instances')
+        return wl.word_heat_maps(0), inst.map(0)
 
     def overlay_words(self, words, image, absolute: bool = False, threshold: Optional[float] = None,
                       color_normalize: bool = True, word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
@@ -498,11 +479,9 @@ class GlobalHeatMap:
         frames)``: the list of :class:`WordHeatMap` that :meth:`segment` returns and ``frames`` uint8 ``[len(words), H,
         W, 3]`` (CPU by default, ``to_cpu=False`` keeps them on the device). At most 96 words; an empty list launches
         nothing. Raises the reference's ``ValueError`` for a word that is not in the prompt."""
-        words = list(words)
-        word_maps, merged, frames = _overlay(self.tokenizer, self.prompt, self.heat_maps[None], words, image, absolute,
-                                             threshold, color_normalize, word_idx, offset_idx, to_cpu,
-                                             'GlobalHeatMap.overlay_words', stack=False)
-        return _word_heat_maps(word_maps[0], words, merged), frames[0]
+        wl, frames = _overlay(self.tokenizer, self.prompt, self.heat_maps[None], words, image, absolute, threshold,
+                              color_normalize, word_idx, offset_idx, to_cpu, 'GlobalHeatMap.overlay_words', stack=False)
+        return wl.word_heat_maps(0), frames[0]
 
 
 def _check_rows(rows, n_rows: int):
@@ -512,57 +491,83 @@ def _check_rows(rows, n_rows: int):
             raise IndexError(f'index {r} is out of bounds for dimension 0 with size {n_rows}')
 
 
-def _word_heat_maps(word_maps: torch.Tensor, words, merged) -> List[WordHeatMap]:
-    """One :class:`WordHeatMap` per word: ``word_maps[i]`` (device ``[xh, xw]``) with the word and its index."""
-    return [WordHeatMap(word_maps[i], w, idx) for i, (w, (_, idx)) in enumerate(zip(words, merged))]
+def _word_heat_map(tokenizer, prompt: str, maps: torch.Tensor, word: str, word_idx, offset_idx: int, what: str):
+    """``daam_word_heat_map`` of ``word`` over ``maps`` ``[..., n_rows, xh, xw]``, one launch per ``[n_rows, xh, xw]``
+    map: returns ``(out, word_idx)``, ``out`` the device ``[..., xh, xw]`` word heat maps."""
+    rows, word_idx = compute_token_merge_indices(tokenizer, prompt, word, word_idx, offset_idx)
+    _require_cuda(maps, what)
+    *lead, n_rows, h, w = maps.shape           # ``lead``: [] for one map, [n_maps] for a stack
+    _check_rows(rows, n_rows)
+    maps = maps.detach().float().contiguous()
+    out = torch.empty((*lead, h, w), dtype=torch.float32, device=maps.device)
+    out_bytes = 4 * h * w                      # one fp32 map of ``out``; ``maps`` holds ``n_rows`` of them per map
+    with torch.cuda.device(maps.device):
+        stream = _stream_ptr(maps.device)
+        for t in range(lead[0] if lead else 1):
+            _native.word_heat_map(maps.data_ptr() + t * n_rows * out_bytes, n_rows, (h, w), rows,
+                                  out.data_ptr() + t * out_bytes, stream)
+    return out, word_idx
 
 
 class _WordList:
-    """What the fused word-list ops over ``maps`` ``[n_maps, n_rows, xh, xw]`` share before they launch, in the order
-    they raise: ``compute_token_merge_indices`` of every word (``word_idx`` may be a list parallel to ``words``; the
-    reference's ``ValueError`` for a word not in the prompt, then the row range as torch's advanced indexing checks
-    it), then the CUDA check. Holds the contiguous fp32 maps and the device word heat maps ``[n_maps, len(words), xh,
-    xw]`` the launch writes."""
+    """One fused word-list call over ``maps`` ``[n_maps, n_rows, xh, xw]``. Its checks run in the order they raise:
+    ``compute_token_merge_indices`` of every word (``word_idx`` may be a list parallel to ``words``; the reference's
+    ``ValueError`` for a word not in the prompt, then the row range as torch's advanced indexing checks it), then the
+    CUDA check. Holds the contiguous fp32 maps, the device word heat maps ``[n_maps, len(words), xh, xw]`` the launch
+    writes, and the size ``out_h, out_w`` the maps expand to over ``image`` (the heat-map grid itself ``on_grid``).
+    ``empty``: there is no word or no map, and nothing to launch."""
 
-    def __init__(self, tokenizer, prompt: str, maps: torch.Tensor, words: List[str], word_idx, offset_idx: int,
-                 what: str):
-        self.n_maps, self.n_rows, self.grid = maps.shape[0], maps.shape[1], tuple(maps.shape[-2:])
+    def __init__(self, tokenizer, prompt: str, maps: torch.Tensor, words, word_idx, offset_idx: int, image,
+                 absolute: bool, threshold: Optional[float], to_cpu: bool, what: str, on_grid: bool = False):
+        self.words = words = list(words)
+        n_maps, n_rows, grid = maps.shape[0], maps.shape[1], tuple(maps.shape[-2:])
+        self.n_maps, self.n_rows, self.grid = n_maps, n_rows, grid
         idxs = list(word_idx) if isinstance(word_idx, (list, tuple)) else [word_idx] * len(words)
         self.merged = [compute_token_merge_indices(tokenizer, prompt, w, i, offset_idx) for w, i in zip(words, idxs)]
-        for rows, _ in self.merged:
-            _check_rows(rows, self.n_rows)
         self.rows = [rows for rows, _ in self.merged]
+        _check_rows([r for rows in self.rows for r in rows], n_rows)
         _require_cuda(maps, what)
-        self.dev = maps.device
+        self.dev = dev = maps.device
         self.maps = maps.detach().float().contiguous()
-        self.word_maps = torch.empty((self.n_maps, len(words)) + self.grid, dtype=torch.float32, device=self.dev)
+        self.word_maps = torch.empty((n_maps, len(words)) + grid, dtype=torch.float32, device=dev)
+        self.out_h, self.out_w = grid if on_grid else _image_size(image, *grid)
+        self.absolute, self.threshold, self.to_cpu = absolute, threshold, to_cpu
+        self.empty = not words or n_maps == 0
 
     def scratch(self, n_floats: int) -> torch.Tensor:
         return torch.empty(n_floats, dtype=torch.float32, device=self.dev)
 
+    def launch(self, entry, *args):
+        """``entry``, a ``_native`` word-list call over ``n_maps`` maps, on the maps' device and its current stream:
+        the arguments every such call starts with, then ``args``."""
+        with torch.cuda.device(self.dev):
+            entry(self.maps.data_ptr(), self.n_maps, self.n_rows, self.grid, self.rows, self.out_h, self.out_w,
+                  self.absolute, self.threshold, *args, _stream_ptr(self.dev))
+
+    def done(self, *results):
+        """``(self, *results)``, the results copied to the host when the call asked for it."""
+        return (self, *[r.cpu() for r in results]) if self.to_cpu else (self, *results)
+
+    def word_heat_maps(self, i: int) -> List[WordHeatMap]:
+        """One :class:`WordHeatMap` per word of map ``i``: its device ``[xh, xw]`` map, the word and its index."""
+        maps = self.word_maps[i]
+        return [WordHeatMap(maps[j], w, idx) for j, (w, (_, idx)) in enumerate(zip(self.words, self.merged))]
+
 
 def _segment(tokenizer, prompt: str, maps: torch.Tensor, words, image, absolute, threshold, word_idx, offset_idx: int,
              to_cpu: bool, what: str):
-    """``daam_segment_words`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(word_maps, merged, labels,
-    scores)``: the device word heat maps ``[n_maps, len(words), xh, xw]``, ``compute_token_merge_indices`` of every
-    word, and ``labels`` / ``scores`` ``[n_maps, H, W]``."""
-    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, what)
-    n_maps, dev = wl.n_maps, wl.dev
-    out_h, out_w = _image_size(image, *wl.grid)
-    if not words or n_maps == 0:
-        labels = torch.zeros((n_maps, out_h, out_w), dtype=torch.uint8, device=dev)
-        scores = torch.full((n_maps, out_h, out_w), float('-inf'), device=dev)
-        return wl.word_maps, wl.merged, (labels.cpu() if to_cpu else labels), (scores.cpu() if to_cpu else scores)
-    labels = torch.empty((n_maps, out_h, out_w), dtype=torch.uint8, device=dev)
-    scores = torch.empty((n_maps, out_h, out_w), dtype=torch.float32, device=dev)
-    scratch = wl.scratch(_native.segment_scratch_floats(n_maps, len(words)))
-    with torch.cuda.device(dev):
-        _native.segment_words(wl.maps.data_ptr(), n_maps, wl.n_rows, wl.grid, wl.rows, out_h, out_w, absolute,
-                              threshold, wl.word_maps.data_ptr(), labels.data_ptr(), scores.data_ptr(),
-                              scratch.data_ptr(), _stream_ptr(dev))
-    if to_cpu:
-        labels, scores = labels.cpu(), scores.cpu()
-    return wl.word_maps, wl.merged, labels, scores
+    """``daam_segment_words`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(wl, labels, scores)``, the
+    :class:`_WordList` and ``labels`` / ``scores`` ``[n_maps, H, W]``."""
+    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, image, absolute, threshold, to_cpu, what)
+    shape = (wl.n_maps, wl.out_h, wl.out_w)
+    if wl.empty:
+        return wl.done(torch.zeros(shape, dtype=torch.uint8, device=wl.dev),
+                       torch.full(shape, float('-inf'), device=wl.dev))
+    labels = torch.empty(shape, dtype=torch.uint8, device=wl.dev)
+    scores = torch.empty(shape, dtype=torch.float32, device=wl.dev)
+    scratch = wl.scratch(_native.segment_scratch_floats(wl.n_maps, len(wl.words)))
+    wl.launch(_native.segment_words, wl.word_maps.data_ptr(), labels.data_ptr(), scores.data_ptr(), scratch.data_ptr())
+    return wl.done(labels, scores)
 
 
 @dataclass
@@ -574,6 +579,13 @@ class RegionOverlap:
     intersection: torch.Tensor
     word_area: torch.Tensor
     region_area: torch.Tensor
+
+    def map(self, i: int) -> 'RegionOverlap':
+        """The overlap of map ``i`` of a stack (``region_area`` has no map axis and stays whole)."""
+        return RegionOverlap(self.intersection[i], self.word_area[i], self.region_area)
+
+    def cpu(self) -> 'RegionOverlap':
+        return RegionOverlap(self.intersection.cpu(), self.word_area.cpu(), self.region_area.cpu())
 
     def iou(self) -> torch.Tensor:
         """``I / (A_w + A_r - I + 1e-8)``: ``compute_iou(mask, region)`` of every pair."""
@@ -592,12 +604,11 @@ class RegionOverlap:
 
 def _region_overlap(tokenizer, prompt: str, maps: torch.Tensor, words, image, regions, absolute, threshold, word_idx,
                     offset_idx: int, to_cpu: bool, what: str):
-    """``daam_region_overlap`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(word_maps, merged, overlap)``: the
-    device word heat maps ``[n_maps, len(words), xh, xw]``, ``compute_token_merge_indices`` of every word, and the
-    :class:`RegionOverlap` with a leading map axis."""
-    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, what)
-    n_maps, grid, dev = wl.n_maps, wl.grid, wl.dev
-    out_h, out_w = _image_size(image, *grid)
+    """``daam_region_overlap`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(wl, overlap)``, the
+    :class:`_WordList` and the :class:`RegionOverlap` with a leading map axis. Without regions no word is measured: the
+    word list then holds no word and no word heat map."""
+    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, image, absolute, threshold, to_cpu, what)
+    n_maps, out_h, out_w, dev = wl.n_maps, wl.out_h, wl.out_w, wl.dev
     if not isinstance(regions, torch.Tensor):
         raise TypeError(f'{what}: regions must be a torch.Tensor, not {type(regions).__name__}')
     if regions.dtype not in (torch.bool, torch.uint8):
@@ -610,31 +621,21 @@ def _region_overlap(tokenizer, prompt: str, maps: torch.Tensor, words, image, re
     _require_cuda(regions, what)
     if regions.device != dev:
         raise ValueError(f'{what}: regions are on {regions.device}, the heat maps on {dev}')
-    n_regions = regions.shape[0]
-    if not words or n_regions == 0 or n_maps == 0:
-        ov = RegionOverlap(torch.zeros((n_maps, n_regions, 0), device=dev), torch.zeros((n_maps, 0), device=dev),
-                           torch.zeros((n_regions,), device=dev))
-        word_maps = torch.empty((n_maps, 0) + grid, dtype=torch.float32, device=dev)
-        return word_maps, [], (_to_cpu(ov) if to_cpu else ov)
+    n_regions, n_words = regions.shape[0], len(wl.words)
+    if wl.empty or n_regions == 0:            # no word is measured: the call returns no word heat maps
+        wl.words, wl.merged = [], []
+        wl.word_maps = torch.empty((n_maps, 0) + wl.grid, dtype=torch.float32, device=dev)
+        return wl.done(RegionOverlap(torch.zeros((n_maps, n_regions, 0), device=dev),
+                                     torch.zeros((n_maps, 0), device=dev), torch.zeros((n_regions,), device=dev)))
     region_bytes = regions.detach().contiguous().view(torch.uint8)
-    inter = torch.empty((n_maps, n_regions, len(words)), dtype=torch.float32, device=dev)
-    area = torch.empty((n_maps, len(words)), dtype=torch.float32, device=dev)
-    scratch = wl.scratch(_native.region_scratch_floats(n_maps, len(words), n_regions, out_h, out_w))
-    with torch.cuda.device(dev):
-        _native.region_overlap(wl.maps.data_ptr(), n_maps, wl.n_rows, grid, wl.rows, out_h, out_w, absolute, threshold,
-                               wl.word_maps.data_ptr(), region_bytes.data_ptr(), n_regions, inter.data_ptr(),
-                               area.data_ptr(), scratch.data_ptr(), _stream_ptr(dev))
+    inter = torch.empty((n_maps, n_regions, n_words), dtype=torch.float32, device=dev)
+    area = torch.empty((n_maps, n_words), dtype=torch.float32, device=dev)
+    scratch = wl.scratch(_native.region_scratch_floats(n_maps, n_words, n_regions, out_h, out_w))
+    wl.launch(_native.region_overlap, wl.word_maps.data_ptr(), region_bytes.data_ptr(), n_regions, inter.data_ptr(),
+              area.data_ptr(), scratch.data_ptr())
     # exact pixel counts (at most 2**24 pixels): what ``region.float().sum()`` gives in compute_iou
     region_area = (region_bytes != 0).sum((-1, -2)).float()
-    ov = RegionOverlap(inter, area, region_area)
-    return wl.word_maps, wl.merged, (_to_cpu(ov) if to_cpu else ov)
-
-
-def _to_cpu(ov):
-    """A :class:`RegionOverlap` or :class:`WordOverlap` with every tensor copied to the host."""
-    if isinstance(ov, WordOverlap):
-        return WordOverlap(ov.intersection.cpu(), ov.word_area.cpu())
-    return RegionOverlap(ov.intersection.cpu(), ov.word_area.cpu(), ov.region_area.cpu())
+    return wl.done(RegionOverlap(inter, area, region_area))
 
 
 @dataclass
@@ -645,6 +646,13 @@ class WordOverlap:
     (``daam/evaluate.py``) in the same fp32 operation order."""
     intersection: torch.Tensor
     word_area: torch.Tensor
+
+    def map(self, i: int) -> 'WordOverlap':
+        """The overlap of map ``i`` of a stack."""
+        return WordOverlap(self.intersection[i], self.word_area[i])
+
+    def cpu(self) -> 'WordOverlap':
+        return WordOverlap(self.intersection.cpu(), self.word_area.cpu())
 
     def iou(self) -> torch.Tensor:
         """``[a, b] = I / (A[a] + A[b] - I + 1e-8)``: ``compute_iou(mask_a, mask_b)`` of every pair (and the DAAM
@@ -672,35 +680,35 @@ class RelationOverlap:
     iod: torch.Tensor
     ioh: torch.Tensor
 
+    def map(self, i: int) -> 'RelationOverlap':
+        """The overlap of map ``i`` of a stack."""
+        return RelationOverlap(self.relations, self.kept, self.words, self.overlap.map(i), self.iou[i], self.iod[i],
+                               self.ioh[i])
+
 
 def _word_overlap(tokenizer, prompt: str, maps: torch.Tensor, words, image, absolute, threshold, word_idx,
                   offset_idx: int, to_cpu: bool, what: str):
-    """``daam_word_overlap`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(word_maps, merged, overlap)``: the
-    device word heat maps ``[n_maps, len(words), xh, xw]``, ``compute_token_merge_indices`` of every word, and the
-    :class:`WordOverlap` with a leading map axis. ``image=None``: the sums run over the heat-map grid."""
-    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, what)
-    n_maps, grid, dev = wl.n_maps, wl.grid, wl.dev
-    out_h, out_w = grid if image is None else _image_size(image, *grid)
-    n = len(words)
-    if not words or n_maps == 0:
-        ov = WordOverlap(torch.zeros((n_maps, n, n), device=dev), torch.zeros((n_maps, n), device=dev))
-        return wl.word_maps, wl.merged, (_to_cpu(ov) if to_cpu else ov)
+    """``daam_word_overlap`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(wl, overlap)``, the
+    :class:`_WordList` and the :class:`WordOverlap` with a leading map axis. ``image=None``: the sums run over the
+    heat-map grid."""
+    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, image, absolute, threshold, to_cpu, what,
+                   on_grid=image is None)
+    n_maps, n, dev = wl.n_maps, len(wl.words), wl.dev
+    if wl.empty:
+        return wl.done(WordOverlap(torch.zeros((n_maps, n, n), device=dev), torch.zeros((n_maps, n), device=dev)))
     inter = torch.empty((n_maps, n, n), dtype=torch.float32, device=dev)
     area = torch.empty((n_maps, n), dtype=torch.float32, device=dev)
-    scratch = wl.scratch(_native.word_overlap_scratch_floats(n_maps, n, out_h, out_w))
-    with torch.cuda.device(dev):
-        _native.word_overlap(wl.maps.data_ptr(), n_maps, wl.n_rows, grid, wl.rows, out_h, out_w, absolute, threshold,
-                             wl.word_maps.data_ptr(), inter.data_ptr(), area.data_ptr(), scratch.data_ptr(),
-                             _stream_ptr(dev))
-    ov = WordOverlap(inter, area)
-    return wl.word_maps, wl.merged, (_to_cpu(ov) if to_cpu else ov)
+    scratch = wl.scratch(_native.word_overlap_scratch_floats(n_maps, n, wl.out_h, wl.out_w))
+    wl.launch(_native.word_overlap, wl.word_maps.data_ptr(), inter.data_ptr(), area.data_ptr(), scratch.data_ptr())
+    return wl.done(WordOverlap(inter, area))
 
 
 def _relation_overlap(tokenizer, prompt: str, maps: torch.Tensor, relations, image, absolute, threshold,
                       offset_idx: int, to_cpu: bool, what: str) -> RelationOverlap:
     """``relation_overlap`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: the distinct endpoints of the edges whose words
     are in the prompt -- one endpoint per row set, so a word given twice, in another case, or as its token index is
-    measured once -- then one ``_word_overlap`` call and a gather; every tensor has a leading map axis."""
+    measured once -- then one ``_word_overlap`` call and a gather (on the host when ``to_cpu``); every tensor has a
+    leading map axis."""
     kept_edges, kept, words, word_idx, ends = [], [], [], [], []
     slot: Dict[Tuple[int, ...], int] = {}
     for e, edge in enumerate(relations):
@@ -725,8 +733,8 @@ def _relation_overlap(tokenizer, prompt: str, maps: torch.Tensor, relations, ima
         raise ValueError(f'{what}: {len(words)} distinct endpoints > {_native.MAX_SEGMENT_WORDS}, the word limit of '
                          f'one word_overlap call')
     labels = [x if isinstance(x, str) else str(x) for x in words]
-    _, _, ov = _word_overlap(tokenizer, prompt, maps, labels, image, absolute, threshold, word_idx, offset_idx, to_cpu,
-                             what)
+    _, ov = _word_overlap(tokenizer, prompt, maps, labels, image, absolute, threshold, word_idx, offset_idx, to_cpu,
+                          what)
     dev = ov.intersection.device
     h = torch.tensor([i for i, _ in ends], dtype=torch.long, device=dev)
     d = torch.tensor([j for _, j in ends], dtype=torch.long, device=dev)
@@ -792,10 +800,10 @@ _INSTANCE_FIELDS = ('count', 'area', 'box', 'sum_yx', 'peak', 'peak_yx')
 
 def _word_instances(tokenizer, prompt: str, maps: torch.Tensor, words, image, threshold, absolute, max_instances: int,
                     word_idx, offset_idx: int, to_cpu: bool, what: str):
-    """``daam_word_instances`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(word_maps, merged, instances)``: the
-    device word heat maps ``[n_maps, len(words), xh, xw]``, ``compute_token_merge_indices`` of every word, and the
-    :class:`WordInstances` with a leading map axis. Scratch: :data:`WORD_INSTANCES_SCRATCH_BYTES`, clipped to the planes
-    the call has, at least one plane."""
+    """``daam_word_instances`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(wl, instances)``, the
+    :class:`_WordList` and the :class:`WordInstances` with a leading map axis. Scratch:
+    :data:`WORD_INSTANCES_SCRATCH_BYTES`, clipped to the planes the call has, at least one plane."""
+    words = list(words)
     if not threshold:
         raise ValueError(f'{what}: threshold must be set (truthy), not {threshold!r}: the instances are the connected '
                          f'components of the mask expand_words(..., threshold) returns')
@@ -805,25 +813,21 @@ def _word_instances(tokenizer, prompt: str, maps: torch.Tensor, words, image, th
                          f'{max_instances!r}')
     if len(words) > _native.MAX_SEGMENT_WORDS:
         raise ValueError(f'{what}: {len(words)} words > {_native.MAX_SEGMENT_WORDS}, the word limit of one call')
-    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, what)
-    n_maps, grid, dev = wl.n_maps, wl.grid, wl.dev
-    out_h, out_w = _image_size(image, *grid)
+    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, image, absolute, threshold, to_cpu, what)
+    n_maps, dev = wl.n_maps, wl.dev
     n, k = len(words), max_instances
-    new = torch.empty if words and n_maps else torch.zeros     # the kernels write every slot
+    new = torch.zeros if wl.empty else torch.empty     # the kernels write every slot
     i32 = dict(dtype=torch.int32, device=dev)
     inst = WordInstances(new((n_maps, n), **i32), new((n_maps, n, k), **i32), new((n_maps, n, k, 4), **i32),
                          new((n_maps, n, k, 2), dtype=torch.int64, device=dev),
                          new((n_maps, n, k), dtype=torch.float32, device=dev), new((n_maps, n, k, 2), **i32))
-    if words and n_maps:
-        plane = _native.word_instances_plane_bytes(out_h, out_w)
+    if not wl.empty:
+        plane = _native.word_instances_plane_bytes(wl.out_h, wl.out_w)
         n_bytes = max(plane, min(WORD_INSTANCES_SCRATCH_BYTES, plane * n_maps * n))
         scratch = torch.empty(n_bytes, dtype=torch.uint8, device=dev)
-        with torch.cuda.device(dev):
-            _native.word_instances(wl.maps.data_ptr(), n_maps, wl.n_rows, grid, wl.rows, out_h, out_w, absolute,
-                                   threshold, k, wl.word_maps.data_ptr(),
-                                   *(getattr(inst, f).data_ptr() for f in _INSTANCE_FIELDS), scratch.data_ptr(),
-                                   n_bytes, _stream_ptr(dev))
-    return wl.word_maps, wl.merged, (inst.cpu() if to_cpu else inst)
+        wl.launch(_native.word_instances, k, wl.word_maps.data_ptr(),
+                  *(getattr(inst, f).data_ptr() for f in _INSTANCE_FIELDS), scratch.data_ptr(), n_bytes)
+    return wl.done(inst)
 
 
 def jet_colormap() -> torch.Tensor:
@@ -865,26 +869,24 @@ def _overlay_image(image, n_maps: int, grid, dev, what: str, stack: bool):
 
 def _overlay(tokenizer, prompt: str, maps: torch.Tensor, words, image, absolute, threshold, color_normalize, word_idx,
              offset_idx: int, to_cpu: bool, what: str, stack: bool):
-    """``daam_overlay_words`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(word_maps, merged, frames)``: the
-    device word heat maps ``[n_maps, len(words), xh, xw]``, ``compute_token_merge_indices`` of every word, and
-    ``frames`` uint8 ``[n_maps, len(words), H, W, 3]``."""
-    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, what)
-    n_maps, dev = wl.n_maps, wl.dev
-    image, out_h, out_w, per_map = _overlay_image(image, n_maps, wl.grid, dev, what, stack)
-    shape = (n_maps, len(words), out_h, out_w, 3)
-    if not words or n_maps == 0:
-        frames = torch.empty(shape, dtype=torch.uint8, device='cpu' if to_cpu else dev)
-        return wl.word_maps, wl.merged, frames
+    """``daam_overlay_words`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(wl, frames)``, the
+    :class:`_WordList` and ``frames`` uint8 ``[n_maps, len(words), H, W, 3]``. The image fixes the size the maps
+    expand to."""
+    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, None, absolute, threshold, to_cpu, what,
+                   on_grid=True)         # the size is the image's, once _overlay_image has checked it
+    n_maps, n_words, dev = wl.n_maps, len(wl.words), wl.dev
+    image, wl.out_h, wl.out_w, per_map = _overlay_image(image, n_maps, wl.grid, dev, what, stack)
+    shape = (n_maps, n_words, wl.out_h, wl.out_w, 3)
+    if wl.empty:
+        return wl.done(torch.empty(shape, dtype=torch.uint8, device=dev))
     image = image.to(dev).contiguous()                   # one copy to the device
     # the kernel writes whole 4-byte words: the frames are a view of a buffer rounded up to them
     buf = torch.empty(_native.overlay_frames_bytes(*shape[:4]), dtype=torch.uint8, device=dev)
-    frames = buf[:n_maps * len(words) * out_h * out_w * 3].view(shape)
-    scratch = wl.scratch(_native.segment_scratch_floats(n_maps, len(words)))
-    with torch.cuda.device(dev):
-        _native.overlay_words(wl.maps.data_ptr(), n_maps, wl.n_rows, wl.grid, wl.rows, out_h, out_w, absolute, threshold,
-                              color_normalize, wl.word_maps.data_ptr(), image.data_ptr(),
-                              out_h * out_w * 3 if per_map else 0, buf.data_ptr(), scratch.data_ptr(), _stream_ptr(dev))
-    return wl.word_maps, wl.merged, (frames.cpu() if to_cpu else frames)
+    frames = buf[:n_maps * n_words * wl.out_h * wl.out_w * 3].view(shape)
+    scratch = wl.scratch(_native.segment_scratch_floats(n_maps, n_words))
+    wl.launch(_native.overlay_words, color_normalize, wl.word_maps.data_ptr(), image.data_ptr(),
+              wl.out_h * wl.out_w * 3 if per_map else 0, buf.data_ptr(), scratch.data_ptr())
+    return wl.done(frames)
 
 
 class GlobalHeatMapStack:
@@ -907,18 +909,8 @@ class GlobalHeatMapStack:
 
     def word_heat_maps(self, word: str, word_idx: int = None, offset_idx: int = 0) -> torch.Tensor:
         """``[maps, xh, xw]``: row ``t`` is ``self[t].compute_word_heat_map(word, word_idx, offset_idx).heatmap``."""
-        rows, _ = compute_token_merge_indices(self.tokenizer, self.prompt, word, word_idx, offset_idx)
-        maps = self.heat_maps
-        _require_cuda(maps, f'{type(self).__name__}.word_heat_maps')
-        steps, n_rows, grid = maps.shape[0], maps.shape[1], tuple(maps.shape[-2:])
-        _check_rows(rows, n_rows)
-        maps = maps.detach().float().contiguous()
-        out = torch.empty((steps,) + grid, dtype=torch.float32, device=maps.device)
-        with torch.cuda.device(maps.device):
-            stream = _stream_ptr(maps.device)
-            for t in range(steps):
-                _native.word_heat_map(maps[t].data_ptr(), n_rows, grid, rows, out[t].data_ptr(), stream)
-        return out
+        return _word_heat_map(self.tokenizer, self.prompt, self.heat_maps, word, word_idx, offset_idx,
+                              f'{type(self).__name__}.word_heat_maps')[0]
 
     def segment(self, words, image, absolute: bool = False, threshold: Optional[float] = None, word_idx=None,
                 offset_idx: int = 0, to_cpu: bool = True):
@@ -926,10 +918,9 @@ class GlobalHeatMapStack:
         ``(word_maps, labels, scores)`` with ``word_maps`` the device ``[maps, len(words), xh, xw]`` word heat maps and
         ``labels`` / ``scores`` ``[maps, H, W]``; row ``t`` equals ``self[t].segment(...)`` bit for bit (min / max
         normalisation per map and word)."""
-        word_maps, _, labels, scores = _segment(self.tokenizer, self.prompt, self.heat_maps, list(words), image,
-                                                absolute, threshold, word_idx, offset_idx, to_cpu,
-                                                f'{type(self).__name__}.segment')
-        return word_maps, labels, scores
+        wl, labels, scores = _segment(self.tokenizer, self.prompt, self.heat_maps, words, image, absolute, threshold,
+                                      word_idx, offset_idx, to_cpu, f'{type(self).__name__}.segment')
+        return wl.word_maps, labels, scores
 
     def region_overlap(self, words, image, regions: torch.Tensor, absolute: bool = False,
                        threshold: Optional[float] = None, word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
@@ -938,10 +929,9 @@ class GlobalHeatMapStack:
         ``overlap`` a :class:`RegionOverlap` with a leading map axis (``intersection`` ``[maps, R, W]``, ``word_area``
         ``[maps, W]``); row ``t`` equals ``self[t].region_overlap(...)`` bit for bit (min / max normalisation per map
         and word). E.g. ``overlap.iou()[:, 0, 0]`` is word 0's IoU with region 0 at every step of a history."""
-        word_maps, _, overlap = _region_overlap(self.tokenizer, self.prompt, self.heat_maps, list(words), image,
-                                                regions, absolute, threshold, word_idx, offset_idx, to_cpu,
-                                                f'{type(self).__name__}.region_overlap')
-        return word_maps, overlap
+        wl, overlap = _region_overlap(self.tokenizer, self.prompt, self.heat_maps, words, image, regions, absolute,
+                                      threshold, word_idx, offset_idx, to_cpu, f'{type(self).__name__}.region_overlap')
+        return wl.word_maps, overlap
 
     def word_overlap(self, words, image=None, absolute: bool = False, threshold: Optional[float] = None,
                      word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
@@ -950,10 +940,9 @@ class GlobalHeatMapStack:
         ``overlap`` a :class:`WordOverlap` with a leading map axis (``intersection`` ``[maps, W, W]``, ``word_area``
         ``[maps, W]``); row ``t`` equals ``self[t].word_overlap(...)`` bit for bit (min / max normalisation per map and
         word). E.g. ``overlap.iou()[:, i, j]`` is the IoU of words ``i`` and ``j`` at every step of a history."""
-        word_maps, _, overlap = _word_overlap(self.tokenizer, self.prompt, self.heat_maps, list(words), image, absolute,
-                                              threshold, word_idx, offset_idx, to_cpu,
-                                              f'{type(self).__name__}.word_overlap')
-        return word_maps, overlap
+        wl, overlap = _word_overlap(self.tokenizer, self.prompt, self.heat_maps, words, image, absolute, threshold,
+                                    word_idx, offset_idx, to_cpu, f'{type(self).__name__}.word_overlap')
+        return wl.word_maps, overlap
 
     def relation_overlap(self, relations, image=None, absolute: bool = False, threshold: Optional[float] = None,
                          offset_idx: int = 0, to_cpu: bool = True) -> 'RelationOverlap':
@@ -970,10 +959,9 @@ class GlobalHeatMapStack:
         ``t`` equals ``self[t].word_instances(...)`` bit for bit (min / max normalisation per map and word). E.g.
         ``instances.count[:, 0]`` is how many blobs word 0 makes at every step of a history. Scratch stays within a
         fixed budget whatever the map count: the planes are labelled in rounds."""
-        word_maps, _, inst = _word_instances(self.tokenizer, self.prompt, self.heat_maps, list(words), image, threshold,
-                                             absolute, max_instances, word_idx, offset_idx, to_cpu,
-                                             f'{type(self).__name__}.word_instances')
-        return word_maps, inst
+        wl, inst = _word_instances(self.tokenizer, self.prompt, self.heat_maps, words, image, threshold, absolute,
+                                   max_instances, word_idx, offset_idx, to_cpu, f'{type(self).__name__}.word_instances')
+        return wl.word_maps, inst
 
     def overlay_words(self, words, image, absolute: bool = False, threshold: Optional[float] = None,
                       color_normalize: bool = True, word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
@@ -983,10 +971,10 @@ class GlobalHeatMapStack:
         (colour scale per map and word). ``image`` is one image for every map, or a uint8 ``[maps, H, W, 3]`` array
         with one per map (e.g. the images of ``compute_image_heat_maps()``). ``frames[:, w]`` is word ``w`` forming over
         a history, frame by frame."""
-        word_maps, _, frames = _overlay(self.tokenizer, self.prompt, self.heat_maps, list(words), image, absolute,
-                                        threshold, color_normalize, word_idx, offset_idx, to_cpu,
-                                        f'{type(self).__name__}.overlay_words', stack=True)
-        return word_maps, frames
+        wl, frames = _overlay(self.tokenizer, self.prompt, self.heat_maps, words, image, absolute, threshold,
+                              color_normalize, word_idx, offset_idx, to_cpu, f'{type(self).__name__}.overlay_words',
+                              stack=True)
+        return wl.word_maps, frames
 
 
 class TimeHeatMaps(GlobalHeatMapStack):
