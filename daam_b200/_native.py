@@ -38,6 +38,16 @@ def region_scratch_floats(n_maps: int, n_words: int, n_regions: int, out_h: int,
     return n_maps * n_words * (64 + (n_regions + 1) * ((out_h + 15) // 16) * ((out_w + 63) // 64))
 
 
+SWEEP_MAX_THRESHOLDS = 64    # DAAM_REGION_SWEEP_MAX_THRESHOLDS: thresholds per daam_region_sweep call
+
+
+def region_sweep_scratch_floats(n_maps: int, n_words: int, n_regions: int, n_thresholds: int, out_h: int,
+                                out_w: int) -> int:
+    """``DAAM_REGION_SWEEP_SCRATCH_FLOATS(n_maps, n_words, n_regions, n_thresholds, out_h, out_w)``: the min / max
+    partials and one histogram per (map, word); the output size does not enter."""
+    return n_maps * n_words * (64 + (n_regions + 1) * n_thresholds)
+
+
 WORD_OVERLAP_CTAS = 256      # DAAM_WORD_OVERLAP_CTAS: daam_word_overlap's CTAs per map
 
 
@@ -63,7 +73,7 @@ def overlay_frames_bytes(n_maps: int, n_words: int, out_h: int, out_w: int) -> i
 
 EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize',
            'daam_finalize_maps', 'daam_finalize_parts', 'daam_finalize_per_key','daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
-           'daam_segment_words', 'daam_region_overlap', 'daam_word_overlap', 'daam_word_instances', 'daam_overlay_words', 'daam_jet_colormap',
+           'daam_segment_words', 'daam_region_overlap', 'daam_region_sweep', 'daam_word_overlap', 'daam_word_instances', 'daam_overlay_words', 'daam_jet_colormap',
            'daam_side_launcher_create', 'daam_side_launcher_destroy',
            'daam_side_launcher_launch', 'daam_side_launcher_join', 'daam_side_launcher_idle', 'daam_abi_version',
            'daam_last_error', 'daam_device_info', 'daam_launch_count')
@@ -170,6 +180,9 @@ def load() -> ctypes.CDLL:
     lib.daam_region_overlap.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
                                         i32, i32, f32, vp, vp, i32, vp, vp, vp, vp]
     lib.daam_region_overlap.restype = ctypes.c_int
+    lib.daam_region_sweep.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
+                                      i32, ctypes.POINTER(f32), i32, vp, vp, i32, vp, vp, vp, vp]
+    lib.daam_region_sweep.restype = ctypes.c_int
     lib.daam_word_overlap.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
                                       i32, i32, f32, vp, vp, vp, vp, vp]
     lib.daam_word_overlap.restype = ctypes.c_int
@@ -431,6 +444,20 @@ def region_overlap(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Se
                                       ctypes.c_void_p(word_maps_ptr), ctypes.c_void_p(regions_ptr), n_regions,
                                       ctypes.c_void_p(intersection_ptr), ctypes.c_void_p(word_area_ptr),
                                       ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
+
+
+def region_sweep(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int,
+                 out_w: int, absolute: bool, thresholds: Sequence[float], word_maps_ptr: int, regions_ptr: int,
+                 n_regions: int, intersection_ptr: int, word_area_ptr: int, scratch_ptr: int, stream: int):
+    """``daam_region_sweep`` over ``n_maps`` maps ``[n_rows, h, w]`` back to back and ``n_regions`` uint8 regions
+    ``[out_h, out_w]``, at ``thresholds`` (passed as a host fp32 array): ``intersection`` ``[n_maps, T, n_regions,
+    n_words]``, ``word_area`` ``[n_maps, T, n_words]``."""
+    taus = (ctypes.c_float * max(len(thresholds), 1))(*thresholds)
+    _check(load().daam_region_sweep(ctypes.c_void_p(maps_ptr), n_maps, n_rows,
+                                    *_word_list(x, rows_per_word, out_h, out_w, absolute, None)[:-2],
+                                    taus, len(thresholds), ctypes.c_void_p(word_maps_ptr), ctypes.c_void_p(regions_ptr),
+                                    n_regions, ctypes.c_void_p(intersection_ptr), ctypes.c_void_p(word_area_ptr),
+                                    ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
 
 
 def word_overlap(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int,

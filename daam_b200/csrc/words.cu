@@ -12,15 +12,17 @@
 //  - expand_words_kernel writes it (one cooperative launch, steps 1, 2 and 4 in one kernel);
 //  - segment_label_kernel keeps each pixel's max / argmax over the words;
 //  - region_tile_kernel sums it over binary image regions (then region_reduce_kernel);
+//  - region_sweep_tile_kernel counts, per region, the pixels where it passes each of a list of thresholds (then
+//    region_sweep_reduce_kernel);
 //  - overlay_kernel blends its jet colour onto the image;
 //  - word_pair_tile_kernel sums m[a] * m[b] over every pair of words (then word_pair_reduce_kernel);
 //  - instance_mask_kernel writes it without threshold for components.cu, which labels the mask m > threshold.
 // The tile kernels run after segment_minmax_kernel (steps 1 and 2, the word maps and min / max partials to global
-// memory); region_tile_kernel, overlay_kernel, word_pair_tile_kernel and instance_mask_kernel share the tile helpers
+// memory); region_tile_kernel, region_sweep_tile_kernel, overlay_kernel, word_pair_tile_kernel and instance_mask_kernel share the tile helpers
 // (block_tile / tile_at, word_bounds, stage_windows, tap tables). expand_words_kernel, segment_minmax_kernel and segment_label_kernel keep
 // their steps inline: written with the helpers, nvcc scheduled them differently and they measured slower. Every consumer's m is expand_words_kernel's
-// value bit for bit. Deterministic: no atomics here (components.cu's are integer atomics, whose results do not depend
-// on their order).
+// value bit for bit. Deterministic: the only atomics here are region_sweep_tile_kernel's integer adds (and
+// components.cu's are integer atomics), whose results do not depend on their order.
 #include <cooperative_groups.h>
 #include <math.h>
 
@@ -379,6 +381,29 @@ __device__ __forceinline__ float warp_reduce_scatter32(float (&s)[32]) {
   return s[0];
 }
 
+// Slot bits of the thread's pixels: bit j of mask[g][k] says tile pixel threadIdx.x + 256 k counts towards slot
+// 32 g + j (slot 0: every pixel of the tile, slot 1 + r: the pixels inside region r of `regions` [n_regions][oh][ow]);
+// each region byte is read once
+__device__ __forceinline__ void region_slot_masks(const unsigned char* regions, int n_regions, int oh, int ow,
+                                                  const Tile& T, unsigned (&mask)[2][kSegPix]) {
+  const long long n = (long long)oh * ow;
+#pragma unroll
+  for (int k = 0; k < kSegPix; ++k) {
+    const int p = threadIdx.x + 256 * k;
+    mask[0][k] = 0u; mask[1][k] = 0u;
+    if (p < T.th * T.tw) {
+      const int py = p / T.tw;
+      const unsigned char* reg = regions + (long long)(T.y0 + py) * ow + T.x0 + p - py * T.tw;
+      unsigned m0 = 1u, m1 = 0u;
+      for (int r = 0; r < n_regions; ++r) {
+        const unsigned bit = __ldg(reg + r * n) != 0 ? 1u : 0u;
+        if (r < 31) m0 |= bit << (r + 1); else m1 |= bit << (r - 31);
+      }
+      mask[0][k] = m0; mask[1][k] = m1;
+    }
+  }
+}
+
 // grid: (tiles of kSegTileH x kSegTileW output pixels, n_maps); dynamic smem: words_per_pass source windows
 __global__ void __launch_bounds__(256) region_tile_kernel(const __grid_constant__ RegionParams R) {
   extern __shared__ __align__(16) float win[];
@@ -392,25 +417,8 @@ __global__ void __launch_bounds__(256) region_tile_kernel(const __grid_constant_
   const int n_slots = R.n_regions + 1;
   for (int w = threadIdx.x; w < n_words; w += blockDim.x) word_bounds(P, map, w, s_lo[w], s_hi[w]);
   fill_tap_tables(P, T, taps);
-  // slot bits of the thread's pixels: bit j of mask[g][k] says pixel k counts towards slot 32 g + j (slot 0: every
-  // pixel of the tile, slot 1 + r: the pixels inside region r); each region byte is read once
-  const long long n = (long long)oh * ow;
   unsigned mask[2][kSegPix];
-#pragma unroll
-  for (int k = 0; k < kSegPix; ++k) {
-    const int p = threadIdx.x + 256 * k;
-    mask[0][k] = 0u; mask[1][k] = 0u;
-    if (p < T.th * T.tw) {
-      const int py = p / T.tw;
-      const unsigned char* reg = R.regions + (long long)(T.y0 + py) * ow + T.x0 + p - py * T.tw;
-      unsigned m0 = 1u, m1 = 0u;
-      for (int r = 0; r < R.n_regions; ++r) {
-        const unsigned bit = __ldg(reg + r * n) != 0 ? 1u : 0u;
-        if (r < 31) m0 |= bit << (r + 1); else m1 |= bit << (r - 31);
-      }
-      mask[0][k] = m0; mask[1][k] = m1;
-    }
-  }
+  region_slot_masks(R.regions, R.n_regions, oh, ow, T, mask);
   const float* word_maps = P.word_maps + (long long)map * n_words * P.mh * P.mw;
   float* partials = R.partials + (long long)map * n_words * n_slots * R.tiles + blockIdx.x;
   for (int w0 = 0; w0 < n_words; w0 += P.words_per_pass) {
@@ -482,6 +490,152 @@ __global__ void __launch_bounds__(256) region_reduce_kernel(const float* __restr
       const long long map = mword / n_words, word = mword - map * n_words;
       intersection[(map * n_regions + slot - 1) * n_words + word] = s;
     }
+  }
+}
+
+// ---- threshold sweeps of word-region overlap: exact counts at up to 64 thresholds in one pass ----------------------
+// With m[w] taken without threshold, R[r] as above and ascending thresholds tau[0 .. T):
+//   intersection[map][k][r][w] = #{p : R[r](p) and m[w](p) > tau[k]},   word_area[map][k][w] = #{p : m[w](p) > tau[k]}
+// A pixel's bucket b = #{k : m > tau[k]} says it passes exactly thresholds 0 .. b - 1, so one histogram of b per
+// (map, word, slot) holds every count: count[k] = sum_{b > k} hist[b]. region_sweep_tile_kernel builds the
+// histograms; pixels of bucket 0 pass nothing and are not counted. Per word and pixel row of a warp (the warp's 32
+// pixels k), the lanes of one bucket meet in __match_any_sync and their leader adds, per slot present in the warp,
+// the popcount of those lanes inside the slot into the CTA's shared histogram of the word. After one barrier per word
+// the CTA adds its nonzero bins to the global histograms `counts` (zeroed before the launch) with integer atomics;
+// region_sweep_reduce_kernel takes the suffix sums. Every count is an integer, so the bits do not depend on the order
+// of the atomics, and below 2^24 pixels every count is exact in fp32.
+constexpr int kMaxThresholds = DAAM_REGION_SWEEP_MAX_THRESHOLDS;
+
+struct SweepParams {
+  WordListParams s;                     // use_threshold 0; words_per_pass 0: m is read from the word maps
+  const unsigned char* regions;         // [n_regions][oh][ow]
+  unsigned* counts;                     // [n_maps][n_words][n_regions + 1][T]: bin b - 1 holds bucket b
+  int n_regions, n_thresholds;
+  float thresholds[kMaxThresholds];     // strictly ascending, finite
+};
+
+// The dynamic shared memory region_sweep_tile_kernel keeps before its windows, in floats: two histograms of a word
+// (double-buffered across words), T bins per slot
+__host__ __device__ __forceinline__ int sweep_smem_floats(int n_regions, int n_thresholds) {
+  return 2 * (n_regions + 1) * n_thresholds;
+}
+
+// grid: (tiles of kSegTileH x kSegTileW output pixels, n_maps); dynamic smem: sweep_smem_floats, then words_per_pass
+// source windows
+__global__ void __launch_bounds__(256) region_sweep_tile_kernel(const __grid_constant__ SweepParams S) {
+  extern __shared__ __align__(16) float smem[];
+  __shared__ float s_lo[kMaxWords], s_hi[kMaxWords];
+  __shared__ float s_tau[kMaxThresholds];
+  __shared__ unsigned lanes[8][kSegPix][kRegionSlots];   // per warp and pixel row: the lanes inside each slot
+  __shared__ TapTables taps;
+  const WordListParams& P = S.s;
+  const int map = blockIdx.y, mh = P.mh, mw = P.mw, n_words = P.n_words, n_thr = S.n_thresholds;
+  const Tile T = block_tile(P);
+  const int n_pix = T.th * T.tw;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int n_slots = S.n_regions + 1, n_bins = n_slots * n_thr;
+  unsigned* hist = reinterpret_cast<unsigned*>(smem);                       // [2][n_slots][T]
+  float* win = smem + sweep_smem_floats(S.n_regions, n_thr);
+  for (int w = threadIdx.x; w < n_words; w += blockDim.x) word_bounds(P, map, w, s_lo[w], s_hi[w]);
+  for (int i = threadIdx.x; i < n_thr; i += blockDim.x) s_tau[i] = S.thresholds[i];
+  for (int i = threadIdx.x; i < 2 * n_bins; i += blockDim.x) hist[i] = 0u;
+  fill_tap_tables(P, T, taps);
+  // the tile's slot masks as lane masks, and which slots each pixel row of the warp touches at all
+  unsigned present[2][kSegPix];
+  {
+    unsigned mask[2][kSegPix];
+    region_slot_masks(S.regions, S.n_regions, P.oh, P.ow, T, mask);
+#pragma unroll
+    for (int k = 0; k < kSegPix; ++k) {
+#pragma unroll
+      for (int g = 0; g < 2; ++g) {
+        present[g][k] = __reduce_or_sync(0xffffffffu, mask[g][k]);
+        for (int j = 0; j < 32 && 32 * g + j < n_slots; ++j) {
+          const unsigned in = __ballot_sync(0xffffffffu, (mask[g][k] >> j) & 1u);
+          if (lane == j) lanes[warp][k][32 * g + j] = in;
+        }
+      }
+    }
+  }
+  __syncthreads();                                     // histograms zeroed, tap tables and lane masks visible
+  const float* word_maps = P.word_maps + (long long)map * n_words * mh * mw;
+  unsigned* counts = S.counts + (long long)map * n_words * n_bins;
+  const bool staged = P.words_per_pass > 0;
+  const int per_pass = staged ? P.words_per_pass : n_words;
+  for (int w0 = 0; w0 < n_words; w0 += per_pass) {
+    const int nw = min(per_pass, n_words - w0);
+    if (staged) stage_windows(P, T, word_maps, w0, nw, win);
+    for (int wi = 0; wi < nw; ++wi) {
+      const int w = w0 + wi;
+      unsigned* h = hist + (w & 1) * n_bins;
+#pragma unroll
+      for (int k = 0; k < kSegPix; ++k) {
+        const int p = threadIdx.x + 256 * k;
+        int b = 0;
+        if (p < n_pix) {
+          const int py = p / T.tw;
+          Taps ty, tx;
+          tile_taps(taps, py, p - py * T.tw, ty, tx);
+          float v;
+          if (staged) {
+            v = bicubic_shared(win + wi * T.wn, T.ww, ty, tx);
+          } else {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) { ty.idx[j] += T.wy; tx.idx[j] += T.wx; }
+            v = bicubic_at(word_maps + (long long)w * mh * mw, mw, ty, tx);
+          }
+          const float m = word_value(P, v, s_lo[w], s_hi[w]);
+          // b = #{k : m > tau[k]}: the passing thresholds are a prefix of the ascending list
+#pragma unroll
+          for (int step = kMaxThresholds; step > 0; step >>= 1)
+            if (b + step <= n_thr && m > s_tau[b + step - 1]) b += step;
+        }
+        const unsigned counted = __ballot_sync(0xffffffffu, b > 0);
+        if (b > 0) {
+          const unsigned peers = __match_any_sync(counted, b);
+          if (lane == __ffs(peers) - 1) {
+            unsigned* bin = h + b - 1;
+#pragma unroll
+            for (int g = 0; g < 2; ++g) {
+              for (unsigned bits = present[g][k]; bits; bits &= bits - 1) {
+                const int slot = 32 * g + __ffs(bits) - 1;
+                const unsigned c = __popc(peers & lanes[warp][k][slot]);
+                if (c) atomicAdd(bin + slot * n_thr, c);
+              }
+            }
+          }
+        }
+      }
+      // one barrier per word: hist[w & 1] is counted into again two words later, after every thread has passed the
+      // next barrier, so it is flushed and zeroed by then
+      __syncthreads();
+      for (int i = threadIdx.x; i < n_bins; i += blockDim.x) {
+        const unsigned c = h[i];
+        if (c) { atomicAdd(counts + (long long)w * n_bins + i, c); h[i] = 0u; }
+      }
+    }
+  }
+}
+
+// grid: ceil(n_out / 256), 256 threads; thread o = (map * n_words + word) * (n_regions + 1) + slot turns its histogram
+// into the counts at every threshold (suffix sums, exact integers)
+__global__ void __launch_bounds__(256) region_sweep_reduce_kernel(const unsigned* __restrict__ counts, long long n_out,
+                                                                  int n_thresholds, int n_words, int n_regions,
+                                                                  float* __restrict__ intersection,
+                                                                  float* __restrict__ area) {
+  const long long o = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= n_out) return;
+  const int n_slots = n_regions + 1, slot = (int)(o % n_slots);
+  const long long mword = o / n_slots, map = mword / n_words, word = mword - map * n_words;
+  const unsigned* hist = counts + o * n_thresholds;
+  // threshold k of (map, word, slot): area[map][k][word] or intersection[map][k][slot - 1][word]
+  const long long stride = slot == 0 ? n_words : (long long)n_regions * n_words;
+  float* dst = slot == 0 ? area + map * n_thresholds * n_words + word
+                         : intersection + (map * n_thresholds * n_regions + slot - 1) * n_words + word;
+  unsigned s = 0;
+  for (int k = n_thresholds - 1; k >= 0; --k) {
+    s += __ldg(hist + k);
+    dst[k * stride] = (float)s;
   }
 }
 
@@ -1042,7 +1196,8 @@ static int launch_tiles(void (*kernel)(Params), Params& k, int n_maps, const Dev
   std::call_once(attr_once[dev.device & 63], [&] {
     const void* kernels[] = {(const void*)segment_minmax_kernel, (const void*)segment_label_kernel,
                              (const void*)region_tile_kernel, (const void*)overlay_kernel,
-                             (const void*)word_pair_tile_kernel, (const void*)instance_mask_kernel};
+                             (const void*)word_pair_tile_kernel, (const void*)instance_mask_kernel,
+                             (const void*)region_sweep_tile_kernel};
     for (const void* f : kernels)
       if (attr_err == cudaSuccess) attr_err = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
   });
@@ -1093,6 +1248,43 @@ extern "C" int daam_region_overlap(const float* global_maps, int32_t n_maps, int
   const long long n_out = (long long)n_maps * n_words * (n_regions + 1);
   region_reduce_kernel<<<(unsigned)((n_out + 7) / 8), 256, 0, stream>>>(p.partials, n_out, p.tiles, n_words, n_regions,
                                                                         intersection, word_area);
+  DAAM_CUDA_TRY(cudaGetLastError());
+  count_launch();
+  return DAAM_OK;
+}
+
+extern "C" int daam_region_sweep(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t mh, int32_t mw,
+                                 const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h,
+                                 int32_t out_w, int32_t absolute, const float* thresholds, int32_t n_thresholds,
+                                 float* word_maps, const uint8_t* regions, int32_t n_regions, float* intersection,
+                                 float* word_area, float* scratch, void* stream_) {
+  const char* name = "daam_region_sweep";
+  if (!global_maps || !rows || !row_begin || !thresholds || !word_maps || !regions || !intersection || !word_area ||
+      !scratch || n_maps <= 0 || mh <= 0 || mw <= 0 || out_h <= 0 || out_w <= 0 || n_rows <= 0 || n_regions <= 0 ||
+      n_thresholds <= 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
+  if (n_thresholds > kMaxThresholds) { set_error("%s: %d thresholds > %d", name, n_thresholds, kMaxThresholds); return DAAM_E_UNSUPPORTED; }
+  if (n_regions > kMaxRegions) { set_error("%s: %d regions > %d", name, n_regions, kMaxRegions); return DAAM_E_UNSUPPORTED; }
+  // the counts are exact in fp32 up to 2^24
+  if ((long long)out_h * out_w > (1LL << 24)) { set_error("%s: a %d x %d output is more than 2^24 pixels", name, out_h, out_w); return DAAM_E_UNSUPPORTED; }
+  for (int k = 0; k < n_thresholds; ++k) {
+    if (!isfinite(thresholds[k])) { set_error("%s: threshold %d is not finite", name, k); return DAAM_E_INVALID; }
+    if (k > 0 && !(thresholds[k] > thresholds[k - 1])) { set_error("%s: thresholds %d and %d are not strictly ascending", name, k - 1, k); return DAAM_E_INVALID; }
+  }
+  static thread_local SweepParams p;
+  DeviceInfo dev;
+  if (int rc = word_list_prepare(name, global_maps, n_maps, n_rows, mh, mw, rows, row_begin, n_words, out_h, out_w,
+                                 absolute, !absolute, 0, 0.f, word_maps, scratch, true, p.s, &dev)) return rc;
+  p.regions = regions; p.n_regions = n_regions; p.n_thresholds = n_thresholds;
+  for (int k = 0; k < n_thresholds; ++k) p.thresholds[k] = thresholds[k];
+  p.counts = reinterpret_cast<unsigned*>(scratch + 64LL * n_maps * n_words);   // after the min / max partials
+  const long long n_out = (long long)n_maps * n_words * (n_regions + 1);
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  DAAM_CUDA_TRY(cudaMemsetAsync(p.counts, 0, (size_t)n_out * n_thresholds * sizeof(unsigned), stream));
+  if (int rc = launch_tiles(region_sweep_tile_kernel, p, n_maps, dev, stream, 0,
+                            (size_t)sweep_smem_floats(n_regions, n_thresholds) * sizeof(float))) return rc;
+  region_sweep_reduce_kernel<<<(unsigned)((n_out + 255) / 256), 256, 0, stream>>>(p.counts, n_out, n_thresholds,
+                                                                                  n_words, n_regions, intersection,
+                                                                                  word_area);
   DAAM_CUDA_TRY(cudaGetLastError());
   count_launch();
   return DAAM_OK;

@@ -10,6 +10,9 @@ against several regions, or every step of a history, use :meth:`GlobalHeatMap.re
 <daam_b200.heatmap.GlobalHeatMap.region_overlap>` / :meth:`GlobalHeatMapStack.region_overlap
 <daam_b200.heatmap.GlobalHeatMapStack.region_overlap>`: three fused launches for every (map, region, word), whose
 ``iou()`` / ``ioa()`` equal ``compute_iou`` / ``compute_ioa`` of each thresholded mask and binary region bit for bit.
+To choose the threshold, or to draw IoU, precision and recall against it, use :meth:`GlobalHeatMap.region_sweep
+<daam_b200.heatmap.GlobalHeatMap.region_sweep>` / :meth:`GlobalHeatMapStack.region_sweep
+<daam_b200.heatmap.GlobalHeatMapStack.region_sweep>`: the same exact counts at up to 64 thresholds in one pass.
 To score every pair of words against each other (``WordHeatMap.compute_ioa``, the DAAM paper's head / dependent
 overlap), use :meth:`GlobalHeatMap.word_overlap <daam_b200.heatmap.GlobalHeatMap.word_overlap>` or, for the relations
 of a parse, :meth:`GlobalHeatMap.relation_overlap <daam_b200.heatmap.GlobalHeatMap.relation_overlap>`, on one map or a

@@ -15,6 +15,7 @@ The spaCy-parsed iterators and matplotlib overlays of the reference are out of s
 """
 from __future__ import annotations
 
+import numbers
 from dataclasses import dataclass
 from functools import lru_cache
 from types import SimpleNamespace
@@ -410,6 +411,29 @@ class GlobalHeatMap:
                                       absolute, threshold, word_idx, offset_idx, to_cpu, 'GlobalHeatMap.region_overlap')
         return wl.word_heat_maps(0), overlap.map(0)
 
+    def region_sweep(self, words, image, regions: torch.Tensor, thresholds, absolute: bool = False, word_idx=None,
+                     offset_idx: int = 0, to_cpu: bool = True):
+        """:meth:`region_overlap` at up to 64 thresholds in one pass: IoU, IoA, precision and recall as functions of the
+        binarisation threshold, for every (word, region) pair. With ``m`` the ``[len(words), H, W]`` that
+        ``expand_words(words, image, absolute, word_idx=word_idx, offset_idx=offset_idx)`` returns (no threshold) and
+        ``R[r] = regions[r] != 0``, the :class:`RegionOverlap` holds the pixel counts ``intersection[k, r, w] = (R[r] &
+        (m[w] > thresholds[k])).sum()`` and ``word_area[k, w] = (m[w] > thresholds[k]).sum()``, fp32 ``[T, R, W]`` and
+        ``[T, W]``, and ``region_area[r]``; ``iou()``, ``ioa()`` and ``region_mean()`` (recall) are ``[T, R, W]``. For
+        every nonzero threshold, slice ``k`` equals ``region_overlap(..., threshold=thresholds[k])`` bit for bit.
+        One memset and three fused launches whatever the number of thresholds; the ``[len(words), H, W]`` stack is
+        never materialised.
+
+        ``thresholds``: 1 to 64 numbers (a sequence, or a 1-D CPU tensor), rounded to fp32 and then strictly ascending
+        and finite, else a ``ValueError`` before anything reaches the device. Every entry is compared literally: unlike
+        ``region_overlap``'s ``threshold``, where 0 means "no threshold", a 0 here counts ``m > 0`` and a negative
+        value is a threshold too. Returns ``(word_heat_maps, overlap)`` as :meth:`region_overlap` does (CPU by default,
+        ``to_cpu=False`` keeps it on the device), with the same limits (96 words, 63 regions, 2**24 image pixels), and
+        an empty word list or region set launches nothing and measures no word (``[T, R, 0]``). Raises the reference's
+        ``ValueError`` for a word that is not in the prompt."""
+        wl, overlap = _region_sweep(self.tokenizer, self.prompt, self.heat_maps[None], words, image, regions,
+                                    thresholds, absolute, word_idx, offset_idx, to_cpu, 'GlobalHeatMap.region_sweep')
+        return wl.word_heat_maps(0), overlap.map(0)
+
     def word_overlap(self, words, image=None, absolute: bool = False, threshold: Optional[float] = None,
                      word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
         """How much each word's expanded map overlaps every other word's: the sums behind ``compute_iou`` /
@@ -574,7 +598,8 @@ def _segment(tokenizer, prompt: str, maps: torch.Tensor, words, image, absolute,
 class RegionOverlap:
     """Sums of word maps over image regions (:meth:`GlobalHeatMap.region_overlap`): ``intersection`` ``[..., R, W]``
     (``sum_p region[r](p) * m[w](p)``), ``word_area`` ``[..., W]`` (``sum_p m[w](p)``) and ``region_area`` ``[R]``
-    (pixels inside each region), fp32. ``...`` is the map axis of a :class:`GlobalHeatMapStack`, absent for one map.
+    (pixels inside each region), fp32. ``...`` is the map axis of a :class:`GlobalHeatMapStack`, absent for one map,
+    followed by the threshold axis of :meth:`GlobalHeatMap.region_sweep` (``[..., T, R, W]``, ``[..., T, W]``).
     The scores are the reference's formulas (``daam/evaluate.py``) in the same fp32 operation order."""
     intersection: torch.Tensor
     word_area: torch.Tensor
@@ -609,33 +634,97 @@ def _region_overlap(tokenizer, prompt: str, maps: torch.Tensor, words, image, re
     word list then holds no word and no word heat map."""
     wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, image, absolute, threshold, to_cpu, what)
     n_maps, out_h, out_w, dev = wl.n_maps, wl.out_h, wl.out_w, wl.dev
+    region_bytes = _region_bytes(wl, regions, what)
+    n_regions, n_words = region_bytes.shape[0], len(wl.words)
+    if wl.empty or n_regions == 0:            # no word is measured: the call returns no word heat maps
+        return wl.done(_no_region_overlap(wl, (), n_regions))
+    inter = torch.empty((n_maps, n_regions, n_words), dtype=torch.float32, device=dev)
+    area = torch.empty((n_maps, n_words), dtype=torch.float32, device=dev)
+    scratch = wl.scratch(_native.region_scratch_floats(n_maps, n_words, n_regions, out_h, out_w))
+    wl.launch(_native.region_overlap, wl.word_maps.data_ptr(), region_bytes.data_ptr(), n_regions, inter.data_ptr(),
+              area.data_ptr(), scratch.data_ptr())
+    return wl.done(RegionOverlap(inter, area, _region_area(region_bytes)))
+
+
+def _region_bytes(wl: _WordList, regions, what: str) -> torch.Tensor:
+    """``regions`` checked against the word list's output size and device, as uint8 ``[R, H, W]`` on the device: a
+    ``[H, W]`` region is one region."""
     if not isinstance(regions, torch.Tensor):
         raise TypeError(f'{what}: regions must be a torch.Tensor, not {type(regions).__name__}')
     if regions.dtype not in (torch.bool, torch.uint8):
         raise TypeError(f'{what}: regions must be bool or uint8, not {regions.dtype}')
     if regions.dim() == 2:
         regions = regions[None]
+    out_h, out_w = wl.out_h, wl.out_w
     if regions.dim() != 3 or tuple(regions.shape[1:]) != (out_h, out_w):
         raise ValueError(f'{what}: regions of shape {tuple(regions.shape)} do not match the expanded maps\' '
                          f'(R, {out_h}, {out_w}) (a [{out_h}, {out_w}] region or a stack of them)')
     _require_cuda(regions, what)
-    if regions.device != dev:
-        raise ValueError(f'{what}: regions are on {regions.device}, the heat maps on {dev}')
-    n_regions, n_words = regions.shape[0], len(wl.words)
-    if wl.empty or n_regions == 0:            # no word is measured: the call returns no word heat maps
-        wl.words, wl.merged = [], []
-        wl.word_maps = torch.empty((n_maps, 0) + wl.grid, dtype=torch.float32, device=dev)
-        return wl.done(RegionOverlap(torch.zeros((n_maps, n_regions, 0), device=dev),
-                                     torch.zeros((n_maps, 0), device=dev), torch.zeros((n_regions,), device=dev)))
-    region_bytes = regions.detach().contiguous().view(torch.uint8)
-    inter = torch.empty((n_maps, n_regions, n_words), dtype=torch.float32, device=dev)
-    area = torch.empty((n_maps, n_words), dtype=torch.float32, device=dev)
-    scratch = wl.scratch(_native.region_scratch_floats(n_maps, n_words, n_regions, out_h, out_w))
-    wl.launch(_native.region_overlap, wl.word_maps.data_ptr(), region_bytes.data_ptr(), n_regions, inter.data_ptr(),
+    if regions.device != wl.dev:
+        raise ValueError(f'{what}: regions are on {regions.device}, the heat maps on {wl.dev}')
+    return regions.detach().contiguous().view(torch.uint8)
+
+
+def _region_area(region_bytes: torch.Tensor) -> torch.Tensor:
+    """Exact pixel counts (at most 2**24 pixels): what ``region.float().sum()`` gives in compute_iou."""
+    return (region_bytes != 0).sum((-1, -2)).float()
+
+
+def _no_region_overlap(wl: _WordList, lead: Tuple[int, ...], n_regions: int) -> RegionOverlap:
+    """The overlap of a call that measures no word: the word list then holds no word and no word heat map, and the
+    sums have a word axis of length 0 after the map axis and ``lead``."""
+    n_maps, dev = wl.n_maps, wl.dev
+    wl.words, wl.merged = [], []
+    wl.word_maps = torch.empty((n_maps, 0) + wl.grid, dtype=torch.float32, device=dev)
+    return RegionOverlap(torch.zeros((n_maps, *lead, n_regions, 0), device=dev),
+                         torch.zeros((n_maps, *lead, 0), device=dev), torch.zeros((n_regions,), device=dev))
+
+
+def _sweep_thresholds(thresholds, what: str) -> List[float]:
+    """``thresholds`` (a sequence of numbers or a 1-D CPU tensor) rounded to fp32, as the Python floats of those fp32
+    values; a ``ValueError`` unless they are 1 to 64 finite, strictly ascending values after the rounding."""
+    if isinstance(thresholds, torch.Tensor):
+        if thresholds.device.type != 'cpu' or thresholds.dim() != 1 or thresholds.dtype == torch.bool \
+                or thresholds.is_complex():
+            raise ValueError(f'{what}: thresholds must be a 1-D real CPU tensor, not {thresholds.dim()}-D '
+                             f'{thresholds.dtype} on {thresholds.device}')
+        taus = thresholds.detach().to(torch.float32)
+    else:
+        try:
+            values = list(thresholds)
+        except TypeError:
+            raise ValueError(f'{what}: thresholds must be a sequence of numbers, not {thresholds!r}') from None
+        if not all(isinstance(x, numbers.Real) and not isinstance(x, bool) for x in values):
+            raise ValueError(f'{what}: thresholds must be numbers, not {values!r}')
+        taus = torch.tensor([float(x) for x in values], dtype=torch.float64).to(torch.float32)
+    n = taus.numel()
+    if not 1 <= n <= _native.SWEEP_MAX_THRESHOLDS:
+        raise ValueError(f'{what}: {n} thresholds; a sweep takes 1 to {_native.SWEEP_MAX_THRESHOLDS}')
+    if not bool(torch.isfinite(taus).all()):
+        raise ValueError(f'{what}: thresholds must be finite in fp32, not {taus.tolist()}')
+    if not bool((taus[1:] > taus[:-1]).all()):
+        raise ValueError(f'{what}: thresholds must be strictly ascending after rounding to fp32, not {taus.tolist()}')
+    return taus.tolist()
+
+
+def _region_sweep(tokenizer, prompt: str, maps: torch.Tensor, words, image, regions, thresholds, absolute, word_idx,
+                  offset_idx: int, to_cpu: bool, what: str):
+    """``daam_region_sweep`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(wl, overlap)``, the
+    :class:`_WordList` and the :class:`RegionOverlap` with a leading map axis and a threshold axis before the region
+    axis. The thresholds are checked first, then everything ``_region_overlap`` checks, in its order."""
+    taus = _sweep_thresholds(thresholds, what)
+    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, image, absolute, taus, to_cpu, what)
+    n_maps, out_h, out_w, dev = wl.n_maps, wl.out_h, wl.out_w, wl.dev
+    region_bytes = _region_bytes(wl, regions, what)
+    n_regions, n_words, n_thr = region_bytes.shape[0], len(wl.words), len(taus)
+    if wl.empty or n_regions == 0:
+        return wl.done(_no_region_overlap(wl, (n_thr,), n_regions))
+    inter = torch.empty((n_maps, n_thr, n_regions, n_words), dtype=torch.float32, device=dev)
+    area = torch.empty((n_maps, n_thr, n_words), dtype=torch.float32, device=dev)
+    scratch = wl.scratch(_native.region_sweep_scratch_floats(n_maps, n_words, n_regions, n_thr, out_h, out_w))
+    wl.launch(_native.region_sweep, wl.word_maps.data_ptr(), region_bytes.data_ptr(), n_regions, inter.data_ptr(),
               area.data_ptr(), scratch.data_ptr())
-    # exact pixel counts (at most 2**24 pixels): what ``region.float().sum()`` gives in compute_iou
-    region_area = (region_bytes != 0).sum((-1, -2)).float()
-    return wl.done(RegionOverlap(inter, area, region_area))
+    return wl.done(RegionOverlap(inter, area, _region_area(region_bytes)))
 
 
 @dataclass
@@ -931,6 +1020,18 @@ class GlobalHeatMapStack:
         and word). E.g. ``overlap.iou()[:, 0, 0]`` is word 0's IoU with region 0 at every step of a history."""
         wl, overlap = _region_overlap(self.tokenizer, self.prompt, self.heat_maps, words, image, regions, absolute,
                                       threshold, word_idx, offset_idx, to_cpu, f'{type(self).__name__}.region_overlap')
+        return wl.word_maps, overlap
+
+    def region_sweep(self, words, image, regions: torch.Tensor, thresholds, absolute: bool = False, word_idx=None,
+                     offset_idx: int = 0, to_cpu: bool = True):
+        """:meth:`GlobalHeatMap.region_sweep` for every map in one call (a memset and three launches whatever the map
+        and threshold counts): returns ``(word_maps, overlap)`` with ``word_maps`` the device ``[maps, len(words), xh, xw]`` word heat
+        maps and ``overlap`` a :class:`RegionOverlap` with a leading map axis (``intersection`` ``[maps, T, R, W]``,
+        ``word_area`` ``[maps, T, W]``); row ``t`` equals ``self[t].region_sweep(...)`` bit for bit (min / max
+        normalisation per map and word). E.g. ``overlap.iou()[:, :, 0, 0]`` is word 0's IoU with region 0 at every
+        step and threshold."""
+        wl, overlap = _region_sweep(self.tokenizer, self.prompt, self.heat_maps, words, image, regions, thresholds,
+                                    absolute, word_idx, offset_idx, to_cpu, f'{type(self).__name__}.region_sweep')
         return wl.word_maps, overlap
 
     def word_overlap(self, words, image=None, absolute: bool = False, threshold: Optional[float] = None,

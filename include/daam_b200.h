@@ -35,7 +35,7 @@ extern "C" {
                                           several prompts and a prompt stride <= 0 take the SIMT kernel;
                                           daam_region_overlap; daam_overlay_words, daam_jet_colormap;
                                           daam_finalize_parts; daam_word_overlap;
-                                          daam_word_instances) */
+                                          daam_word_instances; daam_region_sweep) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_TOKENS 231     /* daam_accumulate: long contexts of 2 or 3 CLIP chunks of 77 tokens (154, 231) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
@@ -358,6 +358,34 @@ int daam_region_overlap(const float* global_maps, int32_t n_maps, int32_t n_rows
                         int32_t absolute, int32_t use_threshold, float threshold, float* word_maps,
                         const uint8_t* regions, int32_t n_regions, float* intersection, float* word_area, float* scratch,
                         void* stream);
+
+/*
+ * Threshold sweep of word-region overlap: daam_region_overlap's pixel counts at n_thresholds thresholds in one pass --
+ * IoU, precision and recall of the reference's evaluation (daam/evaluate.py) as functions of the binarisation
+ * threshold. With m[w] what daam_expand_words writes for word w WITHOUT threshold (same rows / row_begin / absolute)
+ * and R[r](p) = (regions[r][p] != 0), for every map i and threshold k:
+ *   intersection[i][k][r][w] = #{p : R[r](p) and m[w](p) > thresholds[k]}    (fp32 [n_maps][n_thresholds][n_regions][n_words])
+ *   word_area[i][k][w]       = #{p : m[w](p) > thresholds[k]}                 (fp32 [n_maps][n_thresholds][n_words])
+ * compared in fp32 with the very m daam_expand_words thresholds, so for every nonzero thresholds[k] slice k equals what
+ * daam_region_overlap(..., use_threshold = 1, threshold = thresholds[k]) writes, bit for bit. Every entry is a real
+ * threshold: 0 and negative values count m > 0 and m > t (there is no "0 means none"). Arguments as
+ * daam_region_overlap, with use_threshold / threshold replaced by thresholds: host fp32 [n_thresholds], finite and
+ * strictly ascending. scratch: device, >= DAAM_REGION_SWEEP_SCRATCH_FLOATS(...) floats: the 64 min / max floats per
+ * (map, word), then a (n_regions + 1) x n_thresholds histogram per (map, word); it does not grow with the image.
+ * One memset and three launches whatever n_thresholds, n_maps, n_words and n_regions; the [n_words][out_h][out_w]
+ * stack is never written. Every count is an integer sum, so repeated calls give the same bits.
+ * Limits (DAAM_E_UNSUPPORTED): those of daam_region_overlap, and n_thresholds <= 64
+ * (DAAM_REGION_SWEEP_MAX_THRESHOLDS). DAAM_E_INVALID: as daam_region_overlap, plus n_thresholds <= 0, null thresholds,
+ * a threshold that is not finite, thresholds not strictly ascending.
+ */
+#define DAAM_REGION_SWEEP_MAX_THRESHOLDS 64
+#define DAAM_REGION_SWEEP_SCRATCH_FLOATS(n_maps, n_words, n_regions, n_thresholds, out_h, out_w)                     \
+  ((int64_t)(n_maps) * (n_words) * (64 + ((int64_t)(n_regions) + 1) * (n_thresholds)))
+int daam_region_sweep(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t map_h, int32_t map_w,
+                      const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w,
+                      int32_t absolute, const float* thresholds, int32_t n_thresholds, float* word_maps,
+                      const uint8_t* regions, int32_t n_regions, float* intersection, float* word_area,
+                      float* scratch, void* stream);
 
 /*
  * Word-pair overlap: how much each word's expanded map overlaps every other word's, on each of n_maps global maps
