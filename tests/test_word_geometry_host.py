@@ -6,14 +6,18 @@
   contraction) against ``math_bicubic_matrix``: the coordinate term row by row on a grid of ratios, the whole bound on
   the ratios of the GPU table.
 * ``launch_tiles``'s window estimate is never smaller than a tile's actual window.
+* Beside the pair and sweep kernels' own shared buffers, the staged windows stay within 200 KB and none is staged
+  exactly when none fits, over every word, region and threshold count the C ABI accepts; the word-instance rounds take
+  every plane once.
 * The regimes that cannot occur, with the reason."""
 import numpy as np
 import pytest
 import torch
 
 from oracle import daam_oracle as O
-from tests.test_word_geometry_gpu import (CASE_NAMES, CASES, MAX_CHUNKS, REQUIRED, TILE_H, TILE_W, Case, case_regimes,
-                                          expand_per_sm, plan)
+from tests.test_word_geometry_gpu import (CASE_NAMES, CASES, MAX_CHUNKS, MAX_ROUND_PLANES, MAX_SMEM, REQUIRED, TILE_H,
+                                          TILE_W, Case, case_regimes, expand_per_sm, instance_rounds, pair_smem_bytes,
+                                          plan, sweep_smem_bytes, words_per_pass)
 from tests.words64 import expand64, expand_bound, row_motion, word_maps64
 
 SMS = (132, 114, 78)
@@ -201,11 +205,83 @@ def test_window_estimate_covers_every_tile():
 
 # ---- regimes that cannot occur --------------------------------------------------------------------------------------------
 
+# ---- staging beside the pair and sweep buffers, and the instance rounds -----------------------------------------------
+
+WINDOWS = np.arange(1, MAX_SMEM // 4 + 1)          # every window a map of at most 200 KB can have, in floats
+
+
+def _check_staging(before: int, n_words, what: str):
+    assert before <= MAX_SMEM, f'{what}: {before} bytes before the windows'
+    for w in n_words:
+        wpp = words_per_pass(w, WINDOWS, before)
+        assert (before + wpp * WINDOWS * 4 <= MAX_SMEM).all(), f'{what}, {w} words: more than 200 KB'
+        none = wpp == 0
+        assert np.array_equal(none, WINDOWS * 4 > MAX_SMEM - before), \
+            f'{what}, {w} words: no window staged at window {WINDOWS[none != (WINDOWS * 4 > MAX_SMEM - before)][0]}'
+        assert (wpp >= 0).all() and (wpp <= w).all()
+
+
+def test_pair_staging_stays_within_200KB():
+    """For 1 to 96 words, with and without a threshold, and every window: ``pair_smem_bytes + words_per_pass * window
+    <= 200 KB``, and no window is staged exactly when one does not fit beside the pair buffers."""
+    for n_words in range(1, 97):
+        for thr in (False, True):
+            _check_staging(pair_smem_bytes(n_words, thr), [n_words], f'pair, threshold {thr}')
+
+
+def test_sweep_staging_stays_within_200KB():
+    """For R <= 63 regions, T <= 64 thresholds and every window, the same of ``sweep_smem_bytes``. The word count only
+    caps ``words_per_pass`` from above, so 1, 2, 95 and 96 words stand for every count."""
+    for before in sorted({sweep_smem_bytes(r, t) for r in range(1, 64) for t in range(1, 65)}):
+        _check_staging(before, (1, 2, 95, 96), f'sweep, {before} bytes of histograms')
+
+
+def test_the_table_reaches_the_staging_boundaries():
+    """The sweep rows of the table sit on both sides of the boundary: a 196 KB window beside 512 bins fits once,
+    beside 513 it does not."""
+    assert plan(CASES['sweep-one-window-fits'], 132)['fits'] == 1
+    assert plan(CASES['sweep-not-staged-513'], 132)['fits'] == 0
+    assert sweep_smem_bytes(7, 64) + 224 * 224 * 4 == MAX_SMEM
+
+
+ROUND_SHAPES = [(1, 1), (1, 5), (3, 5), (7, 2), (4, 96), (2, 33)]
+
+
+@pytest.mark.parametrize('n_maps,n_words', ROUND_SHAPES, ids=[f'{m}x{w}' for m, w in ROUND_SHAPES])
+def test_instance_rounds_split_the_planes(n_maps, n_words):
+    """For every scratch size from one plane to all of them and past: each (map, word) plane is in exactly one round,
+    no round has more than ``cap`` planes (nor 65535), and a round takes several maps only when every round takes
+    whole maps."""
+    planes = n_maps * n_words
+    for cap in list(range(1, planes + 3)) + [MAX_ROUND_PLANES]:
+        rounds = instance_rounds(n_maps, n_words, cap)
+        seen = np.zeros((n_maps, n_words), np.int64)
+        for m0, nm, w0, nw in rounds:
+            assert 1 <= nm * nw <= min(cap, MAX_ROUND_PLANES), (cap, m0, w0)
+            seen[m0:m0 + nm, w0:w0 + nw] += 1
+        assert (seen == 1).all(), cap
+        if any(nm > 1 for _, nm, _, _ in rounds):
+            assert all(nw == n_words for _, _, _, nw in rounds), cap
+
+
+def test_instance_rounds_at_the_plane_limit():
+    """65535 maps of 96 words with room for every plane: 65535-plane rounds of 682 whole maps."""
+    rounds = instance_rounds(65535, 96, MAX_ROUND_PLANES)
+    assert all(nw == 96 and nm * nw <= MAX_ROUND_PLANES for _, nm, _, nw in rounds)
+    assert sum(nm for _, nm, _, _ in rounds) == 65535 and rounds[0][1] == 682
+
+
 def test_unreachable_regimes():
     """* Several ``expand_words`` launches need more words than ``capacity = per_sm * sm_count >= sm_count``; a call
       has at most 96 words, so they need fewer than 96 SMs, and every H100 has 114 or 132.
     * An empty expand chunk (``begin = chunk * per >= n``) needs ``(chunks - 1) * ceil(n / chunks) >= n``, which
-      ``chunks <= ceil(n / 256)`` rules out: ``chunks * (chunks - 1) >= n`` would be needed, and ``chunks <= 32``."""
+      ``chunks <= ceil(n / 256)`` rules out: ``chunks * (chunks - 1) >= n`` would be needed, and ``chunks <= 32``.
+    * A round of several word-instance maps whose words are split: ``maps_per_round = max(1, cap // n_words) > 1``
+      needs ``cap >= 2 n_words``, and then ``words_per_round = min(cap, n_words)`` is every word."""
+    for n_words in range(1, 97):
+        for cap in range(1, 3 * n_words):
+            if max(1, cap // n_words) > 1:
+                assert min(cap, n_words) == n_words
     for sm in (114, 132):
         for n_words in range(1, 97):
             for mh, mw in ((1, 1), (64, 64), (320, 160)):

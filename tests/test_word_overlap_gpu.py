@@ -13,7 +13,6 @@ relation_overlap, daam_word_overlap) on the GPU.
 * Stacks from the synthetic pipeline: time-resolved, per-image, per-layer and a compact long-prompt map, row t equal to
   the per-map call. Relations: str and int endpoints, skipped words, and the notebook's per-edge loop.
 """
-import math
 from types import SimpleNamespace
 
 import pytest
@@ -23,6 +22,7 @@ from daam_b200 import _native, trace
 from daam_b200.evaluate import compute_ioa, compute_iou
 from daam_b200.heatmap import GlobalHeatMap
 from daam_b200.testing.synthetic import TINY_SPEC, UNetSpec, WhitespaceTokenizer, make_pipeline
+from tests.test_word_geometry_gpu import Case, plan
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
@@ -201,14 +201,11 @@ def test_explicit_word_idx():
 
 
 def pair_words_per_pass(grid, out, n_words, threshold):
-    """The words_per_pass launch_tiles gives word_pair_tile_kernel (words.cu): as many of the tile's source windows (16 x
-    64 output pixels, at most ceil(tile * map / out) + 5 rows / columns of the map) as fit in 200 KB after the pair
+    """The words_per_pass launch_tiles gives word_pair_tile_kernel (words.cu), as ``plan`` of
+    tests/test_word_geometry_gpu.py states it: as many of the tile's source windows as fit in 200 KB after the pair
     table, slots and masks / values. 0: no window fits."""
-    (mh, mw), (oh, ow) = grid, out
-    win = min(mh, math.ceil(16 * mh / oh) + 5) * min(mw, math.ceil(64 * mw / ow) + 5)
-    pairs = n_words * (n_words + 1) // 2
-    before = 4 * ((pairs + 1) // 2 + pairs + n_words + n_words * (33 if threshold else 256))
-    return min(n_words, (200 * 1024 - before) // (win * 4))
+    case = Case('pair', grid, out, n_words=n_words, thresholds=(threshold,))
+    return plan(case, _native.device_info()['sm_count'])['by_t'][threshold]['words_per_pass']
 
 
 # a square map whose tile window is the whole map (224 x 224 floats, 196 KB) over a 16 x 65 output (two tiles: the
