@@ -66,6 +66,18 @@ def word_instances_plane_bytes(out_h: int, out_w: int) -> int:
     return 8 * out_h * out_w + 48 * ((out_h + 1) // 2) * ((out_w + 1) // 2) + 260
 
 
+def region_ranking_plane_bytes(out_h: int, out_w: int) -> int:
+    """``DAAM_REGION_RANKING_PLANE_BYTES(out_h, out_w)``: the scratch bytes daam_region_ranking takes per (map, word)
+    plane of a round."""
+    n = out_h * out_w
+    return 16 * n + 1024 * ((n + 4095) // 4096) + 1540 * ((n + 1023) // 1024) + 512
+
+
+def region_ranking_scratch_bytes(n_planes: int, out_h: int, out_w: int) -> int:
+    """``DAAM_REGION_RANKING_SCRATCH_BYTES(n_planes, out_h, out_w)``: the call's region masks and ``n_planes`` planes."""
+    return 8 * out_h * out_w + n_planes * region_ranking_plane_bytes(out_h, out_w)
+
+
 def overlay_frames_bytes(n_maps: int, n_words: int, out_h: int, out_w: int) -> int:
     """``DAAM_OVERLAY_FRAMES_BYTES(n_maps, n_words, out_h, out_w)``: the frames rounded up to whole 4-byte words."""
     return (n_maps * n_words * out_h * out_w * 3 + 3) // 4 * 4
@@ -73,7 +85,7 @@ def overlay_frames_bytes(n_maps: int, n_words: int, out_h: int, out_w: int) -> i
 
 EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize',
            'daam_finalize_maps', 'daam_finalize_parts', 'daam_finalize_per_key','daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
-           'daam_segment_words', 'daam_region_overlap', 'daam_region_sweep', 'daam_word_overlap', 'daam_word_instances', 'daam_overlay_words', 'daam_jet_colormap',
+           'daam_segment_words', 'daam_region_overlap', 'daam_region_sweep', 'daam_region_ranking', 'daam_word_overlap', 'daam_word_instances', 'daam_overlay_words', 'daam_jet_colormap',
            'daam_side_launcher_create', 'daam_side_launcher_destroy',
            'daam_side_launcher_launch', 'daam_side_launcher_join', 'daam_side_launcher_idle', 'daam_abi_version',
            'daam_last_error', 'daam_device_info', 'daam_launch_count')
@@ -183,6 +195,9 @@ def load() -> ctypes.CDLL:
     lib.daam_region_sweep.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
                                       i32, ctypes.POINTER(f32), i32, vp, vp, i32, vp, vp, vp, vp]
     lib.daam_region_sweep.restype = ctypes.c_int
+    lib.daam_region_ranking.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32,
+                                        i32, i32, vp, vp, i32, vp, vp, vp, i64, vp]
+    lib.daam_region_ranking.restype = ctypes.c_int
     lib.daam_word_overlap.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
                                       i32, i32, f32, vp, vp, vp, vp, vp]
     lib.daam_word_overlap.restype = ctypes.c_int
@@ -458,6 +473,20 @@ def region_sweep(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequ
                                     taus, len(thresholds), ctypes.c_void_p(word_maps_ptr), ctypes.c_void_p(regions_ptr),
                                     n_regions, ctypes.c_void_p(intersection_ptr), ctypes.c_void_p(word_area_ptr),
                                     ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
+
+
+def region_ranking(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int,
+                   out_w: int, absolute: bool, threshold: Optional[float], word_maps_ptr: int, regions_ptr: int,
+                   n_regions: int, u2_ptr: int, ap_ptr: int, scratch_ptr: int, scratch_bytes: int, stream: int):
+    """``daam_region_ranking`` over ``n_maps`` maps ``[n_rows, h, w]`` back to back and ``n_regions`` uint8 regions
+    ``[out_h, out_w]``: ``u2`` int64 and ``ap`` float64 ``[n_maps, n_regions, n_words]``; ``scratch_bytes`` of scratch,
+    at least :func:`region_ranking_scratch_bytes` of one plane. The values are taken without threshold: the call takes
+    no ``use_threshold`` (``threshold`` is ignored)."""
+    vp = ctypes.c_void_p
+    _check(load().daam_region_ranking(vp(maps_ptr), n_maps, n_rows,
+                                      *_word_list(x, rows_per_word, out_h, out_w, absolute, None)[:-2],
+                                      vp(word_maps_ptr), vp(regions_ptr), n_regions, vp(u2_ptr), vp(ap_ptr),
+                                      vp(scratch_ptr), scratch_bytes, vp(stream)))
 
 
 def word_overlap(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int,

@@ -16,7 +16,8 @@
 //    region_sweep_reduce_kernel);
 //  - overlay_kernel blends its jet colour onto the image;
 //  - word_pair_tile_kernel sums m[a] * m[b] over every pair of words (then word_pair_reduce_kernel);
-//  - instance_mask_kernel writes it without threshold for components.cu, which labels the mask m > threshold.
+//  - instance_mask_kernel writes it without threshold for components.cu, which labels the mask m > threshold, and
+//    for ranking.cu, which sorts it and scores it against regions (daam_region_ranking).
 // The tile kernels run after segment_minmax_kernel (steps 1 and 2, the word maps and min / max partials to global
 // memory); region_tile_kernel, region_sweep_tile_kernel, overlay_kernel, word_pair_tile_kernel and instance_mask_kernel share the tile helpers
 // (block_tile / tile_at, word_bounds, stage_windows, tap tables). expand_words_kernel, segment_minmax_kernel and segment_label_kernel keep
@@ -32,6 +33,7 @@
 #include "bicubic.cuh"
 #include "common.cuh"
 #include "components.cuh"
+#include "ranking.cuh"
 
 namespace daam {
 namespace {
@@ -1387,6 +1389,50 @@ extern "C" int daam_word_instances(const float* global_maps, int32_t n_maps, int
       c.out_peak = peak + plane0 * max_instances;
       c.out_peak_yx = peak_yx + plane0 * max_instances * 2;
       if (int rc = launch_components(c, stream)) return rc;
+    }
+  }
+  return DAAM_OK;
+}
+
+extern "C" int daam_region_ranking(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t mh, int32_t mw,
+                                   const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h,
+                                   int32_t out_w, int32_t absolute, float* word_maps, const uint8_t* regions,
+                                   int32_t n_regions, int64_t* u2, double* ap, void* scratch, int64_t scratch_bytes,
+                                   void* stream_) {
+  const char* name = "daam_region_ranking";
+  if (!global_maps || !rows || !row_begin || !word_maps || !regions || !u2 || !ap || !scratch || n_maps <= 0 ||
+      mh <= 0 || mw <= 0 || out_h <= 0 || out_w <= 0 || n_rows <= 0 || n_regions <= 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
+  if (n_regions > kMaxRegions) { set_error("%s: %d regions > %d", name, n_regions, kMaxRegions); return DAAM_E_UNSUPPORTED; }
+  if ((long long)out_h * out_w > (1LL << 24)) { set_error("%s: a %d x %d output is more than 2^24 pixels", name, out_h, out_w); return DAAM_E_UNSUPPORTED; }
+  // the region masks once per call, then the planes of each round
+  const long long mask_bytes = 8LL * out_h * out_w, plane_bytes = ranking_plane_bytes(out_h, out_w);
+  if (scratch_bytes < mask_bytes + plane_bytes) { set_error("%s: %lld scratch bytes < %lld, the masks and one %d x %d plane", name, (long long)scratch_bytes, mask_bytes + plane_bytes, out_h, out_w); return DAAM_E_INVALID; }
+  static thread_local InstanceMaskParams p, q;
+  DeviceInfo dev;
+  if (int rc = word_list_prepare(name, global_maps, n_maps, n_rows, mh, mw, rows, row_begin, n_words, out_h, out_w,
+                                 absolute, !absolute, 0, 0.f, word_maps, nullptr, true, p.s, &dev)) return rc;
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (int rc = launch_region_masks(regions, n_regions, out_h, out_w, scratch, stream)) return rc;
+  // a round: whole maps while a map's planes fit the scratch, else the words of one map in groups
+  const int cap = (int)std::min<long long>((scratch_bytes - mask_bytes) / plane_bytes, 65535);
+  const int maps_per_round = std::max(1, cap / n_words), words_per_round = std::min(cap, (int)n_words);
+  for (int map0 = 0; map0 < n_maps; map0 += maps_per_round) {
+    const int nm = std::min(maps_per_round, n_maps - map0);
+    for (int w0 = 0; w0 < n_words; w0 += words_per_round) {
+      const int nw = std::min(words_per_round, n_words - w0);
+      q = p;
+      q.s.maps = global_maps + map0 * p.s.map_stride;
+      q.s.n_words = nw;
+      for (int i = 0; i <= nw; ++i) q.s.row_begin[i] = p.s.row_begin[w0 + i];
+      q.s.word_maps = word_maps + ((long long)map0 * n_words + w0) * mh * mw;
+      RankingPlanes c;
+      ranking_planes_in(scratch, nm * nw, out_h, out_w, c);
+      q.s.scratch = c.minmax;
+      q.pre = c.pre;
+      if (int rc = launch_tiles(instance_mask_kernel, q, nm, dev, stream)) return rc;
+      c.n_regions = n_regions; c.u2 = reinterpret_cast<long long*>(u2); c.ap = ap;
+      c.n_words_round = nw; c.n_words = n_words; c.map0 = map0; c.w0 = w0;
+      if (int rc = launch_ranking(c, stream)) return rc;
     }
   }
   return DAAM_OK;

@@ -13,6 +13,10 @@ against several regions, or every step of a history, use :meth:`GlobalHeatMap.re
 To choose the threshold, or to draw IoU, precision and recall against it, use :meth:`GlobalHeatMap.region_sweep
 <daam_b200.heatmap.GlobalHeatMap.region_sweep>` / :meth:`GlobalHeatMapStack.region_sweep
 <daam_b200.heatmap.GlobalHeatMapStack.region_sweep>`: the same exact counts at up to 64 thresholds in one pass.
+For scores that need no threshold at all -- the pixel ROC-AUC and average precision of each word's map against each
+region -- use :meth:`GlobalHeatMap.region_ranking <daam_b200.heatmap.GlobalHeatMap.region_ranking>` /
+:meth:`GlobalHeatMapStack.region_ranking <daam_b200.heatmap.GlobalHeatMapStack.region_ranking>`: every plane sorted on
+the device, exact ``u2`` counts and ``ap`` equal to ``roc_auc_score`` / ``average_precision_score``.
 To score every pair of words against each other (``WordHeatMap.compute_ioa``, the DAAM paper's head / dependent
 overlap), use :meth:`GlobalHeatMap.word_overlap <daam_b200.heatmap.GlobalHeatMap.word_overlap>` or, for the relations
 of a parse, :meth:`GlobalHeatMap.relation_overlap <daam_b200.heatmap.GlobalHeatMap.relation_overlap>`, on one map or a

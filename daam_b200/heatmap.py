@@ -27,7 +27,7 @@ from . import _native
 from .utils import compute_token_merge_indices
 
 __all__ = ['GlobalHeatMap', 'RawHeatMapCollection', 'WordHeatMap', 'LayerSlab', 'GlobalHeatMapStack', 'TimeHeatMaps',
-           'ImageHeatMaps', 'LayerHeatMaps', 'FactorHeatMaps', 'HeadHeatMaps', 'RegionOverlap', 'WordOverlap', 'RelationOverlap', 'WordInstances']
+           'ImageHeatMaps', 'LayerHeatMaps', 'FactorHeatMaps', 'HeadHeatMaps', 'RegionOverlap', 'RegionRanking', 'WordOverlap', 'RelationOverlap', 'WordInstances']
 
 RawHeatMapKey = Tuple[int, int, int]  # factor, layer, head
 
@@ -434,6 +434,27 @@ class GlobalHeatMap:
                                     thresholds, absolute, word_idx, offset_idx, to_cpu, 'GlobalHeatMap.region_sweep')
         return wl.word_heat_maps(0), overlap.map(0)
 
+    def region_ranking(self, words, image, regions: torch.Tensor, absolute: bool = False, word_idx=None,
+                       offset_idx: int = 0, to_cpu: bool = True):
+        """Threshold-free scores of each word's expanded map against each image region: pixel ROC-AUC and average
+        precision, exact, for every (word, region) pair at once. With ``m`` the ``[len(words), H, W]`` that
+        ``expand_words(words, image, absolute, word_idx=word_idx, offset_idx=offset_idx)`` returns (no threshold),
+        values compared as fp32 numbers, ``P`` the pixels where ``regions[r] != 0`` and ``N`` the others, the
+        :class:`RegionRanking` holds ``u2[r, w] = sum_{p in P, q in N} (2 [m_p > m_q] + [m_p == m_q])`` (int64, twice
+        the Mann-Whitney U with ties counted half), ``ap[r, w]`` (float64, sklearn's ``average_precision_score`` of
+        ``m[w]`` against the region: the area under the exact precision-recall curve, ties taken together) and
+        ``region_area[r]``; ``auroc()`` is ``roc_auc_score``. Every plane is sorted on the device; the ``[len(words), H,
+        W]`` stack never leaves it, and the results are the same bits on every call.
+
+        Returns ``(word_heat_maps, ranking)``: the list of :class:`WordHeatMap` that :meth:`segment` returns and the
+        :class:`RegionRanking` (CPU by default, ``to_cpu=False`` keeps it on the device). A ``[H, W]`` region is one
+        region. At most 96 words, 63 regions and 2**24 image pixels. An empty word list or region set launches nothing,
+        returns no word heat maps and scores no word (a word axis of length 0). Raises the reference's ``ValueError``
+        for a word that is not in the prompt."""
+        wl, ranking = _region_ranking(self.tokenizer, self.prompt, self.heat_maps[None], words, image, regions,
+                                      absolute, word_idx, offset_idx, to_cpu, 'GlobalHeatMap.region_ranking')
+        return wl.word_heat_maps(0), ranking.map(0)
+
     def word_overlap(self, words, image=None, absolute: bool = False, threshold: Optional[float] = None,
                      word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
         """How much each word's expanded map overlaps every other word's: the sums behind ``compute_iou`` /
@@ -725,6 +746,63 @@ def _region_sweep(tokenizer, prompt: str, maps: torch.Tensor, words, image, regi
     wl.launch(_native.region_sweep, wl.word_maps.data_ptr(), region_bytes.data_ptr(), n_regions, inter.data_ptr(),
               area.data_ptr(), scratch.data_ptr())
     return wl.done(RegionOverlap(inter, area, _region_area(region_bytes)))
+
+
+# Scratch of one region_ranking call: as many (map, word) planes as fit are sorted per round (about 18 bytes a pixel
+# each), so memory does not grow with the number of maps; a plane larger than the budget goes alone.
+REGION_RANKING_SCRATCH_BYTES = 256 << 20
+
+
+@dataclass
+class RegionRanking:
+    """Threshold-free scores of word maps against image regions (:meth:`GlobalHeatMap.region_ranking`): ``u2`` int64
+    ``[..., R, W]`` (twice the Mann-Whitney U of the word's values inside the region against those outside, ties
+    counted half), ``ap`` float64 ``[..., R, W]`` (average precision; NaN for an empty region), ``region_area`` int64
+    ``[R]`` (pixels inside each region) and ``n_pixels`` (pixels of the image). ``...`` is the map axis of a
+    :class:`GlobalHeatMapStack`, absent for one map."""
+    u2: torch.Tensor
+    ap: torch.Tensor
+    region_area: torch.Tensor
+    n_pixels: int
+
+    def map(self, i: int) -> 'RegionRanking':
+        """The scores of map ``i`` of a stack (``region_area`` has no map axis and stays whole)."""
+        return RegionRanking(self.u2[i], self.ap[i], self.region_area, self.n_pixels)
+
+    def cpu(self) -> 'RegionRanking':
+        return RegionRanking(self.u2.cpu(), self.ap.cpu(), self.region_area.cpu(), self.n_pixels)
+
+    def auroc(self) -> torch.Tensor:
+        """float64 ``[..., R, W]``: ``u2 / (2 n_p n_n)``, the pixel ROC-AUC (``roc_auc_score``) of every pair, with
+        ``n_p`` the region's pixels and ``n_n`` the others; NaN when either is 0."""
+        n_p = self.region_area.to(device=self.u2.device, dtype=torch.float64).unsqueeze(-1)
+        n_n = self.n_pixels - n_p
+        denom = 2 * n_p * n_n
+        return torch.where(denom > 0, self.u2.double() / denom.clamp(min=1), torch.full_like(denom, float('nan')))
+
+
+def _region_ranking(tokenizer, prompt: str, maps: torch.Tensor, words, image, regions, absolute, word_idx,
+                    offset_idx: int, to_cpu: bool, what: str):
+    """``daam_region_ranking`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(wl, ranking)``, the
+    :class:`_WordList` and the :class:`RegionRanking` with a leading map axis. Checks as ``_region_overlap``, in its
+    order. Scratch: :data:`REGION_RANKING_SCRATCH_BYTES`, clipped to the planes the call has, at least one plane."""
+    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, image, absolute, None, to_cpu, what)
+    n_maps, out_h, out_w, dev = wl.n_maps, wl.out_h, wl.out_w, wl.dev
+    region_bytes = _region_bytes(wl, regions, what)
+    n_regions, n_words = region_bytes.shape[0], len(wl.words)
+    if wl.empty or n_regions == 0:            # no word is scored: the call returns no word heat maps
+        _no_region_overlap(wl, (), n_regions)
+        return wl.done(RegionRanking(torch.zeros((n_maps, n_regions, 0), dtype=torch.int64, device=dev),
+                                     torch.zeros((n_maps, n_regions, 0), dtype=torch.float64, device=dev),
+                                     torch.zeros((n_regions,), dtype=torch.int64, device=dev), out_h * out_w))
+    u2 = torch.empty((n_maps, n_regions, n_words), dtype=torch.int64, device=dev)
+    ap = torch.empty((n_maps, n_regions, n_words), dtype=torch.float64, device=dev)
+    n_bytes = max(_native.region_ranking_scratch_bytes(1, out_h, out_w),
+                  min(REGION_RANKING_SCRATCH_BYTES, _native.region_ranking_scratch_bytes(n_maps * n_words, out_h, out_w)))
+    scratch = torch.empty(n_bytes, dtype=torch.uint8, device=dev)
+    wl.launch(_native.region_ranking, wl.word_maps.data_ptr(), region_bytes.data_ptr(), n_regions, u2.data_ptr(),
+              ap.data_ptr(), scratch.data_ptr(), n_bytes)
+    return wl.done(RegionRanking(u2, ap, (region_bytes != 0).sum((-1, -2)), out_h * out_w))
 
 
 @dataclass
@@ -1033,6 +1111,18 @@ class GlobalHeatMapStack:
         wl, overlap = _region_sweep(self.tokenizer, self.prompt, self.heat_maps, words, image, regions, thresholds,
                                     absolute, word_idx, offset_idx, to_cpu, f'{type(self).__name__}.region_sweep')
         return wl.word_maps, overlap
+
+    def region_ranking(self, words, image, regions: torch.Tensor, absolute: bool = False, word_idx=None,
+                       offset_idx: int = 0, to_cpu: bool = True):
+        """:meth:`GlobalHeatMap.region_ranking` for every map in one call: returns ``(word_maps, ranking)`` with
+        ``word_maps`` the device ``[maps, len(words), xh, xw]`` word heat maps and ``ranking`` a :class:`RegionRanking`
+        with a leading map axis (``u2`` and ``ap`` ``[maps, R, W]``); row ``t`` equals ``self[t].region_ranking(...)``
+        bit for bit (min / max normalisation per map and word). E.g. ``ranking.auroc()[:, 0, 0]`` is word 0's ROC-AUC
+        against region 0 at every step of a history. Scratch stays within a fixed budget whatever the map count: the
+        planes are sorted in rounds."""
+        wl, ranking = _region_ranking(self.tokenizer, self.prompt, self.heat_maps, words, image, regions, absolute,
+                                      word_idx, offset_idx, to_cpu, f'{type(self).__name__}.region_ranking')
+        return wl.word_maps, ranking
 
     def word_overlap(self, words, image=None, absolute: bool = False, threshold: Optional[float] = None,
                      word_idx=None, offset_idx: int = 0, to_cpu: bool = True):

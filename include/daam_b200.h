@@ -35,7 +35,8 @@ extern "C" {
                                           several prompts and a prompt stride <= 0 take the SIMT kernel;
                                           daam_region_overlap; daam_overlay_words, daam_jet_colormap;
                                           daam_finalize_parts; daam_word_overlap;
-                                          daam_word_instances; daam_region_sweep) */
+                                          daam_word_instances; daam_region_sweep;
+                                          daam_region_ranking) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_TOKENS 231     /* daam_accumulate: long contexts of 2 or 3 CLIP chunks of 77 tokens (154, 231) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
@@ -446,6 +447,37 @@ int daam_word_instances(const float* global_maps, int32_t n_maps, int32_t n_rows
                         int32_t absolute, float threshold, int32_t max_instances, float* word_maps, int32_t* count,
                         int32_t* area, int32_t* box, int64_t* sum_yx, float* peak, int32_t* peak_yx, void* scratch,
                         int64_t scratch_bytes, void* stream);
+
+/*
+ * Region ranking: threshold-free scores of each word's expanded map against each of n_regions binary image regions, on
+ * each of n_maps global maps stored back to back -- pixel ROC-AUC and average precision of an attribution map against
+ * a ground-truth mask, which no threshold sweep gives exactly. With m[w] what daam_expand_words writes for word w
+ * WITHOUT threshold (same rows / row_begin / absolute), values compared as fp32 numbers (-0 and +0 tie), P = {p :
+ * regions[r][p] != 0}, N the other pixels, n_p = |P| and n_n = out_h * out_w - n_p:
+ *   u2[i][r][w] = sum_{p in P} sum_{q in N} (2 [m_p > m_q] + [m_p == m_q])      (int64 [n_maps][n_regions][n_words])
+ * twice the Mann-Whitney U with ties counted half, an exact integer: ROC-AUC = u2 / (2 n_p n_n), undefined when n_p or
+ * n_n is 0. With v_1 > v_2 > ... > v_K the distinct values of m[w], TP_k = #{p in P : m_p >= v_k} and FP_k the same
+ * count over N (TP_0 = 0):
+ *   ap[i][r][w] = sum_k (TP_k - TP_{k-1}) / n_p * TP_k / (TP_k + FP_k)        (double, same shape; NaN when n_p = 0)
+ * sklearn's average_precision_score. Arguments as daam_region_overlap without use_threshold / threshold; u2 and ap on
+ * the device. scratch: device, 8-byte aligned, at least DAAM_REGION_RANKING_SCRATCH_BYTES(1, out_h, out_w): one
+ * uint64 region mask per pixel for the call, then DAAM_REGION_RANKING_PLANE_BYTES(out_h, out_w) (about 18 bytes a
+ * pixel) per (map, word) plane of a round. As many planes go in a round as the scratch holds, whole maps while a map's
+ * planes fit, and the call loops over the rounds: one launch, then eighteen a round (the values, a four-pass radix
+ * sort of every plane of the round, the tie-group counts). The results are the same bits whatever the scratch and on
+ * every call: no float atomics, every sum in a fixed order.
+ * Limits (DAAM_E_UNSUPPORTED): those of daam_region_overlap. DAAM_E_INVALID: as daam_region_overlap, plus
+ * scratch_bytes below DAAM_REGION_RANKING_SCRATCH_BYTES(1, out_h, out_w).
+ */
+#define DAAM_REGION_RANKING_PLANE_BYTES(out_h, out_w)                                                                 \
+  (16 * (int64_t)(out_h) * (out_w) + 1024 * (((int64_t)(out_h) * (out_w) + 4095) / 4096) +                           \
+   1540 * (((int64_t)(out_h) * (out_w) + 1023) / 1024) + 512)
+#define DAAM_REGION_RANKING_SCRATCH_BYTES(n_planes, out_h, out_w)                                                     \
+  (8 * (int64_t)(out_h) * (out_w) + (int64_t)(n_planes) * DAAM_REGION_RANKING_PLANE_BYTES(out_h, out_w))
+int daam_region_ranking(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t map_h, int32_t map_w,
+                        const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w,
+                        int32_t absolute, float* word_maps, const uint8_t* regions, int32_t n_regions, int64_t* u2,
+                        double* ap, void* scratch, int64_t scratch_bytes, void* stream);
 
 /*
  * Heat-map overlays: the reference's plot_overlay (daam/heatmap.py:20-53, :66-75 -- the word map coloured with
