@@ -78,6 +78,27 @@ def region_ranking_scratch_bytes(n_planes: int, out_h: int, out_w: int) -> int:
     return 8 * out_h * out_w + n_planes * region_ranking_plane_bytes(out_h, out_w)
 
 
+REFINE_MAX_RADIUS = 64       # DAAM_REFINE_MAX_RADIUS: the largest radius of daam_refine_words
+
+
+def refine_guide_bytes(out_h: int, out_w: int) -> int:
+    """``DAAM_REFINE_GUIDE_BYTES(out_h, out_w)``: the scratch bytes daam_refine_words takes per image of a round (its
+    mean and the inverse of its regularised covariance, per pixel)."""
+    return 36 * out_h * out_w
+
+
+def refine_plane_bytes(out_h: int, out_w: int) -> int:
+    """``DAAM_REFINE_PLANE_BYTES(out_h, out_w)``: the scratch bytes daam_refine_words takes per (map, word) plane of a
+    round."""
+    return 32 * out_h * out_w + 256
+
+
+def refine_scratch_bytes(n_images: int, n_planes: int, out_h: int, out_w: int) -> int:
+    """``DAAM_REFINE_SCRATCH_BYTES(n_images, n_planes, out_h, out_w)``: ``n_images`` images' statistics and ``n_planes``
+    planes; ``(1, 1)`` is the smallest scratch the call takes."""
+    return n_images * refine_guide_bytes(out_h, out_w) + n_planes * refine_plane_bytes(out_h, out_w)
+
+
 def overlay_frames_bytes(n_maps: int, n_words: int, out_h: int, out_w: int) -> int:
     """``DAAM_OVERLAY_FRAMES_BYTES(n_maps, n_words, out_h, out_w)``: the frames rounded up to whole 4-byte words."""
     return (n_maps * n_words * out_h * out_w * 3 + 3) // 4 * 4
@@ -85,7 +106,7 @@ def overlay_frames_bytes(n_maps: int, n_words: int, out_h: int, out_w: int) -> i
 
 EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize',
            'daam_finalize_maps', 'daam_finalize_parts', 'daam_finalize_per_key','daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
-           'daam_segment_words', 'daam_region_overlap', 'daam_region_sweep', 'daam_region_ranking', 'daam_word_overlap', 'daam_word_instances', 'daam_overlay_words', 'daam_jet_colormap',
+           'daam_segment_words', 'daam_region_overlap', 'daam_region_sweep', 'daam_region_ranking', 'daam_word_overlap', 'daam_word_instances', 'daam_overlay_words', 'daam_refine_words', 'daam_jet_colormap',
            'daam_side_launcher_create', 'daam_side_launcher_destroy',
            'daam_side_launcher_launch', 'daam_side_launcher_join', 'daam_side_launcher_idle', 'daam_abi_version',
            'daam_last_error', 'daam_device_info', 'daam_launch_count')
@@ -207,6 +228,9 @@ def load() -> ctypes.CDLL:
     lib.daam_overlay_words.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
                                        i32, i32, f32, i32, vp, vp, i64, vp, vp, vp]
     lib.daam_overlay_words.restype = ctypes.c_int
+    lib.daam_refine_words.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
+                                      i32, i32, f32, i32, f32, vp, vp, i64, vp, vp, i64, vp]
+    lib.daam_refine_words.restype = ctypes.c_int
     lib.daam_jet_colormap.argtypes = [vp]
     lib.daam_jet_colormap.restype = ctypes.c_int
     lib.daam_side_launcher_create.argtypes = [ctypes.POINTER(vp)]
@@ -527,6 +551,19 @@ def overlay_words(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Seq
                                      int(bool(color_normalize)), ctypes.c_void_p(word_maps_ptr),
                                      ctypes.c_void_p(image_ptr), image_map_stride, ctypes.c_void_p(frames_ptr),
                                      ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
+
+
+def refine_words(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int,
+                 out_w: int, absolute: bool, threshold: Optional[float], radius: int, eps: float, word_maps_ptr: int,
+                 image_ptr: int, image_map_stride: int, out_ptr: int, scratch_ptr: int, scratch_bytes: int, stream: int):
+    """``daam_refine_words`` over ``n_maps`` maps ``[n_rows, h, w]`` back to back; ``image_ptr`` uint8 ``[out_h, out_w,
+    3]``, map ``i``'s at ``image_ptr + i * image_map_stride`` bytes (0: one image for all); ``out`` fp32 ``[n_maps,
+    n_words, out_h, out_w]``; ``scratch_bytes`` of scratch, at least :func:`refine_scratch_bytes` ``(1, 1, ...)``."""
+    vp = ctypes.c_void_p
+    _check(load().daam_refine_words(vp(maps_ptr), n_maps, n_rows,
+                                    *_word_list(x, rows_per_word, out_h, out_w, absolute, threshold), int(radius),
+                                    float(eps), vp(word_maps_ptr), vp(image_ptr), image_map_stride, vp(out_ptr),
+                                    vp(scratch_ptr), scratch_bytes, vp(stream)))
 
 
 def jet_colormap():

@@ -17,7 +17,9 @@
 //  - overlay_kernel blends its jet colour onto the image;
 //  - word_pair_tile_kernel sums m[a] * m[b] over every pair of words (then word_pair_reduce_kernel);
 //  - instance_mask_kernel writes it without threshold for components.cu, which labels the mask m > threshold, and
-//    for ranking.cu, which sorts it and scores it against regions (daam_region_ranking).
+//    for ranking.cu, which sorts it and scores it against regions (daam_region_ranking);
+//  - refine.cu recomputes it from segment_minmax_kernel's word maps and partials and filters it with the image as
+//    guide (daam_refine_words).
 // The tile kernels run after segment_minmax_kernel (steps 1 and 2, the word maps and min / max partials to global
 // memory); region_tile_kernel, region_sweep_tile_kernel, overlay_kernel, word_pair_tile_kernel and instance_mask_kernel share the tile helpers
 // (block_tile / tile_at, word_bounds, stage_windows, tap tables). expand_words_kernel, segment_minmax_kernel and segment_label_kernel keep
@@ -34,6 +36,7 @@
 #include "common.cuh"
 #include "components.cuh"
 #include "ranking.cuh"
+#include "refine.cuh"
 
 namespace daam {
 namespace {
@@ -1168,31 +1171,15 @@ static int tile_count(const WordListParams& p) {
   return ((p.oh + kSegTileH - 1) / kSegTileH) * ((p.ow + kSegTileW - 1) / kSegTileW);
 }
 
-// The tile entry points' launches after word_list_prepare: segment_minmax_kernel over (map, word, chunk), then
-// `kernel` over (tile, map), or over (CTA, map) with `ctas` CTAs per map. `smem_before`: the bytes of dynamic shared
-// memory the kernel keeps before its windows; such a kernel stages as many words' windows as fit beside them (it
-// stages them again per pixel chunk when they take several passes). Sets k.s.chunks and k.s.words_per_pass;
-// words_per_pass 0 (only with smem_before): not one window fits, and the kernel reads the word maps instead.
-template <class Params>
-static int launch_tiles(void (*kernel)(Params), Params& k, int n_maps, const DeviceInfo& dev, cudaStream_t stream,
-                        int ctas = 0, size_t smem_before = 0) {
-  WordListParams& p = k.s;
-  // launch 1: enough (map, word, chunk) CTAs for a few waves, at most kMaxChunks per word and one per 256 pixels
+// Launch 1 of the tile entry points, and all of it for daam_refine_words: segment_minmax_kernel over (map, word, chunk)
+// with enough CTAs for a few waves, at most kMaxChunks per word and one per 256 pixels. Sets p.chunks.
+static int launch_word_maps(WordListParams& p, int n_maps, const DeviceInfo& dev, cudaStream_t stream) {
   const long long n = (long long)p.oh * p.ow, mwords = (long long)n_maps * p.n_words;
   long long chunks = (4LL * dev.sm_count + mwords - 1) / mwords;
   if (chunks > kMaxChunks) chunks = kMaxChunks;
   if (chunks > (n + 255) / 256) chunks = (n + 255) / 256;
   if (chunks < 1 || !p.minmax) chunks = 1;
   p.chunks = (int)chunks;
-  // launch 2: a tile's source window is at most ceil(tile * map / out) + 4 rows (columns), and no more than the map
-  const int win_h = std::min<int>(p.mh, (int)ceil((double)kSegTileH * p.mh / p.oh) + 5);
-  const int win_w = std::min<int>(p.mw, (int)ceil((double)kSegTileW * p.mw / p.ow) + 5);
-  const int win = win_h * win_w;
-  if (smem_before)
-    p.words_per_pass = (int)std::min<size_t>(p.n_words, (kMaxSmem - smem_before) / (win * sizeof(float)));
-  else
-    p.words_per_pass = std::max(1, std::min(p.n_words, kSegStageFloats / win));
-  const size_t smem = smem_before + (size_t)p.words_per_pass * win * sizeof(float);
   static std::once_flag attr_once[64];
   cudaError_t attr_err = cudaSuccess;
   std::call_once(attr_once[dev.device & 63], [&] {
@@ -1207,6 +1194,28 @@ static int launch_tiles(void (*kernel)(Params), Params& k, int n_maps, const Dev
   segment_minmax_kernel<<<(unsigned)(mwords * p.chunks), 256, (size_t)p.mh * p.mw * sizeof(float), stream>>>(p);
   DAAM_CUDA_TRY(cudaGetLastError());
   count_launch();
+  return DAAM_OK;
+}
+
+// The tile entry points' launches after word_list_prepare: launch_word_maps, then `kernel` over (tile, map), or over
+// (CTA, map) with `ctas` CTAs per map. `smem_before`: the bytes of dynamic shared memory the kernel keeps before its
+// windows; such a kernel stages as many words' windows as fit beside them (it stages them again per pixel chunk when
+// they take several passes). Sets k.s.chunks and k.s.words_per_pass; words_per_pass 0 (only with smem_before): not
+// one window fits, and the kernel reads the word maps instead.
+template <class Params>
+static int launch_tiles(void (*kernel)(Params), Params& k, int n_maps, const DeviceInfo& dev, cudaStream_t stream,
+                        int ctas = 0, size_t smem_before = 0) {
+  WordListParams& p = k.s;
+  if (int rc = launch_word_maps(p, n_maps, dev, stream)) return rc;
+  // launch 2: a tile's source window is at most ceil(tile * map / out) + 4 rows (columns), and no more than the map
+  const int win_h = std::min<int>(p.mh, (int)ceil((double)kSegTileH * p.mh / p.oh) + 5);
+  const int win_w = std::min<int>(p.mw, (int)ceil((double)kSegTileW * p.mw / p.ow) + 5);
+  const int win = win_h * win_w;
+  if (smem_before)
+    p.words_per_pass = (int)std::min<size_t>(p.n_words, (kMaxSmem - smem_before) / (win * sizeof(float)));
+  else
+    p.words_per_pass = std::max(1, std::min(p.n_words, kSegStageFloats / win));
+  const size_t smem = smem_before + (size_t)p.words_per_pass * win * sizeof(float);
   kernel<<<dim3(ctas ? ctas : tile_count(p), n_maps), 256, smem, stream>>>(k);
   DAAM_CUDA_TRY(cudaGetLastError());
   count_launch();
@@ -1433,6 +1442,66 @@ extern "C" int daam_region_ranking(const float* global_maps, int32_t n_maps, int
       c.n_regions = n_regions; c.u2 = reinterpret_cast<long long*>(u2); c.ap = ap;
       c.n_words_round = nw; c.n_words = n_words; c.map0 = map0; c.w0 = w0;
       if (int rc = launch_ranking(c, stream)) return rc;
+    }
+  }
+  return DAAM_OK;
+}
+
+extern "C" int daam_refine_words(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t mh, int32_t mw,
+                                 const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h,
+                                 int32_t out_w, int32_t absolute, int32_t use_threshold, float threshold,
+                                 int32_t radius, float eps, float* word_maps, const uint8_t* image,
+                                 int64_t image_map_stride, float* out, void* scratch, int64_t scratch_bytes,
+                                 void* stream_) {
+  const char* name = "daam_refine_words";
+  if (!global_maps || !rows || !row_begin || !word_maps || !image || !out || !scratch || n_maps <= 0 || mh <= 0 ||
+      mw <= 0 || out_h <= 0 || out_w <= 0 || n_rows <= 0 || image_map_stride < 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
+  if (radius < 1 || radius > kRefineMaxRadius) { set_error("%s: radius %d is not in [1, %d]", name, radius, kRefineMaxRadius); return DAAM_E_INVALID; }
+  if (!(eps > 0.f) || !isfinite(eps)) { set_error("%s: eps %g is not finite and > 0", name, (double)eps); return DAAM_E_INVALID; }
+  if ((uintptr_t)scratch & 3) { set_error("%s: scratch must be 4-byte aligned", name); return DAAM_E_INVALID; }
+  // the statistics of one image, then the planes of each round
+  const long long guide_bytes = refine_guide_bytes(out_h, out_w), plane_bytes = refine_plane_bytes(out_h, out_w);
+  if (scratch_bytes < guide_bytes + plane_bytes) { set_error("%s: %lld scratch bytes < %lld, one image's statistics and one %d x %d plane", name, (long long)scratch_bytes, guide_bytes + plane_bytes, out_h, out_w); return DAAM_E_INVALID; }
+  static thread_local WordListParams p, q;
+  DeviceInfo dev;
+  if (int rc = word_list_prepare(name, global_maps, n_maps, n_rows, mh, mw, rows, row_begin, n_words, out_h, out_w,
+                                 absolute, !absolute, 0, 0.f, word_maps, nullptr, true, p, &dev)) return rc;
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  // a round: whole maps while a map's planes (and with one image per map, its statistics) fit the scratch, else the
+  // words of one map in groups
+  const bool per_map = image_map_stride != 0;
+  const long long map_bytes = (per_map ? guide_bytes : 0) + n_words * plane_bytes;
+  const long long whole = std::min<long long>((scratch_bytes - (per_map ? 0 : guide_bytes)) / map_bytes, 65535 / n_words);
+  const int maps_per_round = (int)std::max<long long>(1, std::min<long long>(whole, n_maps));
+  const int words_per_round = whole >= 1 ? (int)n_words
+                                         : (int)std::min<long long>((scratch_bytes - guide_bytes) / plane_bytes, n_words);
+  RefinePlanes c;
+  refine_planes_in(scratch, per_map ? maps_per_round : 1, maps_per_round * words_per_round, out_h, out_w, c);
+  c.image_map_stride = image_map_stride;
+  c.mh = mh; c.mw = mw; c.absolute = p.absolute; c.use_threshold = use_threshold ? 1 : 0; c.threshold = threshold;
+  c.radius = radius; c.eps = eps;
+  const long long n = (long long)out_h * out_w;
+  for (int map0 = 0; map0 < n_maps; map0 += maps_per_round) {
+    const int nm = std::min(maps_per_round, n_maps - map0);
+    for (int w0 = 0; w0 < n_words; w0 += words_per_round) {
+      const int nw = std::min(words_per_round, n_words - w0);
+      q = p;
+      q.maps = global_maps + map0 * p.map_stride;
+      q.n_words = nw;
+      for (int i = 0; i <= nw; ++i) q.row_begin[i] = p.row_begin[w0 + i];
+      const long long plane0 = (long long)map0 * n_words + w0;
+      q.word_maps = word_maps + plane0 * mh * mw;
+      q.scratch = c.minmax;
+      if (int rc = launch_word_maps(q, nm, dev, stream)) return rc;
+      c.word_maps = q.word_maps; c.chunks = q.chunks;
+      c.image = image + map0 * image_map_stride;
+      c.planes = nm * nw; c.words_per_map = nw; c.out = out + plane0 * n;
+      // the statistics of the round's images, kept while the words of one map take several rounds
+      if (w0 == 0 && (per_map || map0 == 0)) {
+        c.guides = per_map ? nm : 1;
+        if (int rc = launch_refine_guides(c, stream)) return rc;
+      }
+      if (int rc = launch_refine(c, dev.device, stream)) return rc;
     }
   }
   return DAAM_OK;

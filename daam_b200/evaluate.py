@@ -23,7 +23,11 @@ of a parse, :meth:`GlobalHeatMap.relation_overlap <daam_b200.heatmap.GlobalHeatM
 stack: three fused launches for every pair, with the same bit-for-bit equality for thresholded masks. For the boxes,
 counts and centroids of each word's thresholded mask (the localisation protocol: the largest connected component's
 box against a ground-truth box), use :meth:`GlobalHeatMap.word_instances <daam_b200.heatmap.GlobalHeatMap.word_instances>`
-and ``WordInstances.box_iou``, on one map or a stack.
+and ``WordInstances.box_iou``, on one map or a stack. To refine the masks against the image before scoring them
+(word boundaries that follow the image's edges rather than the heat-map grid), use :meth:`GlobalHeatMap.refine_words
+<daam_b200.heatmap.GlobalHeatMap.refine_words>` / :meth:`GlobalHeatMapStack.refine_words
+<daam_b200.heatmap.GlobalHeatMapStack.refine_words>`: the guided filter of each word's map with the image as guide,
+fused on the device; score its result with :func:`compute_iou` or torch.
 """
 from __future__ import annotations
 

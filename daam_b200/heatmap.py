@@ -15,6 +15,8 @@ The spaCy-parsed iterators and matplotlib overlays of the reference are out of s
 """
 from __future__ import annotations
 
+import ctypes
+import math
 import numbers
 from dataclasses import dataclass
 from functools import lru_cache
@@ -527,6 +529,29 @@ class GlobalHeatMap:
         wl, frames = _overlay(self.tokenizer, self.prompt, self.heat_maps[None], words, image, absolute, threshold,
                               color_normalize, word_idx, offset_idx, to_cpu, 'GlobalHeatMap.overlay_words', stack=False)
         return wl.word_heat_maps(0), frames[0]
+
+    def refine_words(self, words, image, radius: int = 8, eps: float = 1e-3, absolute: bool = False,
+                     threshold: Optional[float] = None, word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
+        """Edge-aware word maps: each word's expanded map run through the guided filter (He, Sun and Tang, "Guided
+        Image Filtering", TPAMI 2013, colour-guide form) with the image as guide, so that word boundaries follow the
+        image's edges instead of the heat-map grid. With ``m[w]`` what ``expand_words(words, image, absolute,
+        word_idx=word_idx, offset_idx=offset_idx)`` returns (no threshold), ``I`` the image's RGB bytes / 255 and
+        ``mean`` the box mean over the ``(2 radius + 1)^2`` window clipped to the image (border windows shrink):
+        ``mu = mean(I)``, ``Sigma = mean(I I^T) - mu mu^T``, ``a = (Sigma + eps Id)^-1 (mean(I m) - mu mean(m))``,
+        ``b = mean(m) - a . mu`` and ``refined[w] = mean(a) . I + mean(b)``. The result is not clamped: it can
+        overshoot ``[0, 1]`` slightly. With ``threshold`` in effect (Python truthiness, as in ``expand_words``) it is
+        ``(refined > threshold)`` as fp32 1.0 / 0.0. ``eps`` is in the units of ``I^2``: small values keep finer edges.
+
+        ``image``: as :meth:`overlay_words` takes it, a PIL image or a uint8 ``[H, W, 3]`` numpy / torch array at the size
+        ``expand_words`` gives. Returns ``(word_heat_maps, refined)``: the list of :class:`WordHeatMap` that
+        :meth:`segment` returns and ``refined`` fp32 ``[len(words), H, W]`` (CPU by default, ``to_cpu=False`` keeps it
+        on the device). The image statistics come from exact integer window sums; the ``[len(words), H, W]`` stack of
+        ``m`` is never written, and the results are the same bits on every call. ``1 <= radius <= 64``, ``eps`` finite
+        and > 0 (a ``ValueError`` otherwise); at most 96 words. An empty word list launches nothing. Raises the
+        reference's ``ValueError`` for a word that is not in the prompt."""
+        wl, refined = _refine(self.tokenizer, self.prompt, self.heat_maps[None], words, image, radius, eps, absolute,
+                              threshold, word_idx, offset_idx, to_cpu, 'GlobalHeatMap.refine_words', stack=False)
+        return wl.word_heat_maps(0), refined[0]
 
 
 def _check_rows(rows, n_rows: int):
@@ -1056,6 +1081,46 @@ def _overlay(tokenizer, prompt: str, maps: torch.Tensor, words, image, absolute,
     return wl.done(frames)
 
 
+# Scratch of one refine_words call: the image statistics (36 bytes a pixel, per image) and as many (map, word) planes
+# as fit (32 bytes a pixel each) go in a round, so memory does not grow with the number of maps; one image and one
+# plane larger than the budget go alone.
+REFINE_SCRATCH_BYTES = 256 << 20
+
+
+def _refine_args(radius, eps, what: str):
+    """Raises ``ValueError`` unless ``radius`` is an integer in ``[1, 64]`` and ``eps``, rounded to fp32, is finite
+    and > 0."""
+    if isinstance(radius, bool) or not isinstance(radius, int) or not 1 <= radius <= _native.REFINE_MAX_RADIUS:
+        raise ValueError(f'{what}: radius must be an integer in [1, {_native.REFINE_MAX_RADIUS}], not {radius!r}')
+    e32 = ctypes.c_float(float(eps)).value
+    if not (math.isfinite(e32) and e32 > 0):
+        raise ValueError(f'{what}: eps must be finite and > 0 in fp32, not {eps!r}')
+
+
+def _refine(tokenizer, prompt: str, maps: torch.Tensor, words, image, radius, eps, absolute, threshold, word_idx,
+            offset_idx: int, to_cpu: bool, what: str, stack: bool):
+    """``daam_refine_words`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(wl, refined)``, the
+    :class:`_WordList` and ``refined`` fp32 ``[n_maps, len(words), H, W]``. Checks as :func:`_overlay`, in its order,
+    then ``radius`` and ``eps``. Scratch: :data:`REFINE_SCRATCH_BYTES`, clipped to what the call has, at least one
+    image and one plane."""
+    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, None, absolute, threshold, to_cpu, what,
+                   on_grid=True)         # the size is the image's, once _overlay_image has checked it
+    n_maps, n_words, dev = wl.n_maps, len(wl.words), wl.dev
+    image, wl.out_h, wl.out_w, per_map = _overlay_image(image, n_maps, wl.grid, dev, what, stack)
+    _refine_args(radius, eps, what)
+    refined = torch.empty((n_maps, n_words, wl.out_h, wl.out_w), dtype=torch.float32, device=dev)
+    if wl.empty:
+        return wl.done(refined)
+    image = image.to(dev).contiguous()                   # one copy to the device
+    n_bytes = max(_native.refine_scratch_bytes(1, 1, wl.out_h, wl.out_w),
+                  min(REFINE_SCRATCH_BYTES, _native.refine_scratch_bytes(n_maps if per_map else 1, n_maps * n_words,
+                                                                         wl.out_h, wl.out_w)))
+    scratch = torch.empty(n_bytes, dtype=torch.uint8, device=dev)
+    wl.launch(_native.refine_words, radius, eps, wl.word_maps.data_ptr(), image.data_ptr(),
+              wl.out_h * wl.out_w * 3 if per_map else 0, refined.data_ptr(), scratch.data_ptr(), n_bytes)
+    return wl.done(refined)
+
+
 class GlobalHeatMapStack:
     """Global heat maps of one prompt's text stacked along a first axis: ``heat_maps[t]`` is one
     ``[n_rows, xh, xw]`` map. Base of :class:`TimeHeatMaps` (one map per step), :class:`ImageHeatMaps` (one per
@@ -1166,6 +1231,19 @@ class GlobalHeatMapStack:
                               color_normalize, word_idx, offset_idx, to_cpu, f'{type(self).__name__}.overlay_words',
                               stack=True)
         return wl.word_maps, frames
+
+    def refine_words(self, words, image, radius: int = 8, eps: float = 1e-3, absolute: bool = False,
+                     threshold: Optional[float] = None, word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
+        """:meth:`GlobalHeatMap.refine_words` for every map in one call: returns ``(word_maps, refined)`` with
+        ``word_maps`` the device ``[maps, len(words), xh, xw]`` word heat maps and ``refined`` fp32 ``[maps,
+        len(words), H, W]``; row ``t`` equals ``self[t].refine_words(...)`` bit for bit (min / max normalisation per map
+        and word). ``image`` is one image for every map (its statistics are computed once), or a uint8 ``[maps, H, W,
+        3]`` array with one per map (e.g. the images of ``compute_image_heat_maps()``). Scratch stays within a fixed
+        budget whatever the map count: the planes are filtered in rounds."""
+        wl, refined = _refine(self.tokenizer, self.prompt, self.heat_maps, words, image, radius, eps, absolute,
+                              threshold, word_idx, offset_idx, to_cpu, f'{type(self).__name__}.refine_words',
+                              stack=True)
+        return wl.word_maps, refined
 
 
 class TimeHeatMaps(GlobalHeatMapStack):

@@ -36,7 +36,7 @@ extern "C" {
                                           daam_region_overlap; daam_overlay_words, daam_jet_colormap;
                                           daam_finalize_parts; daam_word_overlap;
                                           daam_word_instances; daam_region_sweep;
-                                          daam_region_ranking) */
+                                          daam_region_ranking; daam_refine_words) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_TOKENS 231     /* daam_accumulate: long contexts of 2 or 3 CLIP chunks of 77 tokens (154, 231) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
@@ -511,6 +511,38 @@ int daam_overlay_words(const float* global_maps, int32_t n_maps, int32_t n_rows,
  * float64, piecewise linear through matplotlib's `jet` segment points. out: host fp32 [256][3].
  */
 int daam_jet_colormap(float* out);
+
+/*
+ * Edge-aware word maps: the guided filter (He, Sun and Tang, "Guided Image Filtering", TPAMI 2013, colour-guide form)
+ * of each word's expanded map with the image as guide, on each of n_maps global maps stored back to back. With m[w]
+ * what daam_expand_words writes for word w WITHOUT threshold (same rows / row_begin / absolute), I = image / 255 in
+ * [0, 1]^3, W(x) the (2 radius + 1)^2 window around x clipped to the image, N(x) = |W(x)| and mean_f(x) = sum_{y in
+ * W(x)} f(y) / N(x) (border windows shrink):
+ *   mu = mean(I),  Sigma = mean(I I^T) - mu mu^T,  p = mean(m),  c = mean(I m) - mu p,
+ *   a = (Sigma + eps Id)^-1 c,  b = p - a^T mu,  q(x) = mean(a)(x)^T I(x) + mean(b)(x)
+ * out[i][w] = q, not clamped (it can overshoot [0, 1] slightly), or with use_threshold (q > threshold) as 1.0 / 0.0.
+ * Arguments as daam_overlay_words with color_normalize replaced by radius (1 <= radius <= 64) and eps (finite, > 0, in
+ * the units of I^2); out: device fp32 [n_maps][n_words][out_h][out_w]. scratch: device, 4-byte aligned, at least
+ * DAAM_REFINE_SCRATCH_BYTES(1, 1, out_h, out_w): DAAM_REFINE_GUIDE_BYTES(out_h, out_w) of statistics per image of a
+ * round (mu and the inverse, one image when image_map_stride is 0), then DAAM_REFINE_PLANE_BYTES(out_h, out_w) per
+ * (map, word) plane of a round. As many planes go in a round as the scratch holds, whole maps while a map's planes fit,
+ * and the call loops over the rounds: two launches per image for its statistics (built from exact integer window
+ * sums), then five a round (the word maps, and two separable passes of direct fp32 window sums of at most 2 radius + 1
+ * values each). The [n_words][out_h][out_w] stack of m is never written. The results are the same bits whatever the
+ * scratch and on every call: no atomics.
+ * Limits (DAAM_E_UNSUPPORTED): as daam_overlay_words. DAAM_E_INVALID: as daam_overlay_words, plus radius or eps out of
+ * range, scratch not 4-byte aligned or scratch_bytes below DAAM_REFINE_SCRATCH_BYTES(1, 1, out_h, out_w).
+ */
+#define DAAM_REFINE_MAX_RADIUS 64
+#define DAAM_REFINE_GUIDE_BYTES(out_h, out_w) (36 * (int64_t)(out_h) * (out_w))
+#define DAAM_REFINE_PLANE_BYTES(out_h, out_w) (32 * (int64_t)(out_h) * (out_w) + 256)
+#define DAAM_REFINE_SCRATCH_BYTES(n_images, n_planes, out_h, out_w)                                                    \
+  ((int64_t)(n_images) * DAAM_REFINE_GUIDE_BYTES(out_h, out_w) + (int64_t)(n_planes) * DAAM_REFINE_PLANE_BYTES(out_h, out_w))
+int daam_refine_words(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t map_h, int32_t map_w,
+                      const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w,
+                      int32_t absolute, int32_t use_threshold, float threshold, int32_t radius, float eps,
+                      float* word_maps, const uint8_t* image, int64_t image_map_stride, float* out, void* scratch,
+                      int64_t scratch_bytes, void* stream);
 
 /* Library / device introspection. */
 int daam_abi_version(void);
