@@ -99,6 +99,32 @@ def refine_scratch_bytes(n_images: int, n_planes: int, out_h: int, out_w: int) -
     return n_images * refine_guide_bytes(out_h, out_w) + n_planes * refine_plane_bytes(out_h, out_w)
 
 
+BOUNDARY_MAX_TOLERANCES = 16  # DAAM_BOUNDARY_MAX_TOLERANCES: tolerances of daam_region_boundary / daam_mask_boundary
+
+
+def boundary_tile_rows(out_w: int) -> int:
+    """``DAAM_BOUNDARY_TILE_ROWS(out_w)``: the rows of one query tile of the boundary calls."""
+    return 16 if out_w >= 256 else (4096 + out_w - 1) // out_w
+
+
+def boundary_call_bytes(n_regions: int, out_h: int, out_w: int) -> int:
+    """``DAAM_BOUNDARY_CALL_BYTES(n_regions, out_h, out_w)``: the regions' column distances, once per call (about 4
+    bytes a pixel per region)."""
+    return 8 * n_regions * ((out_h * out_w + 1) // 2)
+
+
+def boundary_plane_bytes(out_h: int, out_w: int) -> int:
+    """``DAAM_BOUNDARY_PLANE_BYTES(out_h, out_w)``: the scratch bytes the boundary calls take per plane of a round."""
+    rows = boundary_tile_rows(out_w)
+    return 16 * ((out_h * out_w + 1) // 2) + 256 + 10080 * ((out_h + rows - 1) // rows)
+
+
+def boundary_scratch_bytes(n_regions: int, n_planes: int, out_h: int, out_w: int) -> int:
+    """``DAAM_BOUNDARY_SCRATCH_BYTES(n_regions, n_planes, out_h, out_w)``: the regions' state and ``n_planes`` planes;
+    ``n_planes = 1`` is the smallest scratch the calls take."""
+    return boundary_call_bytes(n_regions, out_h, out_w) + n_planes * boundary_plane_bytes(out_h, out_w)
+
+
 def overlay_frames_bytes(n_maps: int, n_words: int, out_h: int, out_w: int) -> int:
     """``DAAM_OVERLAY_FRAMES_BYTES(n_maps, n_words, out_h, out_w)``: the frames rounded up to whole 4-byte words."""
     return (n_maps * n_words * out_h * out_w * 3 + 3) // 4 * 4
@@ -106,7 +132,7 @@ def overlay_frames_bytes(n_maps: int, n_words: int, out_h: int, out_w: int) -> i
 
 EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize',
            'daam_finalize_maps', 'daam_finalize_parts', 'daam_finalize_per_key','daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
-           'daam_segment_words', 'daam_region_overlap', 'daam_region_sweep', 'daam_region_ranking', 'daam_word_overlap', 'daam_word_instances', 'daam_overlay_words', 'daam_refine_words', 'daam_jet_colormap',
+           'daam_segment_words', 'daam_region_overlap', 'daam_region_sweep', 'daam_region_ranking', 'daam_region_boundary', 'daam_mask_boundary', 'daam_word_overlap', 'daam_word_instances', 'daam_overlay_words', 'daam_refine_words', 'daam_jet_colormap',
            'daam_side_launcher_create', 'daam_side_launcher_destroy',
            'daam_side_launcher_launch', 'daam_side_launcher_join', 'daam_side_launcher_idle', 'daam_abi_version',
            'daam_last_error', 'daam_device_info', 'daam_launch_count')
@@ -228,6 +254,13 @@ def load() -> ctypes.CDLL:
     lib.daam_overlay_words.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
                                        i32, i32, f32, i32, vp, vp, i64, vp, vp, vp]
     lib.daam_overlay_words.restype = ctypes.c_int
+    lib.daam_region_boundary.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32,
+                                         i32, i32, f32, ctypes.POINTER(f32), i32, vp, vp, i32, vp, vp, vp, vp, vp, vp,
+                                         vp, i64, vp]
+    lib.daam_region_boundary.restype = ctypes.c_int
+    lib.daam_mask_boundary.argtypes = [vp, i32, i32, i32, vp, i32, ctypes.POINTER(f32), i32, vp, vp, vp, vp, vp, vp, vp,
+                                       i64, vp]
+    lib.daam_mask_boundary.restype = ctypes.c_int
     lib.daam_refine_words.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
                                       i32, i32, f32, i32, f32, vp, vp, i64, vp, vp, i64, vp]
     lib.daam_refine_words.restype = ctypes.c_int
@@ -551,6 +584,40 @@ def overlay_words(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Seq
                                      int(bool(color_normalize)), ctypes.c_void_p(word_maps_ptr),
                                      ctypes.c_void_p(image_ptr), image_map_stride, ctypes.c_void_p(frames_ptr),
                                      ctypes.c_void_p(scratch_ptr), ctypes.c_void_p(stream)))
+
+
+def region_boundary(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int,
+                    out_w: int, absolute: bool, threshold: float, tolerances: Sequence[float], word_maps_ptr: int,
+                    regions_ptr: int, n_regions: int, word_boundary_ptr: int, region_boundary_ptr: int,
+                    word_hits_ptr: int, region_hits_ptr: int, max_d2_ptr: int, sum_dist_ptr: int, scratch_ptr: int,
+                    scratch_bytes: int, stream: int):
+    """``daam_region_boundary`` over ``n_maps`` maps ``[n_rows, h, w]`` back to back and ``n_regions`` uint8 regions
+    ``[out_h, out_w]``: ``word_boundary`` int32 ``[n_maps, n_words]``, ``region_boundary`` int32 ``[n_regions]``,
+    ``word_hits`` / ``region_hits`` int32 ``[n_maps, T, n_regions, n_words]``, ``max_d2`` int64 and ``sum_dist`` float64
+    ``[n_maps, n_regions, n_words, 2]``; ``scratch_bytes`` of scratch, at least :func:`boundary_scratch_bytes` of one
+    plane. The threshold is always in effect: the call takes no ``use_threshold``."""
+    vp = ctypes.c_void_p
+    tol = (ctypes.c_float * max(len(tolerances), 1))(*tolerances)
+    _check(load().daam_region_boundary(vp(maps_ptr), n_maps, n_rows,
+                                       *_word_list(x, rows_per_word, out_h, out_w, absolute, None)[:-2],
+                                       float(threshold), tol, len(tolerances), vp(word_maps_ptr), vp(regions_ptr),
+                                       n_regions, vp(word_boundary_ptr), vp(region_boundary_ptr), vp(word_hits_ptr),
+                                       vp(region_hits_ptr), vp(max_d2_ptr), vp(sum_dist_ptr), vp(scratch_ptr),
+                                       scratch_bytes, vp(stream)))
+
+
+def mask_boundary(masks_ptr: int, n_planes: int, out_h: int, out_w: int, regions_ptr: int, n_regions: int,
+                  tolerances: Sequence[float], word_boundary_ptr: int, region_boundary_ptr: int, word_hits_ptr: int,
+                  region_hits_ptr: int, max_d2_ptr: int, sum_dist_ptr: int, scratch_ptr: int, scratch_bytes: int,
+                  stream: int):
+    """``daam_mask_boundary`` over ``n_planes`` uint8 masks ``[out_h, out_w]`` back to back: the outputs of
+    :func:`region_boundary` with ``n_maps * n_words`` replaced by ``n_planes``."""
+    vp = ctypes.c_void_p
+    tol = (ctypes.c_float * max(len(tolerances), 1))(*tolerances)
+    _check(load().daam_mask_boundary(vp(masks_ptr), n_planes, out_h, out_w, vp(regions_ptr), n_regions, tol,
+                                     len(tolerances), vp(word_boundary_ptr), vp(region_boundary_ptr),
+                                     vp(word_hits_ptr), vp(region_hits_ptr), vp(max_d2_ptr), vp(sum_dist_ptr),
+                                     vp(scratch_ptr), scratch_bytes, vp(stream)))
 
 
 def refine_words(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int,

@@ -17,7 +17,8 @@
 //  - overlay_kernel blends its jet colour onto the image;
 //  - word_pair_tile_kernel sums m[a] * m[b] over every pair of words (then word_pair_reduce_kernel);
 //  - instance_mask_kernel writes it without threshold for components.cu, which labels the mask m > threshold, and
-//    for ranking.cu, which sorts it and scores it against regions (daam_region_ranking);
+//    for ranking.cu, which sorts it and scores it against regions (daam_region_ranking), and for boundary.cu, which
+//    measures the boundary of m > threshold against the regions' boundaries (daam_region_boundary);
 //  - refine.cu recomputes it from segment_minmax_kernel's word maps and partials and filters it with the image as
 //    guide (daam_refine_words).
 // The tile kernels run after segment_minmax_kernel (steps 1 and 2, the word maps and min / max partials to global
@@ -33,6 +34,7 @@
 #include <mutex>
 
 #include "bicubic.cuh"
+#include "boundary.cuh"
 #include "common.cuh"
 #include "components.cuh"
 #include "ranking.cuh"
@@ -1442,6 +1444,58 @@ extern "C" int daam_region_ranking(const float* global_maps, int32_t n_maps, int
       c.n_regions = n_regions; c.u2 = reinterpret_cast<long long*>(u2); c.ap = ap;
       c.n_words_round = nw; c.n_words = n_words; c.map0 = map0; c.w0 = w0;
       if (int rc = launch_ranking(c, stream)) return rc;
+    }
+  }
+  return DAAM_OK;
+}
+
+extern "C" int daam_region_boundary(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t mh, int32_t mw,
+                                    const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h,
+                                    int32_t out_w, int32_t absolute, float threshold, const float* tolerances,
+                                    int32_t n_tolerances, float* word_maps, const uint8_t* regions, int32_t n_regions,
+                                    int32_t* word_boundary, int32_t* region_boundary, int32_t* word_hits,
+                                    int32_t* region_hits, int64_t* max_d2, double* sum_dist, void* scratch,
+                                    int64_t scratch_bytes, void* stream_) {
+  const char* name = "daam_region_boundary";
+  if (!global_maps || !rows || !row_begin || !tolerances || !word_maps || !regions || !word_boundary ||
+      !region_boundary || !word_hits || !region_hits || !max_d2 || !sum_dist || !scratch || n_maps <= 0 || mh <= 0 ||
+      mw <= 0 || out_h <= 0 || out_w <= 0 || n_rows <= 0 || n_regions <= 0 || n_tolerances <= 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
+  if (n_tolerances > kBoundaryMaxTolerances) { set_error("%s: %d tolerances > %d", name, n_tolerances, kBoundaryMaxTolerances); return DAAM_E_UNSUPPORTED; }
+  if (n_regions > kMaxRegions) { set_error("%s: %d regions > %d", name, n_regions, kMaxRegions); return DAAM_E_UNSUPPORTED; }
+  if ((long long)out_h * out_w > (1LL << 24)) { set_error("%s: a %d x %d output is more than 2^24 pixels", name, out_h, out_w); return DAAM_E_UNSUPPORTED; }
+  BoundaryPlanes c;
+  if (int rc = boundary_check_tolerances(name, tolerances, n_tolerances, c)) return rc;
+  if (!isfinite(threshold)) { set_error("%s: threshold %g is not finite", name, (double)threshold); return DAAM_E_INVALID; }
+  if (int rc = boundary_check_scratch(name, scratch, scratch_bytes, n_regions, out_h, out_w)) return rc;
+  static thread_local InstanceMaskParams p, q;
+  DeviceInfo dev;
+  if (int rc = word_list_prepare(name, global_maps, n_maps, n_rows, mh, mw, rows, row_begin, n_words, out_h, out_w,
+                                 absolute, !absolute, 0, 0.f, word_maps, nullptr, true, p.s, &dev)) return rc;
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  c.word_boundary = word_boundary; c.region_boundary = region_boundary; c.word_hits = word_hits;
+  c.region_hits = region_hits; c.max_d2 = reinterpret_cast<long long*>(max_d2); c.sum_dist = sum_dist;
+  c.n_words = n_words;
+  boundary_planes_in(scratch, n_regions, 1, out_h, out_w, c);
+  if (int rc = launch_boundary_regions(regions, c, n_maps, stream)) return rc;
+  // a round: whole maps while a map's planes fit the scratch, else the words of one map in groups
+  const int cap = (int)std::min<long long>(
+      (scratch_bytes - boundary_call_bytes(n_regions, out_h, out_w)) / boundary_plane_bytes(out_h, out_w), 65535);
+  const int maps_per_round = std::max(1, cap / n_words), words_per_round = std::min(cap, (int)n_words);
+  for (int map0 = 0; map0 < n_maps; map0 += maps_per_round) {
+    const int nm = std::min(maps_per_round, n_maps - map0);
+    for (int w0 = 0; w0 < n_words; w0 += words_per_round) {
+      const int nw = std::min(words_per_round, n_words - w0);
+      q = p;
+      q.s.maps = global_maps + map0 * p.s.map_stride;
+      q.s.n_words = nw;
+      for (int i = 0; i <= nw; ++i) q.s.row_begin[i] = p.s.row_begin[w0 + i];
+      q.s.word_maps = word_maps + ((long long)map0 * n_words + w0) * mh * mw;
+      boundary_planes_in(scratch, n_regions, nm * nw, out_h, out_w, c);
+      q.s.scratch = c.minmax;
+      q.pre = c.pre;
+      if (int rc = launch_tiles(instance_mask_kernel, q, nm, dev, stream)) return rc;
+      c.n_words_round = nw; c.map0 = map0; c.w0 = w0;
+      if (int rc = launch_boundary_round(c, threshold, nullptr, stream)) return rc;
     }
   }
   return DAAM_OK;

@@ -28,6 +28,12 @@ and ``WordInstances.box_iou``, on one map or a stack. To refine the masks agains
 <daam_b200.heatmap.GlobalHeatMap.refine_words>` / :meth:`GlobalHeatMapStack.refine_words
 <daam_b200.heatmap.GlobalHeatMapStack.refine_words>`: the guided filter of each word's map with the image as guide,
 fused on the device; score its result with :func:`compute_iou` or torch.
+To measure where each word's boundary lies against each region's -- the boundary F-measure at pixel tolerances, the
+Hausdorff distance and the average symmetric surface distance, the scores a smeared or shifted boundary moves and IoU
+barely does -- use :meth:`GlobalHeatMap.region_boundary <daam_b200.heatmap.GlobalHeatMap.region_boundary>` /
+:meth:`GlobalHeatMapStack.region_boundary <daam_b200.heatmap.GlobalHeatMapStack.region_boundary>` on the thresholded
+word masks, or :func:`boundary_scores` on any device masks, such as ``refine_words(...) > t``: every boundary pixel's
+nearest boundary pixel of the other set found exactly on the device, in one call for every (mask, region) pair.
 """
 from __future__ import annotations
 
@@ -35,7 +41,7 @@ import torch
 
 from . import _native
 
-__all__ = ['compute_iou', 'compute_ioa']
+__all__ = ['compute_iou', 'compute_ioa', 'boundary_scores']
 
 
 def _match_size(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
@@ -65,3 +71,65 @@ def compute_ioa(a: torch.Tensor, b: torch.Tensor) -> float:
     a = _match_size(a, b)
     intersection = (a * b).sum()
     return (intersection / (a.sum() + 1e-8)).item()
+
+
+def boundary_scores(masks: torch.Tensor, regions: torch.Tensor, tolerances=None, to_cpu: bool = True):
+    """Boundary scores of device masks against image regions: :meth:`GlobalHeatMap.region_boundary
+    <daam_b200.heatmap.GlobalHeatMap.region_boundary>` with the masks given. ``masks``: bool or uint8 ``[W, H, W']``
+    or ``[M, W, H, W']`` on a CUDA device, any nonzero byte inside; the second-to-last mask axis is the word axis, so
+    ``refine_words(...) > t`` of a heat map (``[words, H, W]``) or of a stack (``[maps, words, H, W]``) gives the shapes
+    ``region_boundary`` gives. ``regions``: bool or uint8 ``[H, W']`` (one region) or ``[R, H, W']`` on the same device.
+    ``tolerances`` as for ``region_boundary`` (``None``: ``ceil(0.008 * sqrt(H**2 + W'**2))``). Returns a
+    :class:`~daam_b200.heatmap.RegionBoundary` (``word_hits`` ``[..., T, R, W]``, ``max_d2`` ``[..., R, W, 2]``, ...,
+    with ``...`` the ``M`` axis of 4-D masks), on the CPU unless ``to_cpu=False``. No mask or no region launches
+    nothing and gives empty axes. At most 63 regions and 2**24 pixels."""
+    from .heatmap import (RegionBoundary, _boundary_outputs, _boundary_pointers, _boundary_scratch,
+                          _boundary_tolerances, _require_cuda, _stream_ptr)
+    what = 'boundary_scores'
+    for name, t in (('masks', masks), ('regions', regions)):
+        if not isinstance(t, torch.Tensor):
+            raise TypeError(f'{what}: {name} must be a torch.Tensor, not {type(t).__name__}')
+        if t.dtype not in (torch.bool, torch.uint8):
+            raise TypeError(f'{what}: {name} must be bool or uint8, not {t.dtype}')
+    if masks.dim() not in (3, 4):
+        raise ValueError(f'{what}: masks must be [W, H, W\'] or [M, W, H, W\'], not {tuple(masks.shape)}')
+    if regions.dim() == 2:
+        regions = regions[None]
+    out_h, out_w = masks.shape[-2:]
+    if regions.dim() != 3 or tuple(regions.shape[1:]) != (out_h, out_w):
+        raise ValueError(f'{what}: regions of shape {tuple(regions.shape)} do not match the masks\' (R, {out_h}, '
+                         f'{out_w}) (a [{out_h}, {out_w}] region or a stack of them)')
+    _require_cuda(masks, what)
+    _require_cuda(regions, what)
+    if regions.device != masks.device:
+        raise ValueError(f'{what}: regions are on {regions.device}, the masks on {masks.device}')
+    if out_h * out_w > 1 << 24:
+        raise ValueError(f'{what}: a {out_h} x {out_w} mask is more than 2**24 pixels')
+    n_regions = regions.shape[0]
+    if n_regions > _native.MAX_REGIONS:
+        raise ValueError(f'{what}: {n_regions} regions > {_native.MAX_REGIONS}, the region limit of one call')
+    tol = _boundary_tolerances(tolerances, out_h, out_w, what)
+    lead = tuple(masks.shape[:-3])
+    n_words, dev = masks.shape[-3], masks.device
+    n_planes = n_words * (lead[0] if lead else 1)
+    if n_planes == 0 or n_regions == 0 or out_h * out_w == 0:
+        out = _boundary_outputs(lead, n_regions, n_words, len(tol), tol, dev, torch.zeros)
+        return out.cpu() if to_cpu else out
+    mask_bytes = masks.detach().contiguous().view(torch.uint8)
+    region_bytes = regions.detach().contiguous().view(torch.uint8)
+    flat = _boundary_outputs((n_planes,), n_regions, 1, len(tol), tol, dev)
+    scratch = _boundary_scratch(n_regions, n_planes, out_h, out_w, dev)
+    with torch.cuda.device(dev):
+        _native.mask_boundary(mask_bytes.data_ptr(), n_planes, out_h, out_w, region_bytes.data_ptr(), n_regions, tol,
+                              *_boundary_pointers(flat), scratch.data_ptr(), scratch.numel(), _stream_ptr(dev))
+    # the call's planes are (mask, word) in order, the plane axis first: move the word axis last
+    m, R, T = n_planes // n_words, n_regions, len(tol)
+    shaped = [flat.word_boundary.reshape(m, n_words),
+              flat.word_hits.reshape(m, n_words, T, R).permute(0, 2, 3, 1),
+              flat.region_hits.reshape(m, n_words, T, R).permute(0, 2, 3, 1),
+              flat.max_d2.reshape(m, n_words, R, 2).permute(0, 2, 1, 3),
+              flat.sum_dist.reshape(m, n_words, R, 2).permute(0, 2, 1, 3)]
+    shaped = [(t if lead else t[0]).contiguous() for t in shaped]
+    out = RegionBoundary(shaped[0], flat.region_boundary, *shaped[1:], flat.tolerances)
+    return out.cpu() if to_cpu else out
+

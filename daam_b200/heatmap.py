@@ -29,7 +29,7 @@ from . import _native
 from .utils import compute_token_merge_indices
 
 __all__ = ['GlobalHeatMap', 'RawHeatMapCollection', 'WordHeatMap', 'LayerSlab', 'GlobalHeatMapStack', 'TimeHeatMaps',
-           'ImageHeatMaps', 'LayerHeatMaps', 'FactorHeatMaps', 'HeadHeatMaps', 'RegionOverlap', 'RegionRanking', 'WordOverlap', 'RelationOverlap', 'WordInstances']
+           'ImageHeatMaps', 'LayerHeatMaps', 'FactorHeatMaps', 'HeadHeatMaps', 'RegionOverlap', 'RegionRanking', 'RegionBoundary', 'WordOverlap', 'RelationOverlap', 'WordInstances']
 
 RawHeatMapKey = Tuple[int, int, int]  # factor, layer, head
 
@@ -457,6 +457,36 @@ class GlobalHeatMap:
                                       absolute, word_idx, offset_idx, to_cpu, 'GlobalHeatMap.region_ranking')
         return wl.word_heat_maps(0), ranking.map(0)
 
+    def region_boundary(self, words, image, regions: torch.Tensor, threshold: float, tolerances=None,
+                        absolute: bool = False, word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
+        """Where each word's mask boundary lies against each image region's boundary: the boundary F-measure at pixel
+        tolerances, the Hausdorff distance and the average symmetric surface distance, exact, for every (word, region)
+        pair at once. With ``A`` the mask ``expand_words(words, image, absolute, threshold, word_idx=word_idx,
+        offset_idx=offset_idx)`` returns for a word, ``B`` the pixels where ``regions[r] != 0``, ``dM`` the pixels of a
+        mask ``M`` with a 4-neighbour outside ``M`` or outside the image, and ``d2`` the squared Euclidean distance
+        between pixel centres to the nearest pixel of the other boundary, the :class:`RegionBoundary` holds
+        ``word_boundary[w] = |dA|``, ``region_boundary[r] = |dB|``, ``word_hits[k, r, w]`` (the ``dA`` pixels with
+        ``d2 <= tolerances[k]**2``), ``region_hits[k, r, w]`` (the ``dB`` pixels likewise), ``max_d2[r, w]`` and
+        ``sum_dist[r, w]`` (both directions); ``f_score()``, ``hausdorff()`` and ``assd()`` are the scores. Every
+        boundary pixel's nearest boundary pixel of the other set is found on the device; the ``[len(words), H, W]``
+        stack never leaves it, and the results are the same bits on every call.
+
+        ``threshold`` is required (the masks are ``expand_words``' thresholded masks) and must be finite.
+        ``tolerances``: 1 to 16 pixel distances, finite, ``>= 0`` and strictly ascending after rounding to fp32; the
+        default ``None`` is DAVIS's rule, one tolerance ``ceil(0.008 * sqrt(H**2 + W**2))`` (6 px at 512 x 512, 12 px
+        at 1024 x 1024). The boundary here is the 4-neighbour boundary; DAVIS's toolkit thins and resizes its
+        boundaries, so its F can differ slightly.
+
+        Returns ``(word_heat_maps, boundary)``: the list of :class:`WordHeatMap` that :meth:`segment` returns and the
+        :class:`RegionBoundary` (CPU by default, ``to_cpu=False`` keeps it on the device). A ``[H, W]`` region is one
+        region. At most 96 words, 63 regions and 2**24 image pixels. An empty word list or region set launches nothing,
+        returns no word heat maps and scores no word (a word axis of length 0). Raises the reference's ``ValueError``
+        for a word that is not in the prompt."""
+        wl, boundary = _region_boundary(self.tokenizer, self.prompt, self.heat_maps[None], words, image, regions,
+                                        threshold, tolerances, absolute, word_idx, offset_idx, to_cpu,
+                                        'GlobalHeatMap.region_boundary')
+        return wl.word_heat_maps(0), boundary.map(0)
+
     def word_overlap(self, words, image=None, absolute: bool = False, threshold: Optional[float] = None,
                      word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
         """How much each word's expanded map overlaps every other word's: the sums behind ``compute_iou`` /
@@ -830,6 +860,162 @@ def _region_ranking(tokenizer, prompt: str, maps: torch.Tensor, words, image, re
     return wl.done(RegionRanking(u2, ap, (region_bytes != 0).sum((-1, -2)), out_h * out_w))
 
 
+# Scratch of one region_boundary / boundary_scores call: the regions' column distances (about 4 bytes a pixel per
+# region) once, then as many planes as fit per round (about 8 bytes a pixel each), so memory does not grow with the
+# number of maps. The regions' state alone can exceed the budget -- 63 regions at 1024 x 1024 take about 264 MB -- and
+# the call then takes the regions and one plane, whatever the budget.
+REGION_BOUNDARY_SCRATCH_BYTES = 256 << 20
+
+
+@dataclass
+class RegionBoundary:
+    """Boundary scores of word masks against image regions (:meth:`GlobalHeatMap.region_boundary`,
+    :func:`daam_b200.evaluate.boundary_scores`). With ``dA`` a word mask's boundary, ``dB`` a region's and ``d2`` the
+    squared distance between pixel centres to the nearest pixel of the other boundary: ``word_boundary`` int32
+    ``[..., W]`` (``|dA|``), ``region_boundary`` int32 ``[R]`` (``|dB|``), ``word_hits`` / ``region_hits`` int32 ``[...,
+    T, R, W]`` (the ``dA`` / ``dB`` pixels within ``tolerances[k]``), ``max_d2`` int64 ``[..., R, W, 2]`` (the largest
+    ``d2`` from ``dA`` and from ``dB``; -1 when either boundary is empty), ``sum_dist`` float64 ``[..., R, W, 2]`` (the
+    sums of ``sqrt(d2)``; 0 when either boundary is empty) and ``tolerances`` fp32 ``[T]``. ``...`` is the map axis of a
+    :class:`GlobalHeatMapStack`, absent for one map."""
+    word_boundary: torch.Tensor
+    region_boundary: torch.Tensor
+    word_hits: torch.Tensor
+    region_hits: torch.Tensor
+    max_d2: torch.Tensor
+    sum_dist: torch.Tensor
+    tolerances: torch.Tensor
+
+    def map(self, i: int) -> 'RegionBoundary':
+        """The scores of map ``i`` of a stack (``region_boundary`` and ``tolerances`` have no map axis and stay whole)."""
+        return RegionBoundary(self.word_boundary[i], self.region_boundary, self.word_hits[i], self.region_hits[i],
+                              self.max_d2[i], self.sum_dist[i], self.tolerances)
+
+    def cpu(self) -> 'RegionBoundary':
+        return RegionBoundary(self.word_boundary.cpu(), self.region_boundary.cpu(), self.word_hits.cpu(),
+                              self.region_hits.cpu(), self.max_d2.cpu(), self.sum_dist.cpu(), self.tolerances.cpu())
+
+    def _sizes(self):
+        """``(|dA|, |dB|)`` as float64, broadcastable to ``[..., R, W]``."""
+        dev = self.word_hits.device
+        n_a = self.word_boundary.to(device=dev, dtype=torch.float64).unsqueeze(-2)
+        n_b = self.region_boundary.to(device=dev, dtype=torch.float64).unsqueeze(-1)
+        return n_a, n_b
+
+    def precision(self) -> torch.Tensor:
+        """float64 ``[..., T, R, W]``: ``word_hits / |dA|``, the share of the word's boundary within the tolerance of
+        the region's; 1 when ``dA`` is empty (DAVIS's ``f_measure``)."""
+        n_a, _ = self._sizes()
+        n_a = n_a.unsqueeze(-3)
+        return torch.where(n_a > 0, self.word_hits.double() / n_a.clamp(min=1), torch.ones_like(n_a))
+
+    def recall(self) -> torch.Tensor:
+        """float64 ``[..., T, R, W]``: ``region_hits / |dB|``, the share of the region's boundary within the tolerance
+        of the word's; 1 when ``dB`` is empty."""
+        _, n_b = self._sizes()
+        n_b = n_b.unsqueeze(-3)
+        return torch.where(n_b > 0, self.region_hits.double() / n_b.clamp(min=1), torch.ones_like(n_b))
+
+    def f_score(self) -> torch.Tensor:
+        """float64 ``[..., T, R, W]``: the boundary F-measure ``2 P R / (P + R)``, 0 when ``P + R = 0``."""
+        p, r = self.precision(), self.recall()
+        s = p + r
+        return torch.where(s > 0, 2 * p * r / torch.where(s > 0, s, torch.ones_like(s)), torch.zeros_like(s))
+
+    def hausdorff(self) -> torch.Tensor:
+        """float64 ``[..., R, W]``: the Hausdorff distance between the boundaries, ``sqrt`` of the larger ``max_d2``;
+        NaN when either boundary is empty."""
+        m = self.max_d2.max(-1).values
+        return torch.where(m >= 0, m.clamp(min=0).double().sqrt(), torch.full_like(m, float('nan'), dtype=torch.float64))
+
+    def assd(self) -> torch.Tensor:
+        """float64 ``[..., R, W]``: the average symmetric surface distance, both directions' sums of distances over
+        ``|dA| + |dB|``; NaN when either boundary is empty."""
+        n_a, n_b = self._sizes()
+        n_a, n_b = torch.broadcast_tensors(n_a, n_b)
+        both = (n_a > 0) & (n_b > 0)
+        return torch.where(both, self.sum_dist.sum(-1) / (n_a + n_b).clamp(min=1),
+                           torch.full_like(n_a, float('nan')))
+
+
+def _boundary_tolerances(tolerances, out_h: int, out_w: int, what: str) -> List[float]:
+    """``tolerances`` (a sequence of numbers or a 1-D CPU tensor; ``None``: DAVIS's ``ceil(0.008 * diagonal)``) rounded
+    to fp32, as the Python floats of those fp32 values; a ``ValueError`` unless they are 1 to 16 finite values ``>= 0``,
+    strictly ascending after the rounding."""
+    if tolerances is None:
+        return [float(math.ceil(0.008 * math.hypot(out_h, out_w)))]
+    if isinstance(tolerances, torch.Tensor):
+        if tolerances.device.type != 'cpu' or tolerances.dim() != 1 or tolerances.dtype == torch.bool \
+                or tolerances.is_complex():
+            raise ValueError(f'{what}: tolerances must be a 1-D real CPU tensor, not {tolerances.dim()}-D '
+                             f'{tolerances.dtype} on {tolerances.device}')
+        tol = tolerances.detach().to(torch.float32)
+    else:
+        try:
+            values = list(tolerances)
+        except TypeError:
+            raise ValueError(f'{what}: tolerances must be a sequence of numbers, not {tolerances!r}') from None
+        if not all(isinstance(x, numbers.Real) and not isinstance(x, bool) for x in values):
+            raise ValueError(f'{what}: tolerances must be numbers, not {values!r}')
+        tol = torch.tensor([float(x) for x in values], dtype=torch.float64).to(torch.float32)
+    n = tol.numel()
+    if not 1 <= n <= _native.BOUNDARY_MAX_TOLERANCES:
+        raise ValueError(f'{what}: {n} tolerances; a call takes 1 to {_native.BOUNDARY_MAX_TOLERANCES}')
+    if not bool((torch.isfinite(tol) & (tol >= 0)).all()):
+        raise ValueError(f'{what}: tolerances must be finite and >= 0 in fp32, not {tol.tolist()}')
+    if not bool((tol[1:] > tol[:-1]).all()):
+        raise ValueError(f'{what}: tolerances must be strictly ascending after rounding to fp32, not {tol.tolist()}')
+    return tol.tolist()
+
+
+def _boundary_outputs(lead: Tuple[int, ...], n_regions: int, n_words: int, n_tol: int, tol: List[float], dev,
+                      new=torch.empty) -> RegionBoundary:
+    """The buffers of a :class:`RegionBoundary` with leading axes ``lead`` (``new``: ``torch.zeros`` for a call that
+    launches nothing)."""
+    i32 = dict(dtype=torch.int32, device=dev)
+    return RegionBoundary(new((*lead, n_words), **i32), new((n_regions,), **i32),
+                          new((*lead, n_tol, n_regions, n_words), **i32), new((*lead, n_tol, n_regions, n_words), **i32),
+                          new((*lead, n_regions, n_words, 2), dtype=torch.int64, device=dev),
+                          new((*lead, n_regions, n_words, 2), dtype=torch.float64, device=dev),
+                          torch.tensor(tol, dtype=torch.float32, device=dev))
+
+
+def _boundary_scratch(n_regions: int, n_planes: int, out_h: int, out_w: int, dev) -> torch.Tensor:
+    """:data:`REGION_BOUNDARY_SCRATCH_BYTES` clipped to the planes the call has, at least the regions and one plane."""
+    n_bytes = max(_native.boundary_scratch_bytes(n_regions, 1, out_h, out_w),
+                  min(REGION_BOUNDARY_SCRATCH_BYTES, _native.boundary_scratch_bytes(n_regions, n_planes, out_h, out_w)))
+    return torch.empty(n_bytes, dtype=torch.uint8, device=dev)
+
+
+def _boundary_pointers(b: RegionBoundary):
+    return (b.word_boundary.data_ptr(), b.region_boundary.data_ptr(), b.word_hits.data_ptr(), b.region_hits.data_ptr(),
+            b.max_d2.data_ptr(), b.sum_dist.data_ptr())
+
+
+def _region_boundary(tokenizer, prompt: str, maps: torch.Tensor, words, image, regions, threshold, tolerances,
+                     absolute, word_idx, offset_idx: int, to_cpu: bool, what: str):
+    """``daam_region_boundary`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(wl, boundary)``, the
+    :class:`_WordList` and the :class:`RegionBoundary` with a leading map axis. Checks as ``_region_overlap``, in its
+    order, then the threshold (set, truthy and finite) and the tolerances. Scratch: :func:`_boundary_scratch`."""
+    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, image, absolute, threshold, to_cpu, what)
+    n_maps, out_h, out_w, dev = wl.n_maps, wl.out_h, wl.out_w, wl.dev
+    region_bytes = _region_bytes(wl, regions, what)
+    if not threshold:
+        raise ValueError(f'{what}: threshold must be set (truthy), not {threshold!r}: the word masks are the masks '
+                         f'expand_words(..., threshold) returns')
+    if not math.isfinite(float(threshold)):
+        raise ValueError(f'{what}: threshold must be finite, not {threshold!r}')
+    tol = _boundary_tolerances(tolerances, out_h, out_w, what)
+    n_regions, n_words = region_bytes.shape[0], len(wl.words)
+    if wl.empty or n_regions == 0:            # no word is scored: the call returns no word heat maps
+        _no_region_overlap(wl, (), n_regions)
+        return wl.done(_boundary_outputs((n_maps,), n_regions, 0, len(tol), tol, dev, torch.zeros))
+    out = _boundary_outputs((n_maps,), n_regions, n_words, len(tol), tol, dev)
+    scratch = _boundary_scratch(n_regions, n_maps * n_words, out_h, out_w, dev)
+    wl.launch(_native.region_boundary, tol, wl.word_maps.data_ptr(), region_bytes.data_ptr(), n_regions,
+              *_boundary_pointers(out), scratch.data_ptr(), scratch.numel())
+    return wl.done(out)
+
+
 @dataclass
 class WordOverlap:
     """Sums of products of word maps (:meth:`GlobalHeatMap.word_overlap`): ``intersection`` ``[..., W, W]``
@@ -1188,6 +1374,19 @@ class GlobalHeatMapStack:
         wl, ranking = _region_ranking(self.tokenizer, self.prompt, self.heat_maps, words, image, regions, absolute,
                                       word_idx, offset_idx, to_cpu, f'{type(self).__name__}.region_ranking')
         return wl.word_maps, ranking
+
+    def region_boundary(self, words, image, regions: torch.Tensor, threshold: float, tolerances=None,
+                        absolute: bool = False, word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
+        """:meth:`GlobalHeatMap.region_boundary` for every map in one call: returns ``(word_maps, boundary)`` with
+        ``word_maps`` the device ``[maps, len(words), xh, xw]`` word heat maps and ``boundary`` a
+        :class:`RegionBoundary` with a leading map axis (``word_hits`` ``[maps, T, R, W]``, ``max_d2`` ``[maps, R, W,
+        2]``, ...); row ``t`` equals ``self[t].region_boundary(...)`` bit for bit (min / max normalisation per map and
+        word). E.g. ``boundary.f_score()[:, 0, 0, 0]`` is word 0's boundary F against region 0 at every step of a
+        history. Scratch stays within a fixed budget whatever the map count: the planes are scored in rounds."""
+        wl, boundary = _region_boundary(self.tokenizer, self.prompt, self.heat_maps, words, image, regions, threshold,
+                                        tolerances, absolute, word_idx, offset_idx, to_cpu,
+                                        f'{type(self).__name__}.region_boundary')
+        return wl.word_maps, boundary
 
     def word_overlap(self, words, image=None, absolute: bool = False, threshold: Optional[float] = None,
                      word_idx=None, offset_idx: int = 0, to_cpu: bool = True):

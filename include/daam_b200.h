@@ -36,7 +36,8 @@ extern "C" {
                                           daam_region_overlap; daam_overlay_words, daam_jet_colormap;
                                           daam_finalize_parts; daam_word_overlap;
                                           daam_word_instances; daam_region_sweep;
-                                          daam_region_ranking; daam_refine_words) */
+                                          daam_region_ranking; daam_refine_words;
+                                          daam_region_boundary, daam_mask_boundary) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_TOKENS 231     /* daam_accumulate: long contexts of 2 or 3 CLIP chunks of 77 tokens (154, 231) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
@@ -543,6 +544,68 @@ int daam_refine_words(const float* global_maps, int32_t n_maps, int32_t n_rows, 
                       int32_t absolute, int32_t use_threshold, float threshold, int32_t radius, float eps,
                       float* word_maps, const uint8_t* image, int64_t image_map_stride, float* out, void* scratch,
                       int64_t scratch_bytes, void* stream);
+
+/*
+ * Boundary scores: where each word's mask boundary lies against each of n_regions binary image regions, on each of
+ * n_maps global maps stored back to back -- the boundary F-measure at pixel tolerances (DAVIS's contour accuracy,
+ * Csurka et al.'s BF score), the Hausdorff distance and the average symmetric surface distance. With A the mask
+ * m[w] > threshold (m what daam_expand_words writes for word w WITHOUT threshold, same rows / row_begin / absolute:
+ * exactly daam_expand_words' thresholded mask), B_r = {p : regions[r][p] != 0}, the boundary of a mask M
+ * dM = {p in M : a 4-neighbour of p is outside M or outside the image}, d2(p, S) = min_{q in S} (p_y - q_y)^2 +
+ * (p_x - q_x)^2 (an exact integer between pixel centres) and theta_k = tolerances[k] (host fp32, compared as
+ * d2 <= theta_k^2 in float64, exactly):
+ *   word_boundary[i][w]      = |dA|                                                 (int32 [n_maps][n_words])
+ *   region_boundary[r]       = |dB_r|                                               (int32 [n_regions])
+ *   word_hits[i][k][r][w]    = #{p in dA : d2(p, dB_r) <= theta_k^2}    (int32 [n_maps][n_tolerances][n_regions][n_words])
+ *   region_hits[i][k][r][w]  = #{q in dB_r : d2(q, dA) <= theta_k^2}    (int32, same shape)
+ *   max_d2[i][r][w][0 / 1]   = max over dA of d2(., dB_r) / over dB_r of d2(., dA); -1 in both when dA or dB_r is
+ *                              empty                                     (int64 [n_maps][n_regions][n_words][2])
+ *   sum_dist[i][r][w][0 / 1] = the same two directions, sum of sqrt(d2), each root in float64; 0 when dA or dB_r is
+ *                              empty                                     (double, same shape)
+ * Boundary precision is word_hits / |dA|, recall region_hits / |dB_r|, the Hausdorff distance sqrt(max of max_d2) and
+ * the ASSD (sum of sum_dist) / (|dA| + |dB_r|). Arguments as daam_region_ranking, plus threshold (finite, always in
+ * effect) and 1 <= n_tolerances <= 16 tolerances, finite, >= 0 and strictly ascending; the outputs on the device.
+ * scratch: device, 8-byte aligned, at least DAAM_BOUNDARY_SCRATCH_BYTES(n_regions, 1, out_h, out_w):
+ * DAAM_BOUNDARY_CALL_BYTES(n_regions, out_h, out_w) for the regions' column distances (about 4 bytes a pixel per
+ * region), then DAAM_BOUNDARY_PLANE_BYTES(out_h, out_w) (about 8 bytes a pixel) per (map, word) plane of a round. As
+ * many planes go in a round as the scratch holds, whole maps while a map's planes fit, and the call loops over the
+ * rounds: two memsets and one launch (the regions' boundaries and column distances), then five launches a round (the
+ * values, the planes' boundaries and column distances, one query pass that finds every boundary pixel's nearest
+ * boundary pixel of the other set, and a fixed-order reduction). The results are the same bits whatever the scratch
+ * and on every call: no float atomics, every sum in an order fixed by pixel positions.
+ * Limits (DAAM_E_UNSUPPORTED): those of daam_region_ranking, plus n_tolerances <= 16. DAAM_E_INVALID: as
+ * daam_region_ranking, plus a bad tolerance list, a non-finite threshold, scratch not 8-byte aligned or scratch_bytes
+ * below DAAM_BOUNDARY_SCRATCH_BYTES(n_regions, 1, out_h, out_w).
+ */
+#define DAAM_BOUNDARY_MAX_TOLERANCES 16
+/* rows of one query tile: 16, or enough for 4096 pixels on narrow images; one tile's partials take 10080 bytes */
+#define DAAM_BOUNDARY_TILE_ROWS(out_w) ((out_w) >= 256 ? 16 : (4096 + (int64_t)(out_w) - 1) / (out_w))
+#define DAAM_BOUNDARY_CALL_BYTES(n_regions, out_h, out_w)                                                             \
+  (8 * (int64_t)(n_regions) * (((int64_t)(out_h) * (out_w) + 1) / 2))
+#define DAAM_BOUNDARY_PLANE_BYTES(out_h, out_w)                                                                       \
+  (16 * (((int64_t)(out_h) * (out_w) + 1) / 2) + 256 +                                                                \
+   10080 * (((int64_t)(out_h) + DAAM_BOUNDARY_TILE_ROWS(out_w) - 1) / DAAM_BOUNDARY_TILE_ROWS(out_w)))
+#define DAAM_BOUNDARY_SCRATCH_BYTES(n_regions, n_planes, out_h, out_w)                                                \
+  (DAAM_BOUNDARY_CALL_BYTES(n_regions, out_h, out_w) + (int64_t)(n_planes) * DAAM_BOUNDARY_PLANE_BYTES(out_h, out_w))
+int daam_region_boundary(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t map_h, int32_t map_w,
+                         const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w,
+                         int32_t absolute, float threshold, const float* tolerances, int32_t n_tolerances,
+                         float* word_maps, const uint8_t* regions, int32_t n_regions, int32_t* word_boundary,
+                         int32_t* region_boundary, int32_t* word_hits, int32_t* region_hits, int64_t* max_d2,
+                         double* sum_dist, void* scratch, int64_t scratch_bytes, void* stream);
+
+/*
+ * Boundary scores of n_planes device masks: daam_region_boundary with A = {p : masks[i][p] != 0} (masks: device uint8
+ * [n_planes][out_h][out_w]) and n_maps * n_words replaced by n_planes in every output shape (word_boundary [n_planes],
+ * word_hits [n_planes][n_tolerances][n_regions], max_d2 [n_planes][n_regions][2], ...). Scratch as daam_region_boundary
+ * with n_planes planes; one launch per call and three a round. Limits: n_regions <= 63, out_h * out_w <= 2^24,
+ * n_tolerances <= 16. DAAM_E_INVALID: a null pointer or non-positive size, a bad tolerance list, scratch not 8-byte
+ * aligned or below DAAM_BOUNDARY_SCRATCH_BYTES(n_regions, 1, out_h, out_w).
+ */
+int daam_mask_boundary(const uint8_t* masks, int32_t n_planes, int32_t out_h, int32_t out_w, const uint8_t* regions,
+                       int32_t n_regions, const float* tolerances, int32_t n_tolerances, int32_t* word_boundary,
+                       int32_t* region_boundary, int32_t* word_hits, int32_t* region_hits, int64_t* max_d2,
+                       double* sum_dist, void* scratch, int64_t scratch_bytes, void* stream);
 
 /* Library / device introspection. */
 int daam_abi_version(void);
