@@ -99,6 +99,22 @@ def refine_scratch_bytes(n_images: int, n_planes: int, out_h: int, out_w: int) -
     return n_images * refine_guide_bytes(out_h, out_w) + n_planes * refine_plane_bytes(out_h, out_w)
 
 
+CRF_MAX_RADIUS = 16          # DAAM_CRF_MAX_RADIUS: the largest radius of daam_segment_crf
+CRF_MAX_ITERATIONS = 64      # the most mean-field updates daam_segment_crf takes
+
+
+def crf_map_bytes(n_labels: int, out_h: int, out_w: int) -> int:
+    """``DAAM_CRF_MAP_BYTES(n_labels, out_h, out_w)``: the scratch bytes daam_segment_crf takes per map of a round (two
+    fp32 Q buffers and the min / max partials)."""
+    return 8 * n_labels * out_h * out_w + 256 * n_labels
+
+
+def crf_scratch_bytes(n_maps: int, n_labels: int, out_h: int, out_w: int) -> int:
+    """``DAAM_CRF_SCRATCH_BYTES(n_maps, n_labels, out_h, out_w)``: ``n_maps`` maps; ``n_maps = 1`` is the smallest
+    scratch the call takes."""
+    return n_maps * crf_map_bytes(n_labels, out_h, out_w)
+
+
 BOUNDARY_MAX_TOLERANCES = 16  # DAAM_BOUNDARY_MAX_TOLERANCES: tolerances of daam_region_boundary / daam_mask_boundary
 
 
@@ -132,7 +148,7 @@ def overlay_frames_bytes(n_maps: int, n_words: int, out_h: int, out_w: int) -> i
 
 EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize',
            'daam_finalize_maps', 'daam_finalize_parts', 'daam_finalize_per_key','daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
-           'daam_segment_words', 'daam_region_overlap', 'daam_region_sweep', 'daam_region_ranking', 'daam_region_boundary', 'daam_mask_boundary', 'daam_word_overlap', 'daam_word_instances', 'daam_overlay_words', 'daam_refine_words', 'daam_jet_colormap',
+           'daam_segment_words', 'daam_region_overlap', 'daam_region_sweep', 'daam_region_ranking', 'daam_region_boundary', 'daam_mask_boundary', 'daam_word_overlap', 'daam_word_instances', 'daam_overlay_words', 'daam_refine_words', 'daam_segment_crf', 'daam_jet_colormap',
            'daam_side_launcher_create', 'daam_side_launcher_destroy',
            'daam_side_launcher_launch', 'daam_side_launcher_join', 'daam_side_launcher_idle', 'daam_abi_version',
            'daam_last_error', 'daam_device_info', 'daam_launch_count')
@@ -264,6 +280,10 @@ def load() -> ctypes.CDLL:
     lib.daam_refine_words.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
                                       i32, i32, f32, i32, f32, vp, vp, i64, vp, vp, i64, vp]
     lib.daam_refine_words.restype = ctypes.c_int
+    lib.daam_segment_crf.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
+                                     i32, i32, f32, f32, i32, i32, f32, f32, f32, f32, f32, vp, vp, i64, vp, vp, vp, vp,
+                                     i64, vp]
+    lib.daam_segment_crf.restype = ctypes.c_int
     lib.daam_jet_colormap.argtypes = [vp]
     lib.daam_jet_colormap.restype = ctypes.c_int
     lib.daam_side_launcher_create.argtypes = [ctypes.POINTER(vp)]
@@ -631,6 +651,24 @@ def refine_words(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequ
                                     *_word_list(x, rows_per_word, out_h, out_w, absolute, threshold), int(radius),
                                     float(eps), vp(word_maps_ptr), vp(image_ptr), image_map_stride, vp(out_ptr),
                                     vp(scratch_ptr), scratch_bytes, vp(stream)))
+
+
+def segment_crf(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int,
+                out_w: int, absolute: bool, threshold: Optional[float], scale: float, iterations: int, radius: int,
+                appearance: float, sigma_xy: float, sigma_rgb: float, smoothness: float, sigma_smooth: float,
+                word_maps_ptr: int, image_ptr: int, image_map_stride: int, labels_ptr: int, scores_ptr: int,
+                probs_ptr: int, scratch_ptr: int, scratch_bytes: int, stream: int):
+    """``daam_segment_crf`` over ``n_maps`` maps ``[n_rows, h, w]`` back to back; ``image_ptr`` uint8 ``[out_h, out_w,
+    3]``, map ``i``'s at ``image_ptr + i * image_map_stride`` bytes (0: one image for all); ``labels`` uint8 and
+    ``scores`` fp32 ``[n_maps, out_h, out_w]``; ``probs_ptr`` fp32 ``[n_maps, L, out_h, out_w]`` or 0;
+    ``scratch_bytes`` of scratch, at least :func:`crf_scratch_bytes` ``(1, L, ...)``."""
+    vp = ctypes.c_void_p
+    _check(load().daam_segment_crf(vp(maps_ptr), n_maps, n_rows,
+                                   *_word_list(x, rows_per_word, out_h, out_w, absolute, threshold), float(scale),
+                                   int(iterations), int(radius), float(appearance), float(sigma_xy), float(sigma_rgb),
+                                   float(smoothness), float(sigma_smooth), vp(word_maps_ptr), vp(image_ptr),
+                                   image_map_stride, vp(labels_ptr), vp(scores_ptr), vp(probs_ptr) if probs_ptr else None,
+                                   vp(scratch_ptr), scratch_bytes, vp(stream)))
 
 
 def jet_colormap():

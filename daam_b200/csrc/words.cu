@@ -20,7 +20,9 @@
 //    for ranking.cu, which sorts it and scores it against regions (daam_region_ranking), and for boundary.cu, which
 //    measures the boundary of m > threshold against the regions' boundaries (daam_region_boundary);
 //  - refine.cu recomputes it from segment_minmax_kernel's word maps and partials and filters it with the image as
-//    guide (daam_refine_words).
+//    guide (daam_refine_words);
+//  - crf.cu recomputes it the same way as the unary logits of a Potts CRF with the image as bilateral guide
+//    (daam_segment_crf).
 // The tile kernels run after segment_minmax_kernel (steps 1 and 2, the word maps and min / max partials to global
 // memory); region_tile_kernel, region_sweep_tile_kernel, overlay_kernel, word_pair_tile_kernel and instance_mask_kernel share the tile helpers
 // (block_tile / tile_at, word_bounds, stage_windows, tap tables). expand_words_kernel, segment_minmax_kernel and segment_label_kernel keep
@@ -37,6 +39,7 @@
 #include "boundary.cuh"
 #include "common.cuh"
 #include "components.cuh"
+#include "crf.cuh"
 #include "ranking.cuh"
 #include "refine.cuh"
 
@@ -1173,7 +1176,7 @@ static int tile_count(const WordListParams& p) {
   return ((p.oh + kSegTileH - 1) / kSegTileH) * ((p.ow + kSegTileW - 1) / kSegTileW);
 }
 
-// Launch 1 of the tile entry points, and all of it for daam_refine_words: segment_minmax_kernel over (map, word, chunk)
+// Launch 1 of the tile entry points, and all of it for daam_refine_words and daam_segment_crf: segment_minmax_kernel over (map, word, chunk)
 // with enough CTAs for a few waves, at most kMaxChunks per word and one per 256 pixels. Sets p.chunks.
 static int launch_word_maps(WordListParams& p, int n_maps, const DeviceInfo& dev, cudaStream_t stream) {
   const long long n = (long long)p.oh * p.ow, mwords = (long long)n_maps * p.n_words;
@@ -1557,6 +1560,62 @@ extern "C" int daam_refine_words(const float* global_maps, int32_t n_maps, int32
       }
       if (int rc = launch_refine(c, dev.device, stream)) return rc;
     }
+  }
+  return DAAM_OK;
+}
+
+extern "C" int daam_segment_crf(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t mh, int32_t mw,
+                                const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h,
+                                int32_t out_w, int32_t absolute, int32_t use_threshold, float threshold, float scale,
+                                int32_t iterations, int32_t radius, float appearance, float sigma_xy, float sigma_rgb,
+                                float smoothness, float sigma_smooth, float* word_maps, const uint8_t* image,
+                                int64_t image_map_stride, uint8_t* labels, float* scores, float* probs, void* scratch,
+                                int64_t scratch_bytes, void* stream_) {
+  const char* name = "daam_segment_crf";
+  if (!global_maps || !rows || !row_begin || !word_maps || !image || !labels || !scores || !scratch || n_maps <= 0 ||
+      mh <= 0 || mw <= 0 || out_h <= 0 || out_w <= 0 || n_rows <= 0 || image_map_stride < 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
+  if (radius < 1 || radius > kCrfMaxRadius) { set_error("%s: radius %d is not in [1, %d]", name, radius, kCrfMaxRadius); return DAAM_E_INVALID; }
+  if (iterations < 0 || iterations > kCrfMaxIterations) { set_error("%s: iterations %d is not in [0, %d]", name, iterations, kCrfMaxIterations); return DAAM_E_INVALID; }
+  const float positive[] = {scale, sigma_xy, sigma_rgb, sigma_smooth};
+  const char* positive_names[] = {"scale", "sigma_xy", "sigma_rgb", "sigma_smooth"};
+  for (int i = 0; i < 4; ++i)
+    if (!(positive[i] > 0.f) || !isfinite(positive[i])) { set_error("%s: %s %g is not finite and > 0", name, positive_names[i], (double)positive[i]); return DAAM_E_INVALID; }
+  if (!(appearance >= 0.f) || !isfinite(appearance)) { set_error("%s: appearance %g is not finite and >= 0", name, (double)appearance); return DAAM_E_INVALID; }
+  if (!(smoothness >= 0.f) || !isfinite(smoothness)) { set_error("%s: smoothness %g is not finite and >= 0", name, (double)smoothness); return DAAM_E_INVALID; }
+  if (use_threshold && !isfinite(threshold)) { set_error("%s: threshold %g is not finite", name, (double)threshold); return DAAM_E_INVALID; }
+  if ((uintptr_t)scratch & 3) { set_error("%s: scratch must be 4-byte aligned", name); return DAAM_E_INVALID; }
+  const int n_labels = n_words + (use_threshold ? 1 : 0);
+  const long long map_bytes = crf_map_bytes(n_labels, out_h, out_w);
+  if (scratch_bytes < map_bytes) { set_error("%s: %lld scratch bytes < %lld, one %d-label %d x %d map", name, (long long)scratch_bytes, map_bytes, n_labels, out_h, out_w); return DAAM_E_INVALID; }
+  static thread_local WordListParams p, q;
+  DeviceInfo dev;
+  if (int rc = word_list_prepare(name, global_maps, n_maps, n_rows, mh, mw, rows, row_begin, n_words, out_h, out_w,
+                                 absolute, !absolute, 0, 0.f, word_maps, nullptr, true, p, &dev)) return rc;
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  // a round: as many whole maps as the scratch holds (a map's labels are coupled: it is never split)
+  const int maps_per_round = (int)std::min<long long>(std::min<long long>(scratch_bytes / map_bytes, 65535), n_maps);
+  static thread_local CrfParams c;
+  crf_tables(radius, appearance, sigma_xy, sigma_rgb, smoothness, sigma_smooth, c);
+  c.image_map_stride = image_map_stride;
+  c.n_words = n_words; c.n_labels = n_labels; c.mh = mh; c.mw = mw; c.oh = out_h; c.ow = out_w;
+  c.absolute = p.absolute; c.use_threshold = use_threshold ? 1 : 0; c.threshold = use_threshold ? threshold : 0.f;
+  c.scale = scale; c.radius = radius; c.q_in = nullptr;
+  const long long n = (long long)out_h * out_w;
+  float* minmax = static_cast<float*>(scratch);
+  float* q_a = minmax + (long long)kCrfChunkFloats * n_labels * maps_per_round;
+  float* q_b = q_a + (long long)n_labels * n * maps_per_round;
+  for (int map0 = 0; map0 < n_maps; map0 += maps_per_round) {
+    const int nm = std::min(maps_per_round, n_maps - map0);
+    q = p;
+    q.maps = global_maps + map0 * p.map_stride;
+    q.word_maps = word_maps + (long long)map0 * n_words * mh * mw;
+    q.scratch = minmax;
+    if (int rc = launch_word_maps(q, nm, dev, stream)) return rc;
+    c.word_maps = q.word_maps; c.minmax = minmax; c.chunks = q.chunks; c.maps = nm;
+    c.image = image + map0 * image_map_stride;
+    c.labels = labels + map0 * n; c.scores = scores + map0 * n;
+    if (int rc = launch_crf(c, iterations, q_a, q_b, probs ? probs + (long long)map0 * n_labels * n : nullptr,
+                            dev.device, stream)) return rc;
   }
   return DAAM_OK;
 }

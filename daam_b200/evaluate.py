@@ -27,7 +27,11 @@ and ``WordInstances.box_iou``, on one map or a stack. To refine the masks agains
 (word boundaries that follow the image's edges rather than the heat-map grid), use :meth:`GlobalHeatMap.refine_words
 <daam_b200.heatmap.GlobalHeatMap.refine_words>` / :meth:`GlobalHeatMapStack.refine_words
 <daam_b200.heatmap.GlobalHeatMapStack.refine_words>`: the guided filter of each word's map with the image as guide,
-fused on the device; score its result with :func:`compute_iou` or torch.
+fused on the device; score its result with :func:`compute_iou` or torch. To let the words compete for each pixel
+with the image's edges as a guide, use :meth:`GlobalHeatMap.segment_crf <daam_b200.heatmap.GlobalHeatMap.segment_crf>`
+/ :meth:`GlobalHeatMapStack.segment_crf <daam_b200.heatmap.GlobalHeatMapStack.segment_crf>`: mean-field inference of
+a Potts CRF over the word maps, a label per pixel as :meth:`GlobalHeatMap.segment` gives, whose ``labels == w + 1``
+masks score with :func:`boundary_scores` like any other.
 To measure where each word's boundary lies against each region's -- the boundary F-measure at pixel tolerances, the
 Hausdorff distance and the average symmetric surface distance, the scores a smeared or shifted boundary moves and IoU
 barely does -- use :meth:`GlobalHeatMap.region_boundary <daam_b200.heatmap.GlobalHeatMap.region_boundary>` /

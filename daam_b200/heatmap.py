@@ -583,6 +583,44 @@ class GlobalHeatMap:
                               threshold, word_idx, offset_idx, to_cpu, 'GlobalHeatMap.refine_words', stack=False)
         return wl.word_heat_maps(0), refined[0]
 
+    def segment_crf(self, words, image, threshold: Optional[float] = None, iterations: int = 5, radius: int = 8,
+                    scale: float = 16.0, appearance: float = 10.0, sigma_xy: float = 8.0, sigma_rgb: float = 13.0,
+                    smoothness: float = 1.0, sigma_smooth: float = 3.0, absolute: bool = False, word_idx=None,
+                    offset_idx: int = 0, probs: bool = False, to_cpu: bool = True):
+        """CRF-refined word segmentation: :meth:`segment`'s labels pulled onto the image's edges by mean-field
+        inference of a Potts CRF (Kraehenbuehl and Koltun, NeurIPS 2011, in the exact windowed form of Teichmann and
+        Cipolla's ConvCRF, BMVC 2019), in which the words compete with one another and with the background.
+
+        With ``m[w]`` what ``expand_words(words, image, absolute, word_idx=word_idx, offset_idx=offset_idx)`` returns
+        (no threshold): with ``threshold`` in effect (Python truthiness, as in :meth:`segment`) there are
+        ``L = len(words) + 1`` labels, label 0 the background with score ``threshold``; without it ``L = len(words)``
+        and no background. Word ``w`` is always label ``w + 1``, with score ``m[w]``. The unary logits are
+        ``z = scale * score`` (fp32). The pairwise kernel of pixels ``x`` and ``y`` in the ``(2 radius + 1)^2`` window
+        around ``x`` (clipped to the image, not renormalised at the border) is ``A[y - x] exp(-|I_x - I_y|^2 / 2
+        sigma_rgb^2) + S[y - x]``, ``I`` the RGB bytes, ``A`` a Gaussian of width ``sigma_xy`` scaled to sum to
+        ``appearance`` over the window's offsets and ``S`` one of width ``sigma_smooth`` summing to ``smoothness``
+        (computed in float64, rounded once to fp32). Then ``Q = softmax(z)`` and ``iterations`` parallel updates
+        ``Q = softmax(z + msg)``, ``msg_l(x) = sum_{y != x} k(x, y) Q_l(y)``.
+
+        Returns ``(word_heat_maps, labels, scores)``, plus ``probs`` when asked: the list of :class:`WordHeatMap` that
+        :meth:`segment` returns, ``labels`` uint8 ``(H, W)`` (the argmax of the last logits, the lowest label on
+        ties), ``scores`` fp32 ``(H, W)`` (the final ``Q`` of that label) and ``probs`` fp32 ``(L, H, W)`` (the final
+        ``Q``), CPU by default, ``to_cpu=False`` keeps them on the device. With ``iterations=0``, or ``appearance =
+        smoothness = 0``, and ``scale`` a power of two, ``labels`` equals :meth:`segment`'s bit for bit (the scaling
+        is exact and the tie rules match: the background wins at ``max m == threshold``, the first word otherwise).
+        Every sum runs in an order fixed by pixel positions, so the results are the same bits on every call.
+
+        ``image``: as :meth:`overlay_words` takes it. ``1 <= radius <= 16``, ``0 <= iterations <= 64``, ``scale``
+        and the sigmas (``sigma_rgb`` in byte units) finite and > 0, ``appearance`` and ``smoothness`` finite and
+        >= 0, a threshold in effect finite (a ``ValueError`` otherwise); at most 96 words. An empty word list
+        launches nothing: every pixel is background with score 1 when the threshold is in effect, label 0 with score
+        0 otherwise. Raises the reference's ``ValueError`` for a word that is not in the prompt."""
+        wl, labels, scores, *q = _segment_crf(self.tokenizer, self.prompt, self.heat_maps[None], words, image,
+                                              threshold, iterations, radius, scale, appearance, sigma_xy, sigma_rgb,
+                                              smoothness, sigma_smooth, absolute, word_idx, offset_idx, probs, to_cpu,
+                                              'GlobalHeatMap.segment_crf', stack=False)
+        return (wl.word_heat_maps(0), labels[0], scores[0]) + ((q[0][0],) if probs else ())
+
 
 def _check_rows(rows, n_rows: int):
     """Raises the ``IndexError`` torch's advanced indexing raises on a row out of ``[-n_rows, n_rows)``."""
@@ -1307,6 +1345,73 @@ def _refine(tokenizer, prompt: str, maps: torch.Tensor, words, image, radius, ep
     return wl.done(refined)
 
 
+# Scratch of one segment_crf call: two fp32 Q buffers per map (8 bytes a pixel per label) and the min / max partials;
+# as many whole maps as fit go in a round, so memory does not grow with the number of maps; one map larger than the
+# budget goes alone.
+CRF_SCRATCH_BYTES = 256 << 20
+
+
+def _crf_args(threshold, iterations, radius, scale, appearance, sigma_xy, sigma_rgb, smoothness, sigma_smooth,
+              what: str):
+    """Raises ``ValueError`` unless ``radius`` is an integer in ``[1, 16]``, ``iterations`` one in ``[0, 64]``, and,
+    rounded to fp32, ``scale`` and the sigmas are finite and > 0, ``appearance`` and ``smoothness`` finite and >= 0,
+    and a threshold in effect finite -- daam_segment_crf's checks, in its order."""
+    def whole(v, lo, hi, name):
+        if isinstance(v, bool) or not isinstance(v, int) or not lo <= v <= hi:
+            raise ValueError(f'{what}: {name} must be an integer in [{lo}, {hi}], not {v!r}')
+
+    def f32(v, name):
+        try:
+            return ctypes.c_float(float(v)).value
+        except (TypeError, ValueError):
+            raise ValueError(f'{what}: {name} must be a number, not {v!r}') from None
+
+    whole(radius, 1, _native.CRF_MAX_RADIUS, 'radius')
+    whole(iterations, 0, _native.CRF_MAX_ITERATIONS, 'iterations')
+    for name, v in (('scale', scale), ('sigma_xy', sigma_xy), ('sigma_rgb', sigma_rgb), ('sigma_smooth', sigma_smooth)):
+        v32 = f32(v, name)
+        if not (math.isfinite(v32) and v32 > 0):
+            raise ValueError(f'{what}: {name} must be finite and > 0 in fp32, not {v!r}')
+    for name, v in (('appearance', appearance), ('smoothness', smoothness)):
+        v32 = f32(v, name)
+        if not (math.isfinite(v32) and v32 >= 0):
+            raise ValueError(f'{what}: {name} must be finite and >= 0 in fp32, not {v!r}')
+    if threshold and not math.isfinite(f32(threshold, 'threshold')):
+        raise ValueError(f'{what}: threshold must be finite in fp32, not {threshold!r}')
+
+
+def _segment_crf(tokenizer, prompt: str, maps: torch.Tensor, words, image, threshold, iterations, radius, scale,
+                 appearance, sigma_xy, sigma_rgb, smoothness, sigma_smooth, absolute, word_idx, offset_idx: int,
+                 probs: bool, to_cpu: bool, what: str, stack: bool):
+    """``daam_segment_crf`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(wl, labels, scores)``, plus
+    ``probs`` fp32 ``[n_maps, L, H, W]`` when asked; ``labels`` uint8 and ``scores`` fp32 ``[n_maps, H, W]``. Checks as
+    :func:`_overlay`, in its order, then the CRF arguments (:func:`_crf_args`). Scratch: :data:`CRF_SCRATCH_BYTES`,
+    clipped to what the call has, at least one map."""
+    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, None, absolute, threshold, to_cpu, what,
+                   on_grid=True)         # the size is the image's, once _overlay_image has checked it
+    n_maps, n_words, dev = wl.n_maps, len(wl.words), wl.dev
+    image, wl.out_h, wl.out_w, per_map = _overlay_image(image, n_maps, wl.grid, dev, what, stack)
+    _crf_args(threshold, iterations, radius, scale, appearance, sigma_xy, sigma_rgb, smoothness, sigma_smooth, what)
+    n_labels = n_words + (1 if threshold else 0)
+    shape = (n_maps, wl.out_h, wl.out_w)
+    labels = torch.zeros(shape, dtype=torch.uint8, device=dev)
+    scores = torch.empty(shape, dtype=torch.float32, device=dev)
+    q = torch.empty((n_maps, n_labels, wl.out_h, wl.out_w), dtype=torch.float32, device=dev) if probs else None
+    if wl.empty:                         # only the background, if any: it takes every pixel with Q = 1
+        scores.fill_(1.0 if n_labels else 0.0)
+        if q is not None:
+            q.fill_(1.0)
+        return wl.done(labels, scores, *([q] if probs else []))
+    image = image.to(dev).contiguous()                   # one copy to the device
+    n_bytes = max(_native.crf_scratch_bytes(1, n_labels, wl.out_h, wl.out_w),
+                  min(CRF_SCRATCH_BYTES, _native.crf_scratch_bytes(n_maps, n_labels, wl.out_h, wl.out_w)))
+    scratch = torch.empty(n_bytes, dtype=torch.uint8, device=dev)
+    wl.launch(_native.segment_crf, scale, iterations, radius, appearance, sigma_xy, sigma_rgb, smoothness,
+              sigma_smooth, wl.word_maps.data_ptr(), image.data_ptr(), wl.out_h * wl.out_w * 3 if per_map else 0,
+              labels.data_ptr(), scores.data_ptr(), q.data_ptr() if probs else 0, scratch.data_ptr(), n_bytes)
+    return wl.done(labels, scores, *([q] if probs else []))
+
+
 class GlobalHeatMapStack:
     """Global heat maps of one prompt's text stacked along a first axis: ``heat_maps[t]`` is one
     ``[n_rows, xh, xw]`` map. Base of :class:`TimeHeatMaps` (one map per step), :class:`ImageHeatMaps` (one per
@@ -1443,6 +1548,22 @@ class GlobalHeatMapStack:
                               threshold, word_idx, offset_idx, to_cpu, f'{type(self).__name__}.refine_words',
                               stack=True)
         return wl.word_maps, refined
+
+    def segment_crf(self, words, image, threshold: Optional[float] = None, iterations: int = 5, radius: int = 8,
+                    scale: float = 16.0, appearance: float = 10.0, sigma_xy: float = 8.0, sigma_rgb: float = 13.0,
+                    smoothness: float = 1.0, sigma_smooth: float = 3.0, absolute: bool = False, word_idx=None,
+                    offset_idx: int = 0, probs: bool = False, to_cpu: bool = True):
+        """:meth:`GlobalHeatMap.segment_crf` for every map in one call: returns ``(word_maps, labels, scores)``, plus
+        ``probs`` when asked, with ``word_maps`` the device ``[maps, len(words), xh, xw]`` word heat maps, ``labels``
+        / ``scores`` ``[maps, H, W]`` and ``probs`` ``[maps, L, H, W]``; row ``t`` equals ``self[t].segment_crf(...)``
+        bit for bit (min / max normalisation per map and word). ``image`` is one image for every map, or a uint8
+        ``[maps, H, W, 3]`` array with one per map (e.g. the images of ``compute_image_heat_maps()``). Scratch stays
+        within a fixed budget whatever the map count: the maps go in rounds of whole maps."""
+        wl, labels, scores, *q = _segment_crf(self.tokenizer, self.prompt, self.heat_maps, words, image, threshold,
+                                              iterations, radius, scale, appearance, sigma_xy, sigma_rgb, smoothness,
+                                              sigma_smooth, absolute, word_idx, offset_idx, probs, to_cpu,
+                                              f'{type(self).__name__}.segment_crf', stack=True)
+        return (wl.word_maps, labels, scores) + tuple(q)
 
 
 class TimeHeatMaps(GlobalHeatMapStack):

@@ -37,7 +37,8 @@ extern "C" {
                                           daam_finalize_parts; daam_word_overlap;
                                           daam_word_instances; daam_region_sweep;
                                           daam_region_ranking; daam_refine_words;
-                                          daam_region_boundary, daam_mask_boundary) */
+                                          daam_region_boundary, daam_mask_boundary;
+                                          daam_segment_crf) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_TOKENS 231     /* daam_accumulate: long contexts of 2 or 3 CLIP chunks of 77 tokens (154, 231) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
@@ -606,6 +607,49 @@ int daam_mask_boundary(const uint8_t* masks, int32_t n_planes, int32_t out_h, in
                        int32_t n_regions, const float* tolerances, int32_t n_tolerances, int32_t* word_boundary,
                        int32_t* region_boundary, int32_t* word_hits, int32_t* region_hits, int64_t* max_d2,
                        double* sum_dist, void* scratch, int64_t scratch_bytes, void* stream);
+
+/*
+ * CRF-refined word segmentation: mean-field inference of a Potts CRF over a word list's maps with the image as a
+ * bilateral guide (Kraehenbuehl and Koltun, "Efficient Inference in Fully Connected CRFs with Gaussian Edge Potentials",
+ * NeurIPS 2011, in the exact windowed form of Teichmann and Cipolla, "Convolutional CRFs for Semantic Segmentation",
+ * BMVC 2019), on each of n_maps global maps stored back to back. With m[w] what daam_expand_words writes for word w
+ * WITHOUT threshold (same rows / row_begin / absolute):
+ *   labels: with use_threshold L = n_words + 1 and label 0 the background with score s_0 = threshold; without it
+ *           L = n_words and no background; word w is always label w + 1 with score s_{w+1} = m[w];
+ *   logits: z_l = scale * s_l in fp32;
+ *   tables: over the window offsets o != 0 with |o_y|, |o_x| <= radius, computed once per call in float64 and rounded
+ *           once to fp32, each normalised over the full window (logit units, whatever the radius):
+ *           A[o] = appearance exp(-|o|^2 / 2 sigma_xy^2) / sum_{o' != 0} exp(-|o'|^2 / 2 sigma_xy^2)
+ *           S[o] = smoothness exp(-|o|^2 / 2 sigma_smooth^2) / sum_{o' != 0} exp(-|o'|^2 / 2 sigma_smooth^2)
+ *   kernel: k(x, y) = A[y - x] exp(-|I_x - I_y|^2 / 2 sigma_rgb^2) + S[y - x], I the RGB bytes (|I_x - I_y|^2 is an
+ *           exact integer), over the window W(x) clipped to the image and not renormalised at the border;
+ *   mean field (parallel updates): Q^0 = softmax_l(z); each of `iterations` updates takes
+ *           msg_l(x) = sum_{y in W(x), y != x} k(x, y) Q_l(y), then Q' = softmax_l(z + msg).
+ * labels[i]: uint8 [n_maps][out_h][out_w], the output label (1 + w for word w, 0 for the background) of the argmax of
+ * the last logits (z when iterations = 0), the lowest label on ties; scores[i]: fp32, the final Q of that label;
+ * probs (may be NULL): fp32 [n_maps][L][out_h][out_w], the final Q. With iterations = 0, or appearance = smoothness =
+ * 0, and scale a power of two, labels equal daam_segment_words' bit for bit. The window walk has a fixed order, the
+ * softmax subtracts the max, takes expf and sums in label order, and there are no atomics: the results are the same
+ * bits on every call and whatever the scratch.
+ * Arguments as daam_overlay_words with color_normalize replaced by the CRF's, plus labels / scores / probs on the
+ * device. scratch: device, 4-byte aligned, at least DAAM_CRF_SCRATCH_BYTES(1, L, out_h, out_w): two fp32 Q buffers and
+ * the min / max partials per map (DAAM_CRF_MAP_BYTES). A map's labels are coupled, so a round takes as many whole maps
+ * as the scratch holds and the call loops over the rounds: 2 + iterations launches a round (the word maps, Q^0, one
+ * fused launch per update).
+ * Limits (DAAM_E_UNSUPPORTED): as daam_overlay_words. DAAM_E_INVALID: as daam_overlay_words, plus radius not in
+ * [1, DAAM_CRF_MAX_RADIUS], iterations not in [0, 64], scale or a sigma not finite and > 0, appearance or smoothness not
+ * finite and >= 0, a threshold in effect that is not finite, scratch not 4-byte aligned or scratch_bytes below one map.
+ * Checked in that order after the null pointers and sizes, and before the word list.
+ */
+#define DAAM_CRF_MAX_RADIUS 16
+#define DAAM_CRF_MAP_BYTES(n_labels, out_h, out_w) (8 * (int64_t)(n_labels) * (out_h) * (out_w) + 256 * (int64_t)(n_labels))
+#define DAAM_CRF_SCRATCH_BYTES(n_maps, n_labels, out_h, out_w) ((int64_t)(n_maps) * DAAM_CRF_MAP_BYTES(n_labels, out_h, out_w))
+int daam_segment_crf(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t map_h, int32_t map_w,
+                     const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w,
+                     int32_t absolute, int32_t use_threshold, float threshold, float scale, int32_t iterations,
+                     int32_t radius, float appearance, float sigma_xy, float sigma_rgb, float smoothness,
+                     float sigma_smooth, float* word_maps, const uint8_t* image, int64_t image_map_stride,
+                     uint8_t* labels, float* scores, float* probs, void* scratch, int64_t scratch_bytes, void* stream);
 
 /* Library / device introspection. */
 int daam_abi_version(void);
