@@ -141,6 +141,16 @@ def boundary_scratch_bytes(n_regions: int, n_planes: int, out_h: int, out_w: int
     return boundary_call_bytes(n_regions, out_h, out_w) + n_planes * boundary_plane_bytes(out_h, out_w)
 
 
+DISTANCE_NONE = 2 ** 31 - 1   # DAAM_DISTANCE_NONE: every pixel of an empty mask (+), of a full one (-)
+DISTANCE_MAX_SIDE = 32767     # DAAM_DISTANCE_MAX_SIDE: the largest out_h and out_w of the distance calls
+
+
+def distance_plane_bytes(out_h: int, out_w: int) -> int:
+    """``DAAM_DISTANCE_PLANE_BYTES(out_h, out_w)``: the scratch bytes daam_word_distance takes per (map, word) plane of a
+    round (its values and min / max partials)."""
+    return 4 * out_h * out_w + 256
+
+
 def overlay_frames_bytes(n_maps: int, n_words: int, out_h: int, out_w: int) -> int:
     """``DAAM_OVERLAY_FRAMES_BYTES(n_maps, n_words, out_h, out_w)``: the frames rounded up to whole 4-byte words."""
     return (n_maps * n_words * out_h * out_w * 3 + 3) // 4 * 4
@@ -148,7 +158,7 @@ def overlay_frames_bytes(n_maps: int, n_words: int, out_h: int, out_w: int) -> i
 
 EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize',
            'daam_finalize_maps', 'daam_finalize_parts', 'daam_finalize_per_key','daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
-           'daam_segment_words', 'daam_region_overlap', 'daam_region_sweep', 'daam_region_ranking', 'daam_region_boundary', 'daam_mask_boundary', 'daam_word_overlap', 'daam_word_instances', 'daam_overlay_words', 'daam_refine_words', 'daam_segment_crf', 'daam_jet_colormap',
+           'daam_segment_words', 'daam_region_overlap', 'daam_region_sweep', 'daam_region_ranking', 'daam_region_boundary', 'daam_mask_boundary', 'daam_word_overlap', 'daam_word_instances', 'daam_overlay_words', 'daam_refine_words', 'daam_segment_crf', 'daam_word_distance', 'daam_mask_distance', 'daam_jet_colormap',
            'daam_side_launcher_create', 'daam_side_launcher_destroy',
            'daam_side_launcher_launch', 'daam_side_launcher_join', 'daam_side_launcher_idle', 'daam_abi_version',
            'daam_last_error', 'daam_device_info', 'daam_launch_count')
@@ -284,6 +294,11 @@ def load() -> ctypes.CDLL:
                                      i32, i32, f32, f32, i32, i32, f32, f32, f32, f32, f32, vp, vp, i64, vp, vp, vp, vp,
                                      i64, vp]
     lib.daam_segment_crf.restype = ctypes.c_int
+    lib.daam_word_distance.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32, i32,
+                                       i32, f32, vp, vp, vp, i64, vp]
+    lib.daam_word_distance.restype = ctypes.c_int
+    lib.daam_mask_distance.argtypes = [vp, i32, i32, i32, vp, vp]
+    lib.daam_mask_distance.restype = ctypes.c_int
     lib.daam_jet_colormap.argtypes = [vp]
     lib.daam_jet_colormap.restype = ctypes.c_int
     lib.daam_side_launcher_create.argtypes = [ctypes.POINTER(vp)]
@@ -638,6 +653,26 @@ def mask_boundary(masks_ptr: int, n_planes: int, out_h: int, out_w: int, regions
                                      len(tolerances), vp(word_boundary_ptr), vp(region_boundary_ptr),
                                      vp(word_hits_ptr), vp(region_hits_ptr), vp(max_d2_ptr), vp(sum_dist_ptr),
                                      vp(scratch_ptr), scratch_bytes, vp(stream)))
+
+
+def word_distance(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int,
+                  out_w: int, absolute: bool, threshold: float, word_maps_ptr: int, signed_d2_ptr: int, scratch_ptr: int,
+                  scratch_bytes: int, stream: int):
+    """``daam_word_distance`` over ``n_maps`` maps ``[n_rows, h, w]`` back to back: ``signed_d2`` int32 ``[n_maps,
+    n_words, out_h, out_w]``; ``scratch_bytes`` of scratch, at least :func:`distance_plane_bytes`. The threshold is
+    always in effect: the call takes no ``use_threshold``."""
+    vp = ctypes.c_void_p
+    _check(load().daam_word_distance(vp(maps_ptr), n_maps, n_rows,
+                                     *_word_list(x, rows_per_word, out_h, out_w, absolute, None)[:-2],
+                                     float(threshold), vp(word_maps_ptr), vp(signed_d2_ptr), vp(scratch_ptr),
+                                     scratch_bytes, vp(stream)))
+
+
+def mask_distance(masks_ptr: int, n_planes: int, out_h: int, out_w: int, signed_d2_ptr: int, stream: int):
+    """``daam_mask_distance`` over ``n_planes`` uint8 masks ``[out_h, out_w]`` back to back: ``signed_d2`` int32
+    ``[n_planes, out_h, out_w]``; no scratch."""
+    vp = ctypes.c_void_p
+    _check(load().daam_mask_distance(vp(masks_ptr), n_planes, out_h, out_w, vp(signed_d2_ptr), vp(stream)))
 
 
 def refine_words(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]], out_h: int,

@@ -18,7 +18,8 @@
 //  - word_pair_tile_kernel sums m[a] * m[b] over every pair of words (then word_pair_reduce_kernel);
 //  - instance_mask_kernel writes it without threshold for components.cu, which labels the mask m > threshold, and
 //    for ranking.cu, which sorts it and scores it against regions (daam_region_ranking), and for boundary.cu, which
-//    measures the boundary of m > threshold against the regions' boundaries (daam_region_boundary);
+//    measures the boundary of m > threshold against the regions' boundaries (daam_region_boundary), and for
+//    distance.cu, which takes the signed distance transform of m > threshold (daam_word_distance);
 //  - refine.cu recomputes it from segment_minmax_kernel's word maps and partials and filters it with the image as
 //    guide (daam_refine_words);
 //  - crf.cu recomputes it the same way as the unary logits of a Potts CRF with the image as bilateral guide
@@ -40,6 +41,7 @@
 #include "common.cuh"
 #include "components.cuh"
 #include "crf.cuh"
+#include "distance.cuh"
 #include "ranking.cuh"
 #include "refine.cuh"
 
@@ -1499,6 +1501,49 @@ extern "C" int daam_region_boundary(const float* global_maps, int32_t n_maps, in
       if (int rc = launch_tiles(instance_mask_kernel, q, nm, dev, stream)) return rc;
       c.n_words_round = nw; c.map0 = map0; c.w0 = w0;
       if (int rc = launch_boundary_round(c, threshold, nullptr, stream)) return rc;
+    }
+  }
+  return DAAM_OK;
+}
+
+extern "C" int daam_word_distance(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t mh, int32_t mw,
+                                  const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h,
+                                  int32_t out_w, int32_t absolute, float threshold, float* word_maps,
+                                  int32_t* signed_d2, void* scratch, int64_t scratch_bytes, void* stream_) {
+  const char* name = "daam_word_distance";
+  if (!global_maps || !rows || !row_begin || !word_maps || !signed_d2 || !scratch || n_maps <= 0 || mh <= 0 ||
+      mw <= 0 || out_h <= 0 || out_w <= 0 || n_rows <= 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
+  if (out_h > kDistanceMaxSide || out_w > kDistanceMaxSide) { set_error("%s: a %d x %d output has a side > %d", name, out_h, out_w, kDistanceMaxSide); return DAAM_E_UNSUPPORTED; }
+  if ((long long)out_h * out_w > (1LL << 24)) { set_error("%s: a %d x %d output is more than 2^24 pixels", name, out_h, out_w); return DAAM_E_UNSUPPORTED; }
+  if (!isfinite(threshold)) { set_error("%s: threshold %g is not finite", name, (double)threshold); return DAAM_E_INVALID; }
+  if (int rc = distance_check_scratch(name, scratch, scratch_bytes, out_h, out_w)) return rc;
+  static thread_local InstanceMaskParams p, q;
+  DeviceInfo dev;
+  if (int rc = word_list_prepare(name, global_maps, n_maps, n_rows, mh, mw, rows, row_begin, n_words, out_h, out_w,
+                                 absolute, !absolute, 0, 0.f, word_maps, nullptr, true, p.s, &dev)) return rc;
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const long long n = (long long)out_h * out_w;
+  // a round: whole maps while a map's planes fit the scratch, else the words of one map in groups; either way the
+  // round's planes are consecutive in signed_d2
+  const int cap = (int)std::min<long long>(scratch_bytes / distance_plane_bytes(out_h, out_w), 65535);
+  const int maps_per_round = std::max(1, cap / n_words), words_per_round = std::min(cap, (int)n_words);
+  for (int map0 = 0; map0 < n_maps; map0 += maps_per_round) {
+    const int nm = std::min(maps_per_round, n_maps - map0);
+    for (int w0 = 0; w0 < n_words; w0 += words_per_round) {
+      const int nw = std::min(words_per_round, n_words - w0);
+      q = p;
+      q.s.maps = global_maps + map0 * p.s.map_stride;
+      q.s.n_words = nw;
+      for (int i = 0; i <= nw; ++i) q.s.row_begin[i] = p.s.row_begin[w0 + i];
+      const long long plane0 = (long long)map0 * n_words + w0;
+      q.s.word_maps = word_maps + plane0 * mh * mw;
+      DistancePlanes c;
+      distance_planes_in(scratch, nm * nw, out_h, out_w, c);
+      q.s.scratch = c.minmax;
+      q.pre = c.pre;
+      if (int rc = launch_tiles(instance_mask_kernel, q, nm, dev, stream)) return rc;
+      if (int rc = launch_distance(c.pre, threshold, nullptr, nm * nw, out_h, out_w, signed_d2 + plane0 * n, stream))
+        return rc;
     }
   }
   return DAAM_OK;

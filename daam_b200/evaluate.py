@@ -38,6 +38,10 @@ barely does -- use :meth:`GlobalHeatMap.region_boundary <daam_b200.heatmap.Globa
 :meth:`GlobalHeatMapStack.region_boundary <daam_b200.heatmap.GlobalHeatMapStack.region_boundary>` on the thresholded
 word masks, or :func:`boundary_scores` on any device masks, such as ``refine_words(...) > t``: every boundary pixel's
 nearest boundary pixel of the other set found exactly on the device, in one call for every (mask, region) pair.
+To grow, shrink or feather a mask -- a word's mask as an inpainting mask, its confident core, the gaps between its
+blobs closed -- use :meth:`GlobalHeatMap.word_distance <daam_b200.heatmap.GlobalHeatMap.word_distance>` on the
+thresholded word masks, or :func:`distance_transform` on any device masks: the exact signed distance transform, whose
+``mask(r)``, ``soft_mask(r, feather=f)`` and ``distance()`` are the edits.
 """
 from __future__ import annotations
 
@@ -45,7 +49,7 @@ import torch
 
 from . import _native
 
-__all__ = ['compute_iou', 'compute_ioa', 'boundary_scores']
+__all__ = ['compute_iou', 'compute_ioa', 'boundary_scores', 'distance_transform']
 
 
 def _match_size(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
@@ -137,3 +141,30 @@ def boundary_scores(masks: torch.Tensor, regions: torch.Tensor, tolerances=None,
     out = RegionBoundary(shaped[0], flat.region_boundary, *shaped[1:], flat.tolerances)
     return out.cpu() if to_cpu else out
 
+
+def distance_transform(masks: torch.Tensor, to_cpu: bool = True):
+    """The exact signed distance transform of device masks: :meth:`GlobalHeatMap.word_distance
+    <daam_b200.heatmap.GlobalHeatMap.word_distance>` with the masks given. ``masks``: bool or uint8 ``[H, W]``,
+    ``[N, H, W]`` or ``[M, N, H, W]`` on a CUDA device, any nonzero byte inside, such as ``refine_words(...) > t``,
+    ``segment_crf(...)[1] == w + 1`` or a mask this call has grown: ``distance_transform(wd.mask(r)).mask(-r)`` is the
+    closing of ``wd``'s masks by the disk of radius ``r``. Returns a :class:`~daam_b200.heatmap.WordDistance` whose
+    ``signed_d2`` has the masks' shape, on the CPU unless ``to_cpu=False``. Two launches; no scratch. An empty shape
+    launches nothing. At most 2**24 pixels and 32767 pixels a side."""
+    from .heatmap import WordDistance, _distance_size, _require_cuda, _stream_ptr
+    what = 'distance_transform'
+    if not isinstance(masks, torch.Tensor):
+        raise TypeError(f'{what}: masks must be a torch.Tensor, not {type(masks).__name__}')
+    if masks.dtype not in (torch.bool, torch.uint8):
+        raise TypeError(f'{what}: masks must be bool or uint8, not {masks.dtype}')
+    if masks.dim() not in (2, 3, 4):
+        raise ValueError(f'{what}: masks must be [H, W], [N, H, W] or [M, N, H, W], not {tuple(masks.shape)}')
+    _require_cuda(masks, what)
+    out_h, out_w = masks.shape[-2:]
+    _distance_size(out_h, out_w, what)
+    out = WordDistance(torch.empty(masks.shape, dtype=torch.int32, device=masks.device))
+    if masks.numel() > 0:
+        mask_bytes = masks.detach().contiguous().view(torch.uint8)
+        with torch.cuda.device(masks.device):
+            _native.mask_distance(mask_bytes.data_ptr(), masks.numel() // (out_h * out_w), out_h, out_w,
+                                  out.signed_d2.data_ptr(), _stream_ptr(masks.device))
+    return out.cpu() if to_cpu else out

@@ -29,7 +29,8 @@ from . import _native
 from .utils import compute_token_merge_indices
 
 __all__ = ['GlobalHeatMap', 'RawHeatMapCollection', 'WordHeatMap', 'LayerSlab', 'GlobalHeatMapStack', 'TimeHeatMaps',
-           'ImageHeatMaps', 'LayerHeatMaps', 'FactorHeatMaps', 'HeadHeatMaps', 'RegionOverlap', 'RegionRanking', 'RegionBoundary', 'WordOverlap', 'RelationOverlap', 'WordInstances']
+           'ImageHeatMaps', 'LayerHeatMaps', 'FactorHeatMaps', 'HeadHeatMaps', 'RegionOverlap', 'RegionRanking', 'RegionBoundary', 'WordOverlap', 'RelationOverlap', 'WordInstances',
+           'WordDistance']
 
 RawHeatMapKey = Tuple[int, int, int]  # factor, layer, head
 
@@ -540,6 +541,30 @@ class GlobalHeatMap:
         wl, inst = _word_instances(self.tokenizer, self.prompt, self.heat_maps[None], words, image, threshold, absolute,
                                    max_instances, word_idx, offset_idx, to_cpu, 'GlobalHeatMap.word_instances')
         return wl.word_heat_maps(0), inst.map(0)
+
+    def word_distance(self, words, image, threshold: float, absolute: bool = False, word_idx=None, offset_idx: int = 0,
+                      to_cpu: bool = True):
+        """How far each pixel lies from each word's mask: the exact signed Euclidean distance transform of the mask
+        ``expand_words(words, image, absolute, threshold, word_idx, offset_idx)`` returns, ``M = pre > threshold``
+        with ``pre`` the expanded map without threshold. The :class:`WordDistance` holds ``signed_d2`` int32
+        ``[len(words), H, W]``: at a pixel outside ``M`` the squared distance between pixel centres to the nearest
+        pixel of ``M`` (``>= 1``), at a pixel of ``M`` minus the squared distance to the nearest pixel outside it
+        (``<= -1``; the image border is not outside, so a mask touching it is not eaten from it); ``+2**31 - 1`` at
+        every pixel of an empty mask and ``-(2**31 - 1)`` of a full one. Its helpers read every edit off it:
+        ``mask(r)`` grows the mask by ``r`` pixels (dilation by a disk; ``r < 0`` erodes), ``soft_mask(r,
+        feather=f)`` adds a linear edge of ``f`` pixels, ``distance()`` is the signed distance itself. E.g.
+        ``word_distance(['dog'], image, 0.4)[1].soft_mask(grow=16, feather=8)[0]`` is an inpainting mask for the dog.
+        Fused on the device in O(H W) work per word whatever the distances; the ``[len(words), H, W]`` stack of
+        values never leaves it, and the results are the same bits on every call.
+
+        Returns ``(word_heat_maps, distance)``: the list of :class:`WordHeatMap` that :meth:`segment` returns and the
+        :class:`WordDistance` (CPU by default, ``to_cpu=False`` keeps it on the device). ``threshold`` must be truthy
+        and finite (a ``ValueError`` otherwise); at most 96 words, 2**24 image pixels and 32767 pixels a side. An
+        empty word list launches nothing and returns an empty word axis. Raises the reference's ``ValueError`` for a
+        word that is not in the prompt."""
+        wl, dist = _word_distance(self.tokenizer, self.prompt, self.heat_maps[None], words, image, threshold, absolute,
+                                  word_idx, offset_idx, to_cpu, 'GlobalHeatMap.word_distance')
+        return wl.word_heat_maps(0), dist.map(0)
 
     def overlay_words(self, words, image, absolute: bool = False, threshold: Optional[float] = None,
                       color_normalize: bool = True, word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
@@ -1246,6 +1271,106 @@ def _word_instances(tokenizer, prompt: str, maps: torch.Tensor, words, image, th
     return wl.done(inst)
 
 
+# Scratch of one word_distance call: as many (map, word) planes as fit are transformed per round, so memory does not
+# grow with the number of maps.
+WORD_DISTANCE_SCRATCH_BYTES = 256 << 20
+
+
+def _real(v, what: str, name: str) -> float:
+    """``v`` as a Python float; a ``ValueError`` unless it is a finite real number."""
+    if isinstance(v, bool) or not isinstance(v, numbers.Real) or not math.isfinite(float(v)):
+        raise ValueError(f'{what}: {name} must be a finite number, not {v!r}')
+    return float(v)
+
+
+@dataclass
+class WordDistance:
+    """Signed distance maps of masks (:meth:`GlobalHeatMap.word_distance`,
+    :func:`daam_b200.evaluate.distance_transform`): ``signed_d2`` int32 ``[..., W, H, W']``, with ``M`` a mask and
+    ``d2`` the squared Euclidean distance between pixel centres, ``min d2`` to ``M`` (``>= 1``) at a pixel outside
+    ``M`` and ``-min d2`` to the pixels outside ``M`` (``<= -1``, the image border not counted as outside) at a pixel
+    of ``M``; every pixel is ``+DISTANCE_NONE`` (``2**31 - 1``) for an empty mask and ``-DISTANCE_NONE`` for a full
+    one. ``...`` is the map axis of a :class:`GlobalHeatMapStack`, absent for one map. The helpers are plain torch on
+    the field's device; the sentinels count as infinitely far."""
+    signed_d2: torch.Tensor
+
+    NONE = _native.DISTANCE_NONE
+
+    def map(self, i: int) -> 'WordDistance':
+        """The distances of map ``i`` of a stack."""
+        return WordDistance(self.signed_d2[i])
+
+    def cpu(self) -> 'WordDistance':
+        return WordDistance(self.signed_d2.cpu())
+
+    def _signed(self) -> torch.Tensor:
+        """float64 signed distance ``sign * sqrt(|d2|)``, ``+-inf`` for the sentinels."""
+        d2 = self.signed_d2
+        s = d2.double().abs().sqrt().copysign(d2.double())
+        return torch.where(d2.abs() == self.NONE, d2.double().sign() * math.inf, s)
+
+    def distance(self) -> torch.Tensor:
+        """fp32 ``[..., W, H, W']``: the signed Euclidean distance, ``sqrt(d2)`` outside the mask and ``-sqrt(d2)``
+        inside, taken in float64 and rounded once; ``+inf`` for an empty mask, ``-inf`` for a full one."""
+        return self._signed().float()
+
+    def mask(self, grow: float = 0.0) -> torch.Tensor:
+        """bool ``[..., W, H, W']``: the mask grown by ``grow`` pixels. ``grow >= 0``: ``signed_d2 <= grow**2``, the
+        binary dilation by the disk ``{dy**2 + dx**2 <= grow**2}`` (``grow = 0`` is the mask itself); ``grow < 0``:
+        ``signed_d2 < -grow**2``, the binary erosion by that disk with the image border counted as inside. The
+        comparison runs in float64. ``distance_transform(wd.mask(r)).mask(-r)`` is the closing by the disk."""
+        g = _real(grow, 'WordDistance.mask', 'grow')
+        d = torch.where(self.signed_d2.abs() == self.NONE, self.signed_d2.double().sign() * math.inf,
+                        self.signed_d2.double())
+        return d <= g * g if g >= 0 else d < -(g * g)
+
+    def soft_mask(self, grow: float = 0.0, *, feather: float) -> torch.Tensor:
+        """fp32 ``[..., W, H, W']``: ``clamp((grow + feather - s) / feather, 0, 1)`` with ``s`` the float64 signed
+        distance, rounded once: 1 inside the mask grown by ``grow`` pixels, falling linearly to 0 over ``feather``
+        pixels beyond it -- an inpainting mask with a soft edge. ``feather`` must be finite and > 0."""
+        g = _real(grow, 'WordDistance.soft_mask', 'grow')
+        f = _real(feather, 'WordDistance.soft_mask', 'feather')
+        if not f > 0:
+            raise ValueError(f'WordDistance.soft_mask: feather must be > 0, not {feather!r}')
+        return ((g + f - self._signed()) / f).clamp(0, 1).float()
+
+
+def _distance_size(out_h: int, out_w: int, what: str):
+    """A ``ValueError`` unless ``out_h, out_w <= 32767`` and ``out_h * out_w <= 2**24``."""
+    if out_h > _native.DISTANCE_MAX_SIDE or out_w > _native.DISTANCE_MAX_SIDE:
+        raise ValueError(f'{what}: a {out_h} x {out_w} image has a side > {_native.DISTANCE_MAX_SIDE}')
+    if out_h * out_w > 1 << 24:
+        raise ValueError(f'{what}: a {out_h} x {out_w} image is more than 2**24 pixels')
+
+
+def _word_distance(tokenizer, prompt: str, maps: torch.Tensor, words, image, threshold, absolute, word_idx,
+                   offset_idx: int, to_cpu: bool, what: str):
+    """``daam_word_distance`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(wl, distance)``, the
+    :class:`_WordList` and the :class:`WordDistance` with a leading map axis. Checks as ``_word_instances``, in its
+    order (the threshold set and finite), then the image size. Scratch: :data:`WORD_DISTANCE_SCRATCH_BYTES`, clipped
+    to the planes the call has, at least one plane."""
+    words = list(words)
+    if not threshold:
+        raise ValueError(f'{what}: threshold must be set (truthy), not {threshold!r}: the distances are those of the '
+                         f'mask expand_words(..., threshold) returns')
+    if not math.isfinite(float(threshold)):
+        raise ValueError(f'{what}: threshold must be finite, not {threshold!r}')
+    if len(words) > _native.MAX_SEGMENT_WORDS:
+        raise ValueError(f'{what}: {len(words)} words > {_native.MAX_SEGMENT_WORDS}, the word limit of one call')
+    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, image, absolute, threshold, to_cpu, what)
+    out_h, out_w = wl.out_h, wl.out_w
+    _distance_size(out_h, out_w, what)
+    shape = (wl.n_maps, len(words), out_h, out_w)
+    if wl.empty or out_h * out_w == 0:
+        return wl.done(WordDistance(torch.zeros(shape, dtype=torch.int32, device=wl.dev)))
+    out = WordDistance(torch.empty(shape, dtype=torch.int32, device=wl.dev))
+    plane = _native.distance_plane_bytes(out_h, out_w)
+    n_bytes = max(plane, min(WORD_DISTANCE_SCRATCH_BYTES, plane * wl.n_maps * len(words)))
+    scratch = torch.empty(n_bytes, dtype=torch.uint8, device=wl.dev)
+    wl.launch(_native.word_distance, wl.word_maps.data_ptr(), out.signed_d2.data_ptr(), scratch.data_ptr(), n_bytes)
+    return wl.done(out)
+
+
 def jet_colormap() -> torch.Tensor:
     """The fp32 ``[256, 3]`` table the overlay kernel colours with: ``L[k] = 255 * jet(k / 255)``, matplotlib's ``jet``
     segment data evaluated in float64 and rounded once to fp32 (``L[0] = (0, 0, 127.5)``, ``L[255] = (127.5, 0, 0)``)."""
@@ -1522,6 +1647,18 @@ class GlobalHeatMapStack:
         wl, inst = _word_instances(self.tokenizer, self.prompt, self.heat_maps, words, image, threshold, absolute,
                                    max_instances, word_idx, offset_idx, to_cpu, f'{type(self).__name__}.word_instances')
         return wl.word_maps, inst
+
+    def word_distance(self, words, image, threshold: float, absolute: bool = False, word_idx=None, offset_idx: int = 0,
+                      to_cpu: bool = True):
+        """:meth:`GlobalHeatMap.word_distance` for every map in one call: returns ``(word_maps, distance)`` with
+        ``word_maps`` the device ``[maps, len(words), xh, xw]`` word heat maps and ``distance`` a :class:`WordDistance`
+        with a leading map axis (``signed_d2`` ``[maps, len(words), H, W]``); row ``t`` equals
+        ``self[t].word_distance(...)`` bit for bit (min / max normalisation per map and word). E.g.
+        ``distance.mask(8)[:, 0]`` is word 0's mask grown by 8 pixels at every step of a history. Scratch stays
+        within a fixed budget whatever the map count: the planes are transformed in rounds."""
+        wl, dist = _word_distance(self.tokenizer, self.prompt, self.heat_maps, words, image, threshold, absolute,
+                                  word_idx, offset_idx, to_cpu, f'{type(self).__name__}.word_distance')
+        return wl.word_maps, dist
 
     def overlay_words(self, words, image, absolute: bool = False, threshold: Optional[float] = None,
                       color_normalize: bool = True, word_idx=None, offset_idx: int = 0, to_cpu: bool = True):

@@ -38,7 +38,8 @@ extern "C" {
                                           daam_word_instances; daam_region_sweep;
                                           daam_region_ranking; daam_refine_words;
                                           daam_region_boundary, daam_mask_boundary;
-                                          daam_segment_crf) */
+                                          daam_segment_crf;
+                                          daam_word_distance, daam_mask_distance) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_TOKENS 231     /* daam_accumulate: long contexts of 2 or 3 CLIP chunks of 77 tokens (154, 231) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
@@ -650,6 +651,47 @@ int daam_segment_crf(const float* global_maps, int32_t n_maps, int32_t n_rows, i
                      int32_t radius, float appearance, float sigma_xy, float sigma_rgb, float smoothness,
                      float sigma_smooth, float* word_maps, const uint8_t* image, int64_t image_map_stride,
                      uint8_t* labels, float* scores, float* probs, void* scratch, int64_t scratch_bytes, void* stream);
+
+/*
+ * Word distance maps: the exact signed squared Euclidean distance transform of each word's mask, on each of n_maps
+ * global maps stored back to back. With M the mask m[w] > threshold (m what daam_expand_words writes for word w
+ * WITHOUT threshold, same rows / row_begin / absolute: exactly daam_expand_words' thresholded mask) and d2 the squared
+ * distance between pixel centres (an exact integer):
+ *   signed_d2[i][w][p] =  min_{q in M} d2(p, q)        (>= 1)  for p outside M,
+ *                      = -min_{q not in M} d2(p, q)    (<= -1) for p in M, q over the image's pixels only: the border
+ *                                                              is not background;
+ *   every pixel is +DAAM_DISTANCE_NONE for an empty mask and -DAAM_DISTANCE_NONE for a mask that fills the image.
+ * signed_d2: int32 [n_maps][n_words][out_h][out_w] on the device. signed_d2 <= r^2 is the mask dilated by the disk of
+ * radius r, signed_d2 < -r^2 the mask eroded by it. Each plane takes a column pass (one thread per column: each
+ * pixel's vertical distance to the nearest pixel of the other class in its column, signed by its class, written to
+ * signed_d2) and a row pass in place (the lower envelope of parabolas of Felzenszwalb and Huttenlocher, "Distance
+ * Transforms of Sampled Functions", Theory of Computing 2012, once per class over each row, every comparison exact in
+ * 64-bit integers): O(out_h * out_w) work per plane, whatever the distances. Integer arithmetic only: the results are
+ * the same bits on every call and whatever the scratch.
+ * Arguments as daam_word_instances without max_instances. scratch: device, 4-byte aligned, at least
+ * DAAM_DISTANCE_PLANE_BYTES(out_h, out_w): the values `pre` and the min / max partials of one (map, word) plane. As
+ * many planes go in a round as the scratch holds, whole maps while a map's planes fit, and the call loops over the
+ * rounds: four launches a round (the word maps, the values, the column pass, the row pass).
+ * Limits (DAAM_E_UNSUPPORTED): those of daam_word_instances, plus out_h, out_w <= 32767 (every d2 stays below
+ * DAAM_DISTANCE_NONE). DAAM_E_INVALID: a null pointer or non-positive size, a non-finite threshold, scratch not 4-byte
+ * aligned or scratch_bytes below DAAM_DISTANCE_PLANE_BYTES(out_h, out_w), then the word list as daam_word_instances.
+ */
+#define DAAM_DISTANCE_NONE INT32_MAX
+#define DAAM_DISTANCE_MAX_SIDE 32767
+#define DAAM_DISTANCE_PLANE_BYTES(out_h, out_w) (4 * (int64_t)(out_h) * (out_w) + 256)
+int daam_word_distance(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t map_h, int32_t map_w,
+                       const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h, int32_t out_w,
+                       int32_t absolute, float threshold, float* word_maps, int32_t* signed_d2, void* scratch,
+                       int64_t scratch_bytes, void* stream);
+
+/*
+ * The signed distance transform of n_planes device masks: daam_word_distance with M = {p : masks[i][p] != 0} (masks:
+ * device uint8 [n_planes][out_h][out_w]; signed_d2: int32 [n_planes][out_h][out_w]). No scratch: the column distances
+ * live in signed_d2. Two launches per 65535 planes. Limits (DAAM_E_UNSUPPORTED): out_h, out_w <= 32767, out_h * out_w
+ * <= 2^24. DAAM_E_INVALID: a null pointer or non-positive size.
+ */
+int daam_mask_distance(const uint8_t* masks, int32_t n_planes, int32_t out_h, int32_t out_w, int32_t* signed_d2,
+                       void* stream);
 
 /* Library / device introspection. */
 int daam_abi_version(void);
