@@ -25,6 +25,7 @@
 #include <algorithm>
 
 #include "boundary.cuh"
+#include "word_value.cuh"
 
 namespace daam {
 namespace {
@@ -38,6 +39,8 @@ constexpr int kBinBytes = kBoundaryRegions * 2 * kBoundaryMaxTolerances * 4;
 constexpr int kMaxBytes = kBoundaryRegions * 2 * 8;
 constexpr int kBoundaryTileBytes = kBinBytes + 2 * kMaxBytes;
 static_assert(kBoundaryTileBytes == 10080, "DAAM_BOUNDARY_PLANE_BYTES counts 10080 bytes per tile");
+static_assert(DAAM_BOUNDARY_PLANE_BYTES(0, 1) == kWordPartialFloats * sizeof(float),
+              "DAAM_BOUNDARY_PLANE_BYTES counts one plane's min / max partials");
 
 struct MaskIn {
   const unsigned char* m;

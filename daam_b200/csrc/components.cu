@@ -17,6 +17,7 @@
 #include <limits.h>
 
 #include "components.cuh"
+#include "word_value.cuh"
 
 namespace daam {
 namespace {
@@ -282,7 +283,7 @@ long long slots(int h, int w) { return (long long)((h + 1) / 2) * ((w + 1) / 2);
 }  // namespace
 
 long long instance_plane_bytes(int h, int w) {
-  return 8LL * h * w + 48 * slots(h, w) + 4 + 64 * sizeof(float);
+  return 8LL * h * w + 48 * slots(h, w) + 4 + kWordPartialFloats * sizeof(float);
 }
 
 void instance_planes_in(void* scratch, int planes, int h, int w, InstancePlanes& p) {

@@ -20,19 +20,19 @@
 
 #include "bicubic.cuh"
 #include "crf.cuh"
+#include "word_value.cuh"
 
 namespace daam {
 namespace {
 
 constexpr int kTileW = 32, kTileH = 8;   // one warp per tile row: conflict-free shared loads at every window offset
 
-// min / max of v per word over segment_minmax_kernel's chunks in order (words.cu's word_bounds)
+// min / max of v per word of map `map`, from segment_minmax_kernel's partials
 __device__ __forceinline__ void crf_bounds(const CrfParams& P, int map, float* lo, float* hi) {
   if (P.absolute) return;
   for (int w = threadIdx.x; w < P.n_words; w += blockDim.x) {
-    const float* slots = P.minmax + 2LL * ((long long)map * P.n_words + w) * P.chunks;
-    float vlo = INFINITY, vhi = -INFINITY;
-    for (int c = 0; c < P.chunks; ++c) { vlo = fminf(vlo, slots[2 * c]); vhi = fmaxf(vhi, slots[2 * c + 1]); }
+    float vlo, vhi;
+    partial_bounds(P.minmax + 2LL * ((long long)map * P.n_words + w) * P.chunks, P.chunks, vlo, vhi);
     lo[w] = vlo; hi[w] = vhi;
   }
 }
@@ -47,7 +47,7 @@ __device__ __forceinline__ float crf_logit(const CrfParams& P, int map, int l, i
     const int w = l - P.use_threshold;
     const float* wm = P.word_maps + ((long long)map * P.n_words + w) * P.mh * P.mw;
     s = bicubic_shared(wm, P.mw, make_taps(y, P.mh, P.oh), make_taps(x, P.mw, P.ow));
-    if (!P.absolute) s = (s - lo[w]) / (hi[w] - lo[w] + 1e-8f);   // words.cu's minmax_normalize
+    if (!P.absolute) s = minmax_normalize(s, lo[w], hi[w]);
   }
   return __fmul_rn(P.scale, s);
 }
@@ -185,7 +185,7 @@ int launch_step(const CrfParams& p, size_t smem, cudaStream_t stream) {
 }  // namespace
 
 long long crf_map_bytes(int n_labels, int h, int w) {
-  return 8LL * n_labels * h * w + 4LL * kCrfChunkFloats * n_labels;
+  return 8LL * n_labels * h * w + 4LL * kWordPartialFloats * n_labels;
 }
 
 void crf_tables(int radius, float appearance, float sigma_xy, float sigma_rgb, float smoothness, float sigma_smooth,

@@ -13,7 +13,6 @@ constexpr int kCrfMaxRadius = DAAM_CRF_MAX_RADIUS;
 constexpr int kCrfTaps = (2 * kCrfMaxRadius + 1) * (2 * kCrfMaxRadius + 1);
 constexpr int kCrfMaxIterations = 64;
 constexpr int kCrfMaxWords = 96;
-constexpr int kCrfChunkFloats = 64;   // min / max partials per label slot: 2 floats for each of up to 32 chunks
 
 // One round of whole maps: what the kernels read and write. Label l's logit is z_l = scale * s_l with s_0 = threshold
 // (use_threshold only) and s_{w + use_threshold} = m[w]; the output label of l is l + 1 - use_threshold.

@@ -20,6 +20,7 @@
 #include <mutex>
 
 #include "distance.cuh"
+#include "word_value.cuh"
 
 namespace daam {
 namespace {
@@ -167,6 +168,8 @@ int launch_planes(const In& in, int planes, int h, int w, int* d, cudaStream_t s
 }  // namespace
 
 long long distance_plane_bytes(int h, int w) { return DAAM_DISTANCE_PLANE_BYTES(h, w); }
+static_assert(DAAM_DISTANCE_PLANE_BYTES(0, 0) == kWordPartialFloats * sizeof(float),
+              "DAAM_DISTANCE_PLANE_BYTES counts one plane's min / max partials");
 
 int distance_check_scratch(const char* name, const void* scratch, long long scratch_bytes, int h, int w) {
   if ((uintptr_t)scratch & 3) { set_error("%s: scratch must be 4-byte aligned", name); return DAAM_E_INVALID; }

@@ -23,6 +23,7 @@
 #include <math.h>
 
 #include "ranking.cuh"
+#include "word_value.cuh"
 
 namespace daam {
 namespace {
@@ -347,7 +348,8 @@ int segs_of(long long n) { return (int)((n + kRankSegment - 1) / kRankSegment); 
 
 long long ranking_plane_bytes(int h, int w) {
   const long long n = (long long)h * w;
-  return 16 * n + 1024LL * tiles_of(n) + 1540LL * segs_of(n) + 512;   // segs_of: ceil(n / 1024)
+  // segs_of: ceil(n / 1024); then n_pos and the min / max partials
+  return 16 * n + 1024LL * tiles_of(n) + 1540LL * segs_of(n) + 4 * 64 + 4 * kWordPartialFloats;
 }
 
 void ranking_planes_in(void* scratch, int planes, int h, int w, RankingPlanes& p) {

@@ -21,6 +21,7 @@
 
 #include "bicubic.cuh"
 #include "refine.cuh"
+#include "word_value.cuh"
 
 namespace daam {
 namespace {
@@ -108,14 +109,10 @@ __global__ void __launch_bounds__(256) refine_row_kernel(const __grid_constant__
   const long long n = (long long)P.oh * ow, row = (long long)y * ow;
   float* buf = P.buf + (long long)p * 8 * n;
   if (kFirst) {
-    // min / max of v over segment_minmax_kernel's chunks in order (words.cu's word_bounds), then m = expand_words' m
+    // m = expand_words' m, from the word map and its min / max partials
     if (threadIdx.x == 0) {
       float vlo = 0.f, vhi = 0.f;
-      if (!P.absolute) {
-        const float* slots = P.minmax + 2LL * p * P.chunks;
-        vlo = INFINITY; vhi = -INFINITY;
-        for (int c = 0; c < P.chunks; ++c) { vlo = fminf(vlo, slots[2 * c]); vhi = fmaxf(vhi, slots[2 * c + 1]); }
-      }
+      if (!P.absolute) partial_bounds(P.minmax + 2LL * p * P.chunks, P.chunks, vlo, vhi);
       s_lo = vlo; s_hi = vhi;
     }
     __syncthreads();
@@ -125,7 +122,7 @@ __global__ void __launch_bounds__(256) refine_row_kernel(const __grid_constant__
     const unsigned char* im = plane_image(P, p) + row * 3;
     for (int x = lo + threadIdx.x; x < hi; x += blockDim.x) {
       float m = bicubic_shared(wm, P.mw, ty, make_taps(x, P.mw, ow));
-      if (!P.absolute) m = (m - vlo) / (vhi - vlo + 1e-8f);
+      if (!P.absolute) m = minmax_normalize(m, vlo, vhi);
       const int i = x - lo;
       st[0][i] = m;
 #pragma unroll
@@ -217,7 +214,7 @@ size_t col_smem(int radius) { return sizeof(float) * 4 * kColW * (kColRows + 2 *
 
 long long refine_guide_bytes(int h, int w) { return 36LL * h * w; }
 
-long long refine_plane_bytes(int h, int w) { return 32LL * h * w + 4 * kRefineChunkFloats; }
+long long refine_plane_bytes(int h, int w) { return 32LL * h * w + 4 * kWordPartialFloats; }
 
 void refine_planes_in(void* scratch, int guides, int planes, int h, int w, RefinePlanes& p) {
   const long long n = (long long)h * w;
@@ -225,7 +222,7 @@ void refine_planes_in(void* scratch, int guides, int planes, int h, int w, Refin
   p.guide = f;
   f += 9 * n * guides;
   p.minmax = f;
-  f += (long long)kRefineChunkFloats * planes;
+  f += (long long)kWordPartialFloats * planes;
   p.buf = f;
   p.guides = guides; p.planes = planes; p.oh = h; p.ow = w;
 }

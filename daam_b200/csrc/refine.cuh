@@ -9,7 +9,6 @@
 namespace daam {
 
 constexpr int kRefineMaxRadius = 64;
-constexpr int kRefineChunkFloats = 64;   // min / max partials per plane: 2 floats for each of up to 32 chunks
 
 // One round of planes (a plane: one (map, word) pair) of n = oh * ow pixels: the scratch buffers, laid out by
 // refine_planes_in, and what the kernels read and write.

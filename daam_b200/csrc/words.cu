@@ -5,7 +5,7 @@
 // (daam/heatmap.py:77-93) over a word list. Every consumer runs the same steps:
 //  1. word map: the gather-mean of the word's rows (word_mean) into shared memory;
 //  2. min / max of the bicubic-interpolated word map v over the image, per chunk of output pixels, then over the
-//     chunks in a fixed order (word_bounds in the tile kernels);
+//     chunks in a fixed order (partial_bounds);
 //  3. the tile kernels stage the source window under a 16 x 64 output tile for a pass of words;
 //  4. per pixel: interpolate (bicubic.cuh), normalise and threshold: m = word_value(v), what expand_as returns.
 // The consumers differ only in what they do with m:
@@ -24,12 +24,14 @@
 //    guide (daam_refine_words);
 //  - crf.cu recomputes it the same way as the unary logits of a Potts CRF with the image as bilateral guide
 //    (daam_segment_crf).
-// The tile kernels run after segment_minmax_kernel (steps 1 and 2, the word maps and min / max partials to global
-// memory); region_tile_kernel, region_sweep_tile_kernel, overlay_kernel, word_pair_tile_kernel and instance_mask_kernel share the tile helpers
-// (block_tile / tile_at, word_bounds, stage_windows, tap tables). expand_words_kernel, segment_minmax_kernel and segment_label_kernel keep
-// their steps inline: written with the helpers, nvcc scheduled them differently and they measured slower. Every consumer's m is expand_words_kernel's
-// value bit for bit. Deterministic: the only atomics here are region_sweep_tile_kernel's integer adds (and
-// components.cu's are integer atomics), whose results do not depend on their order.
+// word_value.cuh defines m's pieces (word_mean, partial_bounds, minmax_normalize): every consumer's m, here and in
+// refine.cu and crf.cu, is built from them and is expand_words_kernel's value bit for bit. The tile kernels run after
+// segment_minmax_kernel (steps 1 and 2, the word maps and min / max partials to global memory) and share the tile
+// helpers (block_tile / tile_at, word_bounds, stage_windows, tap tables, and tile_value in the two that also run
+// without staged windows). expand_words_kernel, segment_minmax_kernel and segment_label_kernel keep their steps
+// inline: written with the helpers, nvcc scheduled them differently and they measured slower. Deterministic: the only
+// atomics here are region_sweep_tile_kernel's integer adds (and components.cu's are integer atomics), whose results do
+// not depend on their order.
 #include <cooperative_groups.h>
 #include <math.h>
 
@@ -44,6 +46,7 @@
 #include "distance.cuh"
 #include "ranking.cuh"
 #include "refine.cuh"
+#include "word_value.cuh"
 
 namespace daam {
 namespace {
@@ -51,19 +54,10 @@ namespace {
 constexpr int kMaxRows = 128;                       // selected rows of daam_word_heat_map
 constexpr int kMaxWords = 96;
 constexpr int kMaxWordRows = 320;                   // selected rows over all words of a launch
-constexpr int kMaxChunks = 32;                      // min / max CTAs per word; scratch holds 2 floats per (word, chunk)
 constexpr int kMaxSmem = 200 * 1024;                // dynamic shared memory: a word map, or a tile kernel's windows
 constexpr int kSegTileH = 16, kSegTileW = 64;       // output tile of one tile-kernel CTA
 constexpr int kSegPix = kSegTileH * kSegTileW / 256;   // output pixels per thread
 constexpr int kSegStageFloats = 12288;              // staged windows per pass when they fit (48 KB)
-
-// The word map at pixel i: the mean of rows[r0 .. r1) of maps [*][xx] (heatmap.py:121-123). Every word map of this
-// file is built with it, so that they are the same bits.
-__device__ __forceinline__ float word_mean(const float* __restrict__ maps, const int* rows, int r0, int r1, int xx, int i) {
-  float s = 0.f;
-  for (int r = r0; r < r1; ++r) s += __ldg(maps + (long long)rows[r] * xx + i);
-  return s / (float)(r1 - r0);
-}
 
 struct RowSel {
   int n;
@@ -95,9 +89,6 @@ struct WordListParams {
 __device__ __forceinline__ float word_map_at(const WordListParams& P, const float* wm, int oy, int ox) {
   return bicubic_shared(wm, P.mw, make_taps(oy, P.mh, P.oh), make_taps(ox, P.mw, P.ow));
 }
-
-// expand_as's min-max normalisation (heatmap.py:88-89)
-__device__ __forceinline__ float minmax_normalize(float v, float lo, float hi) { return (v - lo) / (hi - lo + 1e-8f); }
 
 // v -> m, for a word whose v has min / max lo / hi
 __device__ __forceinline__ float word_value(const WordListParams& P, float v, float lo, float hi) {
@@ -233,10 +224,7 @@ __device__ __forceinline__ Tile block_tile(const WordListParams& P) { return til
 // min / max of v of (map, word w), reduced from segment_minmax_kernel's chunks in a fixed order; 0 / 0 without minmax
 __device__ __forceinline__ void word_bounds(const WordListParams& P, int map, int w, float& lo, float& hi) {
   lo = 0.f; hi = 0.f;
-  if (!P.minmax) return;
-  const float* slots = P.scratch + 2 * ((long long)map * P.n_words + w) * P.chunks;
-  lo = INFINITY; hi = -INFINITY;
-  for (int c = 0; c < P.chunks; ++c) { lo = fminf(lo, slots[2 * c]); hi = fmaxf(hi, slots[2 * c + 1]); }
+  if (P.minmax) partial_bounds(P.scratch + 2 * ((long long)map * P.n_words + w) * P.chunks, P.chunks, lo, hi);
 }
 
 // The source windows of words [w0, w0 + nw) of `word_maps` (one map's) into `win`, one after the other. Barriers on
@@ -278,6 +266,25 @@ __device__ __forceinline__ void tile_taps(const TapTables& tt, int py, int px, T
   }
 }
 
+// m of word w at tile pixel p < T.th * T.tw: from window wi of the pass, or with words_per_pass 0 (no window fits
+// beside the kernel's own shared memory) from word w of `word_maps` (one map's), with the same taps
+__device__ __forceinline__ float tile_value(const WordListParams& P, const Tile& T, const TapTables& tt,
+                                            const float* win, const float* word_maps, int w, int wi, int p, float lo,
+                                            float hi) {
+  const int py = p / T.tw;
+  Taps ty, tx;
+  tile_taps(tt, py, p - py * T.tw, ty, tx);
+  float v;
+  if (P.words_per_pass > 0) {
+    v = bicubic_shared(win + wi * T.wn, T.ww, ty, tx);
+  } else {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) { ty.idx[j] += T.wy; tx.idx[j] += T.wx; }
+    v = bicubic_at(word_maps + (long long)w * P.mh * P.mw, P.mw, ty, tx);
+  }
+  return word_value(P, v, lo, hi);
+}
+
 // ---- segmentation: a per-pixel word label -----------------------------------------------------------------------
 // labels[p] = 1 + argmax_w m[w][p] (lowest w on ties), or 0 where use_threshold and the max is not > threshold;
 // scores[p] = max_w m[w][p], with m[w] taken without threshold. Each pixel keeps the running max / argmax in registers
@@ -302,10 +309,9 @@ __global__ void __launch_bounds__(256) segment_label_kernel(const __grid_constan
   const int wh = make_taps(y0 + th - 1, mh, oh).idx[3] - wy + 1, ww = make_taps(x0 + tw - 1, mw, ow).idx[3] - wx + 1;
   const int wn = wh * ww;
   if (!P.absolute) {
-    for (int w = threadIdx.x; w < n_words; w += blockDim.x) {   // chunks in a fixed order
-      const float* slots = P.scratch + 2 * ((long long)map * n_words + w) * P.chunks;
-      float lo = INFINITY, hi = -INFINITY;
-      for (int c = 0; c < P.chunks; ++c) { lo = fminf(lo, slots[2 * c]); hi = fmaxf(hi, slots[2 * c + 1]); }
+    for (int w = threadIdx.x; w < n_words; w += blockDim.x) {
+      float lo, hi;
+      partial_bounds(P.scratch + 2 * ((long long)map * n_words + w) * P.chunks, P.chunks, lo, hi);
       s_lo[w] = lo; s_hi[w] = hi;
     }
   }
@@ -585,18 +591,7 @@ __global__ void __launch_bounds__(256) region_sweep_tile_kernel(const __grid_con
         const int p = threadIdx.x + 256 * k;
         int b = 0;
         if (p < n_pix) {
-          const int py = p / T.tw;
-          Taps ty, tx;
-          tile_taps(taps, py, p - py * T.tw, ty, tx);
-          float v;
-          if (staged) {
-            v = bicubic_shared(win + wi * T.wn, T.ww, ty, tx);
-          } else {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) { ty.idx[j] += T.wy; tx.idx[j] += T.wx; }
-            v = bicubic_at(word_maps + (long long)w * mh * mw, mw, ty, tx);
-          }
-          const float m = word_value(P, v, s_lo[w], s_hi[w]);
+          const float m = tile_value(P, T, taps, win, word_maps, w, wi, p, s_lo[w], s_hi[w]);
           // b = #{k : m > tau[k]}: the passing thresholds are a prefix of the ascending list
 #pragma unroll
           for (int step = kMaxThresholds; step > 0; step >>= 1)
@@ -718,31 +713,18 @@ __global__ void __launch_bounds__(256) word_pair_tile_kernel(const __grid_consta
     __syncthreads();                                   // the previous tile has read the tap tables and buffers
     fill_tap_tables(P, T, taps);
     if (!staged) __syncthreads();                      // (stage_windows' barriers publish them otherwise)
-    // m of word w (window wi of the pass) at tile pixel p < n_pix
-    auto value = [&](int w, int wi, int p) {
-      const int py = p / T.tw;
-      Taps ty, tx;
-      tile_taps(taps, py, p - py * T.tw, ty, tx);
-      float v;
-      if (staged) {
-        v = bicubic_shared(win + wi * T.wn, T.ww, ty, tx);
-      } else {
-#pragma unroll
-        for (int j = 0; j < 4; ++j) { ty.idx[j] += T.wy; tx.idx[j] += T.wx; }
-        v = bicubic_at(word_maps + (long long)w * mh * mw, mw, ty, tx);
-      }
-      return word_value(P, v, s_lo[w], s_hi[w]);
-    };
     if (P.use_threshold) {
       for (int w0 = 0; w0 < n_words; w0 += per_pass) {
         const int nw = min(per_pass, n_words - w0);
         if (staged) stage_windows(P, T, word_maps, w0, nw, win);
         for (int wi = 0; wi < nw; ++wi) {
+          const int w = w0 + wi;
 #pragma unroll
           for (int k = 0; k < kSegPix; ++k) {
             const int p = threadIdx.x + 256 * k;
-            const unsigned bits = __ballot_sync(0xffffffffu, p < n_pix && value(w0 + wi, wi, p) != 0.f);
-            if (lane == 0) masks[(w0 + wi) * kPairMaskStride + 8 * k + warp] = bits;
+            const bool in = p < n_pix && tile_value(P, T, taps, win, word_maps, w, wi, p, s_lo[w], s_hi[w]) != 0.f;
+            const unsigned bits = __ballot_sync(0xffffffffu, in);
+            if (lane == 0) masks[w * kPairMaskStride + 8 * k + warp] = bits;
           }
         }
       }
@@ -768,7 +750,11 @@ __global__ void __launch_bounds__(256) word_pair_tile_kernel(const __grid_consta
         for (int w0 = 0; w0 < n_words; w0 += per_pass) {
           const int nw = min(per_pass, n_words - w0);
           if (staged && (c0 == 0 || restage)) stage_windows(P, T, word_maps, w0, nw, win);
-          for (int wi = 0; wi < nw; ++wi) vals[(w0 + wi) * kPairChunk + threadIdx.x] = p < n_pix ? value(w0 + wi, wi, p) : 0.f;
+          for (int wi = 0; wi < nw; ++wi) {
+            const int w = w0 + wi;
+            vals[w * kPairChunk + threadIdx.x] =
+                p < n_pix ? tile_value(P, T, taps, win, word_maps, w, wi, p, s_lo[w], s_hi[w]) : 0.f;
+          }
         }
         __syncthreads();
         for (int s = warp; s < n_slots; s += 8) {
@@ -1125,14 +1111,14 @@ static int launch_expand_words(ExpandParams& p, const DeviceInfo& dev, cudaStrea
   while (done < total) {                                // more words than the device holds at once: several launches
     const int batch = total - done < capacity ? total - done : capacity;
     int chunks = capacity / batch;
-    if (chunks > kMaxChunks) chunks = kMaxChunks;
+    if (chunks > kWordChunks) chunks = kWordChunks;
     if (chunks > (n + 255) / 256) chunks = (n + 255) / 256;
     if (chunks < 1) chunks = 1;
     q.s.n_words = batch;
     q.s.chunks = chunks;
     q.out = p.out + (long long)done * n;
     q.s.word_maps = p.s.word_maps ? p.s.word_maps + (long long)done * p.s.mh * p.s.mw : nullptr;
-    q.s.scratch = p.s.scratch + 2LL * kMaxChunks * done;
+    q.s.scratch = p.s.scratch + (long long)kWordPartialFloats * done;
     for (int i = 0; i <= batch; ++i) q.s.row_begin[i] = p.s.row_begin[done + i];
     void* args[] = {&q};
     DAAM_CUDA_TRY(cudaLaunchCooperativeKernel((const void*)expand_words_kernel, dim3(batch * chunks), dim3(256), args, smem,
@@ -1179,11 +1165,11 @@ static int tile_count(const WordListParams& p) {
 }
 
 // Launch 1 of the tile entry points, and all of it for daam_refine_words and daam_segment_crf: segment_minmax_kernel over (map, word, chunk)
-// with enough CTAs for a few waves, at most kMaxChunks per word and one per 256 pixels. Sets p.chunks.
+// with enough CTAs for a few waves, at most kWordChunks per word and one per 256 pixels. Sets p.chunks.
 static int launch_word_maps(WordListParams& p, int n_maps, const DeviceInfo& dev, cudaStream_t stream) {
   const long long n = (long long)p.oh * p.ow, mwords = (long long)n_maps * p.n_words;
   long long chunks = (4LL * dev.sm_count + mwords - 1) / mwords;
-  if (chunks > kMaxChunks) chunks = kMaxChunks;
+  if (chunks > kWordChunks) chunks = kWordChunks;
   if (chunks > (n + 255) / 256) chunks = (n + 255) / 256;
   if (chunks < 1 || !p.minmax) chunks = 1;
   p.chunks = (int)chunks;
@@ -1260,7 +1246,7 @@ extern "C" int daam_region_overlap(const float* global_maps, int32_t n_maps, int
   if (int rc = word_list_prepare(name, global_maps, n_maps, n_rows, mh, mw, rows, row_begin, n_words, out_h, out_w,
                                  absolute, !absolute, use_threshold, threshold, word_maps, scratch, true, p.s, &dev)) return rc;
   p.regions = regions; p.n_regions = n_regions; p.tiles = tile_count(p.s);
-  p.partials = scratch + 64LL * n_maps * n_words;     // after segment_minmax_kernel's min / max partials
+  p.partials = scratch + (long long)kWordPartialFloats * n_maps * n_words;   // after the min / max partials
   const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (int rc = launch_tiles(region_tile_kernel, p, n_maps, dev, stream)) return rc;
   const long long n_out = (long long)n_maps * n_words * (n_regions + 1);
@@ -1294,7 +1280,8 @@ extern "C" int daam_region_sweep(const float* global_maps, int32_t n_maps, int32
                                  absolute, !absolute, 0, 0.f, word_maps, scratch, true, p.s, &dev)) return rc;
   p.regions = regions; p.n_regions = n_regions; p.n_thresholds = n_thresholds;
   for (int k = 0; k < n_thresholds; ++k) p.thresholds[k] = thresholds[k];
-  p.counts = reinterpret_cast<unsigned*>(scratch + 64LL * n_maps * n_words);   // after the min / max partials
+  // after the min / max partials
+  p.counts = reinterpret_cast<unsigned*>(scratch + (long long)kWordPartialFloats * n_maps * n_words);
   const long long n_out = (long long)n_maps * n_words * (n_regions + 1);
   const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   DAAM_CUDA_TRY(cudaMemsetAsync(p.counts, 0, (size_t)n_out * n_thresholds * sizeof(unsigned), stream));
@@ -1324,7 +1311,7 @@ extern "C" int daam_word_overlap(const float* global_maps, int32_t n_maps, int32
                                  absolute, !absolute, use_threshold, threshold, word_maps, scratch, true, p.s, &dev)) return rc;
   p.tiles = tile_count(p.s);
   p.ctas = std::min(p.tiles, kPairCtas);
-  p.partials = scratch + 64LL * n_maps * n_words;     // after segment_minmax_kernel's min / max partials
+  p.partials = scratch + (long long)kWordPartialFloats * n_maps * n_words;   // after the min / max partials
   const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (int rc = launch_tiles(word_pair_tile_kernel, p, n_maps, dev, stream, p.ctas,
                             (size_t)pair_smem_floats(n_words, p.s.use_threshold) * sizeof(float))) return rc;
@@ -1647,7 +1634,7 @@ extern "C" int daam_segment_crf(const float* global_maps, int32_t n_maps, int32_
   c.scale = scale; c.radius = radius; c.q_in = nullptr;
   const long long n = (long long)out_h * out_w;
   float* minmax = static_cast<float*>(scratch);
-  float* q_a = minmax + (long long)kCrfChunkFloats * n_labels * maps_per_round;
+  float* q_a = minmax + (long long)kWordPartialFloats * n_labels * maps_per_round;
   float* q_b = q_a + (long long)n_labels * n * maps_per_round;
   for (int map0 = 0; map0 < n_maps; map0 += maps_per_round) {
     const int nm = std::min(maps_per_round, n_maps - map0);

@@ -51,7 +51,7 @@ DEV = 'cuda'
 THREADS = 256                # threads of every word-list CTA
 TILE_H, TILE_W = 16, 64      # kSegTileH x kSegTileW: a tile kernel's output tile
 STAGE_FLOATS = 12288         # kSegStageFloats: staged windows per pass when they fit (48 KB)
-MAX_CHUNKS = 32              # kMaxChunks
+MAX_CHUNKS = 32              # kWordChunks
 MAX_SMEM = 200 * 1024        # kMaxSmem
 SM_SMEM = 228 * 1024         # shared memory of an H100 SM; 1 KB of it is reserved per CTA
 N_ROWS = 40                  # rows of a synthetic global map: more than any word selects (map_stride > selected rows)
