@@ -7,6 +7,7 @@ ctypes releases the GIL around every foreign call.
 from __future__ import annotations
 
 import ctypes
+import math
 import os
 from typing import Optional, Sequence, Tuple
 
@@ -151,6 +152,40 @@ def distance_plane_bytes(out_h: int, out_w: int) -> int:
     return 4 * out_h * out_w + 256
 
 
+SUPERPIXEL_MAX_CELLS = 65536      # DAAM_SUPERPIXEL_MAX_CELLS: the most cells (ny * nx) of the superpixel grid
+SUPERPIXEL_MAX_ITERATIONS = 64    # the most SLIC passes the superpixel calls take
+
+
+def superpixel_grid(out_h: int, out_w: int, n_segments: int):
+    """``(ny, nx)``: the superpixel calls' cell grid, ``S = sqrt(H W / K)`` in float64 and ``clamp(floor(H / S +
+    0.5), 1, H)`` rows, columns likewise (include/daam_b200.h)."""
+    s = math.sqrt(float(out_h * out_w) / n_segments)
+    return (min(max(math.floor(out_h / s + 0.5), 1), out_h), min(max(math.floor(out_w / s + 0.5), 1), out_w))
+
+
+def superpixel_image_bytes(ny: int, nx: int) -> int:
+    """``DAAM_SUPERPIXEL_IMAGE_BYTES(ny, nx)``: one image's SLIC state (two sets of six int64 sums per cell)."""
+    return 96 * ny * nx
+
+
+def superpixel_box(ny: int, nx: int, out_h: int, out_w: int) -> int:
+    """``DAAM_SUPERPIXEL_BOX(ny, nx, out_h, out_w)``: the most cells a 16 x 64 pixel tile's pixels can reach."""
+    return min(ny, 15 * ny // out_h + 4) * min(nx, 63 * nx // out_w + 4)
+
+
+def superpixel_map_bytes(n_words: int, ny: int, nx: int, out_h: int, out_w: int) -> int:
+    """``DAAM_SUPERPIXEL_MAP_BYTES(n_words, ny, nx, out_h, out_w)``: one map's min / max partials, per-tile sums of
+    each word over each cell of the tile's box, and per-superpixel label and score."""
+    tiles = ((out_h + 15) // 16) * ((out_w + 63) // 64)
+    return 256 * n_words + 8 * ny * nx + 8 * n_words * tiles * superpixel_box(ny, nx, out_h, out_w)
+
+
+def superpixel_scratch_bytes(n_images: int, n_maps: int, n_words: int, ny: int, nx: int, out_h: int, out_w: int) -> int:
+    """``DAAM_SUPERPIXEL_SCRATCH_BYTES(...)``: ``n_images`` images' state and ``n_maps`` maps' buffers; ``(1, 1)`` is
+    the smallest scratch daam_segment_superpixels takes."""
+    return n_images * superpixel_image_bytes(ny, nx) + n_maps * superpixel_map_bytes(n_words, ny, nx, out_h, out_w)
+
+
 def overlay_frames_bytes(n_maps: int, n_words: int, out_h: int, out_w: int) -> int:
     """``DAAM_OVERLAY_FRAMES_BYTES(n_maps, n_words, out_h, out_w)``: the frames rounded up to whole 4-byte words."""
     return (n_maps * n_words * out_h * out_w * 3 + 3) // 4 * 4
@@ -158,7 +193,7 @@ def overlay_frames_bytes(n_maps: int, n_words: int, out_h: int, out_w: int) -> i
 
 EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize',
            'daam_finalize_maps', 'daam_finalize_parts', 'daam_finalize_per_key','daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
-           'daam_segment_words', 'daam_region_overlap', 'daam_region_sweep', 'daam_region_ranking', 'daam_region_boundary', 'daam_mask_boundary', 'daam_word_overlap', 'daam_word_instances', 'daam_overlay_words', 'daam_refine_words', 'daam_segment_crf', 'daam_word_distance', 'daam_mask_distance', 'daam_jet_colormap',
+           'daam_segment_words', 'daam_region_overlap', 'daam_region_sweep', 'daam_region_ranking', 'daam_region_boundary', 'daam_mask_boundary', 'daam_word_overlap', 'daam_word_instances', 'daam_overlay_words', 'daam_refine_words', 'daam_segment_crf', 'daam_word_distance', 'daam_mask_distance', 'daam_image_superpixels', 'daam_segment_superpixels', 'daam_jet_colormap',
            'daam_side_launcher_create', 'daam_side_launcher_destroy',
            'daam_side_launcher_launch', 'daam_side_launcher_join', 'daam_side_launcher_idle', 'daam_abi_version',
            'daam_last_error', 'daam_device_info', 'daam_launch_count')
@@ -299,6 +334,11 @@ def load() -> ctypes.CDLL:
     lib.daam_word_distance.restype = ctypes.c_int
     lib.daam_mask_distance.argtypes = [vp, i32, i32, i32, vp, vp]
     lib.daam_mask_distance.restype = ctypes.c_int
+    lib.daam_image_superpixels.argtypes = [vp, i32, i32, i32, i32, f32, i32, vp, vp, i64, vp]
+    lib.daam_image_superpixels.restype = ctypes.c_int
+    lib.daam_segment_superpixels.argtypes = [vp, i32, i32, i32, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), i32, i32,
+                                             i32, i32, i32, f32, i32, f32, i32, vp, vp, i64, vp, vp, vp, vp, i64, vp]
+    lib.daam_segment_superpixels.restype = ctypes.c_int
     lib.daam_jet_colormap.argtypes = [vp]
     lib.daam_jet_colormap.restype = ctypes.c_int
     lib.daam_side_launcher_create.argtypes = [ctypes.POINTER(vp)]
@@ -704,6 +744,34 @@ def segment_crf(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Seque
                                    float(smoothness), float(sigma_smooth), vp(word_maps_ptr), vp(image_ptr),
                                    image_map_stride, vp(labels_ptr), vp(scores_ptr), vp(probs_ptr) if probs_ptr else None,
                                    vp(scratch_ptr), scratch_bytes, vp(stream)))
+
+
+def image_superpixels(image_ptr: int, n_images: int, out_h: int, out_w: int, n_segments: int, compactness: float,
+                      iterations: int, superpixels_ptr: int, scratch_ptr: int, scratch_bytes: int, stream: int):
+    """``daam_image_superpixels`` over ``n_images`` uint8 images ``[out_h, out_w, 3]`` back to back: ``superpixels``
+    int32 ``[n_images, out_h, out_w]``; ``scratch_bytes`` of scratch, at least :func:`superpixel_image_bytes`."""
+    vp = ctypes.c_void_p
+    _check(load().daam_image_superpixels(vp(image_ptr), n_images, out_h, out_w, int(n_segments), float(compactness),
+                                         int(iterations), vp(superpixels_ptr), vp(scratch_ptr), scratch_bytes,
+                                         vp(stream)))
+
+
+def segment_superpixels(maps_ptr: int, n_maps: int, n_rows: int, x, rows_per_word: Sequence[Sequence[int]],
+                        out_h: int, out_w: int, absolute: bool, threshold: Optional[float], n_segments: int,
+                        compactness: float, iterations: int, word_maps_ptr: int, image_ptr: int,
+                        image_map_stride: int, labels_ptr: int, scores_ptr: int, superpixels_ptr: int,
+                        scratch_ptr: int, scratch_bytes: int, stream: int):
+    """``daam_segment_superpixels`` over ``n_maps`` maps ``[n_rows, h, w]`` back to back; ``image_ptr`` uint8
+    ``[out_h, out_w, 3]``, map ``i``'s at ``image_ptr + i * image_map_stride`` bytes (0: one image for all); ``labels``
+    uint8 and ``scores`` fp32 ``[n_maps, out_h, out_w]``; ``superpixels`` int32 ``[out_h, out_w]`` (one image) or
+    ``[n_maps, out_h, out_w]``; ``scratch_bytes`` of scratch, at least :func:`superpixel_scratch_bytes` ``(1, 1,
+    ...)``."""
+    vp = ctypes.c_void_p
+    _check(load().daam_segment_superpixels(vp(maps_ptr), n_maps, n_rows,
+                                           *_word_list(x, rows_per_word, out_h, out_w, absolute, threshold),
+                                           int(n_segments), float(compactness), int(iterations), vp(word_maps_ptr),
+                                           vp(image_ptr), image_map_stride, vp(labels_ptr), vp(scores_ptr),
+                                           vp(superpixels_ptr), vp(scratch_ptr), scratch_bytes, vp(stream)))
 
 
 def jet_colormap():

@@ -23,9 +23,11 @@
 //  - refine.cu recomputes it from segment_minmax_kernel's word maps and partials and filters it with the image as
 //    guide (daam_refine_words);
 //  - crf.cu recomputes it the same way as the unary logits of a Potts CRF with the image as bilateral guide
-//    (daam_segment_crf).
+//    (daam_segment_crf);
+//  - superpixels.cu recomputes it the same way and averages it over each SLIC superpixel of the image, whose words
+//    then compete per superpixel (daam_segment_superpixels).
 // word_value.cuh defines m's pieces (word_mean, partial_bounds, minmax_normalize): every consumer's m, here and in
-// refine.cu and crf.cu, is built from them and is expand_words_kernel's value bit for bit. The tile kernels run after
+// refine.cu, crf.cu and superpixels.cu, is built from them and is expand_words_kernel's value bit for bit. The tile kernels run after
 // segment_minmax_kernel (steps 1 and 2, the word maps and min / max partials to global memory) and share the tile
 // helpers (block_tile / tile_at, word_bounds, stage_windows, tap tables, and tile_value in the two that also run
 // without staged windows). expand_words_kernel, segment_minmax_kernel and segment_label_kernel keep their steps
@@ -46,6 +48,7 @@
 #include "distance.cuh"
 #include "ranking.cuh"
 #include "refine.cuh"
+#include "superpixels.cuh"
 #include "word_value.cuh"
 
 namespace daam {
@@ -1164,7 +1167,8 @@ static int tile_count(const WordListParams& p) {
   return ((p.oh + kSegTileH - 1) / kSegTileH) * ((p.ow + kSegTileW - 1) / kSegTileW);
 }
 
-// Launch 1 of the tile entry points, and all of it for daam_refine_words and daam_segment_crf: segment_minmax_kernel over (map, word, chunk)
+// Launch 1 of the tile entry points, and all of it for daam_refine_words, daam_segment_crf and daam_segment_superpixels:
+// segment_minmax_kernel over (map, word, chunk)
 // with enough CTAs for a few waves, at most kWordChunks per word and one per 256 pixels. Sets p.chunks.
 static int launch_word_maps(WordListParams& p, int n_maps, const DeviceInfo& dev, cudaStream_t stream) {
   const long long n = (long long)p.oh * p.ow, mwords = (long long)n_maps * p.n_words;
@@ -1648,6 +1652,64 @@ extern "C" int daam_segment_crf(const float* global_maps, int32_t n_maps, int32_
     c.labels = labels + map0 * n; c.scores = scores + map0 * n;
     if (int rc = launch_crf(c, iterations, q_a, q_b, probs ? probs + (long long)map0 * n_labels * n : nullptr,
                             dev.device, stream)) return rc;
+  }
+  return DAAM_OK;
+}
+
+extern "C" int daam_segment_superpixels(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t mh,
+                                        int32_t mw, const int32_t* rows, const int32_t* row_begin, int32_t n_words,
+                                        int32_t out_h, int32_t out_w, int32_t absolute, int32_t use_threshold,
+                                        float threshold, int32_t n_segments, float compactness, int32_t iterations,
+                                        float* word_maps, const uint8_t* image, int64_t image_map_stride,
+                                        uint8_t* labels, float* scores, int32_t* superpixels, void* scratch,
+                                        int64_t scratch_bytes, void* stream_) {
+  const char* name = "daam_segment_superpixels";
+  if (!global_maps || !rows || !row_begin || !word_maps || !image || !labels || !scores || !superpixels || !scratch ||
+      n_maps <= 0 || mh <= 0 || mw <= 0 || out_h <= 0 || out_w <= 0 || n_rows <= 0 || image_map_stride < 0) { set_error("%s: null pointer or non-positive size", name); return DAAM_E_INVALID; }
+  if ((long long)out_h * out_w > (1LL << 24)) { set_error("%s: a %d x %d output is more than 2^24 pixels", name, out_h, out_w); return DAAM_E_UNSUPPORTED; }
+  if (n_segments < 1) { set_error("%s: n_segments %d < 1", name, n_segments); return DAAM_E_INVALID; }
+  if (!(compactness > 0.f) || !isfinite(compactness)) { set_error("%s: compactness %g is not finite and > 0", name, (double)compactness); return DAAM_E_INVALID; }
+  if (iterations < 1 || iterations > kSuperpixelMaxIterations) { set_error("%s: iterations %d is not in [1, %d]", name, iterations, kSuperpixelMaxIterations); return DAAM_E_INVALID; }
+  const SlicGrid g = slic_grid(out_h, out_w, n_segments, compactness);
+  if (g.cells > kSuperpixelMaxCells) { set_error("%s: a %d x %d grid of cells is more than %d", name, g.ny, g.nx, kSuperpixelMaxCells); return DAAM_E_UNSUPPORTED; }
+  if ((uintptr_t)scratch & 7) { set_error("%s: scratch must be 8-byte aligned", name); return DAAM_E_INVALID; }
+  const long long image_bytes = superpixel_image_bytes(g.cells), map_bytes = superpixel_map_bytes(n_words, g);
+  if (scratch_bytes < image_bytes + map_bytes) { set_error("%s: %lld scratch bytes < %lld, one image and one %d-word map", name, (long long)scratch_bytes, image_bytes + map_bytes, n_words); return DAAM_E_INVALID; }
+  static thread_local WordListParams p, q;
+  DeviceInfo dev;
+  if (int rc = word_list_prepare(name, global_maps, n_maps, n_rows, mh, mw, rows, row_begin, n_words, out_h, out_w,
+                                 absolute, !absolute, 0, 0.f, word_maps, nullptr, true, p, &dev)) return rc;
+  const cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  // a round: as many whole maps as the scratch holds (a superpixel's pixels are pooled in one pass); one image's
+  // partition serves every map, or each map has its own
+  const bool per_map = image_map_stride != 0;
+  const long long whole = per_map ? scratch_bytes / (image_bytes + map_bytes) : (scratch_bytes - image_bytes) / map_bytes;
+  const int maps_per_round = (int)std::min<long long>(std::min<long long>(whole, 65535), n_maps);
+  SlicParams s;
+  PoolParams c;
+  s.g = c.g = g;
+  superpixel_scratch_in(scratch, per_map ? maps_per_round : 1, maps_per_round, n_words, g, s, c);
+  float* minmax = const_cast<float*>(c.minmax);
+  s.image_stride = image_map_stride;
+  c.per_map = per_map ? 1 : 0; c.n_words = n_words; c.mh = mh; c.mw = mw; c.absolute = p.absolute;
+  c.use_threshold = use_threshold ? 1 : 0; c.threshold = use_threshold ? threshold : 0.f;
+  const long long n = (long long)out_h * out_w;
+  for (int map0 = 0; map0 < n_maps; map0 += maps_per_round) {
+    const int nm = std::min(maps_per_round, n_maps - map0);
+    q = p;
+    q.maps = global_maps + map0 * p.map_stride;
+    q.word_maps = word_maps + (long long)map0 * n_words * mh * mw;
+    q.scratch = minmax;
+    if (int rc = launch_word_maps(q, nm, dev, stream)) return rc;
+    if (per_map || map0 == 0) {
+      s.images = per_map ? nm : 1;
+      s.image = image + map0 * image_map_stride;
+      s.superpixels = superpixels + (per_map ? map0 * n : 0);
+      if (int rc = launch_slic(s, iterations, dev.device, stream)) return rc;
+    }
+    c.word_maps = q.word_maps; c.chunks = q.chunks; c.maps = nm; c.superpixels = s.superpixels;
+    c.labels = labels + map0 * n; c.scores = scores + map0 * n;
+    if (int rc = launch_pool(c, stream)) return rc;
   }
   return DAAM_OK;
 }

@@ -42,6 +42,10 @@ To grow, shrink or feather a mask -- a word's mask as an inpainting mask, its co
 blobs closed -- use :meth:`GlobalHeatMap.word_distance <daam_b200.heatmap.GlobalHeatMap.word_distance>` on the
 thresholded word masks, or :func:`distance_transform` on any device masks: the exact signed distance transform, whose
 ``mask(r)``, ``soft_mask(r, feather=f)`` and ``distance()`` are the edits.
+To let the words compete per region of the image rather than per pixel, use :meth:`GlobalHeatMap.segment_superpixels
+<daam_b200.heatmap.GlobalHeatMap.segment_superpixels>` / :meth:`GlobalHeatMapStack.segment_superpixels
+<daam_b200.heatmap.GlobalHeatMapStack.segment_superpixels>`: each word's mean over each SLIC superpixel, the labels
+constant over each; :func:`superpixels` gives the partition alone.
 """
 from __future__ import annotations
 
@@ -49,7 +53,7 @@ import torch
 
 from . import _native
 
-__all__ = ['compute_iou', 'compute_ioa', 'boundary_scores', 'distance_transform']
+__all__ = ['compute_iou', 'compute_ioa', 'boundary_scores', 'distance_transform', 'superpixels']
 
 
 def _match_size(a: torch.Tensor, b: torch.Tensor) -> torch.Tensor:
@@ -167,4 +171,35 @@ def distance_transform(masks: torch.Tensor, to_cpu: bool = True):
         with torch.cuda.device(masks.device):
             _native.mask_distance(mask_bytes.data_ptr(), masks.numel() // (out_h * out_w), out_h, out_w,
                                   out.signed_d2.data_ptr(), _stream_ptr(masks.device))
+    return out.cpu() if to_cpu else out
+
+
+def superpixels(image: torch.Tensor, n_segments: int = 1024, compactness: float = 20.0, iterations: int = 10,
+                to_cpu: bool = True):
+    """SLIC superpixels of device images: the partition :meth:`GlobalHeatMap.segment_superpixels
+    <daam_b200.heatmap.GlobalHeatMap.segment_superpixels>` pools over, with the same arguments and the same bits.
+    ``image``: uint8 ``[H, W, 3]`` or ``[N, H, W, 3]`` RGB on a CUDA device. ``compactness`` is on the 0-255 RGB scale
+    (the default of 20 is twice skimage's Lab default, because RGB differences run larger than Lab's). Returns int32
+    ``[H, W]`` or ``[N, H, W]``, each pixel's cluster id ``cy * nx + cx`` (superpixels may be disconnected and empty
+    clusters leave ids unused), on the CPU unless ``to_cpu=False``. ``2 * iterations`` launches. An empty shape
+    launches nothing. At most 2**24 pixels and 65536 cells; ``n_segments`` >= 1, ``compactness`` finite and > 0,
+    ``iterations`` in ``[1, 64]`` (a ``ValueError`` otherwise)."""
+    from .heatmap import _image_superpixels, _require_cuda, _superpixel_args, _superpixel_grid
+    what = 'superpixels'
+    if not isinstance(image, torch.Tensor):
+        raise TypeError(f'{what}: image must be a torch.Tensor, not {type(image).__name__}')
+    if image.dtype != torch.uint8:
+        raise TypeError(f'{what}: image must be uint8, not {image.dtype}')
+    if image.dim() not in (3, 4) or image.shape[-1] != 3:
+        raise ValueError(f'{what}: image must be [H, W, 3] or [N, H, W, 3], not {tuple(image.shape)}')
+    _require_cuda(image, what)
+    out_h, out_w = int(image.shape[-3]), int(image.shape[-2])
+    _superpixel_args(out_h, out_w, n_segments, compactness, iterations, what)
+    n_images = image.numel() // (3 * out_h * out_w) if out_h * out_w else 0
+    if n_images == 0:
+        out = torch.empty(image.shape[:-1], dtype=torch.int32, device=image.device)
+    else:
+        ny, nx = _superpixel_grid(out_h, out_w, n_segments, what)
+        out = _image_superpixels(image.detach().contiguous(), n_images, out_h, out_w, n_segments, compactness,
+                                 iterations, ny, nx).view(image.shape[:-1])
     return out.cpu() if to_cpu else out

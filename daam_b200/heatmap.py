@@ -646,6 +646,43 @@ class GlobalHeatMap:
                                               'GlobalHeatMap.segment_crf', stack=False)
         return (wl.word_heat_maps(0), labels[0], scores[0]) + ((q[0][0],) if probs else ())
 
+    def segment_superpixels(self, words, image, n_segments: int = 1024, compactness: float = 20.0,
+                            iterations: int = 10, threshold: Optional[float] = None, absolute: bool = False,
+                            word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
+        """Superpixel word segmentation: the words compete per region of the image rather than per pixel, so the
+        labels are constant over regions that follow the image's edges instead of the heat-map grid.
+
+        The image is cut into SLIC superpixels (Achanta et al., TPAMI 2012), in the pixel-centric form on the RGB
+        bytes with every step defined exactly (``include/daam_b200.h``): a grid of about ``n_segments`` cells, each
+        cluster started from its cell's middle pixel, and ``iterations`` passes in which each pixel joins the nearest
+        of the 9 clusters around its cell by ``|RGB - centre|^2 + wxy |yx - centre|^2``, ``wxy = compactness^2 *
+        cells / (H W)``. ``compactness`` is on the 0-255 RGB scale: larger values give squarer superpixels, smaller
+        ones follow colour more closely. The default of 20 is twice skimage's Lab default of 10 because RGB
+        differences run larger than Lab's; nobody has measured which value segments DAAM maps best. Superpixels may
+        be disconnected (there is no connectivity step).
+
+        With ``m[w]`` what ``expand_words(words, image, absolute, word_idx=word_idx, offset_idx=offset_idx)`` returns
+        (no threshold), each superpixel ``s`` gets ``mean[w] = fp32(sum_{p in s} m[w](p) / |s|)`` (the sum in float64
+        in a fixed order), ``label = 1 + argmax_w mean[w]`` (the first word on ties), set to 0 (background) where
+        ``threshold`` is in effect (Python truthiness, as in :meth:`segment`) and ``max mean > threshold`` fails, and
+        ``score = max_w mean[w]``; every pixel takes its superpixel's. With ``n_segments = H * W`` every superpixel
+        is one pixel and ``labels`` / ``scores`` equal :meth:`segment`'s bit for bit.
+
+        Returns ``(word_heat_maps, labels, scores, superpixels)``: the list of :class:`WordHeatMap` that
+        :meth:`segment` returns, ``labels`` uint8, ``scores`` fp32 and ``superpixels`` int32 (each pixel's cluster
+        id, ``cy * nx + cx``; empty clusters leave ids unused), all ``(H, W)``, CPU by default, ``to_cpu=False``
+        keeps them on the device. The results are the same bits on every call.
+
+        ``image``: as :meth:`overlay_words` takes it. ``n_segments`` an integer >= 1 whose grid has at most 65536
+        cells, ``compactness`` finite and > 0, ``iterations`` an integer in ``[1, 64]``, at most 2**24 pixels (a
+        ``ValueError`` otherwise); at most 96 words. An empty word list still makes the partition: every pixel is
+        background with score -inf. Raises the reference's ``ValueError`` for a word that is not in the prompt."""
+        wl, labels, scores, sp = _segment_superpixels(self.tokenizer, self.prompt, self.heat_maps[None], words, image,
+                                                      n_segments, compactness, iterations, threshold, absolute,
+                                                      word_idx, offset_idx, to_cpu, 'GlobalHeatMap.segment_superpixels',
+                                                      stack=False)
+        return wl.word_heat_maps(0), labels[0], scores[0], sp
+
 
 def _check_rows(rows, n_rows: int):
     """Raises the ``IndexError`` torch's advanced indexing raises on a row out of ``[-n_rows, n_rows)``."""
@@ -1537,6 +1574,92 @@ def _segment_crf(tokenizer, prompt: str, maps: torch.Tensor, words, image, thres
     return wl.done(labels, scores, *([q] if probs else []))
 
 
+# Scratch of one segment_superpixels call: each image's SLIC state (96 bytes a cell) and each map's per-tile sums (8
+# bytes per word and cell of a tile's box); as many whole maps as fit go in a round, so memory does not grow with the
+# number of maps; one image and one map larger than the budget go alone.
+SUPERPIXEL_SCRATCH_BYTES = 256 << 20
+
+
+def _superpixel_args(out_h: int, out_w: int, n_segments, compactness, iterations, what: str):
+    """Raises ``ValueError`` unless the image has at most 2**24 pixels, ``n_segments`` is an integer >= 1,
+    ``compactness`` rounded to fp32 is finite and > 0 and ``iterations`` is an integer in ``[1, 64]`` -- the superpixel
+    calls' checks, in their order. The cell limit (:func:`_superpixel_grid`) comes next."""
+    if out_h * out_w > 1 << 24:
+        raise ValueError(f'{what}: a {out_h} x {out_w} image is more than 2**24 pixels')
+    if isinstance(n_segments, bool) or not isinstance(n_segments, int) or n_segments < 1:
+        raise ValueError(f'{what}: n_segments must be an integer >= 1, not {n_segments!r}')
+    try:
+        c32 = ctypes.c_float(float(compactness)).value
+    except (TypeError, ValueError):
+        raise ValueError(f'{what}: compactness must be a number, not {compactness!r}') from None
+    if not (math.isfinite(c32) and c32 > 0):
+        raise ValueError(f'{what}: compactness must be finite and > 0 in fp32, not {compactness!r}')
+    top = _native.SUPERPIXEL_MAX_ITERATIONS
+    if isinstance(iterations, bool) or not isinstance(iterations, int) or not 1 <= iterations <= top:
+        raise ValueError(f'{what}: iterations must be an integer in [1, {top}], not {iterations!r}')
+
+
+def _superpixel_grid(out_h: int, out_w: int, n_segments: int, what: str):
+    """``(ny, nx)``, the cell grid of an ``out_h x out_w`` image; ``ValueError`` beyond 65536 cells."""
+    ny, nx = _native.superpixel_grid(out_h, out_w, n_segments)
+    if ny * nx > _native.SUPERPIXEL_MAX_CELLS:
+        raise ValueError(f'{what}: {n_segments} segments of a {out_h} x {out_w} image make a {ny} x {nx} grid, more '
+                         f'than {_native.SUPERPIXEL_MAX_CELLS} cells')
+    return ny, nx
+
+
+def _image_superpixels(image: torch.Tensor, n_images: int, out_h: int, out_w: int, n_segments, compactness,
+                       iterations, ny: int, nx: int) -> torch.Tensor:
+    """``daam_image_superpixels`` of ``n_images`` device images back to back: int32 ``[n_images, out_h, out_w]``.
+    Scratch: :data:`SUPERPIXEL_SCRATCH_BYTES`, clipped to what the call has, at least one image."""
+    dev = image.device
+    out = torch.empty((n_images, out_h, out_w), dtype=torch.int32, device=dev)
+    one = _native.superpixel_image_bytes(ny, nx)
+    n_bytes = max(one, min(SUPERPIXEL_SCRATCH_BYTES // one * one, n_images * one))
+    scratch = torch.empty(n_bytes, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _native.image_superpixels(image.data_ptr(), n_images, out_h, out_w, n_segments, compactness, iterations,
+                                  out.data_ptr(), scratch.data_ptr(), n_bytes, _stream_ptr(dev))
+    return out
+
+
+def _segment_superpixels(tokenizer, prompt: str, maps: torch.Tensor, words, image, n_segments, compactness,
+                         iterations, threshold, absolute, word_idx, offset_idx: int, to_cpu: bool, what: str,
+                         stack: bool):
+    """``daam_segment_superpixels`` over ``maps`` ``[n_maps, n_rows, xh, xw]``: returns ``(wl, labels, scores,
+    superpixels)``, ``labels`` uint8 and ``scores`` fp32 ``[n_maps, H, W]``, ``superpixels`` int32 ``[H, W]`` for one
+    image or ``[n_maps, H, W]`` for one per map. Checks as :func:`_overlay`, in its order, then the superpixel
+    arguments (:func:`_superpixel_args`, :func:`_superpixel_grid`). An empty word list still makes the partition."""
+    wl = _WordList(tokenizer, prompt, maps, words, word_idx, offset_idx, None, absolute, threshold, to_cpu, what,
+                   on_grid=True)         # the size is the image's, once _overlay_image has checked it
+    n_maps, n_words, dev = wl.n_maps, len(wl.words), wl.dev
+    image, wl.out_h, wl.out_w, per_map = _overlay_image(image, n_maps, wl.grid, dev, what, stack)
+    h, w = wl.out_h, wl.out_w
+    _superpixel_args(h, w, n_segments, compactness, iterations, what)
+    ny, nx = _superpixel_grid(h, w, n_segments, what)
+    shape = (n_maps, h, w)
+    n_images = n_maps if per_map else 1
+    if wl.empty:                         # no word: every pixel is background with score -inf, as segment
+        sp = torch.empty((n_images, h, w), dtype=torch.int32, device=dev)
+        if n_images:
+            sp = _image_superpixels(image.to(dev).contiguous(), n_images, h, w, n_segments, compactness, iterations,
+                                    ny, nx)
+        return wl.done(torch.zeros(shape, dtype=torch.uint8, device=dev),
+                       torch.full(shape, float('-inf'), device=dev), sp if per_map else sp[0])
+    image = image.to(dev).contiguous()                   # one copy to the device
+    labels = torch.empty(shape, dtype=torch.uint8, device=dev)
+    scores = torch.empty(shape, dtype=torch.float32, device=dev)
+    sp = torch.empty((n_images, h, w), dtype=torch.int32, device=dev)
+    n_bytes = max(_native.superpixel_scratch_bytes(1, 1, n_words, ny, nx, h, w),
+                  min(SUPERPIXEL_SCRATCH_BYTES,
+                      _native.superpixel_scratch_bytes(n_images, n_maps, n_words, ny, nx, h, w)))
+    scratch = torch.empty(n_bytes, dtype=torch.uint8, device=dev)
+    wl.launch(_native.segment_superpixels, n_segments, compactness, iterations, wl.word_maps.data_ptr(),
+              image.data_ptr(), h * w * 3 if per_map else 0, labels.data_ptr(), scores.data_ptr(), sp.data_ptr(),
+              scratch.data_ptr(), n_bytes)
+    return wl.done(labels, scores, sp if per_map else sp[0])
+
+
 class GlobalHeatMapStack:
     """Global heat maps of one prompt's text stacked along a first axis: ``heat_maps[t]`` is one
     ``[n_rows, xh, xw]`` map. Base of :class:`TimeHeatMaps` (one map per step), :class:`ImageHeatMaps` (one per
@@ -1701,6 +1824,22 @@ class GlobalHeatMapStack:
                                               sigma_smooth, absolute, word_idx, offset_idx, probs, to_cpu,
                                               f'{type(self).__name__}.segment_crf', stack=True)
         return (wl.word_maps, labels, scores) + tuple(q)
+
+    def segment_superpixels(self, words, image, n_segments: int = 1024, compactness: float = 20.0,
+                            iterations: int = 10, threshold: Optional[float] = None, absolute: bool = False,
+                            word_idx=None, offset_idx: int = 0, to_cpu: bool = True):
+        """:meth:`GlobalHeatMap.segment_superpixels` for every map in one call: returns ``(word_maps, labels, scores,
+        superpixels)``, with ``word_maps`` the device ``[maps, len(words), xh, xw]`` word heat maps and ``labels`` /
+        ``scores`` ``[maps, H, W]``; row ``t`` equals ``self[t].segment_superpixels(...)`` bit for bit (min / max
+        normalisation per map and word). ``image`` is one image for every map, whose partition is made once and
+        pooled for every map (``superpixels`` ``[H, W]``), or a uint8 ``[maps, H, W, 3]`` array with one per map
+        (e.g. the images of ``compute_image_heat_maps()``; ``superpixels`` ``[maps, H, W]``). Scratch stays within a
+        fixed budget whatever the map count: the maps go in rounds of whole maps."""
+        wl, labels, scores, sp = _segment_superpixels(self.tokenizer, self.prompt, self.heat_maps, words, image,
+                                                      n_segments, compactness, iterations, threshold, absolute,
+                                                      word_idx, offset_idx, to_cpu,
+                                                      f'{type(self).__name__}.segment_superpixels', stack=True)
+        return wl.word_maps, labels, scores, sp
 
 
 class TimeHeatMaps(GlobalHeatMapStack):

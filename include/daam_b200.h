@@ -39,7 +39,8 @@ extern "C" {
                                           daam_region_ranking; daam_refine_words;
                                           daam_region_boundary, daam_mask_boundary;
                                           daam_segment_crf;
-                                          daam_word_distance, daam_mask_distance) */
+                                          daam_word_distance, daam_mask_distance;
+                                          daam_image_superpixels, daam_segment_superpixels) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_TOKENS 231     /* daam_accumulate: long contexts of 2 or 3 CLIP chunks of 77 tokens (154, 231) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
@@ -692,6 +693,80 @@ int daam_word_distance(const float* global_maps, int32_t n_maps, int32_t n_rows,
  */
 int daam_mask_distance(const uint8_t* masks, int32_t n_planes, int32_t out_h, int32_t out_w, int32_t* signed_d2,
                        void* stream);
+
+/*
+ * SLIC superpixels (Achanta et al., "SLIC Superpixels Compared to State-of-the-Art Superpixel Methods", TPAMI 2012) of
+ * n_images uint8 RGB images [n_images][out_h][out_w][3] stored back to back, in the pixel-centric form on the RGB bytes,
+ * every step defined exactly:
+ *   grid:   S = sqrt(H W / K) in float64 (K = n_segments), ny = clamp(floor(H / S + 0.5), 1, H), nx likewise with W;
+ *           cell row cy holds the pixel rows [floor(cy H / ny), floor((cy + 1) H / ny)), so pixel row y lies in cell row
+ *           floor(((y + 1) ny - 1) / H); columns likewise; cluster k = cy nx + cx, ny nx <= DAAM_SUPERPIXEL_MAX_CELLS;
+ *   start:  each cluster's sums (r, g, b, y, x, n), int64, are those of the one pixel ((y0 + y1 - 1) // 2,
+ *           (x0 + x1 - 1) // 2) of its cell [y0, y1) x [x0, x1) (no gradient perturbation);
+ *   pass:   each pixel takes, among the up to 9 clusters whose cells are within one cell row and column of its own,
+ *           the lowest D = ((dr dr + dg dg) + db db) + wxy ((dy dy) + (dx dx)), the differences to the centre
+ *           sum / n, every operation rounded separately in float64 (no FMA); wxy = c c (ny nx) / (H W) left to right
+ *           in float64, c = compactness (the RGB channels are 0..255); the lowest cluster wins a tie;
+ *   update: between the `iterations` passes each cluster's sums become the integer sums over its pixels; a cluster
+ *           without pixels keeps its sums.
+ * superpixels: int32 [n_images][out_h][out_w], each pixel's cluster after the last pass. Superpixels may be disconnected
+ * and an empty cluster leaves its id unused. The sums are integers (integer atomics, exact whatever their order) and
+ * the distances exact float64 operations: the results are the same bits on every call and whatever the scratch.
+ * scratch: device, 8-byte aligned, at least DAAM_SUPERPIXEL_IMAGE_BYTES(ny, nx): as many images go in a round as it
+ * holds, 2 * iterations launches a round (the start, one launch per pass, one update between passes).
+ * Limits (DAAM_E_UNSUPPORTED): out_h * out_w <= 2^24, ny nx <= DAAM_SUPERPIXEL_MAX_CELLS. DAAM_E_INVALID: a null
+ * pointer or non-positive size, then n_segments < 1, compactness not finite and > 0, iterations not in [1, 64], then
+ * (after the cell limit) scratch not 8-byte aligned or below one image.
+ */
+#define DAAM_SUPERPIXEL_MAX_CELLS 65536
+#define DAAM_SUPERPIXEL_IMAGE_BYTES(ny, nx) (96 * (int64_t)(ny) * (nx))
+/* the cells a 16 x 64 pixel tile's pixels can be assigned to lie in a box of at most this many */
+#define DAAM_SUPERPIXEL_BOX(ny, nx, out_h, out_w)                                                     \
+  ((int64_t)((ny) < 15 * (ny) / (out_h) + 4 ? (ny) : 15 * (ny) / (out_h) + 4) *                         \
+   ((nx) < 63 * (nx) / (out_w) + 4 ? (nx) : 63 * (nx) / (out_w) + 4))
+#define DAAM_SUPERPIXEL_MAP_BYTES(n_words, ny, nx, out_h, out_w)                                        \
+  (256 * (int64_t)(n_words) + 8 * (int64_t)(ny) * (nx) +                                                \
+   8 * (int64_t)(n_words) * (((out_h) + 15) / 16) * (((out_w) + 63) / 64) * DAAM_SUPERPIXEL_BOX(ny, nx, out_h, out_w))
+#define DAAM_SUPERPIXEL_SCRATCH_BYTES(n_images, n_maps, n_words, ny, nx, out_h, out_w)                  \
+  ((int64_t)(n_images) * DAAM_SUPERPIXEL_IMAGE_BYTES(ny, nx) +                                          \
+   (int64_t)(n_maps) * DAAM_SUPERPIXEL_MAP_BYTES(n_words, ny, nx, out_h, out_w))
+int daam_image_superpixels(const uint8_t* image, int32_t n_images, int32_t out_h, int32_t out_w, int32_t n_segments,
+                           float compactness, int32_t iterations, int32_t* superpixels, void* scratch,
+                           int64_t scratch_bytes, void* stream);
+
+/*
+ * Superpixel word segmentation: the words compete per SLIC superpixel of the image rather than per pixel, on each of
+ * n_maps global maps stored back to back. The partition is daam_image_superpixels' of the image, made inside the call:
+ * one for every map with image_map_stride 0, else one per map (map i's image at image + i * image_map_stride). With
+ * m[w] what daam_expand_words writes for word w WITHOUT threshold (same rows / row_begin / absolute) and n_s the
+ * pixel count of superpixel s:
+ *   mean[w][s] = fp32(sum_{p in s} m[w](p) / n_s), the sum in float64 in a fixed order (no float atomics);
+ *   labels[i][p] = 1 + argmax_w mean[w][s(p)] (the lowest word on ties), or 0 (background) where use_threshold and
+ *                  !(max_w mean[w][s(p)] > threshold); scores[i][p] = max_w mean[w][s(p)].
+ * labels: uint8 and scores: fp32 [n_maps][out_h][out_w]; superpixels: int32 [out_h][out_w] with one image, [n_maps]
+ * [out_h][out_w] with one per map. With one-pixel cells (n_segments = out_h * out_w) every superpixel is its pixel and
+ * labels / scores equal daam_segment_words' bit for bit. Each sum of m runs in an order fixed by pixel positions (per
+ * 16 x 64 tile in row-major order, then over the tiles in a fixed order) and the SLIC state is integer: the results
+ * are the same bits on every call and whatever the scratch.
+ * Arguments as daam_segment_crf without its CRF arguments, plus n_segments / compactness / iterations as
+ * daam_image_superpixels and the superpixels output. scratch: device, 8-byte aligned, at least
+ * DAAM_SUPERPIXEL_SCRATCH_BYTES(1, 1, n_words, ny, nx, out_h, out_w): each image's SLIC state
+ * (DAAM_SUPERPIXEL_IMAGE_BYTES) and each map's min / max partials, per-tile sums and per-superpixel results
+ * (DAAM_SUPERPIXEL_MAP_BYTES). A round takes as many whole maps (and with one image per map, their images) as the
+ * scratch holds and the call loops over the rounds: 4 launches a round (the word maps, the tile sums, the
+ * per-superpixel means, the labels), plus 2 * iterations for each round's partitions (the first round's only, with
+ * one image).
+ * Limits (DAAM_E_UNSUPPORTED): out_h * out_w <= 2^24 and ny nx <= DAAM_SUPERPIXEL_MAX_CELLS, then the word list's
+ * (n_words <= 96, as daam_segment_words). DAAM_E_INVALID: a null pointer or non-positive size, then n_segments < 1,
+ * compactness not finite and > 0, iterations not in [1, 64], then (after the cell limit) scratch not 8-byte aligned
+ * or below one image and one map, then the word list as daam_segment_words.
+ */
+int daam_segment_superpixels(const float* global_maps, int32_t n_maps, int32_t n_rows, int32_t map_h, int32_t map_w,
+                             const int32_t* rows, const int32_t* row_begin, int32_t n_words, int32_t out_h,
+                             int32_t out_w, int32_t absolute, int32_t use_threshold, float threshold,
+                             int32_t n_segments, float compactness, int32_t iterations, float* word_maps,
+                             const uint8_t* image, int64_t image_map_stride, uint8_t* labels, float* scores,
+                             int32_t* superpixels, void* scratch, int64_t scratch_bytes, void* stream);
 
 /* Library / device introspection. */
 int daam_abi_version(void);
