@@ -192,7 +192,7 @@ def overlay_frames_bytes(n_maps: int, n_words: int, out_h: int, out_w: int) -> i
 
 
 EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize',
-           'daam_finalize_maps', 'daam_finalize_parts', 'daam_finalize_per_key','daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
+           'daam_finalize_maps', 'daam_finalize_parts', 'daam_finalize_parts_weighted', 'daam_finalize_per_key', 'daam_value_norms','daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
            'daam_segment_words', 'daam_region_overlap', 'daam_region_sweep', 'daam_region_ranking', 'daam_region_boundary', 'daam_mask_boundary', 'daam_word_overlap', 'daam_word_instances', 'daam_overlay_words', 'daam_refine_words', 'daam_segment_crf', 'daam_word_distance', 'daam_mask_distance', 'daam_image_superpixels', 'daam_segment_superpixels', 'daam_jet_colormap',
            'daam_side_launcher_create', 'daam_side_launcher_destroy',
            'daam_side_launcher_launch', 'daam_side_launcher_join', 'daam_side_launcher_idle', 'daam_abi_version',
@@ -285,6 +285,11 @@ def load() -> ctypes.CDLL:
     lib.daam_finalize_parts.argtypes = [ctypes.POINTER(DaamKeyGroup), i32, ctypes.POINTER(DaamMapPart), i32, i32, i32,
                                         i32, vp]
     lib.daam_finalize_parts.restype = ctypes.c_int
+    lib.daam_finalize_parts_weighted.argtypes = [ctypes.POINTER(DaamKeyGroup), i32, ctypes.POINTER(DaamMapPart), i32,
+                                                 i32, i32, i32, ctypes.POINTER(vp), vp]
+    lib.daam_finalize_parts_weighted.restype = ctypes.c_int
+    lib.daam_value_norms.argtypes = [vp, i32, i64, i64, i64, vp, i32, i64, i32, i32, i32, i32, i32, vp, vp]
+    lib.daam_value_norms.restype = ctypes.c_int
     lib.daam_finalize_per_key.argtypes = [ctypes.POINTER(DaamKeyGroup), i32, i32, i32, i32, i32, vp, vp]
     lib.daam_finalize_per_key.restype = ctypes.c_int
     lib.daam_word_heat_map.argtypes = [vp, i32, i32, i32, ctypes.POINTER(i32), i32, vp, vp]
@@ -505,10 +510,13 @@ def finalize_maps(groups: Sequence[DaamKeyGroup], maps: Sequence[DaamMapSel], x,
         _check(lib.daam_finalize_maps(arr, n, sel, len(part), h, w, int(bool(normalize)), ctypes.c_void_p(stream)))
 
 
-def finalize_parts(groups: Sequence[DaamKeyGroup], parts: Sequence[DaamMapPart], x, normalize: bool, stream: int):
+def finalize_parts(groups: Sequence[DaamKeyGroup], parts: Sequence[DaamMapPart], x, normalize: bool, stream: int,
+                   weights: Optional[Sequence[int]] = None):
     """``daam_finalize_parts``: one :class:`DaamMapPart` per output map, each a range of ``groups``. More than
     :data:`FINALIZE_MAX_MAPS` maps go out in several calls, which changes no map's bits. A part that is no range of
-    ``groups``, or has no rows or output, is a ``ValueError`` before anything is loaded or launched."""
+    ``groups``, or has no rows or output, is a ``ValueError`` before anything is loaded or launched. ``weights``: one
+    device pointer per group (``[heads, tokens]`` fp32) -- ``daam_finalize_parts_weighted``; a list of another length
+    is a ``ValueError``."""
     h, w = map_size(x)
     n = len(groups)
     if not parts:
@@ -518,12 +526,28 @@ def finalize_parts(groups: Sequence[DaamKeyGroup], parts: Sequence[DaamMapPart],
             raise ValueError(f'finalize_parts: map {i} reads groups [{part.group_begin}, +{part.group_count}) of {n}')
         if part.n_rows <= 0 or not part.out:
             raise ValueError(f'finalize_parts: map {i} has no rows or no output')
+    if weights is not None and len(weights) != n:
+        raise ValueError(f'finalize_parts: {len(weights)} weight pointers for {n} key groups')
     arr = (DaamKeyGroup * n)(*groups)
     lib = load()
+    wts = None if weights is None else (ctypes.c_void_p * n)(*weights)
     for i in range(0, len(parts), FINALIZE_MAX_MAPS):
         chunk = parts[i:i + FINALIZE_MAX_MAPS]
         sel = (DaamMapPart * len(chunk))(*chunk)
-        _check(lib.daam_finalize_parts(arr, n, sel, len(chunk), h, w, int(bool(normalize)), ctypes.c_void_p(stream)))
+        if wts is None:
+            _check(lib.daam_finalize_parts(arr, n, sel, len(chunk), h, w, int(bool(normalize)), ctypes.c_void_p(stream)))
+        else:
+            _check(lib.daam_finalize_parts_weighted(arr, n, sel, len(chunk), h, w, int(bool(normalize)), wts,
+                                                    ctypes.c_void_p(stream)))
+
+
+def value_norms(value_ptr: int, value_dtype: int, v_strides: Tuple[int, int, int], w_ptr: int, w_dtype: int,
+                w_stride_row: int, n_samples: int, heads: int, tokens: int, head_dim: int, out_dim: int, out_ptr: int,
+                stream: int):
+    """``daam_value_norms``: ``v_strides`` = (sample, token, head) element strides of the value projection."""
+    _check(load().daam_value_norms(ctypes.c_void_p(value_ptr), value_dtype, *v_strides, ctypes.c_void_p(w_ptr), w_dtype,
+                                   w_stride_row, n_samples, heads, tokens, head_dim, out_dim, ctypes.c_void_p(out_ptr),
+                                   ctypes.c_void_p(stream)))
 
 
 def finalize_per_key(groups: Sequence[DaamKeyGroup], x, n_rows: int, normalize: bool, out_ptr: int, stream: int):

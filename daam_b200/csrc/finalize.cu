@@ -49,10 +49,15 @@ struct FinalizeParams {
   // fast kernel only: keys per block of the groups before g that have g's size (the same for every map of the launch)
   int class_keys_before[kMaxGroups];
   MapSel map[kMaxMaps];                   // blockIdx.z selects the map
+  // weighted instances only: the [n_blocks][heads][tokens] weights of group g (its acc layout with h * w = 1), or null.
+  // Last, so that the fields the plain instances read keep their offsets.
+  const float* w[kMaxGroups];
 };
 
 // grid: (ceil(oh*ow / 256), max n_rows, n_maps). One thread = one output element (map, row t, pixel o); it walks every
-// selected key: group by group, block by block, head by head.
+// selected key: group by group, block by block, head by head. kWeighted: each clamped key value is scaled by its weight,
+// `sum = fmaf(w, clamp(v), sum)`, instead of added.
+template <bool kWeighted>
 __global__ void __launch_bounds__(256) finalize_kernel(const __grid_constant__ FinalizeParams P) {
   const int o = blockIdx.x * blockDim.x + threadIdx.x;
   const int t = blockIdx.y;
@@ -77,7 +82,18 @@ __global__ void __launch_bounds__(256) finalize_kernel(const __grid_constant__ F
     const long long head_stride = (long long)G.tokens * hw;
     for (int b = M.block_begin; b < M.block_begin + M.block_count; ++b) {
       const float* base = G.acc + (long long)b * G.heads * head_stride + (long long)t * hw;
-      if (same) {   // scale 1: the cubic weights are exactly (0, 1, 0, 0)
+      if constexpr (kWeighted) {
+        const float* wb = P.w[g] + ((long long)b * G.heads) * G.tokens + t;
+        if (same) {
+#pragma unroll 4
+          for (int head = h0; head < h1; ++head)
+            sum = fmaf(__ldg(wb + head * G.tokens), fmaxf(__ldg(base + head * head_stride + o), 0.f), sum);
+        } else {
+#pragma unroll 2
+          for (int head = h0; head < h1; ++head)
+            sum = fmaf(__ldg(wb + head * G.tokens), fmaxf(bicubic_at(base + head * head_stride, G.w, ty, tx), 0.f), sum);
+        }
+      } else if (same) {   // scale 1: the cubic weights are exactly (0, 1, 0, 0)
 #pragma unroll 4
         for (int head = h0; head < h1; ++head) sum += fmaxf(__ldg(base + head * head_stride + o), 0.f);
       } else {
@@ -124,8 +140,9 @@ struct PhaseWeights {
   }
 };
 
-template <int F>
-__device__ __forceinline__ void add_key(const PhaseWeights<F>& pw, const float (&v)[5][5], float (&acc)[F][F]) {
+template <int F, bool kWeighted>
+__device__ __forceinline__ void add_key(const PhaseWeights<F>& pw, const float (&v)[5][5], float (&acc)[F][F],
+                                        float weight) {
   float r[5][F];                                       // horizontal pass, per source row and output phase
 #pragma unroll
   for (int i = 0; i < 5; ++i)
@@ -145,7 +162,8 @@ __device__ __forceinline__ void add_key(const PhaseWeights<F>& pw, const float (
       float o = 0.f;
 #pragma unroll
       for (int i = 0; i < 4; ++i) o += pw.w[py][i] * r[off + i][px];
-      acc[py][px] += fmaxf(o, 0.f);
+      if constexpr (kWeighted) acc[py][px] = fmaf(weight, fmaxf(o, 0.f), acc[py][px]);
+      else acc[py][px] += fmaxf(o, 0.f);
     }
   }
 }
@@ -215,10 +233,11 @@ struct NextClass {
 };
 
 // `first_buf`: the chunk buffer holding this class's chunk 0 (1 when the previous class prefetched it, else 0 and the
-// chunk is issued here).
-template <int F>
+// chunk is issued here). `weights`: the class's key weights, parallel to `keys` (kWeighted only).
+template <int F, bool kWeighted>
 __device__ __forceinline__ void class_pass(const FinalizeParams& P, int kh, int kw, int nk, int band, int br, float* tile,
-                                           const float* const* keys, float* stage, bool prefetched, const NextClass& next) {
+                                           const float* const* keys, const float* weights, float* stage, bool prefetched,
+                                           const NextClass& next) {
   const int ow = P.ow;
   const ChunkGeom G(kw, F, br);
   const int region = G.region, n_src = G.n_src, kg = G.kg, kc = G.kc;
@@ -255,7 +274,7 @@ __device__ __forceinline__ void class_pass(const FinalizeParams& P, int kh, int 
         for (int i = 0; i < 5; ++i)
 #pragma unroll
           for (int j = 0; j < 5; ++j) v[i][j] = src[i * kw + ix[j]];
-        add_key<F>(pw, v, acc);
+        add_key<F, kWeighted>(pw, v, acc, kWeighted ? weights[c * kc + k] : 1.f);
       }
     }
     __syncthreads();                                   // buffer (c & 1) may be overwritten by chunk c + 2
@@ -287,8 +306,10 @@ __device__ __forceinline__ void class_pass(const FinalizeParams& P, int kh, int 
 // band's `rows` valid rows (rows * ow is a multiple of 4: ow * br is, and a partial last band ends at h * w, which the
 // host checks); when the band has fewer float4s than threads, the spare thread groups take every kg-th key (merged in a
 // fixed order)
+template <bool kWeighted>
 __device__ __forceinline__ void class_pass_identity(const FinalizeParams& P, int nk, int band, int br, int rows, float* tile,
-                                                    const float* const* keys, float* stage, const NextClass& next) {
+                                                    const float* const* keys, const float* weights, float* stage,
+                                                    const NextClass& next) {
   const int ow = P.ow;
   // this pass reads its keys straight from global memory: the next class's first chunk streams in underneath it
   if (next.f) issue_chunk(next.kh, next.kw, next.f, band, br, next.keys, next.nk, 0, stage + kStageFloats);
@@ -305,7 +326,13 @@ __device__ __forceinline__ void class_pass_identity(const FinalizeParams& P, int
 #pragma unroll 8
       for (int k = group; k < nk; k += kg) {
         const float4 v = __ldg(reinterpret_cast<const float4*>(keys[k] + off));
-        acc.x += fmaxf(v.x, 0.f); acc.y += fmaxf(v.y, 0.f); acc.z += fmaxf(v.z, 0.f); acc.w += fmaxf(v.w, 0.f);
+        if constexpr (kWeighted) {
+          const float wk = weights[k];
+          acc.x = fmaf(wk, fmaxf(v.x, 0.f), acc.x); acc.y = fmaf(wk, fmaxf(v.y, 0.f), acc.y);
+          acc.z = fmaf(wk, fmaxf(v.z, 0.f), acc.z); acc.w = fmaf(wk, fmaxf(v.w, 0.f), acc.w);
+        } else {
+          acc.x += fmaxf(v.x, 0.f); acc.y += fmaxf(v.y, 0.f); acc.z += fmaxf(v.z, 0.f); acc.w += fmaxf(v.w, 0.f);
+        }
       }
     }
     if (kg == 1) {                                       // every float4 of the band has one owner
@@ -330,10 +357,17 @@ __device__ __forceinline__ void class_pass_identity(const FinalizeParams& P, int
 }
 
 // grid: (ceil(oh / 4) bands, max n_rows, n_maps); a CTA past its map's bands or rows returns at once. Dynamic smem: two
-// chunk buffers + the band tile (the largest band_rows of the launch * ow floats)
+// chunk buffers + the band tile (the largest band_rows of the launch * ow floats). kWeighted: every key's weight for row
+// t is staged next to its pointer (8 KB more static smem; still two CTAs per SM).
+template <bool kWeighted>
 __global__ void __launch_bounds__(256, 2) finalize_fast_kernel(const __grid_constant__ FinalizeParams P) {
   extern __shared__ __align__(16) float dyn[];
   __shared__ const float* keys[kMaxClassKeys];
+  float* wts = nullptr;
+  if constexpr (kWeighted) {
+    __shared__ float key_weights[kMaxClassKeys];
+    wts = key_weights;
+  }
   float* stage = dyn;                                  // 2 x kStageFloats
   float* tile = dyn + 2 * kStageFloats;
   const MapSel& M = P.map[blockIdx.z];
@@ -351,6 +385,10 @@ __global__ void __launch_bounds__(256, 2) finalize_fast_kernel(const __grid_cons
     const long long first = G.head_sel < 0 ? (long long)M.block_begin * G.heads : (long long)M.block_begin * G.heads + G.head_sel;
     const long long step = G.head_sel < 0 ? 1 : G.heads;
     for (int j = 0; j < per_block * nb; ++j) dst[j] = G.acc + ((first + j * step) * G.tokens + t) * hw;
+    if constexpr (kWeighted) {
+      float* wdst = wts + (dst - keys);
+      for (int j = 0; j < per_block * nb; ++j) wdst[j] = __ldg(P.w[g] + (first + j * step) * G.tokens + t);
+    }
   }
   for (int i = threadIdx.x; i < br * ow; i += blockDim.x) tile[i] = 0.f;
   __syncthreads();
@@ -358,13 +396,14 @@ __global__ void __launch_bounds__(256, 2) finalize_fast_kernel(const __grid_cons
   for (int c = 0; c < M.n_classes; ++c) {                // the map's own classes: maps of one launch differ in them
     const int kh = M.kh[c], kw = M.kw[c], f = ow / kw, nk = (M.key_begin[c + 1] - M.key_begin[c]) * nb;
     const float* const* ck = keys + M.key_begin[c] * nb;
+    const float* cw = kWeighted ? wts + M.key_begin[c] * nb : nullptr;
     NextClass next = {0, 0, 0, 0, nullptr};
     if (c + 1 < M.n_classes && M.kw[c + 1] != ow)
       next = {M.kh[c + 1], M.kw[c + 1], ow / M.kw[c + 1], (M.key_begin[c + 2] - M.key_begin[c + 1]) * nb,
               keys + M.key_begin[c + 1] * nb};
-    if (f == 1) class_pass_identity(P, nk, band, br, rows, tile, ck, stage, next);
-    else if (f == 2) class_pass<2>(P, kh, kw, nk, band, br, tile, ck, stage, prefetched, next);
-    else class_pass<4>(P, kh, kw, nk, band, br, tile, ck, stage, prefetched, next);
+    if (f == 1) class_pass_identity<kWeighted>(P, nk, band, br, rows, tile, ck, cw, stage, next);
+    else if (f == 2) class_pass<2, kWeighted>(P, kh, kw, nk, band, br, tile, ck, cw, stage, prefetched, next);
+    else class_pass<4, kWeighted>(P, kh, kw, nk, band, br, tile, ck, cw, stage, prefetched, next);
     prefetched = next.f != 0;
   }
   __syncthreads();
@@ -460,15 +499,30 @@ static int check_key_groups(const char* name, const daam_key_group* groups, int3
   return DAAM_OK;
 }
 
-// daam_finalize, daam_finalize_maps and daam_finalize_parts, after validation: `maps` are MapSel with out, blocks,
-// groups and n_rows set, and every map is reduced exactly as daam_finalize reduces the map's expanded group list. The
-// kernel choice and the band height are daam_finalize's rule applied per map, to the map's own groups, so the maps of
-// one call take at most two launches (fast and generic, one per kind present) plus one normalisation launch.
+// The fast kernel's dynamic shared memory opt-in, once per device and instance.
+template <bool kWeighted>
+static cudaError_t allow_fast_smem(int device) {
+  static std::once_flag once[64];
+  cudaError_t err = cudaSuccess;
+  std::call_once(once[device & 63], [&] {
+    err = cudaFuncSetAttribute(finalize_fast_kernel<kWeighted>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                               (int)((2 * kStageFloats + 8 * 256) * sizeof(float)));
+  });
+  return err;
+}
+
+// daam_finalize, daam_finalize_maps, daam_finalize_parts and daam_finalize_parts_weighted, after validation: `maps` are
+// MapSel with out, blocks, groups and n_rows set, and every map is reduced exactly as daam_finalize reduces the map's
+// expanded group list. The kernel choice and the band height are daam_finalize's rule applied per map, to the map's own
+// groups, so the maps of one call take at most two launches (fast and generic, one per kind present) plus one
+// normalisation launch. `weights` (one device pointer per group, or null): the weighted instances, same choice.
 static int launch_finalize(const char* name, const daam_key_group* groups, int32_t n_groups, int32_t oh, int32_t ow,
-                           MapSel* maps, int n_maps, int32_t normalize, const DeviceInfo& dev, cudaStream_t stream) {
+                           MapSel* maps, int n_maps, int32_t normalize, const DeviceInfo& dev, cudaStream_t stream,
+                           const float* const* weights = nullptr) {
   static thread_local FinalizeParams p;
   p.n_groups = n_groups; p.oh = oh; p.ow = ow;
   for (int i = 0; i < n_groups; ++i) p.g[i] = groups[i];
+  for (int i = 0; i < n_groups; ++i) p.w[i] = weights ? weights[i] : nullptr;
   const int xx = oh * ow;
   // fast path: every key of the map has one integer factor F = 1 / 2 / 4 on both axes (all SD / SDXL layers that are
   // ever traced) and a 16-byte-aligned key base (cp.async / float4: an aligned slab and h * w a multiple of 4, which
@@ -535,16 +589,18 @@ static int launch_finalize(const char* name, const daam_key_group* groups, int32
       int bands = 0;
       for (int m = 0; m < n; ++m) bands = std::max(bands, (oh + p.map[m].band_rows - 1) / p.map[m].band_rows);
       const size_t smem = (2 * kStageFloats + (size_t)max_br * ow) * sizeof(float);
-      static std::once_flag attr_once[64];
-      cudaError_t attr_err = cudaSuccess;
-      std::call_once(attr_once[dev.device & 63], [&] {
-        attr_err = cudaFuncSetAttribute(finalize_fast_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        (int)((2 * kStageFloats + 8 * 256) * sizeof(float)));
-      });
-      DAAM_CUDA_TRY(attr_err);
-      finalize_fast_kernel<<<dim3(bands, max_rows, n), 256, smem, stream>>>(p);
+      const dim3 grid(bands, max_rows, n);
+      if (weights) {
+        DAAM_CUDA_TRY(allow_fast_smem<true>(dev.device));
+        finalize_fast_kernel<true><<<grid, 256, smem, stream>>>(p);
+      } else {
+        DAAM_CUDA_TRY(allow_fast_smem<false>(dev.device));
+        finalize_fast_kernel<false><<<grid, 256, smem, stream>>>(p);
+      }
+    } else if (weights) {
+      finalize_kernel<true><<<dim3((xx + 255) / 256, max_rows, n), 256, 0, stream>>>(p);
     } else {
-      finalize_kernel<<<dim3((xx + 255) / 256, max_rows, n), 256, 0, stream>>>(p);
+      finalize_kernel<false><<<dim3((xx + 255) / 256, max_rows, n), 256, 0, stream>>>(p);
     }
     DAAM_CUDA_TRY(cudaGetLastError());
     count_launch();
@@ -599,9 +655,10 @@ extern "C" int daam_finalize_maps(const daam_key_group* groups, int32_t n_groups
   return launch_finalize(name, groups, n_groups, oh, ow, sel, n_maps, normalize, dev, static_cast<cudaStream_t>(stream_));
 }
 
-extern "C" int daam_finalize_parts(const daam_key_group* groups, int32_t n_groups, const daam_map_part* maps,
-                                   int32_t n_maps, int32_t oh, int32_t ow, int32_t normalize, void* stream_) {
-  const char* name = "daam_finalize_parts";
+// daam_finalize_parts and daam_finalize_parts_weighted (`weights` null: the plain reduction)
+static int finalize_parts(const char* name, const daam_key_group* groups, int32_t n_groups, const daam_map_part* maps,
+                          int32_t n_maps, int32_t oh, int32_t ow, int32_t normalize, const float* const* weights,
+                          void* stream_) {
   if (!maps || n_maps <= 0) { set_error("%s: no output map", name); return DAAM_E_INVALID; }
   if (n_maps > kMaxMaps) { set_error("%s: %d maps > %d", name, n_maps, kMaxMaps); return DAAM_E_UNSUPPORTED; }
   auto bad_map = [&](int m) {
@@ -625,7 +682,23 @@ extern "C" int daam_finalize_parts(const daam_key_group* groups, int32_t n_group
       }
     sel[m] = make_map(s.out, 0, 1, s.n_rows, s.group_begin, s.group_count);
   }
-  return launch_finalize(name, groups, n_groups, oh, ow, sel, n_maps, normalize, dev, static_cast<cudaStream_t>(stream_));
+  return launch_finalize(name, groups, n_groups, oh, ow, sel, n_maps, normalize, dev, static_cast<cudaStream_t>(stream_),
+                         weights);
+}
+
+extern "C" int daam_finalize_parts(const daam_key_group* groups, int32_t n_groups, const daam_map_part* maps,
+                                   int32_t n_maps, int32_t oh, int32_t ow, int32_t normalize, void* stream_) {
+  return finalize_parts("daam_finalize_parts", groups, n_groups, maps, n_maps, oh, ow, normalize, nullptr, stream_);
+}
+
+extern "C" int daam_finalize_parts_weighted(const daam_key_group* groups, int32_t n_groups, const daam_map_part* maps,
+                                            int32_t n_maps, int32_t oh, int32_t ow, int32_t normalize,
+                                            const float* const* weights, void* stream_) {
+  const char* name = "daam_finalize_parts_weighted";
+  if (!weights) { set_error("%s: null weights", name); return DAAM_E_INVALID; }
+  for (int i = 0; i < n_groups && i < kMaxGroups; ++i)
+    if (!weights[i]) { set_error("%s: null weights of key group %d", name, i); return DAAM_E_INVALID; }
+  return finalize_parts(name, groups, n_groups, maps, n_maps, oh, ow, normalize, weights, stream_);
 }
 
 extern "C" int daam_finalize_per_key(const daam_key_group* groups, int32_t n_groups, int32_t oh, int32_t ow,

@@ -79,6 +79,11 @@ class LayerSlab:
     # images per prompt: a prompt's ``heads`` keys are ``images`` runs of ``heads_per_image`` heads, image-major (key
     # head ``i * heads_per_image + h`` is head h of image i); 1 for slabs that ``RawHeatMapCollection.update`` creates
     images: int = 1
+    # value-norm traces only (trace(pipe, value_norms=True)): ``norms`` [storage rows, heads, tokens] fp32 holds
+    # ``||W_h v||`` of every key and context row, laid out like ``storage`` (or ``acc``) without the pixel axis;
+    # ``norms_changed`` is a device bool, set when a later call of the generation saw other norms than the stored ones
+    norms: Optional[torch.Tensor] = None
+    norms_changed: Optional[torch.Tensor] = None
 
     @property
     def n_prompts(self) -> int:
@@ -118,6 +123,10 @@ class LayerSlab:
             return self.neg if negative else self.acc
         return self.half(self.ranges[step_range], negative)
 
+    def norm_source(self, negative: bool = False) -> torch.Tensor:
+        """The ``[n_prompts, heads, tokens]`` value norms of the keys ``source(..., negative)`` holds."""
+        return self.half(self.norms, negative)
+
     def key_view(self, head: int, prompt: int = 0, step_range: Optional[int] = None,
                  negative: bool = False) -> torch.Tensor:
         src = self.source(step_range, negative)
@@ -137,6 +146,7 @@ class RawHeatMapCollection:
         self.n_ranges = 0                     # range slabs next to every accumulator (trace(step_ranges=[...]))
         self.range_steps: List[int] = []      # UNet forwards each range has received since the last clear()
         self.negative = False                 # slabs also hold the unconditional half (trace(negative=True))
+        self.value_norms = False              # slabs also hold every key's value norms (trace(value_norms=True))
 
     # -- wiring from the tracer -------------------------------------------------------------------------------------
     def bind(self, sync, zero):
@@ -157,7 +167,8 @@ class RawHeatMapCollection:
         shape = (n_prompts, heads, tokens, h * w)
         if slab is None or tuple(slab.acc.shape) != shape or slab.acc.device != torch.device(device) \
                 or slab.factor != factor or (self.time_resolved and slab.step is None) \
-                or (self.n_ranges and slab.ranges is None) or (self.negative and slab.neg is None):
+                or (self.n_ranges and slab.ranges is None) or (self.negative and slab.neg is None) \
+                or (self.value_norms and slab.norms is None):
             if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
                 raise RuntimeError('accumulator slabs cannot be created inside a CUDA-graph capture: run one eager '
                                    'UNet step under trace() before capturing')
@@ -169,6 +180,9 @@ class RawHeatMapCollection:
                 if self.n_ranges else None
             halves = dict(acc=storage[n_prompts:], storage=storage, neg=storage[:n_prompts]) if self.negative \
                 else dict(acc=storage)
+            if self.value_norms:
+                halves.update(norms=torch.zeros(full[:3], dtype=torch.float32, device=device),
+                              norms_changed=torch.zeros((), dtype=torch.bool, device=device))
             slab = LayerSlab(layer_idx, factor, heads, h, w, head_offset=head_offset, step=step, ranges=ranges,
                              images=images, **halves)
             self.slabs[layer_idx] = slab

@@ -12,7 +12,7 @@ import torch
 from . import _native
 
 __all__ = ['cond_half', 'make_layer_desc', 'new_accumulator', 'pack', 'accumulate', 'accumulate_steps',
-           'accumulate_range', 'accumulate_layer', 'attention_probs', 'accumulate_probs']
+           'accumulate_range', 'accumulate_layer', 'attention_probs', 'accumulate_probs', 'value_norms']
 
 _DTYPES = {torch.float32: _native.DAAM_F32, torch.float16: _native.DAAM_F16, torch.bfloat16: _native.DAAM_BF16}
 
@@ -171,3 +171,35 @@ def accumulate_probs(probs: torch.Tensor, acc: torch.Tensor, *, whole_batch: boo
     with torch.cuda.device(probs.device):
         _native.accumulate_probs(probs.data_ptr(), _DTYPES[probs.dtype], first, kept, hw, tokens, acc.data_ptr(),
                                  torch.cuda.current_stream(probs.device).cuda_stream)
+
+
+def value_norms(value: torch.Tensor, weight: torch.Tensor, heads: int, out: Optional[torch.Tensor] = None, *,
+                whole_batch: bool = False) -> torch.Tensor:
+    """``||W_h v||`` for every kept (sample, head, context row) (``daam_value_norms``): ``value [B, T, heads*d]`` as
+    ``to_v`` emits it (last axis contiguous), ``weight [C_out, heads*d]`` the output projection's. The kept slice is
+    :func:`make_layer_desc`'s: the conditional half of a CFG batch (a lone sample: the upper half of its heads), or with
+    ``whole_batch`` every sample. Returns (or fills ``out``) fp32 ``[n_samples, n_heads, T]``, contiguous."""
+    if not (value.is_cuda and weight.is_cuda):
+        raise RuntimeError('daam_b200 computes on CUDA tensors only (there is no CPU fallback)')
+    if value.dtype not in _DTYPES or weight.dtype not in _DTYPES:
+        raise RuntimeError(f'unsupported value / weight dtypes {value.dtype}/{weight.dtype}')
+    if value.stride(-1) != 1:
+        value = value.contiguous()
+    if weight.stride(-1) != 1:
+        weight = weight.contiguous()
+    bsz, tokens, chan = value.shape
+    d = chan // heads
+    if weight.dim() != 2 or weight.shape[1] != chan:
+        raise RuntimeError(f'output projection weight {tuple(weight.shape)} does not take {chan} channels')
+    first, n_samples, head0, n_heads = (0, bsz, 0, heads) if whole_batch else cond_half(bsz, heads)
+    shape = (n_samples, n_heads, tokens)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float32, device=value.device)
+    elif tuple(out.shape) != shape or out.dtype != torch.float32 or not out.is_contiguous():
+        raise RuntimeError(f'value norms must be contiguous fp32 {shape}, got {out.dtype} {tuple(out.shape)}')
+    ve, we = value.element_size(), weight.element_size()
+    _run_on(value.device, None, lambda s: _native.value_norms(
+        value.data_ptr() + (first * value.stride(0) + head0 * d) * ve, _DTYPES[value.dtype],
+        (value.stride(0), value.stride(1), d), weight.data_ptr() + head0 * d * we, _DTYPES[weight.dtype],
+        weight.stride(0), n_samples, n_heads, tokens, d, weight.shape[0], out.data_ptr(), s))
+    return out

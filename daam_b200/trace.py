@@ -26,6 +26,10 @@ exceptions; what differs is what runs underneath.
   prompt (or the empty one). Every layer's slab is twice as tall, ``[uncond x N, cond x N]`` like the batch, and its
   one descriptor covers the whole batch from sample 0, so the launches stay as they are with twice the tiles. Every read
   takes ``negative=True`` and then reduces the lower half against the negative text.
+* ``value_norms=True`` also keeps, per traced layer, ``||W_h v||`` of every (sample, head, context row): what that row
+  carries through that head after the output projection (``daam_value_norms``, once per layer and generation: the
+  context does not change between steps). ``value_weighted=True`` reads then weight every key's clamped map by it
+  (``daam_finalize_parts_weighted``); the accumulate launches do not change.
 
 Accumulators are fp32 regardless of the pipeline dtype (the reference accumulates in the pipeline dtype, SURVEY.md
 section 5); parity is stated against the fp32 oracle fed the same Q/K.
@@ -33,6 +37,7 @@ section 5); parity is stated against the fp32 oracle fed the same Q/K.
 from __future__ import annotations
 
 import inspect
+import weakref
 from pathlib import Path
 from typing import Dict, List, Optional, Tuple, Type, Union
 
@@ -65,15 +70,19 @@ class DiffusionHeatMapHooker(AggregateHooker):
     and 231 tokens, two or three CLIP chunks such as chunked ``prompt_embeds`` give: every context row is accumulated,
     and every read returns the compact ``n_tokens + 2`` rows that :func:`~daam_b200.utils.context_rows` names; any
     other context length raises at the layer call; not with ``time_resolved``, ``step_ranges``, ``save_heads`` or
-    ``load_heads``).
+    ``load_heads``) and ``value_norms`` (also keep every key's value norms, for the ``value_weighted=True`` reads and
+    :meth:`compute_value_norms`; not with ``save_heads`` / ``load_heads`` or CUDA-graph capture).
     """
 
     def __init__(self, pipeline, low_memory: bool = False, load_heads: bool = False, save_heads: bool = False,
                  data_dir: str = None, *, launch: str = 'step', batch_prompts: bool = False,
                  locate_middle_block: bool = False, kernel_flags: int = _native.ACC_AUTO, time_resolved: bool = False,
-                 step_ranges=None, negative: bool = False, long_prompts: bool = False):
+                 step_ranges=None, negative: bool = False, long_prompts: bool = False, value_norms: bool = False):
         if launch not in ('step', 'overlap', 'layer'):
             raise ValueError("launch must be 'step', 'overlap' or 'layer'")
+        if value_norms and (save_heads or load_heads):
+            raise ValueError('value_norms=True does not support save_heads / load_heads: those layer calls replay '
+                             'stored probabilities, not the value projection')
         if long_prompts:
             for name, on in (('time_resolved=True', time_resolved), ('step_ranges', step_ranges is not None),
                              ('save_heads', save_heads), ('load_heads', load_heads)):
@@ -108,6 +117,11 @@ class DiffusionHeatMapHooker(AggregateHooker):
         self.negative = negative
         self.all_heat_maps.negative = negative
         self.long_prompts = long_prompts
+        self.value_norms = value_norms
+        self.all_heat_maps.value_norms = value_norms
+        # value-norm mode: layer -> (slab, weakref to the context, (data_ptr, shape, strides, _version)) of the call
+        # whose norms the slab holds; emptied at every generation's check_inputs
+        self._norms_seen: Dict[int, tuple] = {}
         self.last_image = None
         self.last_images: list = []   # every image of the last generation, prompt-major (``out.images[p * n + i]``)
         self.time_idx = 0
@@ -335,6 +349,25 @@ class DiffusionHeatMapHooker(AggregateHooker):
             raise RuntimeError(f'layer {layer_idx}: negative=True needs classifier-free guidance, but a batch of {bsz} '
                                f'is not a CFG pair batch [uncond x N, cond x N]')
 
+    def _see_values(self, layer_idx: int, ctx: torch.Tensor, value: torch.Tensor, weight: torch.Tensor, heads: int):
+        """Value-norm mode, after the layer's call was queued: the first call of a generation writes the layer's norms
+        into its slab. A later call whose context is the same tensor, unmodified, does nothing (the norms are a function
+        of the context); one with another context recomputes them into scratch and sets the slab's device flag if they
+        differ from the stored ones, with no host synchronisation. A value-weighted read raises on that flag."""
+        slab = self.all_heat_maps.slabs[layer_idx]
+        ident = (ctx.data_ptr(), tuple(ctx.shape), ctx.stride(), ctx._version)
+        seen = self._norms_seen.get(layer_idx)
+        if seen is not None and seen[0] is slab and seen[1]() is ctx and seen[2] == ident:
+            return
+        if seen is None or seen[0] is not slab:            # first call of the generation, or a new slab
+            out = slab.norms.view(-1, slab.heads // slab.images, slab.tokens)
+            ops.value_norms(value, weight, heads, out, whole_batch=self.negative)
+            slab.norms_changed.zero_()
+        else:
+            fresh = ops.value_norms(value, weight, heads, whole_batch=self.negative)
+            slab.norms_changed.logical_or_((fresh.view_as(slab.norms) != slab.norms).any())
+        self._norms_seen[layer_idx] = (slab, weakref.ref(ctx), ident)
+
     def _launch_now(self, own, device):
         """``launch='layer'``: the layer's kernel right away on the current stream (the producer of Q/K may be the
         immediately preceding kernel there, so no EARLY_LOADS)."""
@@ -508,7 +541,7 @@ class DiffusionHeatMapHooker(AggregateHooker):
     # -- finalize -------------------------------------------------------------------------------------------------------
     def compute_global_heat_map(self, prompt=None, factors=None, head_idx=None, layer_idx=None, normalize=False,
                                 prompt_idx: int = 0, *, step_range: Optional[int] = None, negative: bool = False,
-                                image_idx: Optional[int] = None) -> GlobalHeatMap:
+                                image_idx: Optional[int] = None, value_weighted: bool = False) -> GlobalHeatMap:
         """Aggregate across time (already summed in the slabs) and across layers/heads (trace.py:83-132).
 
         Args mirror the reference: ``factors`` restricts the spatial factors, ``head_idx`` / ``layer_idx`` restrict to one
@@ -521,9 +554,17 @@ class DiffusionHeatMapHooker(AggregateHooker):
         With several images per prompt (``num_images_per_prompt``) the map is, as in the reference, the mean over every
         image's keys, and ``head_idx`` indexes images x heads. ``image_idx=i`` keeps image ``i``'s keys only (``head_idx``
         then counts that image's heads); an un-guided batch has only the kept images (see ``ops.cond_half``).
+
+        ``value_weighted=True`` (``trace(pipe, value_norms=True)``): every key's clamped map is scaled by its value norm
+        ``||W_h v||`` for that row before the mean over keys (``daam_finalize_parts_weighted``; same keys, order, rows
+        and normalisation).
         """
         prompt, grid, rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range, layer_idx,
                                                               head_idx, negative, image_idx)
+        if value_weighted:
+            weights = self._weight_ptrs(slabs, prompt_idx, negative, image_idx)
+            maps = self._finalize_parts(groups, [(0, len(groups))], grid, rows, normalize, slabs, weights)[0]
+            return GlobalHeatMap(self.pipe.tokenizer, prompt, maps)
         device = slabs[0].acc.device
         n_fin = _finalized_rows(rows)
         maps = torch.empty((n_fin,) + grid, dtype=torch.float32, device=device)
@@ -592,47 +633,98 @@ class DiffusionHeatMapHooker(AggregateHooker):
 
     def compute_per_head_heat_maps(self, prompt=None, factors=None, normalize=False, prompt_idx: int = 0, *,
                                    step_range: Optional[int] = None, negative: bool = False,
-                                   image_idx: Optional[int] = None):
+                                   image_idx: Optional[int] = None, value_weighted: bool = False):
         """Every ``compute_global_heat_map(layer_idx=l, head_idx=h)`` of the reference's ``--all-heads`` sweep
         (daam/run/generate.py:239-255) in one launch. Returns ``(keys, maps)``: ``keys[i] = (factor, layer, head)`` and
         ``maps[i]`` the ``[n_tokens + 2, xh, xw]`` heat map the reference computes for that single key. ``step_range=i``
         and ``negative=True`` select the slabs as in :meth:`compute_global_heat_map`; ``image_idx=i`` keeps image
-        ``i``'s keys, whose ``head`` then counts that image's heads."""
-        return self._per_head(prompt, factors, normalize, prompt_idx, step_range, negative, image_idx)[1:]
+        ``i``'s keys, whose ``head`` then counts that image's heads. ``value_weighted=True``: ``maps[i]`` is the
+        value-weighted global map of key ``i`` alone, bit for bit."""
+        return self._per_head(prompt, factors, normalize, prompt_idx, step_range, negative, image_idx,
+                              value_weighted)[1:]
 
-    def _per_head(self, prompt, factors, normalize, prompt_idx, step_range, negative, image_idx):
-        """``(prompt, keys, maps)`` of :meth:`compute_per_head_heat_maps`."""
+    def _per_head(self, prompt, factors, normalize, prompt_idx, step_range, negative, image_idx, value_weighted=False):
+        """``(prompt, keys, maps)`` of :meth:`compute_per_head_heat_maps`. Weighted: the per-key maps unnormalised,
+        times each key's norm per row on the device, then normalised -- a single key's weighted global map."""
         prompt, grid, rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range,
                                                               negative=negative, image_idx=image_idx)
         keys = [(slab.factor, slab.layer_idx, head) for slab, g in zip(slabs, groups) for head in range(g.heads)]
         device = slabs[0].acc.device
         n_fin = _finalized_rows(rows)
+        norms = self._key_norms(slabs, prompt_idx, negative, image_idx)[:, :n_fin] if value_weighted else None
         maps = torch.empty((len(keys), n_fin) + grid, dtype=torch.float32, device=device)
+        norm_here = normalize and n_fin == len(rows)
         with torch.cuda.device(device):
-            _native.finalize_per_key(groups, grid, n_fin, normalize and n_fin == len(rows), maps.data_ptr(),
-                                     torch.cuda.current_stream(device).cuda_stream)
+            stream = torch.cuda.current_stream(device).cuda_stream
+            _native.finalize_per_key(groups, grid, n_fin, norm_here and norms is None, maps.data_ptr(), stream)
+            if norms is not None:
+                maps.mul_(norms[:, :, None, None])
+                if norm_here:
+                    _native.normalize_maps(maps.data_ptr(), len(keys), n_fin, grid, stream)
         return prompt, keys, _compact(maps, rows, normalize)
+
+    def compute_value_norms(self, prompt=None, prompt_idx: int = 0, *, negative: bool = False,
+                            image_idx: Optional[int] = None, factors=None):
+        """Which heads carry each word: ``(keys, norms)`` with ``keys`` those of :meth:`compute_per_head_heat_maps`
+        and ``norms[i]`` ``[n_tokens + 2]`` (device fp32) key ``i``'s value norm ``||W_h v||`` of every row of the map
+        (the compact rows of a long context). Needs ``trace(pipe, value_norms=True)``."""
+        prompt, _, rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, None, negative=negative,
+                                                           image_idx=image_idx)
+        keys = [(slab.factor, slab.layer_idx, head) for slab, g in zip(slabs, groups) for head in range(g.heads)]
+        norms = self._key_norms(slabs, prompt_idx, negative, image_idx)
+        return keys, norms.index_select(1, torch.tensor(rows, dtype=torch.long).to(norms.device))
+
+    def _check_weighted(self, slabs):
+        """Raises unless every slab of a read holds value norms that stayed valid for the whole generation."""
+        if not self.value_norms or any(s.norms is None for s in slabs):
+            raise RuntimeError('value-weighted heat maps need a trace declared with trace(pipe, value_norms=True)')
+        changed = torch.stack([s.norms_changed for s in slabs]).cpu()
+        if bool(changed.any()):
+            layer = slabs[int(changed.to(torch.uint8).argmax())].layer_idx
+            raise ValueError(f'layer {layer}: the cross-attention context changed during the generation, so its value '
+                             f'norms are not one set per key: a value-weighted read is undefined (plain reads work)')
+
+    def _weight_ptrs(self, slabs, prompt_idx: int, negative: bool, image_idx: Optional[int]) -> List[int]:
+        """The weights of the key groups ``_read_groups`` made from ``slabs``: each group's acc offset with the pixel
+        axis dropped, in the slab's norms."""
+        self._check_weighted(slabs)
+        out = []
+        for s in slabs:
+            n = s.norm_source(negative)
+            out.append((n[prompt_idx] if image_idx is None else n[prompt_idx, image_idx * s.heads_per_image]).data_ptr())
+        return out
+
+    def _key_norms(self, slabs, prompt_idx: int, negative: bool, image_idx: Optional[int]) -> torch.Tensor:
+        """``[keys, tokens]``: the norms of every key of a per-head read over ``slabs``, in its key order."""
+        self._check_weighted(slabs)
+        parts = []
+        for s in slabs:
+            n = s.norm_source(negative)[prompt_idx]
+            parts.append(n if image_idx is None else n[image_idx * s.heads_per_image:(image_idx + 1) * s.heads_per_image])
+        return torch.cat(parts)
 
     def compute_head_heat_maps(self, prompt=None, factors=None, normalize=False, prompt_idx: int = 0, *,
                                step_range: Optional[int] = None, negative: bool = False,
-                               image_idx: Optional[int] = None) -> HeadHeatMaps:
+                               image_idx: Optional[int] = None, value_weighted: bool = False) -> HeadHeatMaps:
         """:meth:`compute_per_head_heat_maps` as a stack the word-list calls work on: a :class:`HeadHeatMaps` whose
         ``keys[i] = (factor, layer, head)`` labels ``heat_maps[i]``. The stack takes ``keys x rows x xh x xw x 4`` bytes
         (SD-2.1, 175 keys, 12 rows, 64 x 64: 34 MB; the 1100 keys of SDXL's 60 layers: 216 MB); ``factors`` and ``image_idx`` narrow
         it."""
-        prompt, keys, maps = self._per_head(prompt, factors, normalize, prompt_idx, step_range, negative, image_idx)
+        prompt, keys, maps = self._per_head(prompt, factors, normalize, prompt_idx, step_range, negative, image_idx,
+                                            value_weighted)
         return HeadHeatMaps(self.pipe.tokenizer, prompt, maps, keys)
 
     def compute_layer_heat_maps(self, prompt=None, factors=None, head_idx=None, normalize=False, prompt_idx: int = 0, *,
                                 step_range: Optional[int] = None, negative: bool = False,
-                                image_idx: Optional[int] = None) -> LayerHeatMaps:
+                                image_idx: Optional[int] = None, value_weighted: bool = False) -> LayerHeatMaps:
         """Every traced layer's map in one launch (``daam_finalize_parts``): ``heat_maps[i]`` is
         ``compute_global_heat_map(layer_idx=layers[i], ...)`` with the same arguments, bit for bit. One map per layer
         that passes the filters (``head_idx``: the layers that have that head), in the order the layers were traced.
         Returns a :class:`LayerHeatMaps` ``[layers, n_rows, xh, xw]``."""
         prompt, grid, rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range, None, head_idx,
                                                               negative, image_idx)
-        maps = self._finalize_parts(groups, [(i, 1) for i in range(len(groups))], grid, rows, normalize, slabs)
+        weights = self._weight_ptrs(slabs, prompt_idx, negative, image_idx) if value_weighted else None
+        maps = self._finalize_parts(groups, [(i, 1) for i in range(len(groups))], grid, rows, normalize, slabs, weights)
         names = self.layer_names
         return LayerHeatMaps(self.pipe.tokenizer, prompt, maps, [s.layer_idx for s in slabs],
                              [names[s.layer_idx] if s.layer_idx < len(names) else None for s in slabs],
@@ -640,19 +732,22 @@ class DiffusionHeatMapHooker(AggregateHooker):
 
     def compute_factor_heat_maps(self, prompt=None, factors=None, head_idx=None, layer_idx=None, normalize=False,
                                  prompt_idx: int = 0, *, step_range: Optional[int] = None, negative: bool = False,
-                                 image_idx: Optional[int] = None) -> FactorHeatMaps:
+                                 image_idx: Optional[int] = None, value_weighted: bool = False) -> FactorHeatMaps:
         """Every traced resolution's map in one launch (``daam_finalize_parts``): ``heat_maps[j]`` is
         ``compute_global_heat_map(factors={stack.factors[j]}, ...)`` with the same arguments, bit for bit; ``factors``
         keeps some of them. Returns a :class:`FactorHeatMaps` ``[factors, n_rows, xh, xw]``, factors ascending."""
         prompt, grid, rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range, layer_idx,
                                                               head_idx, negative, image_idx)
         order, found, parts = _factor_parts([s.factor for s in slabs])
-        maps = self._finalize_parts([groups[i] for i in order], parts, grid, rows, normalize, slabs)
+        weights = self._weight_ptrs(slabs, prompt_idx, negative, image_idx) if value_weighted else None
+        maps = self._finalize_parts([groups[i] for i in order], parts, grid, rows, normalize, slabs,
+                                    None if weights is None else [weights[i] for i in order])
         return FactorHeatMaps(self.pipe.tokenizer, prompt, maps, found)
 
-    def _finalize_parts(self, groups, parts, grid, rows, normalize, slabs) -> torch.Tensor:
+    def _finalize_parts(self, groups, parts, grid, rows, normalize, slabs, weights=None) -> torch.Tensor:
         """One ``daam_finalize_parts`` over ``groups``: map ``m`` reduces groups ``[begin, begin + count)`` of
-        ``parts[m] = (begin, count)`` as a read of those groups alone does. Returns ``[len(parts), len(rows), xh, xw]``."""
+        ``parts[m] = (begin, count)`` as a read of those groups alone does. Returns ``[len(parts), len(rows), xh, xw]``.
+        ``weights``: one norms pointer per group, ``daam_finalize_parts_weighted``."""
         device = slabs[0].acc.device
         n_fin = _finalized_rows(rows)
         out = torch.empty((len(parts), n_fin) + grid, dtype=torch.float32, device=device)
@@ -660,7 +755,7 @@ class DiffusionHeatMapHooker(AggregateHooker):
                for m, (begin, count) in enumerate(parts)]
         with torch.cuda.device(device):
             _native.finalize_parts(groups, sel, grid, normalize and n_fin == len(rows),
-                                   torch.cuda.current_stream(device).cuda_stream)
+                                   torch.cuda.current_stream(device).cuda_stream, weights)
         return _compact(out, rows, normalize)
 
     def _read_groups(self, prompt, factors, prompt_idx: int, step_range: Optional[int], layer_idx=None, head_idx=None,
@@ -715,6 +810,22 @@ class DiffusionHeatMapHooker(AggregateHooker):
                                f'context length')
         return prompt, self.geometry.grid, context_rows(len(self.pipe.tokenizer.tokenize(prompt)), tokens.pop()), \
             groups, slabs
+
+
+def _check_value_norms(layer_idx: int, attn):
+    """Value-norm mode, at a traced layer call: the norms read ``attn.to_out[0].weight``, so that module must apply
+    exactly that weight (a plain ``nn.Linear``: no unmerged LoRA, no hooks), and the call must run eagerly, since a
+    CUDA-graph replay bypasses the hook that computes them."""
+    proj = attn.to_out[0]
+    plain = isinstance(proj, torch.nn.Linear) and not proj._forward_hooks and not proj._forward_pre_hooks and \
+        (type(proj).forward is torch.nn.Linear.forward or
+         (hasattr(proj, 'lora_layer') and getattr(proj, 'lora_layer') is None))
+    if not plain:
+        raise RuntimeError(f'layer {layer_idx}: value_norms=True needs the output projection to be a plain nn.Linear '
+                           f'(its .weight is what the layer applies), got {type(proj).__name__}; merge any LoRA first')
+    if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
+        raise RuntimeError('value_norms=True cannot be captured into a CUDA graph: the norms are computed by the '
+                           'layer hook, which a graph replay bypasses')
 
 
 def _factor_parts(factors: List[int]) -> Tuple[List[int], List[int], List[Tuple[int, int]]]:
@@ -876,6 +987,7 @@ class PipelineHooker(ObjectHooker):
         negatives = hk_self._negative_prompts(prompt, args, kwargs, len(prompts)) if tr.negative else []
         hk_self.heat_maps.clear()
         tr._restart_history()
+        tr._norms_seen.clear()                       # the value norms of the new generation are computed afresh
         if len(prompts) != len(tr.last_prompts):    # slabs are laid out [prompts][images * heads]: re-derive them
             tr._layer_state.clear()
         tr.last_prompt = prompts[0]
@@ -991,7 +1103,11 @@ class UNetCrossAttentionHooker(ObjectHooker):
             geom = self._geom = (n, tokens, factor, traced and factor != 8)
         tr._gen_idx += 1
         if geom[3]:                                          # skip if too large (trace.py:289)
+            if tr.value_norms:
+                _check_value_norms(self.layer_idx, attn)
             tr._enqueue(self.layer_idx, geom[2], query, key, heads, attn.scale)
+            if tr.value_norms:
+                tr._see_values(self.layer_idx, encoder_hidden_states, value, attn.to_out[0].weight, heads)
 
         d = query.shape[-1] // heads
         q4 = query.view(bsz, n, heads, d).transpose(1, 2)

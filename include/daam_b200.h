@@ -40,7 +40,8 @@ extern "C" {
                                           daam_region_boundary, daam_mask_boundary;
                                           daam_segment_crf;
                                           daam_word_distance, daam_mask_distance;
-                                          daam_image_superpixels, daam_segment_superpixels) */
+                                          daam_image_superpixels, daam_segment_superpixels;
+                                          daam_value_norms, daam_finalize_parts_weighted) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_TOKENS 231     /* daam_accumulate: long contexts of 2 or 3 CLIP chunks of 77 tokens (154, 231) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
@@ -263,6 +264,41 @@ typedef struct daam_map_part {
 } daam_map_part;
 int daam_finalize_parts(const daam_key_group* groups, int32_t n_groups, const daam_map_part* maps, int32_t n_maps,
                         int32_t map_h, int32_t map_w, int32_t normalize, void* stream);
+
+/*
+ * daam_finalize_parts with one weight per key and row (value-weighted heat maps, daam_b200/trace.py
+ * trace(..., value_norms=True)): map m is
+ *   (1 / K) sum_k weight_k[t] * clamp(bicubic(key_k[t]), 0)     (then normalised like daam_finalize if asked)
+ * over the K keys daam_finalize_parts selects for it, in the same key order, kernel choice, band height, group-merge
+ * order and final division by K. The only change is the per-key add: the plain `acc += clamp(o)` becomes
+ * `acc = fmaf(w, clamp(o), acc)`. So weights of 1.0 give daam_finalize_parts' bits, and weights of 2^k give 2^k times
+ * them (without `normalize`, which adds 1e-6 to its denominator).
+ * weights: host array of n_groups device pointers; weights[g] is fp32 [heads][tokens] (the group's acc layout with
+ * h * w = 1), read with the key's head index (head_sel included) at rows [0, n_rows). Weights must be finite and >= 0:
+ * the call cannot check device memory. Limits and errors: those of daam_finalize_parts, and DAAM_E_INVALID for a null
+ * weights array or a null entry.
+ */
+int daam_finalize_parts_weighted(const daam_key_group* groups, int32_t n_groups, const daam_map_part* maps,
+                                 int32_t n_maps, int32_t map_h, int32_t map_w, int32_t normalize,
+                                 const float* const* weights, void* stream);
+
+/*
+ * Value norms (norm-based attention analysis: Kobayashi et al., EMNLP 2020): for sample b, head h and context row j of
+ * one cross-attention layer,
+ *   n[b][h][j] = || W_h v ||_2,   v = value[b][j][h d .. (h + 1) d),   W_h = W[:, h d .. (h + 1) d)
+ * with W = attn.to_out[0].weight ([out_dim][heads * d], row stride w_stride_row elements, columns contiguous) and
+ * `value` what attn.to_v produced: element (b, j, h, e) at value + b * v_stride_sample + j * v_stride_token +
+ * h * v_stride_head + e (elements; the channel axis is contiguous). Point `value` and `w` at head 0 of the first sample
+ * kept, as daam_layer does for K: e.g. the conditional half of a CFG batch, or sample 0 for the whole batch. Both
+ * operands are converted to fp32 (value_dtype and w_dtype: enum daam_dtype, independently).
+ * Arithmetic: y_c = sum_e W_h[c][e] v[e] as an fmaf chain over e ascending from 0, s = sum_c y_c^2 as an fmaf chain
+ * over c ascending from 0, n = sqrtf(s). out: device fp32 [n_samples][heads][tokens].
+ * Limits (DAAM_E_UNSUPPORTED): tokens 77, 154 or 231, head_dim <= DAAM_MAX_HEAD_DIM, out_dim <= 4096,
+ * n_samples * heads <= 65535. DAAM_E_INVALID: a null pointer, a non-positive size or an unknown dtype.
+ */
+int daam_value_norms(const void* value, int32_t value_dtype, int64_t v_stride_sample, int64_t v_stride_token,
+                     int64_t v_stride_head, const void* w, int32_t w_dtype, int64_t w_stride_row, int32_t n_samples,
+                     int32_t heads, int32_t tokens, int32_t head_dim, int32_t out_dim, float* out, void* stream);
 
 /*
  * The reference's --all-heads sweep calls compute_global_heat_map(layer_idx=l, head_idx=h) once per (layer, head)
