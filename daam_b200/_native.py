@@ -191,7 +191,7 @@ def overlay_frames_bytes(n_maps: int, n_words: int, out_h: int, out_w: int) -> i
     return (n_maps * n_words * out_h * out_w * 3 + 3) // 4 * 4
 
 
-EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_finalize',
+EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_accumulate_joint', 'daam_finalize',
            'daam_finalize_maps', 'daam_finalize_parts', 'daam_finalize_parts_weighted', 'daam_finalize_per_key', 'daam_value_norms','daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
            'daam_segment_words', 'daam_region_overlap', 'daam_region_sweep', 'daam_region_ranking', 'daam_region_boundary', 'daam_mask_boundary', 'daam_word_overlap', 'daam_word_instances', 'daam_overlay_words', 'daam_refine_words', 'daam_segment_crf', 'daam_word_distance', 'daam_mask_distance', 'daam_image_superpixels', 'daam_segment_superpixels', 'daam_jet_colormap',
            'daam_side_launcher_create', 'daam_side_launcher_destroy',
@@ -209,6 +209,17 @@ class DaamLayer(ctypes.Structure):
         ('head_dim', ctypes.c_int32), ('dtype', ctypes.c_int32), ('scale', ctypes.c_float),
         ('reserved', ctypes.c_int32),
     ]
+
+
+class DaamJointLayer(ctypes.Structure):
+    """``struct daam_joint_layer`` (include/daam_b200.h): ``daam_layer`` plus the joint softmax's log-sum-exp."""
+    _fields_ = DaamLayer._fields_ + [
+        ('lse', ctypes.c_void_p),
+        ('lse_stride_prompt', ctypes.c_int64), ('lse_stride_head', ctypes.c_int64), ('lse_stride_pixel', ctypes.c_int64),
+    ]
+
+
+JOINT_MAX_TOKENS = 1024   # DAAM_JOINT_MAX_TOKENS: context rows of a daam_accumulate_joint layer
 
 
 class DaamKeyGroup(ctypes.Structure):
@@ -267,6 +278,8 @@ def load() -> ctypes.CDLL:
     i32, u32, i64, vp, f32 = ctypes.c_int32, ctypes.c_uint32, ctypes.c_int64, ctypes.c_void_p, ctypes.c_float
     lib.daam_accumulate.argtypes = [ctypes.POINTER(DaamLayer), i32, u32, vp]
     lib.daam_accumulate.restype = ctypes.c_int
+    lib.daam_accumulate_joint.argtypes = [ctypes.POINTER(DaamJointLayer), i32, u32, vp]
+    lib.daam_accumulate_joint.restype = ctypes.c_int
     lib.daam_accumulate_steps.argtypes = [ctypes.POINTER(DaamLayer), ctypes.POINTER(vp), i32, u32, vp]
     lib.daam_accumulate_steps.restype = ctypes.c_int
     lib.daam_accumulate_range.argtypes = [ctypes.POINTER(DaamLayer), ctypes.POINTER(vp), i32, u32, vp]
@@ -422,6 +435,16 @@ def accumulate(layers, stream: int, flags: int = ACC_AUTO):
     if packed.n == 0:
         return
     rc = load().daam_accumulate(packed.array, packed.n, flags, stream)
+    if rc != 0:
+        _check(rc)
+
+
+def accumulate_joint(layers: Sequence[DaamJointLayer], stream: int):
+    """``daam_accumulate_joint`` over a sequence of :class:`DaamJointLayer` (one launch per kernel class)."""
+    if not layers:
+        return
+    array = (DaamJointLayer * len(layers))(*layers)
+    rc = load().daam_accumulate_joint(array, len(layers), 0, stream)
     if rc != 0:
         _check(rc)
 

@@ -7,7 +7,7 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-SOURCES = ['api.cu', 'accumulate_simt.cu', 'accumulate_mma.cu', 'finalize.cu', 'words.cu', 'components.cu', 'ranking.cu', 'boundary.cu', 'distance.cu', 'refine.cu', 'crf.cu', 'superpixels.cu', 'value_norms.cu', 'probs.cu']
+SOURCES = ['api.cu', 'accumulate_simt.cu', 'accumulate_mma.cu', 'finalize.cu', 'words.cu', 'components.cu', 'ranking.cu', 'boundary.cu', 'distance.cu', 'refine.cu', 'crf.cu', 'superpixels.cu', 'value_norms.cu', 'probs.cu', 'accumulate_joint.cu']
 OUT = os.path.join(HERE, 'libdaam_b200.so')
 NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17', '-Xcompiler', '-fPIC',
               '-I', os.path.join(ROOT, 'include'), '-shared']

@@ -63,3 +63,23 @@ class LatentGeometry:
                 raise RuntimeError(f'layer {layer_idx}: {n} query positions match no level of the {H}x{W} latent '
                                    f'(ceil(H / 2^s) * ceil(W / 2^s) for s = 0, 1, ...)')
             s += 1
+
+
+class JointGeometry:
+    """The heat-map geometry of an MM-DiT (Stable Diffusion 3): the transformer cuts the ``(H, W)`` latent into
+    ``patch_size`` x ``patch_size`` patches, one image token each, so the grid is ``(H / p, W / p)`` and every traced
+    layer's keys have the grid's size and factor 1. ``latent_shape`` is ``None`` until the first transformer forward."""
+
+    def __init__(self, patch_size: int, latent_shape: Optional[Tuple[int, int]] = None):
+        self.patch_size = int(patch_size)
+        self.latent_shape = None if latent_shape is None else (int(latent_shape[0]), int(latent_shape[1]))
+        self.grid: Tuple[int, int] = (0, 0) if latent_shape is None else \
+            (self.latent_shape[0] // self.patch_size, self.latent_shape[1] // self.patch_size)
+
+    def level(self, n: int, layer_idx: int = 0) -> Tuple[int, int, int]:
+        """``(h, w, 1)`` for a layer of ``n`` image tokens; raises ``RuntimeError`` when ``n`` is not the grid's size."""
+        h, w = self.grid
+        if h * w != n:
+            raise RuntimeError(f'layer {layer_idx}: {n} image tokens, but the {self.latent_shape} latent in '
+                               f'{self.patch_size} x {self.patch_size} patches gives {h} x {w}')
+        return h, w, 1

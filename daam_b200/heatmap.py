@@ -147,6 +147,7 @@ class RawHeatMapCollection:
         self.range_steps: List[int] = []      # UNet forwards each range has received since the last clear()
         self.negative = False                 # slabs also hold the unconditional half (trace(negative=True))
         self.value_norms = False              # slabs also hold every key's value norms (trace(value_norms=True))
+        self.joint = False                    # joint-attention slabs: any context of 1 .. 1024 rows (SD3 traces)
 
     # -- wiring from the tracer -------------------------------------------------------------------------------------
     def bind(self, sync, zero):
@@ -161,7 +162,7 @@ class RawHeatMapCollection:
         """Returns (allocating or re-shaping on demand) the zero-initialised slab of a layer and marks it live.
         ``heads`` counts every image's heads of one prompt (``images`` runs of ``heads // images``); ``tokens`` is the
         context length (77, or 154 / 231 in a ``long_prompts`` trace): every context row is accumulated."""
-        if tokens not in _native.CONTEXT_TOKENS:
+        if tokens not in _native.CONTEXT_TOKENS and not (self.joint and 1 <= tokens <= _native.JOINT_MAX_TOKENS):
             raise ValueError(f'a slab holds a context of {_native.CONTEXT_TOKENS} tokens, not {tokens}')
         slab = self.slabs.get(layer_idx)
         shape = (n_prompts, heads, tokens, h * w)

@@ -5,6 +5,10 @@ The tracer's layer indices, and therefore every ``(factor, layer, head)`` key, f
 asked -- the ``mid_block``; inside a block whose class name contains ``CrossAttn`` every
 ``attentions[*].transformer_blocks[*].attn2`` is taken in module order. Names restart at 0 in every block
 (``up-attn-0`` occurs once per up block), exactly like the reference's.
+
+An MM-DiT transformer (Stable Diffusion 3 / 3.5) has no cross-attention: :class:`JointAttentionLocator` takes the joint
+attention ``transformer_blocks[i].attn`` of every block, ``layer_idx = i``, named ``joint-attn-{i}``. The image-only
+``attn2`` some SD3.5 blocks add attends to no text and is not located.
 """
 from __future__ import annotations
 
@@ -12,7 +16,7 @@ from typing import Generic, Iterable, List, Optional, Set, Tuple, TypeVar
 
 import torch.nn as nn
 
-__all__ = ['ModuleLocator', 'UNetCrossAttentionLocator']
+__all__ = ['ModuleLocator', 'UNetCrossAttentionLocator', 'JointAttentionLocator']
 
 ModuleType = TypeVar('ModuleType')
 
@@ -57,4 +61,17 @@ class UNetCrossAttentionLocator(ModuleLocator):
                         names.append(f'{tag}-attn-{position}')
                     position += 1
         self.layer_names[:] = names
+        return found
+
+
+class JointAttentionLocator(ModuleLocator):
+    """``locate(transformer)`` returns ``transformer_blocks[*].attn`` in block order; ``layer_names`` is filled
+    alongside."""
+
+    def __init__(self):
+        self.layer_names: List[str] = []
+
+    def locate(self, model) -> list:
+        found = [block.attn for block in model.transformer_blocks]
+        self.layer_names[:] = [f'joint-attn-{i}' for i in range(len(found))]
         return found

@@ -12,7 +12,8 @@ import torch
 from . import _native
 
 __all__ = ['cond_half', 'make_layer_desc', 'new_accumulator', 'pack', 'accumulate', 'accumulate_steps',
-           'accumulate_range', 'accumulate_layer', 'attention_probs', 'accumulate_probs', 'value_norms']
+           'accumulate_range', 'accumulate_layer', 'attention_probs', 'accumulate_probs', 'value_norms',
+           'make_joint_desc', 'accumulate_joint']
 
 _DTYPES = {torch.float32: _native.DAAM_F32, torch.float16: _native.DAAM_F16, torch.bfloat16: _native.DAAM_BF16}
 
@@ -203,3 +204,44 @@ def value_norms(value: torch.Tensor, weight: torch.Tensor, heads: int, out: Opti
         (value.stride(0), value.stride(1), d), weight.data_ptr() + head0 * d * we, _DTYPES[weight.dtype],
         weight.stride(0), n_samples, n_heads, tokens, d, weight.shape[0], out.data_ptr(), s))
     return out
+
+
+def make_joint_desc(q: torch.Tensor, k: torch.Tensor, lse: torch.Tensor, n_image: int, acc: torch.Tensor, heads: int,
+                    scale: float) -> _native.DaamJointLayer:
+    """One ``daam_joint_layer`` from a joint attention's operands as SDPA takes them: ``q`` / ``k`` ``[B, heads, L, d]``
+    (any strides, ``d`` contiguous; e.g. the concatenation ``[image, context]`` of diffusers' ``JointAttnProcessor2_0``,
+    or a ``[B, L, heads*d]`` projection viewed that way), ``lse`` fp32 ``[B, heads, >= n_image]`` the attention's
+    log-sum-exp (natural log), ``n_image`` the image tokens ahead of the context in ``L``. The kept samples are
+    :func:`cond_half`'s; ``acc`` fp32 ``[n_prompts, n_heads, L - n_image, n_image]`` contiguous."""
+    if not (q.is_cuda and k.is_cuda and lse.is_cuda and acc.is_cuda):
+        raise RuntimeError('daam_b200 computes on CUDA tensors only (there is no CPU fallback)')
+    if q.dtype not in _DTYPES or k.dtype != q.dtype:
+        raise RuntimeError(f'unsupported projection dtypes {q.dtype}/{k.dtype}')
+    if lse.dtype != torch.float32 or lse.dim() != 3:
+        raise RuntimeError(f'lse must be fp32 [B, heads, L], got {lse.dtype} {tuple(lse.shape)}')
+    if q.dim() != 4 or k.dim() != 4 or q.stride(-1) != 1 or k.stride(-1) != 1:
+        raise RuntimeError('q and k must be [B, heads, L, d] with a contiguous d axis')
+    bsz, _, _, d = q.shape
+    tokens = k.shape[2] - n_image
+    first, n_prompts, head0, n_heads = cond_half(bsz, heads)
+    if tuple(acc.shape) != (n_prompts, n_heads, tokens, n_image) or acc.dtype != torch.float32 \
+            or not acc.is_contiguous():
+        raise RuntimeError(f'accumulator must be contiguous fp32 {(n_prompts, n_heads, tokens, n_image)}, '
+                           f'got {acc.dtype} {tuple(acc.shape)}')
+    es = q.element_size()
+    return _native.DaamJointLayer(
+        q=q.data_ptr() + (first * q.stride(0) + head0 * q.stride(1)) * es,
+        k=k.data_ptr() + (first * k.stride(0) + head0 * k.stride(1) + n_image * k.stride(2)) * es,
+        acc=acc.data_ptr(),
+        q_stride_prompt=q.stride(0), q_stride_pixel=q.stride(2), q_stride_head=q.stride(1),
+        k_stride_prompt=k.stride(0), k_stride_token=k.stride(2), k_stride_head=k.stride(1),
+        n_prompts=n_prompts, heads=n_heads, hw=n_image, tokens=tokens, head_dim=d,
+        dtype=_DTYPES[q.dtype], scale=float(scale), reserved=0,
+        lse=lse.data_ptr() + (first * lse.stride(0) + head0 * lse.stride(1)) * 4,
+        lse_stride_prompt=lse.stride(0), lse_stride_head=lse.stride(1), lse_stride_pixel=lse.stride(2))
+
+
+def accumulate_joint(descs, device, stream: Optional[torch.cuda.Stream] = None):
+    """Enqueue ``daam_accumulate_joint`` over the given joint layer descriptors on ``stream`` (default: the current
+    stream of ``device``)."""
+    _run_on(device, stream, lambda s: _native.accumulate_joint(list(descs), s))

@@ -32,6 +32,9 @@ import torch.nn.functional as F
 __all__ = [
     'SyntheticAttention', 'SDPAProcessor', 'SyntheticUNet', 'SyntheticPipeline', 'WhitespaceTokenizer',
     'UNetSpec', 'SD21_SPEC', 'SD21_768_SPEC', 'SDXL_SPEC', 'SD15_SPEC', 'TINY_SPEC', 'TINY15_SPEC', 'TINY96_SPEC', 'make_pipeline',
+    'JointAttnProcessor', 'SyntheticJointAttention', 'JointTransformerBlock', 'SyntheticSD3Transformer',
+    'SentencePieceTokenizer', 'SyntheticSD3Pipeline', 'SD3Spec', 'SD3_MEDIUM_SPEC', 'SD35_LARGE_SPEC', 'TINY_SD3_SPEC',
+    'make_sd3_pipeline',
 ]
 
 
@@ -573,3 +576,233 @@ def make_pipeline(spec: UNetSpec = SD21_SPEC, body: str = 'skeleton', dtype=torc
         unet = SyntheticUNet(spec, body=body)
     torch.random.set_rng_state(gen_state)
     return SyntheticPipeline(unet, dtype=dtype, device=device, seed=seed, cuda_graph=cuda_graph)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Stable Diffusion 3: MM-DiT transformer with joint attention
+# ---------------------------------------------------------------------------------------------------------------
+class JointAttnProcessor:
+    """The un-hooked joint attention: diffusers' ``JointAttnProcessor2_0`` op for op (image projections, optional
+    q / k norms on ``[B, heads, N, d]``, context projections and their norms, concatenation image-then-context, one
+    SDPA, split, ``to_add_out`` unless ``context_pre_only``, ``to_out``)."""
+
+    def __call__(self, attn, hidden_states, encoder_hidden_states=None, attention_mask=None, *args, **kwargs):
+        residual = hidden_states
+        b = hidden_states.shape[0]
+        query, key, value = attn.to_q(hidden_states), attn.to_k(hidden_states), attn.to_v(hidden_states)
+        d = key.shape[-1] // attn.heads
+        query = query.view(b, -1, attn.heads, d).transpose(1, 2)
+        key = key.view(b, -1, attn.heads, d).transpose(1, 2)
+        value = value.view(b, -1, attn.heads, d).transpose(1, 2)
+        if attn.norm_q is not None:
+            query = attn.norm_q(query)
+        if attn.norm_k is not None:
+            key = attn.norm_k(key)
+        if encoder_hidden_states is not None:
+            cq = attn.add_q_proj(encoder_hidden_states).view(b, -1, attn.heads, d).transpose(1, 2)
+            ck = attn.add_k_proj(encoder_hidden_states).view(b, -1, attn.heads, d).transpose(1, 2)
+            cv = attn.add_v_proj(encoder_hidden_states).view(b, -1, attn.heads, d).transpose(1, 2)
+            if attn.norm_added_q is not None:
+                cq = attn.norm_added_q(cq)
+            if attn.norm_added_k is not None:
+                ck = attn.norm_added_k(ck)
+            query = torch.cat([query, cq], dim=2)
+            key = torch.cat([key, ck], dim=2)
+            value = torch.cat([value, cv], dim=2)
+        hidden_states = F.scaled_dot_product_attention(query, key, value, dropout_p=0.0, is_causal=False)
+        hidden_states = hidden_states.transpose(1, 2).reshape(b, -1, attn.heads * d).to(query.dtype)
+        if encoder_hidden_states is not None:
+            hidden_states, encoder_hidden_states = hidden_states[:, :residual.shape[1]], \
+                hidden_states[:, residual.shape[1]:]
+            if not attn.context_pre_only:
+                encoder_hidden_states = attn.to_add_out(encoder_hidden_states)
+        hidden_states = attn.to_out[1](attn.to_out[0](hidden_states))
+        if encoder_hidden_states is not None:
+            return hidden_states, encoder_hidden_states
+        return hidden_states
+
+
+class SyntheticJointAttention(nn.Module):
+    """The attributes of diffusers' ``Attention`` that a joint block's processor reads."""
+
+    def __init__(self, dim: int, heads: int, dim_head: int, qk_norm: bool, context_pre_only: bool):
+        super().__init__()
+        inner = heads * dim_head
+        self.heads = heads
+        self.scale = dim_head ** -0.5
+        self.context_pre_only = context_pre_only
+        self.to_q, self.to_k, self.to_v = (nn.Linear(dim, inner) for _ in range(3))
+        self.add_q_proj, self.add_k_proj, self.add_v_proj = (nn.Linear(dim, inner) for _ in range(3))
+        norm = (lambda: nn.RMSNorm(dim_head, eps=1e-6)) if qk_norm else (lambda: None)
+        self.norm_q, self.norm_k, self.norm_added_q, self.norm_added_k = norm(), norm(), norm(), norm()
+        self.to_out = nn.ModuleList([nn.Linear(inner, dim), nn.Dropout(0.0)])
+        self.to_add_out = None if context_pre_only else nn.Linear(inner, dim)
+        self.processor = JointAttnProcessor()
+
+    def set_processor(self, processor):
+        self.processor = processor
+
+    def forward(self, hidden_states, encoder_hidden_states=None, attention_mask=None, **kwargs):
+        return self.processor(self, hidden_states, encoder_hidden_states=encoder_hidden_states,
+                              attention_mask=attention_mask, **kwargs)
+
+
+class JointTransformerBlock(nn.Module):
+    """An MM-DiT block: the joint attention over the normed image and context streams, then a feed-forward on each
+    (none on the context after the ``context_pre_only`` last block)."""
+
+    def __init__(self, dim, heads, dim_head, qk_norm, context_pre_only):
+        super().__init__()
+        self.context_pre_only = context_pre_only
+        self.norm1 = nn.LayerNorm(dim)
+        self.norm1_context = nn.LayerNorm(dim)
+        self.attn = SyntheticJointAttention(dim, heads, dim_head, qk_norm, context_pre_only)
+        self.ff = nn.Linear(dim, dim)
+        self.ff_context = None if context_pre_only else nn.Linear(dim, dim)
+
+    def forward(self, hidden_states, encoder_hidden_states, temb):
+        x = self.norm1(hidden_states) + temb[:, None]
+        attn_out, ctx_out = self.attn(x, encoder_hidden_states=self.norm1_context(encoder_hidden_states))
+        hidden_states = hidden_states + attn_out
+        hidden_states = hidden_states + self.ff(F.gelu(hidden_states))
+        if self.context_pre_only:
+            return None, hidden_states
+        encoder_hidden_states = encoder_hidden_states + ctx_out
+        return encoder_hidden_states + self.ff_context(F.gelu(encoder_hidden_states)), hidden_states
+
+
+@dataclass
+class SD3Spec:
+    """Shape of an SD3 transformer: ``heads`` heads of ``dim_head`` in each of ``blocks`` joint blocks, a
+    ``sample_size`` latent of ``in_channels`` cut into ``patch_size`` patches, and a context of 77 CLIP rows plus
+    ``t5_rows`` T5 rows (``max_sequence_length``) of ``joint_attention_dim`` channels."""
+    name: str
+    sample_size: int
+    blocks: int
+    heads: int
+    dim_head: int = 64
+    patch_size: int = 2
+    in_channels: int = 16
+    joint_attention_dim: int = 4096
+    t5_rows: int = 256
+    qk_norm: bool = False
+
+
+# public transformer/config.json shapes of stabilityai/stable-diffusion-3-medium-diffusers and
+# stabilityai/stable-diffusion-3.5-large (RMS q / k norm), at their 1024-pixel (128 x 128 latent) size
+SD3_MEDIUM_SPEC = SD3Spec('sd3-medium', 128, 24, 24)
+SD35_LARGE_SPEC = SD3Spec('sd3.5-large', 128, 38, 38, qk_norm=True)
+# small joint trees for the tests: RMS q / k norm, three blocks, a 16-row T5 context (93 rows in all)
+TINY_SD3_SPEC = SD3Spec('tiny-sd3', 32, 3, 2, dim_head=32, in_channels=4, joint_attention_dim=64, t5_rows=16,
+                        qk_norm=True)
+
+
+class SyntheticSD3Transformer(nn.Module):
+    """SD3Transformer2DModel-shaped random-init network: patchify, ``transformer_blocks`` of joint blocks (the last
+    one ``context_pre_only``), unpatchify. ``forward(hidden_states=, encoder_hidden_states=, timestep=)`` returns a
+    1-tuple, as diffusers' does with ``return_dict=False``."""
+
+    def __init__(self, spec: SD3Spec):
+        super().__init__()
+        self.spec = spec
+        dim = spec.heads * spec.dim_head
+        self.config = SimpleNamespace(sample_size=spec.sample_size, patch_size=spec.patch_size,
+                                      in_channels=spec.in_channels, joint_attention_dim=spec.joint_attention_dim)
+        self.pos_embed = nn.Conv2d(spec.in_channels, dim, spec.patch_size, stride=spec.patch_size)
+        self.time_proj = nn.Linear(1, dim)
+        self.context_embedder = nn.Linear(spec.joint_attention_dim, dim)
+        self.transformer_blocks = nn.ModuleList([
+            JointTransformerBlock(dim, spec.heads, spec.dim_head, spec.qk_norm, i == spec.blocks - 1)
+            for i in range(spec.blocks)])
+        self.norm_out = nn.LayerNorm(dim)
+        self.proj_out = nn.Linear(dim, spec.patch_size ** 2 * spec.in_channels)
+
+    def forward(self, hidden_states, encoder_hidden_states, timestep, return_dict: bool = False):
+        b, c, h, w = hidden_states.shape
+        p = self.spec.patch_size
+        x = self.pos_embed(hidden_states).flatten(2).transpose(1, 2)
+        temb = self.time_proj(timestep.reshape(-1, 1).expand(b, 1).to(x.dtype) / 1000)
+        ctx = self.context_embedder(encoder_hidden_states)
+        for block in self.transformer_blocks:
+            ctx, x = block(x, ctx, temb)
+        x = self.proj_out(self.norm_out(x)).view(b, h // p, w // p, p, p, c)
+        return (x.permute(0, 5, 1, 3, 2, 4).reshape(b, c, h, w),)
+
+
+class SentencePieceTokenizer:
+    """T5-tokenizer stand-in: whitespace words, case kept, each cut into pieces of at most 4 characters; a word's
+    first piece carries sentencepiece's ``▁`` word-start marker (so ``'giraffe'`` is ``['▁gira', 'ffe']``)."""
+
+    def tokenize(self, text: str) -> List[str]:
+        out = []
+        for word in text.split():
+            pieces = [word[i:i + 4] for i in range(0, len(word), 4)]
+            out += ['▁' + pieces[0]] + pieces[1:]
+        return out
+
+
+class SyntheticSD3Pipeline:
+    """A StableDiffusion3Pipeline-shaped driver around :class:`SyntheticSD3Transformer`: ``transformer`` and no
+    ``unet``, ``tokenizer`` (CLIP-style) and ``tokenizer_3`` (sentencepiece-style), ``check_inputs`` in diffusers'
+    SD3 parameter order, ``image_processor.postprocess`` and a CFG loop over ``[uncond x N, cond x N]`` batches whose
+    context is 77 CLIP rows then ``max_sequence_length`` T5 rows (seeded gaussian embeddings)."""
+
+    def __init__(self, transformer: SyntheticSD3Transformer, dtype=torch.float32, device='cpu', seed: int = 0):
+        self.transformer = transformer.to(device=device, dtype=dtype).eval()
+        self.dtype, self.device = dtype, torch.device(device)
+        self.vae_scale_factor = 8
+        self.tokenizer = WhitespaceTokenizer()
+        self.tokenizer_3 = SentencePieceTokenizer()
+        self.image_processor = _ImageProcessor()
+        self.seed = seed
+
+    def check_inputs(self, prompt, prompt_2, prompt_3, height, width, negative_prompt=None, negative_prompt_2=None,
+                     negative_prompt_3=None, prompt_embeds=None, negative_prompt_embeds=None, *args, **kwargs):
+        if prompt is None and prompt_embeds is None:
+            raise ValueError('Provide either `prompt` or `prompt_embeds`')
+        if height % (self.vae_scale_factor * self.transformer.spec.patch_size) or \
+                width % (self.vae_scale_factor * self.transformer.spec.patch_size):
+            raise ValueError(f'`height` and `width` must be divisible by '
+                             f'{self.vae_scale_factor * self.transformer.spec.patch_size}')
+
+    @torch.no_grad()
+    def __call__(self, prompt=None, prompt_2=None, prompt_3=None, height: Optional[int] = None,
+                 width: Optional[int] = None, num_inference_steps: int = 28, guidance_scale: float = 7.0,
+                 num_images_per_prompt: int = 1, generator: Optional[torch.Generator] = None,
+                 max_sequence_length: Optional[int] = None):
+        spec = self.transformer.spec
+        height = spec.sample_size * self.vae_scale_factor if height is None else height
+        width = spec.sample_size * self.vae_scale_factor if width is None else width
+        self.check_inputs(prompt, prompt_2, prompt_3, height, width)
+        prompts = [prompt] if isinstance(prompt, str) else list(prompt)
+        rows = 77 + (spec.t5_rows if max_sequence_length is None else max_sequence_length)
+        if generator is None:
+            generator = torch.Generator().manual_seed(self.seed)
+        n = len(prompts) * num_images_per_prompt
+        emb = torch.randn(2, len(prompts), rows, spec.joint_attention_dim, generator=generator)
+        emb = emb.repeat_interleave(num_images_per_prompt, dim=1).reshape(2 * n, rows, -1)
+        lat = torch.randn(n, spec.in_channels, height // self.vae_scale_factor, width // self.vae_scale_factor,
+                          generator=generator)
+        emb, lat = emb.to(self.device, self.dtype), lat.to(self.device, self.dtype)
+        for i in range(num_inference_steps):
+            t = torch.full((2 * n,), 1000.0 * (1.0 - i / max(1, num_inference_steps)), device=self.device)
+            eps = self.transformer(hidden_states=torch.cat([lat, lat]), encoder_hidden_states=emb, timestep=t,
+                                   return_dict=False)[0]
+            eps = eps[:n] + guidance_scale * (eps[n:] - eps[:n])
+            lat = (lat - 0.02 * eps).clamp(-4, 4)
+        images = self.image_processor.postprocess(lat[:, :3].float(), output_type='pil')
+        return SimpleNamespace(images=images, latents=lat)
+
+
+def make_sd3_pipeline(spec: SD3Spec = TINY_SD3_SPEC, dtype=torch.float32, device='cpu', seed: int = 0,
+                      init_on_device: bool = False) -> SyntheticSD3Pipeline:
+    """Random-init SD3-shaped pipeline; weights drawn on the CPU from ``seed`` unless ``init_on_device``."""
+    gen_state = torch.random.get_rng_state()
+    torch.manual_seed(seed)
+    if init_on_device and torch.device(device).type == 'cuda':
+        with torch.device(device):
+            transformer = SyntheticSD3Transformer(spec)
+    else:
+        transformer = SyntheticSD3Transformer(spec)
+    torch.random.set_rng_state(gen_state)
+    return SyntheticSD3Pipeline(transformer, dtype=dtype, device=device, seed=seed)

@@ -37,6 +37,7 @@ section 5); parity is stated against the fp32 oracle fed the same Q/K.
 from __future__ import annotations
 
 import inspect
+import math
 import weakref
 from pathlib import Path
 from typing import Dict, List, Optional, Tuple, Type, Union
@@ -45,14 +46,15 @@ import torch
 import torch.nn.functional as F
 
 from . import _native, ops
-from .geometry import LatentGeometry
+from .geometry import JointGeometry, LatentGeometry
 from .heatmap import (FactorHeatMaps, GlobalHeatMap, HeadHeatMaps, ImageHeatMaps, LayerHeatMaps, LayerSlab,
                       RawHeatMapCollection, TimeHeatMaps)
 from .hook import AggregateHooker, ObjectHooker, UNetCrossAttentionLocator
-from .utils import cache_dir, context_rows
+from .locate import JointAttentionLocator
+from .utils import T5Pieces, cache_dir, context_rows, t5_rows
 
-__all__ = ['trace', 'DiffusionHeatMapHooker', 'GlobalHeatMap', 'UNetCrossAttentionHooker', 'PipelineHooker',
-           'ImageProcessorHooker']
+__all__ = ['trace', 'DiffusionHeatMapHooker', 'GlobalHeatMap', 'UNetCrossAttentionHooker', 'JointAttentionHooker',
+           'PipelineHooker', 'ImageProcessorHooker']
 
 class DiffusionHeatMapHooker(AggregateHooker):
     """Context manager that traces every located cross-attention layer of ``pipeline.unet`` (trace.py:22-59).
@@ -72,6 +74,12 @@ class DiffusionHeatMapHooker(AggregateHooker):
     other context length raises at the layer call; not with ``time_resolved``, ``step_ranges``, ``save_heads`` or
     ``load_heads``) and ``value_norms`` (also keep every key's value norms, for the ``value_weighted=True`` reads and
     :meth:`compute_value_norms`; not with ``save_heads`` / ``load_heads`` or CUDA-graph capture).
+
+    A pipeline whose denoiser is an MM-DiT ``transformer`` and that has no ``unet`` (Stable Diffusion 3 / 3.5) is traced
+    through the joint attention of every ``transformer.transformer_blocks[i].attn`` (:class:`JointAttentionHooker`):
+    a map is the image-query x text-key block of each joint softmax, summed over steps (``daam_accumulate_joint``).
+    Reads return the CLIP rows by default and the T5 rows with ``encoder='t5'``. Such a trace refuses the options it
+    does not implement (see :data:`JOINT_REFUSED`) with a ``ValueError``.
     """
 
     def __init__(self, pipeline, low_memory: bool = False, load_heads: bool = False, save_heads: bool = False,
@@ -101,16 +109,36 @@ class DiffusionHeatMapHooker(AggregateHooker):
                 raise ValueError(f'{name} does not support save_heads / load_heads')
         if len(modes) > 1:
             raise ValueError('step_ranges cannot be combined with time_resolved=True')
+        self.joint = getattr(pipeline, 'unet', None) is None and getattr(pipeline, 'transformer', None) is not None
+        if self.joint:
+            options = dict(time_resolved=time_resolved, step_ranges=step_ranges is not None, negative=negative,
+                           long_prompts=long_prompts, value_norms=value_norms, save_heads=save_heads,
+                           load_heads=load_heads, low_memory=low_memory, locate_middle_block=locate_middle_block)
+            for name in JOINT_REFUSED:
+                if options[name]:
+                    raise ValueError(f'{name} is not supported when tracing the joint attention of an SD3 transformer')
+            if launch == 'overlap':
+                raise ValueError("launch='overlap' is not supported when tracing the joint attention of an SD3 "
+                                 "transformer: use 'step' or 'layer'")
         _native.load()   # fail here, loudly, if the CUDA library is missing
         self.all_heat_maps = RawHeatMapCollection()
-        side = pipeline.unet.config.sample_size * pipeline.vae_scale_factor
-        self.latent_hw = 4096 if side in (512, 1024) else 9216   # 64x64, or 96x96 for the 768-pixel models
-        # the heat-map grid and every layer's (h, w, factor): square until the first UNet forward shows the latent
-        # (a forward pre-hook on the UNet re-derives it whenever the latent's (H, W) changes)
-        self._sample_size = pipeline.unet.config.sample_size
-        self.geometry = LatentGeometry(self.latent_hw, self._sample_size)
-        self.locator = UNetCrossAttentionLocator(restrict={0} if low_memory else None,
-                                                 locate_middle_block=locate_middle_block or load_heads or save_heads)
+        self.all_heat_maps.joint = self.joint
+        if self.joint:
+            # joint mode: the grid is the latent in patches, known from the first transformer forward
+            self.latent_hw = self._sample_size = None
+            self.geometry = JointGeometry(pipeline.transformer.config.patch_size)
+            self.locator = JointAttentionLocator()
+        else:
+            side = pipeline.unet.config.sample_size * pipeline.vae_scale_factor
+            self.latent_hw = 4096 if side in (512, 1024) else 9216   # 64x64, or 96x96 for the 768-pixel models
+            # the heat-map grid and every layer's (h, w, factor): square until the first UNet forward shows the latent
+            # (a forward pre-hook on the UNet re-derives it whenever the latent's (H, W) changes)
+            self._sample_size = pipeline.unet.config.sample_size
+            self.geometry = LatentGeometry(self.latent_hw, self._sample_size)
+            self.locator = UNetCrossAttentionLocator(restrict={0} if low_memory else None,
+                                                     locate_middle_block=locate_middle_block or load_heads or save_heads)
+        self.last_prompts_3: List[Optional[str]] = []   # joint mode: the T5 text (prompt_3) of every prompt, or None
+        self._joint_pending: List[_native.DaamJointLayer] = []   # joint mode: the layer calls of the running forward
         self.last_prompt: str = ''
         self.last_prompts: List[str] = []
         self.last_negative_prompts: List[str] = []   # negative=True: the negative text of every prompt ('' for none)
@@ -164,14 +192,19 @@ class DiffusionHeatMapHooker(AggregateHooker):
         self._slab_ptrs = [_native.StepPointers([0] * 64)
                            for _ in range(1 if time_resolved else self.all_heat_maps.n_ranges)]
 
-        modules = [
-            UNetCrossAttentionHooker(m, self, layer_idx=idx, latent_hw=self.latent_hw, load_heads=load_heads,
-                                     save_heads=save_heads, data_dir=data_dir)
-            for idx, m in enumerate(self.locator.locate(pipeline.unet))
-        ]
+        if self.joint:
+            modules = [JointAttentionHooker(m, self, layer_idx=idx)
+                       for idx, m in enumerate(self.locator.locate(pipeline.transformer))]
+        else:
+            modules = [
+                UNetCrossAttentionHooker(m, self, layer_idx=idx, latent_hw=self.latent_hw, load_heads=load_heads,
+                                         save_heads=save_heads, data_dir=data_dir)
+                for idx, m in enumerate(self.locator.locate(pipeline.unet))
+            ]
         self._attn_hookers = list(modules)
         modules.append(PipelineHooker(pipeline, self))
-        if type(pipeline).__name__ == 'StableDiffusionXLPipeline' and getattr(pipeline, 'image_processor', None):
+        if (self.joint or type(pipeline).__name__ == 'StableDiffusionXLPipeline') \
+                and getattr(pipeline, 'image_processor', None):
             modules.append(ImageProcessorHooker(pipeline.image_processor, self))
         super().__init__(modules)
         self.pipe = pipeline
@@ -203,7 +236,7 @@ class DiffusionHeatMapHooker(AggregateHooker):
 
     def _hook_impl(self):
         super()._hook_impl()
-        unet = self.pipe.unet
+        unet = self.pipe.transformer if self.joint else self.pipe.unet   # the denoiser: one forward per step
         self._forward_hook = None
         self._pre_hook = None
         if self.launch != 'layer' and hasattr(unet, 'register_forward_hook'):
@@ -225,7 +258,13 @@ class DiffusionHeatMapHooker(AggregateHooker):
 
     # -- geometry -----------------------------------------------------------------------------------------------------
     def _see_sample(self, _module, args, kwargs):
-        """UNet forward pre-hook: the latent ``sample`` (``args[0]`` or ``kwargs['sample']``) fixes the geometry."""
+        """UNet forward pre-hook: the latent ``sample`` (``args[0]`` or ``kwargs['sample']``) fixes the geometry; in
+        joint mode the transformer's ``hidden_states``."""
+        if self.joint:
+            sample = args[0] if args else kwargs.get('hidden_states')
+            if sample is not None and tuple(sample.shape[-2:]) != self.geometry.latent_shape:
+                self.geometry = JointGeometry(self.geometry.patch_size, tuple(sample.shape[-2:]))
+            return
         sample = args[0] if args else kwargs.get('sample')
         if sample is not None and tuple(sample.shape[-2:]) != self.geometry.latent_shape:
             self.set_latent_shape(tuple(sample.shape[-2:]))
@@ -368,6 +407,32 @@ class DiffusionHeatMapHooker(AggregateHooker):
             slab.norms_changed.logical_or_((fresh.view_as(slab.norms) != slab.norms).any())
         self._norms_seen[layer_idx] = (slab, weakref.ref(ctx), ident)
 
+    def _enqueue_joint(self, layer_idx: int, q: torch.Tensor, k: torch.Tensor, lse: torch.Tensor, n_image: int,
+                       heads: int, scale: float):
+        """Joint mode: register one layer call, ``q`` / ``k`` ``[B, heads, n_image + T, d]`` (image tokens, then the
+        context) and the attention's ``lse``. Queued for the step launch at the end of the transformer forward, or
+        launched now with ``launch='layer'``."""
+        if not q.is_cuda:
+            raise RuntimeError('daam_b200 traces pipelines that live on a CUDA device only (there is no CPU '
+                               'fallback)')
+        if layer_idx in self._queued:                      # the layer comes round again: a new forward has started
+            self.flush()
+        h, w, factor = self.geometry.level(n_image, layer_idx)
+        _, n_samples, head0, n_heads = ops.cond_half(q.shape[0], heads)
+        n_real, images = self._prompt_layout(layer_idx, n_samples)
+        tokens = k.shape[2] - n_image
+        slab = self.all_heat_maps.slab_for(layer_idx, factor, n_real, images * n_heads, h, w, q.device, head0, images,
+                                           tokens)
+        desc = ops.make_joint_desc(q, k, lse, n_image, slab.acc.view(n_samples, n_heads, tokens, n_image), heads,
+                                   scale)
+        self._device = q.device
+        if self.launch == 'layer':
+            ops.accumulate_joint([desc], q.device)
+            return
+        self._joint_pending.append(desc)
+        self._refs += [q, k, lse]                          # kept alive until the step's launch has been issued
+        self._queued[layer_idx] = self._step_id
+
     def _launch_now(self, own, device):
         """``launch='layer'``: the layer's kernel right away on the current stream (the producer of Q/K may be the
         immediately preceding kernel there, so no EARLY_LOADS)."""
@@ -391,6 +456,12 @@ class DiffusionHeatMapHooker(AggregateHooker):
 
     def flush(self):
         """Issue the queued layer calls as one persistent launch (per pack of 32 layers)."""
+        if self._joint_pending:
+            descs, self._joint_pending = self._joint_pending, []
+            ops.accumulate_joint(descs, self._device)   # on the forward's own stream: the projections may go now
+            self._refs = []
+            self._queued.clear()
+            return
         n = self._n_pending
         if n == 0:
             return
@@ -541,7 +612,8 @@ class DiffusionHeatMapHooker(AggregateHooker):
     # -- finalize -------------------------------------------------------------------------------------------------------
     def compute_global_heat_map(self, prompt=None, factors=None, head_idx=None, layer_idx=None, normalize=False,
                                 prompt_idx: int = 0, *, step_range: Optional[int] = None, negative: bool = False,
-                                image_idx: Optional[int] = None, value_weighted: bool = False) -> GlobalHeatMap:
+                                image_idx: Optional[int] = None, value_weighted: bool = False,
+                                encoder: str = 'clip') -> GlobalHeatMap:
         """Aggregate across time (already summed in the slabs) and across layers/heads (trace.py:83-132).
 
         Args mirror the reference: ``factors`` restricts the spatial factors, ``head_idx`` / ``layer_idx`` restrict to one
@@ -558,20 +630,26 @@ class DiffusionHeatMapHooker(AggregateHooker):
         ``value_weighted=True`` (``trace(pipe, value_norms=True)``): every key's clamped map is scaled by its value norm
         ``||W_h v||`` for that row before the mean over keys (``daam_finalize_parts_weighted``; same keys, order, rows
         and normalisation).
+
+        ``encoder='t5'`` (a joint-attention trace of an SD3 pipeline): the map of the T5 rows of ``prompt_3`` (or of
+        the prompt), in the CLIP map's layout: row 0 is zeros (T5 has no start token), rows ``1 .. n`` the
+        sentencepiece pieces and row ``n + 1`` the T5 EOS, so the word lookup (``pipe.tokenizer_3``, case kept) and
+        every word-list call apply unchanged. The default reads the CLIP rows with ``pipe.tokenizer``.
         """
         prompt, grid, rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range, layer_idx,
-                                                              head_idx, negative, image_idx)
+                                                              head_idx, negative, image_idx, encoder)
+        tokenizer = self._map_tokenizer(encoder, rows)
         if value_weighted:
             weights = self._weight_ptrs(slabs, prompt_idx, negative, image_idx)
             maps = self._finalize_parts(groups, [(0, len(groups))], grid, rows, normalize, slabs, weights)[0]
-            return GlobalHeatMap(self.pipe.tokenizer, prompt, maps)
+            return GlobalHeatMap(tokenizer, prompt, maps)
         device = slabs[0].acc.device
         n_fin = _finalized_rows(rows)
         maps = torch.empty((n_fin,) + grid, dtype=torch.float32, device=device)
         with torch.cuda.device(device):
             _native.finalize(groups, grid, n_fin, normalize and n_fin == len(rows), maps.data_ptr(),
                              torch.cuda.current_stream(device).cuda_stream)
-        return GlobalHeatMap(self.pipe.tokenizer, prompt, _compact(maps, rows, normalize))
+        return GlobalHeatMap(tokenizer, prompt, _t5_start_row(_compact(maps, rows, normalize), encoder))
 
     def compute_image_heat_maps(self, prompt_idx: int = 0, factors=None, layer_idx=None, head_idx=None,
                                 normalize: bool = False, *, step_range: Optional[int] = None,
@@ -633,21 +711,24 @@ class DiffusionHeatMapHooker(AggregateHooker):
 
     def compute_per_head_heat_maps(self, prompt=None, factors=None, normalize=False, prompt_idx: int = 0, *,
                                    step_range: Optional[int] = None, negative: bool = False,
-                                   image_idx: Optional[int] = None, value_weighted: bool = False):
+                                   image_idx: Optional[int] = None, value_weighted: bool = False,
+                                   encoder: str = 'clip'):
         """Every ``compute_global_heat_map(layer_idx=l, head_idx=h)`` of the reference's ``--all-heads`` sweep
         (daam/run/generate.py:239-255) in one launch. Returns ``(keys, maps)``: ``keys[i] = (factor, layer, head)`` and
         ``maps[i]`` the ``[n_tokens + 2, xh, xw]`` heat map the reference computes for that single key. ``step_range=i``
         and ``negative=True`` select the slabs as in :meth:`compute_global_heat_map`; ``image_idx=i`` keeps image
         ``i``'s keys, whose ``head`` then counts that image's heads. ``value_weighted=True``: ``maps[i]`` is the
-        value-weighted global map of key ``i`` alone, bit for bit."""
+        value-weighted global map of key ``i`` alone, bit for bit. ``encoder``: as in :meth:`compute_global_heat_map`."""
         return self._per_head(prompt, factors, normalize, prompt_idx, step_range, negative, image_idx,
-                              value_weighted)[1:]
+                              value_weighted, encoder)[1:3]
 
-    def _per_head(self, prompt, factors, normalize, prompt_idx, step_range, negative, image_idx, value_weighted=False):
+    def _per_head(self, prompt, factors, normalize, prompt_idx, step_range, negative, image_idx, value_weighted=False,
+                  encoder: str = 'clip'):
         """``(prompt, keys, maps)`` of :meth:`compute_per_head_heat_maps`. Weighted: the per-key maps unnormalised,
-        times each key's norm per row on the device, then normalised -- a single key's weighted global map."""
+        times each key's norm per row on the device, then normalised -- a single key's weighted global map. Also
+        returns the map's tokenizer."""
         prompt, grid, rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range,
-                                                              negative=negative, image_idx=image_idx)
+                                                              negative=negative, image_idx=image_idx, encoder=encoder)
         keys = [(slab.factor, slab.layer_idx, head) for slab, g in zip(slabs, groups) for head in range(g.heads)]
         device = slabs[0].acc.device
         n_fin = _finalized_rows(rows)
@@ -661,7 +742,7 @@ class DiffusionHeatMapHooker(AggregateHooker):
                 maps.mul_(norms[:, :, None, None])
                 if norm_here:
                     _native.normalize_maps(maps.data_ptr(), len(keys), n_fin, grid, stream)
-        return prompt, keys, _compact(maps, rows, normalize)
+        return prompt, keys, _t5_start_row(_compact(maps, rows, normalize), encoder), self._map_tokenizer(encoder, rows)
 
     def compute_value_norms(self, prompt=None, prompt_idx: int = 0, *, negative: bool = False,
                             image_idx: Optional[int] = None, factors=None):
@@ -705,28 +786,31 @@ class DiffusionHeatMapHooker(AggregateHooker):
 
     def compute_head_heat_maps(self, prompt=None, factors=None, normalize=False, prompt_idx: int = 0, *,
                                step_range: Optional[int] = None, negative: bool = False,
-                               image_idx: Optional[int] = None, value_weighted: bool = False) -> HeadHeatMaps:
+                               image_idx: Optional[int] = None, value_weighted: bool = False,
+                               encoder: str = 'clip') -> HeadHeatMaps:
         """:meth:`compute_per_head_heat_maps` as a stack the word-list calls work on: a :class:`HeadHeatMaps` whose
         ``keys[i] = (factor, layer, head)`` labels ``heat_maps[i]``. The stack takes ``keys x rows x xh x xw x 4`` bytes
         (SD-2.1, 175 keys, 12 rows, 64 x 64: 34 MB; the 1100 keys of SDXL's 60 layers: 216 MB); ``factors`` and ``image_idx`` narrow
         it."""
-        prompt, keys, maps = self._per_head(prompt, factors, normalize, prompt_idx, step_range, negative, image_idx,
-                                            value_weighted)
-        return HeadHeatMaps(self.pipe.tokenizer, prompt, maps, keys)
+        prompt, keys, maps, tokenizer = self._per_head(prompt, factors, normalize, prompt_idx, step_range, negative,
+                                                       image_idx, value_weighted, encoder)
+        return HeadHeatMaps(tokenizer, prompt, maps, keys)
 
     def compute_layer_heat_maps(self, prompt=None, factors=None, head_idx=None, normalize=False, prompt_idx: int = 0, *,
                                 step_range: Optional[int] = None, negative: bool = False,
-                                image_idx: Optional[int] = None, value_weighted: bool = False) -> LayerHeatMaps:
+                                image_idx: Optional[int] = None, value_weighted: bool = False,
+                                encoder: str = 'clip') -> LayerHeatMaps:
         """Every traced layer's map in one launch (``daam_finalize_parts``): ``heat_maps[i]`` is
         ``compute_global_heat_map(layer_idx=layers[i], ...)`` with the same arguments, bit for bit. One map per layer
         that passes the filters (``head_idx``: the layers that have that head), in the order the layers were traced.
-        Returns a :class:`LayerHeatMaps` ``[layers, n_rows, xh, xw]``."""
+        Returns a :class:`LayerHeatMaps` ``[layers, n_rows, xh, xw]``. ``encoder``: as in
+        :meth:`compute_global_heat_map`."""
         prompt, grid, rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range, None, head_idx,
-                                                              negative, image_idx)
+                                                              negative, image_idx, encoder)
         weights = self._weight_ptrs(slabs, prompt_idx, negative, image_idx) if value_weighted else None
         maps = self._finalize_parts(groups, [(i, 1) for i in range(len(groups))], grid, rows, normalize, slabs, weights)
         names = self.layer_names
-        return LayerHeatMaps(self.pipe.tokenizer, prompt, maps, [s.layer_idx for s in slabs],
+        return LayerHeatMaps(self._map_tokenizer(encoder, rows), prompt, _t5_start_row(maps, encoder), [s.layer_idx for s in slabs],
                              [names[s.layer_idx] if s.layer_idx < len(names) else None for s in slabs],
                              [s.factor for s in slabs])
 
@@ -759,14 +843,28 @@ class DiffusionHeatMapHooker(AggregateHooker):
         return _compact(out, rows, normalize)
 
     def _read_groups(self, prompt, factors, prompt_idx: int, step_range: Optional[int], layer_idx=None, head_idx=None,
-                     negative: bool = False, image_idx: Optional[int] = None):
+                     negative: bool = False, image_idx: Optional[int] = None, encoder: str = 'clip'):
         """What the heat-map reads share: the prompt (default: the generation's, or with ``negative`` its negative
         text), the map grid ``(xh, xw)``, the context rows the map reads (``utils.context_rows``: ``[0, n_tokens + 2)``
         for a 77-token context), and the key groups of prompt ``prompt_idx`` over the live slabs (with ``step_range``:
         over that range's slabs; with ``negative``: their unconditional halves) that pass the filters, with the slabs
         behind them; with ``image_idx`` the groups hold image ``image_idx``'s heads only, and ``head_idx`` counts those.
         Raises when no slab passes, ``IndexError`` for a bad ``image_idx`` and ``ValueError`` when the generation was
-        driven by embeddings and no ``prompt`` text is given."""
+        driven by embeddings and no ``prompt`` text is given.
+
+        A joint-attention trace reads the CLIP rows ``[0, n_tokens + 2)`` of its context, or with ``encoder='t5'`` the
+        T5 rows: the groups then start at context row 76, so that map row ``r`` is context row ``76 + r`` (row 0, the
+        last CLIP row, is zeroed by the read), and the text is ``prompt_3`` when the generation had one."""
+        if encoder not in ('clip', 't5'):
+            raise ValueError(f"encoder must be 'clip' or 't5', got {encoder!r}")
+        if encoder == 't5':
+            if not self.joint:
+                raise ValueError("encoder='t5' reads the T5 rows of a joint-attention (SD3) trace; this trace has "
+                                 "CLIP contexts only")
+            if getattr(self.pipe, 'tokenizer_3', None) is None:
+                raise ValueError("encoder='t5' needs the pipeline's T5 tokenizer (pipe.tokenizer_3)")
+            if prompt is None and prompt_idx < len(self.last_prompts_3):
+                prompt = self.last_prompts_3[prompt_idx]
         if negative:
             self.all_heat_maps.check_negative()
         if prompt is None:
@@ -808,8 +906,38 @@ class DiffusionHeatMapHooker(AggregateHooker):
         if len(tokens) > 1:
             raise RuntimeError(f'the traced layers hold contexts of {sorted(tokens)} tokens: one read reduces one '
                                f'context length')
-        return prompt, self.geometry.grid, context_rows(len(self.pipe.tokenizer.tokenize(prompt)), tokens.pop()), \
-            groups, slabs
+        tokens = tokens.pop()
+        if not self.joint:
+            return prompt, self.geometry.grid, context_rows(len(self.pipe.tokenizer.tokenize(prompt)), tokens), \
+                groups, slabs
+        if encoder == 'clip':
+            return prompt, self.geometry.grid, context_rows(len(self.pipe.tokenizer.tokenize(prompt))), groups, slabs
+        if tokens < _T5_FIRST_ROW + 2:
+            raise RuntimeError(f'a context of {tokens} rows has no T5 rows after the {_T5_FIRST_ROW + 1} CLIP rows')
+        n = t5_rows(len(self.pipe.tokenizer_3.tokenize(prompt)), tokens)
+        for g, slab in zip(groups, slabs):
+            g.acc += _T5_FIRST_ROW * slab.h * slab.w * 4
+        return prompt, self.geometry.grid, list(range(n + 2)), groups, slabs
+
+    def _map_tokenizer(self, encoder: str, rows: List[int]):
+        """The tokenizer of a read's map: the pipeline's CLIP tokenizer, or for a T5 read ``pipe.tokenizer_3`` cut to
+        the map's ``len(rows) - 2`` pieces."""
+        return T5Pieces(self.pipe.tokenizer_3, len(rows) - 2) if encoder == 't5' else self.pipe.tokenizer
+
+
+# trace() options a joint-attention (SD3) trace refuses, besides launch='overlap'
+JOINT_REFUSED = ('time_resolved', 'step_ranges', 'negative', 'long_prompts', 'value_norms', 'save_heads', 'load_heads',
+                 'low_memory', 'locate_middle_block')
+# the context row a T5 read's group starts at: the last of the 77 CLIP rows, so that map row r + 1 is T5 row r
+_T5_FIRST_ROW = 76
+
+
+def _t5_start_row(maps: torch.Tensor, encoder: str) -> torch.Tensor:
+    """A T5 read's maps ``[..., rows, xh, xw]`` with row 0 (the last CLIP row the group starts at) set to zeros: T5
+    has no start token."""
+    if encoder == 't5':
+        maps[..., 0, :, :] = 0
+    return maps
 
 
 def _check_value_norms(layer_idx: int, attn):
@@ -993,6 +1121,10 @@ class PipelineHooker(ObjectHooker):
         tr.last_prompt = prompts[0]
         tr.last_prompts = prompts
         tr.last_negative_prompts = negatives
+        if tr.joint:                                 # SD3: the T5 encoder reads prompt_3 when one is given
+            bound = inspect.signature(hk_self._replaced['check_inputs']).bind(prompt, *args, **kwargs)
+            third = bound.arguments.get('prompt_3', kwargs.get('prompt_3'))
+            tr.last_prompts_3 = [third] * len(prompts) if third is None or isinstance(third, str) else list(third)
         return hk_self.monkey_super('check_inputs', prompt, *args, **kwargs)
 
     def _embeds_count(hk_self, prompt, args, kwargs) -> int:
@@ -1128,6 +1260,85 @@ class UNetCrossAttentionHooker(ObjectHooker):
     @property
     def num_heat_maps(self):
         return len(self.heat_maps)
+
+
+class JointAttentionHooker(ObjectHooker):
+    """The attention processor installed on one joint attention ``transformer_blocks[i].attn`` of an SD3 transformer,
+    in place of diffusers' ``JointAttnProcessor2_0``. It computes what that processor computes, op for op, except that
+    the attention runs through the SDPA op that also returns its log-sum-exp (flash for fp16 / bf16, memory-efficient
+    for fp32): that is the normaliser of the image-query x text-key block the heat map keeps, and the attention had to
+    compute it anyway. The layer call is then queued for ``daam_accumulate_joint``."""
+
+    def __init__(self, module, parent_trace: 'trace', layer_idx: int = 0):
+        super().__init__(module)
+        self.heat_maps = parent_trace.all_heat_maps
+        self.layer_idx = layer_idx
+        self.trace = parent_trace
+
+    def __call__(self, attn, hidden_states, encoder_hidden_states=None, attention_mask=None, *args, **kwargs):
+        if attention_mask is not None:
+            raise ValueError(f'layer {self.layer_idx}: the joint-attention heat map does not take an attention mask '
+                             f'(SD3 passes none)')
+        if encoder_hidden_states is None:                  # no context, no text attention: the block as it was
+            return self.original_processor(attn, hidden_states, encoder_hidden_states, attention_mask, *args,
+                                           **kwargs)
+        if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
+            raise RuntimeError('joint-attention heat maps cannot be captured into a CUDA graph: the layer hook, '
+                               'which a graph replay bypasses, queues every call')
+        residual = hidden_states
+        bsz, heads = hidden_states.shape[0], attn.heads
+        query = attn.to_q(hidden_states)
+        key = attn.to_k(hidden_states)
+        value = attn.to_v(hidden_states)
+        d = key.shape[-1] // heads
+        query = query.view(bsz, -1, heads, d).transpose(1, 2)
+        key = key.view(bsz, -1, heads, d).transpose(1, 2)
+        value = value.view(bsz, -1, heads, d).transpose(1, 2)
+        if attn.norm_q is not None:
+            query = attn.norm_q(query)
+        if attn.norm_k is not None:
+            key = attn.norm_k(key)
+        ctx_q = attn.add_q_proj(encoder_hidden_states).view(bsz, -1, heads, d).transpose(1, 2)
+        ctx_k = attn.add_k_proj(encoder_hidden_states).view(bsz, -1, heads, d).transpose(1, 2)
+        ctx_v = attn.add_v_proj(encoder_hidden_states).view(bsz, -1, heads, d).transpose(1, 2)
+        if attn.norm_added_q is not None:
+            ctx_q = attn.norm_added_q(ctx_q)
+        if attn.norm_added_k is not None:
+            ctx_k = attn.norm_added_k(ctx_k)
+        query = torch.cat([query, ctx_q], dim=2)
+        key = torch.cat([key, ctx_k], dim=2)
+        value = torch.cat([value, ctx_v], dim=2)
+        out, lse = _attention_with_lse(query, key, value)
+        n_image = residual.shape[1]
+        self.trace._gen_idx += 1
+        # the scale SDPA applies when none is given: 1 / sqrt(d), computed in double and used as a float
+        self.trace._enqueue_joint(self.layer_idx, query, key, lse, n_image, heads, 1.0 / math.sqrt(d))
+        hidden_states = out.transpose(1, 2).reshape(bsz, -1, heads * d).to(query.dtype)
+        hidden_states, encoder_hidden_states = hidden_states[:, :n_image], hidden_states[:, n_image:]
+        if not attn.context_pre_only:
+            encoder_hidden_states = attn.to_add_out(encoder_hidden_states)
+        hidden_states = attn.to_out[0](hidden_states)
+        hidden_states = attn.to_out[1](hidden_states)
+        return hidden_states, encoder_hidden_states
+
+    def _hook_impl(self):
+        self.original_processor = self.module.processor
+        self.module.set_processor(self)
+
+    def _unhook_impl(self):
+        self.module.set_processor(self.original_processor)
+
+
+def _attention_with_lse(query: torch.Tensor, key: torch.Tensor, value: torch.Tensor):
+    """``(out, lse)``: SDPA of ``[B, heads, L, d]`` operands with the default scale, and its log-sum-exp (natural log,
+    fp32 ``[B, heads, >= L]``). fp16 / bf16 take the flash kernel, fp32 the memory-efficient one (whose lse is padded
+    to a multiple of 32 queries): the kernels ``F.scaled_dot_product_attention`` picks under the matching
+    ``sdpa_kernel`` backend, so the output has their bits."""
+    if query.dtype in (torch.float16, torch.bfloat16):
+        res = torch.ops.aten._scaled_dot_product_flash_attention(query, key, value, 0.0, False, False)
+    else:
+        res = torch.ops.aten._scaled_dot_product_efficient_attention(query, key, value, None, True, 0.0, False)
+    return res[0], res[1]
 
 
 trace: Type[DiffusionHeatMapHooker] = DiffusionHeatMapHooker

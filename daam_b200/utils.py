@@ -12,7 +12,8 @@ from typing import List, Optional, Tuple, TypeVar
 import numpy as np
 import torch
 
-__all__ = ['set_seed', 'compute_token_merge_indices', 'cache_dir', 'auto_device', 'auto_autocast', 'context_rows']
+__all__ = ['set_seed', 'compute_token_merge_indices', 'cache_dir', 'auto_device', 'auto_autocast', 'context_rows',
+           't5_rows', 'T5Pieces']
 
 T = TypeVar('T')
 
@@ -73,6 +74,26 @@ def context_rows(n_tokens: int, tokens: int = CHUNK_TOKENS) -> List[int]:
     return [0] + rows + [rows[-1] + 1 if rows else 1]
 
 
+SENTENCEPIECE_MARK = '\u2581'   # '▁': the word-start marker of sentencepiece pieces (T5)
+
+
+def t5_rows(n_pieces: int, tokens: int, clip_tokens: int = CHUNK_TOKENS) -> int:
+    """How many T5 pieces of a prompt a joint-attention map has rows for: the ``tokens``-row context is ``clip_tokens``
+    CLIP rows and then the T5 rows, and the pieces are capped so that the T5 EOS row after them still fits."""
+    return max(0, min(int(n_pieces), tokens - clip_tokens - 1))
+
+
+class T5Pieces:
+    """The tokenizer of a T5 heat map: ``tokenizer.tokenize`` cut to the ``n`` pieces the map has rows for, so that
+    the word lookup never names a row past the map."""
+
+    def __init__(self, tokenizer, n: int):
+        self.tokenizer, self.n = tokenizer, n
+
+    def tokenize(self, text: str) -> List[str]:
+        return list(self.tokenizer.tokenize(text))[:self.n]
+
+
 def _pieces(tokenizer, text: str) -> List[str]:
     return [tok.replace('</w>', '') for tok in tokenizer.tokenize(text)]
 
@@ -81,12 +102,19 @@ def compute_token_merge_indices(tokenizer, prompt: str, word: str, word_idx: Opt
                                 offset_idx: int = 0) -> Tuple[List[int], Optional[int]]:
     """Rows of the global heat map that belong to ``word``: every occurrence of the word's token pieces in the
     lower-cased prompt, shifted by one for the SOS row. With ``word_idx`` the lookup is skipped and ``[word_idx + 1]``
-    returned. Raises ``ValueError('Search word ... not found in prompt!')`` like utils.py:86-87."""
+    returned. Raises ``ValueError('Search word ... not found in prompt!')`` like utils.py:86-87.
+
+    A sentencepiece tokenizer (T5: a word's first piece starts with ``▁``) keeps the case, since its vocabulary does:
+    the word's pieces are searched in the pieces of the prompt as written."""
     if word_idx is not None:
         return [word_idx + 1], word_idx
-    haystack = _pieces(tokenizer, prompt.lower())
-    word = word.lower()
     needle = _pieces(tokenizer, word)
+    if needle and needle[0].startswith(SENTENCEPIECE_MARK):
+        haystack = _pieces(tokenizer, prompt)
+    else:
+        haystack = _pieces(tokenizer, prompt.lower())
+        word = word.lower()
+        needle = _pieces(tokenizer, word)
     n = len(needle)
     rows: List[int] = []
     for start in range(len(haystack)):

@@ -41,7 +41,9 @@ extern "C" {
                                           daam_segment_crf;
                                           daam_word_distance, daam_mask_distance;
                                           daam_image_superpixels, daam_segment_superpixels;
-                                          daam_value_norms, daam_finalize_parts_weighted) */
+                                          daam_value_norms, daam_finalize_parts_weighted;
+                                          daam_joint_layer, daam_accumulate_joint; a key group's acc may point at
+                                          any row of a slab, see daam_key_group) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_TOKENS 231     /* daam_accumulate: long contexts of 2 or 3 CLIP chunks of 77 tokens (154, 231) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
@@ -130,6 +132,55 @@ typedef struct daam_layer {
 int daam_accumulate(const daam_layer* layers, int32_t n_layers, uint32_t flags, void* stream);
 
 /*
+ * Joint attention (MM-DiT, Stable Diffusion 3 / 3.5: daam_b200/trace.py traces pipe.transformer's
+ * transformer_blocks[i].attn). Image and context tokens go through ONE softmax over all hw + T keys, so the image-query x
+ * context-key block is not a softmax over the context alone. Its normaliser is the joint attention's log-sum-exp, which
+ * the attention itself returns (SDPA's logsumexp), so the heat map of one layer call is
+ *
+ *   acc[p][head][t][pixel] += exp(scale * <q[p][pixel][head][:], k[p][t][head][:]> - lse[p][head][pixel])
+ *
+ * q: the conditional IMAGE queries (after norm_q where the block has it); k: the conditional CONTEXT keys (after
+ * norm_added_k); lse: fp32, natural-log units, element (p, head, pixel) at lse + p * lse_stride_prompt +
+ * head * lse_stride_head + pixel * lse_stride_pixel, pointing at image query 0 of the first kept sample. Every other
+ * field, stride and rule is daam_layer's (n_prompts counts samples: prompts x images per prompt; the head_dim axis is
+ * contiguous; any int64 strides), except:
+ *  - tokens: any count in [1, DAAM_JOINT_MAX_TOKENS] (SD3: 77 CLIP rows + max_sequence_length T5 rows, 333 or 589);
+ *  - hw: any positive count (SD3 maps are (H / 16) x (W / 16));
+ *  - head_dim: a multiple of 8 up to DAAM_MAX_HEAD_DIM (DAAM_E_UNSUPPORTED otherwise).
+ *
+ * Arithmetic (every element of every layer, every dtype):
+ *   s  = <q, k> in fp32: fp16 / bf16 operands on tensor cores (mma.sync m16n8k16, products exact in fp32, the sum in
+ *        an unspecified order, |s - <q, k>| <= head_dim * 2^-23 * sum_e |q_e k_e| is the bound to test against);
+ *        fp32 operands: an fmaf chain over e ascending from 0 (SIMT kernel);
+ *   c  = fp32(scale * log2(e)),  l = fp32(lse * log2(e))   (log2(e) = 1.4426950408889634f);
+ *   v  = ex2.approx.ftz.f32(fmaf(s, c, -l))                 (relative error <= 2^-22 for v not subnormal);
+ *   acc = acc + v                                            (add.rn.f32).
+ * Each launch adds every element of every layer exactly once, with no atomics: layers whose accumulators share bytes
+ * go to different launches, in call order within a kernel class (16-bit: tensor cores, fp32: SIMT; the classes are
+ * issued 16-bit first). So the result does not depend on timing. All layers of one call of one class share a launch
+ * (up to DAAM_JOINT_MAX_LAYERS per launch).
+ * Errors: DAAM_E_INVALID for a null layer array, a null q / k / acc / lse, a misaligned acc (16 bytes), a non-positive
+ * n_prompts / heads / hw, an unknown dtype or a scale that is not positive; DAAM_E_UNSUPPORTED for tokens or head_dim
+ * outside the limits. `flags` is reserved: pass 0. Arguments are checked before the device is touched.
+ */
+#define DAAM_JOINT_MAX_TOKENS 1024
+#define DAAM_JOINT_MAX_LAYERS 64
+typedef struct daam_joint_layer {
+  const void* q;
+  const void* k;
+  float* acc;
+  int64_t q_stride_prompt, q_stride_pixel, q_stride_head;
+  int64_t k_stride_prompt, k_stride_token, k_stride_head;
+  int32_t n_prompts, heads, hw, tokens, head_dim;
+  int32_t dtype;
+  float scale;
+  int32_t reserved;
+  const float* lse;          /* device fp32 */
+  int64_t lse_stride_prompt, lse_stride_head, lse_stride_pixel;   /* in elements */
+} daam_joint_layer;
+int daam_accumulate_joint(const daam_joint_layer* layers, int32_t n_layers, uint32_t flags, void* stream);
+
+/*
  * Time-resolved heat maps (daam_b200/trace.py, trace(..., time_resolved=True)): daam_accumulate, and also
  *   step_acc[i][p][head][t][pixel] = the value added (flushed like the add)
  * so that one denoising step's per-key maps exist next to the time sum. With acc == 0 beforehand, step_acc equals acc
@@ -198,6 +249,10 @@ int daam_accumulate_probs(const void* probs, int32_t dtype, int32_t first_row, i
  * daam_finalize_maps reads a group as `n_blocks` such blocks back to back ([n_blocks][heads][tokens][h*w] from acc:
  * e.g. a whole slab [prompts][images * heads] with `heads` the heads per image) and head_sel applies inside each block;
  * the other entry points ignore n_blocks (it was `reserved`, callers set it to 0).
+ * `acc` may point at row r0 of such a block instead of row 0, with `tokens` still the block's row count (the head
+ * stride): the group's row t is then the slab's row r0 + t, and the rows a call reads, r0 + [0, n_rows), must lie in
+ * the slab's rows (the caller's condition; the call checks n_rows <= tokens only). The joint-attention T5 read does
+ * this with r0 = 76.
  */
 typedef struct daam_key_group {
   const float* acc;          /* device */
