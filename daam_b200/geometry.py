@@ -15,7 +15,7 @@ from __future__ import annotations
 import math
 from typing import Optional, Tuple
 
-__all__ = ['LatentGeometry']
+__all__ = ['LatentGeometry', 'JointGeometry', 'FluxGeometry']
 
 
 class LatentGeometry:
@@ -82,4 +82,27 @@ class JointGeometry:
         if h * w != n:
             raise RuntimeError(f'layer {layer_idx}: {n} image tokens, but the {self.latent_shape} latent in '
                                f'{self.patch_size} x {self.patch_size} patches gives {h} x {w}')
+        return h, w, 1
+
+
+class FluxGeometry:
+    """The heat-map geometry of a FLUX.1 transformer: the pipeline packs the ``(height / v, width / v)`` latent
+    (``v = vae_scale_factor``) into 2 x 2 patches, one image token each, so the grid is
+    ``(height // 2v, width // 2v)`` and every traced layer's keys have the grid's size and factor 1. ``image_size`` is
+    the ``(height, width)`` in pixels the pipeline passed to ``check_inputs``, ``None`` until then; the packed latent
+    ``[B, hw, 64]`` itself does not say which way round its ``hw`` tokens lie."""
+
+    def __init__(self, vae_scale_factor: int, image_size: Optional[Tuple[int, int]] = None):
+        self.vae_scale_factor = int(vae_scale_factor)
+        self.image_size = None if image_size is None else (int(image_size[0]), int(image_size[1]))
+        cell = 2 * self.vae_scale_factor
+        self.grid: Tuple[int, int] = (0, 0) if image_size is None else \
+            (self.image_size[0] // cell, self.image_size[1] // cell)
+
+    def level(self, n: int, layer_idx: int = 0) -> Tuple[int, int, int]:
+        """``(h, w, 1)`` for a layer of ``n`` image tokens; raises ``RuntimeError`` when ``n`` is not the grid's size."""
+        h, w = self.grid
+        if h * w != n:
+            raise RuntimeError(f'layer {layer_idx}: {n} image tokens, but a {self.image_size} (height, width) image '
+                               f'in {2 * self.vae_scale_factor}-pixel patches gives {h} x {w}')
         return h, w, 1

@@ -8,7 +8,9 @@ asked -- the ``mid_block``; inside a block whose class name contains ``CrossAttn
 
 An MM-DiT transformer (Stable Diffusion 3 / 3.5) has no cross-attention: :class:`JointAttentionLocator` takes the joint
 attention ``transformer_blocks[i].attn`` of every block, ``layer_idx = i``, named ``joint-attn-{i}``. The image-only
-``attn2`` some SD3.5 blocks add attends to no text and is not located.
+``attn2`` some SD3.5 blocks add attends to no text and is not located. A FLUX.1 transformer adds
+``single_transformer_blocks``, whose attention runs over the already-joined ``[text, image]`` sequence: they follow
+the double blocks, ``layer_idx = n_double + j``, named ``single-attn-{j}``.
 """
 from __future__ import annotations
 
@@ -65,13 +67,19 @@ class UNetCrossAttentionLocator(ModuleLocator):
 
 
 class JointAttentionLocator(ModuleLocator):
-    """``locate(transformer)`` returns ``transformer_blocks[*].attn`` in block order; ``layer_names`` is filled
-    alongside."""
+    """``locate(transformer)`` returns ``transformer_blocks[*].attn`` in block order, then (FLUX.1) the
+    ``single_transformer_blocks[*].attn`` in block order; ``layer_names`` is filled alongside. Double block ``i`` is
+    ``layer_idx = i``, named ``joint-attn-{i}``; single block ``j`` is ``layer_idx = n_double + j``, named
+    ``single-attn-{j}``."""
 
     def __init__(self):
         self.layer_names: List[str] = []
 
     def locate(self, model) -> list:
         found = [block.attn for block in model.transformer_blocks]
-        self.layer_names[:] = [f'joint-attn-{i}' for i in range(len(found))]
+        names = [f'joint-attn-{i}' for i in range(len(found))]
+        for j, block in enumerate(getattr(model, 'single_transformer_blocks', None) or ()):
+            found.append(block.attn)
+            names.append(f'single-attn-{j}')
+        self.layer_names[:] = names
         return found

@@ -207,12 +207,16 @@ def value_norms(value: torch.Tensor, weight: torch.Tensor, heads: int, out: Opti
 
 
 def make_joint_desc(q: torch.Tensor, k: torch.Tensor, lse: torch.Tensor, n_image: int, acc: torch.Tensor, heads: int,
-                    scale: float) -> _native.DaamJointLayer:
+                    scale: float, *, text_first: bool = False, whole_batch: bool = False) -> _native.DaamJointLayer:
     """One ``daam_joint_layer`` from a joint attention's operands as SDPA takes them: ``q`` / ``k`` ``[B, heads, L, d]``
     (any strides, ``d`` contiguous; e.g. the concatenation ``[image, context]`` of diffusers' ``JointAttnProcessor2_0``,
-    or a ``[B, L, heads*d]`` projection viewed that way), ``lse`` fp32 ``[B, heads, >= n_image]`` the attention's
+    or a ``[B, L, heads*d]`` projection viewed that way), ``lse`` fp32 ``[B, heads, >= n_image]`` (text-first: ``>= L``) the attention's
     log-sum-exp (natural log), ``n_image`` the image tokens ahead of the context in ``L``. The kept samples are
-    :func:`cond_half`'s; ``acc`` fp32 ``[n_prompts, n_heads, L - n_image, n_image]`` contiguous."""
+    :func:`cond_half`'s; ``acc`` fp32 ``[n_prompts, n_heads, L - n_image, n_image]`` contiguous.
+
+    ``text_first``: ``L`` is ``[context, image]`` (FLUX): the image queries and their lse start at row
+    ``T = L - n_image`` and the context keys at row 0. ``whole_batch``: every sample with every head is kept
+    (a batch without a CFG half), and ``acc`` is ``[B, heads, T, n_image]``."""
     if not (q.is_cuda and k.is_cuda and lse.is_cuda and acc.is_cuda):
         raise RuntimeError('daam_b200 computes on CUDA tensors only (there is no CPU fallback)')
     if q.dtype not in _DTYPES or k.dtype != q.dtype:
@@ -223,21 +227,22 @@ def make_joint_desc(q: torch.Tensor, k: torch.Tensor, lse: torch.Tensor, n_image
         raise RuntimeError('q and k must be [B, heads, L, d] with a contiguous d axis')
     bsz, _, _, d = q.shape
     tokens = k.shape[2] - n_image
-    first, n_prompts, head0, n_heads = cond_half(bsz, heads)
+    first, n_prompts, head0, n_heads = (0, bsz, 0, heads) if whole_batch else cond_half(bsz, heads)
     if tuple(acc.shape) != (n_prompts, n_heads, tokens, n_image) or acc.dtype != torch.float32 \
             or not acc.is_contiguous():
         raise RuntimeError(f'accumulator must be contiguous fp32 {(n_prompts, n_heads, tokens, n_image)}, '
                            f'got {acc.dtype} {tuple(acc.shape)}')
+    q_row, k_row = (tokens, 0) if text_first else (0, n_image)   # first image query, first context key
     es = q.element_size()
     return _native.DaamJointLayer(
-        q=q.data_ptr() + (first * q.stride(0) + head0 * q.stride(1)) * es,
-        k=k.data_ptr() + (first * k.stride(0) + head0 * k.stride(1) + n_image * k.stride(2)) * es,
+        q=q.data_ptr() + (first * q.stride(0) + head0 * q.stride(1) + q_row * q.stride(2)) * es,
+        k=k.data_ptr() + (first * k.stride(0) + head0 * k.stride(1) + k_row * k.stride(2)) * es,
         acc=acc.data_ptr(),
         q_stride_prompt=q.stride(0), q_stride_pixel=q.stride(2), q_stride_head=q.stride(1),
         k_stride_prompt=k.stride(0), k_stride_token=k.stride(2), k_stride_head=k.stride(1),
         n_prompts=n_prompts, heads=n_heads, hw=n_image, tokens=tokens, head_dim=d,
         dtype=_DTYPES[q.dtype], scale=float(scale), reserved=0,
-        lse=lse.data_ptr() + (first * lse.stride(0) + head0 * lse.stride(1)) * 4,
+        lse=lse.data_ptr() + (first * lse.stride(0) + head0 * lse.stride(1) + q_row * lse.stride(2)) * 4,
         lse_stride_prompt=lse.stride(0), lse_stride_head=lse.stride(1), lse_stride_pixel=lse.stride(2))
 
 

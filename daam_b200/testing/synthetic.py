@@ -34,7 +34,10 @@ __all__ = [
     'UNetSpec', 'SD21_SPEC', 'SD21_768_SPEC', 'SDXL_SPEC', 'SD15_SPEC', 'TINY_SPEC', 'TINY15_SPEC', 'TINY96_SPEC', 'make_pipeline',
     'JointAttnProcessor', 'SyntheticJointAttention', 'JointTransformerBlock', 'SyntheticSD3Transformer',
     'SentencePieceTokenizer', 'SyntheticSD3Pipeline', 'SD3Spec', 'SD3_MEDIUM_SPEC', 'SD35_LARGE_SPEC', 'TINY_SD3_SPEC',
-    'make_sd3_pipeline',
+    'make_sd3_pipeline', 'flux_rotary_emb', 'FluxAttnProcessor', 'SyntheticFluxAttention', 'FluxTransformerBlock',
+    'FluxSingleTransformerBlock', 'FluxPosEmbed', 'FluxSpec', 'FLUX_DEV_SPEC', 'FLUX_SCHNELL_SPEC', 'TINY_FLUX_SPEC',
+    'SyntheticFluxTransformer', 'flux_image_ids', 'flux_pack', 'flux_unpack', 'SyntheticFluxPipeline',
+    'make_flux_pipeline',
 ]
 
 
@@ -806,3 +809,361 @@ def make_sd3_pipeline(spec: SD3Spec = TINY_SD3_SPEC, dtype=torch.float32, device
         transformer = SyntheticSD3Transformer(spec)
     torch.random.set_rng_state(gen_state)
     return SyntheticSD3Pipeline(transformer, dtype=dtype, device=device, seed=seed)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# FLUX.1: MM-DiT with double-stream and single-stream blocks, packed latents and 3-axis RoPE
+# ---------------------------------------------------------------------------------------------------------------
+def flux_rotary_emb(x, freqs):
+    """diffusers' ``apply_rotary_emb(x, (cos, sin), use_real=True, use_real_unbind_dim=-1)``: ``x`` ``[B, H, S, D]``,
+    ``cos`` / ``sin`` ``[S, D]``; interleaved real / imaginary pairs, computed in fp32 and cast back."""
+    cos, sin = freqs
+    cos, sin = cos[None, None].to(x.device), sin[None, None].to(x.device)
+    x_real, x_imag = x.reshape(*x.shape[:-1], -1, 2).unbind(-1)
+    x_rotated = torch.stack([-x_imag, x_real], dim=-1).flatten(3)
+    return (x.float() * cos + x_rotated.float() * sin).to(x.dtype)
+
+
+class FluxAttnProcessor:
+    """The un-hooked FLUX attention: diffusers' ``FluxAttnProcessor2_0`` op for op (image projections, q / k norms on
+    ``[B, heads, N, d]``; with a context its projections and norms, concatenated context-then-image; RoPE on q and k;
+    one SDPA; with a context the split, ``to_out`` and ``to_add_out``, else the attention output alone)."""
+
+    def __call__(self, attn, hidden_states, encoder_hidden_states=None, attention_mask=None, image_rotary_emb=None):
+        b = hidden_states.shape[0] if encoder_hidden_states is None else encoder_hidden_states.shape[0]
+        query, key, value = attn.to_q(hidden_states), attn.to_k(hidden_states), attn.to_v(hidden_states)
+        d = key.shape[-1] // attn.heads
+        query = query.view(b, -1, attn.heads, d).transpose(1, 2)
+        key = key.view(b, -1, attn.heads, d).transpose(1, 2)
+        value = value.view(b, -1, attn.heads, d).transpose(1, 2)
+        if attn.norm_q is not None:
+            query = attn.norm_q(query)
+        if attn.norm_k is not None:
+            key = attn.norm_k(key)
+        if encoder_hidden_states is not None:
+            cq = attn.add_q_proj(encoder_hidden_states).view(b, -1, attn.heads, d).transpose(1, 2)
+            ck = attn.add_k_proj(encoder_hidden_states).view(b, -1, attn.heads, d).transpose(1, 2)
+            cv = attn.add_v_proj(encoder_hidden_states).view(b, -1, attn.heads, d).transpose(1, 2)
+            if attn.norm_added_q is not None:
+                cq = attn.norm_added_q(cq)
+            if attn.norm_added_k is not None:
+                ck = attn.norm_added_k(ck)
+            query = torch.cat([cq, query], dim=2)
+            key = torch.cat([ck, key], dim=2)
+            value = torch.cat([cv, value], dim=2)
+        if image_rotary_emb is not None:
+            query = flux_rotary_emb(query, image_rotary_emb)
+            key = flux_rotary_emb(key, image_rotary_emb)
+        hidden_states = F.scaled_dot_product_attention(query, key, value, attn_mask=attention_mask, dropout_p=0.0,
+                                                       is_causal=False)
+        hidden_states = hidden_states.transpose(1, 2).reshape(b, -1, attn.heads * d).to(query.dtype)
+        if encoder_hidden_states is None:
+            return hidden_states
+        encoder_hidden_states, hidden_states = hidden_states[:, :encoder_hidden_states.shape[1]], \
+            hidden_states[:, encoder_hidden_states.shape[1]:]
+        hidden_states = attn.to_out[1](attn.to_out[0](hidden_states))
+        encoder_hidden_states = attn.to_add_out(encoder_hidden_states)
+        return hidden_states, encoder_hidden_states
+
+
+class SyntheticFluxAttention(nn.Module):
+    """The attributes of diffusers' ``Attention`` as FLUX builds it (``qk_norm='rms_norm'``, ``bias=True``): a
+    double-stream attention has the ``add_*_proj`` context projections, their norms, ``to_out`` and ``to_add_out``;
+    a single-stream one (``pre_only``) has neither context projections nor ``to_out``."""
+
+    def __init__(self, dim: int, heads: int, dim_head: int, double: bool):
+        super().__init__()
+        inner = heads * dim_head
+        self.heads = heads
+        self.scale = dim_head ** -0.5
+        self.pre_only = not double
+        self.to_q, self.to_k, self.to_v = (nn.Linear(dim, inner) for _ in range(3))
+        self.norm_q, self.norm_k = nn.RMSNorm(dim_head, eps=1e-6), nn.RMSNorm(dim_head, eps=1e-6)
+        if double:
+            self.add_q_proj, self.add_k_proj, self.add_v_proj = (nn.Linear(dim, inner) for _ in range(3))
+            self.norm_added_q, self.norm_added_k = nn.RMSNorm(dim_head, eps=1e-6), nn.RMSNorm(dim_head, eps=1e-6)
+            self.to_out = nn.ModuleList([nn.Linear(inner, dim), nn.Dropout(0.0)])
+            self.to_add_out = nn.Linear(inner, dim)
+        else:
+            self.add_q_proj = self.add_k_proj = self.add_v_proj = None
+            self.norm_added_q = self.norm_added_k = None
+        self.processor = FluxAttnProcessor()
+
+    def set_processor(self, processor):
+        self.processor = processor
+
+    def forward(self, hidden_states, encoder_hidden_states=None, attention_mask=None, image_rotary_emb=None):
+        return self.processor(self, hidden_states, encoder_hidden_states, attention_mask, image_rotary_emb)
+
+
+class FluxTransformerBlock(nn.Module):
+    """A double-stream block: the joint attention over the modulated image and context streams, then a feed-forward
+    on each. Returns ``(encoder_hidden_states, hidden_states)`` as diffusers' does."""
+
+    def __init__(self, dim, heads, dim_head):
+        super().__init__()
+        self.norm1 = nn.LayerNorm(dim, elementwise_affine=False, eps=1e-6)
+        self.norm1_context = nn.LayerNorm(dim, elementwise_affine=False, eps=1e-6)
+        self.attn = SyntheticFluxAttention(dim, heads, dim_head, double=True)
+        self.ff = nn.Linear(dim, dim)
+        self.ff_context = nn.Linear(dim, dim)
+
+    def forward(self, hidden_states, encoder_hidden_states, temb, image_rotary_emb):
+        x = self.norm1(hidden_states) + temb[:, None]
+        c = self.norm1_context(encoder_hidden_states) + temb[:, None]
+        attn_out, ctx_out = self.attn(hidden_states=x, encoder_hidden_states=c, image_rotary_emb=image_rotary_emb)
+        hidden_states = hidden_states + attn_out
+        hidden_states = hidden_states + self.ff(F.gelu(hidden_states))
+        encoder_hidden_states = encoder_hidden_states + ctx_out
+        encoder_hidden_states = encoder_hidden_states + self.ff_context(F.gelu(encoder_hidden_states))
+        return encoder_hidden_states, hidden_states
+
+
+class FluxSingleTransformerBlock(nn.Module):
+    """A single-stream block on the joined ``[text, image]`` sequence: the attention (``pre_only``, no context
+    argument) in parallel with an MLP, both through ``proj_out``."""
+
+    def __init__(self, dim, heads, dim_head):
+        super().__init__()
+        self.norm = nn.LayerNorm(dim, elementwise_affine=False, eps=1e-6)
+        self.proj_mlp = nn.Linear(dim, dim)
+        self.attn = SyntheticFluxAttention(dim, heads, dim_head, double=False)
+        self.proj_out = nn.Linear(2 * dim, dim)
+
+    def forward(self, hidden_states, temb, image_rotary_emb):
+        x = self.norm(hidden_states) + temb[:, None]
+        mlp = F.gelu(self.proj_mlp(x), approximate='tanh')
+        attn_out = self.attn(hidden_states=x, image_rotary_emb=image_rotary_emb)
+        return hidden_states + self.proj_out(torch.cat([attn_out, mlp], dim=2))
+
+
+class FluxPosEmbed(nn.Module):
+    """diffusers' ``FluxPosEmbed``: per axis of the ``[S, 3]`` position ids, ``get_1d_rotary_pos_embed(dim, pos,
+    theta, use_real=True, repeat_interleave_real=True)`` in float64, concatenated over the axes: ``(cos, sin)``,
+    each fp32 ``[S, sum(axes_dim)]``."""
+
+    def __init__(self, theta: int, axes_dim: Sequence[int]):
+        super().__init__()
+        self.theta, self.axes_dim = theta, tuple(axes_dim)
+
+    def forward(self, ids):
+        pos = ids.float()
+        cos_out, sin_out = [], []
+        for i, dim in enumerate(self.axes_dim):
+            freqs = 1.0 / (self.theta ** (torch.arange(0, dim, 2, dtype=torch.float64, device=ids.device)[:dim // 2]
+                                          / dim))
+            freqs = torch.outer(pos[:, i].double(), freqs)
+            cos_out.append(freqs.cos().repeat_interleave(2, dim=1).float())
+            sin_out.append(freqs.sin().repeat_interleave(2, dim=1).float())
+        return torch.cat(cos_out, dim=-1), torch.cat(sin_out, dim=-1)
+
+
+@dataclass
+class FluxSpec:
+    """Shape of a FLUX.1 transformer: ``double`` double-stream and ``single`` single-stream blocks of ``heads`` heads
+    of ``dim_head`` (RoPE axes ``axes_dim``, summing to ``dim_head``), packed latents of ``in_channels`` (4 x the VAE's
+    channels), a T5 context of ``t5_rows`` rows (``max_sequence_length``) of ``joint_attention_dim`` channels and a
+    ``sample_size`` latent by default (the image is 8 x that)."""
+    name: str
+    double: int
+    single: int
+    heads: int = 24
+    dim_head: int = 128
+    axes_dim: Sequence[int] = (16, 56, 56)
+    in_channels: int = 64
+    joint_attention_dim: int = 4096
+    pooled_projection_dim: int = 768
+    t5_rows: int = 512
+    guidance_embeds: bool = True
+    sample_size: int = 128
+
+
+# public transformer/config.json shapes of black-forest-labs/FLUX.1-dev and FLUX.1-schnell; the pipelines' default
+# max_sequence_length is 512 for dev and 256 for schnell, at the default 1024-pixel (128 x 128 latent) size
+FLUX_DEV_SPEC = FluxSpec('flux.1-dev', 19, 38)
+FLUX_SCHNELL_SPEC = FluxSpec('flux.1-schnell', 19, 38, t5_rows=256, guidance_embeds=False)
+# a small tree for the tests: two double and three single blocks, 2 heads of 32 (RoPE axes 8 / 12 / 12), a 24-row T5
+# context, 256-pixel images by default
+TINY_FLUX_SPEC = FluxSpec('tiny-flux', 2, 3, heads=2, dim_head=32, axes_dim=(8, 12, 12), in_channels=16,
+                          joint_attention_dim=64, pooled_projection_dim=32, t5_rows=24, sample_size=32)
+
+
+class SyntheticFluxTransformer(nn.Module):
+    """FluxTransformer2DModel-shaped random-init network: ``x_embedder`` on the packed latent ``[B, hw, C]``, the
+    timestep / guidance / pooled embedding, ``context_embedder``, RoPE of ``cat(txt_ids, img_ids)``, the
+    ``transformer_blocks``, then the ``single_transformer_blocks`` on ``cat([context, image])``, and the image tokens
+    out. ``forward(hidden_states=, encoder_hidden_states=, pooled_projections=, timestep=, img_ids=, txt_ids=,
+    guidance=)`` returns a 1-tuple, as diffusers' does with ``return_dict=False``."""
+
+    def __init__(self, spec: FluxSpec):
+        super().__init__()
+        self.spec = spec
+        dim = spec.heads * spec.dim_head
+        self.config = SimpleNamespace(patch_size=1, in_channels=spec.in_channels, num_layers=spec.double,
+                                      num_single_layers=spec.single, attention_head_dim=spec.dim_head,
+                                      num_attention_heads=spec.heads, joint_attention_dim=spec.joint_attention_dim,
+                                      pooled_projection_dim=spec.pooled_projection_dim,
+                                      guidance_embeds=spec.guidance_embeds, axes_dims_rope=tuple(spec.axes_dim))
+        self.pos_embed = FluxPosEmbed(10000, spec.axes_dim)
+        self.time_proj = nn.Linear(1, dim)
+        self.guidance_proj = nn.Linear(1, dim) if spec.guidance_embeds else None
+        self.pooled_proj = nn.Linear(spec.pooled_projection_dim, dim)
+        self.context_embedder = nn.Linear(spec.joint_attention_dim, dim)
+        self.x_embedder = nn.Linear(spec.in_channels, dim)
+        self.transformer_blocks = nn.ModuleList([FluxTransformerBlock(dim, spec.heads, spec.dim_head)
+                                                 for _ in range(spec.double)])
+        self.single_transformer_blocks = nn.ModuleList([FluxSingleTransformerBlock(dim, spec.heads, spec.dim_head)
+                                                        for _ in range(spec.single)])
+        self.norm_out = nn.LayerNorm(dim, elementwise_affine=False, eps=1e-6)
+        self.proj_out = nn.Linear(dim, spec.in_channels)
+
+    def forward(self, hidden_states, encoder_hidden_states=None, pooled_projections=None, timestep=None, img_ids=None,
+                txt_ids=None, guidance=None, joint_attention_kwargs=None, return_dict: bool = False):
+        hidden_states = self.x_embedder(hidden_states)
+        dtype = hidden_states.dtype
+        temb = self.time_proj(timestep.reshape(-1, 1).to(dtype))
+        if self.guidance_proj is not None and guidance is not None:
+            temb = temb + self.guidance_proj(guidance.reshape(-1, 1).to(dtype))
+        temb = F.silu(temb + self.pooled_proj(pooled_projections))
+        encoder_hidden_states = self.context_embedder(encoder_hidden_states)
+        image_rotary_emb = self.pos_embed(torch.cat((txt_ids, img_ids), dim=0))
+        for block in self.transformer_blocks:
+            encoder_hidden_states, hidden_states = block(hidden_states, encoder_hidden_states, temb, image_rotary_emb)
+        hidden_states = torch.cat([encoder_hidden_states, hidden_states], dim=1)
+        for block in self.single_transformer_blocks:
+            hidden_states = block(hidden_states, temb, image_rotary_emb)
+        hidden_states = hidden_states[:, encoder_hidden_states.shape[1]:]
+        return (self.proj_out(self.norm_out(hidden_states)),)
+
+
+def flux_image_ids(height: int, width: int, device=None) -> torch.Tensor:
+    """diffusers' ``FluxPipeline._prepare_latent_image_ids`` for a packed ``height x width`` token grid: ``[hw, 3]``
+    with (0, row, column) per token, row-major."""
+    ids = torch.zeros(height, width, 3, device=device)
+    ids[..., 1] += torch.arange(height, device=device)[:, None]
+    ids[..., 2] += torch.arange(width, device=device)[None, :]
+    return ids.reshape(height * width, 3)
+
+
+def flux_pack(latents: torch.Tensor) -> torch.Tensor:
+    """diffusers' ``FluxPipeline._pack_latents``: ``[B, C, H, W]`` -> ``[B, (H/2)(W/2), 4C]`` in 2 x 2 patches."""
+    b, c, h, w = latents.shape
+    latents = latents.view(b, c, h // 2, 2, w // 2, 2).permute(0, 2, 4, 1, 3, 5)
+    return latents.reshape(b, (h // 2) * (w // 2), c * 4)
+
+
+def flux_unpack(latents: torch.Tensor, h: int, w: int) -> torch.Tensor:
+    """The inverse of :func:`flux_pack` for a ``h x w`` token grid: ``[B, hw, 4C]`` -> ``[B, C, 2h, 2w]``."""
+    b, _, c4 = latents.shape
+    latents = latents.view(b, h, w, c4 // 4, 2, 2).permute(0, 3, 1, 4, 2, 5)
+    return latents.reshape(b, c4 // 4, 2 * h, 2 * w)
+
+
+class SyntheticFluxPipeline:
+    """A FluxPipeline-shaped driver around :class:`SyntheticFluxTransformer`: ``transformer`` and no ``unet``,
+    ``tokenizer`` (CLIP-style, for the pooled embedding) and ``tokenizer_2`` (sentencepiece-style, for the T5 context),
+    ``check_inputs`` with diffusers' FLUX signature, called after the default size is filled in, and
+    ``image_processor.postprocess``. There is no CFG: one transformer forward per step over the ``prompts x images``
+    batch (prompt-major), with the guidance scale as an embedding input (dev) -- except that a negative prompt with
+    ``true_cfg_scale > 1`` runs a second forward on the negative embeddings, as diffusers' true CFG does. Latents are
+    packed in 2 x 2 patches; the scheduler is a plain flow-matching Euler step."""
+
+    def __init__(self, transformer: SyntheticFluxTransformer, dtype=torch.float32, device='cpu', seed: int = 0):
+        self.transformer = transformer.to(device=device, dtype=dtype).eval()
+        self.dtype, self.device = dtype, torch.device(device)
+        self.vae_scale_factor = 8
+        self.default_sample_size = transformer.spec.sample_size
+        self.tokenizer = WhitespaceTokenizer()
+        self.tokenizer_2 = SentencePieceTokenizer()
+        self.image_processor = _ImageProcessor()
+        self.seed = seed
+
+    def check_inputs(self, prompt, prompt_2, height, width, negative_prompt=None, negative_prompt_2=None,
+                     prompt_embeds=None, negative_prompt_embeds=None, pooled_prompt_embeds=None,
+                     negative_pooled_prompt_embeds=None, callback_on_step_end_tensor_inputs=None,
+                     max_sequence_length=None):
+        if prompt is None and prompt_embeds is None:
+            raise ValueError('Provide either `prompt` or `prompt_embeds`')
+        if prompt is not None and prompt_embeds is not None:
+            raise ValueError('Cannot forward both `prompt` and `prompt_embeds`')
+        if max_sequence_length is not None and max_sequence_length > 512:
+            raise ValueError(f'`max_sequence_length` cannot be greater than 512 but is {max_sequence_length}')
+
+    def _embeds(self, n: int, rows: int, generator: torch.Generator):
+        spec = self.transformer.spec
+        emb = torch.randn(n, rows, spec.joint_attention_dim, generator=generator)
+        pooled = torch.randn(n, spec.pooled_projection_dim, generator=generator)
+        return emb, pooled
+
+    @torch.no_grad()
+    def __call__(self, prompt=None, prompt_2=None, negative_prompt=None, negative_prompt_2=None,
+                 true_cfg_scale: float = 1.0, height: Optional[int] = None, width: Optional[int] = None,
+                 num_inference_steps: int = 28, guidance_scale: float = 3.5, num_images_per_prompt: int = 1,
+                 generator: Optional[torch.Generator] = None, prompt_embeds: Optional[torch.Tensor] = None,
+                 pooled_prompt_embeds: Optional[torch.Tensor] = None,
+                 negative_prompt_embeds: Optional[torch.Tensor] = None, max_sequence_length: int = 512):
+        """``max_sequence_length``: the T5 rows of the context (diffusers' default 512; the schnell pipeline is run
+        with 256). ``prompt_embeds`` ``[N, T, 4096]`` (with ``pooled_prompt_embeds``) replace the synthetic encoder's
+        draw."""
+        spec = self.transformer.spec
+        height = height or self.default_sample_size * self.vae_scale_factor
+        width = width or self.default_sample_size * self.vae_scale_factor
+        self.check_inputs(prompt, prompt_2, height, width, negative_prompt=negative_prompt,
+                          negative_prompt_2=negative_prompt_2, prompt_embeds=prompt_embeds,
+                          negative_prompt_embeds=negative_prompt_embeds, pooled_prompt_embeds=pooled_prompt_embeds,
+                          max_sequence_length=max_sequence_length)
+        if generator is None:
+            generator = torch.Generator().manual_seed(self.seed)
+        if prompt_embeds is not None:
+            n_prompts = prompt_embeds.shape[0]
+            emb = prompt_embeds.detach().float().cpu()
+            pooled = torch.zeros(n_prompts, spec.pooled_projection_dim) if pooled_prompt_embeds is None \
+                else pooled_prompt_embeds.detach().float().cpu()
+        else:
+            n_prompts = 1 if isinstance(prompt, str) else len(prompt)
+            emb, pooled = self._embeds(n_prompts, max_sequence_length, generator)
+        true_cfg = true_cfg_scale > 1 and (negative_prompt is not None or negative_prompt_embeds is not None)
+        if true_cfg:
+            neg, neg_pooled = self._embeds(n_prompts, emb.shape[1], generator)
+            if negative_prompt_embeds is not None:
+                neg = negative_prompt_embeds.detach().float().cpu()
+        n = n_prompts * num_images_per_prompt
+        rep = lambda t: t.repeat_interleave(num_images_per_prompt, dim=0).to(self.device, self.dtype)
+        emb, pooled = rep(emb), rep(pooled)
+        if true_cfg:
+            neg, neg_pooled = rep(neg), rep(neg_pooled)
+        lh, lw = 2 * (height // (2 * self.vae_scale_factor)), 2 * (width // (2 * self.vae_scale_factor))
+        lat = torch.randn(n, spec.in_channels // 4, lh, lw, generator=generator)
+        lat = flux_pack(lat).to(self.device, self.dtype)
+        img_ids = flux_image_ids(lh // 2, lw // 2, self.device).to(self.dtype)
+        txt_ids = torch.zeros(emb.shape[1], 3, device=self.device, dtype=self.dtype)
+        guidance = torch.full((n,), guidance_scale, device=self.device, dtype=torch.float32) \
+            if spec.guidance_embeds else None
+        sigmas = [1.0 - i / num_inference_steps for i in range(num_inference_steps)] + [0.0]
+        for i in range(num_inference_steps):
+            t = torch.full((n,), sigmas[i], device=self.device, dtype=self.dtype)
+            v = self.transformer(hidden_states=lat, timestep=t, guidance=guidance, pooled_projections=pooled,
+                                 encoder_hidden_states=emb, txt_ids=txt_ids, img_ids=img_ids, return_dict=False)[0]
+            if true_cfg:
+                v_neg = self.transformer(hidden_states=lat, timestep=t, guidance=guidance,
+                                         pooled_projections=neg_pooled, encoder_hidden_states=neg, txt_ids=txt_ids,
+                                         img_ids=img_ids, return_dict=False)[0]
+                v = v_neg + true_cfg_scale * (v - v_neg)
+            lat = (lat + (sigmas[i + 1] - sigmas[i]) * v).clamp(-4, 4)
+        image = flux_unpack(lat, lh // 2, lw // 2)[:, :3].float()
+        images = self.image_processor.postprocess(image, output_type='pil')
+        return SimpleNamespace(images=images, latents=lat)
+
+
+def make_flux_pipeline(spec: FluxSpec = TINY_FLUX_SPEC, dtype=torch.float32, device='cpu', seed: int = 0,
+                       init_on_device: bool = False) -> SyntheticFluxPipeline:
+    """Random-init FLUX-shaped pipeline; weights drawn on the CPU from ``seed`` unless ``init_on_device``."""
+    gen_state = torch.random.get_rng_state()
+    torch.manual_seed(seed)
+    if init_on_device and torch.device(device).type == 'cuda':
+        with torch.device(device):
+            transformer = SyntheticFluxTransformer(spec)
+    else:
+        transformer = SyntheticFluxTransformer(spec)
+    torch.random.set_rng_state(gen_state)
+    return SyntheticFluxPipeline(transformer, dtype=dtype, device=device, seed=seed)

@@ -46,7 +46,7 @@ import torch
 import torch.nn.functional as F
 
 from . import _native, ops
-from .geometry import JointGeometry, LatentGeometry
+from .geometry import FluxGeometry, JointGeometry, LatentGeometry
 from .heatmap import (FactorHeatMaps, GlobalHeatMap, HeadHeatMaps, ImageHeatMaps, LayerHeatMaps, LayerSlab,
                       RawHeatMapCollection, TimeHeatMaps)
 from .hook import AggregateHooker, ObjectHooker, UNetCrossAttentionLocator
@@ -54,7 +54,7 @@ from .locate import JointAttentionLocator
 from .utils import T5Pieces, cache_dir, context_rows, t5_rows
 
 __all__ = ['trace', 'DiffusionHeatMapHooker', 'GlobalHeatMap', 'UNetCrossAttentionHooker', 'JointAttentionHooker',
-           'PipelineHooker', 'ImageProcessorHooker']
+           'FluxAttentionHooker', 'PipelineHooker', 'ImageProcessorHooker']
 
 class DiffusionHeatMapHooker(AggregateHooker):
     """Context manager that traces every located cross-attention layer of ``pipeline.unet`` (trace.py:22-59).
@@ -80,6 +80,12 @@ class DiffusionHeatMapHooker(AggregateHooker):
     a map is the image-query x text-key block of each joint softmax, summed over steps (``daam_accumulate_joint``).
     Reads return the CLIP rows by default and the T5 rows with ``encoder='t5'``. Such a trace refuses the options it
     does not implement (see :data:`JOINT_REFUSED`) with a ``ValueError``.
+
+    A FLUX.1 pipeline (a ``transformer`` with ``single_transformer_blocks``) is traced through the double-stream
+    ``transformer_blocks[i].attn`` and then the single-stream ``single_transformer_blocks[j].attn``
+    (:class:`FluxAttentionHooker`), whose sequences are ``[text, image]``. Every sample of its guidance-distilled batch
+    is kept with all heads, reads return the T5 rows of ``prompt_2`` (or of the prompt), and it refuses what an SD3
+    trace refuses, negative prompts included.
     """
 
     def __init__(self, pipeline, low_memory: bool = False, load_heads: bool = False, save_heads: bool = False,
@@ -110,20 +116,29 @@ class DiffusionHeatMapHooker(AggregateHooker):
         if len(modes) > 1:
             raise ValueError('step_ranges cannot be combined with time_resolved=True')
         self.joint = getattr(pipeline, 'unet', None) is None and getattr(pipeline, 'transformer', None) is not None
+        # FLUX.1: a joint trace whose transformer also has single-stream blocks (text-first, no CFG half)
+        self.flux = self.joint and getattr(pipeline.transformer, 'single_transformer_blocks', None) is not None
         if self.joint:
+            model = 'a FLUX' if self.flux else 'an SD3'
             options = dict(time_resolved=time_resolved, step_ranges=step_ranges is not None, negative=negative,
                            long_prompts=long_prompts, value_norms=value_norms, save_heads=save_heads,
                            load_heads=load_heads, low_memory=low_memory, locate_middle_block=locate_middle_block)
             for name in JOINT_REFUSED:
                 if options[name]:
-                    raise ValueError(f'{name} is not supported when tracing the joint attention of an SD3 transformer')
+                    raise ValueError(f'{name} is not supported when tracing the joint attention of {model} '
+                                     f'transformer')
             if launch == 'overlap':
-                raise ValueError("launch='overlap' is not supported when tracing the joint attention of an SD3 "
-                                 "transformer: use 'step' or 'layer'")
+                raise ValueError(f"launch='overlap' is not supported when tracing the joint attention of {model} "
+                                 f"transformer: use 'step' or 'layer'")
         _native.load()   # fail here, loudly, if the CUDA library is missing
         self.all_heat_maps = RawHeatMapCollection()
         self.all_heat_maps.joint = self.joint
-        if self.joint:
+        if self.flux:
+            # FLUX: the grid is the image size check_inputs receives, in 2 x 2 packed latent patches
+            self.latent_hw = self._sample_size = None
+            self.geometry = FluxGeometry(pipeline.vae_scale_factor)
+            self.locator = JointAttentionLocator()
+        elif self.joint:
             # joint mode: the grid is the latent in patches, known from the first transformer forward
             self.latent_hw = self._sample_size = None
             self.geometry = JointGeometry(pipeline.transformer.config.patch_size)
@@ -138,6 +153,8 @@ class DiffusionHeatMapHooker(AggregateHooker):
             self.locator = UNetCrossAttentionLocator(restrict={0} if low_memory else None,
                                                      locate_middle_block=locate_middle_block or load_heads or save_heads)
         self.last_prompts_3: List[Optional[str]] = []   # joint mode: the T5 text (prompt_3) of every prompt, or None
+        self.last_prompts_2: List[Optional[str]] = []   # FLUX: the T5 text (prompt_2) of every prompt, or None
+        self._flux_tokens: Optional[int] = None   # FLUX: the context rows T of the running transformer forward
         self._joint_pending: List[_native.DaamJointLayer] = []   # joint mode: the layer calls of the running forward
         self.last_prompt: str = ''
         self.last_prompts: List[str] = []
@@ -193,8 +210,8 @@ class DiffusionHeatMapHooker(AggregateHooker):
                            for _ in range(1 if time_resolved else self.all_heat_maps.n_ranges)]
 
         if self.joint:
-            modules = [JointAttentionHooker(m, self, layer_idx=idx)
-                       for idx, m in enumerate(self.locator.locate(pipeline.transformer))]
+            hooker = FluxAttentionHooker if self.flux else JointAttentionHooker
+            modules = [hooker(m, self, layer_idx=idx) for idx, m in enumerate(self.locator.locate(pipeline.transformer))]
         else:
             modules = [
                 UNetCrossAttentionHooker(m, self, layer_idx=idx, latent_hw=self.latent_hw, load_heads=load_heads,
@@ -227,6 +244,9 @@ class DiffusionHeatMapHooker(AggregateHooker):
         if compute_kwargs.get('image_idx') is not None:
             per_prompt = len(self.last_images) // max(1, len(self._texts()))
             image = self.last_images[compute_kwargs.get('prompt_idx', 0) * per_prompt + compute_kwargs['image_idx']]
+        if self.flux:   # a T5 map: its own text (prompt_2 when given) and piece lookup
+            return GenerationExperiment(image, heat_map.heat_maps, heat_map.prompt, seed=seed, id=id, subtype=subtype,
+                                        path=path, tokenizer=heat_map.tokenizer)
         return GenerationExperiment(
             image,
             heat_map.heat_maps,
@@ -259,7 +279,13 @@ class DiffusionHeatMapHooker(AggregateHooker):
     # -- geometry -----------------------------------------------------------------------------------------------------
     def _see_sample(self, _module, args, kwargs):
         """UNet forward pre-hook: the latent ``sample`` (``args[0]`` or ``kwargs['sample']``) fixes the geometry; in
-        joint mode the transformer's ``hidden_states``."""
+        joint mode the transformer's ``hidden_states``. FLUX: the context rows ``T`` of ``encoder_hidden_states``,
+        which the single-stream blocks cannot see (the grid comes from ``check_inputs``)."""
+        if self.flux:
+            ctx = kwargs.get('encoder_hidden_states', args[1] if len(args) > 1 else None)
+            if ctx is not None:
+                self._flux_tokens = ctx.shape[1]
+            return
         if self.joint:
             sample = args[0] if args else kwargs.get('hidden_states')
             if sample is not None and tuple(sample.shape[-2:]) != self.geometry.latent_shape:
@@ -410,21 +436,26 @@ class DiffusionHeatMapHooker(AggregateHooker):
     def _enqueue_joint(self, layer_idx: int, q: torch.Tensor, k: torch.Tensor, lse: torch.Tensor, n_image: int,
                        heads: int, scale: float):
         """Joint mode: register one layer call, ``q`` / ``k`` ``[B, heads, n_image + T, d]`` (image tokens, then the
-        context) and the attention's ``lse``. Queued for the step launch at the end of the transformer forward, or
-        launched now with ``launch='layer'``."""
+        context; FLUX: the context, then the image tokens) and the attention's ``lse``. Queued for the step launch at
+        the end of the transformer forward, or launched now with ``launch='layer'``.
+
+        FLUX keeps every sample of the batch with every head (it has no CFG half)."""
         if not q.is_cuda:
             raise RuntimeError('daam_b200 traces pipelines that live on a CUDA device only (there is no CPU '
                                'fallback)')
         if layer_idx in self._queued:                      # the layer comes round again: a new forward has started
             self.flush()
         h, w, factor = self.geometry.level(n_image, layer_idx)
-        _, n_samples, head0, n_heads = ops.cond_half(q.shape[0], heads)
+        if self.flux:
+            n_samples, head0, n_heads = q.shape[0], 0, heads
+        else:
+            _, n_samples, head0, n_heads = ops.cond_half(q.shape[0], heads)
         n_real, images = self._prompt_layout(layer_idx, n_samples)
         tokens = k.shape[2] - n_image
         slab = self.all_heat_maps.slab_for(layer_idx, factor, n_real, images * n_heads, h, w, q.device, head0, images,
                                            tokens)
         desc = ops.make_joint_desc(q, k, lse, n_image, slab.acc.view(n_samples, n_heads, tokens, n_image), heads,
-                                   scale)
+                                   scale, text_first=self.flux, whole_batch=self.flux)
         self._device = q.device
         if self.launch == 'layer':
             ops.accumulate_joint([desc], q.device)
@@ -613,7 +644,7 @@ class DiffusionHeatMapHooker(AggregateHooker):
     def compute_global_heat_map(self, prompt=None, factors=None, head_idx=None, layer_idx=None, normalize=False,
                                 prompt_idx: int = 0, *, step_range: Optional[int] = None, negative: bool = False,
                                 image_idx: Optional[int] = None, value_weighted: bool = False,
-                                encoder: str = 'clip') -> GlobalHeatMap:
+                                encoder: Optional[str] = None) -> GlobalHeatMap:
         """Aggregate across time (already summed in the slabs) and across layers/heads (trace.py:83-132).
 
         Args mirror the reference: ``factors`` restricts the spatial factors, ``head_idx`` / ``layer_idx`` restrict to one
@@ -634,8 +665,11 @@ class DiffusionHeatMapHooker(AggregateHooker):
         ``encoder='t5'`` (a joint-attention trace of an SD3 pipeline): the map of the T5 rows of ``prompt_3`` (or of
         the prompt), in the CLIP map's layout: row 0 is zeros (T5 has no start token), rows ``1 .. n`` the
         sentencepiece pieces and row ``n + 1`` the T5 EOS, so the word lookup (``pipe.tokenizer_3``, case kept) and
-        every word-list call apply unchanged. The default reads the CLIP rows with ``pipe.tokenizer``.
+        every word-list call apply unchanged. The default (``encoder=None``) is the trace's own encoder: the CLIP rows
+        with ``pipe.tokenizer``, or on a FLUX trace, whose context is T5 rows only, the T5 rows of ``prompt_2`` (or of
+        the prompt) with ``pipe.tokenizer_2``, in the same layout (map row ``r >= 1`` is context row ``r - 1``).
         """
+        encoder = self._encoder(encoder)
         prompt, grid, rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range, layer_idx,
                                                               head_idx, negative, image_idx, encoder)
         tokenizer = self._map_tokenizer(encoder, rows)
@@ -657,9 +691,11 @@ class DiffusionHeatMapHooker(AggregateHooker):
         """Every image's map of prompt ``prompt_idx`` in one launch (``daam_finalize_maps``): ``heat_maps[i]`` is
         ``compute_global_heat_map(image_idx=i, ...)`` with the same arguments, bit for bit (``head_idx`` counts one
         image's heads). ``prompt``: the text, when it is not the generation's (e.g. one driven by ``prompt_embeds``).
-        Returns an :class:`ImageHeatMaps` ``[images, n_rows, xh, xw]``."""
+        Returns an :class:`ImageHeatMaps` ``[images, n_rows, xh, xw]``. The rows are those of the trace's own encoder
+        (a FLUX trace: T5)."""
+        encoder = self._encoder(None)
         prompt, grid, rows, _, slabs = self._read_groups(prompt, factors, prompt_idx, step_range, layer_idx, head_idx,
-                                                         negative, 0)
+                                                         negative, 0, encoder)
         images, n_prompts = slabs[0].images, slabs[0].n_prompts
         if not 0 <= prompt_idx < n_prompts:
             raise IndexError(f'prompt_idx {prompt_idx} is out of range for {n_prompts} prompt(s)')
@@ -672,7 +708,8 @@ class DiffusionHeatMapHooker(AggregateHooker):
         with torch.cuda.device(device):
             _native.finalize_maps(groups, maps, grid, normalize and n_fin == len(rows),
                                   torch.cuda.current_stream(device).cuda_stream)
-        return ImageHeatMaps(self.pipe.tokenizer, prompt, _compact(out, rows, normalize))
+        return ImageHeatMaps(self._map_tokenizer(encoder, rows), prompt,
+                             _t5_start_row(_compact(out, rows, normalize), encoder))
 
     def compute_time_heat_maps(self, prompt_idx: int = 0, normalize: bool = False, *,
                                negative: bool = False, image_idx: Optional[int] = None) -> TimeHeatMaps:
@@ -712,7 +749,7 @@ class DiffusionHeatMapHooker(AggregateHooker):
     def compute_per_head_heat_maps(self, prompt=None, factors=None, normalize=False, prompt_idx: int = 0, *,
                                    step_range: Optional[int] = None, negative: bool = False,
                                    image_idx: Optional[int] = None, value_weighted: bool = False,
-                                   encoder: str = 'clip'):
+                                   encoder: Optional[str] = None):
         """Every ``compute_global_heat_map(layer_idx=l, head_idx=h)`` of the reference's ``--all-heads`` sweep
         (daam/run/generate.py:239-255) in one launch. Returns ``(keys, maps)``: ``keys[i] = (factor, layer, head)`` and
         ``maps[i]`` the ``[n_tokens + 2, xh, xw]`` heat map the reference computes for that single key. ``step_range=i``
@@ -723,10 +760,11 @@ class DiffusionHeatMapHooker(AggregateHooker):
                               value_weighted, encoder)[1:3]
 
     def _per_head(self, prompt, factors, normalize, prompt_idx, step_range, negative, image_idx, value_weighted=False,
-                  encoder: str = 'clip'):
+                  encoder: Optional[str] = None):
         """``(prompt, keys, maps)`` of :meth:`compute_per_head_heat_maps`. Weighted: the per-key maps unnormalised,
         times each key's norm per row on the device, then normalised -- a single key's weighted global map. Also
         returns the map's tokenizer."""
+        encoder = self._encoder(encoder)
         prompt, grid, rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range,
                                                               negative=negative, image_idx=image_idx, encoder=encoder)
         keys = [(slab.factor, slab.layer_idx, head) for slab, g in zip(slabs, groups) for head in range(g.heads)]
@@ -787,7 +825,7 @@ class DiffusionHeatMapHooker(AggregateHooker):
     def compute_head_heat_maps(self, prompt=None, factors=None, normalize=False, prompt_idx: int = 0, *,
                                step_range: Optional[int] = None, negative: bool = False,
                                image_idx: Optional[int] = None, value_weighted: bool = False,
-                               encoder: str = 'clip') -> HeadHeatMaps:
+                               encoder: Optional[str] = None) -> HeadHeatMaps:
         """:meth:`compute_per_head_heat_maps` as a stack the word-list calls work on: a :class:`HeadHeatMaps` whose
         ``keys[i] = (factor, layer, head)`` labels ``heat_maps[i]``. The stack takes ``keys x rows x xh x xw x 4`` bytes
         (SD-2.1, 175 keys, 12 rows, 64 x 64: 34 MB; the 1100 keys of SDXL's 60 layers: 216 MB); ``factors`` and ``image_idx`` narrow
@@ -799,12 +837,13 @@ class DiffusionHeatMapHooker(AggregateHooker):
     def compute_layer_heat_maps(self, prompt=None, factors=None, head_idx=None, normalize=False, prompt_idx: int = 0, *,
                                 step_range: Optional[int] = None, negative: bool = False,
                                 image_idx: Optional[int] = None, value_weighted: bool = False,
-                                encoder: str = 'clip') -> LayerHeatMaps:
+                                encoder: Optional[str] = None) -> LayerHeatMaps:
         """Every traced layer's map in one launch (``daam_finalize_parts``): ``heat_maps[i]`` is
         ``compute_global_heat_map(layer_idx=layers[i], ...)`` with the same arguments, bit for bit. One map per layer
         that passes the filters (``head_idx``: the layers that have that head), in the order the layers were traced.
         Returns a :class:`LayerHeatMaps` ``[layers, n_rows, xh, xw]``. ``encoder``: as in
         :meth:`compute_global_heat_map`."""
+        encoder = self._encoder(encoder)
         prompt, grid, rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range, None, head_idx,
                                                               negative, image_idx, encoder)
         weights = self._weight_ptrs(slabs, prompt_idx, negative, image_idx) if value_weighted else None
@@ -819,14 +858,16 @@ class DiffusionHeatMapHooker(AggregateHooker):
                                  image_idx: Optional[int] = None, value_weighted: bool = False) -> FactorHeatMaps:
         """Every traced resolution's map in one launch (``daam_finalize_parts``): ``heat_maps[j]`` is
         ``compute_global_heat_map(factors={stack.factors[j]}, ...)`` with the same arguments, bit for bit; ``factors``
-        keeps some of them. Returns a :class:`FactorHeatMaps` ``[factors, n_rows, xh, xw]``, factors ascending."""
+        keeps some of them. Returns a :class:`FactorHeatMaps` ``[factors, n_rows, xh, xw]``, factors ascending. The
+        rows are those of the trace's own encoder (a FLUX trace: T5)."""
+        encoder = self._encoder(None)
         prompt, grid, rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range, layer_idx,
-                                                              head_idx, negative, image_idx)
+                                                              head_idx, negative, image_idx, encoder)
         order, found, parts = _factor_parts([s.factor for s in slabs])
         weights = self._weight_ptrs(slabs, prompt_idx, negative, image_idx) if value_weighted else None
         maps = self._finalize_parts([groups[i] for i in order], parts, grid, rows, normalize, slabs,
                                     None if weights is None else [weights[i] for i in order])
-        return FactorHeatMaps(self.pipe.tokenizer, prompt, maps, found)
+        return FactorHeatMaps(self._map_tokenizer(encoder, rows), prompt, _t5_start_row(maps, encoder), found)
 
     def _finalize_parts(self, groups, parts, grid, rows, normalize, slabs, weights=None) -> torch.Tensor:
         """One ``daam_finalize_parts`` over ``groups``: map ``m`` reduces groups ``[begin, begin + count)`` of
@@ -854,17 +895,22 @@ class DiffusionHeatMapHooker(AggregateHooker):
 
         A joint-attention trace reads the CLIP rows ``[0, n_tokens + 2)`` of its context, or with ``encoder='t5'`` the
         T5 rows: the groups then start at context row 76, so that map row ``r`` is context row ``76 + r`` (row 0, the
-        last CLIP row, is zeroed by the read), and the text is ``prompt_3`` when the generation had one."""
+        last CLIP row, is zeroed by the read), and the text is ``prompt_3`` when the generation had one. A FLUX trace
+        reads T5 rows only and its rows are ``[-1, 0, .., n]``: the finalize reads context rows ``[0, n + 1)`` from
+        row 0 of each key, and ``_compact`` puts the zero row -1 stands for ahead of them, so that map row ``r >= 1``
+        is context row ``r - 1`` (T5 has no start token); the text is ``prompt_2`` when the generation had one."""
         if encoder not in ('clip', 't5'):
             raise ValueError(f"encoder must be 'clip' or 't5', got {encoder!r}")
         if encoder == 't5':
             if not self.joint:
                 raise ValueError("encoder='t5' reads the T5 rows of a joint-attention (SD3) trace; this trace has "
                                  "CLIP contexts only")
-            if getattr(self.pipe, 'tokenizer_3', None) is None:
-                raise ValueError("encoder='t5' needs the pipeline's T5 tokenizer (pipe.tokenizer_3)")
-            if prompt is None and prompt_idx < len(self.last_prompts_3):
-                prompt = self.last_prompts_3[prompt_idx]
+            name = 'tokenizer_2' if self.flux else 'tokenizer_3'
+            if getattr(self.pipe, name, None) is None:
+                raise ValueError(f"encoder='t5' needs the pipeline's T5 tokenizer (pipe.{name})")
+            texts = self.last_prompts_2 if self.flux else self.last_prompts_3
+            if prompt is None and prompt_idx < len(texts):
+                prompt = texts[prompt_idx]
         if negative:
             self.all_heat_maps.check_negative()
         if prompt is None:
@@ -912,6 +958,9 @@ class DiffusionHeatMapHooker(AggregateHooker):
                 groups, slabs
         if encoder == 'clip':
             return prompt, self.geometry.grid, context_rows(len(self.pipe.tokenizer.tokenize(prompt))), groups, slabs
+        if self.flux:                                      # T5 rows only: pieces at context rows [0, n), EOS at n
+            n = t5_rows(len(self.pipe.tokenizer_2.tokenize(prompt)), tokens, clip_tokens=0)
+            return prompt, self.geometry.grid, [-1] + list(range(n + 1)), groups, slabs
         if tokens < _T5_FIRST_ROW + 2:
             raise RuntimeError(f'a context of {tokens} rows has no T5 rows after the {_T5_FIRST_ROW + 1} CLIP rows')
         n = t5_rows(len(self.pipe.tokenizer_3.tokenize(prompt)), tokens)
@@ -919,10 +968,22 @@ class DiffusionHeatMapHooker(AggregateHooker):
             g.acc += _T5_FIRST_ROW * slab.h * slab.w * 4
         return prompt, self.geometry.grid, list(range(n + 2)), groups, slabs
 
+    def _encoder(self, encoder: Optional[str]) -> str:
+        """A read's ``encoder``: ``None`` is the trace's own, ``'t5'`` on a FLUX trace (whose context is T5 rows only)
+        and ``'clip'`` otherwise."""
+        if encoder is None:
+            return 't5' if self.flux else 'clip'
+        if self.flux and encoder == 'clip':
+            raise ValueError("encoder='clip': the context of a FLUX transformer holds T5 rows only; read them with "
+                             "encoder='t5' (the default)")
+        return encoder
+
     def _map_tokenizer(self, encoder: str, rows: List[int]):
-        """The tokenizer of a read's map: the pipeline's CLIP tokenizer, or for a T5 read ``pipe.tokenizer_3`` cut to
-        the map's ``len(rows) - 2`` pieces."""
-        return T5Pieces(self.pipe.tokenizer_3, len(rows) - 2) if encoder == 't5' else self.pipe.tokenizer
+        """The tokenizer of a read's map: the pipeline's CLIP tokenizer, or for a T5 read the T5 tokenizer
+        (``pipe.tokenizer_3``; FLUX: ``pipe.tokenizer_2``) cut to the map's ``len(rows) - 2`` pieces."""
+        if encoder != 't5':
+            return self.pipe.tokenizer
+        return T5Pieces(self.pipe.tokenizer_2 if self.flux else self.pipe.tokenizer_3, len(rows) - 2)
 
 
 # trace() options a joint-attention (SD3) trace refuses, besides launch='overlap'
@@ -982,11 +1043,19 @@ def _compact(maps: torch.Tensor, rows: List[int], normalize: bool) -> torch.Tens
     ``rows`` gathered on the device in order (SOS, every prompt token, EOS), then with ``normalize`` divided by the sum
     of compact rows ``1 .. n`` plus 1e-6 (``daam_normalize_maps``: the reference's ``rows[1:-1]`` rule on the compact
     map). When the rows are the prefix itself (every 77-token read, and a long context whose prompt fits its first
-    chunk) the finalize call has normalised already and ``maps`` is returned as it is."""
+    chunk) the finalize call has normalised already and ``maps`` is returned as it is.
+
+    Row -1 (only as ``rows[0]``) stands for a row of zeros: a FLUX T5 map, whose rows are ``[-1, 0, .., n]``, puts it
+    ahead of the ``n + 1`` finalized context rows (T5 has no start token)."""
     if maps.shape[-3] == len(rows):
         return maps
-    index = torch.tensor(rows, dtype=torch.long).to(maps.device)
-    out = maps.index_select(maps.dim() - 3, index)
+    if rows[0] < 0:
+        maps = F.pad(maps, (0, 0, 0, 0, 1, 0))
+        rows = [r + 1 for r in rows]
+    if maps.shape[-3] == len(rows):                        # (the rows are the padded prefix: nothing to gather)
+        out = maps
+    else:
+        out = maps.index_select(maps.dim() - 3, torch.tensor(rows, dtype=torch.long).to(maps.device))
     if normalize:
         grid = tuple(out.shape[-2:])
         with torch.cuda.device(out.device):
@@ -1097,6 +1166,8 @@ class PipelineHooker(ObjectHooker):
 
     def _hooked_check_inputs(hk_self, _, prompt: Union[str, List[str], None], *args, **kwargs):
         tr = hk_self.parent_trace
+        if tr.flux:
+            hk_self._see_flux_inputs(prompt, args, kwargs)
         if prompt is None:
             # a generation driven by prompt_embeds (e.g. chunked long-prompt embeddings): the prompt count comes from
             # them, and no text is recorded (a read then needs prompt=...)
@@ -1121,11 +1192,35 @@ class PipelineHooker(ObjectHooker):
         tr.last_prompt = prompts[0]
         tr.last_prompts = prompts
         tr.last_negative_prompts = negatives
-        if tr.joint:                                 # SD3: the T5 encoder reads prompt_3 when one is given
+        if tr.joint and not tr.flux:                 # SD3: the T5 encoder reads prompt_3 when one is given
             bound = inspect.signature(hk_self._replaced['check_inputs']).bind(prompt, *args, **kwargs)
             third = bound.arguments.get('prompt_3', kwargs.get('prompt_3'))
             tr.last_prompts_3 = [third] * len(prompts) if third is None or isinstance(third, str) else list(third)
         return hk_self.monkey_super('check_inputs', prompt, *args, **kwargs)
+
+    def _see_flux_inputs(hk_self, prompt, args, kwargs):
+        """FLUX, at ``check_inputs(prompt, prompt_2, height, width, negative_prompt=None, negative_prompt_2=None,
+        prompt_embeds=None, negative_prompt_embeds=None, ...)``: refuses negative prompts (with them, true CFG runs a
+        second transformer forward per step that the trace cannot tell from the conditional one), records the T5 text
+        of every prompt (``prompt_2``, else the prompt) and sets the grid from ``height`` / ``width``."""
+        tr = hk_self.parent_trace
+        bound = inspect.signature(hk_self._replaced['check_inputs']).bind(prompt, *args, **kwargs).arguments
+        for name in ('negative_prompt', 'negative_prompt_2', 'negative_prompt_embeds'):
+            if bound.get(name, kwargs.get(name)) is not None:
+                raise ValueError(f'{name} is not supported when tracing the joint attention of a FLUX transformer: '
+                                 f'true CFG runs a second transformer forward per step, which the trace cannot tell '
+                                 f'apart from the conditional one')
+        second = bound.get('prompt_2', kwargs.get('prompt_2'))
+        n = hk_self._embeds_count(prompt, args, kwargs) if prompt is None else \
+            (1 if isinstance(prompt, str) else len(prompt))
+        texts = [prompt] * n if prompt is None or isinstance(prompt, str) else list(prompt)
+        if second is None:
+            tr.last_prompts_2 = texts
+        else:
+            tr.last_prompts_2 = [second] * n if isinstance(second, str) else list(second)
+        height, width = bound.get('height', kwargs.get('height')), bound.get('width', kwargs.get('width'))
+        tr.geometry = FluxGeometry(tr.geometry.vae_scale_factor,
+                                   None if height is None or width is None else (height, width))
 
     def _embeds_count(hk_self, prompt, args, kwargs) -> int:
         """The number of prompts of a ``check_inputs`` call without text: the batch of its ``prompt_embeds`` argument
@@ -1327,6 +1422,86 @@ class JointAttentionHooker(ObjectHooker):
 
     def _unhook_impl(self):
         self.module.set_processor(self.original_processor)
+
+
+class FluxAttentionHooker(JointAttentionHooker):
+    """The attention processor installed on one attention of a FLUX.1 transformer, double-stream
+    (``transformer_blocks[i].attn``, with a context) or single-stream (``single_transformer_blocks[j].attn``, on the
+    joined sequence, ``encoder_hidden_states=None``), in place of diffusers' ``FluxAttnProcessor2_0`` /
+    ``FluxAttnProcessor``. It computes what that processor computes, op for op: projections, q / k norms, for a double
+    block the context projections and norms concatenated ahead of the image as ``[context, image]``, RoPE on q and k,
+    one attention, then ``to_out`` and ``to_add_out`` (double) or the attention output alone (single, ``pre_only``).
+    The attention runs through the SDPA op that also returns the log-sum-exp, as :class:`JointAttentionHooker`'s does.
+    It reads only the submodules both diffusers' ``Attention`` and ``FluxAttention`` have, and ``attn.heads``."""
+
+    def __call__(self, attn, hidden_states, encoder_hidden_states=None, attention_mask=None, image_rotary_emb=None,
+                 *args, **kwargs):
+        if attention_mask is not None:
+            raise ValueError(f'layer {self.layer_idx}: the joint-attention heat map does not take an attention mask '
+                             f'(FLUX passes none)')
+        extra = [f'argument {i + 5}' for i, a in enumerate(args) if a is not None] + \
+            [name for name, value in kwargs.items() if value is not None]
+        if extra:                                          # e.g. an IP-Adapter's ip_hidden_states: not computed here
+            raise ValueError(f'layer {self.layer_idx}: the FLUX heat-map hook computes the plain FLUX attention only, '
+                             f'so it cannot take {", ".join(extra)} (the output would silently differ)')
+        if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
+            raise RuntimeError('FLUX joint-attention heat maps cannot be captured into a CUDA graph: the layer hook, '
+                               'which a graph replay bypasses, queues every call')
+        bsz, heads = hidden_states.shape[0], attn.heads
+        query = attn.to_q(hidden_states)
+        key = attn.to_k(hidden_states)
+        value = attn.to_v(hidden_states)
+        d = key.shape[-1] // heads
+        query = query.view(bsz, -1, heads, d).transpose(1, 2)
+        key = key.view(bsz, -1, heads, d).transpose(1, 2)
+        value = value.view(bsz, -1, heads, d).transpose(1, 2)
+        if attn.norm_q is not None:
+            query = attn.norm_q(query)
+        if attn.norm_k is not None:
+            key = attn.norm_k(key)
+        if encoder_hidden_states is not None:              # double stream: [context, image]
+            tokens = encoder_hidden_states.shape[1]
+            ctx_q = attn.add_q_proj(encoder_hidden_states).view(bsz, -1, heads, d).transpose(1, 2)
+            ctx_k = attn.add_k_proj(encoder_hidden_states).view(bsz, -1, heads, d).transpose(1, 2)
+            ctx_v = attn.add_v_proj(encoder_hidden_states).view(bsz, -1, heads, d).transpose(1, 2)
+            if attn.norm_added_q is not None:
+                ctx_q = attn.norm_added_q(ctx_q)
+            if attn.norm_added_k is not None:
+                ctx_k = attn.norm_added_k(ctx_k)
+            query = torch.cat([ctx_q, query], dim=2)
+            key = torch.cat([ctx_k, key], dim=2)
+            value = torch.cat([ctx_v, value], dim=2)
+        else:                                              # single stream: the text rows come from the forward
+            tokens = self.trace._flux_tokens
+            if tokens is None:
+                raise RuntimeError(f'layer {self.layer_idx}: a single-stream FLUX block was called outside a '
+                                   f'transformer forward, so its context length is unknown')
+        if image_rotary_emb is not None:
+            query = _apply_rotary_emb(query, image_rotary_emb)
+            key = _apply_rotary_emb(key, image_rotary_emb)
+        out, lse = _attention_with_lse(query, key, value)
+        self.trace._gen_idx += 1
+        # the scale SDPA applies when none is given: 1 / sqrt(d), computed in double and used as a float
+        self.trace._enqueue_joint(self.layer_idx, query, key, lse, query.shape[2] - tokens, heads, 1.0 / math.sqrt(d))
+        hidden_states = out.transpose(1, 2).reshape(bsz, -1, heads * d).to(query.dtype)
+        if encoder_hidden_states is None:
+            return hidden_states
+        encoder_hidden_states, hidden_states = hidden_states[:, :tokens], hidden_states[:, tokens:]
+        hidden_states = attn.to_out[0](hidden_states)
+        hidden_states = attn.to_out[1](hidden_states)
+        encoder_hidden_states = attn.to_add_out(encoder_hidden_states)
+        return hidden_states, encoder_hidden_states
+
+
+def _apply_rotary_emb(x: torch.Tensor, freqs) -> torch.Tensor:
+    """diffusers' ``apply_rotary_emb(x, (cos, sin), use_real=True, use_real_unbind_dim=-1)`` on ``x``
+    ``[B, heads, L, d]`` with ``cos`` / ``sin`` ``[L, d]``: the interleaved pairs ``(x0, x1)`` rotate as
+    ``(x0 cos - x1 sin, x1 cos + x0 sin)``, computed in fp32 and cast back."""
+    cos, sin = freqs
+    cos, sin = cos[None, None].to(x.device), sin[None, None].to(x.device)
+    x_real, x_imag = x.reshape(*x.shape[:-1], -1, 2).unbind(-1)
+    x_rotated = torch.stack([-x_imag, x_real], dim=-1).flatten(3)
+    return (x.float() * cos + x_rotated.float() * sin).to(x.dtype)
 
 
 def _attention_with_lse(query: torch.Tensor, key: torch.Tensor, value: torch.Tensor):

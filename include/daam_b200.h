@@ -133,7 +133,9 @@ int daam_accumulate(const daam_layer* layers, int32_t n_layers, uint32_t flags, 
 
 /*
  * Joint attention (MM-DiT, Stable Diffusion 3 / 3.5: daam_b200/trace.py traces pipe.transformer's
- * transformer_blocks[i].attn). Image and context tokens go through ONE softmax over all hw + T keys, so the image-query x
+ * transformer_blocks[i].attn; FLUX.1: also single_transformer_blocks[j].attn, whose sequences are text-first,
+ * [context, image], so q and lse point at row T of the sequence and k at row 0, and every sample is kept since the
+ * batch has no CFG half). Image and context tokens go through ONE softmax over all hw + T keys, so the image-query x
  * context-key block is not a softmax over the context alone. Its normaliser is the joint attention's log-sum-exp, which
  * the attention itself returns (SDPA's logsumexp), so the heat map of one layer call is
  *
