@@ -440,7 +440,9 @@ def accumulate(layers, stream: int, flags: int = ACC_AUTO):
 
 
 def accumulate_joint(layers: Sequence[DaamJointLayer], stream: int):
-    """``daam_accumulate_joint`` over a sequence of :class:`DaamJointLayer` (one launch per kernel class)."""
+    """``daam_accumulate_joint`` over a sequence of :class:`DaamJointLayer`: classes fp16, bf16, fp32 in that order,
+    each in call order, in one launch per class unless a layer overlaps one already in the launch or the launch holds
+    ``DAAM_JOINT_MAX_LAYERS``."""
     if not layers:
         return
     array = (DaamJointLayer * len(layers))(*layers)

@@ -225,8 +225,21 @@ def make_joint_desc(q: torch.Tensor, k: torch.Tensor, lse: torch.Tensor, n_image
         raise RuntimeError(f'lse must be fp32 [B, heads, L], got {lse.dtype} {tuple(lse.shape)}')
     if q.dim() != 4 or k.dim() != 4 or q.stride(-1) != 1 or k.stride(-1) != 1:
         raise RuntimeError('q and k must be [B, heads, L, d] with a contiguous d axis')
-    bsz, _, _, d = q.shape
-    tokens = k.shape[2] - n_image
+    bsz, _, seq, d = q.shape
+    if k.shape[0] != bsz or lse.shape[0] != bsz:
+        raise RuntimeError(f'q, k and lse must have one batch size, got {bsz}, {k.shape[0]} and {lse.shape[0]}')
+    if min(q.shape[1], k.shape[1], lse.shape[1]) < heads:
+        raise RuntimeError(f'q, k and lse must have at least {heads} heads, got {q.shape[1]}, {k.shape[1]} and '
+                           f'{lse.shape[1]}')
+    if k.shape[2] != seq or k.shape[3] != d:
+        raise RuntimeError(f'q and k must have one sequence length and head dim, got {tuple(q.shape[2:])} and '
+                           f'{tuple(k.shape[2:])}')
+    if not 0 < n_image < seq:
+        raise RuntimeError(f'n_image = {n_image} must leave image and context tokens in a sequence of {seq}')
+    lse_rows = seq if text_first else n_image
+    if lse.shape[2] < lse_rows:
+        raise RuntimeError(f'lse has {lse.shape[2]} rows, the kernel reads {lse_rows}')
+    tokens = seq - n_image
     first, n_prompts, head0, n_heads = (0, bsz, 0, heads) if whole_batch else cond_half(bsz, heads)
     if tuple(acc.shape) != (n_prompts, n_heads, tokens, n_image) or acc.dtype != torch.float32 \
             or not acc.is_contiguous():

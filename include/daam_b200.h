@@ -157,10 +157,12 @@ int daam_accumulate(const daam_layer* layers, int32_t n_layers, uint32_t flags, 
  *   c  = fp32(scale * log2(e)),  l = fp32(lse * log2(e))   (log2(e) = 1.4426950408889634f);
  *   v  = ex2.approx.ftz.f32(fmaf(s, c, -l))                 (relative error <= 2^-22 for v not subnormal);
  *   acc = acc + v                                            (add.rn.f32).
- * Each launch adds every element of every layer exactly once, with no atomics: layers whose accumulators share bytes
- * go to different launches, in call order within a kernel class (16-bit: tensor cores, fp32: SIMT; the classes are
- * issued 16-bit first). So the result does not depend on timing. All layers of one call of one class share a launch
- * (up to DAAM_JOINT_MAX_LAYERS per launch).
+ * Each launch adds every element of every layer exactly once, with no atomics. The layers of a call fall into three
+ * kernel classes by dtype, issued in this order: fp16 (tensor cores), bf16 (tensor cores, a kernel of its own) and
+ * fp32 (SIMT); within a class the layers are applied in call order. So layers of different dtypes that share
+ * accumulator bytes add fp16 first, then bf16, then fp32, whatever their call order, and the result does not depend
+ * on timing. The layers of one class share a launch until one of them shares accumulator bytes with a layer already
+ * in it, or the launch holds DAAM_JOINT_MAX_LAYERS: that layer starts the class's next launch.
  * Errors: DAAM_E_INVALID for a null layer array, a null q / k / acc / lse, a misaligned acc (16 bytes), a non-positive
  * n_prompts / heads / hw, an unknown dtype or a scale that is not positive; DAAM_E_UNSUPPORTED for tokens or head_dim
  * outside the limits. `flags` is reserved: pass 0. Arguments are checked before the device is touched.

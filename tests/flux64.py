@@ -5,7 +5,7 @@ bicubic upsample is the identity and every value is already >= 0). Also the per-
 arithmetic as ``include/daam_b200.h`` states it."""
 import torch
 
-LOG2E = 1.4426950408889634
+from tests.joint64 import exp_and_bound
 
 
 def flux_block(q: torch.Tensor, k: torch.Tensor, tokens: int, scale: float) -> torch.Tensor:
@@ -48,22 +48,10 @@ def global_rows(per_layer, n: int, prompt: int = 0, images: int = 1, normalize: 
 
 
 def reference_and_bound(q, k, lse, tokens: int, scale: float):
-    """float64 ``exp(scale32 <q, k> - lse32)`` of every sample, ``[B, heads, T, hw]`` for text-first operands, and the
-    per-element bound of the header's arithmetic: the dot product within d 2^-23 sum|q k|, the three fp32 roundings of
-    the exponent, and ex2.approx within 2^-22."""
+    """:func:`tests.joint64.exp_and_bound` of text-first operands ``[B, heads, T + hw, d]`` over every sample:
+    ``[B, heads, T, hw]`` and its bound."""
     hw = q.shape[2] - tokens
-    qd, kd = q[:, :, tokens:].double(), k[:, :, :tokens].double()
-    d = q.shape[-1]
-    scale32 = float(torch.tensor(scale, dtype=torch.float32))
-    dot = torch.einsum('bhid,bhjd->bhji', qd, kd)
-    absdot = torch.einsum('bhid,bhjd->bhji', qd.abs(), kd.abs())
-    l = lse[:, :, tokens:tokens + hw].double()[:, :, None, :]
-    x = dot * scale32 * LOG2E - l * LOG2E
-    ref = torch.exp2(x)
-    err_x = scale32 * LOG2E * d * 2.0 ** -23 * absdot + (dot.abs() * scale32 * LOG2E + l.abs() * LOG2E
-                                                          + x.abs()) * 2.0 ** -23
-    bound = ref * (torch.exp2(err_x) - 1) * 1.01 + ref * 2.0 ** -21 + 1e-37
-    return ref, bound
+    return exp_and_bound(q[:, :, tokens:], k[:, :, :tokens], lse[:, :, tokens:tokens + hw], scale)
 
 
 def rope64(x: torch.Tensor, ids: torch.Tensor, axes_dim, theta: float = 10000.0) -> torch.Tensor:

@@ -1,8 +1,36 @@
 """float64 restatement of the joint-attention heat map (MM-DiT, Stable Diffusion 3): one softmax over every image and
 context key, of which the image-query x context-key block is kept, summed over the traced calls, averaged over the
 (sample, head) keys of a prompt; the rows of a read are then taken from that mean (factor 1: the bicubic upsample is
-the identity and every value is already >= 0)."""
+the identity and every value is already >= 0). Also the per-element bound of daam_accumulate_joint's arithmetic as
+``include/daam_b200.h`` states it."""
 import torch
+
+LOG2E = 1.4426950408889634
+
+
+def exp_and_bound(q: torch.Tensor, k: torch.Tensor, lse: torch.Tensor, scale: float):
+    """``q`` ``[N, heads, hw, d]`` the kept image queries, ``k`` ``[N, heads, T, d]`` the kept context keys, ``lse``
+    ``[N, heads, hw]`` fp32: the float64 ``exp(scale32 <q, k> - lse32)``, ``[N, heads, T, hw]``, and the per-element
+    bound of the header's arithmetic: the dot product within d 2^-23 sum|q k|, the three fp32 roundings of the
+    exponent, and ex2.approx within 2^-22."""
+    qd, kd = q.double(), k.double()
+    d = q.shape[-1]
+    scale32 = float(torch.tensor(scale, dtype=torch.float32))
+    dot = torch.einsum('bhid,bhjd->bhji', qd, kd)
+    absdot = torch.einsum('bhid,bhjd->bhji', qd.abs(), kd.abs())
+    l = lse.double()[:, :, None, :]
+    x = dot * scale32 * LOG2E - l * LOG2E
+    ref = torch.exp2(x)
+    err_x = scale32 * LOG2E * d * 2.0 ** -23 * absdot + (dot.abs() * scale32 * LOG2E + l.abs() * LOG2E
+                                                          + x.abs()) * 2.0 ** -23
+    bound = ref * (torch.exp2(err_x) - 1) * 1.01 + ref * 2.0 ** -21 + 1e-37
+    return ref, bound
+
+
+def reference_and_bound(q, k, lse, hw: int, scale: float, keep):
+    """:func:`exp_and_bound` of image-first operands ``[B, heads, hw + T, d]`` (lse ``[B, heads, >= hw]``) over the
+    kept samples ``keep``."""
+    return exp_and_bound(q[keep, :, :hw], k[keep, :, hw:], lse[keep, :, :hw], scale)
 
 
 def joint_block(q: torch.Tensor, k: torch.Tensor, n_image: int, scale: float) -> torch.Tensor:

@@ -15,7 +15,6 @@ from tests import joint64
 pytestmark = pytest.mark.gpu
 
 DT = {'fp32': torch.float32, 'fp16': torch.float16, 'bf16': torch.bfloat16}
-LOG2E = 1.4426950408889634
 
 
 def _inputs(dtype, bsz, heads, hw, tokens, d, seed, layout='bhld', spread=1.0):
@@ -37,22 +36,7 @@ def _inputs(dtype, bsz, heads, hw, tokens, d, seed, layout='bhld', spread=1.0):
     return q, k, lse, scale
 
 
-def _reference_and_bound(q, k, lse, hw, scale, keep):
-    """float64 ``exp(scale32 <q, k> - lse32)`` of the kept samples, ``[N, heads, T, hw]``, and the per-element bound of
-    the header's arithmetic: the dot product within d 2^-23 sum|q k|, the three fp32 roundings of the exponent, and
-    ex2.approx within 2^-22."""
-    qd, kd = q[keep, :, :hw].double(), k[keep, :, hw:].double()
-    d = q.shape[-1]
-    scale32 = float(torch.tensor(scale, dtype=torch.float32))
-    dot = torch.einsum('bhid,bhjd->bhji', qd, kd)
-    absdot = torch.einsum('bhid,bhjd->bhji', qd.abs(), kd.abs())
-    l = lse[keep].double()[:, :, None, :]
-    x = dot * scale32 * LOG2E - l * LOG2E
-    ref = torch.exp2(x)
-    err_x = scale32 * LOG2E * d * 2.0 ** -23 * absdot + (dot.abs() * scale32 * LOG2E + l.abs() * LOG2E
-                                                          + x.abs()) * 2.0 ** -23
-    bound = ref * (torch.exp2(err_x) - 1) * 1.01 + ref * 2.0 ** -21 + 1e-37
-    return ref, bound
+_reference_and_bound = joint64.reference_and_bound
 
 
 def _check(got, ref, bound, what):

@@ -31,10 +31,6 @@ import bisect
 import collections
 import dataclasses
 import json
-import os
-import re
-import subprocess
-import sys
 import tempfile
 from dataclasses import dataclass
 from typing import Callable, Dict, List, Optional, Tuple
@@ -45,10 +41,10 @@ import torch
 from daam_b200 import _native
 from tests.reference64 import (ACC_DIMS, FP32_EPS, accumulate_tolerance, assert_close64, desc_maps64, layer_views64,
                                probs_tolerance)
+from tests.util import kernel_events, traced
 
 pytestmark = pytest.mark.gpu
 DEV = 'cuda'
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 TILE = 128                   # kTilePixels
 TOKENS = 77
@@ -657,26 +653,6 @@ def _sm_count() -> int:
     return _native.device_info()['sm_count']
 
 
-def _kernel_events(prof, tmp_dir: str) -> List[Tuple[str, Optional[int]]]:
-    """``(instance, grid.x)`` of every accumulate / attention_probs kernel of a trace, in launch order."""
-    path = os.path.join(tmp_dir, 'launches.pt.trace.json')
-    prof.export_chrome_trace(path)
-    events = []
-    with open(path) as f:
-        trace = json.load(f)
-    for e in trace['traceEvents']:
-        if e.get('cat') != 'kernel':
-            continue
-        m = re.search(r'(accumulate_\w+_kernel|attention_probs_kernel)(<[^<>]*>)?', e['name'])
-        if not m or m.group(1) == 'accumulate_probs_kernel':
-            continue
-        args = e.get('args', {})
-        grid = args.get('grid')
-        events.append((args.get('correlation', e['ts']), e['ts'], m.group(0).replace(' ', ''),
-                       grid[0] if grid else None))
-    return [(inst, grid) for _, _, inst, grid in sorted(events)]
-
-
 def _occupancy_case(inst: str, d: int, sm: int) -> Case:
     """One SIMT layer of 16 sm_count tiles for ``inst`` at head_dim ``d``: its grid is sm_count x the occupancy."""
     entry = {v: k for k, v in SIMT_KERNEL.items()}.get(inst, 'accumulate')
@@ -703,20 +679,12 @@ def _trace_main(request: str):
                 run.call(case.flags)
                 torch.cuda.synchronize()
                 del run
-        print(json.dumps(_kernel_events(prof, tmp)))
+        print(json.dumps(kernel_events(prof, tmp)))
 
 
 def _traced(request: dict) -> List[Tuple[str, Optional[int]]]:
-    """``_trace_main(request)`` in a fresh Python process. A CUDA activity trace taken in a process that has already
-    run tests/test_accumulate_steps_gpu.py (which does not profile) holds no kernel event at all, while the same
-    trace taken before it does (H100, torch 2.11): some CUPTI / Kineto state left by the earlier work is the likely
-    cause, not found yet. A process of its own gives the trace the state a lone run of this module has."""
-    code = f'import tests.test_launch_geometry_gpu as m; m._trace_main({json.dumps(request)!r})'
-    flags = ['-s'] if sys.flags.no_user_site else []
-    out = subprocess.run([sys.executable] + flags + ['-c', code], cwd=ROOT, capture_output=True, text=True,
-                         timeout=900)
-    assert out.returncode == 0, out.stderr[-4000:]
-    return [tuple(e) for e in json.loads(out.stdout.strip().splitlines()[-1])]
+    """``_trace_main(request)`` in a fresh Python process (``tests.util.traced``)."""
+    return traced('tests.test_launch_geometry_gpu', request)
 
 
 # SIMT occupancy, measured: one launch of 16 sm_count tiles per (instance, largest head_dim), grid read from the trace

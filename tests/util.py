@@ -1,9 +1,16 @@
-"""Shared helpers of the test-suite (oracle access, fixture loading, CPU-side recomputation of GPU inputs)."""
+"""Shared helpers of the test-suite (oracle access, fixture loading, CPU-side recomputation of GPU inputs, profiler
+traces of the launches)."""
+import json
 import os
+import re
+import subprocess
+import sys
+from typing import List, Optional, Tuple
 
 import numpy as np
 import torch
 
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
 LAYER_FIXTURES = ['layer_hw256_h2_d64', 'layer_hw1024_h1_d64_peaky', 'layer_hw64_h2_d40', 'layer_hw576_h1_d64']
 
@@ -47,6 +54,40 @@ def assert_elementwise(got, ref, rtol, atol, what=''):
         raise AssertionError(f'{what}: element {i}: got {got.flatten()[i]:.9e} ref {ref.flatten()[i]:.9e} '
                              f'= {worst:.2f} x (atol {atol:.1e} + rtol {rtol:.1e} * |ref|)')
     return worst
+
+
+def kernel_events(prof, tmp_dir: str) -> List[Tuple[str, Optional[int]]]:
+    """``(instance, grid.x)`` of every accumulate / attention_probs kernel of a trace, in launch order."""
+    path = os.path.join(tmp_dir, 'launches.pt.trace.json')
+    prof.export_chrome_trace(path)
+    events = []
+    with open(path) as f:
+        trace = json.load(f)
+    for e in trace['traceEvents']:
+        if e.get('cat') != 'kernel':
+            continue
+        m = re.search(r'(accumulate_\w+_kernel|attention_probs_kernel)(<[^<>]*>)?', e['name'])
+        if not m or m.group(1) == 'accumulate_probs_kernel':
+            continue
+        args = e.get('args', {})
+        grid = args.get('grid')
+        events.append((args.get('correlation', e['ts']), e['ts'], m.group(0).replace(' ', ''),
+                       grid[0] if grid else None))
+    return [(inst, grid) for _, _, inst, grid in sorted(events)]
+
+
+def traced(module: str, request: dict) -> List[Tuple[str, Optional[int]]]:
+    """``module._trace_main(json request)`` in a fresh Python process; it prints the traced ``(instance, grid.x)``
+    list as JSON on its last line. A CUDA activity trace taken in a process that has already run
+    tests/test_accumulate_steps_gpu.py (which does not profile) holds no kernel event at all, while the same trace
+    taken before it does (H100, torch 2.11): some CUPTI / Kineto state left by the earlier work is the likely cause,
+    not found yet. A process of its own gives the trace the state a lone run of the module has."""
+    code = f'import {module} as m; m._trace_main({json.dumps(request)!r})'
+    flags = ['-s'] if sys.flags.no_user_site else []
+    out = subprocess.run([sys.executable] + flags + ['-c', code], cwd=ROOT, capture_output=True, text=True,
+                         timeout=900)
+    assert out.returncode == 0, out.stderr[-4000:]
+    return [tuple(e) for e in json.loads(out.stdout.strip().splitlines()[-1])]
 
 
 class HookRecorder:
