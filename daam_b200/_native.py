@@ -191,7 +191,7 @@ def overlay_frames_bytes(n_maps: int, n_words: int, out_h: int, out_w: int) -> i
     return (n_maps * n_words * out_h * out_w * 3 + 3) // 4 * 4
 
 
-EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_accumulate_joint', 'daam_finalize',
+EXPORTS = ('daam_accumulate', 'daam_accumulate_steps', 'daam_accumulate_range', 'daam_attention_probs', 'daam_accumulate_probs', 'daam_accumulate_joint', 'daam_accumulate_joint_heads', 'daam_finalize',
            'daam_finalize_maps', 'daam_finalize_parts', 'daam_finalize_parts_weighted', 'daam_finalize_per_key', 'daam_value_norms','daam_normalize_maps', 'daam_word_heat_map', 'daam_expand_as', 'daam_expand_words',
            'daam_segment_words', 'daam_region_overlap', 'daam_region_sweep', 'daam_region_ranking', 'daam_region_boundary', 'daam_mask_boundary', 'daam_word_overlap', 'daam_word_instances', 'daam_overlay_words', 'daam_refine_words', 'daam_segment_crf', 'daam_word_distance', 'daam_mask_distance', 'daam_image_superpixels', 'daam_segment_superpixels', 'daam_jet_colormap',
            'daam_side_launcher_create', 'daam_side_launcher_destroy',
@@ -280,6 +280,8 @@ def load() -> ctypes.CDLL:
     lib.daam_accumulate.restype = ctypes.c_int
     lib.daam_accumulate_joint.argtypes = [ctypes.POINTER(DaamJointLayer), i32, u32, vp]
     lib.daam_accumulate_joint.restype = ctypes.c_int
+    lib.daam_accumulate_joint_heads.argtypes = [ctypes.POINTER(DaamJointLayer), i32, u32, vp]
+    lib.daam_accumulate_joint_heads.restype = ctypes.c_int
     lib.daam_accumulate_steps.argtypes = [ctypes.POINTER(DaamLayer), ctypes.POINTER(vp), i32, u32, vp]
     lib.daam_accumulate_steps.restype = ctypes.c_int
     lib.daam_accumulate_range.argtypes = [ctypes.POINTER(DaamLayer), ctypes.POINTER(vp), i32, u32, vp]
@@ -447,6 +449,17 @@ def accumulate_joint(layers: Sequence[DaamJointLayer], stream: int):
         return
     array = (DaamJointLayer * len(layers))(*layers)
     rc = load().daam_accumulate_joint(array, len(layers), 0, stream)
+    if rc != 0:
+        _check(rc)
+
+
+def accumulate_joint_heads(layers: Sequence[DaamJointLayer], stream: int):
+    """``daam_accumulate_joint_heads``: :func:`accumulate_joint` with every sample's heads summed in the kernel and
+    divided by ``heads``, into a head-free accumulator ``[n_prompts][tokens][hw]``; same classes, order and packing."""
+    if not layers:
+        return
+    array = (DaamJointLayer * len(layers))(*layers)
+    rc = load().daam_accumulate_joint_heads(array, len(layers), 0, stream)
     if rc != 0:
         _check(rc)
 

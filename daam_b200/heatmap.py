@@ -84,6 +84,9 @@ class LayerSlab:
     # ``norms_changed`` is a device bool, set when a later call of the generation saw other norms than the stored ones
     norms: Optional[torch.Tensor] = None
     norms_changed: Optional[torch.Tensor] = None
+    # head-reduced joint traces only (trace(pipe, reduce_heads=True)): the number of heads whose mean each row of ``acc``
+    # holds; ``acc`` is then [n_prompts, images, tokens, h*w], one key per image (``heads == images``); 0 otherwise
+    head_mean: int = 0
 
     @property
     def n_prompts(self) -> int:
@@ -148,6 +151,7 @@ class RawHeatMapCollection:
         self.negative = False                 # slabs also hold the unconditional half (trace(negative=True))
         self.value_norms = False              # slabs also hold every key's value norms (trace(value_norms=True))
         self.joint = False                    # joint-attention slabs: any context of 1 .. 1024 rows (SD3 traces)
+        self.reduce_heads = False             # slabs hold each sample's head mean (trace(reduce_heads=True))
 
     # -- wiring from the tracer -------------------------------------------------------------------------------------
     def bind(self, sync, zero):
@@ -158,12 +162,20 @@ class RawHeatMapCollection:
             self._sync()
 
     def slab_for(self, layer_idx: int, factor: int, n_prompts: int, heads: int, h: int, w: int, device,
-                 head_offset: int = 0, images: int = 1, tokens: int = _native.TOKENS) -> LayerSlab:
+                 head_offset: int = 0, images: int = 1, tokens: int = _native.TOKENS, head_mean: int = 0) -> LayerSlab:
         """Returns (allocating or re-shaping on demand) the zero-initialised slab of a layer and marks it live.
         ``heads`` counts every image's heads of one prompt (``images`` runs of ``heads // images``); ``tokens`` is the
-        context length (77, or 154 / 231 in a ``long_prompts`` trace): every context row is accumulated."""
+        context length (77, or 154 / 231 in a ``long_prompts`` trace): every context row is accumulated.
+        ``head_mean``: the slab holds the mean of that many heads per image (``heads == images``), and every live
+        layer must average the same number, or the mean of their rows is not the mean over their keys."""
         if tokens not in _native.CONTEXT_TOKENS and not (self.joint and 1 <= tokens <= _native.JOINT_MAX_TOKENS):
             raise ValueError(f'a slab holds a context of {_native.CONTEXT_TOKENS} tokens, not {tokens}')
+        if head_mean:
+            for other in self.live_slabs():
+                if other.layer_idx != layer_idx and other.head_mean != head_mean:
+                    raise RuntimeError(f'layer {layer_idx}: {head_mean} heads, but layer {other.layer_idx} of the '
+                                       f'same trace has {other.head_mean}: reduce_heads=True averages each layer\'s '
+                                       f'heads, which is the mean over keys only when every layer has as many')
         slab = self.slabs.get(layer_idx)
         shape = (n_prompts, heads, tokens, h * w)
         if slab is None or tuple(slab.acc.shape) != shape or slab.acc.device != torch.device(device) \
@@ -191,6 +203,7 @@ class RawHeatMapCollection:
         elif (slab.h, slab.w) != (h, w):      # same pixel count, other key shape (a transposed latent): re-tag
             slab.h, slab.w = h, w
         slab.images = images                  # (same key count, other split into images: only the tag changes)
+        slab.head_mean = head_mean
         if not slab.touched:
             slab.touched = True
             self._order.append(layer_idx)
@@ -240,6 +253,7 @@ class RawHeatMapCollection:
         """``((factor, layer, head), [77, h, w])`` for every key; with ``step_range=i`` the per-key sums over the steps
         of declared range ``i`` (``trace(pipe, step_ranges=[...])``) instead of over every step; with ``negative`` those
         of the unconditional half of the CFG batch (``trace(pipe, negative=True)``)."""
+        self.check_heads('all_heat_maps.items')
         for slab in self.read_slabs(step_range, negative):
             for head in range(slab.heads):
                 yield (slab.factor, slab.layer_idx, head), slab.key_view(head, prompt, step_range, negative)
@@ -261,6 +275,12 @@ class RawHeatMapCollection:
         if self.range_steps[step_range] == 0:
             raise RuntimeError('No heat maps found for the given parameters.')
         return [s for s in slabs if s.ranges is not None]
+
+    def check_heads(self, what: str):
+        """Raises unless the slabs keep one key per head (not a ``trace(pipe, reduce_heads=True)``)."""
+        if self.reduce_heads:
+            raise RuntimeError(f'{what} reads per-head keys, which a trace(pipe, reduce_heads=True) does not keep: '
+                               f'its layers hold the mean over heads only')
 
     def check_negative(self):
         """Raises unless the slabs keep the unconditional half (``trace(pipe, negative=True)``)."""

@@ -13,7 +13,7 @@ from . import _native
 
 __all__ = ['cond_half', 'make_layer_desc', 'new_accumulator', 'pack', 'accumulate', 'accumulate_steps',
            'accumulate_range', 'accumulate_layer', 'attention_probs', 'accumulate_probs', 'value_norms',
-           'make_joint_desc', 'accumulate_joint']
+           'make_joint_desc', 'accumulate_joint', 'accumulate_joint_heads']
 
 _DTYPES = {torch.float32: _native.DAAM_F32, torch.float16: _native.DAAM_F16, torch.bfloat16: _native.DAAM_BF16}
 
@@ -207,7 +207,8 @@ def value_norms(value: torch.Tensor, weight: torch.Tensor, heads: int, out: Opti
 
 
 def make_joint_desc(q: torch.Tensor, k: torch.Tensor, lse: torch.Tensor, n_image: int, acc: torch.Tensor, heads: int,
-                    scale: float, *, text_first: bool = False, whole_batch: bool = False) -> _native.DaamJointLayer:
+                    scale: float, *, text_first: bool = False, whole_batch: bool = False,
+                    reduce_heads: bool = False) -> _native.DaamJointLayer:
     """One ``daam_joint_layer`` from a joint attention's operands as SDPA takes them: ``q`` / ``k`` ``[B, heads, L, d]``
     (any strides, ``d`` contiguous; e.g. the concatenation ``[image, context]`` of diffusers' ``JointAttnProcessor2_0``,
     or a ``[B, L, heads*d]`` projection viewed that way), ``lse`` fp32 ``[B, heads, >= n_image]`` (text-first: ``>= L``) the attention's
@@ -216,7 +217,8 @@ def make_joint_desc(q: torch.Tensor, k: torch.Tensor, lse: torch.Tensor, n_image
 
     ``text_first``: ``L`` is ``[context, image]`` (FLUX): the image queries and their lse start at row
     ``T = L - n_image`` and the context keys at row 0. ``whole_batch``: every sample with every head is kept
-    (a batch without a CFG half), and ``acc`` is ``[B, heads, T, n_image]``."""
+    (a batch without a CFG half), and ``acc`` is ``[B, heads, T, n_image]``. ``reduce_heads``: the descriptor of
+    :func:`accumulate_joint_heads`, whose ``acc`` has no head axis: ``[n_prompts, T, n_image]`` contiguous fp32."""
     if not (q.is_cuda and k.is_cuda and lse.is_cuda and acc.is_cuda):
         raise RuntimeError('daam_b200 computes on CUDA tensors only (there is no CPU fallback)')
     if q.dtype not in _DTYPES or k.dtype != q.dtype:
@@ -241,10 +243,9 @@ def make_joint_desc(q: torch.Tensor, k: torch.Tensor, lse: torch.Tensor, n_image
         raise RuntimeError(f'lse has {lse.shape[2]} rows, the kernel reads {lse_rows}')
     tokens = seq - n_image
     first, n_prompts, head0, n_heads = (0, bsz, 0, heads) if whole_batch else cond_half(bsz, heads)
-    if tuple(acc.shape) != (n_prompts, n_heads, tokens, n_image) or acc.dtype != torch.float32 \
-            or not acc.is_contiguous():
-        raise RuntimeError(f'accumulator must be contiguous fp32 {(n_prompts, n_heads, tokens, n_image)}, '
-                           f'got {acc.dtype} {tuple(acc.shape)}')
+    shape = (n_prompts, tokens, n_image) if reduce_heads else (n_prompts, n_heads, tokens, n_image)
+    if tuple(acc.shape) != shape or acc.dtype != torch.float32 or not acc.is_contiguous():
+        raise RuntimeError(f'accumulator must be contiguous fp32 {shape}, got {acc.dtype} {tuple(acc.shape)}')
     q_row, k_row = (tokens, 0) if text_first else (0, n_image)   # first image query, first context key
     es = q.element_size()
     return _native.DaamJointLayer(
@@ -263,3 +264,9 @@ def accumulate_joint(descs, device, stream: Optional[torch.cuda.Stream] = None):
     """Enqueue ``daam_accumulate_joint`` over the given joint layer descriptors on ``stream`` (default: the current
     stream of ``device``)."""
     _run_on(device, stream, lambda s: _native.accumulate_joint(list(descs), s))
+
+
+def accumulate_joint_heads(descs, device, stream: Optional[torch.cuda.Stream] = None):
+    """Enqueue ``daam_accumulate_joint_heads`` over descriptors made with ``make_joint_desc(..., reduce_heads=True)``:
+    every sample's head mean of the joint heat map, added into its head-free accumulator."""
+    _run_on(device, stream, lambda s: _native.accumulate_joint_heads(list(descs), s))

@@ -86,12 +86,22 @@ class DiffusionHeatMapHooker(AggregateHooker):
     (:class:`FluxAttentionHooker`), whose sequences are ``[text, image]``. Every sample of its guidance-distilled batch
     is kept with all heads, reads return the T5 rows of ``prompt_2`` (or of the prompt), and it refuses what an SD3
     trace refuses, negative prompts included.
+
+    ``reduce_heads=True`` (SD3 and FLUX traces only) keeps each layer's mean over heads instead of every head: the
+    accumulate kernel (``daam_accumulate_joint_heads``) sums a sample's heads before anything reaches memory, so a
+    layer's slab is ``[prompts, images, T, hw]``, 1/heads of the per-head one. A joint key has its grid's own size, so
+    the finalize neither resamples nor clamps it, and every read that averages over heads returns the same maps up to
+    rounding: the global, layer, factor and image maps, ``to_experiment`` and the word-list calls. Reads of single
+    heads (``head_idx``, :meth:`compute_per_head_heat_maps`, :meth:`compute_head_heat_maps`, ``all_heat_maps.items``)
+    raise. Every traced layer must have the same number of heads. A UNet trace refuses it: there every key is
+    upsampled and clamped before the mean over keys, so the head sum cannot be taken first.
     """
 
     def __init__(self, pipeline, low_memory: bool = False, load_heads: bool = False, save_heads: bool = False,
                  data_dir: str = None, *, launch: str = 'step', batch_prompts: bool = False,
                  locate_middle_block: bool = False, kernel_flags: int = _native.ACC_AUTO, time_resolved: bool = False,
-                 step_ranges=None, negative: bool = False, long_prompts: bool = False, value_norms: bool = False):
+                 step_ranges=None, negative: bool = False, long_prompts: bool = False, value_norms: bool = False,
+                 reduce_heads: bool = False):
         if launch not in ('step', 'overlap', 'layer'):
             raise ValueError("launch must be 'step', 'overlap' or 'layer'")
         if value_norms and (save_heads or load_heads):
@@ -118,6 +128,9 @@ class DiffusionHeatMapHooker(AggregateHooker):
         self.joint = getattr(pipeline, 'unet', None) is None and getattr(pipeline, 'transformer', None) is not None
         # FLUX.1: a joint trace whose transformer also has single-stream blocks (text-first, no CFG half)
         self.flux = self.joint and getattr(pipeline.transformer, 'single_transformer_blocks', None) is not None
+        if reduce_heads and not self.joint:
+            raise ValueError('reduce_heads=True needs a joint-attention (SD3 / FLUX) trace: a UNet layer upsamples and '
+                             'clamps every key before the mean over keys, so the heads cannot be summed first')
         if self.joint:
             model = 'a FLUX' if self.flux else 'an SD3'
             options = dict(time_resolved=time_resolved, step_ranges=step_ranges is not None, negative=negative,
@@ -133,6 +146,8 @@ class DiffusionHeatMapHooker(AggregateHooker):
         _native.load()   # fail here, loudly, if the CUDA library is missing
         self.all_heat_maps = RawHeatMapCollection()
         self.all_heat_maps.joint = self.joint
+        self.reduce_heads = reduce_heads
+        self.all_heat_maps.reduce_heads = reduce_heads
         if self.flux:
             # FLUX: the grid is the image size check_inputs receives, in 2 x 2 packed latent patches
             self.latent_hw = self._sample_size = None
@@ -439,7 +454,8 @@ class DiffusionHeatMapHooker(AggregateHooker):
         context; FLUX: the context, then the image tokens) and the attention's ``lse``. Queued for the step launch at
         the end of the transformer forward, or launched now with ``launch='layer'``.
 
-        FLUX keeps every sample of the batch with every head (it has no CFG half)."""
+        FLUX keeps every sample of the batch with every head (it has no CFG half). With ``reduce_heads`` the slab
+        keeps each sample's mean over its kept heads, one row per sample."""
         if not q.is_cuda:
             raise RuntimeError('daam_b200 traces pipelines that live on a CUDA device only (there is no CPU '
                                'fallback)')
@@ -452,17 +468,27 @@ class DiffusionHeatMapHooker(AggregateHooker):
             _, n_samples, head0, n_heads = ops.cond_half(q.shape[0], heads)
         n_real, images = self._prompt_layout(layer_idx, n_samples)
         tokens = k.shape[2] - n_image
-        slab = self.all_heat_maps.slab_for(layer_idx, factor, n_real, images * n_heads, h, w, q.device, head0, images,
-                                           tokens)
-        desc = ops.make_joint_desc(q, k, lse, n_image, slab.acc.view(n_samples, n_heads, tokens, n_image), heads,
-                                   scale, text_first=self.flux, whole_batch=self.flux)
+        if self.reduce_heads:
+            slab = self.all_heat_maps.slab_for(layer_idx, factor, n_real, images, h, w, q.device, head0, images,
+                                               tokens, head_mean=n_heads)
+            acc = slab.acc.view(n_samples, tokens, n_image)
+        else:
+            slab = self.all_heat_maps.slab_for(layer_idx, factor, n_real, images * n_heads, h, w, q.device, head0,
+                                               images, tokens)
+            acc = slab.acc.view(n_samples, n_heads, tokens, n_image)
+        desc = ops.make_joint_desc(q, k, lse, n_image, acc, heads, scale, text_first=self.flux, whole_batch=self.flux,
+                                   reduce_heads=self.reduce_heads)
         self._device = q.device
         if self.launch == 'layer':
-            ops.accumulate_joint([desc], q.device)
+            self._accumulate_joint([desc], q.device)
             return
         self._joint_pending.append(desc)
         self._refs += [q, k, lse]                          # kept alive until the step's launch has been issued
         self._queued[layer_idx] = self._step_id
+
+    def _accumulate_joint(self, descs, device):
+        """The joint launch of ``descs``: per head, or with ``reduce_heads`` each sample's head mean."""
+        (ops.accumulate_joint_heads if self.reduce_heads else ops.accumulate_joint)(descs, device)
 
     def _launch_now(self, own, device):
         """``launch='layer'``: the layer's kernel right away on the current stream (the producer of Q/K may be the
@@ -489,7 +515,7 @@ class DiffusionHeatMapHooker(AggregateHooker):
         """Issue the queued layer calls as one persistent launch (per pack of 32 layers)."""
         if self._joint_pending:
             descs, self._joint_pending = self._joint_pending, []
-            ops.accumulate_joint(descs, self._device)   # on the forward's own stream: the projections may go now
+            self._accumulate_joint(descs, self._device)   # on the forward's own stream: the projections may go now
             self._refs = []
             self._queued.clear()
             return
@@ -764,6 +790,7 @@ class DiffusionHeatMapHooker(AggregateHooker):
         """``(prompt, keys, maps)`` of :meth:`compute_per_head_heat_maps`. Weighted: the per-key maps unnormalised,
         times each key's norm per row on the device, then normalised -- a single key's weighted global map. Also
         returns the map's tokenizer."""
+        self.all_heat_maps.check_heads('per-head heat maps')
         encoder = self._encoder(encoder)
         prompt, grid, rows, groups, slabs = self._read_groups(prompt, factors, prompt_idx, step_range,
                                                               negative=negative, image_idx=image_idx, encoder=encoder)
@@ -901,6 +928,9 @@ class DiffusionHeatMapHooker(AggregateHooker):
         is context row ``r - 1`` (T5 has no start token); the text is ``prompt_2`` when the generation had one."""
         if encoder not in ('clip', 't5'):
             raise ValueError(f"encoder must be 'clip' or 't5', got {encoder!r}")
+        if head_idx is not None and self.reduce_heads:
+            raise ValueError('head_idx selects one head, but a trace(pipe, reduce_heads=True) keeps the mean over '
+                             'heads only')
         if encoder == 't5':
             if not self.joint:
                 raise ValueError("encoder='t5' reads the T5 rows of a joint-attention (SD3) trace; this trace has "

@@ -43,7 +43,8 @@ extern "C" {
                                           daam_image_superpixels, daam_segment_superpixels;
                                           daam_value_norms, daam_finalize_parts_weighted;
                                           daam_joint_layer, daam_accumulate_joint; a key group's acc may point at
-                                          any row of a slab, see daam_key_group) */
+                                          any row of a slab, see daam_key_group;
+                                          daam_accumulate_joint_heads) */
 #define DAAM_TOKENS 77          /* context length the reference traces (daam/trace.py:194, guard at :289) */
 #define DAAM_MAX_TOKENS 231     /* daam_accumulate: long contexts of 2 or 3 CLIP chunks of 77 tokens (154, 231) */
 #define DAAM_MAX_HEAD_DIM 256   /* any multiple of 8 up to here (SD-1.x deepest level: 1280 channels / 8 heads = 160) */
@@ -183,6 +184,28 @@ typedef struct daam_joint_layer {
   int64_t lse_stride_prompt, lse_stride_head, lse_stride_pixel;   /* in elements */
 } daam_joint_layer;
 int daam_accumulate_joint(const daam_joint_layer* layers, int32_t n_layers, uint32_t flags, void* stream);
+
+/*
+ * Head-reduced joint attention (daam_b200/trace.py, trace(pipe, reduce_heads=True)): daam_accumulate_joint with the
+ * heads of every sample summed before anything reaches the accumulator,
+ *
+ *   acc[p][t][pixel] += fp32(sum_h v_h) / heads
+ *
+ * with v_h = ex2.approx.ftz.f32(fmaf(s_h, c, -l_h)) exactly the value daam_accumulate_joint adds for head h of the
+ * same element (the same dot product, c and l). `acc` is fp32, contiguous [n_prompts][tokens][hw]: one slab row per
+ * kept sample, no head axis. Arithmetic of the head sum and the update:
+ *   sum = v_0;  sum = sum + v_h for h = 1, 2, .., heads - 1    (add.rn.f32, heads ascending, in registers);
+ *   acc = acc + div.rn.f32(sum, heads)                        (add.rn.f32).
+ * A joint key has its grid's own size (factor 1), so the finalize's bicubic taps are 0, 1, 0, 0 and its clamp does
+ * nothing (every value is positive): the global map is linear in the keys, and the mean over the slab rows of the
+ * layers that keep the same head count is the mean over their keys.
+ * Every element is read and written once per launch by one thread, with no atomics, so the bits are the same on every
+ * call and however the layers are split into calls. Layer array, strides, lse, dtypes, kernel classes and their order
+ * (fp16, bf16, fp32), call order within a class, DAAM_JOINT_MAX_LAYERS per launch and the overlap rule (on the
+ * head-free slab) are daam_accumulate_joint's, and so are its checks and error codes; a null or not 16-byte aligned
+ * `acc` is DAAM_E_INVALID. `flags` is reserved: pass 0.
+ */
+int daam_accumulate_joint_heads(const daam_joint_layer* layers, int32_t n_layers, uint32_t flags, void* stream);
 
 /*
  * Time-resolved heat maps (daam_b200/trace.py, trace(..., time_resolved=True)): daam_accumulate, and also
